@@ -289,6 +289,57 @@ def update_case(seed, hz):
     return p, cost, a, ms
 
 
+def pool_fields(nav, ndests, nchunks):
+    """the device field pool read back with pool_get -> (slot[ndests * nchunks], flow[n, 64, 64], los[n, 64, 64]) as
+    pfo_desired_velocity takes it: one slot per (dest, chunk) that holds a flow or a LOS field, the absent half zero
+    (FD_NONE / no LOS, which is what the device reads for a missing field too)"""
+    slot = np.full(ndests * nchunks, -1, np.int32)
+    flow, los = [], []
+    for d in range(ndests):
+        for c in range(nchunks):
+            f, l, _ = nav.pool_get(d, divmod(c, nav.cw))
+            if f is None and l is None:
+                continue
+            slot[d * nchunks + c] = len(flow)
+            flow.append(f if f is not None else np.zeros((64, 64), np.uint8))
+            los.append(l if l is not None else np.zeros((64, 64), np.uint8))
+    return slot, np.array(flow, np.uint8).reshape(-1, 64, 64), np.array(los, np.uint8).reshape(-1, 64, 64)
+
+
+def port_tick(omap, agents, flocks, movestate, work, hz, arrival, pool=None, vdes=None, los=None):
+    """One tick of the point-seek pipeline in the plain-C port (oracle/pf_oracle.c): desired velocity and LOS bit
+    (pfo_desired_velocity over `pool`, else the given `vdes` / `los`), the velocity pass on them (pfo_velocity_work),
+    entity_compute_update on the new velocities (pfo_entity_updates) and the movestate part of entity_apply_update
+    (pfo_entity_apply).
+    agents / movestate: AGENT / MOVESTATE records of the whole population (not modified); flocks: FLOCK records;
+    work: the uids of this tick; arrival: route_arrival_consts of every flock target; pool: pool_fields().
+    -> dict(vdes, los, vel, patches, agents, movestate), the last two after the apply."""
+    import pforacle
+    work = np.ascontiguousarray(work, np.uint32)
+    rec = np.array(agents, capi.AGENT)
+    if pool is not None:
+        vdes, los = omap.desired_velocity(rec, flocks, work, *pool)
+    rec["vdes"][work] = vdes
+    rec["has_dest_los"][work] = los
+    world = pforacle.OracleWorld(omap, rec, flocks, hz)
+    try:
+        vel, _ = world.velocity_work(work)
+        patches = world.entity_updates(movestate, arrival, work, vel, vdes, capi.PATCH)
+    finally:
+        world.close()
+    a2, ms2 = pforacle.entity_apply(rec, movestate, work, patches)
+    return dict(vdes=vdes, los=los, vel=vel, patches=patches, agents=a2, movestate=ms2)
+
+
+PATCH_FLOATS = ("next_velocity", "next_pos", "next_rot", "next_ppos", "next_npos", "next_step", "next_left", "next_nrot",
+                "next_prot")
+
+
+def patch_floats(p):
+    """the 25 floats of a patch (port or device layout) -> float32[n, 25]"""
+    return np.concatenate([p[k].reshape(len(p), -1) for k in PATCH_FLOATS], axis=1)
+
+
 def repair_case(ref, cw, ch, seed, per_chunk=4):
     """Requests for the repair chain of N_DesiredPointSeekVelocity (nav.c:3508-3554) on a map with blockers.
     ref: a pfref.RefMap that already holds the blockers (after update()). Returns (targets FIELD_REQ[n],

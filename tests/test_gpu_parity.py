@@ -235,17 +235,21 @@ def test_agents_vs_port_dense_crowd(nav, pforacle):
     vpref, _, _ = nav.agents_read_debug(len(work))
     assert cases.relerr(vpref, evpref).max() <= VEL_RTOL
     assert cases.relerr(vel, evel).max() <= VEL_RTOL
-    # hz variants and a COMBAT_HELD agent
+    w.close()
+    # the other tick rates (SCALED_MAX_FORCE and max_speed / hz, movement.c:93) and a COMBAT_HELD agent
     rec2 = rec.copy(); rec2["flags"][work[0]] |= capi.FLAG_COMBAT_HELD
-    w2 = pforacle.OracleWorld(om, rec2, fl, 10)
-    evel2, _ = w2.velocity_work(work[:200])
-    nav.agents_upload(rec2, fl, 10)
-    nav.agents_set_work(work[:200])
-    nav.agents_tick(0)
-    vel2 = nav.agents_read_velocities(200)
-    assert (vel2[0] == 0).all()
-    assert cases.relerr(vel2, evel2).max() <= VEL_RTOL
-    w.close(); w2.close()
+    for hz in (10, 5, 1):
+        w2 = pforacle.OracleWorld(om, rec2, fl, hz)
+        evel2, evpref2 = w2.velocity_work(work[:200])
+        w2.close()
+        nav.agents_upload(rec2, fl, hz)
+        nav.agents_set_work(work[:200])
+        nav.agents_tick(0)
+        vel2 = nav.agents_read_velocities(200)
+        vpref2, _, _ = nav.agents_read_debug(200)
+        assert (vel2[0] == 0).all(), hz
+        assert cases.relerr(vpref2, evpref2).max() <= VEL_RTOL, hz
+        assert cases.relerr(vel2, evel2).max() <= VEL_RTOL, hz
 
 
 # ------------------------------------------------------------------ against the compiled reference, if it travelled

@@ -365,6 +365,44 @@ def test_port_entity_update_golden(pforacle, name):
     assert (ms2["vel_hist"][g["work"]] == g["hist"]).all() and (ms2["vel_hist_idx"][g["work"]] == g["hidx"]).all()
 
 
+@pytest.mark.parametrize("name", ["update_hz20", "update_hz10"])
+def test_port_tick_golden(pforacle, name):
+    """cases.port_tick, the per-tick expectation of the device-resident trajectory test, composed end to end on the
+    reference's state-update fixtures: from the reference's desired velocities it must reproduce the reference's
+    velocities, patches and velocity history. Velocities within 1e-6 relative (the port's own bound,
+    test_port_velocity_with_garrisoned_and_los_golden); flags, states, blocking and the history index identical for
+    every work item; the 25 patch floats and the history bit-exact wherever the port's velocity is the reference's,
+    within 1e-4 of max(|x|, 1) elsewhere."""
+    g = gold(name)
+    a = _agents_from_gold(g)
+    rec, fl = capi.pack_agents(a)
+    nav = capi.Nav(hostonly=True)
+    nav.map_create(3, 3, 1); nav.map_upload_layer(0, g["cost"]); nav.map_build_nav(0); nav.route_build(0)
+    arrival = [nav.route_arrival_consts(t) for t in a["flock_target"]]
+    nav.close()
+    work = g["work"]
+    t = cases.port_tick(pforacle.OracleMap(3, 3, g["cost"]), rec, fl, g["ms"].view(capi.MOVESTATE), work, int(g["hz"]),
+                        arrival, vdes=g["vdes"], los=g["los"])
+    assert (cases.relerr(t["vel"], g["vel"]) <= 1e-6).all()
+    p, oi, of = t["patches"], g["patch_i"], g["patch_f"][:, :25]
+    assert (p["flags"] == oi[:, 0].astype(np.uint32)).all() and (p["next_state"] == oi[:, 1]).all() and (p["next_block"] == oi[:, 2]).all()
+    assert {-1, 2, 4} <= set(p["next_state"].tolist())
+    exact = (t["vel"] == g["vel"]).all(axis=1)
+    assert exact.mean() > 0.95
+    got = cases.patch_floats(p)
+    assert (got[exact] == of[exact]).all()
+    assert (np.abs(got - of) <= 1e-4 * np.maximum(np.abs(of), 1.0)).all()
+    ms2 = t["movestate"]
+    assert (ms2["vel_hist_idx"][work] == g["hidx"]).all()
+    assert (ms2["vel_hist"][work][exact] == g["hist"][exact]).all()
+    assert (np.abs(ms2["vel_hist"][work] - g["hist"]) <= 1e-4 * np.maximum(np.abs(g["hist"]), 1.0)).all()
+    # the agent records after the apply: garrisoned entities untouched, everyone else moved to the patch's position
+    garr = (a["flags"][work] & capi.FLAG_GARRISONED) != 0
+    setpos = ((oi[:, 0] & 4) != 0) & ~garr
+    assert (t["agents"]["pos"][work][setpos] == got[setpos][:, [2, 4]]).all()
+    assert (t["agents"]["state"][work][garr] == a["state"][work][garr]).all()
+
+
 def test_port_desired_velocity_golden(pforacle):
     g = gold("agents_3x3")
     a = _agents_from_gold(g)
