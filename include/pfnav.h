@@ -277,6 +277,16 @@ int  pfnav_request_faction(pfnav_ctx *ctx, int faction_id);
 int  pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, float src_x, float src_z,
                              float dst_x, float dst_z, void *stream, uint32_t *out_dest_id,
                              int *out_ok, int *out_n_flow, int *out_n_los);
+/* N_RequestPath (nav.c:3386) for a batch of n requests on one layer against the device field pool. Equivalent, field
+ * for field, to calling pfnav_pool_request_path(ctx, dests[i], layer, src_xz[2i], src_xz[2i+1], dst_xz[2i],
+ * dst_xz[2i+1], ...) for i = 0 .. n-1 in order: a later request sees (reuses, merges into, chains its LOS onto) the
+ * fields an earlier one produced. Per-request outputs may be NULL. Arguments are validated before anything changes
+ * (PFNAV_ERR_ARG: nothing done). If the pool cannot hold request k's fields, requests 0 .. k-1 are done exactly as the
+ * serial calls would have left them, *out_ndone = k and PFNAV_ERR_NOMEM is returned. Launches are asynchronous on
+ * `stream`, like pfnav_pool_request_path's. The portal-graph searches of a large batch run on the device. */
+int  pfnav_pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *dests, int layer, const float *src_xz,
+                              const float *dst_xz, void *stream, uint32_t *out_dest_ids, int32_t *out_ok,
+                              int32_t *out_n_flow, int32_t *out_n_los, int *out_ndone);
 /* Read one pool entry back (4096 B each, pointers may be NULL). *out_has: bit0 flow, bit1 LOS;
  * *out_ffid: the N_FlowFieldID currently mapped for (dest, chunk). */
 int  pfnav_pool_get(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, uint8_t *flow_out,

@@ -13,6 +13,7 @@ FD_NONE, FD_NW, FD_N, FD_NE, FD_W, FD_E, FD_SW, FD_S, FD_SE = range(9)
 TARGET_PORTAL, TARGET_TILE = 0, 1
 FACTION_ID_NONE = 0xF
 ISLAND_NONE = 0xFFFF
+OK, ERR_ARG, ERR_CUDA, ERR_NO_DEVICE, ERR_STATE, ERR_NOMEM = 0, -1, -2, -3, -4, -5      # pfnav_status
 
 FIELD_REQ = np.dtype([
     ("chunk_r", "<i4"), ("chunk_c", "<i4"), ("layer", "<i4"), ("faction_id", "<i4"),
@@ -99,7 +100,7 @@ SYMBOLS = [
     "pfnav_group_create", "pfnav_group_gather", "pfnav_group_destroy", "pfnav_agents_upload_shard",
     "pfnav_pool_request_goals_ex", "pfnav_blockers_batch", "pfnav_map_set_pos",
     "pfnav_agents_upload_formation", "pfnav_agents_upload_movestate_ext", "pfnav_pool_request_entity_fields",
-    "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths",
+    "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
 ]
 
 _lib = None
@@ -175,7 +176,9 @@ def load():
     L.pfnav_map_commit.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
     L.pfnav_pool_request_path.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_void_p,
                                           C.POINTER(C.c_uint32), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
-    L.pfnav_pool_get.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint64)]
+    L.pfnav_pool_request_paths.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
+    L.pfnav_pool_get.argtypes =[C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_uint64)]
     L.pfnav_route_build.argtypes = [C.c_void_p, C.c_int]
     L.pfnav_route_islands_get.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.pfnav_route_edges_get.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
@@ -649,6 +652,23 @@ class Nav:
         _chk(self.L.pfnav_pool_request_path(self.h, dest, layer, src[0], src[1], dst[0], dst[1], C.c_void_p(stream),
                                             C.byref(did), C.byref(ok), C.byref(nf), C.byref(nl)))
         return bool(ok.value), did.value, nf.value, nl.value
+
+    def pool_request_paths(self, dests, src_xz, dst_xz, layer=0, stream=0):
+        """a batch of pool_request_path calls, in order -> ok[n] (bool), dest_id[n], n_flow[n], n_los[n], ndone.
+        ndone < n: the pool could not hold request ndone's fields (PFNAV_ERR_NOMEM); requests before it are done."""
+        dests = np.ascontiguousarray(dests, np.int32).reshape(-1)
+        src = np.ascontiguousarray(src_xz, np.float32).reshape(-1, 2)
+        dst = np.ascontiguousarray(dst_xz, np.float32).reshape(-1, 2)
+        n = len(dests)
+        assert len(src) == n and len(dst) == n
+        ok, nf, nl = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        did = np.zeros(n, np.uint32)
+        ndone = C.c_int(0)
+        rc = self.L.pfnav_pool_request_paths(self.h, n, _p(dests), layer, _p(src), _p(dst), C.c_void_p(stream), _p(did), _p(ok),
+                                             _p(nf), _p(nl), C.byref(ndone))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        return ok.astype(bool), did, nf, nl, ndone.value
 
     def pool_get(self, dest, chunk):
         """-> (flow or None, los or None, ffid)"""

@@ -88,7 +88,7 @@ struct pfnav_ctx {
     std::vector<std::vector<std::vector<portal_t>>> portals;   // [layer][chunk][idx]
     // host-side derived state, owned by the context (no process-global tables: contexts on different threads are independent)
     void *route_state = nullptr;                               // pfnav_route.cu: std::vector<pfnav_route_layer>
-    void *route_dev_state = nullptr;                           // pfnav_route.cu: device copies of the routing tables (k_portal_graph_path)
+    void *route_dev_state = nullptr;                           // pfnav_route.cu: device copies of the routing tables (k_portal_graph_path_warp)
     std::set<std::pair<int, int>> dirty, fdirty;               // pfnav_blockers.cu: (layer, chunk) occupancy / faction mask changed
     void *blk_state = nullptr;                                 // pfnav_blockers.cu: queued blocker ops + device-side refcount state
 

@@ -570,111 +570,141 @@ static bool desc_for_point(const pfnav_ctx *ctx, float px, float pz, tdesc *out)
 
 }   // namespace
 
-// n_request_path (nav.c:1774-2047), request-generation half. Emits, in the reference's order, the
-// flow requests (with the N_FlowFieldID of each, field.c:1952) and LOS requests a cold field cache
-// would have to build for (src -> dst), given which (dest, chunk) entries `have_flow` / `have_los`
-// already hold (arrays of `chunks` entries; have_flow holds the ff_id mapped for the chunk or 0).
-// Returns 1 in *out_ok when a path exists (the function's bool), plus the dest_id.
-extern "C" int pfnav_route_request_path(pfnav_ctx *ctx, int layer, float src_x, float src_z, float dst_x, float dst_z,
-                                        const uint64_t *have_flow, const uint8_t *have_los,
-                                        pfnav_field_req *flow_out, uint64_t *flow_ffid, int32_t *flow_chunk, int max_flow,
-                                        int *n_flow, pfnav_los_req *los_out, int32_t *los_chunk, int max_los, int *n_los,
-                                        uint32_t *out_dest_id, int *out_ok)
+// ------------------------------------------------------------------------------------------
+// n_request_path (nav.c:1774-2047), split at the points where a batch of requests runs its parts in different places:
+//   plan_begin        the global-island test, the same-chunk early outs and n_closest_reachable_portal: read-only walks
+//                     over the routing structure, independent of the field pool (host threads in a batch);
+//   search rounds     AStar_PortalGraphPath to the destination portal; when it fails, plan_after_search runs
+//                     n_closest_reachable_from_location on the host and asks for a second search;
+//   emit_plan         the flow / LOS requests, in the reference's order, given which (dest, chunk) entries the cache
+//                     holds: the only part that depends on the requests before it.
+// ------------------------------------------------------------------------------------------
+namespace {
+
+struct path_plan {
+    tdesc src, dst, dst0;            // dst: where the path ends (moved by the second search's fallback); dst0: as requested
+    uint32_t dest_id = 0;
+    int schunk = 0, dchunk = 0, dst_port = -1;
+    bool emit = false;               // same global island: the destination chunk's field and LOS are requested
+    bool exists = false;             // a portal path was found: the fields along it are requested too
+    int ok = 0;
+    int search = 0;                  // the search round this plan waits for (1 or 2), 0 = decided
+    std::vector<Router::hop> path;
+    float cost = 0.0f;
+};
+
+static void plan_init(const pfnav_ctx *ctx, int layer, const tdesc &src, const tdesc &dst, path_plan &P)
 {
-    PF_ARG(ctx && n_flow && n_los && out_ok && out_dest_id, "args");
-    pfnav_route_layer *prl = route_layer(ctx, layer);
-    PF_ARG(prl, "pfnav_route_build not called");
-    pfnav_route_layer &RL = *prl;
-    const int cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
-    Router R{ctx, RL, layer, cw, ctx->chunk_h};
-    *n_flow = 0; *n_los = 0; *out_ok = 0;
-    // n_update_dirty_local_islands + n_update_all_edge_states (nav.c:1786-1787)
-    for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, RL, layer, ch);
-    tdesc src, dst;
-    PF_ARG(desc_for_point(ctx, src_x, src_z, &src) && desc_for_point(ctx, dst_x, dst_z, &dst), "position outside the map");
-    const uint32_t dest_id = (((uint32_t)dst.chunk_r & 0x3f) << 26) | (((uint32_t)dst.chunk_c & 0x3f) << 20) |
-                             (((uint32_t)dst.tile_r & 0x3f) << 14) | (((uint32_t)dst.tile_c & 0x3f) << 8) |
-                             (((uint32_t)layer & 0xf) << 4) | ((uint32_t)ctx->req_faction & 0xfu);   // n_dest_id (nav.c:839)
-    *out_dest_id = dest_id;
-    const int schunk = src.chunk_r * cw + src.chunk_c, dchunk = dst.chunk_r * cw + dst.chunk_c;
-    if (RL.islands[(size_t)schunk * 4096 + src.tile_r * 64 + src.tile_c] != RL.islands[(size_t)dchunk * 4096 + dst.tile_r * 64 + dst.tile_c])
-        return PFNAV_OK;
-    std::vector<uint64_t> mapped(have_flow, have_flow + chunks);      // local copy of the (dest, chunk) -> ffid mapping
-    std::vector<uint8_t> los_have(have_los, have_los + chunks);
-    std::vector<int> los_index(chunks, -1);
-    auto ffid_tile = [&](int chunk, int tr, int tc) -> uint64_t {
-        return ((uint64_t)layer << 60) | ((uint64_t)1 << 56) | ((uint64_t)tr << 24) | ((uint64_t)tc << 16) |
-               ((uint64_t)(chunk / cw) << 8) | (uint64_t)(chunk % cw);
-    };
-    auto emit_flow = [&](const pfnav_field_req &q, uint64_t id, int chunk) -> bool {
-        if (*n_flow >= max_flow) return false;
-        flow_out[*n_flow] = q; flow_ffid[*n_flow] = id; flow_chunk[*n_flow] = chunk; (*n_flow)++;
-        return true;
-    };
-    auto emit_los = [&](int chunk, int prev_chunk) -> bool {
-        if (*n_los >= max_los) return false;
+    P.src = src; P.dst = dst; P.dst0 = dst;
+    P.dest_id = (((uint32_t)dst.chunk_r & 0x3f) << 26) | (((uint32_t)dst.chunk_c & 0x3f) << 20) |
+                (((uint32_t)dst.tile_r & 0x3f) << 14) | (((uint32_t)dst.tile_c & 0x3f) << 8) |
+                (((uint32_t)layer & 0xf) << 4) | ((uint32_t)ctx->req_faction & 0xfu);      // n_dest_id (nav.c:839)
+    P.schunk = src.chunk_r * ctx->chunk_w + src.chunk_c;
+    P.dchunk = dst.chunk_r * ctx->chunk_w + dst.chunk_c;
+}
+
+// nav.c:1798-1880: up to the first portal-graph search
+static void plan_begin(const Router &R, path_plan &P)
+{
+    const tdesc &src = P.src, &dst = P.dst;
+    const int schunk = P.schunk, dchunk = P.dchunk;
+    if (R.RL.islands[(size_t)schunk * 4096 + src.tile_r * 64 + src.tile_c] != R.RL.islands[(size_t)dchunk * 4096 + dst.tile_r * 64 + dst.tile_c])
+        return;
+    P.emit = true;
+    const uint16_t dst_cl = R.closest_pathable_liid(dchunk, {dst.tile_r, dst.tile_c});
+    if (schunk == dchunk && R.closest_pathable_liid(schunk, {src.tile_r, src.tile_c}) == dst_cl) { P.ok = 1; return; }
+    if (schunk == dchunk) {
+        const bool either = R.blocked_off(schunk, {src.tile_r, src.tile_c}) || R.blocked_off(schunk, {dst.tile_r, dst.tile_c});
+        if (either && R.normally_reachable(schunk, {src.tile_r, src.tile_c}, {dst.tile_r, dst.tile_c})) { P.ok = 1; return; }
+    }
+    P.dst_port = R.closest_reachable_portal(dchunk, {dst.tile_r, dst.tile_c}, true);
+    if (P.dst_port < 0) P.dst_port = R.closest_reachable_portal(dchunk, {dst.tile_r, dst.tile_c}, false);
+    if (P.dst_port < 0) return;
+    P.search = 1;
+}
+
+// nav.c:1882-1939: after search round P.search has set P.exists / P.path / P.cost
+static void plan_after_search(const Router &R, path_plan &P)
+{
+    const int round = P.search;
+    P.search = 0;
+    if (round == 1 && !P.exists) {
+        const tdesc orig = P.dst;
+        tdesc nd = P.dst;
+        P.dst_port = R.closest_reachable_from_location(P.dchunk, P.src, &nd);
+        if (P.dst_port >= 0) P.dst = nd;
+        if (R.closest_pathable_liid(P.dchunk, {P.dst.tile_r, P.dst.tile_c}) != R.closest_pathable_liid(P.dchunk, {orig.tile_r, orig.tile_c}) &&
+            P.src.chunk_r == P.dst.chunk_r && P.src.chunk_c == P.dst.chunk_c) { P.ok = 1; return; }
+        if (P.dst_port >= 0) { P.search = 2; return; }
+    }
+    if (!P.exists) {
+        if (P.src.chunk_r == P.dst.chunk_r && P.src.chunk_c == P.dst.chunk_c) P.ok = 1;
+        return;
+    }
+    P.ok = 1;
+}
+
+static void plan_search_host(const Router &R, path_plan &P)
+{
+    P.exists = R.portal_graph_path(P.src, P.dst, P.dchunk, P.dst_port, P.path, &P.cost);
+}
+
+// the flow and LOS requests of one plan
+struct path_emit {
+    std::vector<pfnav_field_req> fr; std::vector<uint64_t> fid; std::vector<int32_t> fc;
+    std::vector<pfnav_los_req> lr; std::vector<int32_t> lc;
+    void clear() { fr.clear(); fid.clear(); fc.clear(); lr.clear(); lc.clear(); }
+};
+
+// nav.c:1815-1847 (destination chunk) and 1941-2042 (the portal path, walked backwards). mapped[chunk]: the ff_id the
+// cache maps (dest, chunk) to, or 0; los_have[chunk]: its LOS field exists. Both are updated as the cache would be.
+// LOS prev_index: -1 destination chunk, >= 0 a request of this plan, -2 the previous chunk's field already exists.
+static void emit_plan(const Router &R, const pfnav_ctx *ctx, int layer, const path_plan &P, uint64_t *mapped, uint8_t *los_have, path_emit &E)
+{
+    E.clear();
+    if (!P.emit) return;
+    const int cw = ctx->chunk_w, dchunk = P.dchunk;
+    const tdesc &dst0 = P.dst0;
+    std::vector<int> los_index(ctx->chunk_w * ctx->chunk_h, -1);
+    auto emit_los = [&](int chunk, int prev_chunk, const tdesc &tgt) {
         pfnav_los_req q;
         memset(&q, 0, sizeof(q));
         q.chunk_r = chunk / cw; q.chunk_c = chunk % cw; q.layer = layer; q.faction_id = ctx->req_faction;
-        q.tgt_chunk_r = dst.chunk_r; q.tgt_chunk_c = dst.chunk_c; q.tgt_tile_r = dst.tile_r; q.tgt_tile_c = dst.tile_c;
-        // -1: destination chunk; >= 0: request of this batch; -2: the previous chunk's field already
-        // exists (have_los) and the executor substitutes its pool slot into _pad
+        q.tgt_chunk_r = tgt.chunk_r; q.tgt_chunk_c = tgt.chunk_c; q.tgt_tile_r = tgt.tile_r; q.tgt_tile_c = tgt.tile_c;
         q.prev_index = prev_chunk < 0 ? -1 : (los_index[prev_chunk] >= 0 ? los_index[prev_chunk] : -2);
         if (prev_chunk >= 0) { q.prev_chunk_r = prev_chunk / cw; q.prev_chunk_c = prev_chunk % cw; }
-        los_index[chunk] = *n_los;
-        los_out[*n_los] = q; los_chunk[*n_los] = chunk; (*n_los)++;
+        los_index[chunk] = (int)E.lr.size();
+        E.lr.push_back(q); E.lc.push_back(chunk);
         los_have[chunk] = 1;
-        return true;
+    };
+    auto emit_flow = [&](const pfnav_field_req &q, uint64_t id, int chunk) {
+        E.fr.push_back(q); E.fid.push_back(id); E.fc.push_back(chunk);
+        mapped[chunk] = id;
     };
     pfnav_field_req base;
     memset(&base, 0, sizeof(base));
     base.layer = layer; base.faction_id = ctx->req_faction;
-    // destination chunk field + LOS (nav.c:1815-1847)
     if (!mapped[dchunk]) {
         pfnav_field_req q = base;
-        q.chunk_r = dst.chunk_r; q.chunk_c = dst.chunk_c; q.target_type = PFNAV_TARGET_TILE; q.init = 1;
-        q.tile_r = dst.tile_r; q.tile_c = dst.tile_c;
-        const uint64_t id = ffid_tile(dchunk, dst.tile_r, dst.tile_c);
-        if (!emit_flow(q, id, dchunk)) { pfnav_set_error("flow output too small"); return PFNAV_ERR_NOMEM; }
-        mapped[dchunk] = id;
+        q.chunk_r = dst0.chunk_r; q.chunk_c = dst0.chunk_c; q.target_type = PFNAV_TARGET_TILE; q.init = 1;
+        q.tile_r = dst0.tile_r; q.tile_c = dst0.tile_c;
+        emit_flow(q, ((uint64_t)layer << 60) | ((uint64_t)1 << 56) | ((uint64_t)dst0.tile_r << 24) | ((uint64_t)dst0.tile_c << 16) |
+                     ((uint64_t)(dchunk / cw) << 8) | (uint64_t)(dchunk % cw), dchunk);
     }
-    if (!los_have[dchunk] && !emit_los(dchunk, -1)) { pfnav_set_error("los output too small"); return PFNAV_ERR_NOMEM; }
-    const uint16_t dst_cl = R.closest_pathable_liid(dchunk, {dst.tile_r, dst.tile_c});
-    if (schunk == dchunk && R.closest_pathable_liid(schunk, {src.tile_r, src.tile_c}) == dst_cl) { *out_ok = 1; return PFNAV_OK; }
-    if (schunk == dchunk) {
-        const bool either = R.blocked_off(schunk, {src.tile_r, src.tile_c}) || R.blocked_off(schunk, {dst.tile_r, dst.tile_c});
-        if (either && R.normally_reachable(schunk, {src.tile_r, src.tile_c}, {dst.tile_r, dst.tile_c})) { *out_ok = 1; return PFNAV_OK; }
-    }
-    int dst_port = R.closest_reachable_portal(dchunk, {dst.tile_r, dst.tile_c}, true);
-    if (dst_port < 0) dst_port = R.closest_reachable_portal(dchunk, {dst.tile_r, dst.tile_c}, false);
-    if (dst_port < 0) return PFNAV_OK;
-    std::vector<Router::hop> path;
-    float cost;
-    bool exists = R.portal_graph_path(src, dst, dchunk, dst_port, path, &cost);
-    if (!exists) {
-        const tdesc orig = dst;
-        tdesc nd = dst;
-        dst_port = R.closest_reachable_from_location(dchunk, src, &nd);
-        if (dst_port >= 0) dst = nd;
-        if (R.closest_pathable_liid(dchunk, {dst.tile_r, dst.tile_c}) != R.closest_pathable_liid(dchunk, {orig.tile_r, orig.tile_c}) &&
-            src.chunk_r == dst.chunk_r && src.chunk_c == dst.chunk_c) { *out_ok = 1; return PFNAV_OK; }
-        if (dst_port >= 0) exists = R.portal_graph_path(src, dst, dchunk, dst_port, path, &cost);
-    }
-    if (!exists) {
-        if (src.chunk_r == dst.chunk_r && src.chunk_c == dst.chunk_c) *out_ok = 1;
-        return PFNAV_OK;
-    }
+    if (!los_have[dchunk]) emit_los(dchunk, -1, dst0);
+    if (!P.exists) return;
+    const std::vector<Router::hop> &path = P.path;
+    const tdesc &dst = P.dst;
     int prev_los_chunk = dst.chunk_r * cw + dst.chunk_c;
     const uint16_t dst_liid_now = R.closest_pathable_liid(dchunk, {dst.tile_r, dst.tile_c});
-    // walk the portal path backwards (nav.c:1941-2042)
     for (int i = (int)path.size() - 1; i > 0; i--) {
         int next_hop_idx = i;
-        if (i == 1 && path[i].chunk != schunk) next_hop_idx = 0;
+        if (i == 1 && path[i].chunk != P.schunk) next_hop_idx = 0;
         const Router::hop curr_hop = path[std::max(next_hop_idx - 1, 0)];
         const Router::hop next_hop = path[next_hop_idx];
         const auto &cp = R.P(curr_hop.chunk, curr_hop.pi);
         if (cp.conn_chunk == next_hop.chunk && cp.conn_idx == next_hop.pi) continue;
-        if (curr_hop.chunk == dchunk && next_hop.chunk == dchunk && next_hop.pi == dst_port && next_hop.liid == dst_liid_now) continue;
+        if (curr_hop.chunk == dchunk && next_hop.chunk == dchunk && next_hop.pi == P.dst_port && next_hop.liid == dst_liid_now) continue;
         const int chunk = curr_hop.chunk;
         const auto &np = R.P(next_hop.chunk, next_hop.pi);
         const auto &nn = R.P(np.conn_chunk, np.conn_idx);
@@ -692,113 +722,174 @@ extern "C" int pfnav_route_request_path(pfnav_ctx *ctx, int layer, float src_x, 
         if (mapped[chunk]) {
             if (mapped[chunk] != new_id) {
                 q.init = 0;          // merge into the chunk's existing field (nav.c:1994-2010)
-                if (!emit_flow(q, new_id, chunk)) { pfnav_set_error("flow output too small"); return PFNAV_ERR_NOMEM; }
-                mapped[chunk] = new_id;
+                emit_flow(q, new_id, chunk);
             }
         } else {
             q.init = 1;
-            if (!emit_flow(q, new_id, chunk)) { pfnav_set_error("flow output too small"); return PFNAV_ERR_NOMEM; }
-            mapped[chunk] = new_id;
+            emit_flow(q, new_id, chunk);
         }
-        if (!los_have[chunk]) {
-            if (!emit_los(chunk, prev_los_chunk)) { pfnav_set_error("los output too small"); return PFNAV_ERR_NOMEM; }
-        }
+        if (!los_have[chunk]) emit_los(chunk, prev_los_chunk, dst);
         prev_los_chunk = chunk;
     }
-    *out_ok = 1;
+}
+
+template <class F>
+static void parallel_for(int n, F f)
+{
+    const int nthreads = std::max(1, std::min({n, (int)std::thread::hardware_concurrency(), 32}));
+    if (nthreads == 1) { for (int i = 0; i < n; i++) f(i); return; }
+    std::atomic<int> next{0};
+    std::vector<std::thread> pool;
+    auto worker = [&]() { for (int i = next.fetch_add(1); i < n; i = next.fetch_add(1)) f(i); };
+    for (int t = 1; t < nthreads; t++) pool.emplace_back(worker);
+    worker();
+    for (auto &t : pool) t.join();
+}
+
+}   // namespace
+
+static int route_dev_search(pfnav_ctx *ctx, int layer, pfnav_route_layer &RL, const int32_t *req, int n, int32_t *out, int max_hops);
+
+// A search round holding at least this many searches runs on the device (k_portal_graph_path_warp), a smaller one on
+// host threads. tools/bench_route_dev.py on the C2 map, one H100 80GB HBM3 at a 400 W power limit, 16 host threads
+// (DESIGN.md §5): 64 searches take 15.6 ms on the device and 8.6 ms on the host, 1024 take 21.4 ms and 62.2 ms. The
+// device's time is mostly the latency of the longest search, so the two lines cross near 200 searches.
+#define PF_ROUTE_DEVICE_MIN_SEARCHES 256
+
+// One search round over the plans `idx` that wait for it (edge states current).
+static int search_round(pfnav_ctx *ctx, const Router &R, int layer, std::vector<path_plan> &plans, const std::vector<int> &idx)
+{
+    const int n = (int)idx.size();
+    if (n == 0) return PFNAV_OK;
+    std::vector<uint8_t> on_host(n, 1);
+    if (n >= PF_ROUTE_DEVICE_MIN_SEARCHES && ctx->device >= 0) {
+        const int max_hops = 512;
+        const size_t ostride = 4 + 3 * (size_t)max_hops;
+        std::vector<int32_t> req((size_t)n * 8), out((size_t)n * ostride);
+        for (int k = 0; k < n; k++) {
+            const path_plan &P = plans[idx[k]];
+            int32_t *q = &req[(size_t)k * 8];
+            q[0] = P.schunk; q[1] = P.src.tile_r; q[2] = P.src.tile_c;
+            q[3] = P.dchunk; q[4] = P.dst.tile_r; q[5] = P.dst.tile_c; q[6] = P.dchunk; q[7] = P.dst_port;
+        }
+        int rc = route_dev_search(ctx, layer, R.RL, req.data(), n, out.data(), max_hops);
+        if (rc) return rc;
+        for (int k = 0; k < n; k++) {
+            const int32_t *o = &out[(size_t)k * ostride];
+            if (o[0] < 0) continue;             // outgrew the device scratch: the host routine has no limits
+            path_plan &P = plans[idx[k]];
+            on_host[k] = 0;
+            P.exists = o[0] == 1;
+            P.path.clear();
+            if (!P.exists) continue;
+            memcpy(&P.cost, &o[2], 4);
+            for (int h = 0; h < o[1]; h++) P.path.push_back({o[4 + 3 * h], o[4 + 3 * h + 1], (uint16_t)o[4 + 3 * h + 2]});
+        }
+    }
+    parallel_for(n, [&](int k) { if (on_host[k]) plan_search_host(R, plans[idx[k]]); });
     return PFNAV_OK;
 }
 
-// N_RequestPath (nav.c:3386) against the device field pool: route src -> dst exactly as the reference
-// does, then build only the fields the pool does not hold yet, in place, on the device.
-extern "C" int pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, float src_x, float src_z, float dst_x,
-                                       float dst_z, void *stream, uint32_t *out_dest_id, int *out_ok, int *out_n_flow,
-                                       int *out_n_los)
+// Plans every request up to its emission: plan_begin, search round 1, the fallback, search round 2.
+static int plan_requests(pfnav_ctx *ctx, const Router &R, int layer, std::vector<path_plan> &plans)
 {
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
-    PF_NEED_DEVICE(ctx);
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_fields_sync(ctx));
-    const int chunks = ctx->chunk_w * ctx->chunk_h;
-    std::vector<uint8_t> have_los(chunks, 0);
-    for (int c = 0; c < chunks; c++) {
-        const int s = ctx->h_pool_slot[(size_t)dest * chunks + c];
-        have_los[c] = (s >= 0 && (ctx->h_pool_has[s] & 2)) ? 1 : 0;
-    }
-    const int cap = chunks * 4 + 8;
-    std::vector<pfnav_field_req> fr(cap);
-    std::vector<pfnav_los_req> lr(cap);
-    std::vector<uint64_t> fid(cap);
-    std::vector<int32_t> fc(cap), lc(cap);
-    int nf = 0, nl = 0, ok = 0;
-    uint32_t did = 0;
-    int rc = pfnav_route_request_path(ctx, layer, src_x, src_z, dst_x, dst_z, ctx->h_pool_ffid.data() + (size_t)dest * chunks,
-                                      have_los.data(), fr.data(), fid.data(), fc.data(), cap, &nf, lr.data(), lc.data(), cap,
-                                      &nl, &did, &ok);
-    if (rc) return rc;
-    if (out_dest_id) *out_dest_id = did;
-    if (out_ok) *out_ok = ok;
-    if (out_n_flow) *out_n_flow = nf;
-    if (out_n_los) *out_n_los = nl;
-    if (nf == 0 && nl == 0) return PFNAV_OK;
-    ctx->goal_batch.valid = false;          // the staging buffer is about to be reused
-    // flow waves: a request that updates a chunk already written in this batch runs one wave later
-    std::vector<int32_t> fslot(nf), fwave(nf), lslot(nl), ldepth(nl, 0);
-    std::vector<int> seen(chunks, 0);
-    int maxw = 0, maxd = 0;
-    bool evicted = false;
-    {   // slots for everything this request writes (and the previous-chunk LOS fields it reads), all or nothing
-        std::vector<size_t> keys;
-        for (int i = 0; i < nf; i++) keys.push_back((size_t)dest * chunks + fc[i]);
-        for (int i = 0; i < nl; i++) keys.push_back((size_t)dest * chunks + lc[i]);
-        for (int i = 0; i < nl; i++)
-            if (lr[i].prev_index == -2) keys.push_back((size_t)dest * chunks + lr[i].prev_chunk_r * ctx->chunk_w + lr[i].prev_chunk_c);
-        std::vector<int32_t> slots(keys.size());
-        rc = pf_pool_reserve(ctx, keys.data(), keys.size(), slots.data(), &evicted);
+    const int n = (int)plans.size();
+    parallel_for(n, [&](int i) { plan_begin(R, plans[i]); });
+    for (int round = 1; round <= 2; round++) {
+        std::vector<int> idx;
+        for (int i = 0; i < n; i++) if (plans[i].search == round) idx.push_back(i);
+        int rc = search_round(ctx, R, layer, plans, idx);
         if (rc) return rc;
-        for (int i = 0; i < nf; i++) { fslot[i] = slots[i]; ctx->h_pool_has[fslot[i]] |= 1; }
-        for (int i = 0; i < nl; i++) { lslot[i] = slots[nf + i]; ctx->h_pool_has[lslot[i]] |= 2; }
+        parallel_for((int)idx.size(), [&](int k) { plan_after_search(R, plans[idx[k]]); });
     }
-    for (int i = 0; i < nf; i++) {
-        fwave[i] = seen[fc[i]]++;
-        maxw = std::max(maxw, fwave[i]);
-        ctx->h_pool_ffid[(size_t)dest * chunks + fc[i]] = fid[i];
-        ctx->h_pool_req[fslot[i]] = fr[i];
-    }
-    for (int i = 0; i < nl; i++) {
-        if (lr[i].prev_index >= 0) ldepth[i] = ldepth[lr[i].prev_index] + 1;
-        else if (lr[i].prev_index == -2) {
-            const int pchunk = lr[i].prev_chunk_r * ctx->chunk_w + lr[i].prev_chunk_c;
-            lr[i]._pad = ctx->h_pool_slot[(size_t)dest * chunks + pchunk];       // absolute pool slot of prev_los
-        }
-        maxd = std::max(maxd, ldepth[i]);
-    }
+    return PFNAV_OK;
+}
+
+// n_request_path (nav.c:1774-2047), request-generation half. Emits, in the reference's order, the
+// flow requests (with the N_FlowFieldID of each, field.c:1952) and LOS requests a cold field cache
+// would have to build for (src -> dst), given which (dest, chunk) entries `have_flow` / `have_los`
+// already hold (arrays of `chunks` entries; have_flow holds the ff_id mapped for the chunk or 0).
+// Returns 1 in *out_ok when a path exists (the function's bool), plus the dest_id.
+extern "C" int pfnav_route_request_path(pfnav_ctx *ctx, int layer, float src_x, float src_z, float dst_x, float dst_z,
+                                        const uint64_t *have_flow, const uint8_t *have_los,
+                                        pfnav_field_req *flow_out, uint64_t *flow_ffid, int32_t *flow_chunk, int max_flow,
+                                        int *n_flow, pfnav_los_req *los_out, int32_t *los_chunk, int max_los, int *n_los,
+                                        uint32_t *out_dest_id, int *out_ok)
+{
+    PF_ARG(ctx && n_flow && n_los && out_ok && out_dest_id, "args");
+    pfnav_route_layer *prl = route_layer(ctx, layer);
+    PF_ARG(prl, "pfnav_route_build not called");
+    pfnav_route_layer &RL = *prl;
+    const int chunks = ctx->chunk_w * ctx->chunk_h;
+    Router R{ctx, RL, layer, ctx->chunk_w, ctx->chunk_h};
+    *n_flow = 0; *n_los = 0; *out_ok = 0;
+    // n_update_dirty_local_islands + n_update_all_edge_states (nav.c:1786-1787)
+    for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, RL, layer, ch);
+    tdesc src, dst;
+    PF_ARG(desc_for_point(ctx, src_x, src_z, &src) && desc_for_point(ctx, dst_x, dst_z, &dst), "position outside the map");
+    path_plan P;
+    plan_init(ctx, layer, src, dst, P);
+    *out_dest_id = P.dest_id;
+    plan_begin(R, P);
+    while (P.search) { plan_search_host(R, P); plan_after_search(R, P); }
+    std::vector<uint64_t> mapped(have_flow, have_flow + chunks);
+    std::vector<uint8_t> los_have(have_los, have_los + chunks);
+    path_emit E;
+    emit_plan(R, ctx, layer, P, mapped.data(), los_have.data(), E);
+    const int nf = std::min((int)E.fr.size(), std::max(max_flow, 0)), nl = std::min((int)E.lr.size(), std::max(max_los, 0));
+    for (int i = 0; i < nf; i++) { flow_out[i] = E.fr[i]; flow_ffid[i] = E.fid[i]; flow_chunk[i] = E.fc[i]; }
+    for (int i = 0; i < nl; i++) { los_out[i] = E.lr[i]; los_chunk[i] = E.lc[i]; }
+    *n_flow = nf; *n_los = nl;
+    if (nf < (int)E.fr.size()) { pfnav_set_error("flow output too small"); return PFNAV_ERR_NOMEM; }
+    if (nl < (int)E.lr.size()) { pfnav_set_error("los output too small"); return PFNAV_ERR_NOMEM; }
+    *out_ok = P.ok;
+    return PFNAV_OK;
+}
+
+namespace {
+
+// The flow waves and LOS requests of consecutive requests of a batch that go to the device together. Within one
+// segment no pool slot changes owner, so (dest, chunk) keys and slots correspond one to one.
+struct path_segment {
+    std::vector<pfnav_field_req> fr; std::vector<int32_t> fs, fw;
+    std::vector<pfnav_los_req> lr; std::vector<int32_t> ls, ld;
+    std::unordered_map<int32_t, int> writes;          // slot -> flow writes to it so far: the next one goes a wave later
+    std::unordered_map<size_t, int> los_at;           // (dest, chunk) -> its LOS request in lr
+    std::vector<std::pair<int32_t, size_t>> used;     // (slot, key) of every slot written or read
+    void clear() { fr.clear(); fs.clear(); fw.clear(); lr.clear(); ls.clear(); ld.clear(); writes.clear(); los_at.clear(); used.clear(); }
+};
+
+// Upload a segment's requests and launch its flow waves and its one LOS launch on `st`.
+static int launch_segment(pfnav_ctx *ctx, cudaStream_t st, const path_segment &S)
+{
+    const int nf = (int)S.fr.size(), nl = (int)S.lr.size();
+    if (nf == 0 && nl == 0) return PFNAV_OK;
+    int maxw = 0, maxd = 0;
+    for (int i = 0; i < nf; i++) maxw = std::max(maxw, S.fw[i]);
+    for (int i = 0; i < nl; i++) maxd = std::max(maxd, S.ld[i]);
     std::vector<int32_t> fwave_off(maxw + 2, 0), lwave_off(maxd + 2, 0);
-    for (int i = 0; i < nf; i++) fwave_off[fwave[i] + 1]++;
+    for (int i = 0; i < nf; i++) fwave_off[S.fw[i] + 1]++;
     for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
-    for (int i = 0; i < nl; i++) lwave_off[ldepth[i] + 1]++;
+    for (int i = 0; i < nl; i++) lwave_off[S.ld[i] + 1]++;
     for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
     const size_t b_fr = (size_t)nf * sizeof(pfnav_field_req), b_fs = (size_t)nf * 4;
     const size_t b_lr = (size_t)nl * sizeof(pfnav_los_req), b_ls = (size_t)nl * 4;
     const size_t total = b_fr + b_fs + b_lr + b_ls;
-    std::vector<uint8_t> host(total ? total : 1);
+    std::vector<uint8_t> host(total);
     pfnav_field_req *hfr = (pfnav_field_req *)host.data();
     int32_t *hfs = (int32_t *)(host.data() + b_fr);
     pfnav_los_req *hlr = (pfnav_los_req *)(host.data() + b_fr + b_fs);
     int32_t *hls = (int32_t *)(host.data() + b_fr + b_fs + b_lr);
-    {
+    {   // stable order by wave / depth: an LOS request follows the one it reads
         std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1), cur2(lwave_off.begin(), lwave_off.end() - 1), lnew(nl);
-        for (int i = 0; i < nf; i++) { const int k = cur[fwave[i]]++; hfr[k] = fr[i]; hfs[k] = fslot[i]; }
-        for (int i = 0; i < nl; i++) lnew[i] = cur2[ldepth[i]]++;
+        for (int i = 0; i < nf; i++) { const int k = cur[S.fw[i]]++; hfr[k] = S.fr[i]; hfs[k] = S.fs[i]; }
+        for (int i = 0; i < nl; i++) lnew[i] = cur2[S.ld[i]]++;
         for (int i = 0; i < nl; i++) {
-            pfnav_los_req q = lr[i];
+            pfnav_los_req q = S.lr[i];
             if (q.prev_index >= 0) q.prev_index = lnew[q.prev_index];
-            hlr[lnew[i]] = q; hls[lnew[i]] = lslot[i];
+            hlr[lnew[i]] = q; hls[lnew[i]] = S.ls[i];
         }
     }
-    PF_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = pf_stream(ctx, stream);
     if (ctx->plan_buf_bytes < total) {
         PF_CUDA(cudaStreamSynchronize(st));
         cudaFree(ctx->d_plan_buf);
@@ -808,22 +899,172 @@ extern "C" int pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, floa
     }
     uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
     PF_CUDA(cudaMemcpyAsync(dev, host.data(), total, cudaMemcpyHostToDevice, st));
-    if (evicted)      // entries of other destinations lost their slots
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st));
-    else
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot + (size_t)dest * chunks, ctx->h_pool_slot.data() + (size_t)dest * chunks,
-                                (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
-                            cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaStreamSynchronize(st));
+    PF_CUDA(cudaStreamSynchronize(st));      // `host` is pageable and about to go out of scope
     for (int w = 0; w <= maxw; w++) {
         const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
         if (cnt <= 0) continue;
-        rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->d_pool_flow, (const int32_t *)(dev + b_fr) + first, st);
+        int rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->d_pool_flow, (const int32_t *)(dev + b_fr) + first, st);
         if (rc) return rc;
     }
-    if (nl) rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + b_fr + b_fs), nl, ctx->d_pool_los,
-                                  (const int32_t *)(dev + b_fr + b_fs + b_lr), maxd + 1, lwave_off.data(), st);
+    if (nl) return pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + b_fr + b_fs), nl, ctx->d_pool_los,
+                                    (const int32_t *)(dev + b_fr + b_fs + b_lr), maxd + 1, lwave_off.data(), st);
+    return PFNAV_OK;
+}
+
+}   // namespace
+
+// pfnav_pool_request_paths once its arguments are checked: plan every request, then emit and reserve request by
+// request in order -- what the serial calls would do to the pool mirrors -- and launch the device work per segment.
+static int pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *dests, int layer, const float *src_xz, const float *dst_xz,
+                              void *stream, uint32_t *out_dest_ids, int32_t *out_ok, int32_t *out_n_flow, int32_t *out_n_los,
+                              int *out_ndone)
+{
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(pf_fields_sync(ctx));
+    pfnav_route_layer &RL = *route_layer(ctx, layer);
+    const int cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
+    // n_update_all_edge_states (nav.c:1787): the map does not change between the requests of a batch
+    for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, RL, layer, ch);
+    Router R{ctx, RL, layer, cw, ctx->chunk_h};
+    std::vector<path_plan> plans(n);
+    for (int i = 0; i < n; i++) {
+        tdesc s, d;
+        desc_for_point(ctx, src_xz[2 * i], src_xz[2 * i + 1], &s);
+        desc_for_point(ctx, dst_xz[2 * i], dst_xz[2 * i + 1], &d);
+        plan_init(ctx, layer, s, d, plans[i]);
+    }
+    int rc = plan_requests(ctx, R, layer, plans);
+    if (rc) return rc;
+    cudaStream_t st = pf_stream(ctx, stream);
+    path_segment S;
+    path_emit E;
+    std::vector<uint64_t> mapped(chunks);
+    std::vector<uint8_t> los_have(chunks);
+    std::vector<uint8_t> row_touched(ctx->pool_ndests, 0);
+    bool any_evicted = false;
+    int done = 0;
+    for (; done < n; done++) {
+        const path_plan &P = plans[done];
+        const int dest = dests[done];
+        const size_t row = (size_t)dest * chunks;
+        for (int c = 0; c < chunks; c++) {
+            const int s = ctx->h_pool_slot[row + c];
+            los_have[c] = (s >= 0 && (ctx->h_pool_has[s] & 2)) ? 1 : 0;
+        }
+        memcpy(mapped.data(), ctx->h_pool_ffid.data() + row, (size_t)chunks * 8);
+        emit_plan(R, ctx, layer, P, mapped.data(), los_have.data(), E);
+        const int nf = (int)E.fr.size(), nl = (int)E.lr.size();
+        if (out_dest_ids) out_dest_ids[done] = P.dest_id;
+        if (out_ok) out_ok[done] = P.ok;
+        if (out_n_flow) out_n_flow[done] = nf;
+        if (out_n_los) out_n_los[done] = nl;
+        if (nf == 0 && nl == 0) continue;
+        ctx->goal_batch.valid = false;          // the staging buffer is about to be reused
+        // slots for everything this request writes (and the previous-chunk LOS fields it reads), all or nothing
+        std::vector<size_t> keys;
+        for (int i = 0; i < nf; i++) keys.push_back(row + E.fc[i]);
+        for (int i = 0; i < nl; i++) keys.push_back(row + E.lc[i]);
+        for (int i = 0; i < nl; i++)
+            if (E.lr[i].prev_index == -2) keys.push_back(row + E.lr[i].prev_chunk_r * cw + E.lr[i].prev_chunk_c);
+        std::vector<int32_t> slots(keys.size());
+        bool evicted = false;
+        rc = pf_pool_reserve(ctx, keys.data(), keys.size(), slots.data(), &evicted);
+        if (rc) break;
+        any_evicted |= evicted;
+        row_touched[dest] = 1;
+        if (evicted) {
+            // a slot this segment writes or reads now belongs to another (dest, chunk): launch the segment first, so
+            // that its writes and reads stay ordered before this request's
+            bool moved = false;
+            for (const auto &u : S.used) moved |= ctx->h_slot_owner[u.first] != (int64_t)u.second;
+            if (moved) { rc = launch_segment(ctx, st, S); if (rc) return rc; S.clear(); }
+        }
+        for (size_t k = 0; k < keys.size(); k++) S.used.push_back({slots[k], keys[k]});
+        for (int i = 0; i < nf; i++) {
+            const int32_t s = slots[i];
+            ctx->h_pool_has[s] |= 1;
+            ctx->h_pool_ffid[row + E.fc[i]] = E.fid[i];
+            ctx->h_pool_req[s] = E.fr[i];
+            S.fr.push_back(E.fr[i]); S.fs.push_back(s); S.fw.push_back(S.writes[s]++);
+        }
+        const int l0 = (int)S.lr.size();
+        for (int i = 0; i < nl; i++) {
+            const int32_t s = slots[nf + i];
+            ctx->h_pool_has[s] |= 2;
+            pfnav_los_req q = E.lr[i];
+            int depth = 0;
+            if (q.prev_index >= 0) { q.prev_index += l0; depth = S.ld[q.prev_index] + 1; }
+            else if (q.prev_index == -2) {
+                const size_t pkey = row + q.prev_chunk_r * cw + q.prev_chunk_c;
+                auto it = S.los_at.find(pkey);
+                if (it != S.los_at.end()) { q.prev_index = it->second; depth = S.ld[it->second] + 1; }   // built earlier in this segment
+                else q._pad = ctx->h_pool_slot[pkey];                                                      // absolute pool slot of prev_los
+            }
+            S.los_at[row + E.lc[i]] = (int)S.lr.size();
+            S.lr.push_back(q); S.ls.push_back(s); S.ld.push_back(depth);
+        }
+    }
+    int lrc = launch_segment(ctx, st, S);
+    if (lrc) return lrc;
+    if (any_evicted)      // entries of other destinations lost their slots
+        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st));
+    else
+        for (int d = 0; d < ctx->pool_ndests; d++)
+            if (row_touched[d])
+                PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot + (size_t)d * chunks, ctx->h_pool_slot.data() + (size_t)d * chunks,
+                                        (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
+    bool any_touched = any_evicted;
+    for (uint8_t t : row_touched) any_touched |= t != 0;
+    if (any_touched)
+        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
+                                cudaMemcpyHostToDevice, st));
+    if (out_ndone) *out_ndone = done;
+    return rc;
+}
+
+// N_RequestPath (nav.c:3386) for a batch of requests on one layer against the device field pool (pfnav.h).
+extern "C" int pfnav_pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *dests, int layer, const float *src_xz,
+                                        const float *dst_xz, void *stream, uint32_t *out_dest_ids, int32_t *out_ok,
+                                        int32_t *out_n_flow, int32_t *out_n_los, int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_ARG(n >= 0 && (n == 0 || (dests && src_xz && dst_xz)), "n / null arrays");
+    PF_ARG(route_layer(ctx, layer), "pfnav_route_build not called");
+    for (int i = 0; i < n; i++) {
+        tdesc t;
+        PF_ARG(dests[i] >= 0, "dest");
+        PF_ARG(desc_for_point(ctx, src_xz[2 * i], src_xz[2 * i + 1], &t) && desc_for_point(ctx, dst_xz[2 * i], dst_xz[2 * i + 1], &t),
+               "position outside the map");
+    }
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_pool_slot, "pool not created");
+    for (int i = 0; i < n; i++) PF_ARG(dests[i] < ctx->pool_ndests, "dest");
+    if (n == 0) return PFNAV_OK;
+    return pool_request_paths(ctx, n, dests, layer, src_xz, dst_xz, stream, out_dest_ids, out_ok, out_n_flow, out_n_los, out_ndone);
+}
+
+// N_RequestPath (nav.c:3386) against the device field pool: route src -> dst exactly as the reference
+// does, then build only the fields the pool does not hold yet, in place, on the device. The one-request batch.
+extern "C" int pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, float src_x, float src_z, float dst_x,
+                                       float dst_z, void *stream, uint32_t *out_dest_id, int *out_ok, int *out_n_flow,
+                                       int *out_n_los)
+{
+    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
+    PF_ARG(route_layer(ctx, layer), "pfnav_route_build not called");
+    const float s[2] = {src_x, src_z}, d[2] = {dst_x, dst_z};
+    tdesc t;
+    PF_ARG(desc_for_point(ctx, src_x, src_z, &t) && desc_for_point(ctx, dst_x, dst_z, &t), "position outside the map");
+    uint32_t did = 0;
+    int32_t ok = 0, nf = 0, nl = 0;
+    int ndone = 0;
+    const int rc = pool_request_paths(ctx, 1, &dest, layer, s, d, stream, &did, &ok, &nf, &nl, &ndone);
+    if (out_dest_id) *out_dest_id = did;
+    if (out_ok) *out_ok = ok;
+    if (out_n_flow) *out_n_flow = nf;
+    if (out_n_los) *out_n_los = nl;
     return rc;
 }
 
@@ -1077,14 +1318,17 @@ extern "C" int pfnav_route_arrival_consts(pfnav_ctx *ctx, int layer, float tx, f
 }
 
 // ------------------------------------------------------------------------------------------
-// Device-side AStar_PortalGraphPath (a_star.c:429; SURVEY 8f-2): a batch of portal-graph searches, one thread per
-// search. The search itself is the reference's, statement for statement -- N_ClosestPathableLocalIsland (nav.c:5131)
-// for both ends, N_PortalReachableFromTile (:4852) + the travel-cost index for the start portals,
-// neighbours_portal_graph (a_star.c:212), portal_node_penalty (:298), and the 1-indexed binary heap of pqueue.h:109-208
-// whose tie order decides between equal-cost paths -- over device copies of the portal table, the intra-chunk edges with
-// their states, the travel-cost index and the local-island image. Per-search scratch (heap, cost / predecessor table,
-// flood queue) lives in HBM: 0.6 MB per search in flight, a few hundred searches per launch.
-// Not wired into pfnav_pool_request_path yet: the rest of n_request_path (fallback branches, field emission) is host code.
+// Device-side AStar_PortalGraphPath (a_star.c:429; SURVEY 8f-2): a batch of portal-graph searches, one warp per search.
+// The search itself is the reference's, statement for statement -- N_ClosestPathableLocalIsland (nav.c:5131) for both
+// ends, N_PortalReachableFromTile (:4852) + the travel-cost index for the start portals, neighbours_portal_graph
+// (a_star.c:212), portal_node_penalty (:298), and the 1-indexed binary heap of pqueue.h:109-208 whose tie order decides
+// between equal-cost paths -- over device copies of the portal table, the intra-chunk edges with their states, the
+// travel-cost index and the local-island image.
+// Heap pushes and pops, and the cost-table updates that decide them, stay in the reference's serial order on lane 0.
+// The lanes share what surrounds them: the start-portal tests, each expansion's edge tests (compacted in edge order
+// with ballots), the portal_connected_liids scan (an order-preserving dedupe with match / ballot) and the cost-table
+// lookups of the neighbours. The cost / predecessor table is stamped per launch instead of being cleared.
+// Per-search scratch (heap, cost / predecessor table, flood queue) lives in HBM.
 // ------------------------------------------------------------------------------------------
 namespace {
 
@@ -1100,17 +1344,21 @@ struct dev_route {
     int cw, chh, W64;
     float penalty;
 };
-#define GP_HT 8192                // cost / predecessor table slots (open addressing)
+#define GP_HT 16384               // cost / predecessor table slots (open addressing, at most 3/4 used)
 #define GP_PQ 16384               // heap capacity
+#define GP_WARPS 4                // searches per CTA
+#define GP_NONE (~0ull)           // no predecessor (a key never has its top bits set)
+struct gp_slot { uint64_t key, from; float cost; uint32_t stamp; };       // stamp != the launch's: free
 struct gp_scratch {
-    uint64_t hkey[GP_HT]; uint64_t hfrom[GP_HT]; float hcost[GP_HT];
+    gp_slot h[GP_HT];
     float pprio[GP_PQ]; uint64_t pdata[GP_PQ];
-    uint16_t queue[4096]; uint8_t visited[4096];
+    uint32_t visited[1024];       // 4096 flags
+    uint16_t queue[4096];
 };
 struct route_dev_state {
     dev_portal *d_ports = nullptr; int32_t *d_nports = nullptr, *d_port_base = nullptr; dev_edge *d_edges = nullptr;
     uint16_t *d_travel = nullptr; size_t travel_rows = 0, nedges = 0;
-    gp_scratch *d_scratch = nullptr; int scratch_n = 0;
+    gp_scratch *d_scratch = nullptr; int scratch_n = 0; uint32_t stamp = 0;
     void *d_req = nullptr, *d_out = nullptr; size_t req_bytes = 0, out_bytes = 0;
     int layer = -1; uint64_t epoch = ~0ull, generation = 0;
 };
@@ -1121,29 +1369,35 @@ __device__ __forceinline__ uint16_t gp_li(const dev_route &R, int chunk, int r, 
 }
 __device__ __forceinline__ uint64_t gp_key(int chunk, int pi, uint16_t liid) { return ((uint64_t)liid << 32) | ((uint64_t)chunk << 8) | (uint64_t)pi; }
 
-// N_ClosestPathableLocalIsland (nav.c:5131)
-__device__ uint16_t gp_closest_liid(const dev_route &R, gp_scratch &S, int chunk, int tr, int tc)
+// N_ClosestPathableLocalIsland (nav.c:5131). The flood returns the first island tile in the serial queue order, so it
+// stays on lane 0; the lanes clear its visited flags.
+__device__ uint16_t gp_closest_liid(const dev_route &R, gp_scratch &S, int chunk, int tr, int tc, int lane)
 {
     const uint16_t own = gp_li(R, chunk, tr, tc);
     if (own != 0xffff) return own;
-    for (int i = 0; i < 4096; i++) S.visited[i] = 0;
-    int head = 0, tail = 0;
-    S.queue[tail++] = (uint16_t)(tr * 64 + tc);
-    S.visited[tr * 64 + tc] = 1;
-    while (head < tail) {
-        const int cur = S.queue[head++], r = cur >> 6, c = cur & 63;
-        const int dr[4] = {0, 0, -1, 1}, dc[4] = {-1, 1, 0, 0};
-        for (int e = 0; e < 4; e++) {
-            const int nr = r + dr[e], nc = c + dc[e];
-            if (nr < 0 || nr >= 64 || nc < 0 || nc >= 64) continue;
-            if (S.visited[nr * 64 + nc]) continue;
-            const uint16_t l = gp_li(R, chunk, nr, nc);
-            if (l != 0xffff) return l;
-            S.visited[nr * 64 + nc] = 1;
-            S.queue[tail++] = (uint16_t)(nr * 64 + nc);
+    for (int i = lane; i < 1024; i += 32) S.visited[i] = 0;
+    __syncwarp();
+    uint16_t found = 0xffff;
+    if (lane == 0) {
+        uint8_t *vis = (uint8_t *)S.visited;
+        int head = 0, tail = 0;
+        S.queue[tail++] = (uint16_t)(tr * 64 + tc);
+        vis[tr * 64 + tc] = 1;
+        while (head < tail && found == 0xffff) {
+            const int cur = S.queue[head++], r = cur >> 6, c = cur & 63;
+            const int dr[4] = {0, 0, -1, 1}, dc[4] = {-1, 1, 0, 0};
+            for (int e = 0; e < 4; e++) {
+                const int nr = r + dr[e], nc = c + dc[e];
+                if (nr < 0 || nr >= 64 || nc < 0 || nc >= 64) continue;
+                if (vis[nr * 64 + nc]) continue;
+                const uint16_t l = gp_li(R, chunk, nr, nc);
+                if (l != 0xffff) { found = l; break; }
+                vis[nr * 64 + nc] = 1;
+                S.queue[tail++] = (uint16_t)(nr * 64 + nc);
+            }
         }
     }
-    return 0xffff;
+    return (uint16_t)__shfl_sync(0xffffffffu, (int)found, 0);
 }
 
 // N_PortalReachableFromTile (nav.c:4852)
@@ -1162,10 +1416,10 @@ __device__ bool gp_portal_reachable(const dev_route &R, int chunk, const dev_por
     return false;
 }
 
-__device__ __forceinline__ int gp_find(const gp_scratch &S, uint64_t key)       // slot of key, or of the first free slot
+__device__ __forceinline__ int gp_find(const gp_scratch &S, uint64_t key, uint32_t stamp)   // slot of key, or the first free one
 {
-    uint32_t h = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> 51) & (GP_HT - 1);
-    while (S.hkey[h] != 0 && S.hkey[h] != key) h = (h + 1) & (GP_HT - 1);
+    uint32_t h = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> 50) & (GP_HT - 1);
+    while (S.h[h].stamp == stamp && S.h[h].key != key) h = (h + 1) & (GP_HT - 1);
     return (int)h;
 }
 // pq push / pop: pqueue.h:165-208 (strict comparisons, hole sift)
@@ -1199,97 +1453,156 @@ __device__ __forceinline__ uint64_t gp_pop(gp_scratch &S, int &size)
 
 // req: {start chunk, start tile_r, start tile_c, end chunk, end tile_r, end tile_c, finish chunk, finish portal}
 // out (per search, 4 + 3 * max_hops ints): {status (1 found, 0 none, -1 scratch overflow), nhops, cost bits, 0, hops (chunk, portal, liid)...}
-__global__ void k_portal_graph_path(dev_route R, const int32_t *__restrict__ req, int n, gp_scratch *scratch, int32_t *out, int max_hops)
+// stamp: nonzero, different from every earlier launch over the same scratch.
+__global__ void __launch_bounds__(GP_WARPS * 32) k_portal_graph_path_warp(dev_route R, const int32_t *__restrict__ req, int n,
+                                                                         gp_scratch *scratch, int32_t *out, int max_hops, uint32_t stamp)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned FULL = 0xffffffffu;
+    __shared__ uint64_t s_key[GP_WARPS][256];       // this expansion's neighbours, in neighbours_portal_graph's order
+    __shared__ float s_cost[GP_WARPS][256];         // edge cost, then the relaxed cost (< 0: no update)
+    __shared__ int32_t s_slot[GP_WARPS][256];       // the neighbour's table slot when it holds the key, else -1
+    __shared__ uint16_t s_conn[GP_WARPS][256];      // portal_connected_liids
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int i = blockIdx.x * GP_WARPS + w;
     if (i >= n) return;
     gp_scratch &S = scratch[i];
     const int32_t *q = req + (size_t)i * 8;
     int32_t *o = out + (size_t)i * (4 + 3 * max_hops);
-    o[0] = 0; o[1] = 0; o[2] = 0; o[3] = 0;
+    if (lane < 4) o[lane] = 0;
     const int bchunk = q[0], echunk = q[3], fin_chunk = q[6], fin_pi = q[7];
-    const uint16_t start_liid = gp_closest_liid(R, S, bchunk, q[1], q[2]);
+    const uint16_t start_liid = gp_closest_liid(R, S, bchunk, q[1], q[2], lane);
     if (start_liid == 0xffff) return;
-    const uint16_t end_liid = gp_closest_liid(R, S, echunk, q[4], q[5]);
+    const uint16_t end_liid = gp_closest_liid(R, S, echunk, q[4], q[5], lane);
     if (end_liid == 0xffff) return;
-    for (int k = 0; k < GP_HT; k++) S.hkey[k] = 0;
-    int size = 0, nkeys = 0;
-    bool overflow = false;
-    for (int p = 0; p < R.nports[bchunk]; p++) {
-        const dev_portal &P = R.ports[bchunk * 64 + p];
-        if (!gp_portal_reachable(R, bchunk, P, q[1], q[2])) continue;
-        const uint16_t t = R.travel[(size_t)(R.port_base[bchunk] + p) * 4096 + q[1] * 64 + q[2]];
-        if (t == 0xffff) continue;
-        const float cost = (float)t / 8;
-        const uint64_t key = gp_key(bchunk, p, start_liid);
-        const int s = gp_find(S, key);
-        if (S.hkey[s] == 0) { S.hkey[s] = key; S.hfrom[s] = 0; nkeys++; }
-        S.hcost[s] = cost;
-        overflow |= !gp_push(S, size, cost, key);
+    // start portals: reachability and travel cost on the lanes, pushed in portal order
+    const int np = R.nports[bchunk];
+    for (int p = lane; p < np; p += 32) {
+        const dev_portal P = R.ports[bchunk * 64 + p];
+        float c = -1.0f;
+        if (gp_portal_reachable(R, bchunk, P, q[1], q[2])) {
+            const uint16_t t = R.travel[(size_t)(R.port_base[bchunk] + p) * 4096 + q[1] * 64 + q[2]];
+            if (t != 0xffff) c = (float)t / 8;
+        }
+        s_cost[w][p] = c;
     }
+    __syncwarp();
+    int size = 0, nkeys = 0;          // lane 0's
+    bool overflow = false;
+    if (lane == 0)
+        for (int p = 0; p < np; p++) {
+            const float cost = s_cost[w][p];
+            if (cost < 0.0f) continue;
+            const uint64_t key = gp_key(bchunk, p, start_liid);
+            const int s = gp_find(S, key, stamp);
+            if (S.h[s].stamp != stamp) { S.h[s].stamp = stamp; S.h[s].key = key; S.h[s].from = GP_NONE; nkeys++; }
+            S.h[s].cost = cost;
+            overflow |= !gp_push(S, size, cost, key);
+        }
     const uint64_t last = gp_key(fin_chunk, fin_pi, end_liid);
-    while (size > 0 && !overflow) {
-        const uint64_t cur = gp_pop(S, size);
-        if (cur == last) break;
+    while (true) {
+        uint64_t cur = 0;
+        int go = 0;
+        if (lane == 0 && size > 0 && !overflow) { cur = gp_pop(S, size); go = cur != last; }
+        if (!__shfl_sync(FULL, go, 0)) break;
+        cur = __shfl_sync(FULL, cur, 0);
         const int cchunk = (int)((cur >> 8) & 0xffffff), cpi = (int)(cur & 0xff);
         const uint16_t cli = (uint16_t)(cur >> 32);
-        const float base = S.hcost[gp_find(S, cur)];
-        auto relax = [&](uint64_t nk, float step) {
-            const float new_cost = base + step + R.penalty;
-            const int s = gp_find(S, nk);
-            if (S.hkey[s] == 0) {
-                if (nkeys + 1 >= GP_HT * 3 / 4) { overflow = true; return; }
-                S.hkey[s] = nk; nkeys++;
-            } else if (!(new_cost < S.hcost[s])) return;
-            S.hcost[s] = new_cost; S.hfrom[s] = cur;
-            overflow |= !gp_push(S, size, new_cost, nk);
-        };
+        const dev_portal P = R.ports[cchunk * 64 + cpi];
         // neighbours_portal_graph (a_star.c:212): the chunk's own portals over active edges whose portal touches the island ...
-        const dev_portal &P = R.ports[cchunk * 64 + cpi];
         int nout = 0;
-        for (int e = 0; e < P.edge_cnt && nout < 256; e++) {
-            const dev_edge E = R.edges[P.edge_off + e];
-            if (E.es == 1) continue;
-            const dev_portal &NP = R.ports[cchunk * 64 + E.nb];
-            bool reach = false;
-            for (int r = NP.r0; r <= NP.r1 && !reach; r++)
-                for (int c = NP.c0; c <= NP.c1; c++)
-                    if (gp_li(R, cchunk, r, c) == cli) { reach = true; break; }
-            if (!reach) continue;
-            relax(gp_key(cchunk, E.nb, cli), E.cost);
-            nout++;
-        }
-        // ... then the islands of the connected chunk that touch this one across the portal (portal_connected_liids, :151)
-        const dev_portal &C = R.ports[P.conn_chunk * 64 + P.conn_idx];
-        uint16_t conn_liids[256];
-        int nconn = 0;
-        bool full = false;
-        for (int r1 = P.r0; r1 <= P.r1 && !full; r1++)
-            for (int c1 = P.c0; c1 <= P.c1 && !full; c1++) {
-                if (gp_li(R, cchunk, r1, c1) != cli) continue;
-                const int ar = P.chunk_r * 64 + r1, ac = P.chunk_c * 64 + c1;
-                const int cand[4][2] = {{ar - 1, ac}, {ar, ac - 1}, {ar, ac + 1}, {ar + 1, ac}};
-                for (int k = 0; k < 4; k++) {
-                    const int r2 = cand[k][0] - C.chunk_r * 64, c2 = cand[k][1] - C.chunk_c * 64;
-                    if (r2 < C.r0 || r2 > C.r1 || c2 < C.c0 || c2 > C.c1) continue;
-                    if (nconn == 256) { full = true; break; }
-                    const uint16_t nl = gp_li(R, P.conn_chunk, r2, c2);
-                    bool contains = false;
-                    for (int j = 0; j < nconn; j++) if (conn_liids[j] == nl) { contains = true; break; }
-                    if (!contains && nl != 0xffff) conn_liids[nconn++] = nl;
+        for (int e0 = 0; e0 < P.edge_cnt && nout < 256; e0 += 32) {
+            const int e = e0 + lane;
+            bool acc = false;
+            dev_edge E = {0, 1, 0.0f};
+            if (e < P.edge_cnt) {
+                E = R.edges[P.edge_off + e];
+                if (E.es != 1) {
+                    const dev_portal NP = R.ports[cchunk * 64 + E.nb];
+                    for (int r = NP.r0; r <= NP.r1 && !acc; r++)
+                        for (int c = NP.c0; c <= NP.c1; c++)
+                            if (gp_li(R, cchunk, r, c) == cli) { acc = true; break; }
                 }
             }
-        for (int j = 0; j < nconn && nout < 256; j++, nout++) relax(gp_key(P.conn_chunk, P.conn_idx, conn_liids[j]), 1.0f);
+            const unsigned m = __ballot_sync(FULL, acc);
+            const int pos = nout + __popc(m & ((1u << lane) - 1));
+            if (acc && pos < 256) { s_key[w][pos] = gp_key(cchunk, E.nb, cli); s_cost[w][pos] = E.cost; }
+            nout = min(256, nout + __popc(m));
+        }
+        // ... then the islands of the connected chunk that touch this one across the portal (portal_connected_liids, :151):
+        // candidates (portal tile on the island, row-major) x (its four neighbours, in order) inside the connected portal
+        if (nout < 256) {
+            const dev_portal C = R.ports[P.conn_chunk * 64 + P.conn_idx];
+            const int pw = P.c1 - P.c0 + 1, ncand = pw * (P.r1 - P.r0 + 1) * 4;
+            int nconn = 0;
+            for (int t0 = 0; t0 < ncand && nconn < 256; t0 += 32) {
+                const int t = t0 + lane;
+                bool valid = false;
+                uint16_t nl = 0xffff;
+                if (t < ncand) {
+                    const int tile = t >> 2, k = t & 3, r1 = P.r0 + tile / pw, c1 = P.c0 + tile % pw;
+                    if (gp_li(R, cchunk, r1, c1) == cli) {
+                        const int ar = P.chunk_r * 64 + r1 + (k == 0 ? -1 : k == 3 ? 1 : 0);
+                        const int ac = P.chunk_c * 64 + c1 + (k == 1 ? -1 : k == 2 ? 1 : 0);
+                        const int r2 = ar - C.chunk_r * 64, c2 = ac - C.chunk_c * 64;
+                        if (r2 >= C.r0 && r2 <= C.r1 && c2 >= C.c0 && c2 <= C.c1) {
+                            nl = gp_li(R, P.conn_chunk, r2, c2);
+                            valid = nl != 0xffff;
+                        }
+                    }
+                }
+                // new: valid, first of its id in this round, and not listed by an earlier round
+                const unsigned same = __match_any_sync(FULL, valid ? (unsigned)nl : 0x10000u + lane);
+                bool fresh = valid && (same & ((1u << lane) - 1)) == 0;
+                for (int j = 0; j < nconn && fresh; j++) if (s_conn[w][j] == nl) fresh = false;
+                const unsigned m = __ballot_sync(FULL, fresh);
+                const int pos = nconn + __popc(m & ((1u << lane) - 1));
+                if (fresh && pos < 256) s_conn[w][pos] = nl;
+                nconn = min(256, nconn + __popc(m));
+                __syncwarp();
+            }
+            for (int j = lane; j < nconn && nout + j < 256; j += 32) {
+                s_key[w][nout + j] = gp_key(P.conn_chunk, P.conn_idx, s_conn[w][j]);
+                s_cost[w][nout + j] = 1.0f;
+            }
+            nout = min(256, nout + nconn);
+        }
+        __syncwarp();
+        // the neighbours' keys are distinct: look them up on the lanes, then relax in order on lane 0
+        const float base = S.h[gp_find(S, cur, stamp)].cost;
+        for (int j = lane; j < nout; j += 32) {
+            const float new_cost = base + s_cost[w][j] + R.penalty;
+            const int s = gp_find(S, s_key[w][j], stamp);
+            const bool held = S.h[s].stamp == stamp;
+            s_slot[w][j] = held ? s : -1;
+            s_cost[w][j] = (!held || new_cost < S.h[s].cost) ? new_cost : -1.0f;
+        }
+        __syncwarp();
+        if (lane == 0)
+            for (int j = 0; j < nout && !overflow; j++) {
+                const float new_cost = s_cost[w][j];
+                if (new_cost < 0.0f) continue;
+                const uint64_t nk = s_key[w][j];
+                int s = s_slot[w][j];
+                if (s < 0) {
+                    if (nkeys + 1 >= GP_HT * 3 / 4) { overflow = true; break; }
+                    s = gp_find(S, nk, stamp);
+                    S.h[s].stamp = stamp; S.h[s].key = nk; nkeys++;
+                }
+                S.h[s].cost = new_cost; S.h[s].from = cur;
+                overflow |= !gp_push(S, size, new_cost, nk);
+            }
+        __syncwarp();
     }
+    if (lane != 0) return;
     if (overflow) { o[0] = -1; return; }
-    const int ls = gp_find(S, last);
-    if (S.hkey[ls] == 0 || S.hfrom[ls] == 0) return;       // came_from holds no entry for the finish node
+    const int ls = gp_find(S, last, stamp);
+    if (S.h[ls].stamp != stamp || S.h[ls].from == GP_NONE) return;       // came_from holds no entry for the finish node
     int nh = 0;
-    for (uint64_t cur = last; cur != 0; cur = S.hfrom[gp_find(S, cur)]) nh++;
-    o[1] = nh; o[2] = __float_as_int(S.hcost[ls]);
+    for (uint64_t cur = last; cur != GP_NONE; cur = S.h[gp_find(S, cur, stamp)].from) nh++;
+    o[1] = nh; o[2] = __float_as_int(S.h[ls].cost);
     if (nh > max_hops) { o[0] = -1; return; }
     int k = nh;
-    for (uint64_t cur = last; cur != 0; cur = S.hfrom[gp_find(S, cur)]) {
+    for (uint64_t cur = last; cur != GP_NONE; cur = S.h[gp_find(S, cur, stamp)].from) {
         k--;
         o[4 + 3 * k] = (int)((cur >> 8) & 0xffffff); o[4 + 3 * k + 1] = (int)(cur & 0xff); o[4 + 3 * k + 2] = (int)(cur >> 32);
     }
@@ -1367,11 +1680,51 @@ static int route_dev_sync(pfnav_ctx *ctx, int layer, pfnav_route_layer &RL, rout
     return 0;
 }
 
+// n portal-graph searches on the device (k_portal_graph_path_warp), in the layout of pfnav_route_graph_paths. The host
+// edge states must be current; the local islands are the device image, which pfnav_map_commit keeps equal to the host's.
+static int route_dev_search(pfnav_ctx *ctx, int layer, pfnav_route_layer &RL, const int32_t *req, int n, int32_t *out, int max_hops)
+{
+    PF_CUDA(cudaSetDevice(ctx->device));
+    route_dev_state *D = route_dev(ctx);
+    D->epoch = ~0ull;                                                                  // edge states were just refreshed
+    if (route_dev_sync(ctx, layer, RL, D)) return PFNAV_ERR_CUDA;
+    const size_t ostride = 4 + 3 * (size_t)max_hops;
+    const int batch = 4096;                                                            // 588 KB of scratch per search in flight
+    const int want = std::min(std::max(n, 1), batch);
+    if (D->scratch_n < want) {
+        cudaFree(D->d_scratch); D->d_scratch = nullptr; D->scratch_n = 0;
+        PF_CUDA(cudaMalloc(&D->d_scratch, (size_t)want * sizeof(gp_scratch)));
+        PF_CUDA(cudaMemset(D->d_scratch, 0, (size_t)want * sizeof(gp_scratch)));     // no slot carries a stamp yet
+        D->scratch_n = want; D->stamp = 0;
+    }
+    if (D->req_bytes < (size_t)batch * 32) { cudaFree(D->d_req); PF_CUDA(cudaMalloc(&D->d_req, (size_t)batch * 32)); D->req_bytes = (size_t)batch * 32; }
+    if (D->out_bytes < (size_t)batch * ostride * 4) { cudaFree(D->d_out); PF_CUDA(cudaMalloc(&D->d_out, (size_t)batch * ostride * 4)); D->out_bytes = (size_t)batch * ostride * 4; }
+    dev_route R;
+    R.ports = D->d_ports; R.nports = D->d_nports; R.port_base = D->d_port_base; R.edges = D->d_edges; R.travel = D->d_travel;
+    R.liid = ctx->d_liid + (size_t)ctx->W64 * ctx->H64 * layer; R.cw = ctx->chunk_w; R.chh = ctx->chunk_h; R.W64 = ctx->W64;
+    R.penalty = (float)sqrt(pow(64, 2.0f) + pow(64, 2.0f));                          // portal_node_penalty (a_star.c:298)
+    PF_CUDA(cudaDeviceSynchronize());
+    for (int b0 = 0; b0 < n; b0 += batch) {
+        const int nb = std::min(batch, n - b0);
+        if (++D->stamp == 0) {                                                         // the stamps wrapped: start the tables over
+            PF_CUDA(cudaMemset(D->d_scratch, 0, (size_t)D->scratch_n * sizeof(gp_scratch)));
+            D->stamp = 1;
+        }
+        PF_CUDA(cudaMemcpy(D->d_req, req + (size_t)b0 * 8, (size_t)nb * 32, cudaMemcpyHostToDevice));
+        k_portal_graph_path_warp<<<(nb + GP_WARPS - 1) / GP_WARPS, GP_WARPS * 32>>>(R, (const int32_t *)D->d_req, nb, D->d_scratch,
+                                                                                  (int32_t *)D->d_out, max_hops, D->stamp);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+        PF_CUDA(cudaMemcpy(out + (size_t)b0 * ostride, D->d_out, (size_t)nb * ostride * 4, cudaMemcpyDeviceToHost));
+    }
+    return PFNAV_OK;
+}
+
 // AStar_PortalGraphPath for n searches. req: 8 ints per search {start chunk index, start tile r, c, end chunk index, end tile
 // r, c, finish chunk index, finish portal index}; out: (4 + 3 * max_hops) ints per search {status, nhops, cost (float
 // bits), 0, then (chunk, portal, local island) per hop, start to finish}; status 1 = path, 0 = none, -1 = the search
-// outgrew its scratch (heap 16 k entries / 6 k nodes) or max_hops. on_device != 0: the kernel; 0: the host planner's own
-// routine (what pfnav_route_request_path runs), for comparison.
+// outgrew its scratch (heap 16 k entries / 12 k nodes) or max_hops. on_device != 0: the kernel (k_portal_graph_path_warp);
+// 0: the host planner's own routine (what pfnav_route_request_path runs) on host threads, for comparison.
 extern "C" int pfnav_route_graph_paths(pfnav_ctx *ctx, int layer, const int32_t *req, int n, int32_t *out, int max_hops, int on_device)
 {
     PF_ARG(ctx && req && out && n >= 0 && max_hops > 0, "args");
@@ -1388,48 +1741,24 @@ extern "C" int pfnav_route_graph_paths(pfnav_ctx *ctx, int layer, const int32_t 
     if (!on_device) {
         Router R{ctx, *prl, layer, cw, ctx->chunk_h};
         for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, *prl, layer, ch);
-        for (int i = 0; i < n; i++) {
+        parallel_for(n, [&](int i) {          // on host threads, as a batch's search round below the device threshold
             const int32_t *q = req + (size_t)i * 8;
             int32_t *o = out + (size_t)i * ostride;
             memset(o, 0, ostride * 4);
             std::vector<Router::hop> path;
             float cost = 0.0f;
             const tdesc s = {q[0] / cw, q[0] % cw, q[1], q[2]}, e = {q[3] / cw, q[3] % cw, q[4], q[5]};
-            if (!R.portal_graph_path(s, e, q[6], q[7], path, &cost)) continue;
+            if (!R.portal_graph_path(s, e, q[6], q[7], path, &cost)) return;
             o[1] = (int32_t)path.size(); memcpy(&o[2], &cost, 4);
-            if ((int)path.size() > max_hops) { o[0] = -1; continue; }
+            if ((int)path.size() > max_hops) { o[0] = -1; return; }
             for (size_t k = 0; k < path.size(); k++) { o[4 + 3 * k] = path[k].chunk; o[4 + 3 * k + 1] = path[k].pi; o[4 + 3 * k + 2] = path[k].liid; }
             o[0] = 1;
-        }
+        });
         return PFNAV_OK;
     }
     PF_NEED_DEVICE(ctx);
     PF_CUDA(cudaSetDevice(ctx->device));
     { int rc = pfnav_blockers_flush(ctx); if (rc) return rc; }
     for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, *prl, layer, ch);      // n_update_all_edge_states (nav.c:1787)
-    route_dev_state *D = route_dev(ctx);
-    D->epoch = ~0ull;                                                                  // edge states were just refreshed
-    if (route_dev_sync(ctx, layer, *prl, D)) return PFNAV_ERR_CUDA;
-    const int batch = 4096;                                                            // 364 KB of scratch per search in flight
-    if (D->scratch_n < std::min(n, batch)) {
-        cudaFree(D->d_scratch); D->d_scratch = nullptr;
-        PF_CUDA(cudaMalloc(&D->d_scratch, (size_t)std::min(std::max(n, 1), batch) * sizeof(gp_scratch)));
-        D->scratch_n = std::min(std::max(n, 1), batch);
-    }
-    if (D->req_bytes < (size_t)batch * 32) { cudaFree(D->d_req); PF_CUDA(cudaMalloc(&D->d_req, (size_t)batch * 32)); D->req_bytes = (size_t)batch * 32; }
-    if (D->out_bytes < (size_t)batch * ostride * 4) { cudaFree(D->d_out); PF_CUDA(cudaMalloc(&D->d_out, (size_t)batch * ostride * 4)); D->out_bytes = (size_t)batch * ostride * 4; }
-    dev_route R;
-    R.ports = D->d_ports; R.nports = D->d_nports; R.port_base = D->d_port_base; R.edges = D->d_edges; R.travel = D->d_travel;
-    R.liid = ctx->d_liid + (size_t)ctx->W64 * ctx->H64 * layer; R.cw = cw; R.chh = ctx->chunk_h; R.W64 = ctx->W64;
-    R.penalty = (float)sqrt(pow(64, 2.0f) + pow(64, 2.0f));                          // portal_node_penalty (a_star.c:298)
-    PF_CUDA(cudaDeviceSynchronize());
-    for (int b0 = 0; b0 < n; b0 += batch) {
-        const int nb = std::min(batch, n - b0);
-        PF_CUDA(cudaMemcpy(D->d_req, req + (size_t)b0 * 8, (size_t)nb * 32, cudaMemcpyHostToDevice));
-        k_portal_graph_path<<<(nb + 31) / 32, 32>>>(R, (const int32_t *)D->d_req, nb, D->d_scratch, (int32_t *)D->d_out, max_hops);
-        ctx->launches++;
-        PF_CUDA(cudaGetLastError());
-        PF_CUDA(cudaMemcpy(out + (size_t)b0 * ostride, D->d_out, (size_t)nb * ostride * 4, cudaMemcpyDeviceToHost));
-    }
-    return PFNAV_OK;
+    return route_dev_search(ctx, layer, *prl, req, n, out, max_hops);
 }
