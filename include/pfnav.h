@@ -311,6 +311,8 @@ int  pfnav_pool_create(pfnav_ctx *ctx, int ndests, int max_fields);
 /* Store field bytes (HOST, 4096 each; either may be NULL) for (dest, chunk). */
 int  pfnav_pool_put(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c,
                     const uint8_t *flow_field, const uint8_t *los_field);
+/* Empty the pool. Does not block and queues no device work: the host mirrors are reset now, the device copies by the
+ * next entry point that uses the pool, ordered on that call's stream. */
 int  pfnav_pool_clear(pfnav_ctx *ctx);
 /* N_RequestPath's field-building half (nav.c:1819-2042), resident on the device: plan the goal
  * (pfnav_plan_goal), then run the flow waves and the LOS chain straight into the pool slots of
@@ -720,6 +722,11 @@ int  pfnav_agents_rebuild_index(pfnav_ctx *ctx, void *stream);
  * 5 agent velocity (ClearPath). */
 int  pfnav_profile_enable(pfnav_ctx *ctx, int enable);
 int  pfnav_profile_read(pfnav_ctx *ctx, float *ms_out, uint32_t *count_out);
+/* Host wall-clock time of the cold goal-batch path, recorded while profiling is enabled, summed since the last
+ * read and reset by it: ms_out / count_out have 8 entries: 0 pfnav_pool_clear, 1 waits on events and streams,
+ * 2 goal planning, 3 merge and dependency sort, 4 pool slot reservation, 5 packing of the plan, 6 H2D enqueue,
+ * 7 kernel launches (segments of pfnav_pool_request_goals_ex unless noted). */
+int  pfnav_profile_read_host(pfnav_ctx *ctx, double *ms_out, uint32_t *count_out);
 
 /* Number of kernels launched by this context since creation (bench `gpu_launches`). */
 uint64_t pfnav_launch_count(const pfnav_ctx *ctx);

@@ -101,6 +101,7 @@ SYMBOLS = [
     "pfnav_pool_request_goals_ex", "pfnav_blockers_batch", "pfnav_map_set_pos",
     "pfnav_agents_upload_formation", "pfnav_agents_upload_movestate_ext", "pfnav_pool_request_entity_fields",
     "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
+    "pfnav_profile_read_host",
 ]
 
 _lib = None
@@ -226,6 +227,7 @@ def load():
     L.pfnav_agents_rebuild_index.argtypes = [C.c_void_p, C.c_void_p]
     L.pfnav_profile_enable.argtypes = [C.c_void_p, C.c_int]
     L.pfnav_profile_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.pfnav_profile_read_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = L
     return L
 
@@ -815,6 +817,14 @@ class Nav:
         _chk(self.L.pfnav_profile_read(self.h, _p(ms), _p(cnt)))
         names = ["flow", "los", "index", "vdes", "cohesion", "velocity", "update", "apply"]
         return {n: (float(ms[i]), int(cnt[i])) for i, n in enumerate(names)}
+
+    HOST_SEGMENTS = ["clear", "wait", "plan", "merge", "reserve", "pack", "upload", "launch"]
+
+    def profile_read_host(self):
+        """host wall clock of pool_clear / pool_request_goals segments while profiling -> dict name -> (total_ms, count)"""
+        ms = np.zeros(8, np.float64); cnt = np.zeros(8, np.uint32)
+        _chk(self.L.pfnav_profile_read_host(self.h, _p(ms), _p(cnt)))
+        return {n: (float(ms[i]), int(cnt[i])) for i, n in enumerate(self.HOST_SEGMENTS)}
 
     def launch_count(self):
         return int(self.L.pfnav_launch_count(self.h))

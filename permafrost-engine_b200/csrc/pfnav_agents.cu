@@ -1819,26 +1819,26 @@ extern "C" int pfnav_pool_create(pfnav_ctx *ctx, int ndests, int max_fields)
     ctx->h_pool_req.assign(max_fields, pfnav_field_req{});
     ctx->h_pool_ffid.assign(nslots, 0);
     ctx->pool_ndests = ndests; ctx->pool_max = max_fields; ctx->pool_used = 0;
-    ctx->goal_batch.valid = false;
+    ctx->goal_batch.valid = false; ctx->pool_dev_stale = false;
     return PFNAV_OK;
 }
 
 extern "C" int pfnav_pool_clear(pfnav_ctx *ctx)
 {
     PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_fields_sync(ctx));
-    PF_CUDA(cudaMemset(ctx->d_pool_slot, 0xFF, ctx->h_pool_slot.size() * sizeof(int32_t)));
-    PF_CUDA(cudaMemset(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, 0, ctx->pool_max));
+    // host mirrors only: the device copies are reset by the next entry point that uses the pool, on its stream
+    // (pf_pool_refresh), so the clear neither waits for the GPU nor races a tick still reading the slot table
+    pf_host_timer ht(ctx);
     std::fill(ctx->h_pool_slot.begin(), ctx->h_pool_slot.end(), -1);
     std::fill(ctx->h_pool_has.begin(), ctx->h_pool_has.end(), 0);
     std::fill(ctx->h_pool_ffid.begin(), ctx->h_pool_ffid.end(), 0);
-    PF_CUDA(cudaMemset(ctx->d_pool_touch, 0, (size_t)ctx->pool_max * 4));
     std::fill(ctx->h_slot_touch.begin(), ctx->h_slot_touch.end(), 0);
     std::fill(ctx->h_slot_owner.begin(), ctx->h_slot_owner.end(), -1);
     ctx->pool_free.clear();
     ctx->goal_batch.valid = false;
     ctx->pool_used = 0;
+    ctx->pool_dev_stale = true;
+    ht.lap(PF_HPROF_CLEAR);
     return PFNAV_OK;
 }
 
@@ -1850,6 +1850,7 @@ extern "C" int pfnav_pool_put(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c
     PF_ARG(chunk_r >= 0 && chunk_r < ctx->chunk_h && chunk_c >= 0 && chunk_c < ctx->chunk_w, "chunk");
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
+    PF_CUDA(pf_pool_refresh_sync(ctx));
     const size_t si = (size_t)dest * ctx->chunk_w * ctx->chunk_h + chunk_r * ctx->chunk_w + chunk_c;
     int32_t slot = ctx->h_pool_slot[si];
     uint8_t *d_has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096;
@@ -2299,6 +2300,7 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
     pf_prof_scope prof(ctx, st, PF_PROF_VDES);
     if (flags & PFNAV_TICK_VDES_FROM_POOL) {
         PF_ARG(ctx->d_pool_slot, "PFNAV_TICK_VDES_FROM_POOL needs a field pool");
+        PF_CUDA(pf_pool_refresh(ctx, st));
         PoolView pv;
         pv.slot = ctx->d_pool_slot; pv.flow = ctx->d_pool_flow; pv.los = ctx->d_pool_los;
         pv.has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096; pv.ndests = ctx->pool_ndests;
@@ -3123,6 +3125,7 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
     cudaStream_t st = ctx->tick_stream;
+    PF_CUDA(pf_pool_refresh(ctx, st));
     PF_CUDA(cudaDeviceSynchronize());
     const int nwork = (int)ctx->n_work;
     const int chunks = ctx->chunk_w * ctx->chunk_h;

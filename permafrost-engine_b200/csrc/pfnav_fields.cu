@@ -1508,9 +1508,14 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
     if (!ctx) return;
     pfnav_route_forget(ctx);
     pfnav_blockers_forget(ctx);
+    pf_planner_destroy(ctx);
     if (ctx->device < 0) { delete ctx; return; }
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
+    for (int i = 0; i < 2; i++) {
+        cudaFreeHost(ctx->plan_host[i]);
+        if (ctx->plan_host_ev[i]) cudaEventDestroy(ctx->plan_host_ev[i]);
+    }
     pfnav_fields_free(ctx);
     pfnav_agents_free(ctx);
     if (ctx->tick_done) cudaEventDestroy(ctx->tick_done);
@@ -1547,6 +1552,16 @@ extern "C" int pfnav_profile_read(pfnav_ctx *ctx, float *ms_out, uint32_t *count
     }
     ctx->prof_pending.clear();
     cudaGetLastError();
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_profile_read_host(pfnav_ctx *ctx, double *ms_out, uint32_t *count_out)
+{
+    PF_ARG(ctx && ms_out && count_out, "args");
+    for (int i = 0; i < PF_HPROF_SLOTS; i++) {
+        ms_out[i] = ctx->host_ms[i]; count_out[i] = ctx->host_count[i];
+        ctx->host_ms[i] = 0.0; ctx->host_count[i] = 0;
+    }
     return PFNAV_OK;
 }
 

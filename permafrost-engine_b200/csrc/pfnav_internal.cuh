@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <chrono>
 #include <set>
 #include <string>
 #include <utility>
@@ -186,10 +187,21 @@ struct pfnav_ctx {
     bool vel_timed = false; float last_los_ms = -1.0f, last_vel_ms = -1.0f;
     bool los_inflight = false;
 
+    // pfnav_pool_clear resets the host mirrors only; the device slot table, `has` bytes and touch stamps are reset
+    // by the next entry point that uses the pool, ordered on its stream (pf_pool_refresh)
+    bool pool_dev_stale = false;
+    // cold goal batches: the plan is staged in a ring of two pinned buffers (event-guarded reuse) and the goals are
+    // planned on a persistent host thread pool with per-goal scratch (pfnav_plan.cu)
+    void *plan_host[2] = {nullptr, nullptr}; size_t plan_host_bytes[2] = {0, 0};
+    cudaEvent_t plan_host_ev[2] = {nullptr, nullptr}; int plan_host_next = 0;
+    void *planner = nullptr;
+
     // ---- optional per-kernel timing (pfnav_profile_enable) ----
     bool profiling = false;
     struct prof_rec { int slot; cudaEvent_t a, b; };
     std::vector<prof_rec> prof_pending;
+    // host wall-clock segments of pfnav_pool_clear / pfnav_pool_request_goals_ex (pfnav_profile_read_host)
+    double host_ms[8] = {0}; uint32_t host_count[8] = {0};
 };
 
 // Every entry point that takes a `void *stream`: NULL names the context's own non-blocking stream
@@ -216,6 +228,26 @@ static inline cudaError_t pf_fields_sync(pfnav_ctx *ctx)
     if (e == cudaSuccess) ctx->los_inflight = false;
     return e;
 }
+// Bring the device copies of the pool up to date after pfnav_pool_clear: empty slot table, no `has` bytes, zero touch
+// stamps, ordered on `st` after the forked field work (which may still write the pool). Every entry point that reads
+// or writes the device pool calls this first, on the stream it runs on.
+static inline cudaError_t pf_pool_refresh(pfnav_ctx *ctx, cudaStream_t st)
+{
+    if (!ctx->pool_dev_stale) return cudaSuccess;
+    cudaError_t e = pf_fields_join(ctx, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_pool_slot, 0xFF, ctx->h_pool_slot.size() * sizeof(int32_t), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, 0, ctx->pool_max, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_pool_touch, 0, (size_t)ctx->pool_max * 4, st);
+    if (e == cudaSuccess) ctx->pool_dev_stale = false;
+    return e;
+}
+// the same for entry points that go on with blocking copies (legacy default stream): wait for the reset
+static inline cudaError_t pf_pool_refresh_sync(pfnav_ctx *ctx)
+{
+    if (!ctx->pool_dev_stale) return cudaSuccess;
+    cudaError_t e = pf_pool_refresh(ctx, ctx->tick_stream);
+    return e == cudaSuccess ? cudaStreamSynchronize(ctx->tick_stream) : e;
+}
 
 // per (flock, layer) constants of arrived() (movement.c:2170), see pfnav_route.cu
 #define PF_ARRIVAL_MC_MAX 256           /* FIELD_RES_R*2 + FIELD_RES_C*2 (nav.c:4721) */
@@ -239,9 +271,29 @@ int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, st
 
 // pool slots with LRU eviction (pfnav_plan.cu)
 int pf_pool_reserve(pfnav_ctx *ctx, const size_t *keys, size_t n, int32_t *slots_out, bool *out_evicted);
+void pf_planner_destroy(pfnav_ctx *ctx);                         // pfnav_plan.cu: join the goal planner threads
 
 enum { PF_PROF_FLOW = 0, PF_PROF_LOS = 1, PF_PROF_INDEX = 2, PF_PROF_VDES = 3, PF_PROF_COHESION = 4,
        PF_PROF_VELOCITY = 5, PF_PROF_UPDATE = 6, PF_PROF_APPLY = 7, PF_PROF_SLOTS = 8 };
+
+// host segments of a cold goal batch (pfnav_profile_read_host): 0 pfnav_pool_clear, 1 waits on events / streams,
+// 2 planning, 3 merge + dependency sort, 4 pf_pool_reserve, 5 packing, 6 H2D enqueue, 7 kernel launches
+enum { PF_HPROF_CLEAR = 0, PF_HPROF_WAIT = 1, PF_HPROF_PLAN = 2, PF_HPROF_MERGE = 3, PF_HPROF_RESERVE = 4,
+       PF_HPROF_PACK = 5, PF_HPROF_UPLOAD = 6, PF_HPROF_LAUNCH = 7, PF_HPROF_SLOTS = 8 };
+
+// lap timer over consecutive host segments: lap(slot) books the time since the previous lap; off unless profiling
+struct pf_host_timer {
+    pfnav_ctx *ctx; std::chrono::steady_clock::time_point t;
+    explicit pf_host_timer(pfnav_ctx *c) : ctx(c) { if (ctx->profiling) t = std::chrono::steady_clock::now(); }
+    void lap(int slot)
+    {
+        if (!ctx->profiling) return;
+        const auto now = std::chrono::steady_clock::now();
+        ctx->host_ms[slot] += std::chrono::duration<double, std::milli>(now - t).count();
+        ctx->host_count[slot]++;
+        t = now;
+    }
+};
 
 // RAII helper: brackets the launches of one kernel group with events when profiling is on
 struct pf_prof_scope {

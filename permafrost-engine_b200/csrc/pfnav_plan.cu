@@ -13,7 +13,9 @@
 #include "pfnav_internal.cuh"
 #include <algorithm>
 #include <atomic>
-#include <deque>
+#include <condition_variable>
+#include <functional>
+#include <mutex>
 #include <string.h>
 #include <thread>
 
@@ -179,10 +181,32 @@ extern "C" int pfnav_plan_goal(pfnav_ctx *ctx, int layer, int tgt_chunk_r, int t
     const size_t ltiles = (size_t)chunks * 4096;
     const uint16_t *liid = ctx->h_liid.data() + ltiles * layer;
     *n_flow = 0; *n_los = 0;
+    // scratch reused across calls (planner threads are persistent): the BFS queue, and the (chunk, island) nodes
+    // already planned as an open-addressing set whose entries carry the call's generation (no clearing per call)
     struct node { int chunk; uint16_t li; };
-    std::deque<node> q;
-    std::vector<std::vector<uint16_t>> seen(chunks);      // islands already planned per chunk
-    std::vector<int> los_index(chunks, -1), nodes_in_chunk(chunks, 0);
+    struct scratch { std::vector<node> q; std::vector<uint64_t> seen; uint32_t gen = 0; std::vector<int> los_index, nodes_in_chunk; std::vector<uint16_t> first_li; };
+    static thread_local scratch tls;
+    scratch &S = tls;                       // one TLS lookup, not one per use in the loops below
+    size_t tab = 64;
+    while (tab < 2 * ((size_t)std::max(max_flow, 0) + 2)) tab *= 2;        // every insert emits a flow request: load <= 1/2
+    if (S.seen.size() < tab) { S.seen.assign(tab, 0); S.gen = 0; }
+    tab = S.seen.size();
+    int shift = 64;
+    for (size_t t = tab; t > 1; t >>= 1) shift--;                          // Fibonacci hashing: the top log2(tab) bits
+    if (++S.gen == 0) { std::fill(S.seen.begin(), S.seen.end(), 0); S.gen = 1; }
+    const uint64_t gen = (uint64_t)S.gen << 32;
+    auto first_visit = [&](int chunk, uint16_t li) -> bool {      // insert (chunk, island); false if it was there
+        if (S.first_li[chunk] == li) return false;                 // most chunks are reached through one island
+        if (S.first_li[chunk] == 0xFFFF) S.first_li[chunk] = li;
+        const uint64_t key = gen | ((uint64_t)chunk << 16) | li;
+        for (size_t h = (size_t)(((uint64_t)chunk << 16 | li) * 0x9E3779B97F4A7C15ull >> shift);; h = (h + 1) & (tab - 1)) {
+            if (S.seen[h] == key) return false;
+            if ((S.seen[h] >> 32) != (gen >> 32)) { S.seen[h] = key; return true; }
+        }
+    };
+    S.q.clear();
+    S.los_index.assign(chunks, -1); S.nodes_in_chunk.assign(chunks, 0); S.first_li.assign(chunks, 0xFFFF);
+    std::vector<int> &los_index = S.los_index, &nodes_in_chunk = S.nodes_in_chunk;
     const int tchunk = tgt_chunk_r * cw + tgt_chunk_c;
     const uint16_t tli = liid[(size_t)tchunk * 4096 + tgt_tile_r * 64 + tgt_tile_c];
     auto emit_flow = [&](const pfnav_field_req &rq, int chunk) -> bool {
@@ -213,11 +237,10 @@ extern "C" int pfnav_plan_goal(pfnav_ctx *ctx, int layer, int tgt_chunk_r, int t
         los_out[*n_los] = lq; los_chunk[*n_los] = tchunk; (*n_los)++;
     }
     if (tli == 0xFFFF) return PFNAV_OK;      // goal tile impassable/blocked: nothing can flow to it
-    seen[tchunk].push_back(tli);
-    q.push_back({tchunk, tli});
-    while (!q.empty()) {
-        const node cur = q.front();
-        q.pop_front();
+    first_visit(tchunk, tli);
+    S.q.push_back({tchunk, tli});
+    for (size_t head = 0; head < S.q.size(); head++) {
+        const node cur = S.q[head];
         const auto &ports = ctx->portals[layer][cur.chunk];
         for (size_t pi = 0; pi < ports.size(); pi++) {
             const auto &P = ports[pi];                                // portal of the current (parent) chunk
@@ -225,15 +248,15 @@ extern "C" int pfnav_plan_goal(pfnav_ctx *ctx, int layer, int tgt_chunk_r, int t
             const int nchunk = P.conn_chunk;
             // every island M of the neighbour that touches island cur.li across this portal
             const int len = (P.r1 - P.r0) + (P.c1 - P.c0) + 1;
+            uint16_t lastM = 0xFFFF;                                  // a repeat along the portal was just visited
             for (int k = 0; k < len; k++) {
                 const int pr = P.r0 + (P.r1 > P.r0 ? k : 0), pc = P.c0 + (P.c1 > P.c0 ? k : 0);
                 const int qr = Q.r0 + (Q.r1 > Q.r0 ? k : 0), qc = Q.c0 + (Q.c1 > Q.c0 ? k : 0);
                 if (liid[(size_t)cur.chunk * 4096 + pr * 64 + pc] != cur.li) continue;
                 const uint16_t M = liid[(size_t)nchunk * 4096 + qr * 64 + qc];
-                if (M == 0xFFFF) continue;
-                auto &sv = seen[nchunk];
-                if (std::find(sv.begin(), sv.end(), M) != sv.end()) continue;
-                sv.push_back(M);
+                if (M == 0xFFFF || M == lastM) continue;
+                lastM = M;
+                if (!first_visit(nchunk, M)) continue;
                 pfnav_field_req rq = base;
                 rq.chunk_r = Q.chunk_r; rq.chunk_c = Q.chunk_c; rq.target_type = PFNAV_TARGET_PORTAL;
                 rq.port_r0 = Q.r0; rq.port_c0 = Q.c0; rq.port_r1 = Q.r1; rq.port_c1 = Q.c1;
@@ -253,7 +276,7 @@ extern "C" int pfnav_plan_goal(pfnav_ctx *ctx, int layer, int tgt_chunk_r, int t
                     los_index[nchunk] = *n_los;
                     los_out[*n_los] = lq; los_chunk[*n_los] = nchunk; (*n_los)++;
                 }
-                q.push_back({nchunk, M});
+                S.q.push_back({nchunk, M});
             }
         }
     }
@@ -274,16 +297,17 @@ extern "C" int pfnav_plan_goal(pfnav_ctx *ctx, int layer, int tgt_chunk_r, int t
 int pf_pool_reserve(pfnav_ctx *ctx, const size_t *keys, size_t n, int32_t *slots_out, bool *out_evicted)
 {
     if (out_evicted) *out_evicted = false;
+    // the distinct keys without a slot, ascending (a key is marked -2 while it is collected, so repeats are skipped)
     std::vector<size_t> fresh;
     for (size_t i = 0; i < n; i++)
-        if (ctx->h_pool_slot[keys[i]] < 0) fresh.push_back(keys[i]);
+        if (ctx->h_pool_slot[keys[i]] == -1) { ctx->h_pool_slot[keys[i]] = -2; fresh.push_back(keys[i]); }
+    for (size_t key : fresh) ctx->h_pool_slot[key] = -1;
     std::sort(fresh.begin(), fresh.end());
-    fresh.erase(std::unique(fresh.begin(), fresh.end()), fresh.end());
     const size_t avail = ctx->pool_free.size() + (size_t)(ctx->pool_max - ctx->pool_used);
     if (fresh.size() > avail) {
         const size_t k = fresh.size() - avail;
         std::vector<uint32_t> stamp(ctx->h_slot_touch);
-        if (ctx->device >= 0 && ctx->d_pool_touch) {
+        if (ctx->device >= 0 && ctx->d_pool_touch && !ctx->pool_dev_stale) {     // stale: cleared, no tick read a slot since
             PF_CUDA(cudaSetDevice(ctx->device));
             PF_CUDA(cudaDeviceSynchronize());         // ticks on any stream may still be stamping slots (eviction is rare)
             std::vector<uint32_t> dev(ctx->pool_max);
@@ -355,6 +379,82 @@ static int los_forked(pfnav_ctx *ctx)
     return 0;
 }
 
+// Host side of a cold goal batch, owned by the context: persistent planner threads (created on the first batch,
+// joined by pfnav_destroy) and per-goal / merge scratch that keeps its capacity across batches, so that a batch
+// neither spawns threads nor allocates.
+struct pf_planner {
+    struct goal_plan { std::vector<pfnav_field_req> fr; std::vector<pfnav_los_req> lr; std::vector<int32_t> fc, fw, lc; int nf = 0, nl = 0, rc = 0; std::string err; };
+    struct merged {
+        std::vector<pfnav_field_req> fr; std::vector<pfnav_los_req> lr;
+        std::vector<int32_t> fw, ld, slots; std::vector<int> depth, newpos, lnew; std::vector<size_t> fkeys, lkeys, keys;
+        void clear() { fr.clear(); lr.clear(); fw.clear(); ld.clear(); fkeys.clear(); lkeys.clear(); }
+    };
+    std::vector<goal_plan> plans;
+    merged batch;
+
+    explicit pf_planner(int nworkers)
+    {
+        for (int i = 0; i < nworkers; i++) threads.emplace_back([this] { worker(); });
+    }
+    ~pf_planner()
+    {
+        { std::lock_guard<std::mutex> l(m); quit = true; }
+        wake.notify_all();
+        for (auto &t : threads) t.join();
+    }
+    // job(0) .. job(n - 1) on the workers and the calling thread; returns when all have finished
+    void run(int n, std::function<void(int)> f)
+    {
+        if (n <= 1 || threads.empty()) { for (int g = 0; g < n; g++) f(g); return; }
+        {
+            std::lock_guard<std::mutex> l(m);
+            job = std::move(f); njobs = n; next = 0; busy = (int)threads.size(); gen++;
+        }
+        wake.notify_all();
+        drain();
+        std::unique_lock<std::mutex> l(m);
+        done.wait(l, [&] { return busy == 0; });
+    }
+
+private:
+    std::vector<std::thread> threads;
+    std::mutex m;
+    std::condition_variable wake, done;
+    std::function<void(int)> job;
+    int njobs = 0, busy = 0;
+    uint64_t gen = 0;
+    bool quit = false;
+    std::atomic<int> next{0};
+
+    void drain() { for (int g = next.fetch_add(1); g < njobs; g = next.fetch_add(1)) job(g); }
+    void worker()
+    {
+        uint64_t seen = 0;
+        std::unique_lock<std::mutex> l(m);
+        for (;;) {
+            wake.wait(l, [&] { return quit || gen != seen; });
+            if (quit) return;
+            seen = gen;
+            l.unlock();
+            drain();
+            l.lock();
+            if (--busy == 0) done.notify_one();
+        }
+    }
+};
+
+static pf_planner &planner_of(pfnav_ctx *ctx)
+{
+    if (!ctx->planner) ctx->planner = new pf_planner(std::max(1, std::min((int)std::thread::hardware_concurrency(), 32)) - 1);
+    return *(pf_planner *)ctx->planner;
+}
+
+void pf_planner_destroy(pfnav_ctx *ctx)
+{
+    delete (pf_planner *)ctx->planner;
+    ctx->planner = nullptr;
+}
+
 // n_request_path's field-building half, resident on the device, for a batch of goals: plan every
 // goal, then run the flow waves and the LOS dependency waves of ALL goals together straight into the
 // field pool (no host round trip of field bytes; one launch per wave, not per goal).
@@ -404,37 +504,24 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
         }
         gb.valid = false;
     }
-    PF_CUDA(pf_fields_sync(ctx));       // the plan buffer below may still be read by a forked LOS kernel
-    const int cap = chunks * 8 + 8;
-    std::vector<pfnav_field_req> all_fr;
-    std::vector<pfnav_los_req> all_lr;
-    std::vector<int32_t> all_fs, all_fw, all_ls, all_ld;
-    std::vector<size_t> fkeys, lkeys;
+    pf_host_timer ht(ctx);
     for (int g = 0; g < ngoals; g++) PF_ARG(dests[g] >= 0 && dests[g] < ctx->pool_ndests, "dest");
-    // the goals are planned independently of each other (read-only walks over the host mirrors): one host thread each
-    struct goal_plan { std::vector<pfnav_field_req> fr; std::vector<pfnav_los_req> lr; std::vector<int32_t> fc, fw, lc; int nf = 0, nl = 0, rc = 0; std::string err; };
-    std::vector<goal_plan> plans(ngoals);
-    {
-        auto plan_one = [&](int g) {
-            goal_plan &P = plans[g];
-            P.fr.resize(cap); P.lr.resize(cap); P.fc.resize(cap); P.fw.resize(cap); P.lc.resize(cap);
-            P.rc = pfnav_plan_goal(ctx, layer, targets[4 * g], targets[4 * g + 1], targets[4 * g + 2], targets[4 * g + 3],
-                                   P.fr.data(), P.fc.data(), P.fw.data(), cap, &P.nf, P.lr.data(), P.lc.data(), cap, &P.nl);
-            if (P.rc) P.err = pfnav_last_error();          // the error text is thread-local
-        };
-        const int nthreads = std::max(1, std::min({ngoals, (int)std::thread::hardware_concurrency(), 32}));
-        if (nthreads == 1) { for (int g = 0; g < ngoals; g++) plan_one(g); }
-        else {
-            std::atomic<int> next{0};
-            std::vector<std::thread> pool;
-            auto worker = [&]() { for (int g = next.fetch_add(1); g < ngoals; g = next.fetch_add(1)) plan_one(g); };
-            for (int t = 1; t < nthreads; t++) pool.emplace_back(worker);
-            worker();
-            for (auto &t : pool) t.join();
-        }
-    }
+    // the goals are planned independently of each other (read-only walks over the host mirrors) on the planner threads
+    pf_planner &PL = planner_of(ctx);
+    const int cap = chunks * 8 + 8;
+    if ((int)PL.plans.size() < ngoals) PL.plans.resize(ngoals);
+    PL.run(ngoals, [&](int g) {
+        pf_planner::goal_plan &P = PL.plans[g];
+        if ((int)P.fr.size() < cap) { P.fr.resize(cap); P.lr.resize(cap); P.fc.resize(cap); P.fw.resize(cap); P.lc.resize(cap); }
+        P.rc = pfnav_plan_goal(ctx, layer, targets[4 * g], targets[4 * g + 1], targets[4 * g + 2], targets[4 * g + 3],
+                               P.fr.data(), P.fc.data(), P.fw.data(), cap, &P.nf, P.lr.data(), P.lc.data(), cap, &P.nl);
+        if (P.rc) P.err = pfnav_last_error();          // the error text is thread-local
+    });
+    ht.lap(PF_HPROF_PLAN);
+    pf_planner::merged &B = PL.batch;
+    B.clear();
     for (int g = 0; g < ngoals; g++) {
-        goal_plan &P = plans[g];
+        pf_planner::goal_plan &P = PL.plans[g];
         if (P.rc) { pfnav_set_error("%s", P.err.c_str()); return P.rc; }
         const int nf = P.nf, nl = P.nl;
         const pfnav_field_req *fr = P.fr.data(); const pfnav_los_req *lr = P.lr.data();
@@ -448,83 +535,108 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
         };
         for (int i = 0; i < nf; i++) {
             if (held(fc[i], 1)) continue;
-            all_fr.push_back(fr[i]); all_fw.push_back(fw[i]);
-            fkeys.push_back((size_t)dests[g] * chunks + fc[i]);
+            B.fr.push_back(fr[i]); B.fw.push_back(fw[i]);
+            B.fkeys.push_back((size_t)dests[g] * chunks + fc[i]);
         }
-        std::vector<int> depth(nl, 0), newpos(nl, -1);
+        B.depth.assign(nl, 0); B.newpos.assign(nl, -1);
         for (int i = 0; i < nl; i++) {
             if (held(lc[i], 2)) continue;
             pfnav_los_req q = lr[i];
             if (q.prev_index >= 0) {
-                if (newpos[q.prev_index] >= 0) { depth[i] = depth[q.prev_index] + 1; q.prev_index = newpos[q.prev_index]; }
+                if (B.newpos[q.prev_index] >= 0) { B.depth[i] = B.depth[q.prev_index] + 1; q.prev_index = B.newpos[q.prev_index]; }
                 else {
                     q.prev_index = -2;      // parent kept: its absolute pool slot rides in _pad
                     q._pad = ctx->h_pool_slot[(size_t)dests[g] * chunks + q.prev_chunk_r * ctx->chunk_w + q.prev_chunk_c];
                 }
             }
-            newpos[i] = (int)all_lr.size();
-            all_lr.push_back(q); all_ld.push_back(depth[i]);
-            lkeys.push_back((size_t)dests[g] * chunks + lc[i]);
+            B.newpos[i] = (int)B.lr.size();
+            B.lr.push_back(q); B.ld.push_back(B.depth[i]);
+            B.lkeys.push_back((size_t)dests[g] * chunks + lc[i]);
         }
     }
-    if (all_fr.empty() && all_lr.empty()) return PFNAV_OK;
-    const int nf = (int)all_fr.size(), nl = (int)all_lr.size();
-    {   // slots for everything the batch writes, all or nothing (nothing is published before this succeeds)
-        std::vector<size_t> keys(fkeys);
-        keys.insert(keys.end(), lkeys.begin(), lkeys.end());
-        std::vector<int32_t> slots(keys.size());
-        int rc = pf_pool_reserve(ctx, keys.data(), keys.size(), slots.data(), nullptr);
-        if (rc) return rc;
-        all_fs.assign(slots.begin(), slots.begin() + nf);
-        all_ls.assign(slots.begin() + nf, slots.end());
-        for (int i = 0; i < nf; i++) { ctx->h_pool_has[all_fs[i]] |= 1; ctx->h_pool_req[all_fs[i]] = all_fr[i]; }
-        for (int i = 0; i < nl; i++) ctx->h_pool_has[all_ls[i]] |= 2;
-    }
+    if (B.fr.empty() && B.lr.empty()) return PFNAV_OK;
+    const int nf = (int)B.fr.size(), nl = (int)B.lr.size();
     // stable order by wave / depth
     int maxw = 0, maxd = 0;
-    for (int i = 0; i < nf; i++) maxw = std::max(maxw, all_fw[i]);
-    for (int i = 0; i < nl; i++) maxd = std::max(maxd, all_ld[i]);
+    for (int i = 0; i < nf; i++) maxw = std::max(maxw, B.fw[i]);
+    for (int i = 0; i < nl; i++) maxd = std::max(maxd, B.ld[i]);
     std::vector<int32_t> fwave_off(maxw + 2, 0), lwave_off(maxd + 2, 0);
-    for (int i = 0; i < nf; i++) fwave_off[all_fw[i] + 1]++;
+    for (int i = 0; i < nf; i++) fwave_off[B.fw[i] + 1]++;
     for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
-    for (int i = 0; i < nl; i++) lwave_off[all_ld[i] + 1]++;
+    for (int i = 0; i < nl; i++) lwave_off[B.ld[i] + 1]++;
     for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
-    std::vector<int> lnew(nl);
+    B.keys.assign(B.fkeys.begin(), B.fkeys.end());
+    B.keys.insert(B.keys.end(), B.lkeys.begin(), B.lkeys.end());
+    ht.lap(PF_HPROF_MERGE);
+    {   // slots for everything the batch writes, all or nothing (nothing is published before this succeeds)
+        B.slots.resize(B.keys.size());
+        int rc = pf_pool_reserve(ctx, B.keys.data(), B.keys.size(), B.slots.data(), nullptr);
+        if (rc) return rc;
+        const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
+        for (int i = 0; i < nf; i++) { ctx->h_pool_has[fs[i]] |= 1; ctx->h_pool_req[fs[i]] = B.fr[i]; }
+        for (int i = 0; i < nl; i++) ctx->h_pool_has[ls[i]] |= 2;
+    }
+    ht.lap(PF_HPROF_RESERVE);
     const size_t b_fr = (size_t)nf * sizeof(pfnav_field_req), b_fs = (size_t)nf * 4;
     const size_t b_lr = (size_t)nl * sizeof(pfnav_los_req), b_ls = (size_t)nl * 4;
     const size_t total = b_fr + b_fs + b_lr + b_ls;
-    std::vector<uint8_t> host(total);
-    pfnav_field_req *hfr = (pfnav_field_req *)host.data();
-    int32_t *hfs = (int32_t *)(host.data() + b_fr);
-    pfnav_los_req *hlr = (pfnav_los_req *)(host.data() + b_fr + b_fs);
-    int32_t *hls = (int32_t *)(host.data() + b_fr + b_fs + b_lr);
-    {
-        std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1);
-        for (int i = 0; i < nf; i++) { const int k = cur[all_fw[i]]++; hfr[k] = all_fr[i]; hfs[k] = all_fs[i]; }
-        std::vector<int32_t> cur2(lwave_off.begin(), lwave_off.end() - 1);
-        for (int i = 0; i < nl; i++) lnew[i] = cur2[all_ld[i]]++;
-        for (int i = 0; i < nl; i++) {
-            pfnav_los_req q = all_lr[i];
-            if (q.prev_index >= 0) q.prev_index = lnew[q.prev_index];
-            hlr[lnew[i]] = q; hls[lnew[i]] = all_ls[i];
-        }
-    }
+    // the slot table and the `has` bytes travel in the same staging buffer, behind the plan
+    const size_t b_tab = (total + 15) & ~(size_t)15, b_slot = ctx->h_pool_slot.size() * 4;
+    const size_t stage = b_tab + b_slot + (size_t)ctx->pool_max;
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
-    // one staging buffer per context: goal batches are serialised on one stream by the caller
+    // pinned staging ring of two: buffer `ri` was last copied from two batches ago (its event guards the reuse)
+    const int ri = ctx->plan_host_next;
+    ctx->plan_host_next ^= 1;
+    if (!ctx->plan_host_ev[ri]) PF_CUDA(cudaEventCreateWithFlags(&ctx->plan_host_ev[ri], cudaEventDisableTiming));
+    else PF_CUDA(cudaEventSynchronize(ctx->plan_host_ev[ri]));
+    if (ctx->plan_host_bytes[ri] < stage) {      // grow-only
+        cudaFreeHost(ctx->plan_host[ri]);
+        ctx->plan_host[ri] = nullptr; ctx->plan_host_bytes[ri] = 0;
+        PF_CUDA(cudaMallocHost(&ctx->plan_host[ri], stage * 2));
+        ctx->plan_host_bytes[ri] = stage * 2;
+    }
+    ht.lap(PF_HPROF_WAIT);
+    uint8_t *host = (uint8_t *)ctx->plan_host[ri];
+    pfnav_field_req *hfr = (pfnav_field_req *)host;
+    int32_t *hfs = (int32_t *)(host + b_fr);
+    pfnav_los_req *hlr = (pfnav_los_req *)(host + b_fr + b_fs);
+    int32_t *hls = (int32_t *)(host + b_fr + b_fs + b_lr);
+    {
+        const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
+        std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1);
+        for (int i = 0; i < nf; i++) { const int k = cur[B.fw[i]]++; hfr[k] = B.fr[i]; hfs[k] = fs[i]; }
+        std::vector<int32_t> cur2(lwave_off.begin(), lwave_off.end() - 1);
+        B.lnew.resize(nl);
+        for (int i = 0; i < nl; i++) B.lnew[i] = cur2[B.ld[i]]++;
+        for (int i = 0; i < nl; i++) {
+            pfnav_los_req q = B.lr[i];
+            if (q.prev_index >= 0) q.prev_index = B.lnew[q.prev_index];
+            hlr[B.lnew[i]] = q; hls[B.lnew[i]] = ls[i];
+        }
+        memcpy(host + b_tab, ctx->h_pool_slot.data(), b_slot);
+        memcpy(host + b_tab + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
+    }
+    ht.lap(PF_HPROF_PACK);
+    // one device plan buffer per context: the resident fast path relaunches from it, and the previous batch's forked
+    // kernels read it until they finish -- its overwrite is ordered after them (join), growing it waits for them
     if (ctx->plan_buf_bytes < total) {
+        PF_CUDA(pf_fields_sync(ctx));
         PF_CUDA(cudaStreamSynchronize(st));
         cudaFree(ctx->d_plan_buf);
         ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
         PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
         ctx->plan_buf_bytes = total * 2;
     }
+    PF_CUDA(pf_pool_refresh(ctx, st));       // after pfnav_pool_clear: reset the touch stamps (the table is uploaded below)
+    PF_CUDA(pf_fields_join(ctx, st));
     uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
-    PF_CUDA(cudaMemcpyAsync(dev, host.data(), total, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
+    PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_tab, b_slot, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_tab + b_slot, ctx->pool_max,
                             cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaStreamSynchronize(st));      // `host` is pageable and about to go out of scope
+    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    ht.lap(PF_HPROF_UPLOAD);
     const pfnav_field_req *dfr = (const pfnav_field_req *)dev;
     const int32_t *dfs = (const int32_t *)(dev + b_fr);
     const pfnav_los_req *dlr = (const pfnav_los_req *)(dev + b_fr + b_fs);
@@ -541,6 +653,7 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     if (rc) return rc;
     rc = los_forked(ctx);
     if (rc) return rc;
+    ht.lap(PF_HPROF_LAUNCH);
     {
         auto &gb = ctx->goal_batch;
         gb.valid = !missing_only; gb.epoch = ctx->map_epoch; gb.layer = layer;

@@ -447,6 +447,7 @@ extern "C" int pfnav_pool_request_zone(pfnav_ctx *ctx, int dest, int layer, cons
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
     cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_pool_refresh(ctx, st));
     // the chunks the footprint can reach (nav.c:3945-3951; C division truncates toward zero)
     const int reach = 2 * radius;
     auto clampi = [](int v, int lo, int hi) { return std::min(std::max(v, lo), hi); };
@@ -501,6 +502,7 @@ extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const floa
     PF_ARG(radius >= 0 && radius <= 0xFFFF, "radius");
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
+    PF_CUDA(pf_pool_refresh(ctx, ctx->tick_stream));
     uint8_t *d_buf = nullptr;
     PF_CUDA(cudaMalloc(&d_buf, n * 17));
     float2 *d_pos = reinterpret_cast<float2 *>(d_buf), *d_vel = d_pos + n;
@@ -700,10 +702,11 @@ extern "C" int pfnav_pool_request_entity_fields(pfnav_ctx *ctx, int dest, int la
     }
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
+    cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_pool_refresh(ctx, st));
     std::vector<int32_t> slots(n);
     bool evicted = false;
     if ((rc = pf_pool_reserve(ctx, keys.data(), n, slots.data(), &evicted))) return rc;
-    cudaStream_t st = pf_stream(ctx, stream);
     uint8_t *d_out = nullptr;
     PF_CUDA(cudaMalloc(&d_out, n * 4096));
     rc = chunk_fields_launch(ctx, layer, dim, chunks_rc, n, seeds, off, d_out, st);

@@ -921,6 +921,7 @@ static int pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *dests, int l
 {
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
+    PF_CUDA(pf_pool_refresh(ctx, pf_stream(ctx, stream)));
     pfnav_route_layer &RL = *route_layer(ctx, layer);
     const int cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
     // n_update_all_edge_states (nav.c:1787): the map does not change between the requests of a batch
@@ -1081,6 +1082,7 @@ extern "C" int pfnav_pool_get(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c
     if (out_ffid) *out_ffid = ctx->h_pool_ffid[si];
     if (slot < 0) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(pf_pool_refresh(ctx, ctx->tick_stream));
     PF_CUDA(cudaDeviceSynchronize());
     if (flow_out && (*out_has & 1)) PF_CUDA(cudaMemcpy(flow_out, ctx->d_pool_flow + (size_t)slot * 4096, 4096, cudaMemcpyDeviceToHost));
     if (los_out && (*out_has & 2)) PF_CUDA(cudaMemcpy(los_out, ctx->d_pool_los + (size_t)slot * 4096, 4096, cudaMemcpyDeviceToHost));
