@@ -667,6 +667,33 @@ int  pfnav_agents_read_state(pfnav_ctx *ctx, pfnav_agent *agents_out, pfnav_move
 int  pfnav_pool_request_entity_fields(pfnav_ctx *ctx, int dest, int layer, int ref_layer, int target_kind,
                                       const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc, size_t n,
                                       void *stream);
+/* One request of pfnav_pool_request_entity_fields_batch: the arguments of one pfnav_pool_request_entity_fields call,
+ * with its footprints and chunks given as ranges of the batch's shared arrays. */
+typedef struct pfnav_entity_field_req {   /* 32 bytes */
+    int32_t  dest, layer, ref_layer, target_kind;   /* as pfnav_pool_request_entity_fields */
+    uint32_t ent_off, ent_n;                        /* footprints ents[ent_off .. ent_off + ent_n) */
+    uint32_t chunk_off, chunk_n;                    /* (r, c) pairs chunks_rc[2*chunk_off ..] */
+} pfnav_entity_field_req;
+/* N_RequestAsyncEnemySeekField / N_RequestAsyncSurroundField queued during a tick and built at once by
+ * N_AwaitAsyncFields (nav.c:3769-3960): m requests against the device field pool in one call.
+ * - Equivalence: the pool and the remembered footprints end exactly as pfnav_pool_request_entity_fields leaves them when
+ *   called on requests 0 .. m-1 in order: flow bytes, `has` bytes, the ff_id pfnav_pool_get reports, LRU slot choices and
+ *   evictions, and the footprints pfnav_pool_repair starts from. A later request wins: a repeated dest, or a repeated
+ *   (dest, chunk), ends with the last request's field and footprints.
+ * - Ranges of `ents` may overlap: several requests may name the same footprints (one enemy list for several factions).
+ * - The whole batch is validated before anything changes: ranges, chunks, layers, target kinds, TARGET_ENTITY with
+ *   ent_n == 1, the corners of every building footprint a field would use inside the map, and a map shape the padded
+ *   chunk fields support (more than one chunk row and column, or 1 x 1). Failure: PFNAV_ERR_ARG, nothing changed.
+ * - If the pool cannot hold request k's fields, requests 0 .. k-1 are done, *out_ndone = k (may be NULL) and
+ *   PFNAV_ERR_NOMEM is returned; request k changed nothing.
+ * - Launches are asynchronous on `stream` (NULL: the context's stream) and ordered after the field work forked by
+ *   pfnav_pool_request_goals and after pfnav_pool_clear. The inputs are copied before the call returns, so the caller may
+ *   reuse its buffers. The call does not wait for the device (except to evict under pool pressure). The seed frontiers
+ *   are rasterised on the device.
+ * - Host-only context: PFNAV_ERR_NO_DEVICE. */
+int  pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                            const pfnav_footprint *ents, size_t nents,
+                                            const int32_t *chunks_rc, size_t nchunks, void *stream, int *out_ndone);
 
 /* Test / tuning hook for pfnav_agents_tick: 0 = single-pass velocity kernel; 1 (default) = while LOS chains of
  * pfnav_pool_request_goals are still in flight, run the part of the update that does not depend on the

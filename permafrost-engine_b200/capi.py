@@ -74,6 +74,9 @@ REGION_CREATE, REGION_FIXUP, REGION_CELL = 1, 2, 4
 FOOTPRINT = np.dtype([("x", "<f4"), ("z", "<f4"), ("sel_radius", "<f4"), ("is_building", "<u4"), ("corners_xz", "<f4", 8)])
 assert FOOTPRINT.itemsize == 48
 TARGET_ENTITY, TARGET_ENEMIES = 0, 1
+ENTITY_FIELD_REQ = np.dtype([("dest", "<i4"), ("layer", "<i4"), ("ref_layer", "<i4"), ("target_kind", "<i4"),
+                             ("ent_off", "<u4"), ("ent_n", "<u4"), ("chunk_off", "<u4"), ("chunk_n", "<u4")])
+assert ENTITY_FIELD_REQ.itemsize == 32
 
 LOS_PREV_INPLACE = -3
 TICK_VDES_FROM_POOL = 1
@@ -100,6 +103,7 @@ SYMBOLS = [
     "pfnav_group_create", "pfnav_group_gather", "pfnav_group_destroy", "pfnav_agents_upload_shard",
     "pfnav_pool_request_goals_ex", "pfnav_blockers_batch", "pfnav_map_set_pos",
     "pfnav_agents_upload_formation", "pfnav_agents_upload_movestate_ext", "pfnav_pool_request_entity_fields",
+    "pfnav_pool_request_entity_fields_batch",
     "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
     "pfnav_profile_read_host",
 ]
@@ -207,6 +211,8 @@ def load():
     L.pfnav_agents_upload_movestate_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_pool_request_entity_fields.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t,
                                                    C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_pool_request_entity_fields_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                         C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]
     L.pfnav_map_set_pos.argtypes = [C.c_void_p, C.c_float, C.c_float]
     L.pfnav_agents_upload_shard.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,
                                             C.c_int, C.c_uint32]
@@ -751,6 +757,21 @@ class Nav:
         ch = np.ascontiguousarray(chunks, np.int32).reshape(-1, 2)
         _chk(self.L.pfnav_pool_request_entity_fields(self.h, dest, layer, ref_layer, kind, _p(fp), len(fp), _p(ch), len(ch),
                                                      C.c_void_p(stream)))
+
+    def pool_request_entity_fields_batch(self, reqs, footprints, chunks, stream=0):
+        """pool_request_entity_fields for every ENTITY_FIELD_REQ record of `reqs`, in order, in one call; their footprint
+        and chunk ranges index `footprints` and `chunks` (int32[n, 2]) -> ndone. ndone < len(reqs): the pool could not hold
+        request ndone's fields (PFNAV_ERR_NOMEM); requests before it are done."""
+        reqs = np.ascontiguousarray(reqs, ENTITY_FIELD_REQ)
+        fp = np.ascontiguousarray(footprints, FOOTPRINT)
+        ch = np.ascontiguousarray(chunks, np.int32).reshape(-1, 2)
+        ndone = C.c_int(0)
+        rc = self.L.pfnav_pool_request_entity_fields_batch(self.h, _p(reqs) if len(reqs) else None, len(reqs), _p(fp) if len(fp) else None,
+                                                           len(fp), _p(ch) if len(ch) else None, len(ch), C.c_void_p(stream),
+                                                           C.byref(ndone))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        return ndone.value
 
     def route_graph_paths(self, req, max_hops=256, on_device=True, layer=0):
         """AStar_PortalGraphPath batch; req int32[n, 8]; -> status[n], cost[n], list of hop arrays [nhops, 3]"""

@@ -1516,6 +1516,8 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
         cudaFreeHost(ctx->plan_host[i]);
         if (ctx->plan_host_ev[i]) cudaEventDestroy(ctx->plan_host_ev[i]);
     }
+    cudaFree(ctx->d_ent_buf);
+    if (ctx->ent_ev) cudaEventDestroy(ctx->ent_ev);
     pfnav_fields_free(ctx);
     pfnav_agents_free(ctx);
     if (ctx->tick_done) cudaEventDestroy(ctx->tick_done);

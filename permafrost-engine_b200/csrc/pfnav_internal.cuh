@@ -195,6 +195,9 @@ struct pfnav_ctx {
     void *plan_host[2] = {nullptr, nullptr}; size_t plan_host_bytes[2] = {0, 0};
     cudaEvent_t plan_host_ev[2] = {nullptr, nullptr}; int plan_host_next = 0;
     void *planner = nullptr;
+    // entity-field batches (pfnav_region.cu): device scratch for the staged inputs, footprint rows and seed bitmaps,
+    // grown on demand; ent_ev is recorded after the last kernel that reads it
+    void *d_ent_buf = nullptr; size_t ent_buf_bytes = 0; cudaEvent_t ent_ev = nullptr;
 
     // ---- optional per-kernel timing (pfnav_profile_enable) ----
     bool profiling = false;
@@ -272,6 +275,9 @@ int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, st
 // pool slots with LRU eviction (pfnav_plan.cu)
 int pf_pool_reserve(pfnav_ctx *ctx, const size_t *keys, size_t n, int32_t *slots_out, bool *out_evicted);
 void pf_planner_destroy(pfnav_ctx *ctx);                         // pfnav_plan.cu: join the goal planner threads
+// the next of the two pinned staging buffers (plan_host), at least `bytes` long, once the copy that last read it is done;
+// record plan_host_ev[*out_ri] after the copies from it (pfnav_plan.cu)
+int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri);
 
 enum { PF_PROF_FLOW = 0, PF_PROF_LOS = 1, PF_PROF_INDEX = 2, PF_PROF_VDES = 3, PF_PROF_COHESION = 4,
        PF_PROF_VELOCITY = 5, PF_PROF_UPDATE = 6, PF_PROF_APPLY = 7, PF_PROF_SLOTS = 8 };

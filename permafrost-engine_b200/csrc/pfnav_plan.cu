@@ -585,19 +585,10 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     const size_t stage = b_tab + b_slot + (size_t)ctx->pool_max;
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
-    // pinned staging ring of two: buffer `ri` was last copied from two batches ago (its event guards the reuse)
-    const int ri = ctx->plan_host_next;
-    ctx->plan_host_next ^= 1;
-    if (!ctx->plan_host_ev[ri]) PF_CUDA(cudaEventCreateWithFlags(&ctx->plan_host_ev[ri], cudaEventDisableTiming));
-    else PF_CUDA(cudaEventSynchronize(ctx->plan_host_ev[ri]));
-    if (ctx->plan_host_bytes[ri] < stage) {      // grow-only
-        cudaFreeHost(ctx->plan_host[ri]);
-        ctx->plan_host[ri] = nullptr; ctx->plan_host_bytes[ri] = 0;
-        PF_CUDA(cudaMallocHost(&ctx->plan_host[ri], stage * 2));
-        ctx->plan_host_bytes[ri] = stage * 2;
-    }
+    uint8_t *host = nullptr;
+    int ri = 0;
+    if (int rc = pf_plan_host(ctx, stage, &host, &ri)) return rc;
     ht.lap(PF_HPROF_WAIT);
-    uint8_t *host = (uint8_t *)ctx->plan_host[ri];
     pfnav_field_req *hfr = (pfnav_field_req *)host;
     int32_t *hfs = (int32_t *)(host + b_fr);
     pfnav_los_req *hlr = (pfnav_los_req *)(host + b_fr + b_fs);
@@ -662,6 +653,24 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     }
     if (out_n_flow) *out_n_flow = nf;
     if (out_n_los) *out_n_los = nl;
+    return PFNAV_OK;
+}
+
+// pinned staging ring of two: buffer `ri` was last copied from two batches ago (its event guards the reuse)
+int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri)
+{
+    const int ri = ctx->plan_host_next;
+    ctx->plan_host_next ^= 1;
+    if (!ctx->plan_host_ev[ri]) PF_CUDA(cudaEventCreateWithFlags(&ctx->plan_host_ev[ri], cudaEventDisableTiming));
+    else PF_CUDA(cudaEventSynchronize(ctx->plan_host_ev[ri]));
+    if (ctx->plan_host_bytes[ri] < bytes) {      // grow-only
+        cudaFreeHost(ctx->plan_host[ri]);
+        ctx->plan_host[ri] = nullptr; ctx->plan_host_bytes[ri] = 0;
+        PF_CUDA(cudaMallocHost(&ctx->plan_host[ri], bytes * 2));
+        ctx->plan_host_bytes[ri] = bytes * 2;
+    }
+    *out = (uint8_t *)ctx->plan_host[ri];
+    *out_ri = ri;
     return PFNAV_OK;
 }
 

@@ -20,15 +20,18 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <map>
 #include "pfnav_internal.cuh"
 
 namespace {
 
 #include "pfnav_region_kernel.cuh"
+#include "pfnav_tile_geom.cuh"
 }   // namespace
 
 static int region_launch(pfnav_ctx *ctx, int dim, const pfnav_region_req *d_reqs, size_t n, const int32_t *d_seeds,
-                         const int32_t *d_overlay, uint8_t *d_fields, cudaStream_t st, int chunk_out = 0)
+                         const int32_t *d_overlay, uint8_t *d_fields, cudaStream_t st, int chunk_out = 0,
+                         const uint32_t *d_seed_bits = nullptr, const int32_t *d_out_slot = nullptr)
 {
     RegionGrids g;
     g.cost = ctx->d_cost; g.blk = ctx->d_blk; g.fmask = ctx->d_fmask; g.W64 = ctx->W64; g.H64 = ctx->H64;
@@ -37,7 +40,8 @@ static int region_launch(pfnav_ctx *ctx, int dim, const pfnav_region_req *d_reqs
                                  PFNAV_REGION_DIM_MAX * PFNAV_REGION_DIM_MAX * 6));
     const int per_sm = std::max(1, std::min(4, (int)((size_t)(227 * 1024) / (smem + 1024))));
     const int grid = (int)std::min<size_t>(n, (size_t)ctx->sm_count * per_sm);
-    k_region_fields<<<grid, RG_THREADS, smem, st>>>(g, dim, d_reqs, (int)n, d_seeds, d_overlay, d_fields, chunk_out);
+    k_region_fields<<<grid, RG_THREADS, smem, st>>>(g, dim, d_reqs, (int)n, d_seeds, d_overlay, d_fields, chunk_out,
+                                                            d_seed_bits, d_out_slot);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
     return PFNAV_OK;
@@ -559,15 +563,35 @@ extern "C" int pfnav_zone_seeds(pfnav_ctx *ctx, int layer, int chunk_r, int chun
 // BG_SCALE_F (lib/public/bitmap_grid.h:196): the position index compares scaled integers, bounds inclusive (:543)
 static inline int32_t bg_scale_f(float x) { return (int32_t)lrintf(x * 256.0f); }
 
+// contour rings around a target's footprint: field_entity_initial_frontier (field.c:1317; note `layer == GROUND_3X3` for
+// the first ring) and field_enemies_initial_frontier (field.c:1209)
+static inline int entity_rings(int kind, int ref_layer)
+{
+    return kind == PFNAV_TARGET_ENTITY ? (ref_layer == 1) + (ref_layer >= 2) + (ref_layer >= 3)
+                                       : (ref_layer >= 1) + (ref_layer >= 2) + (ref_layer >= 3);
+}
+
+// the scaled search rectangle of chunk (chunk_r, chunk_c), bounds inclusive: field_chunk_bounds (field.c:863) and
+// field.c:1229-1243, in the reference's float arithmetic
+struct search_rect { int32_t mnx, mxx, mnz, mxz; };
+static search_rect enemies_search_rect(const pfnav_ctx *ctx, int chunk_r, int chunk_c)
+{
+    const int x_offset = -(chunk_c * 256), z_offset = chunk_r * 256;
+    const float x_max = ctx->map_x + (float)x_offset, x_min = x_max - 256.0f;
+    const float z_min = ctx->map_z + (float)z_offset, z_max = z_min + 256.0f;
+    const float xlen = x_max - x_min, zlen = z_max - z_min;
+    return {bg_scale_f(x_min - xlen / 2.0f - 16.0f), bg_scale_f(x_max + xlen / 2.0f + 16.0f),
+            bg_scale_f(z_min - zlen / 2.0f - 16.0f), bg_scale_f(z_max + zlen / 2.0f + 16.0f)};
+}
+
 static int entity_seeds(const pfnav_ctx *ctx, int ref_layer, int kind, const pfnav_footprint *ents, size_t nents, int dim,
                         int chunk_r, int chunk_c, std::vector<int32_t> &out)
 {
     int base_r, base_c;
     chunk_region_base(dim, chunk_r, chunk_c, &base_r, &base_c);
     int32_t tiles[512 * 2];
+    const int rings = entity_rings(kind, ref_layer);
     if (kind == PFNAV_TARGET_ENTITY) {
-        // field_entity_initial_frontier (field.c:1317): note `layer == GROUND_3X3` for the first ring
-        const int rings = (ref_layer == 1) + (ref_layer >= 2) + (ref_layer >= 3);
         const int n = pfnav_footprint_tiles(ctx, &ents[0], rings, tiles);
         if (n < 0) { pfnav_set_error("entity field: a building corner lies outside the map"); return PFNAV_ERR_ARG; }
         for (int i = 0; i < n; i++) {
@@ -578,18 +602,11 @@ static int entity_seeds(const pfnav_ctx *ctx, int ref_layer, int kind, const pfn
         return PFNAV_OK;
     }
     // field_enemies_initial_frontier (field.c:1209)
-    const int rings = (ref_layer >= 1) + (ref_layer >= 2) + (ref_layer >= 3);
-    // field_chunk_bounds (field.c:863) and the search rectangle (:1229-1243), in the reference's float arithmetic
-    const int x_offset = -(chunk_c * 256), z_offset = chunk_r * 256;
-    const float x_max = ctx->map_x + (float)x_offset, x_min = x_max - 256.0f;
-    const float z_min = ctx->map_z + (float)z_offset, z_max = z_min + 256.0f;
-    const float xlen = x_max - x_min, zlen = z_max - z_min;
-    const int32_t imnx = bg_scale_f(x_min - xlen / 2.0f - 16.0f), imxx = bg_scale_f(x_max + xlen / 2.0f + 16.0f);
-    const int32_t imnz = bg_scale_f(z_min - zlen / 2.0f - 16.0f), imxz = bg_scale_f(z_max + zlen / 2.0f + 16.0f);
+    const search_rect R = enemies_search_rect(ctx, chunk_r, chunk_c);
     std::vector<uint8_t> has((size_t)dim * dim, 0);
     for (size_t k = 0; k < nents; k++) {
         const int32_t ix = bg_scale_f(ents[k].x), iz = bg_scale_f(ents[k].z);
-        if (ix < imnx || ix > imxx || iz < imnz || iz > imxz) continue;
+        if (ix < R.mnx || ix > R.mxx || iz < R.mnz || iz > R.mxz) continue;
         const int n = pfnav_footprint_tiles(ctx, &ents[k], rings, tiles);
         if (n < 0) { pfnav_set_error("enemies field: a building corner lies outside the map"); return PFNAV_ERR_ARG; }
         for (int i = 0; i < n; i++) {
@@ -672,65 +689,358 @@ extern "C" int pfnav_entity_fields(pfnav_ctx *ctx, int layer, int ref_layer, int
 // N_RequestAsyncSurroundField + N_AwaitAsyncFields leave in the field cache for the chunks the seekers stand on
 // (nav.c:3769-3960), consumed by N_DesiredEnemySeekVelocity / N_DesiredSurroundVelocity (k_desired_velocity).
 // ------------------------------------------------------------------------------------------
+//
+// A batch builds its seed frontiers on the device, in three launches on the caller's stream:
+//   k_footprint_rows    one warp per distinct (circle footprint, ring count) of the batch: the tiles under the circle
+//                       and its contour rings as 32 bit rows, with the circle test and the dilation of the blocker
+//                       rasterisation (pfnav_tile_geom.cuh);
+//   k_entity_seed_bits  one CTA per field: its dim x dim seed bitmap, the union of the footprint rows inside the padded
+//                       window plus the tile lists of the footprints rasterised on the host (buildings, and circles
+//                       whose rings could reach the 512-tile cap of pfnav_footprint_tiles, which truncates in list order);
+//   k_region_fields     (chunk_out with seed_bits and out_slot) integrates every field straight into its pool slot.
+// TARGET_ENEMIES footprints are binned by chunk on the host, with the scaled-integer test of entity_seeds, so the work
+// grows with footprints x 9 and not with fields x footprints. The device work only writes pool slots; when several
+// fields of a batch end in the same slot (a repeated (dest, chunk), or a slot evicted and handed out again inside the
+// batch) only the last is built, which is what the serial calls leave there.
+namespace {
+
+struct fp_job { float x, z, radius; int32_t rings; };
+
+__global__ void __launch_bounds__(128) k_footprint_rows(const fp_job *__restrict__ jobs, int n, geom g, int H64, int W64,
+                                                        int2 *__restrict__ org, uint32_t *__restrict__ rows_out)
+{
+    __shared__ unsigned rows[4][32];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, j = blockIdx.x * 4 + w;
+    if (j >= n) return;
+    const fp_job f = jobs[j];
+    td ct;
+    unsigned u = 0;
+    int r0 = 0, c0 = 0;
+    if (desc_for_point(g, f.x, f.z, &ct)) {          // otherwise no tile under the circle (tile.c:693) and no ring
+        const int nt = (int)ceilf(f.radius / 4);
+        r0 = ct.chunk_r * 64 + ct.tile_r - nt - 3; c0 = ct.chunk_c * 64 + ct.tile_c - nt - 3;
+        rows[w][lane] = 0;
+        __syncwarp();
+        circle_rows(g, H64, W64, v2f{f.x, f.z}, f.radius, nt, r0, c0, rows[w], lane);
+        const unsigned inmap = window_inmap(H64, W64, r0, c0, 2 * nt + 7, lane);
+        u = rows[w][lane];
+        for (int k = 0; k < f.rings; k++) u |= contour_rows(u, inmap, lane);     // each ring around all tiles so far
+    }
+    if (lane == 0) org[j] = make_int2(r0, c0);
+    rows_out[(size_t)j * 32 + lane] = u;
+}
+
+// field f: items[item_off[f] ..) name k_footprint_rows outputs, hitems[hitem_off[f] ..) host tile lists
+__global__ void __launch_bounds__(256) k_entity_seed_bits(const pfnav_region_req *__restrict__ reqs, int dim,
+                                                          const uint32_t *__restrict__ item_off, const int32_t *__restrict__ items,
+                                                          const int2 *__restrict__ org, const uint32_t *__restrict__ rows,
+                                                          const uint32_t *__restrict__ hitem_off, const int32_t *__restrict__ hitems,
+                                                          const uint32_t *__restrict__ htile_off, const int32_t *__restrict__ htiles,
+                                                          uint32_t *__restrict__ bits_out)
+{
+    __shared__ uint32_t bm[PFNAV_REGION_DIM_MAX * PFNAV_REGION_DIM_MAX / 32];
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int wpr = dim >> 5, nw = dim * wpr;           // dim is 64 or 128: whole words per row
+    for (int i = tid; i < nw; i += blockDim.x) bm[i] = 0;
+    __syncthreads();
+    const pfnav_region_req rq = reqs[f];
+    const int base_r = (rq.center_r > 0 && dim > 64) ? rq.center_r * 64 - 32 : rq.center_r * 64;
+    const int base_c = (rq.center_c > 0 && dim > 64) ? rq.center_c * 64 - 32 : rq.center_c * 64;
+    // one thread per (footprint, window row): the row's 32 columns land in at most two bitmap words
+    for (uint32_t t = item_off[f] * 32 + tid; t < item_off[f + 1] * 32; t += blockDim.x) {
+        const int32_t it = items[t >> 5];
+        const int row = t & 31;
+        const uint32_t v = rows[(size_t)it * 32 + row];
+        if (!v) continue;
+        const int2 o = org[it];
+        const int dr = o.x + row - base_r, off = o.y - base_c;      // off: the field column of bit 0
+        if (dr < 0 || dr >= dim || off <= -32 || off >= dim) continue;
+        const uint64_t x = off >= 0 ? (uint64_t)v << (off & 31) : (uint64_t)(v >> -off);
+        const int wc = off >= 0 ? off >> 5 : 0;
+        if ((uint32_t)x) atomicOr(&bm[dr * wpr + wc], (uint32_t)x);
+        if (wc + 1 < wpr && (uint32_t)(x >> 32)) atomicOr(&bm[dr * wpr + wc + 1], (uint32_t)(x >> 32));
+    }
+    for (uint32_t k = hitem_off[f]; k < hitem_off[f + 1]; k++) {
+        const int32_t h = hitems[k];
+        for (uint32_t t = htile_off[h] + tid; t < htile_off[h + 1]; t += blockDim.x) {
+            const int dr = htiles[2 * t] - base_r, dc = htiles[2 * t + 1] - base_c;
+            if (dr >= 0 && dr < dim && dc >= 0 && dc < dim) atomicOr(&bm[dr * wpr + (dc >> 5)], 1u << (dc & 31));
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < nw; i += blockDim.x) bits_out[(size_t)f * nw + i] = bm[i];
+}
+
+}   // namespace
+
+// k_footprint_rows rasterises a circle when its tiles and rings fit the 32 x 32 window and can not reach the 512-tile cap
+// of pfnav_footprint_tiles: then they are the same set, whatever their order
+static bool footprint_on_device(const pfnav_footprint &e, int rings)
+{
+    if (e.is_building || !std::isfinite(e.x) || !std::isfinite(e.z) || !(e.sel_radius >= 0.0f && e.sel_radius <= 64.0f))
+        return false;
+    const int side = 2 * (int)ceil(e.sel_radius / 4) + 1 + 2 * rings;
+    return side * side <= 512;
+}
+
+static bool building_corners_ok(const pfnav_ctx *ctx, const pfnav_footprint &e)
+{
+    if (!e.is_building) return true;
+    const geom g = {ctx->map_x, ctx->map_z, ctx->chunk_w, ctx->chunk_h};
+    td t;
+    for (int i = 0; i < 4; i++)
+        if (!desc_for_point(g, e.corners_xz[2 * i], e.corners_xz[2 * i + 1], &t)) return false;
+    return true;
+}
+
+// TARGET_ENEMIES footprints of one range, binned by the chunks whose search rectangle holds their position
+struct enemy_bins {
+    std::vector<uint32_t> off;           // [chunks + 1]
+    std::vector<uint32_t> ent;           // absolute footprint indices
+    std::vector<uint8_t> bad;            // [chunks]: a building in the bin has a corner outside the map
+};
+
+static void bin_enemies(const pfnav_ctx *ctx, const pfnav_footprint *ents, uint32_t off, uint32_t n, enemy_bins &B)
+{
+    const int cw = ctx->chunk_w, chh = ctx->chunk_h, nch = cw * chh;
+    std::vector<search_rect> rx(cw), rz(chh);
+    for (int c = 0; c < cw; c++) rx[c] = enemies_search_rect(ctx, 0, c);
+    for (int r = 0; r < chh; r++) rz[r] = enemies_search_rect(ctx, r, 0);
+    // the chunks whose rectangle holds a position form a contiguous block (the rectangles are translates)
+    std::vector<int32_t> span((size_t)n * 4);
+    B.off.assign(nch + 1, 0);
+    for (uint32_t k = 0; k < n; k++) {
+        const int32_t ix = bg_scale_f(ents[off + k].x), iz = bg_scale_f(ents[off + k].z);
+        int c0 = cw, c1 = -1, r0 = chh, r1 = -1;
+        for (int c = 0; c < cw; c++) if (ix >= rx[c].mnx && ix <= rx[c].mxx) { c0 = std::min(c0, c); c1 = c; }
+        for (int r = 0; r < chh; r++) if (iz >= rz[r].mnz && iz <= rz[r].mxz) { r0 = std::min(r0, r); r1 = r; }
+        int32_t *s = &span[(size_t)k * 4];
+        s[0] = r0; s[1] = r1; s[2] = c0; s[3] = c1;
+        for (int r = r0; r <= r1; r++)
+            for (int c = c0; c <= c1; c++) B.off[r * cw + c + 1]++;
+    }
+    for (int i = 0; i < nch; i++) B.off[i + 1] += B.off[i];
+    B.ent.resize(B.off[nch]);
+    B.bad.assign(nch, 0);
+    std::vector<uint32_t> cur(B.off.begin(), B.off.end() - 1);
+    for (uint32_t k = 0; k < n; k++) {
+        const int32_t *s = &span[(size_t)k * 4];
+        const bool bad = !building_corners_ok(ctx, ents[off + k]);
+        for (int r = s[0]; r <= s[1]; r++)
+            for (int c = s[2]; c <= s[3]; c++) { B.ent[cur[r * cw + c]++] = off + k; B.bad[r * cw + c] |= bad; }
+    }
+}
+
+extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                                      const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc,
+                                                      size_t nchunks, void *stream, int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_cost && ctx->d_pool_slot, "map / pool not created");
+    PF_ARG(m == 0 || reqs, "reqs");
+    PF_ARG((nents == 0 || ents) && (nchunks == 0 || chunks_rc), "ents / chunks_rc");
+    PF_ARG(m < (1u << 24) && nents < (1u << 24) && nchunks < (1u << 24), "m / nents / nchunks");
+    const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
+    // ---- the whole batch is checked before anything changes
+    bool any_fields = false;
+    for (size_t i = 0; i < m; i++) {
+        const pfnav_entity_field_req &q = reqs[i];
+        PF_ARG(q.dest >= 0 && q.dest < ctx->pool_ndests, "dest");
+        PF_ARG(q.layer >= 0 && q.layer < ctx->nlayers, "layer");
+        PF_ARG((uint64_t)q.ent_off + q.ent_n <= nents, "footprint range");
+        PF_ARG((uint64_t)q.chunk_off + q.chunk_n <= nchunks, "chunk range");
+        int rc = entity_args_ok(ctx, q.ref_layer, q.target_kind, ents + q.ent_off, q.ent_n);
+        if (rc) return rc;
+        for (uint32_t k = 0; k < q.chunk_n; k++) {
+            const int32_t *c = chunks_rc + 2 * ((size_t)q.chunk_off + k);
+            PF_ARG(c[0] >= 0 && c[0] < ctx->chunk_h && c[1] >= 0 && c[1] < cw, "entity field: chunk");
+        }
+        any_fields |= q.chunk_n > 0;
+    }
+    int dim = 0;
+    if (any_fields) {
+        int rc = zone_dim(ctx, &dim);
+        if (rc) return rc;
+    }
+    // TARGET_ENEMIES bins, one per distinct footprint range; building corners of every footprint a field will use
+    std::vector<enemy_bins> bins;
+    std::map<std::pair<uint32_t, uint32_t>, int> bin_of;
+    std::vector<int32_t> req_bin(m, -1);
+    for (size_t i = 0; i < m; i++) {
+        const pfnav_entity_field_req &q = reqs[i];
+        if (q.chunk_n == 0) continue;
+        if (q.target_kind == PFNAV_TARGET_ENTITY) {
+            PF_ARG(building_corners_ok(ctx, ents[q.ent_off]), "entity field: a building corner lies outside the map");
+            continue;
+        }
+        auto it = bin_of.find({q.ent_off, q.ent_n});
+        if (it == bin_of.end()) {
+            it = bin_of.emplace(std::make_pair(q.ent_off, q.ent_n), (int)bins.size()).first;
+            bins.emplace_back();
+            bin_enemies(ctx, ents, q.ent_off, q.ent_n, bins.back());
+        }
+        req_bin[i] = it->second;
+        for (uint32_t k = 0; k < q.chunk_n; k++) {
+            const int32_t *c = chunks_rc + 2 * ((size_t)q.chunk_off + k);
+            PF_ARG(!bins[it->second].bad[c[0] * cw + c[1]], "enemies field: a building corner lies outside the map");
+        }
+    }
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_fields_join(ctx, st));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    // ---- slots request by request, in order: the serial calls' reservations and evictions
+    if (ctx->aux.size() < (size_t)ctx->pool_ndests) ctx->aux.resize(ctx->pool_ndests);
+    struct field_t { uint32_t req; int32_t cr, cc, slot; };
+    std::vector<field_t> fields;
+    std::vector<size_t> keys;
+    std::vector<int32_t> slots;
+    int rc = PFNAV_OK;
+    size_t done = 0;
+    for (; done < m; done++) {
+        const pfnav_entity_field_req &q = reqs[done];
+        const int32_t *crc = chunks_rc + 2 * (size_t)q.chunk_off;
+        if (q.chunk_n) {
+            keys.resize(q.chunk_n); slots.resize(q.chunk_n);
+            for (uint32_t k = 0; k < q.chunk_n; k++) keys[k] = (size_t)q.dest * nch + crc[2 * k] * cw + crc[2 * k + 1];
+            bool evicted = false;
+            if ((rc = pf_pool_reserve(ctx, keys.data(), q.chunk_n, slots.data(), &evicted))) break;
+        }
+        // the footprints stay with the destination: the in-place repairs of its fields start from them (field.c:2334-2360)
+        pfnav_ctx::aux_target &A = ctx->aux[q.dest];
+        A.kind = q.target_kind; A.layer = q.layer; A.ref_layer = q.ref_layer; A.ents.assign(ents + q.ent_off, ents + q.ent_off + q.ent_n);
+        for (uint32_t k = 0; k < q.chunk_n; k++) {
+            ctx->h_pool_has[slots[k]] |= 1;
+            pfnav_field_req fr;
+            memset(&fr, 0, sizeof(fr));
+            fr.chunk_r = crc[2 * k]; fr.chunk_c = crc[2 * k + 1]; fr.layer = q.layer; fr.faction_id = PFNAV_FACTION_ID_NONE;
+            fr.target_type = 2 + q.target_kind;      // beyond the chunk-local kinds: the frontier comes from ctx->aux[dest]
+            fr._pad = q.dest;
+            ctx->h_pool_req[slots[k]] = fr;
+            fields.push_back({(uint32_t)done, crc[2 * k], crc[2 * k + 1], slots[k]});
+        }
+    }
+    if (out_ndone) *out_ndone = (int)done;
+    if (fields.empty()) return rc;
+    ctx->goal_batch.valid = false;
+    // ---- the last field written to each slot, its footprints and their rasters
+    std::vector<int32_t> last(ctx->pool_max, -1);
+    for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
+    std::vector<pfnav_region_req> kreq;
+    std::vector<int32_t> kslot, items, hitems, htiles;
+    std::vector<uint32_t> item_off(1, 0), hitem_off(1, 0), htile_off(1, 0);
+    std::vector<fp_job> jobs;
+    std::vector<int32_t> raster((size_t)4 * nents, -1);      // (rings, footprint) -> job, or -2 - host list
+    auto use = [&](uint32_t e, int rings) {
+        int32_t &id = raster[(size_t)rings * nents + e];
+        if (id == -1) {
+            const pfnav_footprint &E = ents[e];
+            if (footprint_on_device(E, rings)) {
+                id = (int32_t)jobs.size();
+                jobs.push_back({E.x, E.z, E.sel_radius, rings});
+            } else {
+                int32_t tiles[512 * 2];
+                const int n = std::max(pfnav_footprint_tiles(ctx, &E, rings, tiles), 0);    // corners checked above
+                id = -2 - (int32_t)(htile_off.size() - 1);
+                htiles.insert(htiles.end(), tiles, tiles + 2 * n);
+                htile_off.push_back((uint32_t)(htiles.size() / 2));
+            }
+        }
+        if (id >= 0) items.push_back(id);
+        else hitems.push_back(-2 - id);
+    };
+    for (size_t f = 0; f < fields.size(); f++) {
+        const field_t &F = fields[f];
+        if (last[F.slot] != (int32_t)f) continue;
+        const pfnav_entity_field_req &q = reqs[F.req];
+        const int rings = entity_rings(q.target_kind, q.ref_layer);
+        if (q.target_kind == PFNAV_TARGET_ENTITY) use(q.ent_off, rings);
+        else {
+            const enemy_bins &B = bins[req_bin[F.req]];
+            const int c = F.cr * cw + F.cc;
+            for (uint32_t k = B.off[c]; k < B.off[c + 1]; k++) use(B.ent[k], rings);
+        }
+        pfnav_region_req rq = {};
+        rq.layer = q.layer; rq.center_r = F.cr; rq.center_c = F.cc; rq.flags = PFNAV_REGION_CREATE;
+        kreq.push_back(rq); kslot.push_back(F.slot);
+        item_off.push_back((uint32_t)items.size()); hitem_off.push_back((uint32_t)hitems.size());
+    }
+    const size_t nk = kreq.size(), nj = jobs.size();
+    // ---- one pinned staging buffer: the inputs (copied into the device scratch), then the slot table and `has` bytes
+    size_t b_in = 0;
+    auto sec = [&](size_t bytes) { const size_t o = b_in; b_in = (b_in + bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_req = sec(nk * sizeof(pfnav_region_req)), o_slot = sec(nk * 4);
+    const size_t o_ioff = sec(item_off.size() * 4), o_items = sec(items.size() * 4);
+    const size_t o_hoff = sec(hitem_off.size() * 4), o_hitems = sec(hitems.size() * 4);
+    const size_t o_jobs = sec(nj * sizeof(fp_job)), o_toff = sec(htile_off.size() * 4), o_tiles = sec(htiles.size() * 4);
+    const size_t b_slot = ctx->h_pool_slot.size() * 4, stage = b_in + b_slot + (size_t)ctx->pool_max;
+    const size_t o_org = b_in + 0, o_rows = o_org + ((nj * 8 + 15) & ~(size_t)15), o_bits = o_rows + nj * 128;
+    const size_t need = o_bits + nk * ((size_t)dim * dim / 8);
+    uint8_t *host = nullptr;
+    int ri = 0;
+    if ((rc = pf_plan_host(ctx, stage, &host, &ri))) return rc;
+    memcpy(host + o_req, kreq.data(), nk * sizeof(pfnav_region_req));
+    memcpy(host + o_slot, kslot.data(), nk * 4);
+    memcpy(host + o_ioff, item_off.data(), item_off.size() * 4);
+    memcpy(host + o_items, items.data(), items.size() * 4);
+    memcpy(host + o_hoff, hitem_off.data(), hitem_off.size() * 4);
+    memcpy(host + o_hitems, hitems.data(), hitems.size() * 4);
+    memcpy(host + o_jobs, jobs.data(), nj * sizeof(fp_job));
+    memcpy(host + o_toff, htile_off.data(), htile_off.size() * 4);
+    memcpy(host + o_tiles, htiles.data(), htiles.size() * 4);
+    memcpy(host + b_in, ctx->h_pool_slot.data(), b_slot);
+    memcpy(host + b_in + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
+    // the device scratch is reused by the next batch, possibly on another stream: order its overwrite after this batch
+    if (!ctx->ent_ev) PF_CUDA(cudaEventCreateWithFlags(&ctx->ent_ev, cudaEventDisableTiming));
+    else PF_CUDA(cudaStreamWaitEvent(st, ctx->ent_ev, 0));
+    if (ctx->ent_buf_bytes < need) {        // grow-only: the old buffer may still be read by the previous batch
+        PF_CUDA(cudaEventSynchronize(ctx->ent_ev));
+        cudaFree(ctx->d_ent_buf);
+        ctx->d_ent_buf = nullptr; ctx->ent_buf_bytes = 0;
+        PF_CUDA(cudaMalloc(&ctx->d_ent_buf, need * 2));
+        ctx->ent_buf_bytes = need * 2;
+    }
+    uint8_t *dev = (uint8_t *)ctx->d_ent_buf;
+    PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_in, b_slot, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_in + b_slot, ctx->pool_max,
+                            cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    const pfnav_region_req *d_req = (const pfnav_region_req *)(dev + o_req);
+    int2 *d_org = (int2 *)(dev + o_org);
+    uint32_t *d_rows = (uint32_t *)(dev + o_rows), *d_bits = (uint32_t *)(dev + o_bits);
+    if (nj) {
+        const geom g = {ctx->map_x, ctx->map_z, cw, ctx->chunk_h};
+        k_footprint_rows<<<(unsigned)((nj + 3) / 4), 128, 0, st>>>((const fp_job *)(dev + o_jobs), (int)nj, g, ctx->H64, ctx->W64,
+                                                                 d_org, d_rows);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+    }
+    k_entity_seed_bits<<<(unsigned)nk, 256, 0, st>>>(d_req, dim, (const uint32_t *)(dev + o_ioff), (const int32_t *)(dev + o_items),
+                                                     d_org, d_rows, (const uint32_t *)(dev + o_hoff), (const int32_t *)(dev + o_hitems),
+                                                     (const uint32_t *)(dev + o_toff), (const int32_t *)(dev + o_tiles), d_bits);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    const int lrc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, ctx->d_pool_flow, st, 1, d_bits,
+                                  (const int32_t *)(dev + o_slot));
+    if (lrc) return lrc;
+    PF_CUDA(cudaEventRecord(ctx->ent_ev, st));
+    return rc;
+}
+
 extern "C" int pfnav_pool_request_entity_fields(pfnav_ctx *ctx, int dest, int layer, int ref_layer, int target_kind,
                                                 const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc, size_t n,
                                                 void *stream)
 {
     PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
-    PF_NEED_DEVICE(ctx);
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
-    PF_ARG(layer >= 0 && layer < ctx->nlayers, "layer");
-    int rc = entity_args_ok(ctx, ref_layer, target_kind, ents, nents);
+    PF_ARG(nents < (1u << 24) && n < (1u << 24), "nents / n");
+    const pfnav_entity_field_req q = {dest, layer, ref_layer, target_kind, 0, (uint32_t)nents, 0, (uint32_t)n};
+    int rc = pfnav_pool_request_entity_fields_batch(ctx, &q, 1, ents, nents, chunks_rc, n, stream, nullptr);
     if (rc) return rc;
-    // the footprints stay with the destination: the in-place repairs of its fields start from them (field.c:2334-2360)
-    if (ctx->aux.size() < (size_t)ctx->pool_ndests) ctx->aux.resize(ctx->pool_ndests);
-    pfnav_ctx::aux_target &A = ctx->aux[dest];
-    A.kind = target_kind; A.layer = layer; A.ref_layer = ref_layer; A.ents.assign(ents, ents + nents);
-    if (n == 0) return PFNAV_OK;
-    PF_ARG(chunks_rc, "chunks");
-    int dim = 0;
-    if ((rc = zone_dim(ctx, &dim))) return rc;
-    const int chunks = ctx->chunk_w * ctx->chunk_h;
-    std::vector<int32_t> seeds;
-    std::vector<size_t> off(n + 1, 0), keys(n);
-    for (size_t i = 0; i < n; i++) {
-        const int cr = chunks_rc[2 * i], cc = chunks_rc[2 * i + 1];
-        PF_ARG(cr >= 0 && cr < ctx->chunk_h && cc >= 0 && cc < ctx->chunk_w, "entity field: chunk");
-        if ((rc = entity_seeds(ctx, ref_layer, target_kind, ents, nents, dim, cr, cc, seeds))) return rc;
-        off[i + 1] = seeds.size() / 2;
-        keys[i] = (size_t)dest * chunks + cr * ctx->chunk_w + cc;
-    }
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_fields_sync(ctx));
-    cudaStream_t st = pf_stream(ctx, stream);
-    PF_CUDA(pf_pool_refresh(ctx, st));
-    std::vector<int32_t> slots(n);
-    bool evicted = false;
-    if ((rc = pf_pool_reserve(ctx, keys.data(), n, slots.data(), &evicted))) return rc;
-    uint8_t *d_out = nullptr;
-    PF_CUDA(cudaMalloc(&d_out, n * 4096));
-    rc = chunk_fields_launch(ctx, layer, dim, chunks_rc, n, seeds, off, d_out, st);
-    for (size_t i = 0; i < n && rc == 0; i++) {
-        if (cudaMemcpyAsync(ctx->d_pool_flow + (size_t)slots[i] * 4096, d_out + i * 4096, 4096, cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
-            pfnav_set_error("pfnav_pool_request_entity_fields: copy into the pool failed"); rc = PFNAV_ERR_CUDA;
-        }
-        ctx->h_pool_has[slots[i]] |= 1;
-        pfnav_field_req q;
-        memset(&q, 0, sizeof(q));
-        q.chunk_r = chunks_rc[2 * i]; q.chunk_c = chunks_rc[2 * i + 1]; q.layer = layer; q.faction_id = PFNAV_FACTION_ID_NONE;
-        q.target_type = 2 + target_kind;          // beyond the chunk-local kinds: the frontier comes from ctx->aux[dest]
-        q._pad = dest;
-        ctx->h_pool_req[slots[i]] = q;
-    }
-    if (rc == 0) {
-        cudaError_t e = cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) { pfnav_set_error("pfnav_pool_request_entity_fields: %s", cudaGetErrorString(e)); rc = PFNAV_ERR_CUDA; }
-    }
-    cudaFree(d_out);
-    ctx->goal_batch.valid = false;
-    return rc;
+    PF_CUDA(cudaStreamSynchronize(pf_stream(ctx, stream)));      // returns once the fields are in the pool
+    return PFNAV_OK;
 }
 
 // the chunk-local frontier of a TARGET_ENEMIES / TARGET_ENTITY pool destination (field_enemies_initial_frontier /

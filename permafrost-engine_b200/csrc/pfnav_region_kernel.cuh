@@ -121,7 +121,8 @@ __device__ __forceinline__ uint32_t region_flow_dir(const uint32_t *f, int n, in
 __global__ void __launch_bounds__(RG_THREADS, 4) k_region_fields(RegionGrids g, int dim, const pfnav_region_req *__restrict__ reqs,
                                                               int n, const int32_t *__restrict__ seeds,
                                                               const int32_t *__restrict__ overlay, uint8_t *__restrict__ fields,
-                                                              int chunk_out)
+                                                              int chunk_out, const uint32_t *__restrict__ seed_bits = nullptr,
+                                                              const int32_t *__restrict__ out_slot = nullptr)
 {
     extern __shared__ uint32_t rg_smem[];
     RegionSmem s;
@@ -131,7 +132,8 @@ __global__ void __launch_bounds__(RG_THREADS, 4) k_region_fields(RegionGrids g, 
 
     for (int q = blockIdx.x; q < n; q += gridDim.x) {
         const pfnav_region_req rq = reqs[q];
-        uint8_t *out = fields + (size_t)q * (chunk_out ? 4096 : N / 2);
+        // out_slot: field q goes to its pool slot instead of position q
+        uint8_t *out = fields + (size_t)(out_slot ? out_slot[q] : q) * (chunk_out ? 4096 : N / 2);
         const int32_t *ov = overlay + 2 * (size_t)rq.overlay_off;
         __syncthreads();
 
@@ -143,9 +145,11 @@ __global__ void __launch_bounds__(RG_THREADS, 4) k_region_fields(RegionGrids g, 
             const int base_r = rq.center_r * 64 - roff, base_c = rq.center_c * 64 - coff;
             const int32_t *sd = seeds + 2 * (size_t)rq.seed_off;
             region_gather(g, s, rq.layer, base_r, base_c, 0, ov, 0);
+            // seed_bits: the frontier as dim x dim bits (row-major, N / 32 words per field) instead of a tile list
+            const uint32_t *bits = seed_bits ? seed_bits + (size_t)q * (N / 32) : nullptr;
             for (int i = tid; i < N; i += RG_THREADS) {
                 const uint8_t f = s.flg[i];
-                s.dist[i] = RG_INF;
+                s.dist[i] = (bits && ((bits[i >> 5] >> (i & 31)) & 1u)) ? 0u : RG_INF;
                 if ((f & (RG_EXISTS | RG_PASSP)) == (RG_EXISTS | RG_PASSP)) s.flg[i] = f | RG_ENT;
             }
             __syncthreads();
