@@ -393,8 +393,9 @@ int  pfnav_group_arrival_field(pfnav_ctx *ctx, int layer, int dim, uint16_t enem
 /* Group arrival (TARGET_ZONE) fields: a flock arriving at its goal follows one shared field per chunk into the
  * open tiles around the goal (arrival.c:859 -> N_RequestAsyncGroupArrivalField nav.c:3921 -> field task ->
  * N_FlowFieldUpdate field.c:2050 -> field_update_zone :1810). The seeds are the first pi * radius^2 open tiles of a
- * best-first flood from the centre (field_zone_initial_frontier, field.c:1683; computed on the host with the
- * reference's heap order), the integration runs on the device over the chunk padded by half a chunk, and the
+ * best-first flood from the centre (field_zone_initial_frontier, field.c:1683, in the reference's heap order: on the
+ * host in pfnav_zone_seeds / pfnav_zone_fields, on the device in the pool requests), the integration runs on the device
+ * over the chunk padded by half a chunk, and the
  * chunk's 64 x 64 window is written one direction per byte. Call pfnav_map_commit first when blockers changed.
  * Only maps with more than one chunk row AND column (or exactly 1 x 1) are accepted: with one of the two the
  * reference indexes its padded buffer out of bounds. centre_r / centre_c: absolute nav tile of the zone centre. */
@@ -405,9 +406,39 @@ int  pfnav_zone_fields(pfnav_ctx *ctx, int layer, int centre_r, int centre_c, in
                        size_t n, uint8_t *out_fields);
 /* N_RequestAsyncGroupArrivalField + N_AwaitAsyncFields (nav.c:3921, 3958): the zone fields of every chunk within
  * reach (2 * radius tiles) of the world-space centre go into pool destination `dest` as its flow fields. A centre
- * outside the map requests nothing. Returns when the fields are in the pool. */
+ * outside the map requests nothing. Returns when the fields are in the pool. The one-request case of
+ * pfnav_pool_request_zones followed by a synchronise of `stream`. */
 int  pfnav_pool_request_zone(pfnav_ctx *ctx, int dest, int layer, const float *centre_xz, int radius, void *stream,
                              int *out_nfields);
+/* One request of pfnav_pool_request_zones: the arguments of one pfnav_pool_request_zone call. */
+typedef struct pfnav_zone_req {        /* 24 bytes */
+    int32_t dest, layer;
+    float   centre_x, centre_z;        /* world space, as pfnav_pool_request_zone's centre_xz */
+    int32_t radius;                    /* 0 .. 0xFFFF */
+    int32_t _pad;
+} pfnav_zone_req;
+/* N_RequestAsyncGroupArrivalField calls queued during a tick and built at once by N_AwaitAsyncFields: m zone requests
+ * against the device field pool in one call.
+ * - Equivalence: the pool ends exactly as pfnav_pool_request_zone(ctx, reqs[i].dest, ...) leaves it when called for
+ *   i = 0 .. m-1 in order: flow bytes, `has` bits, the (dest, chunk) -> slot mapping pfnav_pool_get exposes, ff_ids and
+ *   the pool's remaining capacity. Zone fields take a fresh slot for a (dest, chunk) without one; they never evict and
+ *   never reuse slots freed by eviction. A repeated (dest, chunk) ends with the last request's field.
+ *   out_nfields[i] (may be NULL) = the fields request i put in the pool.
+ * - A centre outside the map requests nothing: out_nfields[i] = 0, and the request counts as done.
+ * - The whole batch is validated before anything changes: dest, layer, radius, null pointers, and a map shape the padded
+ *   chunk fields support (more than one chunk row and column, or 1 x 1) when any centre lies on the map. Failure:
+ *   PFNAV_ERR_ARG, *out_ndone = 0, nothing changed. This differs from pfnav_pool_request_zone before the batch existed:
+ *   on a map with one chunk row or column it reserved its pool slots before rejecting the request.
+ * - If chunk j of request k does not fit the pool, requests 0 .. k-1 are done, request k's chunks before j stay reserved
+ *   without fields (as the single call leaves them), *out_ndone = k (may be NULL) and PFNAV_ERR_NOMEM is returned.
+ * - Launches are asynchronous on `stream` (NULL: the context's stream) and ordered after the field work forked by
+ *   pfnav_pool_request_goals and after pfnav_pool_clear. The inputs are copied before the call returns. The call does not
+ *   wait for the device. The seed floods (field_zone_initial_frontier, field.c:1683) run on the device, or on the host
+ *   when the batch's flood budgets add up to at most ten times its largest one (a few large zones, a single request):
+ *   a device flood runs on one lane and the batch waits for its longest flood. Results are identical either way.
+ * - Host-only context: PFNAV_ERR_NO_DEVICE. */
+int  pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, void *stream,
+                              int32_t *out_nfields, int *out_ndone);
 /* N_DesiredGroupArrivalVelocity (nav.c:3561) for n world positions against pool destination `dest`:
  * out_vel[n][2] = N_FlowDir of the tile's direction; out_flags[n]: bit 0 = the call returned true (position and centre on
  * the map, chunk field present), bit 1 = *out_at_slot (FD_NONE within `radius` tiles of the centre). HOST buffers. */

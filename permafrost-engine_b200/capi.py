@@ -77,6 +77,8 @@ TARGET_ENTITY, TARGET_ENEMIES = 0, 1
 ENTITY_FIELD_REQ = np.dtype([("dest", "<i4"), ("layer", "<i4"), ("ref_layer", "<i4"), ("target_kind", "<i4"),
                              ("ent_off", "<u4"), ("ent_n", "<u4"), ("chunk_off", "<u4"), ("chunk_n", "<u4")])
 assert ENTITY_FIELD_REQ.itemsize == 32
+ZONE_REQ = np.dtype([("dest", "<i4"), ("layer", "<i4"), ("centre_x", "<f4"), ("centre_z", "<f4"), ("radius", "<i4"), ("_pad", "<i4")])
+assert ZONE_REQ.itemsize == 24
 
 LOS_PREV_INPLACE = -3
 TICK_VDES_FROM_POOL = 1
@@ -103,7 +105,7 @@ SYMBOLS = [
     "pfnav_group_create", "pfnav_group_gather", "pfnav_group_destroy", "pfnav_agents_upload_shard",
     "pfnav_pool_request_goals_ex", "pfnav_blockers_batch", "pfnav_map_set_pos",
     "pfnav_agents_upload_formation", "pfnav_agents_upload_movestate_ext", "pfnav_pool_request_entity_fields",
-    "pfnav_pool_request_entity_fields_batch",
+    "pfnav_pool_request_entity_fields_batch", "pfnav_pool_request_zones",
     "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
     "pfnav_profile_read_host",
 ]
@@ -158,6 +160,7 @@ def load():
     L.pfnav_zone_seeds.argtypes = [C.c_void_p] + [C.c_int] * 6 + [C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfnav_zone_fields.argtypes = [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_pool_request_zone.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int)]
+    L.pfnav_pool_request_zones.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
     L.pfnav_group_arrival_velocity.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.pfnav_group_arrival_field.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_uint16, C.c_void_p, C.c_size_t, C.c_void_p,
                                             C.c_void_p, C.c_size_t, C.c_void_p]
@@ -482,6 +485,18 @@ class Nav:
         c = np.ascontiguousarray(centre_xz, np.float32); n = C.c_int(0)
         _chk(self.L.pfnav_pool_request_zone(self.h, dest, layer, _p(c), int(radius), C.c_void_p(stream), C.byref(n)))
         return n.value
+
+    def pool_request_zones(self, reqs, stream=0):
+        """pool_request_zone for every ZONE_REQ record of `reqs`, in order, in one asynchronous call -> (ndone, nfields
+        int32[len(reqs)]). ndone < len(reqs): the pool could not hold request ndone's fields (PFNAV_ERR_NOMEM); requests
+        before it are done."""
+        reqs = np.ascontiguousarray(reqs, ZONE_REQ)
+        nf = np.zeros(len(reqs), np.int32); ndone = C.c_int(0)
+        rc = self.L.pfnav_pool_request_zones(self.h, _p(reqs) if len(reqs) else None, len(reqs), C.c_void_p(stream),
+                                             _p(nf) if len(reqs) else None, C.byref(ndone))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        return ndone.value, nf
 
     def group_arrival_velocity(self, dest, centre_xz, radius, pos_xz):
         c = np.ascontiguousarray(centre_xz, np.float32); pos = np.ascontiguousarray(pos_xz, np.float32).reshape(-1, 2)

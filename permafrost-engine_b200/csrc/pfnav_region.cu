@@ -27,6 +27,7 @@ namespace {
 
 #include "pfnav_region_kernel.cuh"
 #include "pfnav_tile_geom.cuh"
+#include "pfnav_zone_kernel.cuh"
 }   // namespace
 
 static int region_launch(pfnav_ctx *ctx, int dim, const pfnav_region_req *d_reqs, size_t n, const int32_t *d_seeds,
@@ -435,62 +436,219 @@ extern "C" int pfnav_zone_fields(pfnav_ctx *ctx, int layer, int centre_r, int ce
     return rc;
 }
 
+// The device scratch of the entity and zone field batches (context-owned, grow-only): the next batch may run on another
+// stream, so its overwrite is ordered after the last batch's kernels through ent_ev; record ent_ev after the kernels
+// that read it.
+static int batch_scratch(pfnav_ctx *ctx, cudaStream_t st, size_t need, uint8_t **out)
+{
+    if (!ctx->ent_ev) PF_CUDA(cudaEventCreateWithFlags(&ctx->ent_ev, cudaEventDisableTiming));
+    else PF_CUDA(cudaStreamWaitEvent(st, ctx->ent_ev, 0));
+    if (ctx->ent_buf_bytes < need) {        // grow-only: the old buffer may still be read by the previous batch
+        PF_CUDA(cudaEventSynchronize(ctx->ent_ev));
+        cudaFree(ctx->d_ent_buf);
+        ctx->d_ent_buf = nullptr; ctx->ent_buf_bytes = 0;
+        PF_CUDA(cudaMalloc(&ctx->d_ent_buf, need * 2));
+        ctx->ent_buf_bytes = need * 2;
+    }
+    *out = (uint8_t *)ctx->d_ent_buf;
+    return PFNAV_OK;
+}
+
+// the pool entries a zone batch changed: slot table entries fresh[2i] = fresh[2i + 1], `has` bytes has[slot[i]] = hasv[i]
+__global__ void k_pool_scatter(const int32_t *__restrict__ fresh, int nfresh, int32_t *__restrict__ slot_table,
+                               const int32_t *__restrict__ slot, const uint8_t *__restrict__ hasv, int nhas, uint8_t *__restrict__ has)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < nfresh) slot_table[fresh[2 * i]] = fresh[2 * i + 1];
+    if (i < nhas) has[slot[i]] = hasv[i];
+}
+
+// A batch floods its zone seeds on the host when the sum of its floods' budgets is at most this many times the largest one.
+// The device replays a flood on one lane, about ten times slower per popped tile than the host (H100, DESIGN.md §5), and
+// a batch waits for its longest flood; the host floods one field after another.
+#define PF_ZONE_HOST_POP_RATIO 10
+
+// N_RequestAsyncGroupArrivalField (nav.c:3921) for m requests, in the order of the serial calls. Slots follow the single
+// call's rule (a fresh slot from pool_used, no eviction, no pool_free reuse, only `has` bit 0), request by request and
+// chunk by chunk. The device work writes pool slots only: when several fields of the batch land in one slot (a repeated
+// (dest, chunk)), only the last is flooded and integrated, which is what the serial calls leave there.
+extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, void *stream, int32_t *out_nfields,
+                                        int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_cost && ctx->d_pool_slot, "map / pool not created");
+    PF_ARG(m == 0 || reqs, "reqs");
+    PF_ARG(m < (1u << 24), "m");
+    // ---- the whole batch is checked before anything changes
+    std::vector<int32_t> ctile(2 * m);
+    std::vector<uint8_t> on_map(m);
+    bool any_on_map = false;
+    for (size_t i = 0; i < m; i++) {
+        const pfnav_zone_req &q = reqs[i];
+        PF_ARG(q.dest >= 0 && q.dest < ctx->pool_ndests, "dest");
+        PF_ARG(q.layer >= 0 && q.layer < ctx->nlayers, "layer");
+        PF_ARG(q.radius >= 0 && q.radius <= 0xFFFF, "radius");
+        on_map[i] = region_tile_for_point(ctx, q.centre_x, q.centre_z, &ctile[2 * i]);      // nav.c:3931
+        any_on_map |= on_map[i] != 0;
+    }
+    int dim = 0;
+    if (any_on_map) {
+        int rc = zone_dim(ctx, &dim);
+        if (rc) return rc;
+    }
+    if (out_nfields) std::fill(out_nfields, out_nfields + m, 0);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_fields_join(ctx, st));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    // ---- slots request by request, in order
+    const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
+    struct field_t { uint32_t req; int32_t cr, cc, slot; };
+    std::vector<field_t> fields;
+    std::vector<int32_t> fresh;             // (slot table index, slot) of every new reservation
+    int rc = PFNAV_OK;
+    size_t done = 0;
+    for (; done < m; done++) {
+        if (!on_map[done]) continue;
+        const pfnav_zone_req &q = reqs[done];
+        const int r0 = ctile[2 * done], c0 = ctile[2 * done + 1];
+        // the chunks the footprint can reach (nav.c:3945-3951; C division truncates toward zero)
+        const int reach = 2 * q.radius;
+        auto clampi = [](int v, int lo, int hi) { return std::min(std::max(v, lo), hi); };
+        const int min_cr = clampi((r0 - reach) / 64, 0, ctx->chunk_h - 1), max_cr = clampi((r0 + reach) / 64, 0, ctx->chunk_h - 1);
+        const int min_cc = clampi((c0 - reach) / 64, 0, cw - 1), max_cc = clampi((c0 + reach) / 64, 0, cw - 1);
+        const size_t first = fields.size();
+        for (int cr = min_cr; cr <= max_cr && rc == PFNAV_OK; cr++)
+            for (int cc = min_cc; cc <= max_cc; cc++) {
+                const size_t si = (size_t)q.dest * nch + cr * cw + cc;
+                int32_t slot = ctx->h_pool_slot[si];
+                if (slot < 0) {
+                    if (ctx->pool_used >= ctx->pool_max) {
+                        pfnav_set_error("pfnav_pool_request_zone: pool full (%d fields)", ctx->pool_max);
+                        rc = PFNAV_ERR_NOMEM;
+                        break;
+                    }
+                    slot = ctx->pool_used++;
+                    ctx->h_pool_slot[si] = slot;
+                    fresh.push_back((int32_t)si); fresh.push_back(slot);
+                }
+                fields.push_back({(uint32_t)done, cr, cc, slot});
+            }
+        if (rc) {                       // request `done` keeps its reservations, unbuilt, as the single call leaves them
+            fields.resize(first);
+            break;
+        }
+        for (size_t f = first; f < fields.size(); f++) ctx->h_pool_has[fields[f].slot] |= 1;
+        if (out_nfields) out_nfields[done] = (int32_t)(fields.size() - first);
+    }
+    if (out_ndone) *out_ndone = (int)done;
+    if (fields.empty() && fresh.empty()) return rc;
+    if (!fields.empty()) ctx->goal_batch.valid = false;
+    // ---- one flood + one integration per slot: the last field written to it
+    std::vector<int32_t> last(ctx->pool_max, -1);
+    for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
+    std::vector<zone_job> jobs;
+    std::vector<pfnav_region_req> kreq;
+    std::vector<int32_t> kslot;
+    uint64_t pops = 0, max_pops = 0;        // the floods' budgets: what each costs on the host / the device's critical chain
+    for (size_t f = 0; f < fields.size(); f++) {
+        const field_t &F = fields[f];
+        if (last[F.slot] != (int32_t)f) continue;
+        const pfnav_zone_req &q = reqs[F.req];
+        size_t budget = (size_t)(M_PI * q.radius * q.radius + 0.5);         // field.c:1843
+        if (budget > (size_t)dim * dim) budget = (size_t)dim * dim;
+        zone_job j;
+        j.layer = q.layer; j.centre_r = ctile[2 * F.req]; j.centre_c = ctile[2 * F.req + 1]; j.budget = (int32_t)budget;
+        chunk_region_base(dim, F.cr, F.cc, &j.base_r, &j.base_c);
+        const int cdr = j.centre_r - j.base_r, cdc = j.centre_c - j.base_c;
+        if (cdr >= 0 && cdr < dim && cdc >= 0 && cdc < dim) { pops += budget; max_pops = std::max<uint64_t>(max_pops, budget); }
+        jobs.push_back(j);
+        pfnav_region_req rq = {};
+        rq.layer = q.layer; rq.center_r = F.cr; rq.center_c = F.cc; rq.flags = PFNAV_REGION_CREATE;
+        kreq.push_back(rq); kslot.push_back(F.slot);
+    }
+    const size_t nk = kreq.size();
+    // ---- where the floods run: a device flood is one lane's serial chain, and the batch waits for the longest one; the
+    // host floods one field after another. Small batches (a few large zones) flood on the host as seed lists.
+    const bool host_floods = pops <= PF_ZONE_HOST_POP_RATIO * max_pops;
+    std::vector<int32_t> seeds;
+    if (host_floods) {
+        const size_t ltiles = (size_t)ctx->chunk_w * ctx->chunk_h * 4096;
+        for (size_t k = 0; k < nk; k++) {
+            const zone_job &j = jobs[k];
+            const zone_map zm = { ctx->h_cost.data() + ltiles * j.layer, ctx->h_blk.data() + ltiles * j.layer, ctx->chunk_w, ctx->chunk_h };
+            kreq[k].seed_off = (int32_t)(seeds.size() / 2);
+            zone_initial_frontier(zm, j.centre_r, j.centre_c, j.base_r, j.base_c, dim, (size_t)j.budget, seeds);
+            kreq[k].seed_n = (int32_t)(seeds.size() / 2) - kreq[k].seed_off;
+        }
+    }
+    // the `has` bytes of the written slots (h_pool_has after the batch)
+    std::vector<uint8_t> hasv(nk);
+    for (size_t k = 0; k < nk; k++) hasv[k] = ctx->h_pool_has[kslot[k]];
+    // ---- one pinned staging buffer with the inputs, copied into the device scratch. The device slot table and `has`
+    // bytes equal the host mirrors except for what this batch changed: k_pool_scatter writes only those entries.
+    size_t b_in = 0;
+    auto sec = [&](size_t bytes) { const size_t o = b_in; b_in = (b_in + bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_req = sec(nk * sizeof(pfnav_region_req)), o_slot = sec(nk * 4);
+    const size_t o_jobs = sec(host_floods ? 0 : nk * sizeof(zone_job)), o_seeds = sec(seeds.size() * 4);
+    const size_t o_fresh = sec(fresh.size() * 4), o_hasv = sec(nk);
+    const size_t stage = b_in;
+    const size_t o_bits = b_in, need = o_bits + (host_floods ? 0 : nk * ((size_t)dim * dim / 8)) + 16;
+    uint8_t *host = nullptr, *dev = nullptr;
+    int ri = 0;
+    int lrc = pf_plan_host(ctx, stage, &host, &ri);
+    if (lrc) return lrc;
+    memcpy(host + o_req, kreq.data(), nk * sizeof(pfnav_region_req));
+    memcpy(host + o_slot, kslot.data(), nk * 4);
+    if (!host_floods) memcpy(host + o_jobs, jobs.data(), nk * sizeof(zone_job));
+    memcpy(host + o_seeds, seeds.data(), seeds.size() * 4);
+    memcpy(host + o_fresh, fresh.data(), fresh.size() * 4);
+    memcpy(host + o_hasv, hasv.data(), nk);
+    if ((lrc = batch_scratch(ctx, st, need, &dev))) return lrc;
+    PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    const int nscatter = (int)std::max(fresh.size() / 2, nk);
+    k_pool_scatter<<<(unsigned)((nscatter + 255) / 256), 256, 0, st>>>((const int32_t *)(dev + o_fresh), (int)(fresh.size() / 2),
+                                                                        ctx->d_pool_slot, (const int32_t *)(dev + o_slot),
+                                                                        (const uint8_t *)(dev + o_hasv), (int)nk,
+                                                                        ctx->d_pool_los + (size_t)ctx->pool_max * 4096);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    if (nk && host_floods) {
+        if ((lrc = region_launch(ctx, dim, (const pfnav_region_req *)(dev + o_req), nk, (const int32_t *)(dev + o_seeds),
+                                 (const int32_t *)dev, ctx->d_pool_flow, st, 1, nullptr, (const int32_t *)(dev + o_slot))))
+            return lrc;
+    } else if (nk) {
+        const pfnav_region_req *d_req = (const pfnav_region_req *)(dev + o_req);
+        uint32_t *d_bits = (uint32_t *)(dev + o_bits);
+        const size_t smem = ((size_t)dim * dim + 1) * 4 + 3 * ((size_t)dim * dim / 8);
+        PF_CUDA(cudaFuncSetAttribute(k_zone_seed_bits, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (PFNAV_REGION_DIM_MAX * PFNAV_REGION_DIM_MAX + 1) * 4 + 3 * PFNAV_REGION_DIM_MAX * PFNAV_REGION_DIM_MAX / 8));
+        k_zone_seed_bits<<<(unsigned)nk, 32, smem, st>>>(ctx->d_cost, ctx->d_blk, ctx->H64, ctx->W64, dim, (const zone_job *)(dev + o_jobs),
+                                                          (int)nk, d_bits);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+        if ((lrc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, ctx->d_pool_flow, st, 1, d_bits,
+                                 (const int32_t *)(dev + o_slot))))
+            return lrc;
+    }
+    PF_CUDA(cudaEventRecord(ctx->ent_ev, st));
+    return rc;
+}
+
 extern "C" int pfnav_pool_request_zone(pfnav_ctx *ctx, int dest, int layer, const float *centre_xz, int radius, void *stream,
                                        int *out_nfields)
 {
-    PF_ARG(ctx && ctx->d_cost, "map not created");
+    PF_ARG(ctx, "ctx");
     PF_NEED_DEVICE(ctx);
-    PF_ARG(ctx->d_pool_slot, "pool not created");
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
-    PF_ARG(layer >= 0 && layer < ctx->nlayers, "layer");
     PF_ARG(centre_xz, "centre");
-    PF_ARG(radius >= 0 && radius <= 0xFFFF, "radius");
-    if (out_nfields) *out_nfields = 0;
-    int32_t c[2];
-    if (!region_tile_for_point(ctx, centre_xz[0], centre_xz[1], c)) return PFNAV_OK;       // nav.c:3931
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_fields_sync(ctx));
-    cudaStream_t st = pf_stream(ctx, stream);
-    PF_CUDA(pf_pool_refresh(ctx, st));
-    // the chunks the footprint can reach (nav.c:3945-3951; C division truncates toward zero)
-    const int reach = 2 * radius;
-    auto clampi = [](int v, int lo, int hi) { return std::min(std::max(v, lo), hi); };
-    const int min_cr = clampi((c[0] - reach) / 64, 0, ctx->chunk_h - 1), max_cr = clampi((c[0] + reach) / 64, 0, ctx->chunk_h - 1);
-    const int min_cc = clampi((c[1] - reach) / 64, 0, ctx->chunk_w - 1), max_cc = clampi((c[1] + reach) / 64, 0, ctx->chunk_w - 1);
-    std::vector<int32_t> chunks;
-    for (int cr = min_cr; cr <= max_cr; cr++)
-        for (int cc = min_cc; cc <= max_cc; cc++) { chunks.push_back(cr); chunks.push_back(cc); }
-    const size_t n = chunks.size() / 2;
-    const int nchunks = ctx->chunk_w * ctx->chunk_h;
-    // pool slots first, so that a full pool fails before any work is queued
-    std::vector<int32_t> slots(n);
-    for (size_t i = 0; i < n; i++) {
-        const size_t si = (size_t)dest * nchunks + chunks[2 * i] * ctx->chunk_w + chunks[2 * i + 1];
-        int slot = ctx->h_pool_slot[si];
-        if (slot < 0) {
-            if (ctx->pool_used >= ctx->pool_max) { pfnav_set_error("pfnav_pool_request_zone: pool full (%d fields)", ctx->pool_max); return PFNAV_ERR_NOMEM; }
-            slot = ctx->pool_used++;
-            ctx->h_pool_slot[si] = slot;
-            PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot + si, &ctx->h_pool_slot[si], sizeof(int32_t), cudaMemcpyHostToDevice, st));
-        }
-        slots[i] = slot;
-    }
-    uint8_t *d_tmp = nullptr;
-    PF_CUDA(cudaMalloc(&d_tmp, n * 4096));
-    int rc = zone_fields_launch(ctx, layer, c[0], c[1], radius, chunks.data(), n, d_tmp, st);
-    uint8_t *d_has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096;
-    for (size_t i = 0; i < n && rc == 0; i++) {
-        ctx->h_pool_has[slots[i]] |= 1;
-        if (cudaMemcpyAsync(ctx->d_pool_flow + (size_t)slots[i] * 4096, d_tmp + i * 4096, 4096, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
-            cudaMemcpyAsync(d_has + slots[i], &ctx->h_pool_has[slots[i]], 1, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-            pfnav_set_error("pfnav_pool_request_zone: pool copy failed"); rc = PFNAV_ERR_CUDA;
-        }
-    }
-    cudaStreamSynchronize(st);
-    cudaFree(d_tmp);
-    ctx->goal_batch.valid = false;
-    if (rc == 0 && out_nfields) *out_nfields = (int)n;
-    return rc;
+    const pfnav_zone_req q = {dest, layer, centre_xz[0], centre_xz[1], radius, 0};
+    int rc = pfnav_pool_request_zones(ctx, &q, 1, stream, out_nfields, nullptr);
+    if (rc) return rc;
+    PF_CUDA(cudaStreamSynchronize(pf_stream(ctx, stream)));      // returns once the fields are in the pool
+    return PFNAV_OK;
 }
 
 extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius, const float *pos_xz,
@@ -992,17 +1150,8 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
     memcpy(host + o_tiles, htiles.data(), htiles.size() * 4);
     memcpy(host + b_in, ctx->h_pool_slot.data(), b_slot);
     memcpy(host + b_in + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
-    // the device scratch is reused by the next batch, possibly on another stream: order its overwrite after this batch
-    if (!ctx->ent_ev) PF_CUDA(cudaEventCreateWithFlags(&ctx->ent_ev, cudaEventDisableTiming));
-    else PF_CUDA(cudaStreamWaitEvent(st, ctx->ent_ev, 0));
-    if (ctx->ent_buf_bytes < need) {        // grow-only: the old buffer may still be read by the previous batch
-        PF_CUDA(cudaEventSynchronize(ctx->ent_ev));
-        cudaFree(ctx->d_ent_buf);
-        ctx->d_ent_buf = nullptr; ctx->ent_buf_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_ent_buf, need * 2));
-        ctx->ent_buf_bytes = need * 2;
-    }
-    uint8_t *dev = (uint8_t *)ctx->d_ent_buf;
+    uint8_t *dev = nullptr;
+    if ((rc = batch_scratch(ctx, st, need, &dev))) return rc;
     PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
     PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_in, b_slot, cudaMemcpyHostToDevice, st));
     PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_in + b_slot, ctx->pool_max,
