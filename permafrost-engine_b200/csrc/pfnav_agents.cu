@@ -2266,13 +2266,15 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
     // ClearPath that does not depend on the preferred velocity (neighbours, velocity obstacles, admissible
     // ray intersections) runs now, next to them; only the choice waits for the fields.
     // Policy: splitting costs ~5-30 % extra work (phase B rebuilds the obstacles), so it pays only while the LOS
-    // chains outlast a good part of phase A. Both durations are measured on the previous tick.
+    // chains outlast a good part of phase A. Both durations are measured on the previous tick. With the level-parallel
+    // LOS kernel the C2 cold chain (~1.7 ms) is about half the velocity time, and splitting there still saves ~0.9 ms
+    // of a 6 ms step (H100 SXM, 400 W): a quarter of phase A is the bar, not a half.
     if (ctx->vel_timed && cudaEventQuery(ctx->ev_vel1) == cudaSuccess) {
         float ms = 0.0f;
         if (cudaEventElapsedTime(&ms, ctx->ev_vel0, ctx->ev_vel1) == cudaSuccess) ctx->last_vel_ms = ms;
     }
     bool worth = true;
-    if (ctx->last_los_ms > 0.0f && ctx->last_vel_ms > 0.0f) worth = ctx->last_los_ms > 0.5f * ctx->last_vel_ms;
+    if (ctx->last_los_ms > 0.0f && ctx->last_vel_ms > 0.0f) worth = ctx->last_los_ms > 0.25f * ctx->last_vel_ms;
     bool two_phase = ctx->two_phase && (ctx->two_phase_force ||
                                         (worth && ctx->los_inflight && cudaEventQuery(ctx->ev_los) == cudaErrorNotReady));
     cudaGetLastError();

@@ -20,8 +20,10 @@
 //   * K1g general costs (transient 0-cost tiles, nav.c:359): one CTA per field, Bellman-Ford
 //     relaxation on u32 distances in shared memory, then the reference's 8-neighbour rule.
 //   * K3 LOS field: order-dependent (heap pop order among equal priorities is observable,
-//     SURVEY.md 8a-2), so lane 0 of a warp replays the reference's binary heap exactly in
-//     shared memory while the whole warp does tile staging, padding and the store.
+//     SURVEY.md 8a-2). k_los_level runs the wavefront level by level across the warp and checks,
+//     per level, a certificate that the reference's pop order cannot have changed the result;
+//     a field whose certificate fails is rebuilt by lane 0 replaying the reference's binary heap
+//     exactly in shared memory (k_los_b's replay) while the whole warp stages, pads and stores.
 #include "pfnav_internal.cuh"
 #include <stdarg.h>
 #include <string.h>
@@ -92,52 +94,7 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, u
         : "memory");
 }
 
-// ------------------------------------------------------------------------------------------
-// bit helpers
-// ------------------------------------------------------------------------------------------
-// 4 byte-masks (0xFF/0x00) -> 4 bits
-__device__ __forceinline__ uint32_t bytemask_to_bits(uint32_t m)
-{
-    return (((m & 0x01010101u) * 0x01020408u) >> 24) & 0xFu;
-}
-// bits for 16 cost bytes: impassable (==0xFF) and "not unit" (!= 1)
-__device__ __forceinline__ void cost16_bits(const uint4 v, uint32_t &imp, uint32_t &nonunit)
-{
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    imp = 0; nonunit = 0;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        imp |= bytemask_to_bits(__vcmpeq4(w[i], 0xFFFFFFFFu)) << (4 * i);
-        nonunit |= bytemask_to_bits(__vcmpne4(w[i], 0x01010101u)) << (4 * i);
-    }
-}
-// bits for 8 u16 blockers: nonzero
-__device__ __forceinline__ uint32_t blk8_bits(const uint4 v)
-{
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-    uint32_t r = 0;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        uint32_t b = ((w[i] & 0xFFFFu) ? 1u : 0u) | ((w[i] >> 16) ? 2u : 0u);
-        r |= b << (2 * i);
-    }
-    return r;
-}
-// 4 bits -> 4 bytes (bit j -> bit 0 of byte j)
-__device__ __forceinline__ uint32_t spread4(uint32_t x) { return ((x & 0xFu) * 0x00204081u) & 0x01010101u; }
-
-__device__ __forceinline__ uint64_t shfl_up64(uint64_t v, uint32_t lane)
-{
-    uint32_t lo = __shfl_up_sync(0xffffffffu, (uint32_t)v, 1);
-    uint32_t hi = __shfl_up_sync(0xffffffffu, (uint32_t)(v >> 32), 1);
-    return lane == 0 ? 0ull : (((uint64_t)hi << 32) | lo);
-}
-__device__ __forceinline__ uint64_t shfl_down64(uint64_t v, uint32_t lane)
-{
-    uint32_t lo = __shfl_down_sync(0xffffffffu, (uint32_t)v, 1);
-    uint32_t hi = __shfl_down_sync(0xffffffffu, (uint32_t)(v >> 32), 1);
-    return lane == 31 ? 0ull : (((uint64_t)hi << 32) | lo);
-}
+#include "pfnav_los_kernel.cuh"   // bit helpers, FlowGrids, k_los_b, k_los_level
 
 // ------------------------------------------------------------------------------------------
 // Map-state kernels
@@ -242,16 +199,6 @@ __global__ void k_unit_flags(const uint8_t *__restrict__ cost, uint8_t *__restri
 // ------------------------------------------------------------------------------------------
 // K1: flow field, unit-cost fast path. One warp per field.
 // ------------------------------------------------------------------------------------------
-struct FlowGrids {
-    const uint8_t *cost;     // [layer][H64][W64]
-    const uint16_t *blk;
-    const uint16_t *liid;
-    const uint8_t *unit;     // [layer][chunks]
-    int W64, H64, chunk_w, chunk_h;
-    const uint16_t *fmask;   // [layer][H64][W64] bit f <=> faction f holds a blocker refcount on the tile
-    uint16_t enemies[16];    // enemies[f]: factions at war with f
-};
-
 // field_tile_passable_no_enemies (field.c:179): a blocked tile stays passable for an "attacking" request when
 // every faction holding a refcount on it is an enemy of the requesting faction
 __device__ __forceinline__ bool blocked_for(const FlowGrids &g, int faction_id, size_t off)
@@ -721,12 +668,9 @@ k_flow_repair(FlowGrids g, const pfnav_field_req *__restrict__ reqs, const int32
 }
 
 // ------------------------------------------------------------------------------------------
-// K3: LOS field. One warp per field; lane 0 replays the reference heap exactly.
+// K3: LOS field, bit-row replay (k_los). One warp per field; lane 0 replays the reference heap exactly. The byte-state
+// replay k_los_b and the default, level-parallel k_los_level are in pfnav_los_kernel.cuh.
 // ------------------------------------------------------------------------------------------
-#define LOS_WARPS_PER_CTA 4
-// previous-chunk field bytes may have been written by another SM during this launch (dependency-driven
-// scheduling): read them through L2
-#define LOS_PREV_LOAD(p) __ldcg(p)
 struct __align__(16) LosSmem {
     uint64_t pass[64];       // cost != 0xFF && blockers == 0
     uint64_t open[64];       // pass && cost <= 1  (neighbour_costs[i] > 1 test, field.c:2211)
@@ -737,20 +681,6 @@ struct __align__(16) LosSmem {
 };
 
 static_assert(sizeof(LosSmem) % 16 == 0, "LosSmem must keep 16-byte alignment per warp");
-
-struct LosMapInfo {
-    float map_x, map_z;
-};
-
-// OR 64 bits into a shared-memory row with two native 32-bit reductions (a 64-bit shared atomicOr
-// compiles to a compare-and-swap spin loop)
-__device__ __forceinline__ void or_row(uint64_t *row, uint64_t bits)
-{
-    unsigned *w = reinterpret_cast<unsigned *>(row);
-    const unsigned lo = (unsigned)bits, hi = (unsigned)(bits >> 32);
-    if (lo) atomicOr(w, lo);
-    if (hi) atomicOr(w + 1, hi);
-}
 
 // field_create_wavefront_blocked_line (field.c:463-517)
 __device__ void los_blocked_line(LosSmem &s, const LosMapInfo mi, int tgt_cr, int tgt_cc, int tgt_r, int tgt_c,
@@ -1080,310 +1010,6 @@ k_los(FlowGrids g, LosMapInfo mi, const pfnav_los_req *__restrict__ reqs, int n,
     }
 }
 
-// Byte-state variant of the LOS replay (k_los_b): one state byte per tile in a 66 x 66 array whose border ring
-// carries LB_BORDER, so the four neighbour tests of a pop are four byte loads + mask compares with no bounds
-// checks and no 64-bit variable shifts (the bit-row form spends ~75 of its ~300 instructions per pop on those).
-#define LB_BLK    0x01   /* wavefront_blocked                                             */
-#define LB_OPEN   0x02   /* passable for this request and cost <= 1                        */
-#define LB_ASG    0x04   /* integration_field < INF (was pushed / is a seed)               */
-#define LB_VIS    0x08   /* visible                                                        */
-#define LB_PASS   0x10   /* plain passable (field_is_los_corner, field.c:435)              */
-#define LB_BORDER 0x20   /* outside the chunk                                              */
-#define LB_W 66
-struct __align__(16) LosSmemB {
-    uint8_t  st[LB_W * LB_W + 12];   // 4368
-    uint64_t blkrow[64], visrow[64]; // bit rows for the final padding pass
-    uint16_t heap[4104];
-};
-static_assert(sizeof(LosSmemB) % 16 == 0, "LosSmemB must keep 16-byte alignment per warp");
-
-// field_create_wavefront_blocked_line (field.c:463-517) on the byte array
-__device__ void los_blocked_line_b(LosSmemB &s, const LosMapInfo mi, int tgt_cr, int tgt_cc, int tgt_r, int tgt_c,
-                                   int cr, int cc, int r, int c)
-{
-    const float tbx = (mi.map_x - (float)(tgt_cc * 256)) - (float)(tgt_c * 4);
-    const float tbz = (mi.map_z + (float)(tgt_cr * 256)) + (float)(tgt_r * 4);
-    const float cbx = (mi.map_x - (float)(cc * 256)) - (float)(c * 4);
-    const float cbz = (mi.map_z + (float)(cr * 256)) + (float)(r * 4);
-    const float tcx = tbx - 4.0f / 2.0f, tcz = tbz + 4.0f / 2.0f;
-    const float ccx = cbx - 4.0f / 2.0f, ccz = cbz + 4.0f / 2.0f;
-    float sx_ = tcx - ccx, sz_ = tcz - ccz;
-    const float len = sqrtf(sx_ * sx_ + sz_ * sz_);
-    sx_ = sx_ / len;
-    sz_ = sz_ / len;
-    if (!(len > 0.0f)) {
-        // line from the target tile to itself: NaN slope, INT_MIN deltas, wrapped error term -- the reference walks the
-        // row towards column 0 (see los_blocked_line)
-        for (int idx0 = (r + 1) * LB_W + (c + 1); !(s.st[idx0] & LB_BORDER); idx0--) s.st[idx0] |= LB_BLK;
-        return;
-    }
-    const int dx = abs((int)(sx_ * 1000));
-    const int dy = -abs((int)(sz_ * 1000));
-    const int sx = sx_ > 0.0f ? 1 : -1;
-    const int sy = sz_ < 0.0f ? 1 : -1;
-    int err = dx + dy, e2;
-    int idx = (r + 1) * LB_W + (c + 1);
-    uint8_t v = s.st[idx];
-    // the walk ends on the border ring (LB_BORDER), which is never written
-    while (!(v & LB_BORDER)) {
-        s.st[idx] = v | LB_BLK;
-        e2 = 2 * err;
-        if (e2 >= dy) { err += dy; idx += sx; }
-        if (e2 <= dx) { err += dx; idx += sy * LB_W; }
-        v = s.st[idx];
-    }
-}
-
-// Heap of the byte-state kernel: entries = prio2 << 13 | padded index ((r + 1) * 66 + c + 1 < 8192), so that a pop needs
-// no unpacking and no address arithmetic before its four state loads. heap_remove_root is heap_pop without the read of
-// the root: the caller reads h[1] first and issues the neighbour loads BEFORE the sift, whose dependent chain then hides them.
-__device__ __forceinline__ void heap_remove_root13(uint16_t *h, int &size, uint32_t lowp)
-{
-    const uint16_t x = h[size];
-    size--;
-    int root = 1;
-    if ((uint32_t)(x >> 13) != lowp) {
-        const uint32_t *h2 = reinterpret_cast<const uint32_t *>(h);      // children 2k, 2k+1 share one aligned word
-        while (true) {
-            const int l = root * 2;
-            if (l > size) break;
-            const uint32_t two = h2[root];
-            const bool dl = ((two >> 13) & 0x7u) == lowp, dr = l < size && (two >> 29) == lowp;
-            if (!(dl || dr)) break;
-            h[root] = (uint16_t)(dl ? two : two >> 16);
-            root = dl ? l : l + 1;
-        }
-    }
-    h[root] = x;
-}
-
-__global__ void __launch_bounds__(LOS_WARPS_PER_CTA * 32)
-k_los_b(FlowGrids g, LosMapInfo mi, const pfnav_los_req *__restrict__ reqs, int n,
-      uint8_t *fields, const int32_t *__restrict__ out_slot, unsigned *counter, int *done,
-      unsigned long long *trace)
-{
-    extern __shared__ __align__(16) uint8_t smem_raw[];
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    LosSmemB &s = reinterpret_cast<LosSmemB *>(smem_raw)[warp];
-    // Dependency-driven scheduling: requests are sorted so that a request's prev_index is smaller than
-    // its own index; warps take indices in order from a global counter and wait (only) for the one
-    // field they depend on. No barrier between dependency levels: the LOS phase costs the slowest
-    // chain, not the sum over levels of the slowest field of each level.
-    for (;;) {
-        int i = 0;
-        if (lane == 0) i = (int)atomicAdd(counter, 1u);
-        i = __shfl_sync(0xffffffffu, i, 0);
-        if (i >= n) break;
-        const pfnav_los_req q = reqs[i];
-        unsigned long long t_take = 0, t_ready = 0;
-        if (trace && lane == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_take));
-        if (q.prev_index >= 0) {
-            if (lane == 0) {
-                volatile int *flag = done + q.prev_index;
-                while (*flag == 0) __nanosleep(100);
-            }
-            __syncwarp();
-            __threadfence();
-        }
-        if (trace && lane == 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_ready));
-        // A chunk other than the destination whose shared edge with the previous chunk carries no
-        // `visible` and no `wavefront_blocked` tile starts with an empty frontier and draws no line
-        // (field.c:2157-2195): the field is all zero. Most chunks far from the goal end here.
-        if (!(q.chunk_r == q.tgt_chunk_r && q.chunk_c == q.tgt_chunk_c)) {
-            const uint8_t *prev = fields + (size_t)(q.prev_index >= 0 ? (out_slot ? out_slot[q.prev_index] : q.prev_index) : q._pad) * 4096;
-            int pe; bool horiz;
-            if (q.prev_chunk_r < q.chunk_r)      { horiz = false; pe = 63; }
-            else if (q.prev_chunk_r > q.chunk_r) { horiz = false; pe = 0;  }
-            else if (q.prev_chunk_c < q.chunk_c) { horiz = true;  pe = 63; }
-            else                                 { horiz = true;  pe = 0;  }
-            uint32_t any = 0;
-            for (int e = lane; e < 64; e += 32) any |= LOS_PREV_LOAD(horiz ? prev + e * 64 + pe : prev + pe * 64 + e);
-            if (!__any_sync(0xffffffffu, any != 0)) {
-                uint4 *d4 = reinterpret_cast<uint4 *>(fields + (size_t)(out_slot ? out_slot[i] : i) * 4096);
-                for (int j = lane; j < 256; j += 32) d4[j] = make_uint4(0, 0, 0, 0);
-                __threadfence();
-                __syncwarp();
-                if (lane == 0) {
-                    *(volatile int *)(done + i) = 1;
-                    if (trace) {
-                        unsigned long long t_done; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_done));
-                        trace[4 * (size_t)i] = t_take; trace[4 * (size_t)i + 1] = t_ready; trace[4 * (size_t)i + 2] = t_done; trace[4 * (size_t)i + 3] = (unsigned long long)(unsigned)(q.prev_index + 1) << 32;
-                    }
-                }
-                continue;
-            }
-        }
-        // ---- stage tile -> bit rows (2 rows per lane) ----
-#pragma unroll
-        for (int rr = 0; rr < 2; rr++) {
-            const int row = 2 * lane + rr;
-            const size_t off = ((size_t)q.layer * g.H64 + q.chunk_r * 64 + row) * g.W64 + q.chunk_c * 64;
-            const uint4 *pc = reinterpret_cast<const uint4 *>(g.cost + off);
-            const uint4 *pb = reinterpret_cast<const uint4 *>(g.blk + off);
-            uint64_t p = 0, blocked = 0, gt1 = 0;
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const uint4 v = __ldg(pc + j);
-                uint32_t imp, n1;
-                cost16_bits(v, imp, n1);
-                p |= (uint64_t)((~imp) & 0xFFFFu) << (16 * j);
-                // cost > 1  <=>  cost not in {0, 1}
-                const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-                uint32_t g1 = 0;
-#pragma unroll
-                for (int e = 0; e < 4; e++)
-                    g1 |= bytemask_to_bits(__vcmpgtu4(w[e], 0x01010101u)) << (4 * e);
-                gt1 |= (uint64_t)g1 << (16 * j);
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++) blocked |= (uint64_t)blk8_bits(__ldg(pb + j)) << (8 * j);
-            // an "attacking" request (dest_id carries a faction, field.c:2095) walks over tiles blocked only by its
-            // enemies (field_tile_passable_no_enemies, field.c:179); the corner test keeps the plain rule (field.c:435)
-            uint64_t blocked_f = blocked;
-            if (q.faction_id != PFNAV_FACTION_ID_NONE && blocked) {
-                const uint16_t en = g.enemies[q.faction_id & 0xF];
-                const uint16_t *pf = g.fmask + off;
-                for (uint64_t rest = blocked; rest; rest &= rest - 1) {
-                    const int c = __ffsll((long long)rest) - 1;
-                    if ((pf[c] & ~en) == 0) blocked_f &= ~(1ull << c);
-                }
-            }
-            const uint64_t passb = p & ~blocked, openb = p & ~blocked_f & ~gt1;
-            uint8_t *rowp = s.st + (row + 1) * LB_W + 1;
-#pragma unroll 8
-            for (int c = 0; c < 64; c++)
-                rowp[c] = (uint8_t)((((passb >> c) & 1) ? LB_PASS : 0) | (((openb >> c) & 1) ? LB_OPEN : 0));
-            rowp[-1] = LB_BORDER; rowp[64] = LB_BORDER;
-        }
-        for (int c = lane; c < LB_W; c += 32) { s.st[c] = LB_BORDER; s.st[65 * LB_W + c] = LB_BORDER; }
-        __syncwarp();
-
-        unsigned npops = 0;
-        if (lane == 0) {
-            uint16_t *h = s.heap;
-            int size = 0;
-            const bool dest_chunk = (q.chunk_r == q.tgt_chunk_r && q.chunk_c == q.tgt_chunk_c);
-            if (dest_chunk) {
-                h[++size] = (uint16_t)((q.tgt_tile_r + 1) * LB_W + q.tgt_tile_c + 1);
-                s.st[(q.tgt_tile_r + 1) * LB_W + q.tgt_tile_c + 1] |= LB_ASG;
-            } else {
-                // carry the shared edge over from the previous chunk's field (field.c:2122-2196)
-                const uint8_t *prev = fields + (size_t)(q.prev_index >= 0 ? (out_slot ? out_slot[q.prev_index] : q.prev_index) : q._pad) * 4096;
-                bool horizontal; int curr_edge, prev_edge;
-                if (q.prev_chunk_r < q.chunk_r)      { horizontal = false; curr_edge = 0;  prev_edge = 63; }
-                else if (q.prev_chunk_r > q.chunk_r) { horizontal = false; curr_edge = 63; prev_edge = 0;  }
-                else if (q.prev_chunk_c < q.chunk_c) { horizontal = true;  curr_edge = 0;  prev_edge = 63; }
-                else                                 { horizontal = true;  curr_edge = 63; prev_edge = 0;  }
-                for (int e = 0; e < 64; e++) {
-                    const int r = horizontal ? e : curr_edge, c = horizontal ? curr_edge : e;
-                    const uint8_t pv = LOS_PREV_LOAD(horizontal ? prev + e * 64 + prev_edge : prev + prev_edge * 64 + e);
-                    const int idx = (r + 1) * LB_W + c + 1;
-                    // struct assignment overwrites both flags of the edge tile
-                    s.st[idx] = (uint8_t)((s.st[idx] & ~(LB_VIS | LB_BLK)) | ((pv & 1) ? LB_VIS : 0) | ((pv & 2) ? LB_BLK : 0));
-                    if (pv & 2)
-                        los_blocked_line_b(s, mi, q.tgt_chunk_r, q.tgt_chunk_c, q.tgt_tile_r, q.tgt_tile_c,
-                                           q.chunk_r, q.chunk_c, r, c);
-                    if (pv & 1) {
-                        h[++size] = (uint16_t)idx;                // priority 0: an append, all seeds are equal
-                        s.st[idx] |= LB_ASG;
-                    }
-                }
-            }
-            while (size > 0) {
-                npops++;
-                const uint32_t cur = h[1];
-                const uint32_t pidx = cur & 0x1FFFu;
-                const uint16_t nprio = (uint16_t)((((cur >> 13) + 1) & 3) << 13);
-                uint8_t *ctr = s.st + pidx;
-                // neighbour order of field_neighbours_grid_los: (-1,0) (0,-1) (0,+1) (+1,0); the four states are read
-                // before anything of this pop is written (the list is collected first, field.c:2205) -- and before the
-                // sift, which touches only the heap array
-                const uint32_t s0 = ctr[-LB_W], s1 = ctr[-1], s2 = ctr[1], s3 = ctr[LB_W];
-                heap_remove_root13(h, size, cur >> 13);
-                const uint32_t TM = LB_BLK | LB_BORDER | LB_OPEN;
-                const bool v0 = (s0 & TM) == LB_OPEN, v1 = (s1 & TM) == LB_OPEN, v2 = (s2 & TM) == LB_OPEN, v3 = (s3 & TM) == LB_OPEN;
-                const bool p0 = v0 && !(s0 & LB_ASG), p1 = v1 && !(s1 & LB_ASG), p2 = v2 && !(s2 & LB_ASG), p3 = v3 && !(s3 & LB_ASG);
-                if (v0) ctr[-LB_W] = (uint8_t)(s0 | LB_VIS | LB_ASG);
-                if (v1) ctr[-1] = (uint8_t)(s1 | LB_VIS | LB_ASG);
-                if (v2) ctr[1] = (uint8_t)(s2 | LB_VIS | LB_ASG);
-                if (v3) ctr[LB_W] = (uint8_t)(s3 | LB_VIS | LB_ASG);
-                const uint16_t base0 = (uint16_t)(nprio | pidx);
-                int sz = size;
-                if (p0) h[++sz] = (uint16_t)(base0 - LB_W);
-                if (p1) h[++sz] = (uint16_t)(base0 - 1);
-                if (p2) h[++sz] = (uint16_t)(base0 + 1);
-                if (p3) h[++sz] = (uint16_t)(base0 + LB_W);
-                size = sz;
-                if (!((s0 & TM) && (s1 & TM) && (s2 & TM) && (s3 & TM))) {
-                    // an impassable (or cost > 1) neighbour that is inside the chunk and not wavefront-blocked:
-                    // field_is_los_corner (field.c:435), then the blocked line
-                    const int r = (int)(pidx / LB_W) - 1, c = (int)(pidx % LB_W) - 1;
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        const uint32_t se = e == 0 ? s0 : e == 1 ? s1 : e == 2 ? s2 : s3;
-                        if (se & TM) continue;
-                        const int rr = e == 0 ? r - 1 : e == 3 ? r + 1 : r, cc = e == 1 ? c - 1 : e == 2 ? c + 1 : c;
-                        const uint8_t *nb = s.st + (rr + 1) * LB_W + (cc + 1);
-                        bool corner = false;
-                        if (rr > 0 && rr < 63) corner = ((nb[-LB_W] ^ nb[LB_W]) & LB_PASS) != 0;
-                        if (!corner && cc > 0 && cc < 63) corner = ((nb[-1] ^ nb[1]) & LB_PASS) != 0;
-                        if (!corner) continue;
-                        los_blocked_line_b(s, mi, q.tgt_chunk_r, q.tgt_chunk_c, q.tgt_tile_r, q.tgt_tile_c,
-                                           q.chunk_r, q.chunk_c, rr, cc);
-                    }
-                }
-            }
-        }
-        __syncwarp();
-        // ---- bytes -> bit rows for the padding pass ----
-#pragma unroll
-        for (int rr = 0; rr < 2; rr++) {
-            const int row = 2 * lane + rr;
-            const uint8_t *rowp = s.st + (row + 1) * LB_W + 1;
-            uint64_t bb = 0, vv = 0;
-#pragma unroll 8
-            for (int c = 0; c < 64; c++) {
-                const uint32_t v = rowp[c];
-                bb |= (uint64_t)(v & LB_BLK) << c;
-                vv |= (uint64_t)((v >> 3) & 1) << c;
-            }
-            s.blkrow[row] = bb; s.visrow[row] = vv;
-        }
-        __syncwarp();
-        // ---- field_pad_wavefront (field.c:519): clear `visible` within 1 tile of a blocked tile ----
-        uint8_t *dst = fields + (size_t)(out_slot ? out_slot[i] : i) * 4096;
-#pragma unroll
-        for (int rr = 0; rr < 2; rr++) {
-            const int row = 2 * lane + rr;
-            uint64_t b = s.blkrow[row];
-            if (row > 0) b |= s.blkrow[row - 1];
-            if (row < 63) b |= s.blkrow[row + 1];
-            b = b | (b << 1) | (b >> 1);
-            const uint64_t vis = s.visrow[row] & ~b, w = s.blkrow[row];
-            uint4 *d4 = reinterpret_cast<uint4 *>(dst + row * 64);
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                uint32_t o[4];
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int sh = j * 16 + e * 4;
-                    o[e] = spread4((uint32_t)(vis >> sh)) | (spread4((uint32_t)(w >> sh)) << 1);
-                }
-                d4[j] = make_uint4(o[0], o[1], o[2], o[3]);
-            }
-        }
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) {
-            *(volatile int *)(done + i) = 1;
-            if (trace) {
-                unsigned long long t_done; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_done));
-                trace[4 * (size_t)i] = t_take; trace[4 * (size_t)i + 1] = t_ready; trace[4 * (size_t)i + 2] = t_done; trace[4 * (size_t)i + 3] = ((unsigned long long)(unsigned)(q.prev_index + 1) << 32) | (npops + 1);
-            }
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------
 // Host side: context + map state
 // ------------------------------------------------------------------------------------------
@@ -1476,6 +1102,8 @@ int pfnav_fields_init(pfnav_ctx *ctx)
     PF_CUDA(cudaFuncSetAttribute(k_flow_unit<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  FLOW_WARPS_PER_CTA * FLOW_SMEM_PER_WARP + 128));
     PF_CUDA(cudaFuncSetAttribute(k_los_b, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(LOS_WARPS_PER_CTA * sizeof(LosSmemB))));
+    PF_CUDA(cudaFuncSetAttribute(k_los_level, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)(LOS_WARPS_PER_CTA * sizeof(LosSmemB))));
     PF_CUDA(cudaFuncSetAttribute(k_los, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)(LOS_WARPS_PER_CTA * sizeof(LosSmem))));
     return 0;
@@ -2098,7 +1726,7 @@ int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint
     PF_CUDA(cudaSetDevice(ctx->device));
     const FlowGrids g = grids_of(ctx);
     LosMapInfo mi{ctx->map_x, ctx->map_z};
-    const size_t smem = LOS_WARPS_PER_CTA * (ctx->los_variant == 1 ? sizeof(LosSmemB) : sizeof(LosSmem));
+    const size_t smem = LOS_WARPS_PER_CTA * (ctx->los_variant != 0 ? sizeof(LosSmemB) : sizeof(LosSmem));
     (void)n_waves; (void)h_wave_offsets;        // requests are dependency-sorted; the kernel schedules them itself
     cudaStream_t st = pf_stream(ctx, stream);
     // scheduler state: [counter][done flags]. ONE buffer per context: the warps of a launch spin on its flags, so a
@@ -2126,7 +1754,11 @@ int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint
     // waves of the same batch -- and with them every later launch, the block scheduler serves grids in order --
     // are not held up until LOS CTAs retire. The makespan is one chain's latency, not a matter of warp count.
     const int grid = std::max(1, std::min((int)((n + LOS_WARPS_PER_CTA - 1) / LOS_WARPS_PER_CTA), ctx->sm_count * 2));
-    if (ctx->los_variant == 1)
+    if (ctx->los_variant == 2)
+        k_los_level<<<grid, LOS_WARPS_PER_CTA * 32, smem, st>>>(g, mi, d_reqs, (int)n, d_out_fields, d_out_slot,
+                                                                (unsigned *)ctx->d_los_sched, (int *)ctx->d_los_sched + 1,
+                                                                ctx->los_trace_on ? ctx->d_los_trace : nullptr);
+    else if (ctx->los_variant == 1)
         k_los_b<<<grid, LOS_WARPS_PER_CTA * 32, smem, st>>>(g, mi, d_reqs, (int)n, d_out_fields, d_out_slot,
                                                             (unsigned *)ctx->d_los_sched, (int *)ctx->d_los_sched + 1,
                                                             ctx->los_trace_on ? ctx->d_los_trace : nullptr);
@@ -2215,7 +1847,8 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
 }
 
 // Per-field trace of the last LOS launch (debug / profiling aid): for request i, out[4i..4i+3] =
-// {taken, dependency satisfied, finished} in %globaltimer ns, and (prev_index + 1) << 32 | (1 + heap pops; 0 = zero-filled early out).
+// {taken, dependency satisfied, finished} in %globaltimer ns, and (prev_index + 1) << 32 | (1 + heap pops; 0 = zero-filled early out),
+// the low half OR-ed with LOS_TRACE_REPLAYED (bit 31) when k_los_level's certificate failed and the field was replayed.
 extern "C" int pfnav_los_trace(pfnav_ctx *ctx, int enable, unsigned long long *out, size_t cap, size_t *out_n)
 {
     PF_ARG(ctx, "ctx");
@@ -2231,10 +1864,11 @@ extern "C" int pfnav_los_trace(pfnav_ctx *ctx, int enable, unsigned long long *o
     return PFNAV_OK;
 }
 
-// Test / tuning hook: 0 = bit-row LOS kernel (k_los), 1 = byte-state LOS kernel (k_los_b). Same results.
+// Test / tuning hook: 0 = bit-row LOS kernel (k_los), 1 = byte-state LOS kernel (k_los_b), 2 = level-parallel LOS
+// kernel with the replay as fallback (k_los_level, the default). Same results.
 extern "C" int pfnav_set_los_variant(pfnav_ctx *ctx, int variant)
 {
-    PF_ARG(ctx && (variant == 0 || variant == 1), "variant");
+    PF_ARG(ctx && variant >= 0 && variant <= 2, "variant");
     ctx->los_variant = variant;
     return PFNAV_OK;
 }

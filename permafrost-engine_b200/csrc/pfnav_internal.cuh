@@ -79,7 +79,7 @@ struct pfnav_ctx {
     CUtensorMap tmap_cost, tmap_blk; // rank-3 {x, y, layer}, box 64x64x1
     void *d_stage = nullptr; size_t stage_bytes = 0;   // upload staging
     unsigned long long *d_los_trace = nullptr; size_t los_trace_cap = 0, los_trace_n = 0; bool los_trace_on = false;
-    int los_variant = 1;
+    int los_variant = 2;
     void *d_los_sched = nullptr; size_t los_sched_bytes = 0;   // LOS scheduler: work counter + per-request done flags
     cudaEvent_t ev_los_sched = nullptr;                        // recorded after every LOS launch: the next one waits for it
     // host mirrors (chunk-blocked, [layer][chunk][64][64]) for the host-side planner
