@@ -673,6 +673,48 @@ typedef struct pfnav_patch {            /* struct movestate_patch (movement.c:24
  * pfnav_route_build(layer). */
 int  pfnav_route_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, int32_t *out_nearest_ok,
                                 float *out_nearest_xz, float *out_mc_xz, size_t cap, int32_t *out_mc_n);
+/* Map point queries (seam B3, src/navigation/public/nav.h), answered in batches on the device. */
+enum pfnav_map_query_kind {
+    PFNAV_QUERY_PATHABLE = 0,            /* N_PositionPathable (nav.c:4055): the tile under (x, z) is not 0xFF        */
+    PFNAV_QUERY_BLOCKED,                 /* N_PositionBlocked (nav.c:4070): the tile under (x, z) holds a blocker     */
+    PFNAV_QUERY_ADJACENT_IMPASSABLE,     /* N_IsAdjacentToImpassable (nav.c:4745): one of the 4 neighbours of the tile
+                                          * under (x, z) has cost 0xFF or a blocker                                   */
+    PFNAV_QUERY_CLOSEST_PATHABLE,        /* N_ClosestPathable (nav.c:4126): the nearest tile to (x, z) that is
+                                          * neither impassable nor blocked                                            */
+    PFNAV_QUERY_MAXIMALLY_CLOSE,         /* N_IsMaximallyClose (nav.c:4707) of (x, z) to (dst_x, dst_z)               */
+    PFNAV_QUERY_DEST_ID                  /* N_DestIDForPos / N_DestIDForPosAttacking (nav.c:839) of (x, z)            */
+};
+typedef struct pfnav_map_query_req {         /* 32 bytes */
+    int32_t kind, layer;                 /* enum pfnav_map_query_kind; 0 <= layer < nlayers                            */
+    float   x, z;                        /* the position (CLOSEST_PATHABLE: the target, DEST_ID: the destination)     */
+    float   dst_x, dst_z;                /* MAXIMALLY_CLOSE: the destination                                          */
+    float   tolerance;                   /* MAXIMALLY_CLOSE: finite                                                   */
+    int32_t faction_id;                  /* DEST_ID: PFNAV_FACTION_ID_NONE = N_DestIDForPos, 0..14 = ...Attacking      */
+} pfnav_map_query_req;
+typedef struct pfnav_map_query_result {  /* 16 bytes */
+    int32_t  ok;                         /* the reference function's bool (DEST_ID, CLOSEST_PATHABLE: a tile exists)  */
+    uint32_t dest_id;                    /* DEST_ID: the dest_id_t                                                    */
+    float    x, z;                       /* CLOSEST_PATHABLE: *out -- the query point when its tile is free, else the
+                                          * M_Tile_Bounds corner of the tile found                                    */
+} pfnav_map_query_result;
+/* n map queries against the COMMITTED map: blocker counts as the last pfnav_map_commit left them (the state the
+ * reader contexts and the tick see), costs as last uploaded. pfnav_blockers_* changes not yet committed are not seen.
+ * - Buffers are on the host; the call returns when out[0 .. n) is filled.
+ * - Work is queued on `stream` (NULL: the context's stream), ordered after pfnav_map_commit and after the field work
+ *   forked by pfnav_pool_request_goals, like the pool entry points.
+ * - A query point outside the map box gives ok = 0 for every kind.
+ * - CLOSEST_PATHABLE: breadth-first from the tile under (x, z), neighbours (0,-1) (0,+1) (-1,0) (+1,0); the first tile
+ *   dequeued whose cost is not 0xFF and that holds no blocker. ok = 0 when there is none.
+ * - MAXIMALLY_CLOSE: ok = some tile centre n_closest_island_tiles (nav.c:1226) lists for the destination -- the
+ *   closest tiles of its global island without blockers, at most 256 -- lies within `tolerance` of (x, z). It does not
+ *   include the N_IsAdjacentToImpassable test that arrived() (movement.c:2170) adds; combine the two kinds for that.
+ * - The searches run on the device over a window around the start tile; a search that leaves it is finished on the
+ *   host in the same call. Results are identical either way.
+ * - Everything is validated before anything runs: null pointers (n > 0), kind, layer, a finite tolerance and
+ *   pfnav_route_build(layer) (the global islands) for MAXIMALLY_CLOSE, faction_id in 0..15 for DEST_ID. Failure:
+ *   PFNAV_ERR_ARG, out untouched. n == 0 is valid. Host-only context: PFNAV_ERR_NO_DEVICE. */
+int  pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfnav_map_query_result *out, void *stream);
+
 /* HOST array of n_agents records, uid == index. */
 int  pfnav_agents_upload_movestate(pfnav_ctx *ctx, const pfnav_movestate *ms, size_t n);
 /* After pfnav_agents_tick on the same stream: entity_compute_update for every work item, reading the

@@ -79,6 +79,12 @@ ENTITY_FIELD_REQ = np.dtype([("dest", "<i4"), ("layer", "<i4"), ("ref_layer", "<
 assert ENTITY_FIELD_REQ.itemsize == 32
 ZONE_REQ = np.dtype([("dest", "<i4"), ("layer", "<i4"), ("centre_x", "<f4"), ("centre_z", "<f4"), ("radius", "<i4"), ("_pad", "<i4")])
 assert ZONE_REQ.itemsize == 24
+QUERY_PATHABLE, QUERY_BLOCKED, QUERY_ADJACENT_IMPASSABLE, QUERY_CLOSEST_PATHABLE, QUERY_MAXIMALLY_CLOSE, QUERY_DEST_ID = range(6)
+MAP_QUERY = np.dtype([("kind", "<i4"), ("layer", "<i4"), ("x", "<f4"), ("z", "<f4"), ("dst_x", "<f4"), ("dst_z", "<f4"),
+                      ("tolerance", "<f4"), ("faction_id", "<i4")])
+assert MAP_QUERY.itemsize == 32
+MAP_QUERY_RESULT = np.dtype([("ok", "<i4"), ("dest_id", "<u4"), ("x", "<f4"), ("z", "<f4")])
+assert MAP_QUERY_RESULT.itemsize == 16
 
 LOS_PREV_INPLACE = -3
 TICK_VDES_FROM_POOL = 1
@@ -107,7 +113,7 @@ SYMBOLS = [
     "pfnav_agents_upload_formation", "pfnav_agents_upload_movestate_ext", "pfnav_pool_request_entity_fields",
     "pfnav_pool_request_entity_fields_batch", "pfnav_pool_request_zones",
     "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
-    "pfnav_profile_read_host",
+    "pfnav_profile_read_host", "pfnav_map_query",
 ]
 
 _lib = None
@@ -161,7 +167,8 @@ def load():
     L.pfnav_zone_fields.argtypes = [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_pool_request_zone.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int)]
     L.pfnav_pool_request_zones.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]
-    L.pfnav_group_arrival_velocity.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.pfnav_map_query.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.pfnav_group_arrival_velocity.argtypes =[C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.pfnav_group_arrival_field.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_uint16, C.c_void_p, C.c_size_t, C.c_void_p,
                                             C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_agents_upload_movestate.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
@@ -468,6 +475,16 @@ class Nav:
         nearest = np.zeros(2, np.float32); mc = np.zeros((256, 2), np.float32)
         _chk(self.L.pfnav_route_arrival_consts(self.h, layer, float(target_xz[0]), float(target_xz[1]), C.byref(ok), _p(nearest), _p(mc), 256, C.byref(n)))
         return ok.value, nearest, mc[:n.value].copy()
+
+    def map_query(self, queries, stream=0, out=None):
+        """pfnav_map_query: MAP_QUERY records -> MAP_QUERY_RESULT records (answers from the committed map). `out`, when
+        given, is the MAP_QUERY_RESULT array the call fills (left untouched when the call fails)."""
+        q = np.ascontiguousarray(queries, MAP_QUERY)
+        if out is None:
+            out = np.zeros(len(q), MAP_QUERY_RESULT)
+        assert out.dtype == MAP_QUERY_RESULT and out.flags.c_contiguous and len(out) >= len(q)
+        _chk(self.L.pfnav_map_query(self.h, _p(q) if len(q) else None, len(q), _p(out) if len(q) else None, C.c_void_p(stream)))
+        return out
 
     def zone_seeds(self, chunk, centre, radius, layer=0):
         out = np.zeros((4 * 4096, 2), np.int32); n = C.c_size_t(0)

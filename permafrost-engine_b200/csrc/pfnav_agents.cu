@@ -28,6 +28,7 @@
 #include <algorithm>
 #include <math.h>
 #include <string.h>
+#include "pfnav_map_view.cuh"
 
 #define EPS_F (1.0f / 1024)
 #define FULL 0xffffffffu
@@ -53,11 +54,6 @@ __device__ __forceinline__ v2 v2_truncate(v2 a, float max_len)
 // ------------------------------------------------------------------------------------------
 // Map / pool views
 // ------------------------------------------------------------------------------------------
-struct MapView {
-    const uint8_t *cost; const uint16_t *blk;   // [layer][H64][W64]
-    int W64, H64, chunk_w, chunk_h;
-    float map_x, map_z;
-};
 struct PoolView {
     const int32_t *slot;     // [ndests][chunks]
     const uint8_t *flow;     // [max][4096]
@@ -72,41 +68,6 @@ struct GridView {
     const int32_t *ix, *iy; const uint32_t *id;
     int grid_w, grid_h; int32_t origin_x, origin_y;
 };
-
-struct tile_desc { int chunk_r, chunk_c, tile_r, tile_c; };
-
-// M_Tile_DescForPoint2D with the nav resolution (tile.c:547; n_res nav.c:240): returns false
-// outside the map box.
-__device__ __forceinline__ bool desc_for_point(const MapView &m, float px, float pz, tile_desc &out)
-{
-    const float width = (float)(m.chunk_w * 256), height = (float)(m.chunk_h * 256);
-    if (px > m.map_x || px < m.map_x - width) return false;
-    if (pz < m.map_z || pz > m.map_z + height) return false;
-    int chunk_r = (int)(fabs((double)(m.map_z - pz)) / 256.0);
-    int chunk_c = (int)(fabs((double)(m.map_x - px)) / 256.0);
-    chunk_r = min(max(chunk_r, 0), m.chunk_h - 1);
-    chunk_c = min(max(chunk_c, 0), m.chunk_w - 1);
-    const float base_x = m.map_x - (float)chunk_c * 256.0f;
-    const float base_z = m.map_z + (float)chunk_r * 256.0f;
-    int tile_r = (int)(fabs((double)(base_z - pz)) / 4);
-    int tile_c = (int)(fabs((double)(base_x - px)) / 4);
-    out.chunk_r = chunk_r; out.chunk_c = chunk_c;
-    out.tile_r = min(max(tile_r, 0), 63);
-    out.tile_c = min(max(tile_c, 0), 63);
-    return true;
-}
-
-// M_NavPositionPathable / M_NavPositionBlocked (map.c:817, 831): both false outside the map box.
-__device__ __forceinline__ void probe_tile(const MapView &m, int layer, float px, float pz, bool &pathable,
-                                           bool &blocked)
-{
-    tile_desc td;
-    pathable = false; blocked = false;
-    if (!desc_for_point(m, px, pz, td)) return;
-    const size_t off = ((size_t)layer * m.H64 + td.chunk_r * 64 + td.tile_r) * m.W64 + td.chunk_c * 64 + td.tile_c;
-    pathable = m.cost[off] != 0xFF;
-    blocked = m.blk[off] > 0;
-}
 
 // Entity_NavLayerWithRadius (entity.c:554)
 __device__ __forceinline__ int nav_layer_for(uint32_t flags, float radius)
@@ -2456,13 +2417,6 @@ __device__ quat turn_toward(const quat &cur, const quat &target, float max_deg)
     const float len = (float)sqrt((double)(f.x * f.x + f.y * f.y + f.z * f.z + f.w * f.w));
     f.x = f.x / len; f.y = f.y / len; f.z = f.z / len; f.w = f.w / len;
     return f;
-}
-
-// n_tile_blocked (nav.c:235)
-__device__ __forceinline__ bool tile_blocked_abs(const MapView &m, int layer, int ar, int ac)
-{
-    const size_t off = ((size_t)layer * m.H64 + ar) * m.W64 + ac;
-    return m.cost[off] == 0xFF || m.blk[off] > 0;
 }
 
 struct UpdateParams { int hz; float turn_rate; float adj_query_r; };

@@ -1146,6 +1146,7 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
     }
     cudaFree(ctx->d_ent_buf);
     if (ctx->ent_ev) cudaEventDestroy(ctx->ent_ev);
+    cudaFree(ctx->d_mq_buf);
     pfnav_fields_free(ctx);
     pfnav_agents_free(ctx);
     if (ctx->tick_done) cudaEventDestroy(ctx->tick_done);

@@ -90,6 +90,8 @@ struct pfnav_ctx {
     // host-side derived state, owned by the context (no process-global tables: contexts on different threads are independent)
     void *route_state = nullptr;                               // pfnav_route.cu: std::vector<pfnav_route_layer>
     void *route_dev_state = nullptr;                           // pfnav_route.cu: device copies of the routing tables (k_portal_graph_path_warp)
+    uint16_t *d_gisl = nullptr;                                // pfnav_route.cu: global islands, [layer][H64][W64] (pfnav_map_query)
+    void *d_mq_buf = nullptr; size_t mq_buf_bytes = 0;         // pfnav_query.cu: the inputs and outputs of one query batch
     std::set<std::pair<int, int>> dirty, fdirty;               // pfnav_blockers.cu: (layer, chunk) occupancy / faction mask changed
     void *blk_state = nullptr;                                 // pfnav_blockers.cu: queued blocker ops + device-side refcount state
 
@@ -258,7 +260,13 @@ struct pf_arrival_consts {
     int32_t nearest_ok; float nearest[2]; int32_t mc_n;
     float mc[PF_ARRIVAL_MC_MAX][2];
 };
-int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arrival_consts *out);
+// which: the searches to run; PF_ARRIVAL_MC needs pfnav_route_build(layer)
+enum { PF_ARRIVAL_NEAREST = 1, PF_ARRIVAL_MC = 2 };
+int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arrival_consts *out,
+                         int which = PF_ARRIVAL_NEAREST | PF_ARRIVAL_MC);
+// the device image of the global islands of `layer` ([H64][W64] u16, uploaded by pfnav_route_build), or nullptr when
+// the layer's routing structure is not built (pfnav_route.cu)
+const uint16_t *pfnav_route_dev_islands(const pfnav_ctx *ctx, int layer);
 
 // seeds of the flow-field repair chain (pfnav_route.cu), 64 rows x 64 bits
 int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int arg, uint64_t *mask);

@@ -209,6 +209,24 @@ int pfnav_route_refresh_edges(pfnav_ctx *ctx, int layer, int chunk)
     return flipped;
 }
 
+// The global islands of one layer as a row-major device image (ctx->d_gisl, [layer][H64][W64]) for the map queries.
+// They ignore blockers, so only a rebuild changes them.
+static int route_upload_islands(pfnav_ctx *ctx, int layer, const pfnav_route_layer &RL)
+{
+    const size_t ltiles = (size_t)ctx->W64 * ctx->H64;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    if (!ctx->d_gisl) PF_CUDA(cudaMalloc(&ctx->d_gisl, ltiles * ctx->nlayers * 2));
+    std::vector<uint16_t> img(ltiles);
+    for (int ch = 0; ch < ctx->chunk_w * ctx->chunk_h; ch++)
+        for (int r = 0; r < 64; r++)
+            memcpy(img.data() + (size_t)((ch / ctx->chunk_w) * 64 + r) * ctx->W64 + (ch % ctx->chunk_w) * 64,
+                   RL.islands.data() + (size_t)ch * 4096 + r * 64, 128);
+    PF_CUDA(cudaDeviceSynchronize());          // a query on a non-blocking stream may still read the old image
+    PF_CUDA(cudaMemcpy(ctx->d_gisl + ltiles * layer, img.data(), ltiles * 2, cudaMemcpyHostToDevice));
+    PF_CUDA(cudaDeviceSynchronize());
+    return PFNAV_OK;
+}
+
 // Build the routing structure of one layer (needs pfnav_map_build_nav first).
 extern "C" int pfnav_route_build(pfnav_ctx *ctx, int layer)
 {
@@ -299,8 +317,15 @@ extern "C" int pfnav_route_build(pfnav_ctx *ctx, int layer)
     }
     for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, RL, layer, ch);
     { static std::atomic<uint64_t> next_generation{1}; RL.generation = next_generation++; }
-    RL.built = true;
-    return PFNAV_OK;
+    RL.built = ctx->device < 0 || route_upload_islands(ctx, layer, RL) == PFNAV_OK;
+    return RL.built ? PFNAV_OK : PFNAV_ERR_CUDA;
+}
+
+// the device image of one layer's global islands, for pfnav_map_query
+const uint16_t *pfnav_route_dev_islands(const pfnav_ctx *ctx, int layer)
+{
+    if (!route_layer(ctx, layer) || !ctx->d_gisl) return nullptr;
+    return ctx->d_gisl + (size_t)layer * ctx->W64 * ctx->H64;
 }
 
 // Read-back for parity tests: islands and the edge table of one portal (neighbour ref, state, cost)
@@ -1100,15 +1125,14 @@ extern "C" int pfnav_pool_get(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c
 //     from the target (the target tile itself is never reported: it is marked visited up front and the
 //     {0,0} delta is skipped), as "tile centres" map_pos -/+ (abs tile index) * 4 (nav.c:4729-4732)
 // ------------------------------------------------------------------------------------------
-int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arrival_consts *out)
+int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arrival_consts *out, int which)
 {
     out->nearest_ok = 0; out->nearest[0] = out->nearest[1] = 0.0f; out->mc_n = 0;
     const pfnav_route_layer *prl = route_layer(ctx, layer);
-    if (!prl) {
+    if (!prl && (which & PF_ARRIVAL_MC)) {
         pfnav_set_error("pfnav_agents_compute_updates: pfnav_route_build(layer %d) is needed (global islands, nav.c:1731)", layer);
         return PFNAV_ERR_ARG;
     }
-    const pfnav_route_layer &RL = *prl;
     tdesc t;
     if (!desc_for_point(ctx, tx, tz, &t)) return PFNAV_OK;       // target outside the map: the reference asserts
     const int cw = ctx->chunk_w, chh = ctx->chunk_h, W = cw * 64, H = chh * 64;
@@ -1118,9 +1142,10 @@ int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arriv
     };
     const int tr = t.chunk_r * 64 + t.tile_r, tc = t.chunk_c * 64 + t.tile_c;
     // ---- N_ClosestPathable ----
-    if (!blocked(tr, tc)) {
+    const bool nearest = which & PF_ARRIVAL_NEAREST;
+    if (nearest && !blocked(tr, tc)) {
         out->nearest_ok = 1; out->nearest[0] = tx; out->nearest[1] = tz;
-    } else {
+    } else if (nearest) {
         std::vector<uint8_t> vis((size_t)W * H, 0);
         std::vector<int> q; q.push_back(tr * W + tc);
         for (size_t qi = 0; qi < q.size(); qi++) {
@@ -1143,7 +1168,8 @@ int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arriv
         }
     }
     // ---- n_closest_island_tiles(target, giid(target), ignore_blockers = false, maxout = 256) ----
-    {
+    if (which & PF_ARRIVAL_MC) {
+        const pfnav_route_layer &RL = *prl;
         const uint16_t giid = RL.islands[(size_t)(t.chunk_r * cw + t.chunk_c) * 4096 + t.tile_r * 64 + t.tile_c];
         std::vector<uint8_t> vis((size_t)W * H, 0);
         std::vector<int> q; q.push_back(tr * W + tc);
@@ -1621,6 +1647,12 @@ static route_dev_state *route_dev(pfnav_ctx *ctx)
 
 void pfnav_route_dev_forget(pfnav_ctx *ctx)
 {
+    if (ctx->d_gisl) {
+        cudaSetDevice(ctx->device);
+        cudaDeviceSynchronize();
+        cudaFree(ctx->d_gisl);
+        ctx->d_gisl = nullptr;
+    }
     route_dev_state *D = (route_dev_state *)ctx->route_dev_state;
     if (!D) return;
     if (ctx->device >= 0) {
