@@ -349,6 +349,29 @@ int  pfnav_fields_join(pfnav_ctx *ctx, void *stream);
  * FD_NONE (2) repairs the field in place: N_FlowFieldUpdateToNearestPathable when the tile is non-passable,
  * N_FlowFieldUpdateIslandToNearest otherwise. Blocking; needs pfnav_route_build. The caller re-runs the tick. */
 int  pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nrepairs);
+/* pfnav_pool_repair in device rounds: the same representatives, requests and repairs in the same order, leaving exactly
+ * the pool pfnav_pool_repair leaves (flow and LOS bytes, `has` bits, ff_ids, slot mapping and LRU state, entity-field
+ * footprints) and the same *out_nrequests / *out_nrepairs. The LOS-state requests are one request batch; the
+ * desired-velocity requests and repairs run in rounds of one request batch and one launch of predicated repairs (a
+ * repair applies only if its tile still has no direction when its turn comes); the enemy-seek / surround repairs are one
+ * launch. A round ends only where a request's emission depends on a byte written earlier in the round, would write a
+ * slot with a pending repair, or would evict. *out_nrounds: the rounds that launched work. Pointers may be NULL.
+ * Ordered on `stream` (NULL: the context's stream) after forked field work and pfnav_pool_clear; it waits for the device
+ * only to read back each phase's representatives and the bytes they stand on, at round boundaries (the round's request
+ * upload and its gather) and once at the end, never per entity. Errors as
+ * pfnav_pool_repair's: PFNAV_ERR_ARG (no agents / pool, pfnav_route_build missing where a request needs it),
+ * PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_NOMEM at representative k leaves 0 .. k-1 done as the serial
+ * loop leaves them. */
+int  pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nrequests, int *out_nrepairs, int *out_nrounds);
+/* TEST / MEASUREMENT HOOK, not part of the engine-facing API: what the last pfnav_pool_repair_batch call did.
+ * out6[0..2] = representatives (distinct misses) of phase 0 (LOS state), 1 (desired velocity), 2 (enemy-seek /
+ * surround); out6[3..5] = rounds the desired-velocity phase ended by rule (i) a request needing a byte written earlier in
+ * the round, (ii) a request writing a slot with a pending repair, (iii) a reservation that would evict. */
+int  pfnav_pool_repair_batch_stats(pfnav_ctx *ctx, int *out6);
+/* TEST HOOK, not part of the engine-facing API: the seeds (64 rows of 64 bits, bit c = column c) of a repair of a TARGET_TILE field of chunk
+ * (chunk_r, chunk_c) on `layer`, as the host builds them (kind / arg as in pfnav_flow_fields_repair). Works on a
+ * host-only context. */
+int  pfnav_repair_seed_mask(pfnav_ctx *ctx, int layer, int chunk_r, int chunk_c, int kind, int arg, uint64_t *out_rows);
 
 /* ---------------------------------------------------------------------------------------- */
 /* Region fields (SURVEY.md 8f-1): the dim x dim "cell arrival" fields a formation builds for every cell and

@@ -102,7 +102,7 @@ SYMBOLS = [
     "pfnav_agents_upload", "pfnav_agents_set_work", "pfnav_agents_tick",
     "pfnav_agents_read_velocities", "pfnav_agents_read_debug", "pfnav_ents_in_circle",
     "pfnav_agents_device_ptrs", "pfnav_agents_rebuild_index", "pfnav_launch_count", "pfnav_profile_enable",
-    "pfnav_profile_read", "pfnav_map_cost_from_tiles", "pfnav_map_get_layer", "pfnav_fields_join", "pfnav_flow_fields_repair", "pfnav_pool_repair", "pfnav_set_enemy_factions", "pfnav_request_faction", "pfnav_set_two_phase", "pfnav_los_trace", "pfnav_set_los_variant", "pfnav_blockers_incref_obb", "pfnav_blockers_decref_obb",
+    "pfnav_profile_read", "pfnav_map_cost_from_tiles", "pfnav_map_get_layer", "pfnav_fields_join", "pfnav_flow_fields_repair", "pfnav_pool_repair", "pfnav_pool_repair_batch", "pfnav_pool_repair_batch_stats", "pfnav_repair_seed_mask", "pfnav_set_enemy_factions", "pfnav_request_faction", "pfnav_set_two_phase", "pfnav_los_trace", "pfnav_set_los_variant", "pfnav_blockers_incref_obb", "pfnav_blockers_decref_obb",
     "pfnav_map_upload_factions", "pfnav_agents_upload_movestate", "pfnav_agents_compute_updates",
     "pfnav_agents_read_patches", "pfnav_agents_apply_updates", "pfnav_agents_read_state",
     "pfnav_region_fields", "pfnav_region_fields_dev", "pfnav_group_arrival_field", "pfnav_blockers_get_factions",
@@ -151,6 +151,9 @@ def load():
     L.pfnav_los_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfnav_map_upload_factions.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
     L.pfnav_pool_repair.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.pfnav_pool_repair_batch.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.pfnav_pool_repair_batch_stats.argtypes = [C.c_void_p, C.c_void_p]
+    L.pfnav_repair_seed_mask.argtypes = [C.c_void_p] + [C.c_int] * 5 + [C.c_void_p]
     L.pfnav_flow_fields_repair.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_region_fields.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                       C.c_size_t, C.c_void_p]
@@ -525,6 +528,25 @@ class Nav:
         a, b = C.c_int(0), C.c_int(0)
         _chk(self.L.pfnav_pool_repair(self.h, C.byref(a), C.byref(b)))
         return a.value, b.value
+
+    def pool_repair_batch(self, stream=None):
+        """pool_repair in device rounds -> (nrequests, nrepairs, nrounds); the pool ends up exactly as pool_repair leaves it"""
+        a, b, r = C.c_int(0), C.c_int(0), C.c_int(0)
+        _chk(self.L.pfnav_pool_repair_batch(self.h, C.c_void_p(stream or 0), C.byref(a), C.byref(b), C.byref(r)))
+        return a.value, b.value, r.value
+
+    def pool_repair_batch_stats(self):
+        """test / measurement hook: the last pool_repair_batch -> ((LOS, desired-velocity, enemy-field representatives),
+        (rounds ended by rule (i), (ii), (iii)))"""
+        out = np.zeros(6, np.int32)
+        _chk(self.L.pfnav_pool_repair_batch_stats(self.h, _p(out)))
+        return tuple(int(v) for v in out[:3]), tuple(int(v) for v in out[3:])
+
+    def repair_seed_mask(self, chunk, kind, arg, layer=0):
+        """the host's seeds of a repair of a TARGET_TILE field of `chunk` -> bool[64, 64]"""
+        rows = np.zeros(64, np.uint64)
+        _chk(self.L.pfnav_repair_seed_mask(self.h, layer, chunk[0], chunk[1], kind, arg, _p(rows)))
+        return np.unpackbits(rows.view(np.uint8), bitorder="little").reshape(64, 64).astype(bool)
 
     def los_trace(self, enable=True, read_cap=0):
         """arm / read the per-field LOS trace -> uint64[n, 4] = taken, ready, done (ns), 1 + pops"""

@@ -27,6 +27,7 @@
 #include "pfnav_internal.cuh"
 #include <algorithm>
 #include <math.h>
+#include <memory>
 #include <string.h>
 #include "pfnav_map_view.cuh"
 
@@ -1746,6 +1747,7 @@ void pfnav_agents_free(pfnav_ctx *ctx)
     ctx->d_enter = nullptr; ctx->d_ttiles = nullptr; ctx->cap_formation = ctx->cap_ms_ext = ctx->cap_enter = ctx->cap_ttiles = 0;
     if (ctx->update_done) cudaEventDestroy(ctx->update_done);
     cudaFree(ctx->d_los_out); cudaFree(ctx->d_work_count); cudaFree(ctx->d_scan_tmp);
+    cudaFree(ctx->d_rep_buf); ctx->d_rep_buf = nullptr; ctx->rep_buf_bytes = 0;
     ctx->d_agents = nullptr; ctx->d_records = nullptr; ctx->d_flocks = nullptr; ctx->d_flock_start = nullptr;
     ctx->d_flock_members = nullptr; ctx->d_cohesion = nullptr; ctx->d_cell_count = nullptr; ctx->d_cell_start = nullptr;
     ctx->d_cell_fill = nullptr; ctx->d_sorted_ix = nullptr; ctx->d_sorted_iy = nullptr; ctx->d_sorted_id = nullptr;
@@ -3204,6 +3206,379 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     if (nrep) ctx->goal_batch.valid = false;      // pool bytes changed under a resident plan
     if (out_nrequests) *out_nrequests = nreq;
     if (out_nrepairs) *out_nrepairs = nrep;
+    return PFNAV_OK;
+}
+
+// ---- pfnav_pool_repair_batch: representative selection and the round gather ----
+__device__ __forceinline__ uint64_t rep_key(const pf_miss &r, int kind)
+{
+    uint64_t key = ((uint64_t)r.dest << 40) | ((uint64_t)r.chunk << 20);
+    if (kind >= 1) key |= (r.liid == 0xFFFF ? (0x10000u | (uint32_t)r.tile) : (uint32_t)r.liid);
+    return key;
+}
+__device__ __forceinline__ uint32_t rep_hash(uint64_t key, uint32_t mask)
+{
+    key ^= key >> 33; key *= 0xff51afd7ed558ccdull; key ^= key >> 33;
+    return (uint32_t)key & mask;
+}
+
+// the first work index of every key among the misses (open addressing; keys are never ~0)
+__global__ void k_rep_mark(const pf_miss *__restrict__ miss, const uint32_t *__restrict__ cnt, uint32_t cap, int kind,
+                           unsigned long long *__restrict__ hkey, uint32_t *__restrict__ hwi, uint32_t hmask)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= min(cnt[0], cap)) return;
+    const pf_miss r = miss[i];
+    const unsigned long long key = rep_key(r, kind);
+    for (uint32_t h = rep_hash(key, hmask);; h = (h + 1) & hmask) {
+        const unsigned long long prev = atomicCAS(&hkey[h], ~0ull, key);
+        if (prev == ~0ull || prev == key) { atomicMin(&hwi[h], r.wi); return; }
+    }
+}
+
+// a miss that holds its key's first work index is the representative: place it at its work index
+__global__ void k_rep_flag(const pf_miss *__restrict__ miss, const uint32_t *__restrict__ cnt, uint32_t cap, int kind,
+                           const unsigned long long *__restrict__ hkey, const uint32_t *__restrict__ hwi, uint32_t hmask,
+                           pf_miss *__restrict__ by_wi, uint32_t *__restrict__ flag)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= min(cnt[0], cap)) return;
+    const pf_miss r = miss[i];
+    const unsigned long long key = rep_key(r, kind);
+    uint32_t h = rep_hash(key, hmask);
+    while (hkey[h] != key) h = (h + 1) & hmask;
+    if (hwi[h] != r.wi) return;
+    by_wi[r.wi] = r;
+    flag[r.wi] = 1;
+}
+
+// ordered compaction of the flagged work indices (one CTA): out = the representatives in work order, cnt[1] = their number
+#define REP_COMPACT_THREADS 1024
+__global__ void __launch_bounds__(REP_COMPACT_THREADS)
+k_rep_compact(const pf_miss *__restrict__ by_wi, const uint32_t *__restrict__ flag, int nwork, pf_miss *__restrict__ out,
+              uint32_t *__restrict__ cnt)
+{
+    __shared__ uint32_t part[REP_COMPACT_THREADS];
+    const int tid = threadIdx.x, per = (nwork + REP_COMPACT_THREADS - 1) / REP_COMPACT_THREADS;
+    const int lo = min(tid * per, nwork), hi = min(lo + per, nwork);
+    uint32_t n = 0;
+    for (int w = lo; w < hi; w++) n += flag[w];
+    part[tid] = n;
+    __syncthreads();
+    for (int d = 1; d < REP_COMPACT_THREADS; d <<= 1) {     // inclusive scan
+        const uint32_t v = tid >= d ? part[tid - d] : 0;
+        __syncthreads();
+        part[tid] += v;
+        __syncthreads();
+    }
+    uint32_t o = part[tid] - n;
+    for (int w = lo; w < hi; w++)
+        if (flag[w]) out[o++] = by_wi[w];
+    if (tid == REP_COMPACT_THREADS - 1) cnt[1] = part[tid];
+}
+
+// the direction byte of the tiles the remaining representatives stand on, at a round boundary
+__global__ void k_repair_gather(const int2 *__restrict__ slot_tile, int n, const uint8_t *__restrict__ flow, uint8_t *__restrict__ out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int2 st = slot_tile[i];
+    out[i] = st.x < 0 ? 0xFF : (flow[(size_t)st.x * 4096 + st.y] & 0xF);
+}
+
+// The on-miss chain of pfnav_pool_repair in device rounds (pfnav.h, DESIGN.md §3 a-4). Same phases, same representatives,
+// same decisions; the serial loop's per-representative read-backs become predicates the device evaluates (k_repair_chain)
+// or answers the host already holds, and a round ends only where neither is enough.
+extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nrequests, int *out_nrepairs, int *out_nrounds)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_agents && ctx->d_pool_slot, "agents / pool missing");
+    int *stats = ctx->repair_stats;           // pfnav_pool_repair_batch_stats
+    for (int k = 0; k < 6; k++) stats[k] = 0;
+    if (out_nrequests) *out_nrequests = 0;
+    if (out_nrepairs) *out_nrepairs = 0;
+    if (out_nrounds) *out_nrounds = 0;
+    if (ctx->n_work == 0) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_fields_join(ctx, st));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    const int nwork = (int)ctx->n_work;
+    const int chunks = ctx->chunk_w * ctx->chunk_h;
+    uint32_t cap = 1;
+    while (cap < 2u * (uint32_t)nwork) cap <<= 1;
+    // scratch: misses, misses by work index, representatives, flags, hash keys, hash minima, counters, gather in / out
+    const size_t b_m = (size_t)nwork * sizeof(pf_miss);
+    const size_t o_bywi = b_m, o_reps = 2 * b_m, o_flag = 3 * b_m, o_hkey = (o_flag + (size_t)nwork * 4 + 7) & ~(size_t)7;
+    const size_t o_hwi = o_hkey + (size_t)cap * 8, o_cnt = o_hwi + (size_t)cap * 4, o_gin = (o_cnt + 16 + 7) & ~(size_t)7;
+    const size_t o_gout = o_gin + (size_t)nwork * 8, total = o_gout + (size_t)nwork;
+    if (ctx->rep_buf_bytes < total) {
+        PF_CUDA(cudaStreamSynchronize(st));
+        cudaFree(ctx->d_rep_buf);
+        ctx->d_rep_buf = nullptr; ctx->rep_buf_bytes = 0;
+        if (cudaMalloc(&ctx->d_rep_buf, total) != cudaSuccess) { pfnav_set_error("cudaMalloc"); return PFNAV_ERR_NOMEM; }
+        ctx->rep_buf_bytes = total;
+    }
+    uint8_t *buf = (uint8_t *)ctx->d_rep_buf;
+    pf_miss *d_miss = (pf_miss *)buf, *d_bywi = (pf_miss *)(buf + o_bywi), *d_reps = (pf_miss *)(buf + o_reps);
+    uint32_t *d_flag = (uint32_t *)(buf + o_flag), *d_hwi = (uint32_t *)(buf + o_hwi), *d_cnt = (uint32_t *)(buf + o_cnt);
+    unsigned long long *d_hkey = (unsigned long long *)(buf + o_hkey);
+    int2 *d_gin = (int2 *)(buf + o_gin);
+    uint8_t *d_gout = buf + o_gout;
+    PF_CUDA(cudaMemsetAsync(d_cnt + 2, 0, 4, st));           // repairs applied by k_repair_chain
+    MapView m;
+    m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
+    m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
+    std::vector<int> flock_of_dest(ctx->pool_ndests, -1);
+    for (size_t f = 0; f < ctx->h_flocks.size(); f++)
+        if (ctx->h_flocks[f].dest >= 0 && ctx->h_flocks[f].dest < ctx->pool_ndests) flock_of_dest[ctx->h_flocks[f].dest] = (int)f;
+    int nreq = 0, nrounds = 0;
+    // the misses of one phase, one per key, first in work order, read back in work order
+    auto collect = [&](int kind, std::vector<pf_miss> &reps) -> int {
+        PoolView pv;
+        pv.slot = ctx->d_pool_slot; pv.flow = ctx->d_pool_flow; pv.los = ctx->d_pool_los;
+        pv.has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096; pv.ndests = ctx->pool_ndests;
+        pv.touch = nullptr; pv.tick_no = 0;
+        PF_CUDA(cudaMemsetAsync(d_cnt, 0, 8, st));
+        PF_CUDA(cudaMemsetAsync(d_flag, 0, (size_t)nwork * 4, st));
+        PF_CUDA(cudaMemsetAsync(d_hkey, 0xFF, (size_t)cap * 8, st));
+        PF_CUDA(cudaMemsetAsync(d_hwi, 0xFF, (size_t)cap * 4, st));
+        const unsigned nb = (nwork + 127) / 128;
+        k_collect_misses<<<nb, 128, 0, st>>>(m, pv, ctx->d_liid, ctx->d_agents, ctx->d_flocks, ctx->d_work, nwork, kind, d_miss,
+                                             d_cnt, (uint32_t)nwork, ctx->d_ms_ext, ctx->nlayers);
+        k_rep_mark<<<nb, 128, 0, st>>>(d_miss, d_cnt, (uint32_t)nwork, kind, d_hkey, d_hwi, cap - 1);
+        k_rep_flag<<<nb, 128, 0, st>>>(d_miss, d_cnt, (uint32_t)nwork, kind, d_hkey, d_hwi, cap - 1, d_bywi, d_flag);
+        k_rep_compact<<<1, REP_COMPACT_THREADS, 0, st>>>(d_bywi, d_flag, nwork, d_reps, d_cnt);
+        ctx->launches += 4;
+        PF_CUDA(cudaGetLastError());
+        uint32_t nrep = 0;
+        PF_CUDA(cudaMemcpyAsync(&nrep, d_cnt + 1, 4, cudaMemcpyDeviceToHost, st));
+        PF_CUDA(cudaStreamSynchronize(st));
+        reps.resize(std::min<uint32_t>(nrep, (uint32_t)nwork));
+        if (!reps.empty()) {
+            PF_CUDA(cudaMemcpyAsync(reps.data(), d_reps, reps.size() * sizeof(pf_miss), cudaMemcpyDeviceToHost, st));
+            PF_CUDA(cudaStreamSynchronize(st));
+        }
+        stats[kind] = (int)reps.size();
+        return 0;
+    };
+    auto key_of = [&](const pf_miss &r) { return (size_t)r.dest * chunks + r.chunk; };
+    auto has_flow = [&](int slot) { return slot >= 0 && (ctx->h_pool_has[slot] & 1); };
+    // the path requests of a phase's representatives, planned up front (flock target, flock layer)
+    auto plan = [&](const std::vector<pf_miss> &reps, pf_path_batch **out) -> int {
+        const size_t n = reps.size();
+        std::vector<int32_t> dests(n), layers(n);
+        std::vector<float> src(2 * n), dst(2 * n);
+        for (size_t i = 0; i < n; i++) {
+            const int f = flock_of_dest[reps[i].dest];
+            const pfnav_flock &fl = ctx->h_flocks[f < 0 ? 0 : f];
+            dests[i] = reps[i].dest; layers[i] = f < 0 ? -1 : fl.layer;
+            src[2 * i] = reps[i].px; src[2 * i + 1] = reps[i].pz;
+            dst[2 * i] = f < 0 ? 0.0f : fl.target[0]; dst[2 * i + 1] = f < 0 ? 0.0f : fl.target[1];
+        }
+        return pf_path_batch_begin(ctx, (int)n, dests.data(), layers.data(), src.data(), dst.data(), st, out);
+    };
+    using batch_ptr = std::unique_ptr<pf_path_batch, void (*)(pf_path_batch *)>;
+    std::vector<pf_miss> reps;
+    int rc = 0;
+    pf_path_probe pr;
+    // ---- LOS state (N_HasDestLOS, nav.c:4038-4045): one request batch, skipping a (dest, chunk) whose LOS field an
+    //      earlier representative's request built ----
+    if ((rc = collect(0, reps))) return rc;
+    if (!reps.empty()) {
+        pf_path_batch *pb = nullptr;
+        if ((rc = plan(reps, &pb))) return rc;
+        batch_ptr B(pb, pf_path_batch_end);
+        bool any = false;
+        for (size_t i = 0; i < reps.size() && !rc; i++) {
+            const int slot = ctx->h_pool_slot[key_of(reps[i])];
+            if (slot >= 0 && (ctx->h_pool_has[slot] & 2)) continue;
+            if (flock_of_dest[reps[i].dest] < 0) continue;
+            if ((rc = pf_path_batch_probe(pb, (int)i, &pr))) break;    // PFNAV_ERR_ARG, as pfnav_pool_request_path's
+            if (pr.nf + pr.nl == 0) continue;
+            if ((rc = pf_path_batch_commit(pb, nullptr))) break;
+            nreq++; any = true;
+        }
+        int frc = pf_path_batch_flush(pb);
+        if (frc) return frc;
+        nrounds += any;
+        if (rc) return rc;
+    }
+    // ---- desired velocity (N_DesiredPointSeekVelocity, nav.c:3483-3554): requests and predicated repairs in rounds ----
+    if ((rc = collect(1, reps))) return rc;
+    if (!reps.empty()) {
+        const size_t n = reps.size();
+        pf_path_batch *pb = nullptr;
+        if ((rc = plan(reps, &pb))) return rc;
+        batch_ptr B(pb, pf_path_batch_end);
+        // what each representative's tile holds at the start of the round: its slot then, and the direction byte
+        std::vector<int32_t> slot0(n);
+        std::vector<uint8_t> dir0(n, 0);
+        std::vector<uint8_t> written(ctx->pool_max, 0), chained(ctx->pool_max, 0);
+        std::vector<int32_t> touched;                     // slots marked in written / chained this round
+        std::vector<pf_chain_item> items;
+        std::vector<uint64_t> masks;
+        bool pending = false;
+        std::vector<int2> gin;
+        std::vector<uint8_t> gout;
+        // read the bytes representatives from.. stand on, as the pool holds them once the work queued so far is done
+        auto gather = [&](size_t from) -> int {
+            gin.clear();
+            for (size_t k = from; k < n; k++) {
+                const int s = ctx->h_pool_slot[key_of(reps[k])];
+                slot0[k] = has_flow(s) ? s : -1;
+                gin.push_back(make_int2(slot0[k], reps[k].tile));
+            }
+            if (gin.empty()) return 0;
+            gout.resize(gin.size());
+            PF_CUDA(cudaMemcpyAsync(d_gin, gin.data(), gin.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+            k_repair_gather<<<((unsigned)gin.size() + 127) / 128, 128, 0, st>>>(d_gin, (int)gin.size(), ctx->d_pool_flow, d_gout);
+            ctx->launches++;
+            PF_CUDA(cudaGetLastError());
+            PF_CUDA(cudaMemcpyAsync(gout.data(), d_gout, gout.size(), cudaMemcpyDeviceToHost, st));
+            PF_CUDA(cudaStreamSynchronize(st));
+            for (size_t k = from; k < n; k++) dir0[k] = gout[k - from];
+            return 0;
+        };
+        // end the round: launch its requests and chain items, then gather for the representatives still to come
+        auto boundary = [&](size_t from) -> int {
+            int r2 = pf_path_batch_flush(pb);
+            if (r2) return r2;
+            if ((r2 = pfnav_repair_chain_launch(ctx, st, items, masks, d_cnt + 2))) return r2;
+            nrounds += pending;
+            items.clear(); masks.clear();
+            for (int32_t s : touched) written[s] = chained[s] = 0;
+            touched.clear();
+            pending = false;
+            return gather(from);
+        };
+        if ((rc = gather(0))) return rc;
+        auto mark = [&](std::vector<uint8_t> &v, int32_t s) { if (!written[s] && !chained[s]) touched.push_back(s); v[s] = 1; };
+        std::vector<int32_t> wslots;
+        for (size_t i = 0; i < n;) {
+            const pf_miss &r = reps[i];
+            const size_t key = key_of(r);
+            if (flock_of_dest[r.dest] < 0) { i++; continue; }       // no request, no repair (nav.c:3501)
+            // step a of the serial loop: the tile's direction before the request, if the host knows it
+            const int s = ctx->h_pool_slot[key];
+            int dir = -1;                                            // -1: no flow field
+            bool known = true;
+            if (has_flow(s)) {
+                if (written[s] || chained[s] || s != slot0[i]) known = false;
+                else dir = dir0[i];
+            }
+            if (!pf_path_batch_planned(pb, (int)i)) {
+                // the serial request fails (PFNAV_ERR_ARG) unless an earlier representative served this tile
+                if (!known) { stats[3]++; if ((rc = boundary(i))) break; continue; }
+                if (dir > 0) { i++; continue; }
+                rc = pf_path_batch_probe(pb, (int)i, &pr);
+                break;
+            }
+            if ((rc = pf_path_batch_probe(pb, (int)i, &pr))) break;
+            if (pr.nf + pr.nl > 0) {
+                if (!known) { stats[3]++; if ((rc = boundary(i))) break; continue; }         // rule (i)
+                if (dir > 0) { i++; continue; }                                                // served: no request
+                bool hit = false;
+                for (int32_t ws : pr.write_slots) hit |= chained[ws] != 0;
+                if (hit || (pr.would_evict && pending)) {                                     // rules (ii), (iii)
+                    stats[hit ? 4 : 5]++;
+                    if ((rc = boundary(i))) break;
+                    continue;
+                }
+                if ((rc = pf_path_batch_commit(pb, &wslots))) break;
+                nreq++; pending = true;
+                for (int32_t ws : wslots) mark(written, ws);
+            } else if (known && dir > 0) { i++; continue; }
+            if (!pr.ok) { i++; continue; }                           // no path from here: zero vector, nothing repaired
+            const int sl = ctx->h_pool_slot[key];
+            if (!has_flow(sl)) { i++; continue; }                    // no field: nothing to repair
+            pf_chain_item it;
+            it.q = ctx->h_pool_req[sl]; it.slot = sl; it.tile = r.tile; it.always = 0; it.mask = -1;
+            if (r.liid == 0xFFFF) { it.kind = PFNAV_REPAIR_NEAREST_PATHABLE; it.arg = ((r.tile >> 6) << 8) | (r.tile & 63); }
+            else                  { it.kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; it.arg = r.liid; }
+            std::vector<uint64_t> mask(64);
+            const int src = it.kind == 0 ? pfnav_repair_start_check(ctx, it.q, it.arg)
+                                         : pfnav_repair_seeds(ctx, it.q, it.kind, it.arg, mask.data());
+            if (src) {
+                // the serial loop fails here only if the repair runs: decide on the byte as the round leaves it. With
+                // nothing pending, nothing ran since the last gather and the byte read there is still the pool's.
+                const int keep = src;
+                if (pending && (rc = boundary(i))) break;
+                if (dir0[i] == 0) { rc = keep; break; }
+                i++;
+                continue;
+            }
+            if (it.kind == 1) { it.mask = (int32_t)(masks.size() / 64); masks.insert(masks.end(), mask.begin(), mask.end()); }
+            items.push_back(it);
+            mark(chained, sl);
+            pending = true;
+            i++;
+        }
+        if (pending || !items.empty()) {
+            const int rc2 = boundary(n);
+            if (!rc) rc = rc2;
+        } else {
+            const int rc2 = pf_path_batch_flush(pb);
+            if (!rc) rc = rc2;
+        }
+        if (rc) return rc;
+    }
+    // ---- enemy-seek / surround fields: in-place repairs only (nav.c:3647-3675, 3729-3757), one launch ----
+    if ((rc = collect(2, reps))) return rc;
+    {
+        std::vector<pf_chain_item> items;
+        std::vector<uint64_t> masks;
+        for (size_t i = 0; i < reps.size(); i++) {
+            const pf_miss &r = reps[i];
+            const int slot = ctx->h_pool_slot[key_of(r)];
+            if (!has_flow(slot)) continue;
+            const pfnav_field_req tg = ctx->h_pool_req[slot];
+            if ((tg.target_type & 0xFF) < 2) continue;
+            const bool surround = (tg.target_type & 0xFF) == 2 + PFNAV_TARGET_ENTITY;
+            pf_chain_item it;
+            it.q = tg; it.slot = slot; it.tile = r.tile; it.mask = -1;
+            if (r.liid == 0xFFFF) { it.kind = PFNAV_REPAIR_NEAREST_PATHABLE; it.arg = ((r.tile >> 6) << 8) | (r.tile & 63); it.always = surround; }
+            else                  { it.kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; it.arg = r.liid; it.always = 0; }
+            std::vector<uint64_t> mask(64);
+            const int src = it.kind == 0 ? pfnav_repair_start_check(ctx, it.q, it.arg)
+                                         : pfnav_repair_seeds(ctx, it.q, it.kind, it.arg, mask.data());
+            if (src) {
+                // fails only if the repair runs: apply what comes before it, then read the byte
+                if ((rc = pfnav_repair_chain_launch(ctx, st, items, masks, d_cnt + 2))) return rc;
+                if (!items.empty()) nrounds++;
+                items.clear(); masks.clear();
+                uint8_t d = 0;
+                PF_CUDA(cudaMemcpyAsync(&d, ctx->d_pool_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost, st));
+                PF_CUDA(cudaStreamSynchronize(st));
+                if (it.always || (d & 0xF) == 0) { rc = src; break; }
+                continue;
+            }
+            if (it.kind == 1) { it.mask = (int32_t)(masks.size() / 64); masks.insert(masks.end(), mask.begin(), mask.end()); }
+            items.push_back(it);
+        }
+        if (!items.empty()) {
+            const int rc2 = pfnav_repair_chain_launch(ctx, st, items, masks, d_cnt + 2);
+            if (!rc) rc = rc2;
+            nrounds++;
+        }
+    }
+    if (rc) return rc;
+    uint32_t nrep = 0;
+    PF_CUDA(cudaMemcpyAsync(&nrep, d_cnt + 2, 4, cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    if (nrep) ctx->goal_batch.valid = false;      // pool bytes changed under a resident plan
+    if (out_nrequests) *out_nrequests = nreq;
+    if (out_nrepairs) *out_nrepairs = (int)nrep;
+    if (out_nrounds) *out_nrounds = nrounds;
+    return PFNAV_OK;
+}
+
+// Test / measurement hook: what the last pfnav_pool_repair_batch call did (pfnav.h).
+extern "C" int pfnav_pool_repair_batch_stats(pfnav_ctx *ctx, int *out6)
+{
+    PF_ARG(ctx && out6, "args");
+    for (int k = 0; k < 6; k++) out6[k] = ctx->repair_stats[k];
     return PFNAV_OK;
 }
 

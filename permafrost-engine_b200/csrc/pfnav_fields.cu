@@ -95,6 +95,7 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, u
 }
 
 #include "pfnav_los_kernel.cuh"   // bit helpers, FlowGrids, k_los_b, k_los_level
+#include "pfnav_repair_kernel.cuh"   // kind-0 repair seeds of k_repair_chain
 
 // ------------------------------------------------------------------------------------------
 // Map-state kernels
@@ -665,6 +666,147 @@ k_flow_repair(FlowGrids g, const pfnav_field_req *__restrict__ reqs, const int32
         }
         __syncthreads();
     }
+}
+
+// ------------------------------------------------------------------------------------------
+// K1c: one round of the on-miss chain of pfnav_pool_repair_batch. One CTA per pool slot that has items in the round;
+// it walks the slot's items in the serial loop's order and applies an item only if the tile it names still has no
+// direction when the item's turn comes (or always, for the surround variant on a blocked tile): the serial loop's
+// read-back before the repair, answered where the byte lives. The integration is k_flow_repair's, restated so that
+// kernel stays as it is; kind-0 seeds are flooded in the CTA (pfnav_repair_kernel.cuh), kind-1 seeds come from the host.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(FLOWG_THREADS)
+k_repair_chain(FlowGrids g, const pf_chain_item *__restrict__ items, const int32_t *__restrict__ group_off, int ngroups,
+               const uint64_t *__restrict__ host_masks, uint8_t *__restrict__ fields, uint32_t *__restrict__ count)
+{
+    __shared__ uint32_t dist[4096];
+    __shared__ uint8_t cost[4096];       // raw cost_base
+    __shared__ uint8_t dom[4096];        // 1 = tile takes part in the integration, 2 = seed
+    __shared__ uint64_t seed[64];
+    __shared__ repair_seed_smem ss;
+    __shared__ int changed, apply;
+    const int tid = threadIdx.x;
+    for (int gi = blockIdx.x; gi < ngroups; gi += gridDim.x) {
+        for (int it = group_off[gi]; it < group_off[gi + 1]; it++) {
+            const pf_chain_item item = items[it];
+            const pfnav_field_req q = item.q;
+            const int kind = item.kind;
+            uint8_t *dst = fields + (size_t)item.slot * 4096;
+            __syncthreads();
+            if (tid == 0) apply = item.always || (dst[item.tile] & 0xF) == 0;
+            __syncthreads();
+            if (!apply) continue;
+            const size_t lbase = (size_t)q.layer * g.H64 * g.W64;
+            if (kind == 0)       // arg = start_r << 8 | start_c
+                repair_nearest_pathable_seeds(g.cost, g.blk, lbase, g.W64, q.chunk_r, q.chunk_c,
+                                              ((item.arg >> 8) << 6) | (item.arg & 63), ss, seed);
+            else if (tid < 64) seed[tid] = host_masks[(size_t)item.mask * 64 + tid];
+            __syncthreads();
+            for (int t = tid; t < 4096; t += FLOWG_THREADS) {
+                const size_t off = lbase + (size_t)(q.chunk_r * 64 + (t >> 6)) * g.W64 + q.chunk_c * 64 + (t & 63);
+                const uint8_t c = g.cost[off];
+                const bool pass = c != 0xFF && !blocked_for(g, q.faction_id, off);
+                const bool sd = (seed[t >> 6] >> (t & 63)) & 1;
+                cost[t] = c;
+                dom[t] = sd ? 2 : (kind == 0 ? !pass : pass) ? 1 : 0;
+                dist[t] = sd ? 0u : 0xFFFFFFFFu;
+            }
+            do {
+                __syncthreads();
+                if (tid == 0) changed = 0;
+                __syncthreads();
+                bool ch = false;
+                for (int t = tid; t < 4096; t += FLOWG_THREADS) {
+                    if (dom[t] != 1) continue;
+                    const int r = t >> 6, cc = t & 63;
+                    uint32_t m = 0xFFFFFFFFu;
+                    if (r > 0)   m = min(m, dist[t - 64]);
+                    if (r < 63)  m = min(m, dist[t + 64]);
+                    if (cc > 0)  m = min(m, dist[t - 1]);
+                    if (cc < 63) m = min(m, dist[t + 1]);
+                    if (m != 0xFFFFFFFFu && m + cost[t] < dist[t]) { dist[t] = m + cost[t]; ch = true; }
+                }
+                if (ch) changed = 1;
+                __syncthreads();
+            } while (changed);
+
+            const bool up = q.next_chunk_r < q.chunk_r, down = q.next_chunk_r > q.chunk_r;
+            const bool left = q.next_chunk_c < q.chunk_c;
+            const uint8_t fix = up ? 2 : down ? 7 : left ? 4 : 5;
+            for (int t = tid; t < 4096; t += FLOWG_THREADS) {
+                const uint32_t d = dist[t];
+                if (d == 0xFFFFFFFFu) continue;
+                if (d == 0) {
+                    if (kind == 1) dst[t] = (q.target_type == PFNAV_TARGET_PORTAL) ? fix : 0;
+                    continue;
+                }
+                const int r = t >> 6, c = t & 63;
+                const uint32_t INF = 0xFFFFFFFFu;
+                const uint32_t dn = r > 0 ? dist[t - 64] : INF, ds = r < 63 ? dist[t + 64] : INF;
+                const uint32_t dw = c > 0 ? dist[t - 1] : INF, de = c < 63 ? dist[t + 1] : INF;
+                const uint32_t dnw = (r > 0 && c > 0) ? dist[t - 65] : INF, dne = (r > 0 && c < 63) ? dist[t - 63] : INF;
+                const uint32_t dsw = (r < 63 && c > 0) ? dist[t + 63] : INF, dse = (r < 63 && c < 63) ? dist[t + 65] : INF;
+                uint32_t m = min(min(dn, ds), min(dw, de));
+                if (dn != INF && dw != INF) m = min(m, dnw);
+                if (dn != INF && de != INF) m = min(m, dne);
+                if (ds != INF && dw != INF) m = min(m, dsw);
+                if (ds != INF && de != INF) m = min(m, dse);
+                uint8_t dir;   // field.c:405-428 priority N,S,E,W,NW,NE,SW,SE
+                if (dn == m) dir = 2; else if (ds == m) dir = 7; else if (de == m) dir = 5; else if (dw == m) dir = 4;
+                else if (dnw == m) dir = 1; else if (dne == m) dir = 3; else if (dsw == m) dir = 6; else dir = 8;
+                dst[t] = dir;
+            }
+            if (tid == 0) atomicAdd(count, 1u);
+            __syncthreads();      // the next item of this slot reads the bytes written here
+        }
+    }
+}
+
+static FlowGrids grids_of(const pfnav_ctx *ctx);
+
+int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pf_chain_item> &items,
+                              const std::vector<uint64_t> &masks, uint32_t *d_count)
+{
+    if (items.empty()) return PFNAV_OK;
+    // group by slot, serial order inside a group (a stable sort)
+    std::vector<int32_t> order(items.size());
+    for (size_t i = 0; i < items.size(); i++) order[i] = (int32_t)i;
+    std::stable_sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return items[a].slot < items[b].slot; });
+    std::vector<pf_chain_item> sorted(items.size());
+    std::vector<int32_t> off;
+    for (size_t k = 0; k < order.size(); k++) {
+        sorted[k] = items[order[k]];
+        if (k == 0 || sorted[k].slot != sorted[k - 1].slot) off.push_back((int32_t)k);
+    }
+    off.push_back((int32_t)sorted.size());
+    const int ngroups = (int)off.size() - 1;
+    const size_t b_item = sorted.size() * sizeof(pf_chain_item), b_mask = masks.size() * 8, b_off = off.size() * 4;
+    const size_t a_mask = (b_item + 15) & ~(size_t)15, a_off = a_mask + b_mask, total = a_off + b_off;
+    if (ctx->plan_buf_bytes < total) {
+        PF_CUDA(cudaStreamSynchronize(st));
+        cudaFree(ctx->d_plan_buf);
+        ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
+        PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
+        ctx->plan_buf_bytes = total * 2;
+    }
+    // staged in the pinned ring (pf_plan_host): the copy is asynchronous and the host does not wait for it
+    uint8_t *host = nullptr;
+    int ri = 0;
+    int rc = pf_plan_host(ctx, total, &host, &ri);
+    if (rc) return rc;
+    memcpy(host, sorted.data(), b_item);
+    if (b_mask) memcpy(host + a_mask, masks.data(), b_mask);
+    memcpy(host + a_off, off.data(), b_off);
+    uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
+    ctx->goal_batch.valid = false;          // the staging buffer is reused
+    PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    k_repair_chain<<<(unsigned)std::min(ngroups, ctx->sm_count * 8), FLOWG_THREADS, 0, st>>>(
+        grids_of(ctx), (const pf_chain_item *)dev, (const int32_t *)(dev + a_off), ngroups, (const uint64_t *)(dev + a_mask),
+        ctx->d_pool_flow, d_count);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
 }
 
 // ------------------------------------------------------------------------------------------

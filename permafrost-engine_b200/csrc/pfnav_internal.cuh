@@ -200,6 +200,9 @@ struct pfnav_ctx {
     // entity-field batches (pfnav_region.cu): device scratch for the staged inputs, footprint rows and seed bitmaps,
     // grown on demand; ent_ev is recorded after the last kernel that reads it
     void *d_ent_buf = nullptr; size_t ent_buf_bytes = 0; cudaEvent_t ent_ev = nullptr;
+    // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand
+    void *d_rep_buf = nullptr; size_t rep_buf_bytes = 0;
+    int repair_stats[6] = {0, 0, 0, 0, 0, 0};                  // the last call: representatives per phase, rounds ended per rule
 
     // ---- optional per-kernel timing (pfnav_profile_enable) ----
     bool profiling = false;
@@ -273,6 +276,38 @@ int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int a
 
 int pfnav_flow_repair_pool(pfnav_ctx *ctx, const pfnav_field_req *targets, const int32_t *kinds, const int32_t *args,
                            const int32_t *slots, size_t n);
+// the argument checks pfnav_repair_seeds makes of a kind-0 repair, without building its seeds (pfnav_route.cu)
+int pfnav_repair_start_check(pfnav_ctx *ctx, const pfnav_field_req &q, int arg);
+
+// One predicated repair of pfnav_pool_repair_batch (k_repair_chain, pfnav_fields.cu): applied to pool slot `slot` when its
+// turn comes if the direction of `tile` is FD_NONE then, or always (`always`: the surround variant on a blocked tile).
+// kind 0 builds its seeds on the device from start tile `arg`; kind 1 reads mask row block `mask` (64 x u64).
+struct pf_chain_item {
+    pfnav_field_req q;
+    int32_t slot, tile, kind, arg, always, mask;
+};
+// Launch one round of chain items on `st`: items grouped by slot (one CTA per group, items in order); the repairs
+// applied are added to *d_count. The item and mask arrays are copied on `st` before the call returns.
+int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pf_chain_item> &items,
+                              const std::vector<uint64_t> &masks, uint32_t *d_count);
+
+// Staged path requests against the pool (pfnav_route.cu), shared by pfnav_pool_request_paths and pfnav_pool_repair_batch:
+// begin plans requests i = 0 .. n-1 (each on its own layer) up front; probe emits request i against the pool mirrors as
+// they are now without changing anything; commit reserves and stages the probed emission (PFNAV_ERR_NOMEM: nothing
+// changed); flush launches what is staged on the stream and uploads the slot table and `has` bytes.
+struct pf_path_batch;
+struct pf_path_probe {
+    int nf = 0, nl = 0, ok = 0; uint32_t dest_id = 0;
+    bool would_evict = false;                 // the reservation needs more slots than are free
+    std::vector<int32_t> write_slots;         // slots already mapped that the emission writes
+};
+int  pf_path_batch_begin(pfnav_ctx *ctx, int n, const int32_t *dests, const int32_t *layers, const float *src_xz,
+                         const float *dst_xz, cudaStream_t st, pf_path_batch **out);
+bool pf_path_batch_planned(const pf_path_batch *B, int i);     // false: the layer is not routed or a point is off the map
+int  pf_path_batch_probe(pf_path_batch *B, int i, pf_path_probe *out);
+int  pf_path_batch_commit(pf_path_batch *B, std::vector<int32_t> *out_slots);   // out: the slots written
+int  pf_path_batch_flush(pf_path_batch *B);
+void pf_path_batch_end(pf_path_batch *B);
 
 int pfnav_fmask_push_chunk(pfnav_ctx *ctx, int layer, int chunk);
 int pfnav_blockers_flush(pfnav_ctx *ctx);                        // pfnav_blockers.cu: apply the queued blocker operations now

@@ -23,6 +23,7 @@
 #include <deque>
 #include <float.h>
 #include <math.h>
+#include <memory>
 #include <string.h>
 #include <unordered_map>
 
@@ -938,112 +939,203 @@ static int launch_segment(pfnav_ctx *ctx, cudaStream_t st, const path_segment &S
 
 }   // namespace
 
+// The staged form of a path-request batch (pfnav_internal.cuh): every request planned up front, then emitted against
+// the pool mirrors one by one in the caller's order, reserved, and staged into a segment for the device.
+struct pf_path_batch {
+    pfnav_ctx *ctx = nullptr;
+    cudaStream_t st = nullptr;
+    std::vector<int32_t> dests, layers;
+    std::vector<path_plan> plans;
+    std::vector<uint8_t> planned;              // the request's layer is routed and both of its points are on the map
+    path_segment S;
+    path_emit E;                               // the emission of the last probed request
+    int probed = -1;
+    std::vector<size_t> keys;                  // its (dest, chunk) keys: flow writes, LOS writes, LOS parents read
+    std::vector<uint64_t> mapped;
+    std::vector<uint8_t> los_have, row_touched;
+    bool any_evicted = false;
+};
+
+int pf_path_batch_begin(pfnav_ctx *ctx, int n, const int32_t *dests, const int32_t *layers, const float *src_xz,
+                        const float *dst_xz, cudaStream_t st, pf_path_batch **out)
+{
+    *out = nullptr;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(pf_fields_sync(ctx));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    std::unique_ptr<pf_path_batch> B(new pf_path_batch);
+    B->ctx = ctx; B->st = st;
+    B->dests.assign(dests, dests + n); B->layers.assign(layers, layers + n);
+    B->plans.resize(n); B->planned.assign(n, 0);
+    const int cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
+    B->mapped.resize(chunks); B->los_have.resize(chunks); B->row_touched.assign(ctx->pool_ndests, 0);
+    std::vector<tdesc> s(n), d(n);
+    std::set<int> used_layers;
+    for (int i = 0; i < n; i++) {
+        B->planned[i] = route_layer(ctx, layers[i]) && desc_for_point(ctx, src_xz[2 * i], src_xz[2 * i + 1], &s[i]) &&
+                        desc_for_point(ctx, dst_xz[2 * i], dst_xz[2 * i + 1], &d[i]);
+        if (B->planned[i]) used_layers.insert(layers[i]);
+    }
+    for (int layer : used_layers) {
+        pfnav_route_layer &RL = *route_layer(ctx, layer);
+        // n_update_all_edge_states (nav.c:1787): the map does not change between the requests of a batch
+        for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, RL, layer, ch);
+        Router R{ctx, RL, layer, cw, ctx->chunk_h};
+        std::vector<int> idx;
+        for (int i = 0; i < n; i++) if (B->planned[i] && layers[i] == layer) idx.push_back(i);
+        std::vector<path_plan> plans(idx.size());
+        for (size_t k = 0; k < idx.size(); k++) plan_init(ctx, layer, s[idx[k]], d[idx[k]], plans[k]);
+        int rc = plan_requests(ctx, R, layer, plans);
+        if (rc) return rc;
+        for (size_t k = 0; k < idx.size(); k++) B->plans[idx[k]] = std::move(plans[k]);
+    }
+    *out = B.release();
+    return PFNAV_OK;
+}
+
+void pf_path_batch_end(pf_path_batch *B) { delete B; }
+
+bool pf_path_batch_planned(const pf_path_batch *B, int i) { return B->planned[i] != 0; }
+
+int pf_path_batch_probe(pf_path_batch *B, int i, pf_path_probe *out)
+{
+    pfnav_ctx *ctx = B->ctx;
+    PF_ARG(B->planned[i], "pfnav_route_build not called, or a position outside the map");
+    const int layer = B->layers[i], cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
+    const size_t row = (size_t)B->dests[i] * chunks;
+    for (int c = 0; c < chunks; c++) {
+        const int s = ctx->h_pool_slot[row + c];
+        B->los_have[c] = (s >= 0 && (ctx->h_pool_has[s] & 2)) ? 1 : 0;
+    }
+    memcpy(B->mapped.data(), ctx->h_pool_ffid.data() + row, (size_t)chunks * 8);
+    Router R{ctx, *route_layer(ctx, layer), layer, cw, ctx->chunk_h};
+    path_emit &E = B->E;
+    emit_plan(R, ctx, layer, B->plans[i], B->mapped.data(), B->los_have.data(), E);
+    const int nf = (int)E.fr.size(), nl = (int)E.lr.size();
+    B->probed = i;
+    out->dest_id = B->plans[i].dest_id; out->ok = B->plans[i].ok; out->nf = nf; out->nl = nl;
+    out->would_evict = false;
+    out->write_slots.clear();
+    // slots for everything this request writes (and the previous-chunk LOS fields it reads), all or nothing
+    std::vector<size_t> &keys = B->keys;
+    keys.clear();
+    for (int k = 0; k < nf; k++) keys.push_back(row + E.fc[k]);
+    for (int k = 0; k < nl; k++) keys.push_back(row + E.lc[k]);
+    for (int k = 0; k < nl; k++)
+        if (E.lr[k].prev_index == -2) keys.push_back(row + E.lr[k].prev_chunk_r * cw + E.lr[k].prev_chunk_c);
+    std::vector<size_t> fresh;
+    for (size_t k = 0; k < keys.size(); k++) {
+        const int32_t s = ctx->h_pool_slot[keys[k]];
+        if (k < (size_t)(nf + nl) && s >= 0) out->write_slots.push_back(s);
+        if (s < 0) fresh.push_back(keys[k]);
+    }
+    std::sort(fresh.begin(), fresh.end());
+    const size_t nfresh = std::unique(fresh.begin(), fresh.end()) - fresh.begin();
+    out->would_evict = nfresh > ctx->pool_free.size() + (size_t)(ctx->pool_max - ctx->pool_used);
+    return PFNAV_OK;
+}
+
+int pf_path_batch_commit(pf_path_batch *B, std::vector<int32_t> *out_slots)
+{
+    pfnav_ctx *ctx = B->ctx;
+    const path_emit &E = B->E;
+    const int dest = B->dests[B->probed], cw = ctx->chunk_w;
+    const size_t row = (size_t)dest * cw * ctx->chunk_h;
+    const int nf = (int)E.fr.size(), nl = (int)E.lr.size();
+    if (out_slots) out_slots->clear();
+    if (nf == 0 && nl == 0) return PFNAV_OK;
+    ctx->goal_batch.valid = false;          // the staging buffer is about to be reused
+    const std::vector<size_t> &keys = B->keys;
+    std::vector<int32_t> slots(keys.size());
+    bool evicted = false;
+    int rc = pf_pool_reserve(ctx, keys.data(), keys.size(), slots.data(), &evicted);
+    if (rc) return rc;
+    path_segment &S = B->S;
+    B->any_evicted |= evicted;
+    B->row_touched[dest] = 1;
+    if (evicted) {
+        // a slot this segment writes or reads now belongs to another (dest, chunk): launch the segment first, so
+        // that its writes and reads stay ordered before this request's
+        bool moved = false;
+        for (const auto &u : S.used) moved |= ctx->h_slot_owner[u.first] != (int64_t)u.second;
+        if (moved) { rc = launch_segment(ctx, B->st, S); if (rc) return rc; S.clear(); }
+    }
+    for (size_t k = 0; k < keys.size(); k++) S.used.push_back({slots[k], keys[k]});
+    for (int i = 0; i < nf; i++) {
+        const int32_t s = slots[i];
+        ctx->h_pool_has[s] |= 1;
+        ctx->h_pool_ffid[row + E.fc[i]] = E.fid[i];
+        ctx->h_pool_req[s] = E.fr[i];
+        S.fr.push_back(E.fr[i]); S.fs.push_back(s); S.fw.push_back(S.writes[s]++);
+    }
+    const int l0 = (int)S.lr.size();
+    for (int i = 0; i < nl; i++) {
+        const int32_t s = slots[nf + i];
+        ctx->h_pool_has[s] |= 2;
+        pfnav_los_req q = E.lr[i];
+        int depth = 0;
+        if (q.prev_index >= 0) { q.prev_index += l0; depth = S.ld[q.prev_index] + 1; }
+        else if (q.prev_index == -2) {
+            const size_t pkey = row + q.prev_chunk_r * cw + q.prev_chunk_c;
+            auto it = S.los_at.find(pkey);
+            if (it != S.los_at.end()) { q.prev_index = it->second; depth = S.ld[it->second] + 1; }   // built earlier in this segment
+            else q._pad = ctx->h_pool_slot[pkey];                                                      // absolute pool slot of prev_los
+        }
+        S.los_at[row + E.lc[i]] = (int)S.lr.size();
+        S.lr.push_back(q); S.ls.push_back(s); S.ld.push_back(depth);
+    }
+    if (out_slots) out_slots->assign(slots.begin(), slots.begin() + nf + nl);
+    return PFNAV_OK;
+}
+
+int pf_path_batch_flush(pf_path_batch *B)
+{
+    pfnav_ctx *ctx = B->ctx;
+    cudaStream_t st = B->st;
+    const int chunks = ctx->chunk_w * ctx->chunk_h;
+    int rc = launch_segment(ctx, st, B->S);
+    if (rc) return rc;
+    B->S.clear();
+    if (B->any_evicted)      // entries of other destinations lost their slots
+        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st));
+    else
+        for (int d = 0; d < ctx->pool_ndests; d++)
+            if (B->row_touched[d])
+                PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot + (size_t)d * chunks, ctx->h_pool_slot.data() + (size_t)d * chunks,
+                                        (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
+    bool any_touched = B->any_evicted;
+    for (uint8_t t : B->row_touched) any_touched |= t != 0;
+    if (any_touched)
+        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
+                                cudaMemcpyHostToDevice, st));
+    std::fill(B->row_touched.begin(), B->row_touched.end(), 0);
+    B->any_evicted = false;
+    return PFNAV_OK;
+}
+
 // pfnav_pool_request_paths once its arguments are checked: plan every request, then emit and reserve request by
 // request in order -- what the serial calls would do to the pool mirrors -- and launch the device work per segment.
 static int pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *dests, int layer, const float *src_xz, const float *dst_xz,
                               void *stream, uint32_t *out_dest_ids, int32_t *out_ok, int32_t *out_n_flow, int32_t *out_n_los,
                               int *out_ndone)
 {
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_fields_sync(ctx));
-    PF_CUDA(pf_pool_refresh(ctx, pf_stream(ctx, stream)));
-    pfnav_route_layer &RL = *route_layer(ctx, layer);
-    const int cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
-    // n_update_all_edge_states (nav.c:1787): the map does not change between the requests of a batch
-    for (int ch = 0; ch < chunks; ch++) update_edge_states(ctx, RL, layer, ch);
-    Router R{ctx, RL, layer, cw, ctx->chunk_h};
-    std::vector<path_plan> plans(n);
-    for (int i = 0; i < n; i++) {
-        tdesc s, d;
-        desc_for_point(ctx, src_xz[2 * i], src_xz[2 * i + 1], &s);
-        desc_for_point(ctx, dst_xz[2 * i], dst_xz[2 * i + 1], &d);
-        plan_init(ctx, layer, s, d, plans[i]);
-    }
-    int rc = plan_requests(ctx, R, layer, plans);
+    const std::vector<int32_t> layers(n, layer);
+    pf_path_batch *pb = nullptr;
+    int rc = pf_path_batch_begin(ctx, n, dests, layers.data(), src_xz, dst_xz, pf_stream(ctx, stream), &pb);
     if (rc) return rc;
-    cudaStream_t st = pf_stream(ctx, stream);
-    path_segment S;
-    path_emit E;
-    std::vector<uint64_t> mapped(chunks);
-    std::vector<uint8_t> los_have(chunks);
-    std::vector<uint8_t> row_touched(ctx->pool_ndests, 0);
-    bool any_evicted = false;
+    std::unique_ptr<pf_path_batch, void (*)(pf_path_batch *)> B(pb, pf_path_batch_end);
+    pf_path_probe pr;
     int done = 0;
     for (; done < n; done++) {
-        const path_plan &P = plans[done];
-        const int dest = dests[done];
-        const size_t row = (size_t)dest * chunks;
-        for (int c = 0; c < chunks; c++) {
-            const int s = ctx->h_pool_slot[row + c];
-            los_have[c] = (s >= 0 && (ctx->h_pool_has[s] & 2)) ? 1 : 0;
-        }
-        memcpy(mapped.data(), ctx->h_pool_ffid.data() + row, (size_t)chunks * 8);
-        emit_plan(R, ctx, layer, P, mapped.data(), los_have.data(), E);
-        const int nf = (int)E.fr.size(), nl = (int)E.lr.size();
-        if (out_dest_ids) out_dest_ids[done] = P.dest_id;
-        if (out_ok) out_ok[done] = P.ok;
-        if (out_n_flow) out_n_flow[done] = nf;
-        if (out_n_los) out_n_los[done] = nl;
-        if (nf == 0 && nl == 0) continue;
-        ctx->goal_batch.valid = false;          // the staging buffer is about to be reused
-        // slots for everything this request writes (and the previous-chunk LOS fields it reads), all or nothing
-        std::vector<size_t> keys;
-        for (int i = 0; i < nf; i++) keys.push_back(row + E.fc[i]);
-        for (int i = 0; i < nl; i++) keys.push_back(row + E.lc[i]);
-        for (int i = 0; i < nl; i++)
-            if (E.lr[i].prev_index == -2) keys.push_back(row + E.lr[i].prev_chunk_r * cw + E.lr[i].prev_chunk_c);
-        std::vector<int32_t> slots(keys.size());
-        bool evicted = false;
-        rc = pf_pool_reserve(ctx, keys.data(), keys.size(), slots.data(), &evicted);
-        if (rc) break;
-        any_evicted |= evicted;
-        row_touched[dest] = 1;
-        if (evicted) {
-            // a slot this segment writes or reads now belongs to another (dest, chunk): launch the segment first, so
-            // that its writes and reads stay ordered before this request's
-            bool moved = false;
-            for (const auto &u : S.used) moved |= ctx->h_slot_owner[u.first] != (int64_t)u.second;
-            if (moved) { rc = launch_segment(ctx, st, S); if (rc) return rc; S.clear(); }
-        }
-        for (size_t k = 0; k < keys.size(); k++) S.used.push_back({slots[k], keys[k]});
-        for (int i = 0; i < nf; i++) {
-            const int32_t s = slots[i];
-            ctx->h_pool_has[s] |= 1;
-            ctx->h_pool_ffid[row + E.fc[i]] = E.fid[i];
-            ctx->h_pool_req[s] = E.fr[i];
-            S.fr.push_back(E.fr[i]); S.fs.push_back(s); S.fw.push_back(S.writes[s]++);
-        }
-        const int l0 = (int)S.lr.size();
-        for (int i = 0; i < nl; i++) {
-            const int32_t s = slots[nf + i];
-            ctx->h_pool_has[s] |= 2;
-            pfnav_los_req q = E.lr[i];
-            int depth = 0;
-            if (q.prev_index >= 0) { q.prev_index += l0; depth = S.ld[q.prev_index] + 1; }
-            else if (q.prev_index == -2) {
-                const size_t pkey = row + q.prev_chunk_r * cw + q.prev_chunk_c;
-                auto it = S.los_at.find(pkey);
-                if (it != S.los_at.end()) { q.prev_index = it->second; depth = S.ld[it->second] + 1; }   // built earlier in this segment
-                else q._pad = ctx->h_pool_slot[pkey];                                                      // absolute pool slot of prev_los
-            }
-            S.los_at[row + E.lc[i]] = (int)S.lr.size();
-            S.lr.push_back(q); S.ls.push_back(s); S.ld.push_back(depth);
-        }
+        if ((rc = pf_path_batch_probe(pb, done, &pr))) break;
+        if (out_dest_ids) out_dest_ids[done] = pr.dest_id;
+        if (out_ok) out_ok[done] = pr.ok;
+        if (out_n_flow) out_n_flow[done] = pr.nf;
+        if (out_n_los) out_n_los[done] = pr.nl;
+        if ((rc = pf_path_batch_commit(pb, nullptr))) break;
     }
-    int lrc = launch_segment(ctx, st, S);
+    int lrc = pf_path_batch_flush(pb);
     if (lrc) return lrc;
-    if (any_evicted)      // entries of other destinations lost their slots
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st));
-    else
-        for (int d = 0; d < ctx->pool_ndests; d++)
-            if (row_touched[d])
-                PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot + (size_t)d * chunks, ctx->h_pool_slot.data() + (size_t)d * chunks,
-                                        (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
-    bool any_touched = any_evicted;
-    for (uint8_t t : row_touched) any_touched |= t != 0;
-    if (any_touched)
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
-                                cudaMemcpyHostToDevice, st));
     if (out_ndone) *out_ndone = done;
     return rc;
 }
@@ -1214,6 +1306,19 @@ int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arriv
 //           nearest (Manhattan) to the field's own frontier     (field_closest_tiles_local, field.c:1010)
 // mask: 64 rows of 64 bits.
 // ------------------------------------------------------------------------------------------
+// The argument checks of a kind-0 repair (its seeds are built on the device by pfnav_repair_batch).
+int pfnav_repair_start_check(pfnav_ctx *ctx, const pfnav_field_req &q, int arg)
+{
+    const int chunk = q.chunk_r * ctx->chunk_w + q.chunk_c;
+    const uint8_t *cost = L_cost(ctx, q.layer, chunk);
+    const uint16_t *blk = L_blk(ctx, q.layer, chunk);
+    const int sr = arg >> 8, sc = arg & 0xFF;
+    PF_ARG(sr >= 0 && sr < 64 && sc >= 0 && sc < 64, "repair start tile");
+    PF_ARG(!(cost[sr * 64 + sc] != 0xFF && blk[sr * 64 + sc] == 0),
+           "N_FlowFieldUpdateToNearestPathable needs a non-passable start tile (field.c:1455)");
+    return PFNAV_OK;
+}
+
 int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int arg, uint64_t *mask)
 {
     memset(mask, 0, 64 * sizeof(uint64_t));
@@ -1225,8 +1330,8 @@ int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int a
     static const int dr4[4] = {0, 0, -1, 1}, dc4[4] = {-1, 1, 0, 0};
     if (kind == 0) {
         const int sr = arg >> 8, sc = arg & 0xFF;
-        PF_ARG(sr >= 0 && sr < 64 && sc >= 0 && sc < 64, "repair start tile");
-        PF_ARG(!passable(sr, sc), "N_FlowFieldUpdateToNearestPathable needs a non-passable start tile (field.c:1455)");
+        int rc = pfnav_repair_start_check(ctx, q, arg);
+        if (rc) return rc;
         std::vector<uint8_t> vis(4096, 0);
         std::vector<int> fq; fq.push_back(sr * 64 + sc);
         vis[sr * 64 + sc] = 1;
@@ -1317,6 +1422,19 @@ int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int a
     }
     for (int t : newf) mask[t >> 6] |= 1ull << (t & 63);
     return PFNAV_OK;
+}
+
+// The seeds of a repair of a TARGET_TILE field (pfnav.h), host side; works on host-only contexts.
+extern "C" int pfnav_repair_seed_mask(pfnav_ctx *ctx, int layer, int chunk_r, int chunk_c, int kind, int arg, uint64_t *out_rows)
+{
+    PF_ARG(ctx && out_rows && ctx->chunk_w > 0, "map not created");
+    PF_ARG(layer >= 0 && layer < ctx->nlayers && chunk_r >= 0 && chunk_r < ctx->chunk_h && chunk_c >= 0 && chunk_c < ctx->chunk_w,
+           "layer / chunk");
+    PF_ARG(kind == PFNAV_REPAIR_NEAREST_PATHABLE || kind == PFNAV_REPAIR_ISLAND_TO_NEAREST, "repair kind");
+    pfnav_field_req q;
+    memset(&q, 0, sizeof(q));
+    q.layer = layer; q.chunk_r = chunk_r; q.chunk_c = chunk_c; q.target_type = PFNAV_TARGET_TILE;
+    return pfnav_repair_seeds(ctx, q, kind, arg, out_rows);
 }
 
 // N_RequestPathAttacking (nav.c:3393): the faction carried by the path requests that follow -- packed into the
