@@ -695,6 +695,34 @@ static v2 clearpath(cpent ent, v2 des_v, cpent *dyn, int ndyn, cpent *stat, int 
     return (v2){0.0f, 0.0f};
 }
 
+void pfo_clearpath(const float *self5, const float *vpref2, const float *dyn5, int ndyn, const float *stat5, int nstat,
+                   float max_len, float *out2)
+{
+    cpent self = {{self5[0], self5[1]}, {self5[2], self5[3]}, self5[4]};
+    cpent dyn[MAX_NEIGHBOURS], stat[MAX_NEIGHBOURS];
+    for(int i = 0; i < ndyn; i++) dyn[i] = (cpent){{dyn5[5*i], dyn5[5*i+1]}, {dyn5[5*i+2], dyn5[5*i+3]}, dyn5[5*i+4]};
+    for(int i = 0; i < nstat; i++) stat[i] = (cpent){{stat5[5*i], stat5[5*i+1]}, {stat5[5*i+2], stat5[5*i+3]}, stat5[5*i+4]};
+    v2 nv = v2_truncate(clearpath(self, (v2){vpref2[0], vpref2[1]}, dyn, ndyn, stat, nstat), max_len);
+    out2[0] = nv.x; out2[1] = nv.z;
+}
+
+void pfo_inside_pcr(const float *rays4, int n_rays, const float *pts2, long n, uint8_t *out)
+{
+    line2 rays[4 * MAX_NEIGHBOURS];
+    for(int i = 0; i < n_rays; i++) rays[i] = (line2){{rays4[4*i], rays4[4*i+1]}, {rays4[4*i+2], rays4[4*i+3]}};
+    for(long i = 0; i < n; i++) out[i] = inside_pcr(rays, n_rays, (v2){pts2[2*i], pts2[2*i+1]});
+}
+
+void pfo_line_isect(const float *lines4, long n, float *out3)
+{
+    for(long i = 0; i < n; i++) {
+        const float *l = lines4 + 8 * i;
+        v2 p = {0.0f, 0.0f};
+        bool ok = infinite_line_isect((line2){{l[0], l[1]}, {l[2], l[3]}}, (line2){{l[4], l[5]}, {l[6], l[7]}}, &p);
+        out3[3*i] = ok ? 1.0f : 0.0f; out3[3*i+1] = p.x; out3[3*i+2] = p.z;
+    }
+}
+
 /* ------------------------------------------------------------------------------------------
  * move_velocity_work (game/movement.c:3395) for the point-seek states
  * ---------------------------------------------------------------------------------------- */

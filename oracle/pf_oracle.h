@@ -66,6 +66,14 @@ int  pfo_ents_in_circle(const pfo_world *w, float x, float z, float range, uint3
 /* vdes / has_dest_los are taken from the agent records. out_vel/out_vpref: 2 floats per work item */
 void pfo_velocity_work(const pfo_world *w, const uint32_t *work, size_t nwork, float *out_vel,
                        float *out_vpref);
+/* G_ClearPath_NewVelocity (clearpath.c:694) then vec2_truncate(max_len) (movement.c:3464), as pfo_velocity_work runs it.
+ * self5 / dyn5 / stat5: {px, pz, vx, vz, radius}; ndyn, nstat <= 32 */
+void pfo_clearpath(const float *self5, const float *vpref2, const float *dyn5, int ndyn, const float *stat5, int nstat,
+                   float max_len, float *out2);
+/* inside_pcr (clearpath.c:249) over a ray table rays4 = [n_rays] {px, pz, dx, dz} (left, right per obstacle) */
+void pfo_inside_pcr(const float *rays4, int n_rays, const float *pts2, long n, uint8_t *out);
+/* C_InfiniteLineIntersection (collision.c:820): lines4 = [n][2] {px, pz, dx, dz}; out3 = {ok, x, z} */
+void pfo_line_isect(const float *lines4, long n, float *out3);
 /* N_DesiredPointSeekVelocity + N_HasDestLOS against caller-supplied fields: slot[dest*chunks+chunk]
  * indexes flow/los (4096 B each), -1 = absent (nav.c:3468, 4026, 3407) */
 void pfo_desired_velocity(const pfo_map *map, const pfo_agent *agents, const pfo_flock *flocks,

@@ -52,6 +52,9 @@ def lib():
         L.pfo_group_arrival_velocity.argtypes = [C.POINTER(_Map), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                                  C.c_int, C.c_void_p, C.c_void_p]
         L.pfo_region_field_update_to_nearest_pathable.argtypes = [C.POINTER(_Map)] + [C.c_int] * 5 + [C.c_void_p, C.c_int, C.c_void_p]
+        L.pfo_clearpath.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p]
+        L.pfo_inside_pcr.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_long, C.c_void_p]
+        L.pfo_line_isect.argtypes = [C.c_void_p, C.c_long, C.c_void_p]
         _lib = L
     return _lib
 
@@ -171,6 +174,35 @@ class OracleMap:
         lib().pfo_desired_velocity(C.byref(self.m), _p(agents), _p(flocks), _p(work), len(work), _p(slot),
                                    _p(flow), _p(los), _p(vdes), _p(lo))
         return vdes, lo
+
+
+def clearpath(self5, vpref, dyn, stat, max_len=float("inf")):
+    """G_ClearPath_NewVelocity then vec2_truncate(max_len); self5 / dyn / stat rows: {px, pz, vx, vz, radius}"""
+    self5 = np.ascontiguousarray(self5, np.float32)
+    vpref = np.ascontiguousarray(vpref, np.float32)
+    dyn = np.ascontiguousarray(dyn, np.float32).reshape(-1, 5)
+    stat = np.ascontiguousarray(stat, np.float32).reshape(-1, 5)
+    assert len(dyn) <= 32 and len(stat) <= 32
+    out = np.zeros(2, np.float32)
+    lib().pfo_clearpath(_p(self5), _p(vpref), _p(dyn), len(dyn), _p(stat), len(stat), float(max_len), _p(out))
+    return out
+
+
+def inside_pcr(rays4, pts):
+    """inside_pcr over the ray table rays4 [n_rays][4] {px, pz, dx, dz} for every point of pts [n][2] -> bool [n]"""
+    rays4 = np.ascontiguousarray(rays4, np.float32).reshape(-1, 4)
+    pts = np.ascontiguousarray(pts, np.float32).reshape(-1, 2)
+    out = np.zeros(len(pts), np.uint8)
+    lib().pfo_inside_pcr(_p(rays4), len(rays4), _p(pts), len(pts), _p(out))
+    return out.astype(bool)
+
+
+def line_isect(lines):
+    """C_InfiniteLineIntersection for lines [n][2][4] {px, pz, dx, dz} -> [n][3] {ok, x, z}"""
+    lines = np.ascontiguousarray(lines, np.float32).reshape(-1, 8)
+    out = np.zeros((len(lines), 3), np.float32)
+    lib().pfo_line_isect(_p(lines), len(lines), _p(out))
+    return out
 
 
 def entity_apply(agents, movestate, work, patches):

@@ -55,7 +55,7 @@ def test_los_golden(nav, variant):
     try:
         _los_golden(nav)
     finally:
-        nav.set_los_variant(1)
+        nav.set_los_variant(2)          # the shipped default (k_los_level)
 
 
 def _los_golden(nav):
@@ -903,12 +903,12 @@ def test_los_blocked_destination_tile(nav, pforacle):
             reqs.append(capi.los_req((td[0], td[1]), td))
     assert len(reqs) >= 12
     reqs = np.concatenate(reqs)
-    for variant in (1, 0):
+    for variant in (2, 1, 0):
         nav.set_los_variant(variant)
         try:
             got = nav.los_fields_create(reqs)
         finally:
-            nav.set_los_variant(1)
+            nav.set_los_variant(2)
         exp = om.los_fields_create(reqs)
         bad = np.nonzero((got != exp).reshape(len(reqs), -1).any(axis=1))[0]
         assert len(bad) == 0, (variant, bad[:10])

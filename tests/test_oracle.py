@@ -830,3 +830,17 @@ def test_port_los_blocked_destination_tile_vs_ref(pforacle, pfref):
         assert n >= 12
     finally:
         ref.close()
+
+
+@pytest.mark.parametrize("family", ["random", "forced_retries", "equal_distances", "point_ties", "degenerate_neighbours",
+                                    "early_end", "degenerate_geometry", "overflow"])
+def test_port_clearpath_vs_ref(pfref, pforacle, family):
+    """pfo_clearpath (the port's clearpath() + vec2_truncate) against the reference's G_ClearPath_NewVelocity on the case
+    families the device source is checked with (tests/test_clearpath_emu.py), bit for bit"""
+    import clearpath_cases as cc
+    cs = cc.FAMILIES[family](np.random.default_rng(0xC1EA9), 200)
+    for i in range(len(cs)):
+        s5, vp, dyn, stat, _ = cs.case(i)
+        got = pforacle.clearpath(s5, vp, dyn, stat)
+        want = pfref.clearpath(s5, vp, dyn, stat)
+        assert not np.isnan(got).any() and (got == want).all(), (family, i, got, want)
