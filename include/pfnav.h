@@ -163,7 +163,10 @@ int  pfnav_blockers_get_factions(pfnav_ctx *ctx, int layer, uint8_t *out);
 /* N_Update + N_ApplyDeferredInvalidations (nav.c:2119-2223): for every chunk whose occupancy
  * changed, recompute the local islands, refresh the portal edge states, push the chunk's blockers +
  * islands to the device, and invalidate the pool: entries AT the chunk, and -- when an edge state
- * flipped -- every field of every destination routed THROUGH it (fieldcache.c:460-545). */
+ * flipped -- every field of every destination routed THROUGH it (fieldcache.c:460-545).
+ * The ops pfnav_agents_apply_updates_ex / pfnav_agents_set_blocking left on the device are applied here too, after the
+ * host-queued ones; it reads their count back (and the few whose circle is wider than the device's bit window, which
+ * take the host rasteriser). */
 int  pfnav_map_commit(pfnav_ctx *ctx, int *out_ndirty);
 
 /* ---------------------------------------------------------------------------------------- */
@@ -752,6 +755,45 @@ int  pfnav_agents_read_patches(pfnav_ctx *ctx, pfnav_patch *out, size_t maxout);
  * velocity history, position, interpolation fields, next rotation), then refreshes the neighbour
  * records; follow with pfnav_agents_rebuild_index before the next tick. */
 int  pfnav_agents_apply_updates(pfnav_ctx *ctx, void *stream);
+
+/* Blockers of stopping and starting units on the device (opt-in). entity_apply_update's entity_finish_moving ->
+ * entity_block (movement.c:580, 685) increfs the blockers under a unit that stops; SET_MOVING (:2750-2755) ->
+ * entity_unblock (:560-600) releases them. pfnav_blocking is ms->blocking plus what entity_block recorded, one per entity,
+ * kept on the device. 32 bytes. */
+typedef struct pfnav_blocking {
+    uint32_t blocking;               /* 0 / 1 */
+    int32_t  faction_id;             /* the entity's faction (0..15); used for the ops it takes */
+    float    stop_x, stop_z;         /* where its current block was taken (valid when blocking) */
+    float    stop_radius;            /* the range that block was taken with */
+    uint32_t _pad[3];
+} pfnav_blocking;
+/* HOST array, one record per entity (uid order). Describes blocks the caller has already counted (for example through
+ * pfnav_blockers_* at load): it queues no op. blocking must be 0 or 1, faction_id 0..15. */
+int  pfnav_agents_upload_blocking(pfnav_ctx *ctx, const pfnav_blocking *b, size_t n);
+/* Read the device's blocking table back (waits for the device). */
+int  pfnav_agents_read_blocking(pfnav_ctx *ctx, pfnav_blocking *out, size_t maxout);
+#define PFNAV_APPLY_BLOCKERS (1u << 0)
+/* flags == 0: pfnav_agents_apply_updates. PFNAV_APPLY_BLOCKERS: the same apply, and for every work item, in work order:
+ *   block   - the patch has SET_STATE with next_block != 0, the entity is not GARRISONED and not blocking: incref a circle
+ *             at its snapshot position (the position before this apply, G_Pos_GetXZFrom(gamestate.positions),
+ *             movement.c:583) with range = its radius, its blocking record's faction_id and its flags; the record keeps
+ *             stop_x / stop_z / stop_radius and blocking = 1;
+ *   unblock - the patch has SET_MOVING and the entity is blocking: decref exactly the recorded circle (the entity's
+ *             current flags pick the layers), blocking = 0.
+ * The ops are decided and compacted in work order on the device into a context-owned op buffer that pfnav_map_commit
+ * applies after the ops queued through pfnav_blockers_* (the result equals pfnav_blockers_batch with these ops appended).
+ * Asynchronous on `stream`; it waits for the device only when the op buffer has to grow. Calls that use the blocking
+ * table (this one, pfnav_agents_set_blocking, upload / read) are ordered by the caller, for example on one stream.
+ * Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_ARG for an unknown flag or PFNAV_APPLY_BLOCKERS without
+ * blocking records for the uploaded population; PFNAV_ERR_STATE (nothing changed) on a context in a multi-GPU job
+ * (pfnav_mgpu_init / pfnav_group_create, or an own range that is not the whole population): the map is replicated and
+ * a rank's ops would reach only its own copy. Exchanging ops between ranks is not supported. */
+int  pfnav_agents_apply_updates_ex(pfnav_ctx *ctx, uint32_t flags, void *stream);
+/* The engine's own entity_block (block != 0) / entity_unblock (block == 0) for commands (stop, new move order) for n
+ * uids, with the rules and the op buffer of PFNAV_APPLY_BLOCKERS: blocking at the entity's current position. Repeats
+ * (within a call or across calls) change nothing. Errors as pfnav_agents_apply_updates_ex's, and PFNAV_ERR_ARG for a uid
+ * outside the population. */
+int  pfnav_agents_set_blocking(pfnav_ctx *ctx, const uint32_t *uids, size_t n, int block, void *stream);
 /* Read the (updated) entity snapshot back: agents_out / ms_out may be NULL. */
 int  pfnav_agents_read_state(pfnav_ctx *ctx, pfnav_agent *agents_out, pfnav_movestate *ms_out, size_t maxout);
 

@@ -62,6 +62,10 @@ MOVESTATE_EXT = np.dtype([
     ("target_range", "<f4"), ("target_prev_pos", "<f4", 2), ("_padf", "<f4"), ("target_dir", "<f4", 4), ("rot", "<f4", 4)])
 assert MOVESTATE_EXT.itemsize == 64
 NULL_UID = 0xFFFFFFFF
+BLOCKING = np.dtype([("blocking", "<u4"), ("faction_id", "<i4"), ("stop_x", "<f4"), ("stop_z", "<f4"), ("stop_radius", "<f4"),
+                     ("_pad", "<u4", 3)])
+assert BLOCKING.itemsize == 32
+APPLY_BLOCKERS = 1
 TODO_SURROUND_QUERY, TODO_USE_SURROUND_FIELD, TODO_DROP_SURROUND_FIELD = 1, 2, 4
 
 REGION_REQ = np.dtype([
@@ -113,7 +117,8 @@ SYMBOLS = [
     "pfnav_agents_upload_formation", "pfnav_agents_upload_movestate_ext", "pfnav_pool_request_entity_fields",
     "pfnav_pool_request_entity_fields_batch", "pfnav_pool_request_zones",
     "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
-    "pfnav_profile_read_host", "pfnav_map_query",
+    "pfnav_profile_read_host", "pfnav_map_query", "pfnav_agents_upload_blocking", "pfnav_agents_read_blocking",
+    "pfnav_agents_apply_updates_ex", "pfnav_agents_set_blocking",
 ]
 
 _lib = None
@@ -178,6 +183,10 @@ def load():
     L.pfnav_agents_compute_updates.argtypes = [C.c_void_p, C.c_void_p]
     L.pfnav_agents_read_patches.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_apply_updates.argtypes = [C.c_void_p, C.c_void_p]
+    L.pfnav_agents_apply_updates_ex.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+    L.pfnav_agents_upload_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_agents_read_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_agents_set_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
     L.pfnav_agents_read_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -855,6 +864,26 @@ class Nav:
 
     def agents_apply_updates(self, stream=0):
         _chk(self.L.pfnav_agents_apply_updates(self.h, C.c_void_p(stream)))
+
+    def agents_apply_updates_ex(self, flags=APPLY_BLOCKERS, stream=0):
+        """pfnav_agents_apply_updates_ex: flags = 0 is agents_apply_updates; APPLY_BLOCKERS also takes / releases the
+        blockers of stopping / starting units on the device (applied by the next map_commit)"""
+        _chk(self.L.pfnav_agents_apply_updates_ex(self.h, int(flags), C.c_void_p(stream)))
+
+    def agents_upload_blocking(self, b):
+        """BLOCKING records, one per entity (uid order); describes blocks already counted, queues no op"""
+        b = np.ascontiguousarray(b, BLOCKING)
+        _chk(self.L.pfnav_agents_upload_blocking(self.h, _p(b) if len(b) else None, len(b)))
+
+    def agents_read_blocking(self, n):
+        out = np.zeros(n, BLOCKING)
+        _chk(self.L.pfnav_agents_read_blocking(self.h, _p(out) if n else None, n))
+        return out
+
+    def agents_set_blocking(self, uids, block=True, stream=0):
+        """the engine's entity_block (block=True) / entity_unblock for the listed uids; repeats change nothing"""
+        u = np.ascontiguousarray(uids, np.uint32).reshape(-1)
+        _chk(self.L.pfnav_agents_set_blocking(self.h, _p(u) if len(u) else None, len(u), 1 if block else 0, C.c_void_p(stream)))
 
     def agents_read_state(self, n, movestate=True):
         a = np.zeros(n, AGENT)

@@ -954,6 +954,8 @@ void pfnav_agents_free(pfnav_ctx *ctx)
     if (ctx->update_done) cudaEventDestroy(ctx->update_done);
     cudaFree(ctx->d_los_out); cudaFree(ctx->d_work_count); cudaFree(ctx->d_scan_tmp);
     cudaFree(ctx->d_rep_buf); ctx->d_rep_buf = nullptr; ctx->rep_buf_bytes = 0;
+    cudaFree(ctx->d_blocking); ctx->d_blocking = nullptr; ctx->blocking_n = 0;
+    cudaFree(ctx->d_block_uids); ctx->d_block_uids = nullptr; ctx->cap_block_uids = 0;
     ctx->d_agents = nullptr; ctx->d_records = nullptr; ctx->d_flocks = nullptr; ctx->d_flock_start = nullptr;
     ctx->d_flock_members = nullptr; ctx->d_cohesion = nullptr; ctx->d_cell_count = nullptr; ctx->d_cell_start = nullptr;
     ctx->d_cell_fill = nullptr; ctx->d_sorted_ix = nullptr; ctx->d_sorted_iy = nullptr; ctx->d_sorted_id = nullptr;
@@ -1998,6 +2000,144 @@ __global__ void k_entity_apply(pfnav_agent *__restrict__ agents, pfnav_movestate
     rec[uid] = r;
 }
 
+// entity_block / entity_unblock (movement.c:560-600) per item, staged for pf_blocker_ops_append: ops[2i..2i+1], desc[i],
+// per-block narrow | wide << 32 counts. patches != nullptr: the apply's rules (block on SET_STATE with next_block, unblock
+// on SET_MOVING, in that order); it runs BEFORE k_entity_apply, so a.pos is still the tick's snapshot position.
+// patches == nullptr: pfnav_agents_set_blocking, block (mode 1) or unblock (mode 0) every listed uid.
+__global__ void __launch_bounds__(PF_OPS_BLOCK) k_blocking_decide(const pfnav_agent *__restrict__ agents, pfnav_blocking *__restrict__ blk,
+                                                                  const uint32_t *__restrict__ uids, int n,
+                                                                  const pfnav_patch *__restrict__ patches, int mode, pf_op_stage s)
+{
+    __shared__ unsigned long long part[PF_OPS_BLOCK / 32];
+    const int i = blockIdx.x * PF_OPS_BLOCK + threadIdx.x;
+    unsigned nops = 0, desc = 0;
+    if (i < n) {
+        const uint32_t uid = uids[i];
+        const pfnav_agent a = agents[uid];
+        pfnav_blocking b = blk[uid];
+        bool want_block, want_unblock;
+        if (patches) {
+            const uint32_t pf = patches[i].flags;
+            want_block = (pf & PFNAV_UPDATE_SET_STATE) && patches[i].next_block != 0;
+            want_unblock = (pf & PFNAV_UPDATE_SET_MOVING) != 0;
+        } else {
+            want_block = mode != 0; want_unblock = mode == 0;
+        }
+        if (want_block && !(a.flags & PFNAV_FLAG_GARRISONED) && !b.blocking) {
+            b.blocking = 1; b.stop_x = a.pos[0]; b.stop_z = a.pos[1]; b.stop_radius = a.radius;
+            s.ops[2 * i + nops] = {b.stop_x, b.stop_z, b.stop_radius, b.faction_id, a.flags, +1};
+            desc |= (pf_op_wide(b.stop_radius) ? 4u : 0u) << nops;
+            nops++;
+        }
+        if (want_unblock && b.blocking) {
+            b.blocking = 0;
+            s.ops[2 * i + nops] = {b.stop_x, b.stop_z, b.stop_radius, b.faction_id, a.flags, -1};
+            desc |= (pf_op_wide(b.stop_radius) ? 4u : 0u) << nops;
+            nops++;
+        }
+        if (nops) blk[uid] = b;
+        s.desc[i] = (uint8_t)(desc | nops);
+    }
+    const unsigned nwide = ((desc >> 2) & 1u) + ((desc >> 3) & 1u);
+    unsigned long long v = (unsigned long long)(nops - nwide) | (unsigned long long)nwide << 32;
+    for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xFFFFFFFFu, v, o);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long t = 0;
+        for (int w = 0; w < PF_OPS_BLOCK / 32; w++) t += part[w];
+        s.bsum[blockIdx.x] = t;
+    }
+}
+
+// the checks every entry point of the blocking table makes; need_records: the table must describe this population
+static int blocking_check(pfnav_ctx *ctx, bool need_records)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_agents, "agents not uploaded");
+    if (ctx->mgpu || ctx->shard_lo > 0 || ctx->shard_hi < ctx->n_agents) {
+        pfnav_set_error("device blocking: the context is part of a multi-GPU job (its ops would reach only its own copy of the map)");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(!need_records || (ctx->d_blocking && ctx->blocking_n == ctx->n_agents), "no blocking records uploaded for this population");
+    return PFNAV_OK;
+}
+
+static int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n, const pfnav_patch *d_patches, int mode)
+{
+    pf_op_stage s;
+    int rc = pf_blocker_ops_stage(ctx, (size_t)n, &s);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    k_blocking_decide<<<(n + PF_OPS_BLOCK - 1) / PF_OPS_BLOCK, PF_OPS_BLOCK, 0, st>>>(ctx->d_agents, ctx->d_blocking, d_uids, n,
+                                                                                     d_patches, mode, s);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return pf_blocker_ops_append(ctx, st, (size_t)n, ctx->blocking_any_fac);
+}
+
+extern "C" int pfnav_agents_upload_blocking(pfnav_ctx *ctx, const pfnav_blocking *b, size_t n)
+{
+    int rc = blocking_check(ctx, false);
+    if (rc) return rc;
+    PF_ARG(b || n == 0, "null records");
+    PF_ARG(n == ctx->n_agents, "one blocking record per uploaded agent");
+    bool any_fac = false;
+    for (size_t i = 0; i < n; i++) {
+        PF_ARG(b[i].blocking <= 1, "blocking must be 0 or 1");
+        PF_ARG(b[i].faction_id >= 0 && b[i].faction_id <= 15, "faction_id must lie in 0..15");
+        any_fac |= b[i].faction_id < 15;
+    }
+    PF_CUDA(cudaSetDevice(ctx->device));
+    if (n > ctx->blocking_n || !ctx->d_blocking) {
+        PF_CUDA(cudaDeviceSynchronize());
+        cudaFree(ctx->d_blocking); ctx->d_blocking = nullptr; ctx->blocking_n = 0;
+        PF_CUDA(cudaMalloc(&ctx->d_blocking, std::max<size_t>(n, 1) * sizeof(pfnav_blocking)));
+    }
+    if (n) PF_CUDA(cudaMemcpy(ctx->d_blocking, b, n * sizeof(pfnav_blocking), cudaMemcpyHostToDevice));
+    ctx->blocking_n = n; ctx->blocking_any_fac = any_fac;
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_agents_read_blocking(pfnav_ctx *ctx, pfnav_blocking *out, size_t maxout)
+{
+    int rc = blocking_check(ctx, true);
+    if (rc) return rc;
+    PF_ARG(out || maxout == 0, "out == NULL");
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(cudaDeviceSynchronize());
+    const size_t n = std::min(maxout, ctx->blocking_n);
+    if (n) PF_CUDA(cudaMemcpy(out, ctx->d_blocking, n * sizeof(pfnav_blocking), cudaMemcpyDeviceToHost));
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_agents_set_blocking(pfnav_ctx *ctx, const uint32_t *uids, size_t n, int block, void *stream)
+{
+    int rc = blocking_check(ctx, true);
+    if (rc) return rc;
+    PF_ARG(uids || n == 0, "uids == NULL");
+    // a repeated uid changes nothing after its first occurrence: keep the first, so that one thread owns each entity
+    std::vector<uint32_t> list;
+    list.reserve(n);
+    std::vector<uint8_t> seen(ctx->n_agents, 0);
+    for (size_t i = 0; i < n; i++) {
+        PF_ARG(uids[i] < ctx->n_agents, "uid outside the population");
+        if (!seen[uids[i]]) { seen[uids[i]] = 1; list.push_back(uids[i]); }
+    }
+    if (list.empty()) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    if (list.size() > ctx->cap_block_uids) {
+        PF_CUDA(cudaDeviceSynchronize());
+        cudaFree(ctx->d_block_uids); ctx->d_block_uids = nullptr; ctx->cap_block_uids = 0;
+        PF_CUDA(cudaMalloc(&ctx->d_block_uids, list.size() * 2 * sizeof(uint32_t)));
+        ctx->cap_block_uids = list.size() * 2;
+    }
+    PF_CUDA(cudaMemcpyAsync(ctx->d_block_uids, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    return blocking_emit(ctx, st, ctx->d_block_uids, (int)list.size(), nullptr, block ? 1 : 0);
+}
+
 extern "C" int pfnav_agents_upload_movestate(pfnav_ctx *ctx, const pfnav_movestate *ms, size_t n)
 {
     PF_ARG(ctx && ctx->d_agents && ms, "agents not uploaded / ms == NULL");
@@ -2175,11 +2315,26 @@ extern "C" int pfnav_agents_read_patches(pfnav_ctx *ctx, pfnav_patch *out, size_
 
 extern "C" int pfnav_agents_apply_updates(pfnav_ctx *ctx, void *stream)
 {
-    PF_ARG(ctx && ctx->d_patches && ctx->update_done, "no update pass has run");
+    return pfnav_agents_apply_updates_ex(ctx, 0, stream);
+}
+
+extern "C" int pfnav_agents_apply_updates_ex(pfnav_ctx *ctx, uint32_t flags, void *stream)
+{
+    PF_ARG(ctx, "ctx");
+    if (flags) {
+        PF_ARG((flags & ~PFNAV_APPLY_BLOCKERS) == 0, "unknown apply flag");
+        int rc = blocking_check(ctx, true);
+        if (rc) return rc;
+    }
+    PF_ARG(ctx->d_patches && ctx->update_done, "no update pass has run");
     if (ctx->n_work == 0) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
     const int nwork = (int)ctx->n_work;
+    if (flags & PFNAV_APPLY_BLOCKERS) {     // before the apply: it reads the snapshot positions the apply overwrites
+        int rc = blocking_emit(ctx, st, ctx->d_work, nwork, ctx->d_patches, 0);
+        if (rc) return rc;
+    }
     pf_prof_scope prof(ctx, st, PF_PROF_APPLY);
     k_entity_apply<<<(nwork + 127) / 128, 128, 0, st>>>(ctx->d_agents, ctx->d_movestate, ctx->d_records, ctx->d_work, nwork,
                                                        ctx->d_patches, ctx->d_ms_ext);

@@ -186,7 +186,15 @@ struct blk_state {
     void *d_ops = nullptr; size_t ops_bytes = 0;
     void *d_out = nullptr; size_t out_bytes = 0;
     uint64_t applied_ops = 0;
+    // ops decided on the device (pf_blocker_ops_*): narrow ones for k_blockers_circles, wide ones for the host rasteriser,
+    // d_dev_cnt = {narrow, wide} pending; dev_bound: an upper bound of either count, known without reading them
+    pfnav_blocker_op *d_dev_narrow = nullptr, *d_dev_wide = nullptr; size_t dev_cap = 0, dev_bound = 0;
+    uint32_t *d_dev_cnt = nullptr;
+    bool dev_pending = false, dev_fac = false;
+    // staging of one producer launch: 2 ops + 1 descriptor per item, a count pair and an offset pair per block
+    void *d_stage = nullptr; size_t stage_items = 0;
 };
+static_assert(CIRCLE_MAX_NT == 12, "pf_op_wide (pfnav_internal.cuh) restates the bit window of k_blockers_circles");
 static blk_state *state_of(pfnav_ctx *ctx, bool create)
 {
     if (!ctx->blk_state && create) ctx->blk_state = new blk_state();
@@ -275,6 +283,59 @@ __global__ void k_blockers_tiles(const tile_op *__restrict__ ops, int nops, appl
     if (i >= nops) return;
     const tile_op o = ops[i];
     apply_tile(a, o.layer, o.ar, o.ac, o.faction, o.delta);
+}
+
+// exclusive prefix sum over the CTA of a packed pair of counts (low / high 32 bits); *total = the CTA's sum
+__device__ __forceinline__ unsigned long long cta_excl_scan(unsigned long long v, unsigned long long *warp_tot, unsigned long long *total)
+{
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    unsigned long long incl = v;
+    for (int d = 1; d < 32; d <<= 1) { const unsigned long long t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
+    __syncthreads();                        // warp_tot may still be read by the previous call
+    if (lane == 31) warp_tot[w] = incl;
+    __syncthreads();
+    unsigned long long before = 0, all = 0;
+    for (int k = 0; k < nw; k++) { const unsigned long long t = warp_tot[k]; if (k < w) before += t; all += t; }
+    *total = all;
+    return before + incl - v;
+}
+
+// offsets of the producer blocks behind the ops already pending; advances the pending counts
+__global__ void __launch_bounds__(1024) k_ops_offsets(const unsigned long long *__restrict__ bsum, int nb, uint32_t *cnt,
+                                                      unsigned long long *__restrict__ boff)
+{
+    __shared__ unsigned long long warp_tot[32];
+    const unsigned long long base = (unsigned long long)cnt[0] | (unsigned long long)cnt[1] << 32;
+    unsigned long long carry = 0;
+    for (int b0 = 0; b0 < nb; b0 += 1024) {
+        const int b = b0 + threadIdx.x;
+        const unsigned long long v = b < nb ? bsum[b] : 0ull;
+        unsigned long long tot;
+        const unsigned long long ex = cta_excl_scan(v, warp_tot, &tot);
+        if (b < nb) boff[b] = base + carry + ex;
+        carry += tot;
+    }
+    if (threadIdx.x == 0) { cnt[0] = (uint32_t)(base + carry); cnt[1] = (uint32_t)((base + carry) >> 32); }
+}
+
+// move the staged ops of each item, in item order, to the narrow / wide op buffers
+__global__ void __launch_bounds__(PF_OPS_BLOCK) k_ops_compact(const pfnav_blocker_op *__restrict__ ops, const uint8_t *__restrict__ desc, int n,
+                                                              const unsigned long long *__restrict__ boff,
+                                                              pfnav_blocker_op *__restrict__ narrow, pfnav_blocker_op *__restrict__ wide)
+{
+    __shared__ unsigned long long warp_tot[PF_OPS_BLOCK / 32];
+    const int i = blockIdx.x * PF_OPS_BLOCK + threadIdx.x;
+    const unsigned d = i < n ? desc[i] : 0u, nops = d & 3u;
+    unsigned nwide = 0;
+    for (unsigned k = 0; k < nops; k++) nwide += (d >> (2 + k)) & 1u;
+    unsigned long long tot;
+    const unsigned long long off = boff[blockIdx.x] +
+        cta_excl_scan((unsigned long long)(nops - nwide) | (unsigned long long)nwide << 32, warp_tot, &tot);
+    uint32_t on = (uint32_t)off, ow = (uint32_t)(off >> 32);
+    for (unsigned k = 0; k < nops; k++) {
+        if ((d >> (2 + k)) & 1u) wide[ow++] = ops[2 * (size_t)i + k];
+        else narrow[on++] = ops[2 * (size_t)i + k];
+    }
 }
 
 __device__ __forceinline__ int uf_find(volatile int *L, int x)
@@ -383,6 +444,10 @@ static int ensure_buf(void **p, size_t *cap, size_t bytes)
     return 0;
 }
 
+static size_t stage_blocks(size_t items) { return (items + PF_OPS_BLOCK - 1) / PF_OPS_BLOCK; }
+static size_t stage_desc_off(size_t items) { return items * 2 * sizeof(pfnav_blocker_op); }
+static size_t stage_bsum_off(size_t items) { return (stage_desc_off(items) + items + 7) & ~(size_t)7; }
+
 // d_fac of one layer from the host counts ([chunk][15][4096] -> [15][H64][W64])
 static int fac_push_layer(pfnav_ctx *ctx, blk_state *st, int layer)
 {
@@ -405,17 +470,30 @@ static int fac_push_layer(pfnav_ctx *ctx, blk_state *st, int layer)
     return 0;
 }
 
+static int blockers_circle(pfnav_ctx *ctx, float x, float z, float range, int faction_id, uint32_t flags, int delta);
+
 // Apply the queued operations on the device and bring the touched chunks' mirrors up to date; fills ctx->dirty
 // (passable set changed) and ctx->fdirty (a faction mask changed) for pfnav_map_commit.
 static int device_flush(pfnav_ctx *ctx)
 {
     blk_state *st = state_of(ctx, false);
-    if (!st || ctx->device < 0 || (st->circles.empty() && st->tiles.empty())) return PFNAV_OK;
+    if (!st || ctx->device < 0 || (st->circles.empty() && st->tiles.empty() && !st->dev_pending)) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));         // forked LOS chains still read the map that is about to change
     // ticks / field launches on the context stream or on caller streams (all non-blocking, so not ordered against
     // the default stream used below) may still read the grids
     PF_CUDA(cudaDeviceSynchronize());
+    // ops decided on the device go after the host-queued ones; the counts are additive, so where they are counted does
+    // not change the result. The few wider than the bit window are read back and rasterised on the host.
+    uint32_t dev_cnt[2] = {0, 0};
+    if (st->dev_pending) {
+        PF_CUDA(cudaMemcpy(dev_cnt, st->d_dev_cnt, sizeof(dev_cnt), cudaMemcpyDeviceToHost));
+        if (dev_cnt[1]) {
+            std::vector<pfnav_blocker_op> wide(dev_cnt[1]);
+            PF_CUDA(cudaMemcpy(wide.data(), st->d_dev_wide, wide.size() * sizeof(pfnav_blocker_op), cudaMemcpyDeviceToHost));
+            for (const pfnav_blocker_op &o : wide) blockers_circle(ctx, o.x, o.z, o.range, o.faction_id, o.flags, o.delta);
+        }
+    }
     const int chunks = ctx->chunk_w * ctx->chunk_h, nslots = chunks * ctx->nlayers;
     const size_t ltiles = (size_t)ctx->W64 * ctx->H64;
     if (st->nslots != nslots) {
@@ -428,6 +506,7 @@ static int device_flush(pfnav_ctx *ctx)
     bool need_fac = false;
     for (const auto &o : st->circles) need_fac |= (o.faction_id >= 0 && o.faction_id < 15);
     for (const auto &o : st->tiles) need_fac |= (o.faction >= 0 && o.faction < 15);
+    need_fac |= dev_cnt[0] && st->dev_fac;
     if (need_fac && !st->d_fac) {
         PF_CUDA(cudaMalloc(&st->d_fac, ltiles * 15 * ctx->nlayers));
         for (int l = 0; l < ctx->nlayers; l++) { int rc = fac_push_layer(ctx, st, l); if (rc) return rc; }
@@ -448,7 +527,15 @@ static int device_flush(pfnav_ctx *ctx)
         k_blockers_tiles<<<(unsigned)((ntl + 255) / 256), 256>>>((const tile_op *)st->d_ops, (int)ntl, a);
         ctx->launches++;
     }
-    st->applied_ops += nc + ntl;
+    if (dev_cnt[0]) {
+        k_blockers_circles<<<(dev_cnt[0] + 3) / 4, 128>>>(st->d_dev_narrow, (int)dev_cnt[0], a);
+        ctx->launches++;
+    }
+    if (st->dev_pending) {
+        PF_CUDA(cudaMemset(st->d_dev_cnt, 0, 2 * sizeof(uint32_t)));     // done by the blocking read of the results below
+        st->dev_pending = false; st->dev_fac = false; st->dev_bound = 0;
+    }
+    st->applied_ops += nc + ntl + dev_cnt[0];
     st->circles.clear(); st->tiles.clear();
     finish_args f;
     f.nlayers = ctx->nlayers; f.chunk_w = ctx->chunk_w; f.chunk_h = ctx->chunk_h; f.W64 = ctx->W64; f.H64 = ctx->H64;
@@ -601,6 +688,66 @@ int pfnav_footprint_tiles(const pfnav_ctx *ctx, const pfnav_footprint *e, int ri
     return (int)n;
 }
 
+// Staging for a producer of nitems items (k_blocking_decide) and room for 2 * nitems more pending device ops. Growing
+// waits for the device (the pending ops are copied over); a steady tick reuses the buffers without waiting.
+int pf_blocker_ops_stage(pfnav_ctx *ctx, size_t nitems, pf_op_stage *out)
+{
+    PF_ARG(ctx->d_cost, "map not created");
+    blk_state *st = state_of(ctx, true);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    const size_t need = st->dev_bound + 2 * nitems;
+    if (!st->d_dev_cnt) {
+        PF_CUDA(cudaMalloc(&st->d_dev_cnt, 2 * sizeof(uint32_t)));
+        PF_CUDA(cudaMemset(st->d_dev_cnt, 0, 2 * sizeof(uint32_t)));
+        PF_CUDA(cudaDeviceSynchronize());
+    }
+    if (need > st->dev_cap) {
+        const size_t cap = std::max(need, 2 * st->dev_cap);
+        pfnav_blocker_op *n = nullptr, *w = nullptr;
+        PF_CUDA(cudaDeviceSynchronize());
+        PF_CUDA(cudaMalloc(&n, cap * sizeof(pfnav_blocker_op)));
+        PF_CUDA(cudaMalloc(&w, cap * sizeof(pfnav_blocker_op)));
+        if (st->dev_bound) {
+            PF_CUDA(cudaMemcpy(n, st->d_dev_narrow, st->dev_bound * sizeof(pfnav_blocker_op), cudaMemcpyDeviceToDevice));
+            PF_CUDA(cudaMemcpy(w, st->d_dev_wide, st->dev_bound * sizeof(pfnav_blocker_op), cudaMemcpyDeviceToDevice));
+        }
+        cudaFree(st->d_dev_narrow); cudaFree(st->d_dev_wide);
+        st->d_dev_narrow = n; st->d_dev_wide = w; st->dev_cap = cap;
+    }
+    if (nitems > st->stage_items) {
+        const size_t items = std::max(nitems, 2 * st->stage_items);
+        PF_CUDA(cudaDeviceSynchronize());
+        cudaFree(st->d_stage); st->d_stage = nullptr; st->stage_items = 0;
+        PF_CUDA(cudaMalloc(&st->d_stage, stage_bsum_off(items) + 2 * stage_blocks(items) * sizeof(unsigned long long)));
+        st->stage_items = items;
+    }
+    uint8_t *base = (uint8_t *)st->d_stage;
+    out->ops = (pfnav_blocker_op *)base;
+    out->desc = base + stage_desc_off(st->stage_items);
+    out->bsum = (unsigned long long *)(base + stage_bsum_off(st->stage_items));
+    return PFNAV_OK;
+}
+
+// compact what the producer staged behind the pending device ops, on `st`
+int pf_blocker_ops_append(pfnav_ctx *ctx, cudaStream_t s, size_t nitems, bool any_fac)
+{
+    blk_state *st = state_of(ctx, false);
+    if (!nitems) return PFNAV_OK;
+    uint8_t *base = (uint8_t *)st->d_stage;
+    const size_t nb = stage_blocks(nitems);
+    const unsigned long long *bsum = (const unsigned long long *)(base + stage_bsum_off(st->stage_items));
+    unsigned long long *boff = (unsigned long long *)(base + stage_bsum_off(st->stage_items)) + stage_blocks(st->stage_items);
+    k_ops_offsets<<<1, 1024, 0, s>>>(bsum, (int)nb, st->d_dev_cnt, boff);
+    k_ops_compact<<<(unsigned)nb, PF_OPS_BLOCK, 0, s>>>((const pfnav_blocker_op *)base, base + stage_desc_off(st->stage_items),
+                                                         (int)nitems, boff, st->d_dev_narrow, st->d_dev_wide);
+    ctx->launches += 2;
+    PF_CUDA(cudaGetLastError());
+    st->dev_bound += 2 * nitems;
+    st->dev_pending = true;
+    st->dev_fac |= any_fac;
+    return PFNAV_OK;
+}
+
 // the map is going away (pfnav_map_create / pfnav_destroy): queued operations and the device-side counts with it
 void pfnav_blockers_forget(pfnav_ctx *ctx)
 {
@@ -611,6 +758,7 @@ void pfnav_blockers_forget(pfnav_ctx *ctx)
         cudaSetDevice(ctx->device);
         cudaDeviceSynchronize();
         cudaFree(st->d_fac); cudaFree(st->d_touched); cudaFree(st->d_ops); cudaFree(st->d_out);
+        cudaFree(st->d_dev_narrow); cudaFree(st->d_dev_wide); cudaFree(st->d_dev_cnt); cudaFree(st->d_stage);
     }
     delete st;
     ctx->blk_state = nullptr;

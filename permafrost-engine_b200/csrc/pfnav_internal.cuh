@@ -203,6 +203,10 @@ struct pfnav_ctx {
     // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand
     void *d_rep_buf = nullptr; size_t rep_buf_bytes = 0;
     int repair_stats[6] = {0, 0, 0, 0, 0, 0};                  // the last call: representatives per phase, rounds ended per rule
+    // blocking table of pfnav_agents_upload_blocking (uid order, blocking_n records; 0 = none uploaded) and the uid list
+    // of pfnav_agents_set_blocking
+    pfnav_blocking *d_blocking = nullptr; size_t blocking_n = 0; bool blocking_any_fac = false;
+    uint32_t *d_block_uids = nullptr; size_t cap_block_uids = 0;
 
     // ---- optional per-kernel timing (pfnav_profile_enable) ----
     bool profiling = false;
@@ -312,6 +316,17 @@ void pf_path_batch_end(pf_path_batch *B);
 int pfnav_fmask_push_chunk(pfnav_ctx *ctx, int layer, int chunk);
 int pfnav_blockers_flush(pfnav_ctx *ctx);                        // pfnav_blockers.cu: apply the queued blocker operations now
 int pfnav_blockers_factions_uploaded(pfnav_ctx *ctx, int layer); // pfnav_blockers.cu: host faction counts of a layer were replaced
+// Blocker ops decided on the device (pfnav_blockers.cu). A producer kernel handles `nitems` items in blocks of
+// PF_OPS_BLOCK threads; item i writes its 0..2 ops to ops[2i], ops[2i + 1] and desc[i] = nops | wide(op 0) << 2 | wide(op 1)
+// << 3 (wide: the circle exceeds the bit window of k_blockers_circles, pf_op_wide), and the block's thread 0 writes
+// bsum[block] = its narrow count | wide count << 32. pf_blocker_ops_stage sizes the staging for nitems and the op buffer
+// for 2 * nitems more pending ops; pf_blocker_ops_append compacts the staged ops in item order behind the pending ones
+// (on `st`, no host wait). pfnav_map_commit applies them.
+#define PF_OPS_BLOCK 256
+struct pf_op_stage { pfnav_blocker_op *ops; uint8_t *desc; unsigned long long *bsum; };
+int pf_blocker_ops_stage(pfnav_ctx *ctx, size_t nitems, pf_op_stage *out);
+int pf_blocker_ops_append(pfnav_ctx *ctx, cudaStream_t st, size_t nitems, bool any_fac);
+__host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(range >= 0.0f && (int)ceilf(range / 4) <= 12); }
 
 int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, std::vector<int> &out);     // pfnav_region.cu
 
