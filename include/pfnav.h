@@ -560,7 +560,15 @@ int  pfnav_agents_upload(pfnav_ctx *ctx, const pfnav_agent *agents, size_t n,
  *       pfnav_group_create(ctxs, n, &g); per context pfnav_agents_upload_shard; pfnav_group_gather(g); ticks ...
  *
  * uids stay global (index into the whole population); work lists, movestate uploads, velocity / patch / state
- * read-backs of a context cover its OWN range only. */
+ * read-backs of a context cover its OWN range only.
+ *
+ * A job that shares blockers (pfnav_mgpu_share_blockers / pfnav_group_share_blockers) lets each member take its own
+ * entities' blockers on the device; per tick and member, in this order:
+ *       pfnav_agents_compute_updates -> pfnav_agents_apply_updates_ex(PFNAV_APPLY_BLOCKERS)
+ *       -> pfnav_agents_set_blocking for commands, on the rank that owns the uids
+ *       -> pfnav_mgpu_exchange_blocker_ops (every rank) / pfnav_group_exchange_blocker_ops (once)
+ *       -> pfnav_blockers_* / pfnav_blockers_batch for host ops (buildings, load-time blocks), on every rank
+ *       -> pfnav_map_commit -> pfnav_mgpu_gather / pfnav_group_gather */
 typedef struct pfnav_group pfnav_group;
 #define PFNAV_MGPU_ID_BYTES 128
 int  pfnav_mgpu_shard_range(size_t n_total, int rank, int world, size_t *lo, size_t *hi);
@@ -574,6 +582,36 @@ int  pfnav_mgpu_gather(pfnav_ctx *ctx, void *stream);
 int  pfnav_group_create(pfnav_ctx **ctxs, int world, pfnav_group **out);
 int  pfnav_group_gather(pfnav_group *g);       /* on every member's own context stream */
 void pfnav_group_destroy(pfnav_group *g);
+/* Opt-in: the members of this job take their owned entities' blockers on the device. Call on every rank (NCCL)
+ * or once per group; it only sets state. Afterwards the blocking entry points work on the members, and a member's
+ * device-decided ops must go through an exchange before they are applied:
+ *   - the blocking table of a member covers its own range [shard_lo, shard_hi), like pfnav_agents_upload_movestate,
+ *     pfnav_agents_read_state and pfnav_agents_set_work: pfnav_agents_upload_blocking takes shard_hi - shard_lo
+ *     records, pfnav_agents_read_blocking returns that range, pfnav_agents_set_blocking rejects a uid outside it with
+ *     PFNAV_ERR_ARG (nothing changed), and PFNAV_APPLY_BLOCKERS works on the member's work list (owned uids);
+ *   - no commit before the exchange: while a member holds device-decided ops that were not exchanged, every entry point
+ *     that would apply them (pfnav_map_commit, pfnav_blockers_get, pfnav_blockers_get_factions, field and path
+ *     requests that apply queued ops first) returns PFNAV_ERR_STATE and applies nothing;
+ *   - ops queued on the host (pfnav_blockers_*, pfnav_blockers_batch) are not exchanged: the engine sends them to
+ *     every rank, as without the opt-in.
+ * Without the opt-in nothing changes: the blocking entry points return PFNAV_ERR_STATE on a member of a job.
+ * Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE on a context in no job; PFNAV_ERR_ARG for
+ * pfnav_mgpu_share_blockers on a group member, or group members holding populations of different sizes;
+ * pfnav_group_share_blockers: PFNAV_ERR_STATE when two distinct member devices cannot access each other's memory
+ * (checked up front, so that an exchange never fails halfway). pfnav_group_destroy / pfnav_mgpu_finalize end the
+ * opt-in with the job. */
+int  pfnav_mgpu_share_blockers(pfnav_ctx *ctx);
+int  pfnav_group_share_blockers(pfnav_group *g);
+/* Every member ends up with every member's pending device ops (its own first, then the others' in rank order; ops a
+ * previous exchange already delivered are not sent again). Blocking, like pfnav_map_commit: it waits for each member's
+ * device first. NCCL: a collective that every rank calls (an all-gather of the op counts, one read of them, then a
+ * group of broadcasts on `stream`). Group: peer copies on the members' context streams; before it returns, each
+ * member's stream waits until every peer has finished reading its ops.
+ * Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE when the context is in no job or its job has not
+ * opted in; PFNAV_ERR_ARG for pfnav_mgpu_exchange_blocker_ops on a group member, or group members holding populations
+ * of different sizes. */
+int  pfnav_mgpu_exchange_blocker_ops(pfnav_ctx *ctx, void *stream);
+int  pfnav_group_exchange_blocker_ops(pfnav_group *g);
 /* move_copy_gamestate (movement.c:3607) for this context's own range [lo, hi) of a population of n_total entities;
  * shard[i] is entity lo + i, `flock` fields index the GLOBAL flock table. The snapshot is complete after the next
  * pfnav_mgpu_gather / pfnav_group_gather. On a context outside any multi-GPU job lo = 0, hi = n_total is the whole
@@ -786,13 +824,15 @@ int  pfnav_agents_read_blocking(pfnav_ctx *ctx, pfnav_blocking *out, size_t maxo
  * table (this one, pfnav_agents_set_blocking, upload / read) are ordered by the caller, for example on one stream.
  * Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_ARG for an unknown flag or PFNAV_APPLY_BLOCKERS without
  * blocking records for the uploaded population; PFNAV_ERR_STATE (nothing changed) on a context in a multi-GPU job
- * (pfnav_mgpu_init / pfnav_group_create, or an own range that is not the whole population): the map is replicated and
- * a rank's ops would reach only its own copy. Exchanging ops between ranks is not supported. */
+ * (pfnav_mgpu_init / pfnav_group_create, or an own range that is not the whole population) that does not share
+ * blockers: the map is replicated and a rank's ops would reach only its own copy. A job that shares blockers
+ * (pfnav_mgpu_share_blockers / pfnav_group_share_blockers) exchanges them before the commit; its members' tables
+ * cover their own ranges (see there). On a single context the own range is the whole population. */
 int  pfnav_agents_apply_updates_ex(pfnav_ctx *ctx, uint32_t flags, void *stream);
 /* The engine's own entity_block (block != 0) / entity_unblock (block == 0) for commands (stop, new move order) for n
  * uids, with the rules and the op buffer of PFNAV_APPLY_BLOCKERS: blocking at the entity's current position. Repeats
- * (within a call or across calls) change nothing. Errors as pfnav_agents_apply_updates_ex's, and PFNAV_ERR_ARG for a uid
- * outside the population. */
+ * (within a call or across calls) change nothing. Errors as pfnav_agents_apply_updates_ex's, and PFNAV_ERR_ARG (nothing
+ * changed) for a uid outside the context's own range (the population, on a single context). */
 int  pfnav_agents_set_blocking(pfnav_ctx *ctx, const uint32_t *uids, size_t n, int block, void *stream);
 /* Read the (updated) entity snapshot back: agents_out / ms_out may be NULL. */
 int  pfnav_agents_read_state(pfnav_ctx *ctx, pfnav_agent *agents_out, pfnav_movestate *ms_out, size_t maxout);

@@ -118,7 +118,8 @@ SYMBOLS = [
     "pfnav_pool_request_entity_fields_batch", "pfnav_pool_request_zones",
     "pfnav_set_cohesion_mode", "pfnav_agents_clearpath_stats", "pfnav_route_graph_paths", "pfnav_pool_request_paths",
     "pfnav_profile_read_host", "pfnav_map_query", "pfnav_agents_upload_blocking", "pfnav_agents_read_blocking",
-    "pfnav_agents_apply_updates_ex", "pfnav_agents_set_blocking",
+    "pfnav_agents_apply_updates_ex", "pfnav_agents_set_blocking", "pfnav_mgpu_share_blockers", "pfnav_group_share_blockers",
+    "pfnav_mgpu_exchange_blocker_ops", "pfnav_group_exchange_blocker_ops",
 ]
 
 _lib = None
@@ -247,6 +248,10 @@ def load():
     L.pfnav_group_gather.argtypes = [C.c_void_p]
     L.pfnav_group_destroy.argtypes = [C.c_void_p]
     L.pfnav_group_destroy.restype = None
+    L.pfnav_mgpu_share_blockers.argtypes = [C.c_void_p]
+    L.pfnav_group_share_blockers.argtypes = [C.c_void_p]
+    L.pfnav_mgpu_exchange_blocker_ops.argtypes = [C.c_void_p, C.c_void_p]
+    L.pfnav_group_exchange_blocker_ops.argtypes = [C.c_void_p]
     L.pfnav_agents_tick.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     L.pfnav_agents_read_velocities.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
@@ -786,6 +791,14 @@ class Nav:
     def mgpu_finalize(self):
         _chk(self.L.pfnav_mgpu_finalize(self.h))
 
+    def mgpu_share_blockers(self):
+        """opt in: this rank takes its own entities' blockers on the device; call on every rank"""
+        _chk(self.L.pfnav_mgpu_share_blockers(self.h))
+
+    def mgpu_exchange_blocker_ops(self, stream=0):
+        """collective: every rank ends up with every rank's pending device-decided blocker ops (before map_commit)"""
+        _chk(self.L.pfnav_mgpu_exchange_blocker_ops(self.h, C.c_void_p(stream)))
+
     def agents_set_work(self, uids=None):
         if uids is None:
             _chk(self.L.pfnav_agents_set_work(self.h, None, 0))
@@ -963,6 +976,14 @@ class Group:
 
     def gather(self):
         _chk(load().pfnav_group_gather(self.g))
+
+    def share_blockers(self):
+        """opt in: the members take their own entities' blockers on the device"""
+        _chk(load().pfnav_group_share_blockers(self.g))
+
+    def exchange_blocker_ops(self):
+        """every member ends up with every member's pending device-decided blocker ops (before map_commit)"""
+        _chk(load().pfnav_group_exchange_blocker_ops(self.g))
 
     def close(self):
         if self.g:

@@ -2050,14 +2050,17 @@ __global__ void __launch_bounds__(PF_OPS_BLOCK) k_blocking_decide(const pfnav_ag
     }
 }
 
-// the checks every entry point of the blocking table makes; need_records: the table must describe this population
+// the checks every entry point of the blocking table makes; need_records: the table must describe this population.
+// A member of a multi-GPU job takes part only when the job shares blockers (its ops then reach every member's map
+// through the exchange); its table covers its own range [shard_lo, shard_hi), at the same index as on one context.
 static int blocking_check(pfnav_ctx *ctx, bool need_records)
 {
     PF_ARG(ctx, "ctx");
     PF_NEED_DEVICE(ctx);
     PF_ARG(ctx->d_agents, "agents not uploaded");
-    if (ctx->mgpu || ctx->shard_lo > 0 || ctx->shard_hi < ctx->n_agents) {
-        pfnav_set_error("device blocking: the context is part of a multi-GPU job (its ops would reach only its own copy of the map)");
+    if (!pf_mgpu_shares_blockers(ctx) && (ctx->mgpu || ctx->shard_lo > 0 || ctx->shard_hi < ctx->n_agents)) {
+        pfnav_set_error("device blocking: the context is part of a multi-GPU job that does not share blockers (its ops "
+                        "would reach only its own copy of the map)");
         return PFNAV_ERR_STATE;
     }
     PF_ARG(!need_records || (ctx->d_blocking && ctx->blocking_n == ctx->n_agents), "no blocking records uploaded for this population");
@@ -2082,7 +2085,7 @@ extern "C" int pfnav_agents_upload_blocking(pfnav_ctx *ctx, const pfnav_blocking
     int rc = blocking_check(ctx, false);
     if (rc) return rc;
     PF_ARG(b || n == 0, "null records");
-    PF_ARG(n == ctx->n_agents, "one blocking record per uploaded agent");
+    PF_ARG(n == ctx->shard_hi - ctx->shard_lo, "one blocking record per uploaded agent (of this context's own range)");
     bool any_fac = false;
     for (size_t i = 0; i < n; i++) {
         PF_ARG(b[i].blocking <= 1, "blocking must be 0 or 1");
@@ -2090,13 +2093,14 @@ extern "C" int pfnav_agents_upload_blocking(pfnav_ctx *ctx, const pfnav_blocking
         any_fac |= b[i].faction_id < 15;
     }
     PF_CUDA(cudaSetDevice(ctx->device));
-    if (n > ctx->blocking_n || !ctx->d_blocking) {
+    const size_t all = ctx->n_agents;        // uid-indexed; only the own range is held
+    if (all > ctx->blocking_n || !ctx->d_blocking) {
         PF_CUDA(cudaDeviceSynchronize());
         cudaFree(ctx->d_blocking); ctx->d_blocking = nullptr; ctx->blocking_n = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_blocking, std::max<size_t>(n, 1) * sizeof(pfnav_blocking)));
+        PF_CUDA(cudaMalloc(&ctx->d_blocking, std::max<size_t>(all, 1) * sizeof(pfnav_blocking)));
     }
-    if (n) PF_CUDA(cudaMemcpy(ctx->d_blocking, b, n * sizeof(pfnav_blocking), cudaMemcpyHostToDevice));
-    ctx->blocking_n = n; ctx->blocking_any_fac = any_fac;
+    if (n) PF_CUDA(cudaMemcpy(ctx->d_blocking + ctx->shard_lo, b, n * sizeof(pfnav_blocking), cudaMemcpyHostToDevice));
+    ctx->blocking_n = all; ctx->blocking_any_fac = any_fac;
     return PFNAV_OK;
 }
 
@@ -2107,8 +2111,8 @@ extern "C" int pfnav_agents_read_blocking(pfnav_ctx *ctx, pfnav_blocking *out, s
     PF_ARG(out || maxout == 0, "out == NULL");
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(cudaDeviceSynchronize());
-    const size_t n = std::min(maxout, ctx->blocking_n);
-    if (n) PF_CUDA(cudaMemcpy(out, ctx->d_blocking, n * sizeof(pfnav_blocking), cudaMemcpyDeviceToHost));
+    const size_t n = std::min(maxout, ctx->shard_hi - ctx->shard_lo);       // this context's own entity range
+    if (n) PF_CUDA(cudaMemcpy(out, ctx->d_blocking + ctx->shard_lo, n * sizeof(pfnav_blocking), cudaMemcpyDeviceToHost));
     return PFNAV_OK;
 }
 
@@ -2122,7 +2126,7 @@ extern "C" int pfnav_agents_set_blocking(pfnav_ctx *ctx, const uint32_t *uids, s
     list.reserve(n);
     std::vector<uint8_t> seen(ctx->n_agents, 0);
     for (size_t i = 0; i < n; i++) {
-        PF_ARG(uids[i] < ctx->n_agents, "uid outside the population");
+        PF_ARG(uids[i] >= ctx->shard_lo && uids[i] < ctx->shard_hi, "uid outside this context's own entity range");
         if (!seen[uids[i]]) { seen[uids[i]] = 1; list.push_back(uids[i]); }
     }
     if (list.empty()) return PFNAV_OK;

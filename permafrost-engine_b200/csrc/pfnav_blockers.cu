@@ -191,6 +191,10 @@ struct blk_state {
     pfnav_blocker_op *d_dev_narrow = nullptr, *d_dev_wide = nullptr; size_t dev_cap = 0, dev_bound = 0;
     uint32_t *d_dev_cnt = nullptr;
     bool dev_pending = false, dev_fac = false;
+    // member of a job that shares blockers (pfnav_mgpu_share_blockers): the leading dev_sent = {narrow, wide} pending ops
+    // are held by every member since the last exchange; dev_unexchanged: ops were decided after it
+    uint32_t dev_sent[2] = {0, 0};
+    bool dev_unexchanged = false;
     // staging of one producer launch: 2 ops + 1 descriptor per item, a count pair and an offset pair per block
     void *d_stage = nullptr; size_t stage_items = 0;
 };
@@ -478,6 +482,12 @@ static int device_flush(pfnav_ctx *ctx)
 {
     blk_state *st = state_of(ctx, false);
     if (!st || ctx->device < 0 || (st->circles.empty() && st->tiles.empty() && !st->dev_pending)) return PFNAV_OK;
+    if (st->dev_unexchanged && pf_mgpu_shares_blockers(ctx)) {
+        // the other members would never count these ops: their copies of the map would diverge from this one
+        pfnav_set_error("device blockers: ops decided since the last exchange have not been exchanged "
+                        "(pfnav_mgpu_exchange_blocker_ops / pfnav_group_exchange_blocker_ops)");
+        return PFNAV_ERR_STATE;
+    }
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));         // forked LOS chains still read the map that is about to change
     // ticks / field launches on the context stream or on caller streams (all non-blocking, so not ordered against
@@ -534,6 +544,7 @@ static int device_flush(pfnav_ctx *ctx)
     if (st->dev_pending) {
         PF_CUDA(cudaMemset(st->d_dev_cnt, 0, 2 * sizeof(uint32_t)));     // done by the blocking read of the results below
         st->dev_pending = false; st->dev_fac = false; st->dev_bound = 0;
+        st->dev_sent[0] = st->dev_sent[1] = 0; st->dev_unexchanged = false;
     }
     st->applied_ops += nc + ntl + dev_cnt[0];
     st->circles.clear(); st->tiles.clear();
@@ -690,12 +701,10 @@ int pfnav_footprint_tiles(const pfnav_ctx *ctx, const pfnav_footprint *e, int ri
 
 // Staging for a producer of nitems items (k_blocking_decide) and room for 2 * nitems more pending device ops. Growing
 // waits for the device (the pending ops are copied over); a steady tick reuses the buffers without waiting.
-int pf_blocker_ops_stage(pfnav_ctx *ctx, size_t nitems, pf_op_stage *out)
+// the pending op count pair, and room for `need` pending ops in each op buffer; growing waits for the device and keeps
+// the pending ops
+static int dev_ops_reserve(blk_state *st, size_t need)
 {
-    PF_ARG(ctx->d_cost, "map not created");
-    blk_state *st = state_of(ctx, true);
-    PF_CUDA(cudaSetDevice(ctx->device));
-    const size_t need = st->dev_bound + 2 * nitems;
     if (!st->d_dev_cnt) {
         PF_CUDA(cudaMalloc(&st->d_dev_cnt, 2 * sizeof(uint32_t)));
         PF_CUDA(cudaMemset(st->d_dev_cnt, 0, 2 * sizeof(uint32_t)));
@@ -714,6 +723,15 @@ int pf_blocker_ops_stage(pfnav_ctx *ctx, size_t nitems, pf_op_stage *out)
         cudaFree(st->d_dev_narrow); cudaFree(st->d_dev_wide);
         st->d_dev_narrow = n; st->d_dev_wide = w; st->dev_cap = cap;
     }
+    return 0;
+}
+
+int pf_blocker_ops_stage(pfnav_ctx *ctx, size_t nitems, pf_op_stage *out)
+{
+    PF_ARG(ctx->d_cost, "map not created");
+    blk_state *st = state_of(ctx, true);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    if (dev_ops_reserve(st, st->dev_bound + 2 * nitems)) return PFNAV_ERR_CUDA;
     if (nitems > st->stage_items) {
         const size_t items = std::max(nitems, 2 * st->stage_items);
         PF_CUDA(cudaDeviceSynchronize());
@@ -745,6 +763,48 @@ int pf_blocker_ops_append(pfnav_ctx *ctx, cudaStream_t s, size_t nitems, bool an
     st->dev_bound += 2 * nitems;
     st->dev_pending = true;
     st->dev_fac |= any_fac;
+    st->dev_unexchanged = true;
+    return PFNAV_OK;
+}
+
+static void ops_view_fill(const blk_state *st, pf_ops_view *out)
+{
+    out->narrow = st->d_dev_narrow; out->wide = st->d_dev_wide; out->d_cnt = st->d_dev_cnt;
+    out->sent[0] = st->dev_sent[0]; out->sent[1] = st->dev_sent[1];
+    out->fac = st->dev_fac;
+}
+
+int pf_blocker_ops_view(pfnav_ctx *ctx, pf_ops_view *out)
+{
+    PF_ARG(ctx->d_cost, "map not created");
+    blk_state *st = state_of(ctx, true);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(cudaDeviceSynchronize());        // the ops may have been decided on any stream
+    if (dev_ops_reserve(st, 0)) return PFNAV_ERR_CUDA;
+    ops_view_fill(st, out);
+    return PFNAV_OK;
+}
+
+int pf_blocker_ops_reserve(pfnav_ctx *ctx, size_t need, pf_ops_view *out)
+{
+    blk_state *st = state_of(ctx, false);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    if (dev_ops_reserve(st, need)) return PFNAV_ERR_CUDA;
+    ops_view_fill(st, out);
+    return PFNAV_OK;
+}
+
+int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac)
+{
+    blk_state *st = state_of(ctx, false);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    // synchronous: a producer on any stream that follows appends behind the new counts
+    PF_CUDA(cudaMemcpy(st->d_dev_cnt, cnt, 2 * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    st->dev_bound = std::max(st->dev_bound, (size_t)std::max(cnt[0], cnt[1]));
+    st->dev_pending |= cnt[0] != 0 || cnt[1] != 0;
+    st->dev_fac |= any_fac;
+    st->dev_sent[0] = cnt[0]; st->dev_sent[1] = cnt[1];
+    st->dev_unexchanged = false;
     return PFNAV_OK;
 }
 

@@ -203,8 +203,8 @@ struct pfnav_ctx {
     // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand
     void *d_rep_buf = nullptr; size_t rep_buf_bytes = 0;
     int repair_stats[6] = {0, 0, 0, 0, 0, 0};                  // the last call: representatives per phase, rounds ended per rule
-    // blocking table of pfnav_agents_upload_blocking (uid order, blocking_n records; 0 = none uploaded) and the uid list
-    // of pfnav_agents_set_blocking
+    // blocking table of pfnav_agents_upload_blocking (uid order, blocking_n records, of which the own range
+    // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
     pfnav_blocking *d_blocking = nullptr; size_t blocking_n = 0; bool blocking_any_fac = false;
     uint32_t *d_block_uids = nullptr; size_t cap_block_uids = 0;
 
@@ -326,6 +326,16 @@ int pfnav_blockers_factions_uploaded(pfnav_ctx *ctx, int layer); // pfnav_blocke
 struct pf_op_stage { pfnav_blocker_op *ops; uint8_t *desc; unsigned long long *bsum; };
 int pf_blocker_ops_stage(pfnav_ctx *ctx, size_t nitems, pf_op_stage *out);
 int pf_blocker_ops_append(pfnav_ctx *ctx, cudaStream_t st, size_t nitems, bool any_fac);
+// The exchange of device-decided ops between the members of a job (pfnav_mgpu.cu). pf_blocker_ops_view waits for the
+// device and describes the member's pending ops: the count pair on the device, the leading `sent` ops every member
+// already holds, and whether any op may carry a faction. pf_blocker_ops_reserve makes room for `need` ops in each buffer
+// (keeping the pending ones; the pointers may change). pf_blocker_ops_exchanged: the buffers now hold cnt = {narrow,
+// wide} ops, all of them held by every member.
+struct pf_ops_view { pfnav_blocker_op *narrow, *wide; uint32_t *d_cnt; uint32_t sent[2]; bool fac; };
+int pf_blocker_ops_view(pfnav_ctx *ctx, pf_ops_view *out);
+int pf_blocker_ops_reserve(pfnav_ctx *ctx, size_t need, pf_ops_view *out);
+int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac);
+bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx);             // pfnav_mgpu.cu: member of a job that opted in
 __host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(range >= 0.0f && (int)ceilf(range / 4) <= 12); }
 
 int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, std::vector<int> &out);     // pfnav_region.cu

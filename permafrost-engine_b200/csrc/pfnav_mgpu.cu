@@ -65,7 +65,16 @@ struct pf_mgpu {
     int rank = 0, world = 1;
     pf_nccl_comm comm = nullptr;                 // NCCL transport
     pfnav_group *group = nullptr;                // in-process transport
+    bool share_blockers = false;                 // pfnav_mgpu_share_blockers / pfnav_group_share_blockers
+    uint32_t *d_xcnt = nullptr;                  // NCCL: the exchange's all-gathered count records, PF_XCNT words per rank
 };
+#define PF_XCNT 8                                // {narrow, wide, sent narrow, sent wide, faction flag, 0, 0, 0}
+
+bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx)
+{
+    const pf_mgpu *m = (const pf_mgpu *)ctx->mgpu;
+    return m && m->share_blockers;
+}
 
 #define PF_NCCL(call)                                                                                  \
     do {                                                                                               \
@@ -127,6 +136,7 @@ extern "C" int pfnav_mgpu_finalize(pfnav_ctx *ctx)
     if (!m) return PFNAV_OK;
     PF_ARG(!m->group, "member of an in-process group: pfnav_group_destroy");
     if (ctx->device >= 0) { cudaSetDevice(ctx->device); cudaDeviceSynchronize(); }
+    cudaFree(m->d_xcnt);
     if (m->comm) g_nccl.CommDestroy(m->comm);
     delete m;
     ctx->mgpu = nullptr;
@@ -191,6 +201,85 @@ extern "C" int pfnav_mgpu_gather(pfnav_ctx *ctx, void *stream)
     ctx->members_stale = false;
     if (members) return pfnav_agents_finish_snapshot(ctx, st, true);
     return pfnav_agents_rebuild_index(ctx, st);
+}
+
+// ------------------------------------------------------------------------------------------
+// Shared device blockers. The map is replicated, so the ops a member decides on the device (PFNAV_APPLY_BLOCKERS,
+// pfnav_agents_set_blocking) must reach every member before any of them commits. Blocker counts are additive and a
+// commit's result does not depend on the order of its ops, so every member only needs the union of the members' ops:
+// the exchange appends the peers' new ops (those after their `sent` prefix) behind the member's own, in rank order.
+// ------------------------------------------------------------------------------------------
+static int not_shared(const char *fn)
+{
+    pfnav_set_error("%s: the context is not in a multi-GPU job that shares blockers (pfnav_mgpu_share_blockers / "
+                    "pfnav_group_share_blockers)", fn);
+    return PFNAV_ERR_STATE;
+}
+
+extern "C" int pfnav_mgpu_share_blockers(pfnav_ctx *ctx)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    pf_mgpu *m = (pf_mgpu *)ctx->mgpu;
+    if (!m) {
+        pfnav_set_error("pfnav_mgpu_share_blockers: pfnav_mgpu_init not called");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(!m->group, "member of an in-process group: pfnav_group_share_blockers");
+    m->share_blockers = true;
+    return PFNAV_OK;
+}
+
+// NCCL: all-gather of every rank's count record, one read of them, then a group of broadcasts (the all-gather-v
+// idiom) that puts each rank's new narrow and wide ops behind the receiver's own. Every rank makes the same calls in
+// the same order, from the gathered counts.
+extern "C" int pfnav_mgpu_exchange_blocker_ops(pfnav_ctx *ctx, void *stream)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    pf_mgpu *m = (pf_mgpu *)ctx->mgpu;
+    if (!m) return not_shared(__func__);
+    PF_ARG(!m->group, "member of an in-process group: pfnav_group_exchange_blocker_ops");
+    if (!m->share_blockers) return not_shared(__func__);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    pf_ops_view v;
+    int rc = pf_blocker_ops_view(ctx, &v);
+    if (rc) return rc;
+    const int world = m->world, rank = m->rank;
+    if (!m->d_xcnt) PF_CUDA(cudaMalloc(&m->d_xcnt, (size_t)world * PF_XCNT * sizeof(uint32_t)));
+    uint32_t *mine = m->d_xcnt + (size_t)rank * PF_XCNT;
+    const uint32_t tail[PF_XCNT - 2] = {v.sent[0], v.sent[1], v.fac ? 1u : 0u, 0, 0, 0};
+    PF_CUDA(cudaMemcpyAsync(mine, v.d_cnt, 2 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(mine + 2, tail, sizeof(tail), cudaMemcpyHostToDevice, st));
+    PF_NCCL(g_nccl.AllGather(mine, m->d_xcnt, PF_XCNT * sizeof(uint32_t), /*ncclInt8*/ 0, m->comm, st));
+    std::vector<uint32_t> all((size_t)world * PF_XCNT);
+    PF_CUDA(cudaMemcpyAsync(all.data(), m->d_xcnt, all.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    uint32_t cnt[2] = {all[(size_t)rank * PF_XCNT], all[(size_t)rank * PF_XCNT + 1]};
+    bool fac = false;
+    for (int r = 0; r < world; r++) {
+        const uint32_t *x = &all[(size_t)r * PF_XCNT];
+        fac |= x[4] != 0;
+        if (r != rank) { cnt[0] += x[0] - x[2]; cnt[1] += x[1] - x[3]; }
+    }
+    if ((rc = pf_blocker_ops_reserve(ctx, std::max(cnt[0], cnt[1]), &v))) return rc;
+    pfnav_blocker_op *buf[2] = {v.narrow, v.wide};
+    size_t off[2] = {all[(size_t)rank * PF_XCNT], all[(size_t)rank * PF_XCNT + 1]};
+    PF_NCCL(g_nccl.GroupStart());
+    for (int r = 0; r < world; r++) {
+        const uint32_t *x = &all[(size_t)r * PF_XCNT];
+        for (int k = 0; k < 2; k++) {
+            const size_t seg = x[k] - x[2 + k];
+            if (!seg) continue;
+            pfnav_blocker_op *send = buf[k] + x[2 + k];               // read on the root only
+            pfnav_blocker_op *recv = r == rank ? send : buf[k] + off[k];
+            if (r != rank) off[k] += seg;
+            PF_NCCL(g_nccl.Broadcast(send, recv, seg * sizeof(pfnav_blocker_op), /*ncclInt8*/ 0, r, m->comm, st));
+        }
+    }
+    PF_NCCL(g_nccl.GroupEnd());
+    return pf_blocker_ops_exchanged(ctx, cnt, fac);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -280,6 +369,83 @@ extern "C" int pfnav_group_gather(pfnav_group *g)
         c->members_stale = false;
         rc = members ? pfnav_agents_finish_snapshot(c, c->tick_stream, true) : pfnav_agents_rebuild_index(c, c->tick_stream);
         if (rc) return rc;
+    }
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_group_share_blockers(pfnav_group *g)
+{
+    PF_ARG(g, "group");
+    const int world = (int)g->ctxs.size();
+    for (int i = 0; i < world; i++)
+        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents, "members hold populations of different sizes");
+    // the exchange copies between every pair of member devices: refuse up front rather than fail halfway through one
+    for (int i = 0; i < world; i++)
+        for (int j = 0; j < world; j++) {
+            const int di = g->ctxs[i]->device, dj = g->ctxs[j]->device;
+            if (di == dj) continue;
+            int can = 0;
+            PF_CUDA(cudaDeviceCanAccessPeer(&can, di, dj));
+            if (!can) {
+                pfnav_set_error("pfnav_group_share_blockers: device %d cannot access the memory of device %d", di, dj);
+                return PFNAV_ERR_STATE;
+            }
+        }
+    for (int i = 0; i < world; i++) ((pf_mgpu *)g->ctxs[i]->mgpu)->share_blockers = true;
+    return PFNAV_OK;
+}
+
+// In-process group: every member's counts are read once, its buffers grown, and its stream pulls the peers' new ops
+// behind its own with cudaMemcpyPeerAsync. Every member's stream then waits until every peer has finished pulling, so
+// that nothing a member does next (an emit, a commit's reset, a buffer growth) reaches ops a peer is still copying.
+extern "C" int pfnav_group_exchange_blocker_ops(pfnav_group *g)
+{
+    PF_ARG(g, "group");
+    const int world = (int)g->ctxs.size();
+    if (!((pf_mgpu *)g->ctxs[0]->mgpu)->share_blockers) return not_shared(__func__);
+    int rc;
+    std::vector<pf_ops_view> v(world);
+    std::vector<uint32_t> cnt(2 * (size_t)world), seg(2 * (size_t)world);
+    uint32_t tot[2] = {0, 0};
+    bool fac = false;
+    for (int i = 0; i < world; i++)
+        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents, "members hold populations of different sizes");
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        if ((rc = pf_blocker_ops_view(c, &v[i]))) return rc;        // waits for the member's device
+        PF_CUDA(cudaMemcpy(&cnt[2 * i], v[i].d_cnt, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        for (int k = 0; k < 2; k++) { seg[2 * i + k] = cnt[2 * i + k] - v[i].sent[k]; tot[k] += seg[2 * i + k]; }
+        fac |= v[i].fac;
+    }
+    std::vector<uint32_t> after(2 * (size_t)world);
+    for (int i = 0; i < world; i++) {
+        for (int k = 0; k < 2; k++) after[2 * i + k] = cnt[2 * i + k] + tot[k] - seg[2 * i + k];
+        if ((rc = pf_blocker_ops_reserve(g->ctxs[i], std::max(after[2 * i], after[2 * i + 1]), &v[i]))) return rc;
+    }
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        pfnav_blocker_op *dst[2] = {v[i].narrow, v[i].wide};
+        size_t off[2] = {cnt[2 * i], cnt[2 * i + 1]};
+        for (int p = 0; p < world; p++) {
+            if (p == i) continue;
+            const pfnav_blocker_op *src[2] = {v[p].narrow, v[p].wide};
+            for (int k = 0; k < 2; k++) {
+                const size_t n = seg[2 * p + k];
+                if (!n) continue;
+                PF_CUDA(cudaMemcpyPeerAsync(dst[k] + off[k], c->device, src[k] + v[p].sent[k], g->ctxs[p]->device,
+                                            n * sizeof(pfnav_blocker_op), c->tick_stream));
+                off[k] += n;
+            }
+        }
+        PF_CUDA(cudaEventRecord(g->pulled[i], c->tick_stream));
+    }
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        for (int p = 0; p < world; p++)
+            if (p != i) PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->pulled[p], 0));
+        if ((rc = pf_blocker_ops_exchanged(c, &after[2 * i], fac))) return rc;
     }
     return PFNAV_OK;
 }
