@@ -612,6 +612,42 @@ int  pfnav_group_share_blockers(pfnav_group *g);
  * of different sizes. */
 int  pfnav_mgpu_exchange_blocker_ops(pfnav_ctx *ctx, void *stream);
 int  pfnav_group_exchange_blocker_ops(pfnav_group *g);
+/* pfnav_pool_request_goals_ex for a whole job: the members' flocks may head for the same destinations, and each
+ * (dest, chunk) field is built on ONE member and copied to the members that need it. Every rank calls the NCCL form with
+ * the same arguments; the group form is called once.
+ *   - Equivalence: every member's pool ends exactly as pfnav_pool_request_goals_ex(member, same arguments) would leave
+ *     it: flow and LOS bytes, `has` bits, the (dest, chunk) -> slot mapping and the ff_ids pfnav_pool_get reports, and
+ *     the member's own LRU choices and evictions. Members keep their own pools, slots and eviction histories (their
+ *     ticks read different slots, so their device touch stamps differ). out_n_flow / out_n_los are the member's solo
+ *     counts; the group form takes arrays of `world` entries, member i's at [i] (either may be NULL).
+ *   - Each field is built once: every goal has one owner member, which builds every field of the goal that any member
+ *     lacks (the union of the members' missing (dest, chunk) sets; with flags == 0 the goal's whole plan). Each member
+ *     writes only the fields it lacks. Owners follow from the plan, which every member computes alike from the
+ *     replicated map: the goal with the longest LOS chain first, to the member with the fewest fields so far, ties to
+ *     the lower rank. A field one member keeps equals the one the owner rebuilds for another member: every commit that
+ *     changed the map under it dropped it from every pool alike -- the premise PFNAV_REQUEST_MISSING_ONLY rests on.
+ *     As in the solo call, a destination repeated in one batch must name the same target each time.
+ *   - All or nothing across the job: every member validates the arguments and its state (dest, layer, no device blocker
+ *     ops decided since the last exchange) and dry-runs its reservation before any pool changes. If any member's pool
+ *     cannot hold its fields, EVERY member returns PFNAV_ERR_NOMEM and no pool changes -- unlike the solo call, where
+ *     only the member that does not fit fails. An argument or state error on one rank is returned by every rank.
+ *   - Streams: asynchronous on the device like the solo call, with one host wait: NCCL all-gathers one record per member
+ *     on `stream` and reads it (a group reads its members' host state). The owners' flow waves and LOS chains run on the
+ *     context's field streams and are joined on `stream` before the exchange: NCCL broadcasts the owners' staging
+ *     segments on `stream`; a group member pulls them with peer copies on its context stream, and its stream waits
+ *     until the peers have finished reading its own segment. The copies into the pool follow on the same stream; the
+ *     next pool reader joins them like a solo batch's LOS chains.
+ *   - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE on a context in no job, for the NCCL form on
+ *     a group member, for device blocker ops not yet exchanged, and for a group whose members sit on distinct devices
+ *     without peer access (refused up front); PFNAV_ERR_ARG for bad arguments or members whose maps or pools differ in
+ *     shape; PFNAV_ERR_NOMEM as above. The single-context entry points are unchanged. */
+int  pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
+                                 uint32_t flags, void *stream, int *out_n_flow, int *out_n_los);
+int  pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
+                                  uint32_t flags, int *out_n_flow, int *out_n_los);
+/* TEST HOOK: this member's part in its last job goal batch: the flow / LOS requests it built for the job (*out_n_flow,
+ * *out_n_los) and the owner rank of goals 0 .. max_goals - 1 (-1: no member lacked a field of the goal). */
+int  pfnav_mgpu_fields_stats(pfnav_ctx *ctx, int *out_n_flow, int *out_n_los, int32_t *out_owner, int max_goals);
 /* move_copy_gamestate (movement.c:3607) for this context's own range [lo, hi) of a population of n_total entities;
  * shard[i] is entity lo + i, `flock` fields index the GLOBAL flock table. The snapshot is complete after the next
  * pfnav_mgpu_gather / pfnav_group_gather. On a context outside any multi-GPU job lo = 0, hi = n_total is the whole

@@ -120,6 +120,7 @@ SYMBOLS = [
     "pfnav_profile_read_host", "pfnav_map_query", "pfnav_agents_upload_blocking", "pfnav_agents_read_blocking",
     "pfnav_agents_apply_updates_ex", "pfnav_agents_set_blocking", "pfnav_mgpu_share_blockers", "pfnav_group_share_blockers",
     "pfnav_mgpu_exchange_blocker_ops", "pfnav_group_exchange_blocker_ops",
+    "pfnav_mgpu_request_goals_ex", "pfnav_group_request_goals_ex", "pfnav_mgpu_fields_stats",
 ]
 
 _lib = None
@@ -252,6 +253,11 @@ def load():
     L.pfnav_group_share_blockers.argtypes = [C.c_void_p]
     L.pfnav_mgpu_exchange_blocker_ops.argtypes = [C.c_void_p, C.c_void_p]
     L.pfnav_group_exchange_blocker_ops.argtypes = [C.c_void_p]
+    L.pfnav_mgpu_request_goals_ex.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_uint32, C.c_void_p,
+                                              C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.pfnav_group_request_goals_ex.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_uint32, C.c_void_p,
+                                               C.c_void_p]
+    L.pfnav_mgpu_fields_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p, C.c_int]
     L.pfnav_agents_tick.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     L.pfnav_agents_read_velocities.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
@@ -799,6 +805,22 @@ class Nav:
         """collective: every rank ends up with every rank's pending device-decided blocker ops (before map_commit)"""
         _chk(self.L.pfnav_mgpu_exchange_blocker_ops(self.h, C.c_void_p(stream)))
 
+    def mgpu_request_goals_ex(self, dests, targets, layer=0, flags=0, stream=0):
+        """collective: pool_request_goals for the whole job, each field built on one rank -> this rank's solo (nf, nl)"""
+        dests = np.ascontiguousarray(dests, np.int32)
+        targets = np.ascontiguousarray(targets, np.int32).reshape(-1, 4)
+        nf, nl = C.c_int(0), C.c_int(0)
+        _chk(self.L.pfnav_mgpu_request_goals_ex(self.h, len(dests), _p(dests), layer, _p(targets), flags, C.c_void_p(stream),
+                                                C.byref(nf), C.byref(nl)))
+        return nf.value, nl.value
+
+    def mgpu_fields_stats(self, ngoals):
+        """test hook: this member's last job goal batch -> (flow requests built, LOS requests built, owner per goal)"""
+        nf, nl = C.c_int(0), C.c_int(0)
+        owner = np.zeros(ngoals, np.int32)
+        _chk(self.L.pfnav_mgpu_fields_stats(self.h, C.byref(nf), C.byref(nl), _p(owner), ngoals))
+        return nf.value, nl.value, owner
+
     def agents_set_work(self, uids=None):
         if uids is None:
             _chk(self.L.pfnav_agents_set_work(self.h, None, 0))
@@ -984,6 +1006,14 @@ class Group:
     def exchange_blocker_ops(self):
         """every member ends up with every member's pending device-decided blocker ops (before map_commit)"""
         _chk(load().pfnav_group_exchange_blocker_ops(self.g))
+
+    def request_goals_ex(self, dests, targets, layer=0, flags=0):
+        """pool_request_goals for every member, each field built on one member -> per-member solo counts (nf[], nl[])"""
+        dests = np.ascontiguousarray(dests, np.int32)
+        targets = np.ascontiguousarray(targets, np.int32).reshape(-1, 4)
+        nf, nl = np.zeros(len(self.navs), np.int32), np.zeros(len(self.navs), np.int32)
+        _chk(load().pfnav_group_request_goals_ex(self.g, len(dests), _p(dests), layer, _p(targets), flags, _p(nf), _p(nl)))
+        return nf, nl
 
     def close(self):
         if self.g:

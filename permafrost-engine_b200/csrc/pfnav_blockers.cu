@@ -794,6 +794,12 @@ int pf_blocker_ops_reserve(pfnav_ctx *ctx, size_t need, pf_ops_view *out)
     return PFNAV_OK;
 }
 
+bool pf_blocker_ops_unexchanged(pfnav_ctx *ctx)
+{
+    const blk_state *st = state_of(ctx, false);
+    return st && st->dev_unexchanged;
+}
+
 int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac)
 {
     blk_state *st = state_of(ctx, false);

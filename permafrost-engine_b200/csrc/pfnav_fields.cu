@@ -1289,6 +1289,7 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
     cudaFree(ctx->d_ent_buf);
     if (ctx->ent_ev) cudaEventDestroy(ctx->ent_ev);
     cudaFree(ctx->d_mq_buf);
+    cudaFree(ctx->d_job_stage);
     pfnav_fields_free(ctx);
     pfnav_agents_free(ctx);
     if (ctx->tick_done) cudaEventDestroy(ctx->tick_done);

@@ -207,6 +207,10 @@ struct pfnav_ctx {
     // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
     pfnav_blocking *d_blocking = nullptr; size_t blocking_n = 0; bool blocking_any_fac = false;
     uint32_t *d_block_uids = nullptr; size_t cap_block_uids = 0;
+    // goal batches of a multi-GPU job (pfnav_mgpu_request_goals_ex): the staging buffer of the fields built for the job,
+    // 4096-byte blocks, grown on demand; the last call's owner of every goal and the requests this member built
+    uint8_t *d_job_stage = nullptr; size_t job_stage_bytes = 0;
+    std::vector<int32_t> job_owner; int job_built[2] = {0, 0};
 
     // ---- optional per-kernel timing (pfnav_profile_enable) ----
     bool profiling = false;
@@ -336,6 +340,7 @@ int pf_blocker_ops_view(pfnav_ctx *ctx, pf_ops_view *out);
 int pf_blocker_ops_reserve(pfnav_ctx *ctx, size_t need, pf_ops_view *out);
 int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac);
 bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx);             // pfnav_mgpu.cu: member of a job that opted in
+bool pf_blocker_ops_unexchanged(pfnav_ctx *ctx);                // pfnav_blockers.cu: ops decided since the last exchange
 __host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(range >= 0.0f && (int)ceilf(range / 4) <= 12); }
 
 int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, std::vector<int> &out);     // pfnav_region.cu
@@ -346,6 +351,29 @@ void pf_planner_destroy(pfnav_ctx *ctx);                         // pfnav_plan.c
 // the next of the two pinned staging buffers (plan_host), at least `bytes` long, once the copy that last read it is done;
 // record plan_host_ev[*out_ri] after the copies from it (pfnav_plan.cu)
 int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri);
+
+// One member's part of a goal batch of a multi-GPU job (pfnav_plan.cu; the transports are in pfnav_mgpu.cu).
+//   pf_job_plan   plans the batch on the member's planner threads and describes what pfnav_pool_request_goals_ex would
+//                 write, changing nothing: lack[g * chunks + c] (bit 0 flow, bit 1 LOS: the member lacks that field of
+//                 goal g), the solo counts and whether the member's reservation would succeed. The merged plan stays in
+//                 the member's planner until pf_job_launch.
+//   pf_job_launch takes `uni`, the OR of every member's lack bytes: assigns every goal with a field in `uni` to one
+//                 owner, lays the owners' fields out in the staging buffer (segment of rank r: blocks [seg[r], seg[r+1])),
+//                 reserves the member's slots exactly as the solo call does, uploads its slot table and `has` bytes,
+//                 and builds the fields of the goals `rank` owns into its segment; `st` is joined after the builds.
+//   pf_job_scatter (after the exchange of the segments) copies every field the member lacks from the staging buffer
+//                 into its pool slot, on `st`, and makes the next pool reader wait for it.
+struct pf_job {
+    int ngoals = 0, layer = 0; uint32_t flags = 0;
+    const int32_t *dests = nullptr, *targets = nullptr;
+    bool fits = true; int nf = 0, nl = 0;           // pf_job_plan
+    std::vector<uint8_t> lack;
+    std::vector<size_t> seg;                        // pf_job_launch: world + 1 block offsets
+    const void *d_items = nullptr; int nitems = 0;  // the member's copies from staging into its pool
+};
+int pf_job_plan(pfnav_ctx *ctx, pf_job &J);
+int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int rank, cudaStream_t st);
+int pf_job_scatter(pfnav_ctx *ctx, pf_job &J, cudaStream_t st);
 
 enum { PF_PROF_FLOW = 0, PF_PROF_LOS = 1, PF_PROF_INDEX = 2, PF_PROF_VDES = 3, PF_PROF_COHESION = 4,
        PF_PROF_VELOCITY = 5, PF_PROF_UPDATE = 6, PF_PROF_APPLY = 7, PF_PROF_SLOTS = 8 };

@@ -67,6 +67,7 @@ struct pf_mgpu {
     pfnav_group *group = nullptr;                // in-process transport
     bool share_blockers = false;                 // pfnav_mgpu_share_blockers / pfnav_group_share_blockers
     uint32_t *d_xcnt = nullptr;                  // NCCL: the exchange's all-gathered count records, PF_XCNT words per rank
+    uint8_t *d_xgoal = nullptr; size_t xgoal_bytes = 0;   // NCCL: the goal batch's all-gathered member records
 };
 #define PF_XCNT 8                                // {narrow, wide, sent narrow, sent wide, faction flag, 0, 0, 0}
 
@@ -137,6 +138,7 @@ extern "C" int pfnav_mgpu_finalize(pfnav_ctx *ctx)
     PF_ARG(!m->group, "member of an in-process group: pfnav_group_destroy");
     if (ctx->device >= 0) { cudaSetDevice(ctx->device); cudaDeviceSynchronize(); }
     cudaFree(m->d_xcnt);
+    cudaFree(m->d_xgoal);
     if (m->comm) g_nccl.CommDestroy(m->comm);
     delete m;
     ctx->mgpu = nullptr;
@@ -373,13 +375,10 @@ extern "C" int pfnav_group_gather(pfnav_group *g)
     return PFNAV_OK;
 }
 
-extern "C" int pfnav_group_share_blockers(pfnav_group *g)
+// an exchange copies between every pair of member devices: refuse up front rather than fail halfway through one
+static int peer_check(const pfnav_group *g, const char *fn)
 {
-    PF_ARG(g, "group");
     const int world = (int)g->ctxs.size();
-    for (int i = 0; i < world; i++)
-        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents, "members hold populations of different sizes");
-    // the exchange copies between every pair of member devices: refuse up front rather than fail halfway through one
     for (int i = 0; i < world; i++)
         for (int j = 0; j < world; j++) {
             const int di = g->ctxs[i]->device, dj = g->ctxs[j]->device;
@@ -387,10 +386,20 @@ extern "C" int pfnav_group_share_blockers(pfnav_group *g)
             int can = 0;
             PF_CUDA(cudaDeviceCanAccessPeer(&can, di, dj));
             if (!can) {
-                pfnav_set_error("pfnav_group_share_blockers: device %d cannot access the memory of device %d", di, dj);
+                pfnav_set_error("%s: device %d cannot access the memory of device %d", fn, di, dj);
                 return PFNAV_ERR_STATE;
             }
         }
+    return 0;
+}
+
+extern "C" int pfnav_group_share_blockers(pfnav_group *g)
+{
+    PF_ARG(g, "group");
+    const int world = (int)g->ctxs.size();
+    for (int i = 0; i < world; i++)
+        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents, "members hold populations of different sizes");
+    if (int rc = peer_check(g, __func__)) return rc;
     for (int i = 0; i < world; i++) ((pf_mgpu *)g->ctxs[i]->mgpu)->share_blockers = true;
     return PFNAV_OK;
 }
@@ -446,6 +455,182 @@ extern "C" int pfnav_group_exchange_blocker_ops(pfnav_group *g)
         for (int p = 0; p < world; p++)
             if (p != i) PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->pulled[p], 0));
         if ((rc = pf_blocker_ops_exchanged(c, &after[2 * i], fac))) return rc;
+    }
+    return PFNAV_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Goal batches of a job (pfnav_plan.cu: pf_job_*). Every member plans the whole batch and describes itself in one
+// record -- its verdict on the arguments, whether its pool can hold its fields, the (goal, chunk) fields it lacks --
+// and every member reads every record before anything changes. Then each goal's owner builds the union of the lacked
+// fields into its staging segment, the segments are exchanged (segment r is rank r's), and every member copies the
+// fields it lacks into its own slots. The owners and the segment sizes follow from the plan and the union, which every
+// member computes alike, so no count is exchanged.
+// ------------------------------------------------------------------------------------------
+static void job_init(pf_job &J, int ngoals, const int32_t *dests, int layer, const int32_t *targets, uint32_t flags)
+{
+    J.ngoals = ngoals; J.dests = dests; J.layer = layer; J.targets = targets; J.flags = flags;
+}
+
+// NCCL: one all-gather of the member records on `stream` (and a host wait for it), the owners' builds, a group of
+// broadcasts (one per owner with a non-empty segment) on `stream`, the copies into the pool on `stream`.
+extern "C" int pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
+                                           uint32_t flags, void *stream, int *out_n_flow, int *out_n_los)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    pf_mgpu *m = (pf_mgpu *)ctx->mgpu;
+    if (!m) {
+        pfnav_set_error("pfnav_mgpu_request_goals_ex: pfnav_mgpu_init not called");
+        return PFNAV_ERR_STATE;
+    }
+    if (m->group) {
+        pfnav_set_error("pfnav_mgpu_request_goals_ex: member of an in-process group: pfnav_group_request_goals_ex");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(ctx->d_pool_slot, "pool not created");
+    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
+    if (out_n_flow) *out_n_flow = 0;
+    if (out_n_los) *out_n_los = 0;
+    if (ngoals == 0) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    pf_job J;
+    job_init(J, ngoals, dests, layer, targets, flags);
+    const int local = pf_job_plan(ctx, J);
+    const std::string local_err = local ? pfnav_last_error() : "";
+    // record: {verdict, fits, 0, 0} then one lack byte per (goal, chunk); every rank has the same goal count and map
+    const int world = m->world, rank = m->rank;
+    const size_t nlack = (size_t)ngoals * ctx->chunk_w * ctx->chunk_h, rec = 16 + ((nlack + 15) & ~(size_t)15);
+    if (m->xgoal_bytes < rec * world) {
+        cudaFree(m->d_xgoal);
+        m->d_xgoal = nullptr; m->xgoal_bytes = 0;
+        PF_CUDA(cudaMalloc(&m->d_xgoal, rec * world));
+        m->xgoal_bytes = rec * world;
+    }
+    std::vector<uint8_t> all(rec * world, 0);
+    uint8_t *mine = all.data() + rec * rank;
+    const int32_t hdr[4] = {local, J.fits ? 1 : 0, 0, 0};
+    memcpy(mine, hdr, sizeof(hdr));
+    if (!local) memcpy(mine + 16, J.lack.data(), nlack);
+    PF_CUDA(cudaMemcpyAsync(m->d_xgoal + rec * rank, mine, rec, cudaMemcpyHostToDevice, st));
+    PF_NCCL(g_nccl.AllGather(m->d_xgoal + rec * rank, m->d_xgoal, rec, /*ncclInt8*/ 0, m->comm, st));
+    PF_CUDA(cudaMemcpyAsync(all.data(), m->d_xgoal, all.size(), cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    std::vector<uint8_t> uni(nlack, 0);
+    int refused = -1, refused_rc = 0, full = -1;
+    for (int r = 0; r < world; r++) {
+        int32_t h[4];
+        memcpy(h, all.data() + rec * r, sizeof(h));
+        if (h[0] && refused < 0) { refused = r; refused_rc = h[0]; }
+        if (!h[1] && full < 0) full = r;
+        const uint8_t *l = all.data() + rec * r + 16;
+        for (size_t k = 0; k < nlack; k++) uni[k] |= l[k];
+    }
+    if (local) {
+        pfnav_set_error("%s", local_err.c_str());
+        return local;
+    }
+    if (refused >= 0) {
+        pfnav_set_error("pfnav_mgpu_request_goals_ex: rank %d refused the batch (error %d); no rank changed its pool", refused, refused_rc);
+        return refused_rc;
+    }
+    if (full >= 0) {
+        pfnav_set_error("pfnav_mgpu_request_goals_ex: the field pool of rank %d cannot hold its fields; no rank changed its pool", full);
+        return PFNAV_ERR_NOMEM;
+    }
+    int rc = pf_job_launch(ctx, J, uni.data(), world, rank, st);
+    if (rc) return rc;
+    if (J.seg[world]) {
+        PF_NCCL(g_nccl.GroupStart());
+        for (int r = 0; r < world; r++) {
+            const size_t n = J.seg[r + 1] - J.seg[r];
+            if (!n) continue;
+            uint8_t *p = ctx->d_job_stage + J.seg[r] * 4096;           // sent from the root, received in place elsewhere
+            PF_NCCL(g_nccl.Broadcast(p, p, n * 4096, /*ncclInt8*/ 0, r, m->comm, st));
+        }
+        PF_NCCL(g_nccl.GroupEnd());
+    }
+    if ((rc = pf_job_scatter(ctx, J, st))) return rc;
+    if (out_n_flow) *out_n_flow = J.nf;
+    if (out_n_los) *out_n_los = J.nl;
+    return PFNAV_OK;
+}
+
+// In-process group: the records are read on the host; member i pulls every owner's segment into its staging with
+// cudaMemcpyPeerAsync on its context stream, copies what it lacks into its pool, and then waits until every peer has
+// finished pulling its own segment. out_n_flow / out_n_los: `world` entries, member i's solo counts.
+extern "C" int pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
+                                            uint32_t flags, int *out_n_flow, int *out_n_los)
+{
+    PF_ARG(g, "group");
+    const int world = (int)g->ctxs.size();
+    const pfnav_ctx *c0 = g->ctxs[0];
+    for (int i = 0; i < world; i++) {
+        const pfnav_ctx *c = g->ctxs[i];
+        PF_ARG(c->d_pool_slot, "pool not created");
+        PF_ARG(c->chunk_w == c0->chunk_w && c->chunk_h == c0->chunk_h && c->pool_ndests == c0->pool_ndests,
+               "members hold maps or pools of different shapes");
+    }
+    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
+    int rc = peer_check(g, __func__);
+    if (rc) return rc;
+    for (int i = 0; i < world; i++) {
+        if (out_n_flow) out_n_flow[i] = 0;
+        if (out_n_los) out_n_los[i] = 0;
+    }
+    if (ngoals == 0) return PFNAV_OK;
+    std::vector<pf_job> J(world);
+    for (int i = 0; i < world; i++) {
+        job_init(J[i], ngoals, dests, layer, targets, flags);
+        if ((rc = pf_job_plan(g->ctxs[i], J[i]))) return rc;            // no member has changed anything yet
+    }
+    for (int i = 0; i < world; i++)
+        if (!J[i].fits) {
+            pfnav_set_error("pfnav_group_request_goals_ex: the field pool of member %d cannot hold its fields; no member "
+                            "changed its pool", i);
+            return PFNAV_ERR_NOMEM;
+        }
+    std::vector<uint8_t> uni(J[0].lack.size(), 0);
+    for (int i = 0; i < world; i++)
+        for (size_t k = 0; k < uni.size(); k++) uni[k] |= J[i].lack[k];
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        if ((rc = pf_job_launch(c, J[i], uni.data(), world, i, c->tick_stream))) return rc;
+    }
+    const std::vector<size_t> &seg = J[0].seg;
+    if (seg[world]) {
+        for (int r = 0; r < world; r++) {
+            if (seg[r + 1] == seg[r]) continue;
+            PF_CUDA(cudaSetDevice(g->ctxs[r]->device));
+            PF_CUDA(cudaEventRecord(g->ready[r], g->ctxs[r]->tick_stream));      // owner r's segment is built
+        }
+        for (int i = 0; i < world; i++) {
+            pfnav_ctx *c = g->ctxs[i];
+            PF_CUDA(cudaSetDevice(c->device));
+            for (int p = 0; p < world; p++) {
+                const size_t n = seg[p + 1] - seg[p];
+                if (p == i || !n) continue;
+                const pfnav_ctx *src = g->ctxs[p];
+                PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->ready[p], 0));
+                PF_CUDA(cudaMemcpyPeerAsync(c->d_job_stage + seg[p] * 4096, c->device, src->d_job_stage + seg[p] * 4096,
+                                            src->device, n * 4096, c->tick_stream));
+            }
+            PF_CUDA(cudaEventRecord(g->pulled[i], c->tick_stream));
+        }
+        for (int i = 0; i < world; i++) {
+            pfnav_ctx *c = g->ctxs[i];
+            PF_CUDA(cudaSetDevice(c->device));
+            if ((rc = pf_job_scatter(c, J[i], c->tick_stream))) return rc;
+            // the member's next batch writes its staging: only after every peer has pulled its segment of this one
+            for (int p = 0; p < world; p++)
+                if (p != i) PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->pulled[p], 0));
+        }
+    }
+    for (int i = 0; i < world; i++) {
+        if (out_n_flow) out_n_flow[i] = J[i].nf;
+        if (out_n_los) out_n_los[i] = J[i].nl;
     }
     return PFNAV_OK;
 }

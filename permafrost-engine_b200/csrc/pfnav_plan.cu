@@ -455,58 +455,13 @@ void pf_planner_destroy(pfnav_ctx *ctx)
     ctx->planner = nullptr;
 }
 
-// n_request_path's field-building half, resident on the device, for a batch of goals: plan every
-// goal, then run the flow waves and the LOS dependency waves of ALL goals together straight into the
-// field pool (no host round trip of field bytes; one launch per wave, not per goal).
-// targets: 4 ints per goal {chunk_r, chunk_c, tile_r, tile_c}. Asynchronous on `stream`.
-extern "C" int pfnav_pool_request_goals(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer,
-                                        const int32_t *targets, void *stream, int *out_n_flow, int *out_n_los)
+// Plan every goal of a batch on the planner threads (independent read-only walks over the host mirrors) and merge what
+// the batch writes into the planner's `batch`: every request, or with `missing_only` those whose (dest, chunk) field the
+// pool does not hold. Changes nothing but the planner's scratch.
+static int plan_batch(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer, const int32_t *targets, bool missing_only,
+                      pf_host_timer &ht)
 {
-    return pfnav_pool_request_goals_ex(ctx, ngoals, dests, layer, targets, 0, stream, out_n_flow, out_n_los);
-}
-
-extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer,
-                                           const int32_t *targets, uint32_t flags, void *stream, int *out_n_flow, int *out_n_los)
-{
-    const bool missing_only = (flags & PFNAV_REQUEST_MISSING_ONLY) != 0;
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
-    PF_NEED_DEVICE(ctx);
-    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
-    if (out_n_flow) *out_n_flow = 0;
-    if (out_n_los) *out_n_los = 0;
-    if (ngoals == 0) return PFNAV_OK;
     const int chunks = ctx->chunk_w * ctx->chunk_h;
-    {   // fast path: the same batch on an unchanged map and pool -> the plan is still resident on the device
-        auto &gb = ctx->goal_batch;
-        if (!missing_only && gb.valid && gb.epoch == ctx->map_epoch && gb.layer == layer && (int)gb.dests.size() == ngoals &&
-            memcmp(gb.dests.data(), dests, (size_t)ngoals * 4) == 0 && memcmp(gb.targets.data(), targets, (size_t)ngoals * 16) == 0) {
-            PF_CUDA(cudaSetDevice(ctx->device));
-            cudaStream_t st = pf_stream(ctx, stream);
-            const uint8_t *dev = (const uint8_t *)ctx->d_plan_buf;
-            int rc = los_fork(ctx, st);          // the LOS chains do not read flow fields: fork before the flow waves
-            if (rc) return rc;
-            for (size_t w = 0; w + 1 < gb.fwave_off.size(); w++) {
-                const int first = gb.fwave_off[w], cnt = gb.fwave_off[w + 1] - first;
-                if (cnt <= 0) continue;
-                rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->d_pool_flow,
-                                       (const int32_t *)(dev + gb.b_fr) + first, ctx->flow_stream);
-                if (rc) return rc;
-            }
-            const int32_t one_wave[2] = {0, gb.nl};
-            rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + gb.b_fr + gb.b_fs), gb.nl, ctx->d_pool_los,
-                                  (const int32_t *)(dev + gb.b_fr + gb.b_fs + gb.b_lr), 1, one_wave, ctx->field_stream);
-            if (rc) return rc;
-            rc = los_forked(ctx);
-            if (rc) return rc;
-            if (out_n_flow) *out_n_flow = gb.nf;
-            if (out_n_los) *out_n_los = gb.nl;
-            return PFNAV_OK;
-        }
-        gb.valid = false;
-    }
-    pf_host_timer ht(ctx);
-    for (int g = 0; g < ngoals; g++) PF_ARG(dests[g] >= 0 && dests[g] < ctx->pool_ndests, "dest");
-    // the goals are planned independently of each other (read-only walks over the host mirrors) on the planner threads
     pf_planner &PL = planner_of(ctx);
     const int cap = chunks * 8 + 8;
     if ((int)PL.plans.size() < ngoals) PL.plans.resize(ngoals);
@@ -554,6 +509,96 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
             B.lkeys.push_back((size_t)dests[g] * chunks + lc[i]);
         }
     }
+    B.keys.assign(B.fkeys.begin(), B.fkeys.end());
+    B.keys.insert(B.keys.end(), B.lkeys.begin(), B.lkeys.end());
+    return PFNAV_OK;
+}
+
+// slots for everything a merged batch writes, all or nothing, and their `has` bits and flow requests
+static int reserve_batch(pfnav_ctx *ctx, pf_planner::merged &B)
+{
+    const int nf = (int)B.fr.size(), nl = (int)B.lr.size();
+    B.slots.resize(B.keys.size());
+    int rc = pf_pool_reserve(ctx, B.keys.data(), B.keys.size(), B.slots.data(), nullptr);
+    if (rc) return rc;
+    const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
+    for (int i = 0; i < nf; i++) { ctx->h_pool_has[fs[i]] |= 1; ctx->h_pool_req[fs[i]] = B.fr[i]; }
+    for (int i = 0; i < nl; i++) ctx->h_pool_has[ls[i]] |= 2;
+    return PFNAV_OK;
+}
+
+// pf_pool_reserve's verdict on `keys` without its changes
+static bool pool_fits(const pfnav_ctx *ctx, const std::vector<size_t> &keys)
+{
+    std::vector<size_t> fresh;
+    std::vector<uint8_t> pinned(ctx->pool_max, 0);
+    for (size_t key : keys) {
+        const int s = ctx->h_pool_slot[key];
+        if (s >= 0) pinned[s] = 1;
+        else fresh.push_back(key);
+    }
+    std::sort(fresh.begin(), fresh.end());
+    const size_t nfresh = (size_t)(std::unique(fresh.begin(), fresh.end()) - fresh.begin());
+    const size_t avail = ctx->pool_free.size() + (size_t)(ctx->pool_max - ctx->pool_used);
+    if (nfresh <= avail) return true;
+    size_t cand = 0;
+    for (int s = 0; s < ctx->pool_used; s++) cand += ctx->h_slot_owner[s] >= 0 && !pinned[s];
+    return cand >= nfresh - avail;
+}
+
+// n_request_path's field-building half, resident on the device, for a batch of goals: plan every
+// goal, then run the flow waves and the LOS dependency waves of ALL goals together straight into the
+// field pool (no host round trip of field bytes; one launch per wave, not per goal).
+// targets: 4 ints per goal {chunk_r, chunk_c, tile_r, tile_c}. Asynchronous on `stream`.
+extern "C" int pfnav_pool_request_goals(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer,
+                                        const int32_t *targets, void *stream, int *out_n_flow, int *out_n_los)
+{
+    return pfnav_pool_request_goals_ex(ctx, ngoals, dests, layer, targets, 0, stream, out_n_flow, out_n_los);
+}
+
+extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer,
+                                           const int32_t *targets, uint32_t flags, void *stream, int *out_n_flow, int *out_n_los)
+{
+    const bool missing_only = (flags & PFNAV_REQUEST_MISSING_ONLY) != 0;
+    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
+    if (out_n_flow) *out_n_flow = 0;
+    if (out_n_los) *out_n_los = 0;
+    if (ngoals == 0) return PFNAV_OK;
+    {   // fast path: the same batch on an unchanged map and pool -> the plan is still resident on the device
+        auto &gb = ctx->goal_batch;
+        if (!missing_only && gb.valid && gb.epoch == ctx->map_epoch && gb.layer == layer && (int)gb.dests.size() == ngoals &&
+            memcmp(gb.dests.data(), dests, (size_t)ngoals * 4) == 0 && memcmp(gb.targets.data(), targets, (size_t)ngoals * 16) == 0) {
+            PF_CUDA(cudaSetDevice(ctx->device));
+            cudaStream_t st = pf_stream(ctx, stream);
+            const uint8_t *dev = (const uint8_t *)ctx->d_plan_buf;
+            int rc = los_fork(ctx, st);          // the LOS chains do not read flow fields: fork before the flow waves
+            if (rc) return rc;
+            for (size_t w = 0; w + 1 < gb.fwave_off.size(); w++) {
+                const int first = gb.fwave_off[w], cnt = gb.fwave_off[w + 1] - first;
+                if (cnt <= 0) continue;
+                rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->d_pool_flow,
+                                       (const int32_t *)(dev + gb.b_fr) + first, ctx->flow_stream);
+                if (rc) return rc;
+            }
+            const int32_t one_wave[2] = {0, gb.nl};
+            rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + gb.b_fr + gb.b_fs), gb.nl, ctx->d_pool_los,
+                                  (const int32_t *)(dev + gb.b_fr + gb.b_fs + gb.b_lr), 1, one_wave, ctx->field_stream);
+            if (rc) return rc;
+            rc = los_forked(ctx);
+            if (rc) return rc;
+            if (out_n_flow) *out_n_flow = gb.nf;
+            if (out_n_los) *out_n_los = gb.nl;
+            return PFNAV_OK;
+        }
+        gb.valid = false;
+    }
+    pf_host_timer ht(ctx);
+    for (int g = 0; g < ngoals; g++) PF_ARG(dests[g] >= 0 && dests[g] < ctx->pool_ndests, "dest");
+    int rc = plan_batch(ctx, ngoals, dests, layer, targets, missing_only, ht);
+    if (rc) return rc;
+    pf_planner::merged &B = planner_of(ctx).batch;
     if (B.fr.empty() && B.lr.empty()) return PFNAV_OK;
     const int nf = (int)B.fr.size(), nl = (int)B.lr.size();
     // stable order by wave / depth
@@ -565,17 +610,8 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
     for (int i = 0; i < nl; i++) lwave_off[B.ld[i] + 1]++;
     for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
-    B.keys.assign(B.fkeys.begin(), B.fkeys.end());
-    B.keys.insert(B.keys.end(), B.lkeys.begin(), B.lkeys.end());
     ht.lap(PF_HPROF_MERGE);
-    {   // slots for everything the batch writes, all or nothing (nothing is published before this succeeds)
-        B.slots.resize(B.keys.size());
-        int rc = pf_pool_reserve(ctx, B.keys.data(), B.keys.size(), B.slots.data(), nullptr);
-        if (rc) return rc;
-        const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
-        for (int i = 0; i < nf; i++) { ctx->h_pool_has[fs[i]] |= 1; ctx->h_pool_req[fs[i]] = B.fr[i]; }
-        for (int i = 0; i < nl; i++) ctx->h_pool_has[ls[i]] |= 2;
-    }
+    if ((rc = reserve_batch(ctx, B))) return rc;       // all or nothing: nothing is published before this succeeds
     ht.lap(PF_HPROF_RESERVE);
     const size_t b_fr = (size_t)nf * sizeof(pfnav_field_req), b_fs = (size_t)nf * 4;
     const size_t b_lr = (size_t)nl * sizeof(pfnav_los_req), b_ls = (size_t)nl * 4;
@@ -632,7 +668,7 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     const int32_t *dfs = (const int32_t *)(dev + b_fr);
     const pfnav_los_req *dlr = (const pfnav_los_req *)(dev + b_fr + b_fs);
     const int32_t *dls = (const int32_t *)(dev + b_fr + b_fs + b_lr);
-    int rc = los_fork(ctx, st);
+    rc = los_fork(ctx, st);
     if (rc) return rc;
     for (int w = 0; w <= maxw; w++) {
         const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
@@ -689,5 +725,284 @@ extern "C" int pfnav_fields_join(pfnav_ctx *ctx, void *stream)
     PF_NEED_DEVICE(ctx);
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_join(ctx, pf_stream(ctx, stream)));
+    return PFNAV_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Goal batches of a multi-GPU job (pfnav_mgpu_request_goals_ex / pfnav_group_request_goals_ex; the exchanges are in
+// pfnav_mgpu.cu). The map is replicated, so every member plans the same requests for the same goals; members differ
+// only in which fields their pools still hold. For every goal ONE member, its owner, builds the union of the fields any
+// member lacks into its segment of a staging buffer; the segments are exchanged and every member copies the fields IT
+// lacks into its own slots. Each member reserves exactly the keys its solo call would (the same merged batch, the same
+// pf_pool_reserve), so its slots, evictions and `has` bits are the solo call's. The bytes are the solo call's too: a
+// field is a function of its request and the replicated map, and a field one member keeps equals the one the owner
+// rebuilds for another member, because every commit that changed the map under it dropped it from every pool alike
+// (pfnav_map_commit decides what to drop from the replicated map and the dirty chunks only) -- the premise
+// PFNAV_REQUEST_MISSING_ONLY already rests on.
+// ------------------------------------------------------------------------------------------
+
+// one 4096-byte field per CTA: block it.src of the source buffer of its kind (0 flow, 1 LOS) to block it.dst of the
+// destination buffer of that kind
+struct pf_field_copy { int32_t src, dst, kind; };
+__global__ void __launch_bounds__(256) k_field_copy(const uint8_t *flow_src, const uint8_t *los_src, uint8_t *flow_dst,
+                                                    uint8_t *los_dst, const pf_field_copy *items)
+{
+    const pf_field_copy it = items[blockIdx.x];
+    const uint4 *s = (const uint4 *)((it.kind ? los_src : flow_src) + (size_t)it.src * 4096);
+    uint4 *d = (uint4 *)((it.kind ? los_dst : flow_dst) + (size_t)it.dst * 4096);
+    d[threadIdx.x] = s[threadIdx.x];
+}
+
+static int field_copy_launch(pfnav_ctx *ctx, const uint8_t *flow_src, const uint8_t *los_src, uint8_t *flow_dst,
+                             uint8_t *los_dst, const pf_field_copy *d_items, int n, cudaStream_t st)
+{
+    if (!n) return 0;
+    k_field_copy<<<n, 4096 / sizeof(uint4), 0, st>>>(flow_src, los_src, flow_dst, los_dst, d_items);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int pf_job_plan(pfnav_ctx *ctx, pf_job &J)
+{
+    const int chunks = ctx->chunk_w * ctx->chunk_h;
+    const bool missing_only = (J.flags & PFNAV_REQUEST_MISSING_ONLY) != 0;
+    J.fits = true; J.nf = J.nl = 0;
+    J.lack.assign((size_t)J.ngoals * chunks, 0);
+    for (int g = 0; g < J.ngoals; g++) PF_ARG(J.dests[g] >= 0 && J.dests[g] < ctx->pool_ndests, "dest");
+    PF_ARG(J.layer >= 0 && J.layer < ctx->nlayers, "layer");
+    if (pf_mgpu_shares_blockers(ctx) && pf_blocker_ops_unexchanged(ctx)) {
+        pfnav_set_error("goal batch of a job: device blocker ops decided since the last exchange have not been exchanged "
+                        "(pfnav_mgpu_exchange_blocker_ops / pfnav_group_exchange_blocker_ops)");
+        return PFNAV_ERR_STATE;
+    }
+    if (J.ngoals == 0) return PFNAV_OK;
+    pf_host_timer ht(ctx);
+    int rc = plan_batch(ctx, J.ngoals, J.dests, J.layer, J.targets, missing_only, ht);
+    if (rc) return rc;
+    const pf_planner::merged &B = planner_of(ctx).batch;
+    J.nf = (int)B.fr.size(); J.nl = (int)B.lr.size();
+    J.fits = pool_fits(ctx, B.keys);
+    for (int g = 0; g < J.ngoals; g++)
+        for (int c = 0; c < chunks; c++) {
+            const int sl = missing_only ? ctx->h_pool_slot[(size_t)J.dests[g] * chunks + c] : -1;
+            J.lack[(size_t)g * chunks + c] = (uint8_t)(~(sl >= 0 ? ctx->h_pool_has[sl] : 0) & 3);
+        }
+    return PFNAV_OK;
+}
+
+int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int rank, cudaStream_t st)
+{
+    const int chunks = ctx->chunk_w * ctx->chunk_h, ngoals = J.ngoals;
+    pf_planner &PL = planner_of(ctx);
+    pf_planner::merged &B = PL.batch;               // this member's solo batch, merged by pf_job_plan
+    ctx->job_built[0] = ctx->job_built[1] = 0;
+    J.nitems = 0; J.d_items = nullptr;
+    // ---- owners: the goal with the longest LOS chain among its union fields first, to the member with the fewest union
+    // fields so far, ties to the lower rank (a LOS chain's latency is per chain: this spreads chains, not just fields)
+    std::vector<int> work(ngoals, 0), chain(ngoals, 0), depth, order;
+    for (int g = 0; g < ngoals; g++) {
+        const pf_planner::goal_plan &P = PL.plans[g];
+        const uint8_t *u = uni + (size_t)g * chunks;
+        for (int i = 0; i < P.nf; i++) work[g] += (u[P.fc[i]] & 1) != 0;
+        depth.assign(P.nl, 0);
+        for (int i = 0; i < P.nl; i++) {
+            if (!(u[P.lc[i]] & 2)) continue;
+            const int p = P.lr[i].prev_index;
+            depth[i] = p >= 0 && (u[P.lc[p]] & 2) ? depth[p] + 1 : 0;
+            chain[g] = std::max(chain[g], depth[i] + 1);
+            work[g]++;
+        }
+        if (work[g]) order.push_back(g);
+    }
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return chain[a] > chain[b]; });
+    std::vector<int32_t> &owner = ctx->job_owner;
+    owner.assign(ngoals, -1);
+    std::vector<int64_t> load(world, 0);
+    for (int g : order) {
+        int r = 0;
+        for (int k = 1; k < world; k++) if (load[k] < load[r]) r = k;
+        owner[g] = r;
+        load[r] += work[g];
+    }
+    // ---- staging blocks: owner by owner, goal by goal, a goal's union flow fields (one per chunk) then its LOS fields
+    std::vector<int32_t> fblk((size_t)ngoals * chunks, -1), lblk((size_t)ngoals * chunks, -1);
+    J.seg.assign(world + 1, 0);
+    int32_t next = 0;
+    for (int r = 0; r < world; r++) {
+        J.seg[r] = (size_t)next;
+        for (int g = 0; g < ngoals; g++) {
+            if (owner[g] != r) continue;
+            const pf_planner::goal_plan &P = PL.plans[g];
+            const uint8_t *u = uni + (size_t)g * chunks;
+            int32_t *fb = fblk.data() + (size_t)g * chunks, *lb = lblk.data() + (size_t)g * chunks;
+            for (int i = 0; i < P.nf; i++)
+                if ((u[P.fc[i]] & 1) && fb[P.fc[i]] < 0) fb[P.fc[i]] = next++;
+            for (int i = 0; i < P.nl; i++)
+                if (u[P.lc[i]] & 2) lb[P.lc[i]] = next++;
+        }
+    }
+    J.seg[world] = (size_t)next;
+    if (!next) return PFNAV_OK;                     // every member holds every field: nothing to build or copy
+    // ---- what this member builds: its goals' union fields, into staging. A rebuilt LOS field whose parent is in the
+    // union reads the parent from staging; a parent that every member keeps is copied from this member's pool into a
+    // block behind the segments first, before anything of this batch is written.
+    std::vector<pfnav_field_req> bfr; std::vector<int32_t> bfw, bfs;
+    std::vector<pfnav_los_req> blr; std::vector<int32_t> bld, bls;
+    std::vector<pf_field_copy> parents;
+    std::vector<int> newpos;
+    int32_t extra = next;
+    for (int g = 0; g < ngoals; g++) {
+        if (owner[g] != rank) continue;
+        const pf_planner::goal_plan &P = PL.plans[g];
+        const uint8_t *u = uni + (size_t)g * chunks;
+        const size_t gi = (size_t)g * chunks, row = (size_t)J.dests[g] * chunks;
+        for (int i = 0; i < P.nf; i++)
+            if (u[P.fc[i]] & 1) { bfr.push_back(P.fr[i]); bfw.push_back(P.fw[i]); bfs.push_back(fblk[gi + P.fc[i]]); }
+        newpos.assign(P.nl, -1);
+        for (int i = 0; i < P.nl; i++) {
+            if (!(u[P.lc[i]] & 2)) continue;
+            pfnav_los_req q = P.lr[i];
+            int d = 0;
+            if (q.prev_index >= 0) {
+                const int p = q.prev_index;
+                if (newpos[p] >= 0) { d = bld[newpos[p]] + 1; q.prev_index = newpos[p]; }
+                else {
+                    parents.push_back({ctx->h_pool_slot[row + P.lc[p]], extra, 1});
+                    q.prev_index = -2; q._pad = extra++;
+                }
+            }
+            newpos[i] = (int)blr.size();
+            blr.push_back(q); bld.push_back(d); bls.push_back(lblk[gi + P.lc[i]]);
+        }
+    }
+    // ---- this member's own slots, exactly as its solo call reserves them
+    int rc = 0;
+    if (!B.keys.empty() && (rc = reserve_batch(ctx, B))) return rc;
+    ctx->goal_batch.valid = false;
+    // ---- the fields this member lacks: staging block -> its slot (a flow field once per (goal, chunk))
+    std::vector<pf_field_copy> items;
+    std::vector<uint8_t> seen((size_t)ngoals * chunks, 0);
+    for (int g = 0; g < ngoals; g++) {
+        const pf_planner::goal_plan &P = PL.plans[g];
+        const size_t gi = (size_t)g * chunks, row = (size_t)J.dests[g] * chunks;
+        for (int i = 0; i < P.nf; i++) {
+            const int c = P.fc[i];
+            if (!(J.lack[gi + c] & 1) || seen[gi + c]) continue;
+            seen[gi + c] = 1;
+            items.push_back({fblk[gi + c], ctx->h_pool_slot[row + c], 0});
+        }
+        for (int i = 0; i < P.nl; i++)
+            if (J.lack[gi + P.lc[i]] & 2) items.push_back({lblk[gi + P.lc[i]], ctx->h_pool_slot[row + P.lc[i]], 1});
+    }
+    // ---- pack: builds in wave / depth order, the copies, then the slot table and the `has` bytes
+    const int nf = (int)bfr.size(), nl = (int)blr.size(), np = (int)parents.size(), ni = (int)items.size();
+    int maxw = 0, maxd = 0;
+    for (int i = 0; i < nf; i++) maxw = std::max(maxw, bfw[i]);
+    for (int i = 0; i < nl; i++) maxd = std::max(maxd, bld[i]);
+    std::vector<int32_t> fwave_off(maxw + 2, 0), lwave_off(maxd + 2, 0);
+    for (int i = 0; i < nf; i++) fwave_off[bfw[i] + 1]++;
+    for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
+    for (int i = 0; i < nl; i++) lwave_off[bld[i] + 1]++;
+    for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
+    size_t off = 0;
+    auto sec = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
+    const size_t o_fr = sec((size_t)nf * sizeof(pfnav_field_req)), o_fs = sec((size_t)nf * 4);
+    const size_t o_lr = sec((size_t)nl * sizeof(pfnav_los_req)), o_ls = sec((size_t)nl * 4);
+    const size_t o_pc = sec((size_t)np * sizeof(pf_field_copy)), o_it = sec((size_t)ni * sizeof(pf_field_copy));
+    const size_t total = off, b_slot = ctx->h_pool_slot.size() * 4;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    uint8_t *host = nullptr;
+    int ri = 0;
+    if ((rc = pf_plan_host(ctx, total + b_slot + (size_t)ctx->pool_max, &host, &ri))) return rc;
+    {
+        pfnav_field_req *hfr = (pfnav_field_req *)(host + o_fr);
+        int32_t *hfs = (int32_t *)(host + o_fs), *hls = (int32_t *)(host + o_ls);
+        pfnav_los_req *hlr = (pfnav_los_req *)(host + o_lr);
+        std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1);
+        for (int i = 0; i < nf; i++) { const int k = cur[bfw[i]]++; hfr[k] = bfr[i]; hfs[k] = bfs[i]; }
+        std::vector<int32_t> cur2(lwave_off.begin(), lwave_off.end() - 1), lnew(nl);
+        for (int i = 0; i < nl; i++) lnew[i] = cur2[bld[i]]++;
+        for (int i = 0; i < nl; i++) {
+            pfnav_los_req q = blr[i];
+            if (q.prev_index >= 0) q.prev_index = lnew[q.prev_index];
+            hlr[lnew[i]] = q; hls[lnew[i]] = bls[i];
+        }
+        memcpy(host + o_pc, parents.data(), (size_t)np * sizeof(pf_field_copy));
+        memcpy(host + o_it, items.data(), (size_t)ni * sizeof(pf_field_copy));
+        memcpy(host + total, ctx->h_pool_slot.data(), b_slot);
+        memcpy(host + total + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
+    }
+    // the plan buffer and the staging buffer: the previous batch's kernels and exchange may still read them, so growing
+    // either waits for the device (a group member's stream has waited for its peers' reads of its staging)
+    const size_t need = (size_t)extra * 4096;
+    if (ctx->plan_buf_bytes < total || ctx->job_stage_bytes < need) {
+        PF_CUDA(pf_fields_sync(ctx));
+        PF_CUDA(cudaDeviceSynchronize());
+        if (ctx->plan_buf_bytes < total) {
+            cudaFree(ctx->d_plan_buf);
+            ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
+            PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
+            ctx->plan_buf_bytes = total * 2;
+        }
+        if (ctx->job_stage_bytes < need) {
+            cudaFree(ctx->d_job_stage);
+            ctx->d_job_stage = nullptr; ctx->job_stage_bytes = 0;
+            PF_CUDA(cudaMalloc(&ctx->d_job_stage, need * 2));
+            ctx->job_stage_bytes = need * 2;
+        }
+    }
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    PF_CUDA(pf_fields_join(ctx, st));
+    uint8_t *dev = (uint8_t *)ctx->d_plan_buf, *stage = ctx->d_job_stage;
+    PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + total, b_slot, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + total + b_slot, ctx->pool_max,
+                            cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    if ((rc = field_copy_launch(ctx, nullptr, ctx->d_pool_los, nullptr, stage, (const pf_field_copy *)(dev + o_pc), np, st)))
+        return rc;
+    // the owner's builds: flow waves and LOS chains on the context's field streams, as in the solo call; the exchange
+    // that follows on `st` reads what they wrote
+    if ((rc = los_fork(ctx, st))) return rc;
+    for (int w = 0; w <= maxw; w++) {
+        const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
+        if (cnt <= 0) continue;
+        rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)(dev + o_fr) + first, cnt, stage,
+                               (const int32_t *)(dev + o_fs) + first, ctx->flow_stream);
+        if (rc) return rc;
+    }
+    if (nl && (rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + o_lr), nl, stage, (const int32_t *)(dev + o_ls),
+                                     maxd + 1, lwave_off.data(), ctx->field_stream)))
+        return rc;
+    if ((rc = los_forked(ctx))) return rc;
+    PF_CUDA(pf_fields_join(ctx, st));
+    ctx->job_built[0] = nf; ctx->job_built[1] = nl;
+    J.d_items = dev + o_it; J.nitems = ni;
+    return PFNAV_OK;
+}
+
+int pf_job_scatter(pfnav_ctx *ctx, pf_job &J, cudaStream_t st)
+{
+    if (J.seg.empty() || J.seg.back() == 0) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    int rc = field_copy_launch(ctx, ctx->d_job_stage, ctx->d_job_stage, ctx->d_pool_flow, ctx->d_pool_los,
+                               (const pf_field_copy *)J.d_items, J.nitems, st);
+    if (rc) return rc;
+    // the next pool reader on any stream joins the copies the way it joins a solo batch's forked builds
+    PF_CUDA(cudaEventRecord(ctx->ev_flow, st));
+    PF_CUDA(cudaEventRecord(ctx->ev_los, st));
+    ctx->los_inflight = true;
+    return PFNAV_OK;
+}
+
+// TEST HOOK: the last goal batch of a job on this member -- the flow / LOS requests it built for the job, and the
+// owner of every goal (-1: no member lacked a field of it)
+extern "C" int pfnav_mgpu_fields_stats(pfnav_ctx *ctx, int *out_n_flow, int *out_n_los, int32_t *out_owner, int max_goals)
+{
+    PF_ARG(ctx && max_goals >= 0 && (max_goals == 0 || out_owner), "args");
+    if (out_n_flow) *out_n_flow = ctx->job_built[0];
+    if (out_n_los) *out_n_los = ctx->job_built[1];
+    for (int g = 0; g < max_goals; g++) out_owner[g] = g < (int)ctx->job_owner.size() ? ctx->job_owner[g] : -1;
     return PFNAV_OK;
 }
