@@ -645,8 +645,45 @@ int  pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dest
                                  uint32_t flags, void *stream, int *out_n_flow, int *out_n_los);
 int  pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
                                   uint32_t flags, int *out_n_flow, int *out_n_los);
-/* TEST HOOK: this member's part in its last job goal batch: the flow / LOS requests it built for the job (*out_n_flow,
- * *out_n_los) and the owner rank of goals 0 .. max_goals - 1 (-1: no member lacked a field of the goal). */
+/* pfnav_pool_request_zones for a whole job: a flock arriving as a group needs its zone fields on every member that holds
+ * one of its units, and each (dest, chunk) field is built on ONE member and copied to every member. Every rank calls the
+ * NCCL form with the same arguments; the group form is called once. pfnav_mgpu_request_entity_fields_batch /
+ * pfnav_group_request_entity_fields_batch (below, after pfnav_pool_request_entity_fields_batch) do the same for
+ * enemy-seek and surround fields, with the same contract.
+ *   - Equivalence: every member's pool ends exactly as the solo call with the same arguments would leave it: flow bytes,
+ *     `has` bits, the (dest, chunk) -> slot mapping and the ff_ids pfnav_pool_get reports, and the member's own slot
+ *     choices (pool_used order for zones, which are never evicted; LRU evictions for entity fields). For entity fields
+ *     also the footprints each destination remembers, which pfnav_pool_repair / pfnav_pool_repair_batch start from.
+ *     Members keep their own pools and histories, so their slots may differ. out_nfields (zones) is per request and the
+ *     same on every member; the group form takes one array of m entries.
+ *   - Each field is built once. A field depends on its request and the replicated map only (centre, radius, layer and
+ *     chunk; footprints, kind, layer, ref_layer and chunk), and neither batch skips a field the pool holds: every member
+ *     writes the same keys with the same bytes, the last request naming a key deciding them. Every written key has one
+ *     owner, computed alike on every member from the arguments: each request costs the flood budgets
+ *     (min(pi r^2, dim^2)) of its fields whose window holds the centre (zones) or its field count (entity fields),
+ *     counting only the keys it writes last; the most expensive request goes first, to the member with the least cost
+ *     so far, ties to the lower rank. A request's keys are built by its owner into a staging buffer, and every member
+ *     copies every key it holds at the end into its own slot.
+ *   - All or nothing across the job: every member validates the arguments and its state (pool created, no device
+ *     blocker ops decided since the last exchange) and dry-runs its reservation before any pool changes. If one member
+ *     refuses, every member returns that error; if one member's pool cannot hold the batch, EVERY member returns
+ *     PFNAV_ERR_NOMEM. Either way no pool changes -- unlike the solo calls, which keep the requests before the one that
+ *     did not fit (out_ndone). NCCL all-gathers one {verdict, fits} record per member on `stream` and reads it on the
+ *     host; nothing else is exchanged before the builds.
+ *   - Streams: the owners' builds run on `stream` (NCCL) or the context stream (group), as the solo call's do. NCCL
+ *     broadcasts the owners' staging segments on `stream` (grouped); a group member pulls them with peer copies on its
+ *     context stream, and its stream waits until the peers have finished reading its own segment. The copies into the
+ *     pool follow on the same stream, and the next pool reader joins them like a goal batch's.
+ *   - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE on a context in no job, for the NCCL form on
+ *     a group member, for device blocker ops not yet exchanged, and for a group whose members sit on distinct devices
+ *     without peer access; PFNAV_ERR_ARG for bad arguments or members whose maps or pools differ in shape;
+ *     PFNAV_ERR_NOMEM as above. The single-context entry points are unchanged. */
+int  pfnav_mgpu_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, void *stream, int32_t *out_nfields);
+int  pfnav_group_request_zones(pfnav_group *g, const pfnav_zone_req *reqs, size_t m, int32_t *out_nfields);
+/* TEST HOOK: this member's part in its last job batch of any kind. Goal batches: the flow / LOS requests it built for
+ * the job (*out_n_flow, *out_n_los) and the owner rank of goals 0 .. max_goals - 1 (-1: no member lacked a field of the
+ * goal). Zone and entity-field batches: the fields it built, 0, and the owner rank of requests 0 .. max_goals - 1 (-1:
+ * the request writes no key -- centred off the map, or every key it names is written again by a later request). */
 int  pfnav_mgpu_fields_stats(pfnav_ctx *ctx, int *out_n_flow, int *out_n_los, int32_t *out_owner, int max_goals);
 /* move_copy_gamestate (movement.c:3607) for this context's own range [lo, hi) of a population of n_total entities;
  * shard[i] is entity lo + i, `flock` fields index the GLOBAL flock table. The snapshot is complete after the next
@@ -908,6 +945,16 @@ typedef struct pfnav_entity_field_req {   /* 32 bytes */
 int  pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
                                             const pfnav_footprint *ents, size_t nents,
                                             const int32_t *chunks_rc, size_t nchunks, void *stream, int *out_ndone);
+/* pfnav_pool_request_entity_fields_batch for a whole job: every member with units of a faction seeking enemies needs
+ * that faction's enemy fields. Each (dest, chunk) field is built on one member and copied to every member; the contract
+ * is pfnav_mgpu_request_zones' (equivalence including the remembered footprints, owners, all or nothing with no
+ * out_ndone, streams, errors). Every rank calls the NCCL form with the same arguments; the group form is called once. */
+int  pfnav_mgpu_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                            const pfnav_footprint *ents, size_t nents,
+                                            const int32_t *chunks_rc, size_t nchunks, void *stream);
+int  pfnav_group_request_entity_fields_batch(pfnav_group *g, const pfnav_entity_field_req *reqs, size_t m,
+                                             const pfnav_footprint *ents, size_t nents,
+                                             const int32_t *chunks_rc, size_t nchunks);
 
 /* Test / tuning hook for pfnav_agents_tick: 0 = single-pass velocity kernel; 1 (default) = while LOS chains of
  * pfnav_pool_request_goals are still in flight, run the part of the update that does not depend on the

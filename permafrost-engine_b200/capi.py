@@ -121,6 +121,8 @@ SYMBOLS = [
     "pfnav_agents_apply_updates_ex", "pfnav_agents_set_blocking", "pfnav_mgpu_share_blockers", "pfnav_group_share_blockers",
     "pfnav_mgpu_exchange_blocker_ops", "pfnav_group_exchange_blocker_ops",
     "pfnav_mgpu_request_goals_ex", "pfnav_group_request_goals_ex", "pfnav_mgpu_fields_stats",
+    "pfnav_mgpu_request_zones", "pfnav_group_request_zones", "pfnav_mgpu_request_entity_fields_batch",
+    "pfnav_group_request_entity_fields_batch",
 ]
 
 _lib = None
@@ -258,6 +260,12 @@ def load():
     L.pfnav_group_request_goals_ex.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_uint32, C.c_void_p,
                                                C.c_void_p]
     L.pfnav_mgpu_fields_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p, C.c_int]
+    L.pfnav_mgpu_request_zones.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.pfnav_group_request_zones.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_mgpu_request_entity_fields_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                         C.c_size_t, C.c_void_p]
+    L.pfnav_group_request_entity_fields_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                          C.c_size_t]
     L.pfnav_agents_tick.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     L.pfnav_agents_read_velocities.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
@@ -814,8 +822,28 @@ class Nav:
                                                 C.byref(nf), C.byref(nl)))
         return nf.value, nl.value
 
+    def mgpu_request_zones(self, reqs, stream=0):
+        """collective: pool_request_zones for the whole job, each field built on one rank -> nfields int32[len(reqs)];
+        all or nothing across the ranks"""
+        reqs = np.ascontiguousarray(reqs, ZONE_REQ)
+        nf = np.zeros(len(reqs), np.int32)
+        _chk(self.L.pfnav_mgpu_request_zones(self.h, _p(reqs) if len(reqs) else None, len(reqs), C.c_void_p(stream),
+                                             _p(nf) if len(reqs) else None))
+        return nf
+
+    def mgpu_request_entity_fields_batch(self, reqs, footprints, chunks, stream=0):
+        """collective: pool_request_entity_fields_batch for the whole job, each field built on one rank; all or nothing
+        across the ranks"""
+        reqs = np.ascontiguousarray(reqs, ENTITY_FIELD_REQ)
+        fp = np.ascontiguousarray(footprints, FOOTPRINT)
+        ch = np.ascontiguousarray(chunks, np.int32).reshape(-1, 2)
+        _chk(self.L.pfnav_mgpu_request_entity_fields_batch(self.h, _p(reqs) if len(reqs) else None, len(reqs),
+                                                           _p(fp) if len(fp) else None, len(fp), _p(ch) if len(ch) else None,
+                                                           len(ch), C.c_void_p(stream)))
+
     def mgpu_fields_stats(self, ngoals):
-        """test hook: this member's last job goal batch -> (flow requests built, LOS requests built, owner per goal)"""
+        """test hook: this member's last job batch -> (fields built: flow requests or zone / entity fields, LOS requests
+        built, owner per goal or request)"""
         nf, nl = C.c_int(0), C.c_int(0)
         owner = np.zeros(ngoals, np.int32)
         _chk(self.L.pfnav_mgpu_fields_stats(self.h, C.byref(nf), C.byref(nl), _p(owner), ngoals))
@@ -1014,6 +1042,24 @@ class Group:
         nf, nl = np.zeros(len(self.navs), np.int32), np.zeros(len(self.navs), np.int32)
         _chk(load().pfnav_group_request_goals_ex(self.g, len(dests), _p(dests), layer, _p(targets), flags, _p(nf), _p(nl)))
         return nf, nl
+
+    def request_zones(self, reqs):
+        """pool_request_zones for every member, each field built on one member -> nfields int32[len(reqs)] (the same on
+        every member); all or nothing across the members"""
+        reqs = np.ascontiguousarray(reqs, ZONE_REQ)
+        nf = np.zeros(len(reqs), np.int32)
+        _chk(load().pfnav_group_request_zones(self.g, _p(reqs) if len(reqs) else None, len(reqs), _p(nf) if len(reqs) else None))
+        return nf
+
+    def request_entity_fields_batch(self, reqs, footprints, chunks):
+        """pool_request_entity_fields_batch for every member, each field built on one member; all or nothing across the
+        members"""
+        reqs = np.ascontiguousarray(reqs, ENTITY_FIELD_REQ)
+        fp = np.ascontiguousarray(footprints, FOOTPRINT)
+        ch = np.ascontiguousarray(chunks, np.int32).reshape(-1, 2)
+        _chk(load().pfnav_group_request_entity_fields_batch(self.g, _p(reqs) if len(reqs) else None, len(reqs),
+                                                            _p(fp) if len(fp) else None, len(fp), _p(ch) if len(ch) else None,
+                                                            len(ch)))
 
     def close(self):
         if self.g:

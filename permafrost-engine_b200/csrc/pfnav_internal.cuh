@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <chrono>
+#include <memory>
 #include <set>
 #include <string>
 #include <utility>
@@ -207,8 +208,10 @@ struct pfnav_ctx {
     // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
     pfnav_blocking *d_blocking = nullptr; size_t blocking_n = 0; bool blocking_any_fac = false;
     uint32_t *d_block_uids = nullptr; size_t cap_block_uids = 0;
-    // goal batches of a multi-GPU job (pfnav_mgpu_request_goals_ex): the staging buffer of the fields built for the job,
-    // 4096-byte blocks, grown on demand; the last call's owner of every goal and the requests this member built
+    // goal, zone and entity-field batches of a multi-GPU job (pfnav_mgpu_request_goals_ex, ..._zones,
+    // ..._entity_fields_batch): the staging buffer of the fields built for the job, 4096-byte blocks (a zone or entity
+    // batch keeps its copy list behind them), grown on demand; the last call's owner of every goal or request and the
+    // requests this member built
     uint8_t *d_job_stage = nullptr; size_t job_stage_bytes = 0;
     std::vector<int32_t> job_owner; int job_built[2] = {0, 0};
 
@@ -363,9 +366,20 @@ int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri);
 //                 and builds the fields of the goals `rank` owns into its segment; `st` is joined after the builds.
 //   pf_job_scatter (after the exchange of the segments) copies every field the member lacks from the staging buffer
 //                 into its pool slot, on `st`, and makes the next pool reader wait for it.
+// Zone and entity-field batches (kind PF_JOB_ZONES / PF_JOB_ENTITY) take the same three steps: pf_job_plan validates
+// and dry-runs the member's reservation (pf_aux_job_plan, pfnav_region.cu; no lack record: every member writes every key
+// the arguments name), pf_job_launch reserves, lays out the owners' fields (pf_job_layout) and builds the member's own
+// (pf_aux_job_launch), pf_job_scatter copies.
+enum { PF_JOB_GOALS = 0, PF_JOB_ZONES = 1, PF_JOB_ENTITY = 2 };
 struct pf_job {
+    int kind = PF_JOB_GOALS;
     int ngoals = 0, layer = 0; uint32_t flags = 0;
     const int32_t *dests = nullptr, *targets = nullptr;
+    size_t m = 0;                                   // zone / entity-field requests
+    const pfnav_zone_req *zreqs = nullptr; const pfnav_entity_field_req *ereqs = nullptr;
+    const pfnav_footprint *ents = nullptr; size_t nents = 0; const int32_t *chunks_rc = nullptr; size_t nchunks = 0;
+    std::vector<int32_t> nfields;                   // zones: fields per request (pf_job_launch)
+    std::shared_ptr<void> aux;                      // pfnav_region.cu: the validated batch, from pf_job_plan to pf_job_launch
     bool fits = true; int nf = 0, nl = 0;           // pf_job_plan
     std::vector<uint8_t> lack;
     std::vector<size_t> seg;                        // pf_job_launch: world + 1 block offsets
@@ -374,6 +388,30 @@ struct pf_job {
 int pf_job_plan(pfnav_ctx *ctx, pf_job &J);
 int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int rank, cudaStream_t st);
 int pf_job_scatter(pfnav_ctx *ctx, pf_job &J, cudaStream_t st);
+int pf_job_check_state(pfnav_ctx *ctx);
+int pf_aux_job_plan(pfnav_ctx *ctx, pf_job &J);
+int pf_aux_job_launch(pfnav_ctx *ctx, pf_job &J, int world, int rank, cudaStream_t st);
+// one field copy of k_field_copy: block src of the source buffer of its kind (0 flow, 1 LOS) to block dst
+struct pf_field_copy { int32_t src, dst, kind; };
+//   pf_job_layout  owners and staging blocks of a zone or entity-field batch: field f of the batch (in the order the
+//                  serial calls write them) is written by request freq[f] to key fkey[f] and costs fcost[f]. A key
+//                  belongs to the request that writes it last; a request costs what its last-written keys cost. The most
+//                  expensive request first, to the member with the least cost so far, ties to the lower rank; sets
+//                  ctx->job_owner (-1: the request writes no key last) and J.seg; blk[f]: the field's staging block, -1
+//                  when a later field writes its key.
+//   pf_job_stage   grows the staging buffer to the job's blocks with `items` behind them and uploads the items, the
+//                  member's slot table and its `has` bytes on `st` (J.d_items, J.nitems for pf_job_scatter).
+void pf_job_layout(pfnav_ctx *ctx, pf_job &J, const std::vector<int32_t> &freq, const std::vector<size_t> &fkey,
+                   const std::vector<int64_t> &fcost, int world, std::vector<int32_t> &blk);
+int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &items, int world, cudaStream_t st);
+// the host pool state pf_pool_reserve can change for a batch naming `keys`: saved before a dry run, restored after it
+struct pf_pool_saved {
+    std::vector<size_t> keys; std::vector<int32_t> kslot, free_slots; std::vector<int64_t> owner;
+    std::vector<uint64_t> ffid; std::vector<uint8_t> has; std::vector<uint32_t> touch;
+    int used = 0; uint64_t evictions = 0; bool gb_valid = false;
+};
+void pf_pool_save(const pfnav_ctx *ctx, std::vector<size_t> keys, pf_pool_saved &S);
+void pf_pool_restore(pfnav_ctx *ctx, const pf_pool_saved &S);
 
 enum { PF_PROF_FLOW = 0, PF_PROF_LOS = 1, PF_PROF_INDEX = 2, PF_PROF_VDES = 3, PF_PROF_COHESION = 4,
        PF_PROF_VELOCITY = 5, PF_PROF_UPDATE = 6, PF_PROF_APPLY = 7, PF_PROF_SLOTS = 8 };

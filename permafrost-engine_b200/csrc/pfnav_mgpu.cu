@@ -460,48 +460,59 @@ extern "C" int pfnav_group_exchange_blocker_ops(pfnav_group *g)
 }
 
 // ------------------------------------------------------------------------------------------
-// Goal batches of a job (pfnav_plan.cu: pf_job_*). Every member plans the whole batch and describes itself in one
-// record -- its verdict on the arguments, whether its pool can hold its fields, the (goal, chunk) fields it lacks --
-// and every member reads every record before anything changes. Then each goal's owner builds the union of the lacked
-// fields into its staging segment, the segments are exchanged (segment r is rank r's), and every member copies the
-// fields it lacks into its own slots. The owners and the segment sizes follow from the plan and the union, which every
-// member computes alike, so no count is exchanged.
+// Batches of a job (pfnav_plan.cu: pf_job_*; zone and entity-field batches: pfnav_region.cu). Every member plans the
+// whole batch and describes itself in one record -- its verdict on the arguments, whether its pool can hold its fields,
+// and for a goal batch the (goal, chunk) fields it lacks -- and every member reads every record before anything changes.
+// Then each goal's or request's owner builds its fields into its staging segment, the segments are exchanged (segment
+// r is rank r's), and every member copies the fields it needs into its own slots. The owners and the segment sizes
+// follow from the plan (and a goal batch's union of lacks), which every member computes alike, so no count is exchanged.
 // ------------------------------------------------------------------------------------------
 static void job_init(pf_job &J, int ngoals, const int32_t *dests, int layer, const int32_t *targets, uint32_t flags)
 {
     J.ngoals = ngoals; J.dests = dests; J.layer = layer; J.targets = targets; J.flags = flags;
 }
 
-// NCCL: one all-gather of the member records on `stream` (and a host wait for it), the owners' builds, a group of
-// broadcasts (one per owner with a non-empty segment) on `stream`, the copies into the pool on `stream`.
-extern "C" int pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
-                                           uint32_t flags, void *stream, int *out_n_flow, int *out_n_los)
+static void job_init_zones(pf_job &J, const pfnav_zone_req *reqs, size_t m)
+{
+    J.kind = PF_JOB_ZONES; J.zreqs = reqs; J.m = m;
+}
+
+static void job_init_entity(pf_job &J, const pfnav_entity_field_req *reqs, size_t m, const pfnav_footprint *ents, size_t nents,
+                            const int32_t *chunks_rc, size_t nchunks)
+{
+    J.kind = PF_JOB_ENTITY; J.ereqs = reqs; J.m = m; J.ents = ents; J.nents = nents; J.chunks_rc = chunks_rc; J.nchunks = nchunks;
+}
+
+// the NCCL form's member: a context of a job, not of an in-process group
+static int nccl_member(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_mgpu **out)
 {
     PF_ARG(ctx, "ctx");
     PF_NEED_DEVICE(ctx);
     pf_mgpu *m = (pf_mgpu *)ctx->mgpu;
     if (!m) {
-        pfnav_set_error("pfnav_mgpu_request_goals_ex: pfnav_mgpu_init not called");
+        pfnav_set_error("%s: pfnav_mgpu_init not called", fn);
         return PFNAV_ERR_STATE;
     }
     if (m->group) {
-        pfnav_set_error("pfnav_mgpu_request_goals_ex: member of an in-process group: pfnav_group_request_goals_ex");
+        pfnav_set_error("%s: member of an in-process group: %s", fn, group_fn);
         return PFNAV_ERR_STATE;
     }
     PF_ARG(ctx->d_pool_slot, "pool not created");
-    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
-    if (out_n_flow) *out_n_flow = 0;
-    if (out_n_los) *out_n_los = 0;
-    if (ngoals == 0) return PFNAV_OK;
-    PF_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = pf_stream(ctx, stream);
-    pf_job J;
-    job_init(J, ngoals, dests, layer, targets, flags);
+    *out = m;
+    return PFNAV_OK;
+}
+
+// NCCL: one all-gather of the member records on `stream` (and a host wait for it), the owners' builds, a group of
+// broadcasts (one per owner with a non-empty segment) on `stream`, the copies into the pool on `stream`.
+static int nccl_job(pfnav_ctx *ctx, pf_mgpu *m, pf_job &J, cudaStream_t st, const char *fn)
+{
     const int local = pf_job_plan(ctx, J);
     const std::string local_err = local ? pfnav_last_error() : "";
-    // record: {verdict, fits, 0, 0} then one lack byte per (goal, chunk); every rank has the same goal count and map
+    // record: {verdict, fits, 0, 0} then, for a goal batch, one lack byte per (goal, chunk); every rank has the same
+    // arguments and map
     const int world = m->world, rank = m->rank;
-    const size_t nlack = (size_t)ngoals * ctx->chunk_w * ctx->chunk_h, rec = 16 + ((nlack + 15) & ~(size_t)15);
+    const size_t nlack = J.kind == PF_JOB_GOALS ? (size_t)J.ngoals * ctx->chunk_w * ctx->chunk_h : 0;
+    const size_t rec = 16 + ((nlack + 15) & ~(size_t)15);
     if (m->xgoal_bytes < rec * world) {
         cudaFree(m->d_xgoal);
         m->d_xgoal = nullptr; m->xgoal_bytes = 0;
@@ -512,7 +523,7 @@ extern "C" int pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     uint8_t *mine = all.data() + rec * rank;
     const int32_t hdr[4] = {local, J.fits ? 1 : 0, 0, 0};
     memcpy(mine, hdr, sizeof(hdr));
-    if (!local) memcpy(mine + 16, J.lack.data(), nlack);
+    if (!local && nlack) memcpy(mine + 16, J.lack.data(), nlack);
     PF_CUDA(cudaMemcpyAsync(m->d_xgoal + rec * rank, mine, rec, cudaMemcpyHostToDevice, st));
     PF_NCCL(g_nccl.AllGather(m->d_xgoal + rec * rank, m->d_xgoal, rec, /*ncclInt8*/ 0, m->comm, st));
     PF_CUDA(cudaMemcpyAsync(all.data(), m->d_xgoal, all.size(), cudaMemcpyDeviceToHost, st));
@@ -532,11 +543,11 @@ extern "C" int pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
         return local;
     }
     if (refused >= 0) {
-        pfnav_set_error("pfnav_mgpu_request_goals_ex: rank %d refused the batch (error %d); no rank changed its pool", refused, refused_rc);
+        pfnav_set_error("%s: rank %d refused the batch (error %d); no rank changed its pool", fn, refused, refused_rc);
         return refused_rc;
     }
     if (full >= 0) {
-        pfnav_set_error("pfnav_mgpu_request_goals_ex: the field pool of rank %d cannot hold its fields; no rank changed its pool", full);
+        pfnav_set_error("%s: the field pool of rank %d cannot hold its fields; no rank changed its pool", fn, full);
         return PFNAV_ERR_NOMEM;
     }
     int rc = pf_job_launch(ctx, J, uni.data(), world, rank, st);
@@ -551,17 +562,11 @@ extern "C" int pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
         }
         PF_NCCL(g_nccl.GroupEnd());
     }
-    if ((rc = pf_job_scatter(ctx, J, st))) return rc;
-    if (out_n_flow) *out_n_flow = J.nf;
-    if (out_n_los) *out_n_los = J.nl;
-    return PFNAV_OK;
+    return pf_job_scatter(ctx, J, st);
 }
 
-// In-process group: the records are read on the host; member i pulls every owner's segment into its staging with
-// cudaMemcpyPeerAsync on its context stream, copies what it lacks into its pool, and then waits until every peer has
-// finished pulling its own segment. out_n_flow / out_n_los: `world` entries, member i's solo counts.
-extern "C" int pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
-                                            uint32_t flags, int *out_n_flow, int *out_n_los)
+// the group form's members: pools created, maps and pools of one shape, peer access between their devices
+static int group_members(pfnav_group *g, const char *fn)
 {
     PF_ARG(g, "group");
     const int world = (int)g->ctxs.size();
@@ -572,23 +577,21 @@ extern "C" int pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const in
         PF_ARG(c->chunk_w == c0->chunk_w && c->chunk_h == c0->chunk_h && c->pool_ndests == c0->pool_ndests,
                "members hold maps or pools of different shapes");
     }
-    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
-    int rc = peer_check(g, __func__);
-    if (rc) return rc;
-    for (int i = 0; i < world; i++) {
-        if (out_n_flow) out_n_flow[i] = 0;
-        if (out_n_los) out_n_los[i] = 0;
-    }
-    if (ngoals == 0) return PFNAV_OK;
-    std::vector<pf_job> J(world);
-    for (int i = 0; i < world; i++) {
-        job_init(J[i], ngoals, dests, layer, targets, flags);
+    return peer_check(g, fn);
+}
+
+// In-process group: the records are read on the host; member i pulls every owner's segment into its staging with
+// cudaMemcpyPeerAsync on its context stream, copies what it needs into its pool, and then waits until every peer has
+// finished pulling its own segment.
+static int group_job(pfnav_group *g, std::vector<pf_job> &J, const char *fn)
+{
+    const int world = (int)g->ctxs.size();
+    int rc = 0;
+    for (int i = 0; i < world; i++)
         if ((rc = pf_job_plan(g->ctxs[i], J[i]))) return rc;            // no member has changed anything yet
-    }
     for (int i = 0; i < world; i++)
         if (!J[i].fits) {
-            pfnav_set_error("pfnav_group_request_goals_ex: the field pool of member %d cannot hold its fields; no member "
-                            "changed its pool", i);
+            pfnav_set_error("%s: the field pool of member %d cannot hold its fields; no member changed its pool", fn, i);
             return PFNAV_ERR_NOMEM;
         }
     std::vector<uint8_t> uni(J[0].lack.size(), 0);
@@ -628,9 +631,100 @@ extern "C" int pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const in
                 if (p != i) PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->pulled[p], 0));
         }
     }
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_mgpu_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
+                                           uint32_t flags, void *stream, int *out_n_flow, int *out_n_los)
+{
+    pf_mgpu *m = nullptr;
+    if (int rc = nccl_member(ctx, __func__, "pfnav_group_request_goals_ex", &m)) return rc;
+    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
+    if (out_n_flow) *out_n_flow = 0;
+    if (out_n_los) *out_n_los = 0;
+    if (ngoals == 0) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    pf_job J;
+    job_init(J, ngoals, dests, layer, targets, flags);
+    if (int rc = nccl_job(ctx, m, J, pf_stream(ctx, stream), __func__)) return rc;
+    if (out_n_flow) *out_n_flow = J.nf;
+    if (out_n_los) *out_n_los = J.nl;
+    return PFNAV_OK;
+}
+
+// out_n_flow / out_n_los: `world` entries, member i's solo counts
+extern "C" int pfnav_group_request_goals_ex(pfnav_group *g, int ngoals, const int32_t *dests, int layer, const int32_t *targets,
+                                            uint32_t flags, int *out_n_flow, int *out_n_los)
+{
+    if (int rc = group_members(g, __func__)) return rc;
+    const int world = (int)g->ctxs.size();
+    PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
+    for (int i = 0; i < world; i++) {
+        if (out_n_flow) out_n_flow[i] = 0;
+        if (out_n_los) out_n_los[i] = 0;
+    }
+    if (ngoals == 0) return PFNAV_OK;
+    std::vector<pf_job> J(world);
+    for (int i = 0; i < world; i++) job_init(J[i], ngoals, dests, layer, targets, flags);
+    if (int rc = group_job(g, J, __func__)) return rc;
     for (int i = 0; i < world; i++) {
         if (out_n_flow) out_n_flow[i] = J[i].nf;
         if (out_n_los) out_n_los[i] = J[i].nl;
     }
     return PFNAV_OK;
+}
+
+extern "C" int pfnav_mgpu_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, void *stream, int32_t *out_nfields)
+{
+    pf_mgpu *mg = nullptr;
+    if (int rc = nccl_member(ctx, __func__, "pfnav_group_request_zones", &mg)) return rc;
+    PF_ARG(m == 0 || reqs, "reqs");
+    if (out_nfields) std::fill(out_nfields, out_nfields + m, 0);
+    if (m == 0) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    pf_job J;
+    job_init_zones(J, reqs, m);
+    if (int rc = nccl_job(ctx, mg, J, pf_stream(ctx, stream), __func__)) return rc;
+    if (out_nfields) std::copy(J.nfields.begin(), J.nfields.end(), out_nfields);
+    return PFNAV_OK;
+}
+
+// out_nfields: m entries, the same on every member
+extern "C" int pfnav_group_request_zones(pfnav_group *g, const pfnav_zone_req *reqs, size_t m, int32_t *out_nfields)
+{
+    if (int rc = group_members(g, __func__)) return rc;
+    PF_ARG(m == 0 || reqs, "reqs");
+    if (out_nfields) std::fill(out_nfields, out_nfields + m, 0);
+    if (m == 0) return PFNAV_OK;
+    std::vector<pf_job> J(g->ctxs.size());
+    for (pf_job &j : J) job_init_zones(j, reqs, m);
+    if (int rc = group_job(g, J, __func__)) return rc;
+    if (out_nfields) std::copy(J[0].nfields.begin(), J[0].nfields.end(), out_nfields);
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_mgpu_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                                      const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc,
+                                                      size_t nchunks, void *stream)
+{
+    pf_mgpu *mg = nullptr;
+    if (int rc = nccl_member(ctx, __func__, "pfnav_group_request_entity_fields_batch", &mg)) return rc;
+    PF_ARG(m == 0 || reqs, "reqs");
+    if (m == 0) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    pf_job J;
+    job_init_entity(J, reqs, m, ents, nents, chunks_rc, nchunks);
+    return nccl_job(ctx, mg, J, pf_stream(ctx, stream), __func__);
+}
+
+extern "C" int pfnav_group_request_entity_fields_batch(pfnav_group *g, const pfnav_entity_field_req *reqs, size_t m,
+                                                       const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc,
+                                                       size_t nchunks)
+{
+    if (int rc = group_members(g, __func__)) return rc;
+    PF_ARG(m == 0 || reqs, "reqs");
+    if (m == 0) return PFNAV_OK;
+    std::vector<pf_job> J(g->ctxs.size());
+    for (pf_job &j : J) job_init_entity(j, reqs, m, ents, nents, chunks_rc, nchunks);
+    return group_job(g, J, __func__);
 }

@@ -350,6 +350,28 @@ int pf_pool_reserve(pfnav_ctx *ctx, const size_t *keys, size_t n, int32_t *slots
     return PFNAV_OK;
 }
 
+// pf_pool_reserve changes the slot-table entries of the keys it is given and of the owners of the slots it evicts, and
+// per-slot and free-list state: save those, so that a dry run of a batch's reservations can be undone exactly
+void pf_pool_save(const pfnav_ctx *ctx, std::vector<size_t> keys, pf_pool_saved &S)
+{
+    S.keys = std::move(keys);
+    S.kslot.resize(S.keys.size());
+    for (size_t i = 0; i < S.keys.size(); i++) S.kslot[i] = ctx->h_pool_slot[S.keys[i]];
+    S.owner = ctx->h_slot_owner; S.has = ctx->h_pool_has; S.touch = ctx->h_slot_touch; S.free_slots = ctx->pool_free;
+    S.ffid.assign(ctx->pool_max, 0);
+    for (int s = 0; s < ctx->pool_max; s++) if (S.owner[s] >= 0) S.ffid[s] = ctx->h_pool_ffid[(size_t)S.owner[s]];
+    S.used = ctx->pool_used; S.evictions = ctx->pool_evictions; S.gb_valid = ctx->goal_batch.valid;
+}
+
+void pf_pool_restore(pfnav_ctx *ctx, const pf_pool_saved &S)
+{
+    for (size_t i = 0; i < S.keys.size(); i++) ctx->h_pool_slot[S.keys[i]] = S.kslot[i];
+    for (int s = 0; s < ctx->pool_max; s++)
+        if (S.owner[s] >= 0) { ctx->h_pool_slot[(size_t)S.owner[s]] = s; ctx->h_pool_ffid[(size_t)S.owner[s]] = S.ffid[s]; }
+    ctx->h_slot_owner = S.owner; ctx->h_pool_has = S.has; ctx->h_slot_touch = S.touch; ctx->pool_free = S.free_slots;
+    ctx->pool_used = S.used; ctx->pool_evictions = S.evictions; ctx->goal_batch.valid = S.gb_valid;
+}
+
 // The flow waves and the LOS dependency chains of a goal batch each get a context-owned stream (the flow kernels
 // need ~100 KB of shared memory per CTA and would otherwise queue the caller's stream behind the persistent LOS
 // CTAs that hold most of it).
@@ -743,7 +765,6 @@ extern "C" int pfnav_fields_join(pfnav_ctx *ctx, void *stream)
 
 // one 4096-byte field per CTA: block it.src of the source buffer of its kind (0 flow, 1 LOS) to block it.dst of the
 // destination buffer of that kind
-struct pf_field_copy { int32_t src, dst, kind; };
 __global__ void __launch_bounds__(256) k_field_copy(const uint8_t *flow_src, const uint8_t *los_src, uint8_t *flow_dst,
                                                     uint8_t *los_dst, const pf_field_copy *items)
 {
@@ -763,19 +784,27 @@ static int field_copy_launch(pfnav_ctx *ctx, const uint8_t *flow_src, const uint
     return 0;
 }
 
+// a job's batch reads the replicated map: refused while this member holds device blocker ops its peers have not seen
+int pf_job_check_state(pfnav_ctx *ctx)
+{
+    if (pf_mgpu_shares_blockers(ctx) && pf_blocker_ops_unexchanged(ctx)) {
+        pfnav_set_error("batch of a job: device blocker ops decided since the last exchange have not been exchanged "
+                        "(pfnav_mgpu_exchange_blocker_ops / pfnav_group_exchange_blocker_ops)");
+        return PFNAV_ERR_STATE;
+    }
+    return PFNAV_OK;
+}
+
 int pf_job_plan(pfnav_ctx *ctx, pf_job &J)
 {
+    if (J.kind != PF_JOB_GOALS) return pf_aux_job_plan(ctx, J);
     const int chunks = ctx->chunk_w * ctx->chunk_h;
     const bool missing_only = (J.flags & PFNAV_REQUEST_MISSING_ONLY) != 0;
     J.fits = true; J.nf = J.nl = 0;
     J.lack.assign((size_t)J.ngoals * chunks, 0);
     for (int g = 0; g < J.ngoals; g++) PF_ARG(J.dests[g] >= 0 && J.dests[g] < ctx->pool_ndests, "dest");
     PF_ARG(J.layer >= 0 && J.layer < ctx->nlayers, "layer");
-    if (pf_mgpu_shares_blockers(ctx) && pf_blocker_ops_unexchanged(ctx)) {
-        pfnav_set_error("goal batch of a job: device blocker ops decided since the last exchange have not been exchanged "
-                        "(pfnav_mgpu_exchange_blocker_ops / pfnav_group_exchange_blocker_ops)");
-        return PFNAV_ERR_STATE;
-    }
+    if (int rc = pf_job_check_state(ctx)) return rc;
     if (J.ngoals == 0) return PFNAV_OK;
     pf_host_timer ht(ctx);
     int rc = plan_batch(ctx, J.ngoals, J.dests, J.layer, J.targets, missing_only, ht);
@@ -793,6 +822,7 @@ int pf_job_plan(pfnav_ctx *ctx, pf_job &J)
 
 int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int rank, cudaStream_t st)
 {
+    if (J.kind != PF_JOB_GOALS) return pf_aux_job_launch(ctx, J, world, rank, st);
     const int chunks = ctx->chunk_w * ctx->chunk_h, ngoals = J.ngoals;
     pf_planner &PL = planner_of(ctx);
     pf_planner::merged &B = PL.batch;               // this member's solo batch, merged by pf_job_plan
@@ -996,8 +1026,76 @@ int pf_job_scatter(pfnav_ctx *ctx, pf_job &J, cudaStream_t st)
     return PFNAV_OK;
 }
 
-// TEST HOOK: the last goal batch of a job on this member -- the flow / LOS requests it built for the job, and the
-// owner of every goal (-1: no member lacked a field of it)
+// Zone and entity-field batches of a job (pfnav_region.cu: pf_aux_job_*). Neither batch skips a field the pool holds and
+// neither field reads another pool field, so every member writes the same keys with the same bytes: the keys, their
+// owners and the staging layout follow from the arguments alone.
+void pf_job_layout(pfnav_ctx *ctx, pf_job &J, const std::vector<int32_t> &freq, const std::vector<size_t> &fkey,
+                   const std::vector<int64_t> &fcost, int world, std::vector<int32_t> &blk)
+{
+    const size_t n = freq.size();
+    // the last writer of every key: the last field of each run of equal keys, in (key, field) order
+    std::vector<int32_t> ord(n);
+    for (size_t f = 0; f < n; f++) ord[f] = (int32_t)f;
+    std::sort(ord.begin(), ord.end(), [&](int32_t a, int32_t b) { return fkey[a] != fkey[b] ? fkey[a] < fkey[b] : a < b; });
+    std::vector<uint8_t> kept(n, 0);
+    for (size_t i = 0; i < n; i++) kept[ord[i]] = i + 1 == n || fkey[ord[i + 1]] != fkey[ord[i]];
+    std::vector<int64_t> cost(J.m, 0);
+    std::vector<uint8_t> writes(J.m, 0);
+    for (size_t f = 0; f < n; f++) if (kept[f]) { cost[freq[f]] += fcost[f]; writes[freq[f]] = 1; }
+    std::vector<int32_t> order;
+    for (size_t i = 0; i < J.m; i++) if (writes[i]) order.push_back((int32_t)i);
+    std::stable_sort(order.begin(), order.end(), [&](int32_t a, int32_t b) { return cost[a] > cost[b]; });
+    std::vector<int32_t> &owner = ctx->job_owner;
+    owner.assign(J.m, -1);
+    std::vector<int64_t> load(world, 0);
+    for (int32_t i : order) {
+        int r = 0;
+        for (int k = 1; k < world; k++) if (load[k] < load[r]) r = k;
+        owner[i] = r;
+        load[r] += cost[i];
+    }
+    blk.assign(n, -1);
+    J.seg.assign(world + 1, 0);
+    int32_t next = 0;
+    for (int r = 0; r < world; r++) {
+        J.seg[r] = (size_t)next;
+        for (size_t f = 0; f < n; f++) if (kept[f] && owner[freq[f]] == r) blk[f] = next++;
+    }
+    J.seg[world] = (size_t)next;
+}
+
+int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &items, int world, cudaStream_t st)
+{
+    const size_t o_items = J.seg[world] * 4096, b_items = items.size() * sizeof(pf_field_copy);
+    const size_t b_slot = ctx->h_pool_slot.size() * 4, need = o_items + b_items;
+    // the previous batch's builds, exchange and copies may still read the staging buffer: growing it waits for the
+    // device (a group member's stream has waited for its peers' reads of its staging)
+    if (ctx->job_stage_bytes < need) {
+        PF_CUDA(pf_fields_sync(ctx));
+        PF_CUDA(cudaDeviceSynchronize());
+        cudaFree(ctx->d_job_stage);
+        ctx->d_job_stage = nullptr; ctx->job_stage_bytes = 0;
+        PF_CUDA(cudaMalloc(&ctx->d_job_stage, need * 2));
+        ctx->job_stage_bytes = need * 2;
+    }
+    uint8_t *host = nullptr;
+    int ri = 0;
+    if (int rc = pf_plan_host(ctx, b_items + b_slot + (size_t)ctx->pool_max, &host, &ri)) return rc;
+    memcpy(host, items.data(), b_items);
+    memcpy(host + b_items, ctx->h_pool_slot.data(), b_slot);
+    memcpy(host + b_items + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
+    if (b_items) PF_CUDA(cudaMemcpyAsync(ctx->d_job_stage + o_items, host, b_items, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_items, b_slot, cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_items + b_slot, ctx->pool_max,
+                            cudaMemcpyHostToDevice, st));
+    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    J.d_items = ctx->d_job_stage + o_items; J.nitems = (int)items.size();
+    return PFNAV_OK;
+}
+
+// TEST HOOK: the last batch of a job on this member, of any kind. Goal batches: the flow / LOS requests it built for the
+// job, and the owner of every goal (-1: no member lacked a field of it). Zone and entity-field batches: the fields it
+// built, 0, and the owner of every request (-1: the request writes no key last)
 extern "C" int pfnav_mgpu_fields_stats(pfnav_ctx *ctx, int *out_n_flow, int *out_n_los, int32_t *out_owner, int max_goals)
 {
     PF_ARG(ctx && max_goals >= 0 && (max_goals == 0 || out_owner), "args");

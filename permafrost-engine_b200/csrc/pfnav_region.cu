@@ -463,27 +463,21 @@ __global__ void k_pool_scatter(const int32_t *__restrict__ fresh, int nfresh, in
     if (i < nhas) has[slot[i]] = hasv[i];
 }
 
-// A batch floods its zone seeds on the host when the sum of its floods' budgets is at most this many times the largest one.
-// The device replays a flood on one lane, about ten times slower per popped tile than the host (H100, DESIGN.md §5), and
-// a batch waits for its longest flood; the host floods one field after another.
-#define PF_ZONE_HOST_POP_RATIO 10
+// A zone or entity field of a batch: request `req` writes chunk (cr, cc) of its destination into `slot` (a pool slot, or a
+// staging block when a job member builds it for the job)
+struct aux_field { uint32_t req; int32_t cr, cc, slot; };
 
-// N_RequestAsyncGroupArrivalField (nav.c:3921) for m requests, in the order of the serial calls. Slots follow the single
-// call's rule (a fresh slot from pool_used, no eviction, no pool_free reuse, only `has` bit 0), request by request and
-// chunk by chunk. The device work writes pool slots only: when several fields of the batch land in one slot (a repeated
-// (dest, chunk)), only the last is flooded and integrated, which is what the serial calls leave there.
-extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, void *stream, int32_t *out_nfields,
-                                        int *out_ndone)
+// The stages of a zone batch, shared by pfnav_pool_request_zones and the job form (pf_aux_job_*). zone_validate checks
+// the whole batch before anything changes: ctile[2i..] is request i's centre tile when on_map[i] (nav.c:3931), *dim the
+// window of its fields.
+static int zone_validate(const pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, std::vector<int32_t> &ctile,
+                         std::vector<uint8_t> &on_map, int *dim)
 {
-    if (out_ndone) *out_ndone = 0;
-    PF_ARG(ctx, "ctx");
-    PF_NEED_DEVICE(ctx);
     PF_ARG(ctx->d_cost && ctx->d_pool_slot, "map / pool not created");
     PF_ARG(m == 0 || reqs, "reqs");
     PF_ARG(m < (1u << 24), "m");
-    // ---- the whole batch is checked before anything changes
-    std::vector<int32_t> ctile(2 * m);
-    std::vector<uint8_t> on_map(m);
+    ctile.assign(2 * m, 0);
+    on_map.assign(m, 0);
     bool any_on_map = false;
     for (size_t i = 0; i < m; i++) {
         const pfnav_zone_req &q = reqs[i];
@@ -493,35 +487,50 @@ extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *re
         on_map[i] = region_tile_for_point(ctx, q.centre_x, q.centre_z, &ctile[2 * i]);      // nav.c:3931
         any_on_map |= on_map[i] != 0;
     }
-    int dim = 0;
-    if (any_on_map) {
-        int rc = zone_dim(ctx, &dim);
-        if (rc) return rc;
-    }
-    if (out_nfields) std::fill(out_nfields, out_nfields + m, 0);
-    PF_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = pf_stream(ctx, stream);
-    PF_CUDA(pf_fields_join(ctx, st));
-    PF_CUDA(pf_pool_refresh(ctx, st));
-    // ---- slots request by request, in order
+    *dim = 0;
+    return any_on_map ? zone_dim(ctx, dim) : PFNAV_OK;
+}
+
+// the chunks request q's footprint can reach, rows {min, max} then columns (nav.c:3945-3951; C division truncates toward zero)
+static void zone_chunks(const pfnav_ctx *ctx, const pfnav_zone_req &q, const int32_t *ctile, int out[4])
+{
+    const int r0 = ctile[0], c0 = ctile[1], reach = 2 * q.radius;
+    auto clampi = [](int v, int lo, int hi) { return std::min(std::max(v, lo), hi); };
+    out[0] = clampi((r0 - reach) / 64, 0, ctx->chunk_h - 1); out[1] = clampi((r0 + reach) / 64, 0, ctx->chunk_h - 1);
+    out[2] = clampi((c0 - reach) / 64, 0, ctx->chunk_w - 1); out[3] = clampi((c0 + reach) / 64, 0, ctx->chunk_w - 1);
+}
+
+// the flood of zone request q's field of chunk (cr, cc) -> its budget when the window holds the centre (what the flood
+// pops; field.c:1843), else 0
+static uint64_t zone_flood(const pfnav_zone_req &q, const int32_t *ctile, int dim, int cr, int cc, zone_job *j)
+{
+    size_t budget = (size_t)(M_PI * q.radius * q.radius + 0.5);         // field.c:1843
+    if (budget > (size_t)dim * dim) budget = (size_t)dim * dim;
+    j->layer = q.layer; j->centre_r = ctile[0]; j->centre_c = ctile[1]; j->budget = (int32_t)budget;
+    chunk_region_base(dim, cr, cc, &j->base_r, &j->base_c);
+    const int cdr = j->centre_r - j->base_r, cdc = j->centre_c - j->base_c;
+    return cdr >= 0 && cdr < dim && cdc >= 0 && cdc < dim ? budget : 0;
+}
+
+// Slots request by request, in order, by the single call's rule (a fresh slot from pool_used, no eviction, no pool_free
+// reuse, only `has` bit 0), chunk by chunk. fresh: (slot table index, slot) of every new reservation. On
+// PFNAV_ERR_NOMEM, *out_done is the request that did not fit: it keeps its reservations, unbuilt, as the single call
+// leaves them.
+static int zone_reserve(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, const std::vector<int32_t> &ctile,
+                        const std::vector<uint8_t> &on_map, std::vector<aux_field> &fields, std::vector<int32_t> &fresh,
+                        int32_t *out_nfields, size_t *out_done)
+{
     const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
-    struct field_t { uint32_t req; int32_t cr, cc, slot; };
-    std::vector<field_t> fields;
-    std::vector<int32_t> fresh;             // (slot table index, slot) of every new reservation
     int rc = PFNAV_OK;
     size_t done = 0;
     for (; done < m; done++) {
         if (!on_map[done]) continue;
         const pfnav_zone_req &q = reqs[done];
-        const int r0 = ctile[2 * done], c0 = ctile[2 * done + 1];
-        // the chunks the footprint can reach (nav.c:3945-3951; C division truncates toward zero)
-        const int reach = 2 * q.radius;
-        auto clampi = [](int v, int lo, int hi) { return std::min(std::max(v, lo), hi); };
-        const int min_cr = clampi((r0 - reach) / 64, 0, ctx->chunk_h - 1), max_cr = clampi((r0 + reach) / 64, 0, ctx->chunk_h - 1);
-        const int min_cc = clampi((c0 - reach) / 64, 0, cw - 1), max_cc = clampi((c0 + reach) / 64, 0, cw - 1);
+        int ch[4];
+        zone_chunks(ctx, q, &ctile[2 * done], ch);
         const size_t first = fields.size();
-        for (int cr = min_cr; cr <= max_cr && rc == PFNAV_OK; cr++)
-            for (int cc = min_cc; cc <= max_cc; cc++) {
+        for (int cr = ch[0]; cr <= ch[1] && rc == PFNAV_OK; cr++)
+            for (int cc = ch[2]; cc <= ch[3]; cc++) {
                 const size_t si = (size_t)q.dest * nch + cr * cw + cc;
                 int32_t slot = ctx->h_pool_slot[si];
                 if (slot < 0) {
@@ -536,38 +545,41 @@ extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *re
                 }
                 fields.push_back({(uint32_t)done, cr, cc, slot});
             }
-        if (rc) {                       // request `done` keeps its reservations, unbuilt, as the single call leaves them
+        if (rc) {
             fields.resize(first);
             break;
         }
         for (size_t f = first; f < fields.size(); f++) ctx->h_pool_has[fields[f].slot] |= 1;
         if (out_nfields) out_nfields[done] = (int32_t)(fields.size() - first);
     }
-    if (out_ndone) *out_ndone = (int)done;
-    if (fields.empty() && fresh.empty()) return rc;
-    if (!fields.empty()) ctx->goal_batch.valid = false;
-    // ---- one flood + one integration per slot: the last field written to it
-    std::vector<int32_t> last(ctx->pool_max, -1);
-    for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
+    *out_done = done;
+    return rc;
+}
+
+// A batch floods its zone seeds on the host when the sum of its floods' budgets is at most this many times the largest one.
+// The device replays a flood on one lane, about ten times slower per popped tile than the host (H100, DESIGN.md §5), and
+// a batch waits for its longest flood; the host floods one field after another.
+#define PF_ZONE_HOST_POP_RATIO 10
+
+// One flood + one integration per field of F, into block F[k].slot of d_out (the pool's flow fields, or a job's staging).
+// scatter: the pool entries the batch changed (fresh, and the `has` bytes of the F slots) go to the device first;
+// k_pool_scatter writes only those, since the device slot table and `has` bytes equal the host mirrors otherwise.
+static int zone_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_zone_req *reqs, const std::vector<int32_t> &ctile, int dim,
+                      const std::vector<aux_field> &F, const std::vector<int32_t> &fresh, bool scatter, uint8_t *d_out)
+{
     std::vector<zone_job> jobs;
     std::vector<pfnav_region_req> kreq;
     std::vector<int32_t> kslot;
     uint64_t pops = 0, max_pops = 0;        // the floods' budgets: what each costs on the host / the device's critical chain
-    for (size_t f = 0; f < fields.size(); f++) {
-        const field_t &F = fields[f];
-        if (last[F.slot] != (int32_t)f) continue;
-        const pfnav_zone_req &q = reqs[F.req];
-        size_t budget = (size_t)(M_PI * q.radius * q.radius + 0.5);         // field.c:1843
-        if (budget > (size_t)dim * dim) budget = (size_t)dim * dim;
+    for (const aux_field &f : F) {
+        const pfnav_zone_req &q = reqs[f.req];
         zone_job j;
-        j.layer = q.layer; j.centre_r = ctile[2 * F.req]; j.centre_c = ctile[2 * F.req + 1]; j.budget = (int32_t)budget;
-        chunk_region_base(dim, F.cr, F.cc, &j.base_r, &j.base_c);
-        const int cdr = j.centre_r - j.base_r, cdc = j.centre_c - j.base_c;
-        if (cdr >= 0 && cdr < dim && cdc >= 0 && cdc < dim) { pops += budget; max_pops = std::max<uint64_t>(max_pops, budget); }
+        const uint64_t b = zone_flood(q, &ctile[2 * f.req], dim, f.cr, f.cc, &j);
+        pops += b; max_pops = std::max(max_pops, b);
         jobs.push_back(j);
         pfnav_region_req rq = {};
-        rq.layer = q.layer; rq.center_r = F.cr; rq.center_c = F.cc; rq.flags = PFNAV_REGION_CREATE;
-        kreq.push_back(rq); kslot.push_back(F.slot);
+        rq.layer = q.layer; rq.center_r = f.cr; rq.center_c = f.cc; rq.flags = PFNAV_REGION_CREATE;
+        kreq.push_back(rq); kslot.push_back(f.slot);
     }
     const size_t nk = kreq.size();
     // ---- where the floods run: a device flood is one lane's serial chain, and the batch waits for the longest one; the
@@ -585,15 +597,14 @@ extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *re
         }
     }
     // the `has` bytes of the written slots (h_pool_has after the batch)
-    std::vector<uint8_t> hasv(nk);
-    for (size_t k = 0; k < nk; k++) hasv[k] = ctx->h_pool_has[kslot[k]];
-    // ---- one pinned staging buffer with the inputs, copied into the device scratch. The device slot table and `has`
-    // bytes equal the host mirrors except for what this batch changed: k_pool_scatter writes only those entries.
+    std::vector<uint8_t> hasv(scatter ? nk : 0);
+    for (size_t k = 0; k < hasv.size(); k++) hasv[k] = ctx->h_pool_has[kslot[k]];
+    // ---- one pinned staging buffer with the inputs, copied into the device scratch
     size_t b_in = 0;
     auto sec = [&](size_t bytes) { const size_t o = b_in; b_in = (b_in + bytes + 15) & ~(size_t)15; return o; };
     const size_t o_req = sec(nk * sizeof(pfnav_region_req)), o_slot = sec(nk * 4);
     const size_t o_jobs = sec(host_floods ? 0 : nk * sizeof(zone_job)), o_seeds = sec(seeds.size() * 4);
-    const size_t o_fresh = sec(fresh.size() * 4), o_hasv = sec(nk);
+    const size_t o_fresh = sec(fresh.size() * 4), o_hasv = sec(hasv.size());
     const size_t stage = b_in;
     const size_t o_bits = b_in, need = o_bits + (host_floods ? 0 : nk * ((size_t)dim * dim / 8)) + 16;
     uint8_t *host = nullptr, *dev = nullptr;
@@ -605,20 +616,22 @@ extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *re
     if (!host_floods) memcpy(host + o_jobs, jobs.data(), nk * sizeof(zone_job));
     memcpy(host + o_seeds, seeds.data(), seeds.size() * 4);
     memcpy(host + o_fresh, fresh.data(), fresh.size() * 4);
-    memcpy(host + o_hasv, hasv.data(), nk);
+    memcpy(host + o_hasv, hasv.data(), hasv.size());
     if ((lrc = batch_scratch(ctx, st, need, &dev))) return lrc;
     PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
-    const int nscatter = (int)std::max(fresh.size() / 2, nk);
-    k_pool_scatter<<<(unsigned)((nscatter + 255) / 256), 256, 0, st>>>((const int32_t *)(dev + o_fresh), (int)(fresh.size() / 2),
-                                                                        ctx->d_pool_slot, (const int32_t *)(dev + o_slot),
-                                                                        (const uint8_t *)(dev + o_hasv), (int)nk,
-                                                                        ctx->d_pool_los + (size_t)ctx->pool_max * 4096);
-    ctx->launches++;
-    PF_CUDA(cudaGetLastError());
+    const int nscatter = (int)std::max(fresh.size() / 2, hasv.size());
+    if (nscatter) {
+        k_pool_scatter<<<(unsigned)((nscatter + 255) / 256), 256, 0, st>>>((const int32_t *)(dev + o_fresh), (int)(fresh.size() / 2),
+                                                                            ctx->d_pool_slot, (const int32_t *)(dev + o_slot),
+                                                                            (const uint8_t *)(dev + o_hasv), (int)hasv.size(),
+                                                                            ctx->d_pool_los + (size_t)ctx->pool_max * 4096);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+    }
     if (nk && host_floods) {
         if ((lrc = region_launch(ctx, dim, (const pfnav_region_req *)(dev + o_req), nk, (const int32_t *)(dev + o_seeds),
-                                 (const int32_t *)dev, ctx->d_pool_flow, st, 1, nullptr, (const int32_t *)(dev + o_slot))))
+                                 (const int32_t *)dev, d_out, st, 1, nullptr, (const int32_t *)(dev + o_slot))))
             return lrc;
     } else if (nk) {
         const pfnav_region_req *d_req = (const pfnav_region_req *)(dev + o_req);
@@ -630,12 +643,48 @@ extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *re
                                                           (int)nk, d_bits);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
-        if ((lrc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, ctx->d_pool_flow, st, 1, d_bits,
+        if ((lrc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, d_out, st, 1, d_bits,
                                  (const int32_t *)(dev + o_slot))))
             return lrc;
     }
     PF_CUDA(cudaEventRecord(ctx->ent_ev, st));
-    return rc;
+    return PFNAV_OK;
+}
+
+// N_RequestAsyncGroupArrivalField (nav.c:3921) for m requests, in the order of the serial calls (zone_reserve). The
+// device work writes pool slots only: when several fields of the batch land in one slot (a repeated (dest, chunk)), only
+// the last is flooded and integrated, which is what the serial calls leave there.
+extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, void *stream, int32_t *out_nfields,
+                                        int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    std::vector<int32_t> ctile;
+    std::vector<uint8_t> on_map;
+    int dim = 0;
+    int rc = zone_validate(ctx, reqs, m, ctile, on_map, &dim);
+    if (rc) return rc;
+    if (out_nfields) std::fill(out_nfields, out_nfields + m, 0);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_fields_join(ctx, st));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    std::vector<aux_field> fields;
+    std::vector<int32_t> fresh;
+    size_t done = 0;
+    rc = zone_reserve(ctx, reqs, m, ctile, on_map, fields, fresh, out_nfields, &done);
+    if (out_ndone) *out_ndone = (int)done;
+    if (fields.empty() && fresh.empty()) return rc;
+    if (!fields.empty()) ctx->goal_batch.valid = false;
+    // ---- one flood + one integration per slot: the last field written to it
+    std::vector<int32_t> last(ctx->pool_max, -1);
+    for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
+    std::vector<aux_field> build;
+    for (size_t f = 0; f < fields.size(); f++)
+        if (last[fields[f].slot] == (int32_t)f) build.push_back(fields[f]);
+    const int lrc = zone_build(ctx, st, reqs, ctile, dim, build, fresh, true, ctx->d_pool_flow);
+    return lrc ? lrc : rc;
 }
 
 extern "C" int pfnav_pool_request_zone(pfnav_ctx *ctx, int dest, int layer, const float *centre_xz, int radius, void *stream,
@@ -989,19 +1038,19 @@ static void bin_enemies(const pfnav_ctx *ctx, const pfnav_footprint *ents, uint3
     }
 }
 
-extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
-                                                      const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc,
-                                                      size_t nchunks, void *stream, int *out_ndone)
+// The stages of an entity-field batch, shared by pfnav_pool_request_entity_fields_batch and the job form
+// (pf_aux_job_*). entity_validate checks the whole batch before anything changes and bins the TARGET_ENEMIES footprints,
+// one bin per distinct footprint range (req_bin[i]: request i's).
+struct entity_batch { int dim = 0; std::vector<enemy_bins> bins; std::vector<int32_t> req_bin; };
+
+static int entity_validate(const pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m, const pfnav_footprint *ents,
+                           size_t nents, const int32_t *chunks_rc, size_t nchunks, entity_batch &E)
 {
-    if (out_ndone) *out_ndone = 0;
-    PF_ARG(ctx, "ctx");
-    PF_NEED_DEVICE(ctx);
     PF_ARG(ctx->d_cost && ctx->d_pool_slot, "map / pool not created");
     PF_ARG(m == 0 || reqs, "reqs");
     PF_ARG((nents == 0 || ents) && (nchunks == 0 || chunks_rc), "ents / chunks_rc");
     PF_ARG(m < (1u << 24) && nents < (1u << 24) && nchunks < (1u << 24), "m / nents / nchunks");
-    const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
-    // ---- the whole batch is checked before anything changes
+    const int cw = ctx->chunk_w;
     bool any_fields = false;
     for (size_t i = 0; i < m; i++) {
         const pfnav_entity_field_req &q = reqs[i];
@@ -1017,15 +1066,15 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
         }
         any_fields |= q.chunk_n > 0;
     }
-    int dim = 0;
+    E.dim = 0;
     if (any_fields) {
-        int rc = zone_dim(ctx, &dim);
+        int rc = zone_dim(ctx, &E.dim);
         if (rc) return rc;
     }
     // TARGET_ENEMIES bins, one per distinct footprint range; building corners of every footprint a field will use
-    std::vector<enemy_bins> bins;
     std::map<std::pair<uint32_t, uint32_t>, int> bin_of;
-    std::vector<int32_t> req_bin(m, -1);
+    E.bins.clear();
+    E.req_bin.assign(m, -1);
     for (size_t i = 0; i < m; i++) {
         const pfnav_entity_field_req &q = reqs[i];
         if (q.chunk_n == 0) continue;
@@ -1035,24 +1084,27 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
         }
         auto it = bin_of.find({q.ent_off, q.ent_n});
         if (it == bin_of.end()) {
-            it = bin_of.emplace(std::make_pair(q.ent_off, q.ent_n), (int)bins.size()).first;
-            bins.emplace_back();
-            bin_enemies(ctx, ents, q.ent_off, q.ent_n, bins.back());
+            it = bin_of.emplace(std::make_pair(q.ent_off, q.ent_n), (int)E.bins.size()).first;
+            E.bins.emplace_back();
+            bin_enemies(ctx, ents, q.ent_off, q.ent_n, E.bins.back());
         }
-        req_bin[i] = it->second;
+        E.req_bin[i] = it->second;
         for (uint32_t k = 0; k < q.chunk_n; k++) {
             const int32_t *c = chunks_rc + 2 * ((size_t)q.chunk_off + k);
-            PF_ARG(!bins[it->second].bad[c[0] * cw + c[1]], "enemies field: a building corner lies outside the map");
+            PF_ARG(!E.bins[it->second].bad[c[0] * cw + c[1]], "enemies field: a building corner lies outside the map");
         }
     }
-    PF_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = pf_stream(ctx, stream);
-    PF_CUDA(pf_fields_join(ctx, st));
-    PF_CUDA(pf_pool_refresh(ctx, st));
-    // ---- slots request by request, in order: the serial calls' reservations and evictions
-    if (ctx->aux.size() < (size_t)ctx->pool_ndests) ctx->aux.resize(ctx->pool_ndests);
-    struct field_t { uint32_t req; int32_t cr, cc, slot; };
-    std::vector<field_t> fields;
+    return PFNAV_OK;
+}
+
+// Slots request by request, in order: the serial calls' reservations and evictions, and the footprints each destination
+// remembers. On an error, *out_done is the request that failed. fields == nullptr: a dry run that only reserves (the
+// caller undoes it with pf_pool_restore).
+static int entity_reserve(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m, const pfnav_footprint *ents,
+                          const int32_t *chunks_rc, std::vector<aux_field> *fields, size_t *out_done)
+{
+    const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
+    if (fields && ctx->aux.size() < (size_t)ctx->pool_ndests) ctx->aux.resize(ctx->pool_ndests);
     std::vector<size_t> keys;
     std::vector<int32_t> slots;
     int rc = PFNAV_OK;
@@ -1066,6 +1118,7 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
             bool evicted = false;
             if ((rc = pf_pool_reserve(ctx, keys.data(), q.chunk_n, slots.data(), &evicted))) break;
         }
+        if (!fields) continue;
         // the footprints stay with the destination: the in-place repairs of its fields start from them (field.c:2334-2360)
         pfnav_ctx::aux_target &A = ctx->aux[q.dest];
         A.kind = q.target_kind; A.layer = q.layer; A.ref_layer = q.ref_layer; A.ents.assign(ents + q.ent_off, ents + q.ent_off + q.ent_n);
@@ -1077,15 +1130,20 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
             fr.target_type = 2 + q.target_kind;      // beyond the chunk-local kinds: the frontier comes from ctx->aux[dest]
             fr._pad = q.dest;
             ctx->h_pool_req[slots[k]] = fr;
-            fields.push_back({(uint32_t)done, crc[2 * k], crc[2 * k + 1], slots[k]});
+            fields->push_back({(uint32_t)done, crc[2 * k], crc[2 * k + 1], slots[k]});
         }
     }
-    if (out_ndone) *out_ndone = (int)done;
-    if (fields.empty()) return rc;
-    ctx->goal_batch.valid = false;
-    // ---- the last field written to each slot, its footprints and their rasters
-    std::vector<int32_t> last(ctx->pool_max, -1);
-    for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
+    *out_done = done;
+    return rc;
+}
+
+// The fields F (each into block F[k].slot of d_out: the pool's flow fields, or a job's staging): their footprints,
+// rasters, seed bitmaps and integrations. upload_pool: the slot table and the `has` bytes travel in the same pinned
+// staging buffer and go to the device first.
+static int entity_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_field_req *reqs, const pfnav_footprint *ents,
+                        size_t nents, const entity_batch &E, const std::vector<aux_field> &F, bool upload_pool, uint8_t *d_out)
+{
+    const int cw = ctx->chunk_w, dim = E.dim;
     std::vector<pfnav_region_req> kreq;
     std::vector<int32_t> kslot, items, hitems, htiles;
     std::vector<uint32_t> item_off(1, 0), hitem_off(1, 0), htile_off(1, 0);
@@ -1094,13 +1152,13 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
     auto use = [&](uint32_t e, int rings) {
         int32_t &id = raster[(size_t)rings * nents + e];
         if (id == -1) {
-            const pfnav_footprint &E = ents[e];
-            if (footprint_on_device(E, rings)) {
+            const pfnav_footprint &P = ents[e];
+            if (footprint_on_device(P, rings)) {
                 id = (int32_t)jobs.size();
-                jobs.push_back({E.x, E.z, E.sel_radius, rings});
+                jobs.push_back({P.x, P.z, P.sel_radius, rings});
             } else {
                 int32_t tiles[512 * 2];
-                const int n = std::max(pfnav_footprint_tiles(ctx, &E, rings, tiles), 0);    // corners checked above
+                const int n = std::max(pfnav_footprint_tiles(ctx, &P, rings, tiles), 0);    // corners checked above
                 id = -2 - (int32_t)(htile_off.size() - 1);
                 htiles.insert(htiles.end(), tiles, tiles + 2 * n);
                 htile_off.push_back((uint32_t)(htiles.size() / 2));
@@ -1109,20 +1167,18 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
         if (id >= 0) items.push_back(id);
         else hitems.push_back(-2 - id);
     };
-    for (size_t f = 0; f < fields.size(); f++) {
-        const field_t &F = fields[f];
-        if (last[F.slot] != (int32_t)f) continue;
-        const pfnav_entity_field_req &q = reqs[F.req];
+    for (const aux_field &f : F) {
+        const pfnav_entity_field_req &q = reqs[f.req];
         const int rings = entity_rings(q.target_kind, q.ref_layer);
         if (q.target_kind == PFNAV_TARGET_ENTITY) use(q.ent_off, rings);
         else {
-            const enemy_bins &B = bins[req_bin[F.req]];
-            const int c = F.cr * cw + F.cc;
+            const enemy_bins &B = E.bins[E.req_bin[f.req]];
+            const int c = f.cr * cw + f.cc;
             for (uint32_t k = B.off[c]; k < B.off[c + 1]; k++) use(B.ent[k], rings);
         }
         pfnav_region_req rq = {};
-        rq.layer = q.layer; rq.center_r = F.cr; rq.center_c = F.cc; rq.flags = PFNAV_REGION_CREATE;
-        kreq.push_back(rq); kslot.push_back(F.slot);
+        rq.layer = q.layer; rq.center_r = f.cr; rq.center_c = f.cc; rq.flags = PFNAV_REGION_CREATE;
+        kreq.push_back(rq); kslot.push_back(f.slot);
         item_off.push_back((uint32_t)items.size()); hitem_off.push_back((uint32_t)hitems.size());
     }
     const size_t nk = kreq.size(), nj = jobs.size();
@@ -1133,12 +1189,14 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
     const size_t o_ioff = sec(item_off.size() * 4), o_items = sec(items.size() * 4);
     const size_t o_hoff = sec(hitem_off.size() * 4), o_hitems = sec(hitems.size() * 4);
     const size_t o_jobs = sec(nj * sizeof(fp_job)), o_toff = sec(htile_off.size() * 4), o_tiles = sec(htiles.size() * 4);
-    const size_t b_slot = ctx->h_pool_slot.size() * 4, stage = b_in + b_slot + (size_t)ctx->pool_max;
+    const size_t b_slot = upload_pool ? ctx->h_pool_slot.size() * 4 : 0, b_has = upload_pool ? (size_t)ctx->pool_max : 0;
+    const size_t stage = b_in + b_slot + b_has;
     const size_t o_org = b_in + 0, o_rows = o_org + ((nj * 8 + 15) & ~(size_t)15), o_bits = o_rows + nj * 128;
     const size_t need = o_bits + nk * ((size_t)dim * dim / 8);
     uint8_t *host = nullptr;
     int ri = 0;
-    if ((rc = pf_plan_host(ctx, stage, &host, &ri))) return rc;
+    int rc = pf_plan_host(ctx, stage, &host, &ri);
+    if (rc) return rc;
     memcpy(host + o_req, kreq.data(), nk * sizeof(pfnav_region_req));
     memcpy(host + o_slot, kslot.data(), nk * 4);
     memcpy(host + o_ioff, item_off.data(), item_off.size() * 4);
@@ -1148,14 +1206,18 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
     memcpy(host + o_jobs, jobs.data(), nj * sizeof(fp_job));
     memcpy(host + o_toff, htile_off.data(), htile_off.size() * 4);
     memcpy(host + o_tiles, htiles.data(), htiles.size() * 4);
-    memcpy(host + b_in, ctx->h_pool_slot.data(), b_slot);
-    memcpy(host + b_in + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
+    if (upload_pool) {
+        memcpy(host + b_in, ctx->h_pool_slot.data(), b_slot);
+        memcpy(host + b_in + b_slot, ctx->h_pool_has.data(), b_has);
+    }
     uint8_t *dev = nullptr;
     if ((rc = batch_scratch(ctx, st, need, &dev))) return rc;
     PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_in, b_slot, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_in + b_slot, ctx->pool_max,
-                            cudaMemcpyHostToDevice, st));
+    if (upload_pool) {
+        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_in, b_slot, cudaMemcpyHostToDevice, st));
+        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_in + b_slot, b_has,
+                                cudaMemcpyHostToDevice, st));
+    }
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
     const pfnav_region_req *d_req = (const pfnav_region_req *)(dev + o_req);
     int2 *d_org = (int2 *)(dev + o_org);
@@ -1172,11 +1234,151 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
                                                      (const uint32_t *)(dev + o_toff), (const int32_t *)(dev + o_tiles), d_bits);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
-    const int lrc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, ctx->d_pool_flow, st, 1, d_bits,
-                                  (const int32_t *)(dev + o_slot));
-    if (lrc) return lrc;
+    if ((rc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, d_out, st, 1, d_bits,
+                            (const int32_t *)(dev + o_slot))))
+        return rc;
     PF_CUDA(cudaEventRecord(ctx->ent_ev, st));
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                                      const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc,
+                                                      size_t nchunks, void *stream, int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    entity_batch E;
+    int rc = entity_validate(ctx, reqs, m, ents, nents, chunks_rc, nchunks, E);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    PF_CUDA(pf_fields_join(ctx, st));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    std::vector<aux_field> fields;
+    size_t done = 0;
+    rc = entity_reserve(ctx, reqs, m, ents, chunks_rc, &fields, &done);
+    if (out_ndone) *out_ndone = (int)done;
+    if (fields.empty()) return rc;
+    ctx->goal_batch.valid = false;
+    // ---- the last field written to each slot
+    std::vector<int32_t> last(ctx->pool_max, -1);
+    for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
+    std::vector<aux_field> build;
+    for (size_t f = 0; f < fields.size(); f++)
+        if (last[fields[f].slot] == (int32_t)f) build.push_back(fields[f]);
+    const int lrc = entity_build(ctx, st, reqs, ents, nents, E, build, true, ctx->d_pool_flow);
+    return lrc ? lrc : rc;
+}
+
+// ------------------------------------------------------------------------------------------
+// Zone and entity-field batches of a multi-GPU job (pfnav_mgpu_request_zones / pfnav_group_request_zones,
+// pfnav_mgpu_request_entity_fields_batch / pfnav_group_request_entity_fields_batch; the exchanges are in pfnav_mgpu.cu,
+// the owners and the staging layout in pfnav_plan.cu). A field of either batch depends on its request and the replicated
+// map only -- no LOS chains, no parents, no pool field read -- and neither batch skips a field the pool holds, so every
+// member writes the same keys with the same bytes, and the last request that names a key decides them. Each member
+// reserves exactly as its solo call does (zone_reserve / entity_reserve), so its slots, evictions, `has` bits, remembered
+// footprints and counts are the solo call's; the owner of a key builds it into staging with the solo call's build
+// (zone_build / entity_build, blocks as slots), and every member copies every key it holds at the end into its slot.
+// ------------------------------------------------------------------------------------------
+struct aux_job_batch { std::vector<int32_t> ctile; std::vector<uint8_t> on_map; entity_batch E; int dim = 0; };
+
+int pf_aux_job_plan(pfnav_ctx *ctx, pf_job &J)
+{
+    J.fits = true; J.nf = J.nl = 0;
+    J.lack.clear();
+    auto S = std::make_shared<aux_job_batch>();
+    const bool zones = J.kind == PF_JOB_ZONES;
+    int rc = zones ? zone_validate(ctx, J.zreqs, J.m, S->ctile, S->on_map, &S->dim)
+                   : entity_validate(ctx, J.ereqs, J.m, J.ents, J.nents, J.chunks_rc, J.nchunks, S->E);
+    if (rc) return rc;
+    if ((rc = pf_job_check_state(ctx))) return rc;
+    J.aux = S;
+    const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
+    if (zones) {        // the distinct keys without a slot, each a fresh slot from pool_used
+        std::vector<size_t> fresh;
+        for (size_t i = 0; i < J.m; i++) {
+            if (!S->on_map[i]) continue;
+            int ch[4];
+            zone_chunks(ctx, J.zreqs[i], &S->ctile[2 * i], ch);
+            for (int cr = ch[0]; cr <= ch[1]; cr++)
+                for (int cc = ch[2]; cc <= ch[3]; cc++) {
+                    const size_t si = (size_t)J.zreqs[i].dest * nch + cr * cw + cc;
+                    if (ctx->h_pool_slot[si] < 0) fresh.push_back(si);
+                }
+        }
+        std::sort(fresh.begin(), fresh.end());
+        J.fits = (size_t)(std::unique(fresh.begin(), fresh.end()) - fresh.begin()) <= (size_t)(ctx->pool_max - ctx->pool_used);
+        return PFNAV_OK;
+    }
+    // entity fields: the reservations with their evictions, undone
+    std::vector<size_t> keys;
+    for (size_t i = 0; i < J.m; i++) {
+        const pfnav_entity_field_req &q = J.ereqs[i];
+        for (uint32_t k = 0; k < q.chunk_n; k++) {
+            const int32_t *c = J.chunks_rc + 2 * ((size_t)q.chunk_off + k);
+            keys.push_back((size_t)q.dest * nch + c[0] * cw + c[1]);
+        }
+    }
+    pf_pool_saved saved;
+    pf_pool_save(ctx, std::move(keys), saved);
+    size_t done = 0;
+    rc = entity_reserve(ctx, J.ereqs, J.m, J.ents, J.chunks_rc, nullptr, &done);
+    pf_pool_restore(ctx, saved);
+    if (rc == PFNAV_ERR_NOMEM) { J.fits = false; rc = PFNAV_OK; }
     return rc;
+}
+
+int pf_aux_job_launch(pfnav_ctx *ctx, pf_job &J, int world, int rank, cudaStream_t st)
+{
+    const aux_job_batch &S = *(const aux_job_batch *)J.aux.get();
+    const bool zones = J.kind == PF_JOB_ZONES;
+    const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
+    ctx->job_built[0] = ctx->job_built[1] = 0;
+    J.nitems = 0; J.d_items = nullptr;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(pf_fields_join(ctx, st));
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    // ---- this member's own slots, exactly as its solo call reserves them (the dry run said they fit)
+    std::vector<aux_field> fields;
+    std::vector<int32_t> fresh;
+    size_t done = 0;
+    J.nfields.assign(J.m, 0);
+    int rc = zones ? zone_reserve(ctx, J.zreqs, J.m, S.ctile, S.on_map, fields, fresh, J.nfields.data(), &done)
+                   : entity_reserve(ctx, J.ereqs, J.m, J.ents, J.chunks_rc, &fields, &done);
+    if (rc) return rc;
+    if (!fields.empty()) ctx->goal_batch.valid = false;
+    // ---- owners and staging blocks: `fields` lists what the serial calls write, the same on every member
+    const size_t n = fields.size();
+    std::vector<int32_t> freq(n), blk;
+    std::vector<size_t> fkey(n);
+    std::vector<int64_t> fcost(n, 1);
+    for (size_t f = 0; f < n; f++) {
+        const aux_field &F = fields[f];
+        freq[f] = (int32_t)F.req;
+        fkey[f] = (size_t)(zones ? J.zreqs[F.req].dest : J.ereqs[F.req].dest) * nch + F.cr * cw + F.cc;
+        zone_job j;
+        if (zones) fcost[f] = (int64_t)zone_flood(J.zreqs[F.req], &S.ctile[2 * F.req], S.dim, F.cr, F.cc, &j);
+    }
+    pf_job_layout(ctx, J, freq, fkey, fcost, world, blk);
+    if (!J.seg[world]) return PFNAV_OK;
+    // ---- the member's copies (every written key it still holds) and the owner's builds (blocks in place of slots)
+    std::vector<pf_field_copy> items;
+    std::vector<aux_field> own;
+    for (size_t f = 0; f < n; f++) {
+        if (blk[f] < 0) continue;
+        const int32_t s = ctx->h_pool_slot[fkey[f]];
+        if (s >= 0) items.push_back({blk[f], s, 0});
+        if (ctx->job_owner[freq[f]] == rank) own.push_back({fields[f].req, fields[f].cr, fields[f].cc, blk[f]});
+    }
+    if ((rc = pf_job_stage(ctx, J, items, world, st))) return rc;
+    if (!own.empty()) {
+        rc = zones ? zone_build(ctx, st, J.zreqs, S.ctile, S.dim, own, std::vector<int32_t>(), false, ctx->d_job_stage)
+                   : entity_build(ctx, st, J.ereqs, J.ents, J.nents, S.E, own, false, ctx->d_job_stage);
+        if (rc) return rc;
+    }
+    ctx->job_built[0] = (int)own.size();
+    return PFNAV_OK;
 }
 
 extern "C" int pfnav_pool_request_entity_fields(pfnav_ctx *ctx, int dest, int layer, int ref_layer, int target_kind,
