@@ -45,6 +45,8 @@ struct PoolView {
     uint32_t *touch;         // [max] last tick that read the slot (LRU stamp), may be NULL
     uint32_t tick_no;
 };
+// touch == nullptr: the kernel stamps no slot
+static PoolView pool_view(const pf_pool &P, uint32_t *touch, uint32_t tick_no) { return {P.d_slot, P.d_flow, P.d_los, P.d_has, P.ndests, touch, tick_no}; }
 struct GridView {
     const uint32_t *cell_start, *cell_count;
     const int32_t *ix, *iy; const uint32_t *id;
@@ -964,87 +966,6 @@ void pfnav_agents_free(pfnav_ctx *ctx)
     ctx->cap_agents = ctx->cap_flocks = ctx->cap_cells = ctx->cap_work = 0;
 }
 
-// ---- field pool ----
-extern "C" int pfnav_pool_create(pfnav_ctx *ctx, int ndests, int max_fields)
-{
-    PF_ARG(ctx && ctx->d_cost, "map not created");
-    PF_NEED_DEVICE(ctx);
-    PF_ARG(ndests > 0 && max_fields > 0, "ndests/max_fields");
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(cudaDeviceSynchronize());
-    cudaFree(ctx->d_pool_slot); cudaFree(ctx->d_pool_flow); cudaFree(ctx->d_pool_los); cudaFree(ctx->d_pool_touch);
-    ctx->d_pool_slot = nullptr; ctx->d_pool_flow = nullptr; ctx->d_pool_los = nullptr; ctx->d_pool_touch = nullptr;
-    ctx->los_inflight = false;
-    const size_t nslots = (size_t)ndests * ctx->chunk_w * ctx->chunk_h;
-    PF_CUDA(cudaMalloc(&ctx->d_pool_slot, nslots * sizeof(int32_t)));
-    PF_CUDA(cudaMalloc(&ctx->d_pool_flow, (size_t)max_fields * 4096));
-    // LOS region carries a trailing `has` byte per slot
-    PF_CUDA(cudaMalloc(&ctx->d_pool_los, (size_t)max_fields * 4096 + max_fields));
-    PF_CUDA(cudaMemset(ctx->d_pool_slot, 0xFF, nslots * sizeof(int32_t)));
-    PF_CUDA(cudaMemset(ctx->d_pool_los + (size_t)max_fields * 4096, 0, max_fields));
-    PF_CUDA(cudaMalloc(&ctx->d_pool_touch, (size_t)max_fields * 4));
-    PF_CUDA(cudaMemset(ctx->d_pool_touch, 0, (size_t)max_fields * 4));
-    ctx->h_slot_touch.assign(max_fields, 0); ctx->h_slot_owner.assign(max_fields, -1); ctx->pool_free.clear();
-    ctx->h_pool_slot.assign(nslots, -1);
-    ctx->h_pool_has.assign(max_fields, 0);
-    ctx->h_pool_req.assign(max_fields, pfnav_field_req{});
-    ctx->h_pool_ffid.assign(nslots, 0);
-    ctx->pool_ndests = ndests; ctx->pool_max = max_fields; ctx->pool_used = 0;
-    ctx->goal_batch.valid = false; ctx->pool_dev_stale = false;
-    return PFNAV_OK;
-}
-
-extern "C" int pfnav_pool_clear(pfnav_ctx *ctx)
-{
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
-    // host mirrors only: the device copies are reset by the next entry point that uses the pool, on its stream
-    // (pf_pool_refresh), so the clear neither waits for the GPU nor races a tick still reading the slot table
-    pf_host_timer ht(ctx);
-    std::fill(ctx->h_pool_slot.begin(), ctx->h_pool_slot.end(), -1);
-    std::fill(ctx->h_pool_has.begin(), ctx->h_pool_has.end(), 0);
-    std::fill(ctx->h_pool_ffid.begin(), ctx->h_pool_ffid.end(), 0);
-    std::fill(ctx->h_slot_touch.begin(), ctx->h_slot_touch.end(), 0);
-    std::fill(ctx->h_slot_owner.begin(), ctx->h_slot_owner.end(), -1);
-    ctx->pool_free.clear();
-    ctx->goal_batch.valid = false;
-    ctx->pool_used = 0;
-    ctx->pool_dev_stale = true;
-    ht.lap(PF_HPROF_CLEAR);
-    return PFNAV_OK;
-}
-
-extern "C" int pfnav_pool_put(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, const uint8_t *flow_field,
-                              const uint8_t *los_field)
-{
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
-    PF_ARG(chunk_r >= 0 && chunk_r < ctx->chunk_h && chunk_c >= 0 && chunk_c < ctx->chunk_w, "chunk");
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_fields_sync(ctx));
-    PF_CUDA(pf_pool_refresh_sync(ctx));
-    const size_t si = (size_t)dest * ctx->chunk_w * ctx->chunk_h + chunk_r * ctx->chunk_w + chunk_c;
-    int32_t slot = ctx->h_pool_slot[si];
-    uint8_t *d_has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096;
-    if (slot < 0) {
-        bool evicted = false;
-        int rc = pf_pool_reserve(ctx, &si, 1, &slot, &evicted);
-        if (rc) return rc;
-        if (evicted) {
-            PF_CUDA(cudaMemcpy(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice));
-            PF_CUDA(cudaMemcpy(d_has, ctx->h_pool_has.data(), ctx->pool_max, cudaMemcpyHostToDevice));
-        } else {
-            PF_CUDA(cudaMemcpy(ctx->d_pool_slot + si, &slot, sizeof(int32_t), cudaMemcpyHostToDevice));
-        }
-    }
-    uint8_t has = ctx->h_pool_has[slot];
-    if (flow_field) { PF_CUDA(cudaMemcpy(ctx->d_pool_flow + (size_t)slot * 4096, flow_field, 4096, cudaMemcpyHostToDevice)); has |= 1; }
-    if (los_field) { PF_CUDA(cudaMemcpy(ctx->d_pool_los + (size_t)slot * 4096, los_field, 4096, cudaMemcpyHostToDevice)); has |= 2; }
-    ctx->h_pool_has[slot] = has;
-    PF_CUDA(cudaMemcpy(d_has + slot, &has, 1, cudaMemcpyHostToDevice));
-    ctx->goal_batch.valid = false;
-    return PFNAV_OK;
-}
-
 // ---- agents ----
 template <typename T>
 static int ensure(T *&p, size_t &cap, size_t need)
@@ -1470,12 +1391,9 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
     {
     pf_prof_scope prof(ctx, st, PF_PROF_VDES);
     if (flags & PFNAV_TICK_VDES_FROM_POOL) {
-        PF_ARG(ctx->d_pool_slot, "PFNAV_TICK_VDES_FROM_POOL needs a field pool");
+        PF_ARG(ctx->pool.d_slot, "PFNAV_TICK_VDES_FROM_POOL needs a field pool");
         PF_CUDA(pf_pool_refresh(ctx, st));
-        PoolView pv;
-        pv.slot = ctx->d_pool_slot; pv.flow = ctx->d_pool_flow; pv.los = ctx->d_pool_los;
-        pv.has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096; pv.ndests = ctx->pool_ndests;
-        pv.touch = ctx->d_pool_touch; pv.tick_no = ctx->tick_no;
+        const PoolView pv = pool_view(ctx->pool, ctx->pool.d_touch, ctx->tick_no);
         k_desired_velocity<<<(nwork + 127) / 128, 128, 0, st>>>(m, pv, ctx->d_agents, ctx->d_flocks, ctx->d_work, nwork,
                                                                ctx->d_vdes_out, ctx->d_los_out, ctx->d_work_count,
                                                                ctx->d_ms_ext, ctx->d_formation);
@@ -2439,7 +2357,7 @@ __global__ void k_collect_misses(MapView m, PoolView pool, const uint16_t *__res
 // reference would have found served by an earlier entity's request does not request again.
 extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nrepairs)
 {
-    PF_ARG(ctx && ctx->d_agents && ctx->d_pool_slot, "agents / pool missing");
+    PF_ARG(ctx && ctx->d_agents && ctx->pool.d_slot, "agents / pool missing");
     if (out_nrequests) *out_nrequests = 0;
     if (out_nrepairs) *out_nrepairs = 0;
     if (ctx->n_work == 0) return PFNAV_OK;
@@ -2456,15 +2374,12 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     MapView m;
     m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
     m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
-    std::vector<int> flock_of_dest(ctx->pool_ndests, -1);
+    std::vector<int> flock_of_dest(ctx->pool.ndests, -1);
     for (size_t f = 0; f < ctx->h_flocks.size(); f++)
-        if (ctx->h_flocks[f].dest >= 0 && ctx->h_flocks[f].dest < ctx->pool_ndests) flock_of_dest[ctx->h_flocks[f].dest] = (int)f;
+        if (ctx->h_flocks[f].dest >= 0 && ctx->h_flocks[f].dest < ctx->pool.ndests) flock_of_dest[ctx->h_flocks[f].dest] = (int)f;
     int nreq = 0, nrep = 0, rc = 0;
     auto collect = [&](int kind, std::vector<pf_miss> &reps) -> int {
-        PoolView pv;
-        pv.slot = ctx->d_pool_slot; pv.flow = ctx->d_pool_flow; pv.los = ctx->d_pool_los;
-        pv.has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096; pv.ndests = ctx->pool_ndests;
-        pv.touch = nullptr; pv.tick_no = 0;
+        const PoolView pv = pool_view(ctx->pool, nullptr, 0);
         PF_CUDA(cudaMemsetAsync(d_cnt, 0, 4, st));
         k_collect_misses<<<(nwork + 127) / 128, 128, 0, st>>>(m, pv, ctx->d_liid, ctx->d_agents, ctx->d_flocks, ctx->d_work, nwork,
                                                              kind, d_miss, d_cnt, (uint32_t)nwork, ctx->d_ms_ext, ctx->nlayers);
@@ -2501,8 +2416,7 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     // ---- LOS state (N_HasDestLOS, nav.c:4038-4045) ----
     if (!(rc = collect(0, reps))) {
         for (const pf_miss &r : reps) {
-            const int slot = ctx->h_pool_slot[(size_t)r.dest * chunks + r.chunk];
-            if (slot >= 0 && (ctx->h_pool_has[slot] & 2)) continue;          // an earlier entity's request built it
+            if (ctx->pool.has_of((size_t)r.dest * chunks + r.chunk) & 2) continue;          // an earlier entity's request built it
             int ok;
             if ((rc = request_from(r, &ok))) break;
         }
@@ -2511,12 +2425,12 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     if (!rc && !(rc = collect(1, reps))) {
         for (const pf_miss &r : reps) {
             auto dir_now = [&](int *dir) -> int {          // the tile's direction as the pool holds it right now, -1 = no field
-                const int slot = ctx->h_pool_slot[(size_t)r.dest * chunks + r.chunk];
+                const int slot = ctx->pool.slot[(size_t)r.dest * chunks + r.chunk];
                 *dir = -1;
-                if (slot < 0 || !(ctx->h_pool_has[slot] & 1)) return 0;
+                if (slot < 0 || !(ctx->pool.has[slot] & 1)) return 0;
                 uint8_t d = 0;
                 PF_CUDA(cudaDeviceSynchronize());
-                PF_CUDA(cudaMemcpy(&d, ctx->d_pool_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost));
+                PF_CUDA(cudaMemcpy(&d, ctx->pool.d_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost));
                 *dir = d & 0xF;
                 return 0;
             };
@@ -2528,8 +2442,8 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
             if (!ok) continue;                                            // no path from here: zero vector, nothing repaired (nav.c:3501)
             if ((rc = dir_now(&dir))) break;
             if (dir != 0) continue;                                       // case 1: the path query fixed it (or no field: no path)
-            const int slot = ctx->h_pool_slot[(size_t)r.dest * chunks + r.chunk];
-            const pfnav_field_req tg = ctx->h_pool_req[slot];
+            const int slot = ctx->pool.slot[(size_t)r.dest * chunks + r.chunk];
+            const pfnav_field_req tg = ctx->pool.req[slot];
             int32_t kind, arg;
             if (r.liid == 0xFFFF) { kind = PFNAV_REPAIR_NEAREST_PATHABLE; arg = ((r.tile >> 6) << 8) | (r.tile & 63); }
             else                  { kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; arg = r.liid; }
@@ -2541,14 +2455,14 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     // ---- enemy-seek / surround fields: in-place repairs only (nav.c:3647-3675, 3729-3757) ----
     if (!rc && !(rc = collect(2, reps))) {
         for (const pf_miss &r : reps) {
-            const int slot = ctx->h_pool_slot[(size_t)r.dest * chunks + r.chunk];
-            if (slot < 0 || !(ctx->h_pool_has[slot] & 1)) continue;
+            const int slot = ctx->pool.slot[(size_t)r.dest * chunks + r.chunk];
+            if (slot < 0 || !(ctx->pool.has[slot] & 1)) continue;
             uint8_t d = 0;
             if (cudaDeviceSynchronize() != cudaSuccess ||
-                cudaMemcpy(&d, ctx->d_pool_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost) != cudaSuccess) {
+                cudaMemcpy(&d, ctx->pool.d_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost) != cudaSuccess) {
                 pfnav_set_error("pfnav_pool_repair: read-back failed"); rc = PFNAV_ERR_CUDA; break;
             }
-            const pfnav_field_req tg = ctx->h_pool_req[slot];
+            const pfnav_field_req tg = ctx->pool.req[slot];
             if ((tg.target_type & 0xFF) < 2) continue;
             const bool surround = (tg.target_type & 0xFF) == 2 + PFNAV_TARGET_ENTITY;
             int32_t kind, arg;
@@ -2656,7 +2570,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
 {
     PF_ARG(ctx, "ctx");
     PF_NEED_DEVICE(ctx);
-    PF_ARG(ctx->d_agents && ctx->d_pool_slot, "agents / pool missing");
+    PF_ARG(ctx->d_agents && ctx->pool.d_slot, "agents / pool missing");
     int *stats = ctx->repair_stats;           // pfnav_pool_repair_batch_stats
     for (int k = 0; k < 6; k++) stats[k] = 0;
     if (out_nrequests) *out_nrequests = 0;
@@ -2693,16 +2607,13 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
     MapView m;
     m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
     m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
-    std::vector<int> flock_of_dest(ctx->pool_ndests, -1);
+    std::vector<int> flock_of_dest(ctx->pool.ndests, -1);
     for (size_t f = 0; f < ctx->h_flocks.size(); f++)
-        if (ctx->h_flocks[f].dest >= 0 && ctx->h_flocks[f].dest < ctx->pool_ndests) flock_of_dest[ctx->h_flocks[f].dest] = (int)f;
+        if (ctx->h_flocks[f].dest >= 0 && ctx->h_flocks[f].dest < ctx->pool.ndests) flock_of_dest[ctx->h_flocks[f].dest] = (int)f;
     int nreq = 0, nrounds = 0;
     // the misses of one phase, one per key, first in work order, read back in work order
     auto collect = [&](int kind, std::vector<pf_miss> &reps) -> int {
-        PoolView pv;
-        pv.slot = ctx->d_pool_slot; pv.flow = ctx->d_pool_flow; pv.los = ctx->d_pool_los;
-        pv.has = ctx->d_pool_los + (size_t)ctx->pool_max * 4096; pv.ndests = ctx->pool_ndests;
-        pv.touch = nullptr; pv.tick_no = 0;
+        const PoolView pv = pool_view(ctx->pool, nullptr, 0);
         PF_CUDA(cudaMemsetAsync(d_cnt, 0, 8, st));
         PF_CUDA(cudaMemsetAsync(d_flag, 0, (size_t)nwork * 4, st));
         PF_CUDA(cudaMemsetAsync(d_hkey, 0xFF, (size_t)cap * 8, st));
@@ -2727,7 +2638,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
         return 0;
     };
     auto key_of = [&](const pf_miss &r) { return (size_t)r.dest * chunks + r.chunk; };
-    auto has_flow = [&](int slot) { return slot >= 0 && (ctx->h_pool_has[slot] & 1); };
+    auto has_flow = [&](int slot) { return slot >= 0 && (ctx->pool.has[slot] & 1); };
     // the path requests of a phase's representatives, planned up front (flock target, flock layer)
     auto plan = [&](const std::vector<pf_miss> &reps, pf_path_batch **out) -> int {
         const size_t n = reps.size();
@@ -2755,8 +2666,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
         batch_ptr B(pb, pf_path_batch_end);
         bool any = false;
         for (size_t i = 0; i < reps.size() && !rc; i++) {
-            const int slot = ctx->h_pool_slot[key_of(reps[i])];
-            if (slot >= 0 && (ctx->h_pool_has[slot] & 2)) continue;
+            if (ctx->pool.has_of(key_of(reps[i])) & 2) continue;
             if (flock_of_dest[reps[i].dest] < 0) continue;
             if ((rc = pf_path_batch_probe(pb, (int)i, &pr))) break;    // PFNAV_ERR_ARG, as pfnav_pool_request_path's
             if (pr.nf + pr.nl == 0) continue;
@@ -2778,7 +2688,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
         // what each representative's tile holds at the start of the round: its slot then, and the direction byte
         std::vector<int32_t> slot0(n);
         std::vector<uint8_t> dir0(n, 0);
-        std::vector<uint8_t> written(ctx->pool_max, 0), chained(ctx->pool_max, 0);
+        std::vector<uint8_t> written(ctx->pool.max, 0), chained(ctx->pool.max, 0);
         std::vector<int32_t> touched;                     // slots marked in written / chained this round
         std::vector<pf_chain_item> items;
         std::vector<uint64_t> masks;
@@ -2789,14 +2699,14 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
         auto gather = [&](size_t from) -> int {
             gin.clear();
             for (size_t k = from; k < n; k++) {
-                const int s = ctx->h_pool_slot[key_of(reps[k])];
+                const int s = ctx->pool.slot[key_of(reps[k])];
                 slot0[k] = has_flow(s) ? s : -1;
                 gin.push_back(make_int2(slot0[k], reps[k].tile));
             }
             if (gin.empty()) return 0;
             gout.resize(gin.size());
             PF_CUDA(cudaMemcpyAsync(d_gin, gin.data(), gin.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
-            k_repair_gather<<<((unsigned)gin.size() + 127) / 128, 128, 0, st>>>(d_gin, (int)gin.size(), ctx->d_pool_flow, d_gout);
+            k_repair_gather<<<((unsigned)gin.size() + 127) / 128, 128, 0, st>>>(d_gin, (int)gin.size(), ctx->pool.d_flow, d_gout);
             ctx->launches++;
             PF_CUDA(cudaGetLastError());
             PF_CUDA(cudaMemcpyAsync(gout.data(), d_gout, gout.size(), cudaMemcpyDeviceToHost, st));
@@ -2824,7 +2734,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
             const size_t key = key_of(r);
             if (flock_of_dest[r.dest] < 0) { i++; continue; }       // no request, no repair (nav.c:3501)
             // step a of the serial loop: the tile's direction before the request, if the host knows it
-            const int s = ctx->h_pool_slot[key];
+            const int s = ctx->pool.slot[key];
             int dir = -1;                                            // -1: no flow field
             bool known = true;
             if (has_flow(s)) {
@@ -2854,10 +2764,10 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
                 for (int32_t ws : wslots) mark(written, ws);
             } else if (known && dir > 0) { i++; continue; }
             if (!pr.ok) { i++; continue; }                           // no path from here: zero vector, nothing repaired
-            const int sl = ctx->h_pool_slot[key];
+            const int sl = ctx->pool.slot[key];
             if (!has_flow(sl)) { i++; continue; }                    // no field: nothing to repair
             pf_chain_item it;
-            it.q = ctx->h_pool_req[sl]; it.slot = sl; it.tile = r.tile; it.always = 0; it.mask = -1;
+            it.q = ctx->pool.req[sl]; it.slot = sl; it.tile = r.tile; it.always = 0; it.mask = -1;
             if (r.liid == 0xFFFF) { it.kind = PFNAV_REPAIR_NEAREST_PATHABLE; it.arg = ((r.tile >> 6) << 8) | (r.tile & 63); }
             else                  { it.kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; it.arg = r.liid; }
             std::vector<uint64_t> mask(64);
@@ -2894,9 +2804,9 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
         std::vector<uint64_t> masks;
         for (size_t i = 0; i < reps.size(); i++) {
             const pf_miss &r = reps[i];
-            const int slot = ctx->h_pool_slot[key_of(r)];
+            const int slot = ctx->pool.slot[key_of(r)];
             if (!has_flow(slot)) continue;
-            const pfnav_field_req tg = ctx->h_pool_req[slot];
+            const pfnav_field_req tg = ctx->pool.req[slot];
             if ((tg.target_type & 0xFF) < 2) continue;
             const bool surround = (tg.target_type & 0xFF) == 2 + PFNAV_TARGET_ENTITY;
             pf_chain_item it;
@@ -2912,7 +2822,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
                 if (!items.empty()) nrounds++;
                 items.clear(); masks.clear();
                 uint8_t d = 0;
-                PF_CUDA(cudaMemcpyAsync(&d, ctx->d_pool_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost, st));
+                PF_CUDA(cudaMemcpyAsync(&d, ctx->pool.d_flow + (size_t)slot * 4096 + r.tile, 1, cudaMemcpyDeviceToHost, st));
                 PF_CUDA(cudaStreamSynchronize(st));
                 if (it.always || (d & 0xF) == 0) { rc = src; break; }
                 continue;

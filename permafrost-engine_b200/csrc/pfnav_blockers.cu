@@ -909,35 +909,21 @@ extern "C" int pfnav_map_commit(pfnav_ctx *ctx, int *out_ndirty)
             }
             const int flipped = pfnav_route_refresh_edges(ctx, layer, chunk);
             nd++;
-            if (!ctx->h_pool_slot.empty()) {
-                for (int d = 0; d < ctx->pool_ndests; d++) {
-                    const size_t si = (size_t)d * chunks + chunk;
-                    const int slot = ctx->h_pool_slot[si];
-                    if (slot < 0 || !ctx->h_pool_has[slot]) continue;
-                    pool_touched = true;
-                    if (flipped > 0) {
-                        // N_FC_InvalidateAllThroughChunk: the whole path of this destination goes
-                        for (int c2 = 0; c2 < chunks; c2++) {
-                            const int s2 = ctx->h_pool_slot[(size_t)d * chunks + c2];
-                            if (s2 >= 0) ctx->h_pool_has[s2] = 0;
-                            ctx->h_pool_ffid[(size_t)d * chunks + c2] = 0;
-                        }
-                    } else {
-                        ctx->h_pool_has[slot] = 0;
-                        ctx->h_pool_ffid[si] = 0;
-                    }
-                }
+            for (int d = 0; d < ctx->pool.ndests; d++) {
+                if (!ctx->pool.has_of((size_t)d * chunks + chunk)) continue;
+                pool_touched = true;
+                if (flipped <= 0) pf_pool_drop(ctx, d, chunk);
+                else for (int c = 0; c < chunks; c++) pf_pool_drop(ctx, d, c);   // N_FC_InvalidateAllThroughChunk: the whole path goes
             }
         }
         ctx->dirty.clear();
-        ctx->map_epoch++;
+        ctx->map_epoch++;          // the resident goal plan is not relaunched on a changed map
         if (pool_touched && ctx->device >= 0) {
             PF_CUDA(cudaSetDevice(ctx->device));
             PF_CUDA(cudaDeviceSynchronize());     // a tick on a non-blocking stream may still read the flags
-            PF_CUDA(cudaMemcpy(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
+            PF_CUDA(cudaMemcpy(ctx->pool.d_has, ctx->pool.has.data(), ctx->pool.max,
                                cudaMemcpyHostToDevice));
         }
-        ctx->goal_batch.valid = false;
     }
     if (out_ndirty) *out_ndirty = nd;
     return PFNAV_OK;

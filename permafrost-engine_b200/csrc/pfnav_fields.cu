@@ -803,7 +803,7 @@ int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
     k_repair_chain<<<(unsigned)std::min(ngroups, ctx->sm_count * 8), FLOWG_THREADS, 0, st>>>(
         grids_of(ctx), (const pf_chain_item *)dev, (const int32_t *)(dev + a_off), ngroups, (const uint64_t *)(dev + a_mask),
-        ctx->d_pool_flow, d_count);
+        ctx->pool.d_flow, d_count);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
     return PFNAV_OK;
@@ -1264,8 +1264,7 @@ void pfnav_fields_free(pfnav_ctx *ctx)
     cudaFree(ctx->d_stage); ctx->d_stage = nullptr;
     cudaFree(ctx->d_los_sched); ctx->d_los_sched = nullptr; ctx->los_sched_bytes = 0;
     cudaFree(ctx->d_los_trace); ctx->d_los_trace = nullptr; ctx->los_trace_cap = 0;
-    cudaFree(ctx->d_pool_slot); cudaFree(ctx->d_pool_flow); cudaFree(ctx->d_pool_los); cudaFree(ctx->d_pool_touch);
-    ctx->d_pool_slot = nullptr; ctx->d_pool_flow = nullptr; ctx->d_pool_los = nullptr; ctx->d_pool_touch = nullptr;
+    pf_pool_free(ctx);
     if (ctx->ev_los_sched) { cudaEventDestroy(ctx->ev_los_sched); ctx->ev_los_sched = nullptr; }
 }
 
@@ -1367,16 +1366,8 @@ extern "C" int pfnav_map_create(pfnav_ctx *ctx, int chunk_w, int chunk_h, int nl
     pfnav_blockers_forget(ctx);
     ctx->h_fac.clear(); ctx->h_fmask.clear();
     // the field pool is sized ndests x (chunks of the OLD map): it does not carry over either
-    if (ctx->device >= 0 && ctx->d_pool_slot) {
-        PF_CUDA(cudaSetDevice(ctx->device));
-        PF_CUDA(cudaDeviceSynchronize());
-        cudaFree(ctx->d_pool_slot); cudaFree(ctx->d_pool_flow); cudaFree(ctx->d_pool_los); cudaFree(ctx->d_pool_touch);
-        ctx->d_pool_slot = nullptr; ctx->d_pool_flow = nullptr; ctx->d_pool_los = nullptr; ctx->d_pool_touch = nullptr;
-    }
-    ctx->pool_ndests = 0; ctx->pool_max = 0; ctx->pool_used = 0;
-    ctx->h_pool_slot.clear(); ctx->h_pool_has.clear(); ctx->h_pool_req.clear(); ctx->h_pool_ffid.clear();
-    ctx->h_slot_owner.clear(); ctx->h_slot_touch.clear(); ctx->pool_free.clear(); ctx->aux.clear();
-    ctx->goal_batch.valid = false;
+    if (int rc = pf_pool_free(ctx)) return rc;
+    ctx->aux.clear();
     ctx->chunk_w = chunk_w; ctx->chunk_h = chunk_h; ctx->nlayers = nlayers;
     ctx->W64 = chunk_w * 64; ctx->H64 = chunk_h * 64;
     ctx->map_x = map_x; ctx->map_z = map_z;
@@ -1838,7 +1829,7 @@ int pfnav_flow_repair_pool(pfnav_ctx *ctx, const pfnav_field_req *targets, const
     if (e == cudaSuccess) {
         // one CTA per request, serialised per slot by launching requests that share a slot one after another
         k_flow_repair<<<1, FLOWG_THREADS, 0, st>>>(grids_of(ctx), (const pfnav_field_req *)d_req, (const int32_t *)d_kind,
-                                                  (const uint64_t *)d_mask, (int)n, ctx->d_pool_flow, (const int32_t *)d_slot);
+                                                  (const uint64_t *)d_mask, (int)n, ctx->pool.d_flow, (const int32_t *)d_slot);
         ctx->launches++;
         e = cudaGetLastError();
     }

@@ -11,10 +11,9 @@
 #include <utility>
 #include <vector>
 #include "../../include/pfnav.h"
+#include "pfnav_pool_host.h"
 
 #define PFNAV_VERSION 100
-
-void pfnav_set_error(const char *fmt, ...);
 
 #define PF_CUDA(call)                                                                       \
     do {                                                                                    \
@@ -96,13 +95,8 @@ struct pfnav_ctx {
     std::set<std::pair<int, int>> dirty, fdirty;               // pfnav_blockers.cu: (layer, chunk) occupancy / faction mask changed
     void *blk_state = nullptr;                                 // pfnav_blockers.cu: queued blocker ops + device-side refcount state
 
-    // ---- field pool ----
-    int pool_ndests = 0, pool_max = 0, pool_used = 0;
-    int32_t *d_pool_slot = nullptr;   // [ndests][chunks] -> slot or -1
-    std::vector<int32_t> h_pool_slot;
-    std::vector<uint8_t> h_pool_has;
-    std::vector<pfnav_field_req> h_pool_req;   // [slot]: the last request applied to the slot (== flow_field::target, field.c:2076)
-    std::vector<uint64_t> h_pool_ffid;     // [ndests][chunks]: ff_id currently mapped (dest, chunk) -> field, 0 = none
+    // ---- field pool (pfnav_pool.cu, pfnav_pool_host.h) ----
+    pf_pool pool;
     void *d_plan_buf = nullptr; size_t plan_buf_bytes = 0;    // request staging for pfnav_pool_request_goal
     // The plan of the last goal batch stays resident on the device: re-requesting the same goals on an
     // unchanged map (map_epoch) relaunches the kernels without re-planning or re-uploading anything.
@@ -111,16 +105,7 @@ struct pfnav_ctx {
         bool valid = false; uint64_t epoch = 0; int layer = 0; std::vector<int32_t> dests, targets;
         int nf = 0, nl = 0; std::vector<int32_t> fwave_off; size_t b_fr = 0, b_fs = 0, b_lr = 0, b_ls = 0;
     } goal_batch;
-    uint8_t *d_pool_flow = nullptr;   // [max][4096]
-    uint8_t *d_pool_los = nullptr;    // [max][4096]
-    // LRU eviction (fieldcache.c:59-71 keeps CONFIG_*_CACHE_SZ entries per LRU cache): every slot remembers the last
-    // tick that read it (device side, written by the desired-velocity kernels) or requested it (host side)
-    uint32_t *d_pool_touch = nullptr;             // [max] last tick number a work item read the slot
-    std::vector<uint32_t> h_slot_touch;           // [max] last tick number a request named the slot
-    std::vector<int64_t>  h_slot_owner;           // [max] dest * chunks + chunk, or -1 (free)
-    std::vector<int32_t>  pool_free;              // evicted slots, reused before pool_used grows
     uint32_t tick_no = 1;                         // advanced by pfnav_agents_tick
-    uint64_t pool_evictions = 0;
     // TARGET_ENEMIES / TARGET_ENTITY destinations (pfnav_pool_request_entity_fields): what their repairs start from
     struct aux_target { int kind = -1, layer = 0, ref_layer = 0; std::vector<pfnav_footprint> ents; };
     std::vector<aux_target> aux;
@@ -190,9 +175,6 @@ struct pfnav_ctx {
     bool vel_timed = false; float last_los_ms = -1.0f, last_vel_ms = -1.0f;
     bool los_inflight = false;
 
-    // pfnav_pool_clear resets the host mirrors only; the device slot table, `has` bytes and touch stamps are reset
-    // by the next entry point that uses the pool, ordered on its stream (pf_pool_refresh)
-    bool pool_dev_stale = false;
     // cold goal batches: the plan is staged in a ring of two pinned buffers (event-guarded reuse) and the goals are
     // planned on a persistent host thread pool with per-goal scratch (pfnav_plan.cu)
     void *plan_host[2] = {nullptr, nullptr}; size_t plan_host_bytes[2] = {0, 0};
@@ -247,27 +229,6 @@ static inline cudaError_t pf_fields_sync(pfnav_ctx *ctx)
     if (e == cudaSuccess) ctx->los_inflight = false;
     return e;
 }
-// Bring the device copies of the pool up to date after pfnav_pool_clear: empty slot table, no `has` bytes, zero touch
-// stamps, ordered on `st` after the forked field work (which may still write the pool). Every entry point that reads
-// or writes the device pool calls this first, on the stream it runs on.
-static inline cudaError_t pf_pool_refresh(pfnav_ctx *ctx, cudaStream_t st)
-{
-    if (!ctx->pool_dev_stale) return cudaSuccess;
-    cudaError_t e = pf_fields_join(ctx, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_pool_slot, 0xFF, ctx->h_pool_slot.size() * sizeof(int32_t), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, 0, ctx->pool_max, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_pool_touch, 0, (size_t)ctx->pool_max * 4, st);
-    if (e == cudaSuccess) ctx->pool_dev_stale = false;
-    return e;
-}
-// the same for entry points that go on with blocking copies (legacy default stream): wait for the reset
-static inline cudaError_t pf_pool_refresh_sync(pfnav_ctx *ctx)
-{
-    if (!ctx->pool_dev_stale) return cudaSuccess;
-    cudaError_t e = pf_pool_refresh(ctx, ctx->tick_stream);
-    return e == cudaSuccess ? cudaStreamSynchronize(ctx->tick_stream) : e;
-}
-
 // per (flock, layer) constants of arrived() (movement.c:2170), see pfnav_route.cu
 #define PF_ARRIVAL_MC_MAX 256           /* FIELD_RES_R*2 + FIELD_RES_C*2 (nav.c:4721) */
 struct pf_arrival_consts {
@@ -348,8 +309,19 @@ __host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(rang
 
 int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, std::vector<int> &out);     // pfnav_region.cu
 
-// pool slots with LRU eviction (pfnav_plan.cu)
+// ---- pfnav_pool.cu: the device pool, and the pool mutators of a context, each of which drops the resident goal plan
+// Bring the device copies of the pool up to date after pfnav_pool_clear: empty slot table, no `has` bytes, zero touch
+// stamps, ordered on `st` after the forked field work (which may still write the pool). Every entry point that reads
+// or writes the device pool calls this first, on the stream it runs on.
+cudaError_t pf_pool_refresh(pfnav_ctx *ctx, cudaStream_t st);
+int pf_pool_free(pfnav_ctx *ctx);                          // forget every slot: pfnav_destroy, pfnav_map_create, pfnav_pool_create
+// pfnav_pool_host.h's reservation, with the device's touch stamps when it must evict
 int pf_pool_reserve(pfnav_ctx *ctx, const size_t *keys, size_t n, int32_t *slots_out, bool *out_evicted);
+int32_t pf_pool_zone_take(pfnav_ctx *ctx, size_t key);     // the zone rule: the key's slot, -1 when the pool is full
+void pf_pool_drop(pfnav_ctx *ctx, int dest, int chunk);    // pfnav_map_commit: the map changed under the key's fields
+// copy the slot table and the `has` bytes into `host` (pinned, pool.table_bytes() long) and enqueue their two copies to
+// the device on `st`; the caller records the event that guards the reuse of `host` after them
+int pf_pool_stage_table(pfnav_ctx *ctx, uint8_t *host, cudaStream_t st);
 void pf_planner_destroy(pfnav_ctx *ctx);                         // pfnav_plan.cu: join the goal planner threads
 // the next of the two pinned staging buffers (plan_host), at least `bytes` long, once the copy that last read it is done;
 // record plan_host_ev[*out_ri] after the copies from it (pfnav_plan.cu)
@@ -367,9 +339,10 @@ int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri);
 //   pf_job_scatter (after the exchange of the segments) copies every field the member lacks from the staging buffer
 //                 into its pool slot, on `st`, and makes the next pool reader wait for it.
 // Zone and entity-field batches (kind PF_JOB_ZONES / PF_JOB_ENTITY) take the same three steps: pf_job_plan validates
-// and dry-runs the member's reservation (pf_aux_job_plan, pfnav_region.cu; no lack record: every member writes every key
-// the arguments name), pf_job_launch reserves, lays out the owners' fields (pf_job_layout) and builds the member's own
-// (pf_aux_job_launch), pf_job_scatter copies.
+// and takes the verdict of the member's reservation (pf_aux_job_plan, pfnav_region.cu: pf_pool_zone_fits, or
+// pf_pool_fits of each request; no lack record: every member writes every key the arguments name), pf_job_launch
+// reserves, lays out the owners' fields (pf_job_layout) and builds the member's own (pf_aux_job_launch), pf_job_scatter
+// copies.
 enum { PF_JOB_GOALS = 0, PF_JOB_ZONES = 1, PF_JOB_ENTITY = 2 };
 struct pf_job {
     int kind = PF_JOB_GOALS;
@@ -404,15 +377,6 @@ struct pf_field_copy { int32_t src, dst, kind; };
 void pf_job_layout(pfnav_ctx *ctx, pf_job &J, const std::vector<int32_t> &freq, const std::vector<size_t> &fkey,
                    const std::vector<int64_t> &fcost, int world, std::vector<int32_t> &blk);
 int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &items, int world, cudaStream_t st);
-// the host pool state pf_pool_reserve can change for a batch naming `keys`: saved before a dry run, restored after it
-struct pf_pool_saved {
-    std::vector<size_t> keys; std::vector<int32_t> kslot, free_slots; std::vector<int64_t> owner;
-    std::vector<uint64_t> ffid; std::vector<uint8_t> has; std::vector<uint32_t> touch;
-    int used = 0; uint64_t evictions = 0; bool gb_valid = false;
-};
-void pf_pool_save(const pfnav_ctx *ctx, std::vector<size_t> keys, pf_pool_saved &S);
-void pf_pool_restore(pfnav_ctx *ctx, const pf_pool_saved &S);
-
 enum { PF_PROF_FLOW = 0, PF_PROF_LOS = 1, PF_PROF_INDEX = 2, PF_PROF_VDES = 3, PF_PROF_COHESION = 4,
        PF_PROF_VELOCITY = 5, PF_PROF_UPDATE = 6, PF_PROF_APPLY = 7, PF_PROF_SLOTS = 8 };
 

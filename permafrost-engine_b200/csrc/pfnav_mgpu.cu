@@ -497,7 +497,7 @@ static int nccl_member(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_
         pfnav_set_error("%s: member of an in-process group: %s", fn, group_fn);
         return PFNAV_ERR_STATE;
     }
-    PF_ARG(ctx->d_pool_slot, "pool not created");
+    PF_ARG(ctx->pool.d_slot, "pool not created");
     *out = m;
     return PFNAV_OK;
 }
@@ -573,8 +573,8 @@ static int group_members(pfnav_group *g, const char *fn)
     const pfnav_ctx *c0 = g->ctxs[0];
     for (int i = 0; i < world; i++) {
         const pfnav_ctx *c = g->ctxs[i];
-        PF_ARG(c->d_pool_slot, "pool not created");
-        PF_ARG(c->chunk_w == c0->chunk_w && c->chunk_h == c0->chunk_h && c->pool_ndests == c0->pool_ndests,
+        PF_ARG(c->pool.d_slot, "pool not created");
+        PF_ARG(c->chunk_w == c0->chunk_w && c->chunk_h == c0->chunk_h && c->pool.ndests == c0->pool.ndests,
                "members hold maps or pools of different shapes");
     }
     return peer_check(g, fn);

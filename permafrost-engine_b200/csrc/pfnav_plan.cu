@@ -283,95 +283,6 @@ extern "C" int pfnav_plan_goal(pfnav_ctx *ctx, int layer, int tgt_chunk_r, int t
     return PFNAV_OK;
 }
 
-// ------------------------------------------------------------------------------------------
-// Pool slots with LRU eviction. The reference keeps its fields in LRU caches of fixed capacity
-// (fieldcache.c:59-71; CONFIG_FLOW_CACHE_SZ / CONFIG_LOS_CACHE_SZ, config.h:64-65): a request that finds the
-// cache full evicts the least recently used entry, and an agent that later misses it re-requests its path
-// (nav.c:3484-3506 == pfnav_pool_repair). Here one slot holds the flow AND the LOS field of a (dest, chunk);
-// "recently used" = the last tick whose desired-velocity pass read the slot (device side) or whose request
-// named it (host side); ties go to the lower slot index.
-// pf_pool_reserve: slots for the (dest, chunk) keys a request batch is about to write -- all or nothing: on
-// PFNAV_ERR_NOMEM nothing was changed. keys may repeat. *out_evicted: slot-table entries of OTHER keys changed
-// (the caller re-uploads the whole table and the `has` bytes).
-// ------------------------------------------------------------------------------------------
-int pf_pool_reserve(pfnav_ctx *ctx, const size_t *keys, size_t n, int32_t *slots_out, bool *out_evicted)
-{
-    if (out_evicted) *out_evicted = false;
-    // the distinct keys without a slot, ascending (a key is marked -2 while it is collected, so repeats are skipped)
-    std::vector<size_t> fresh;
-    for (size_t i = 0; i < n; i++)
-        if (ctx->h_pool_slot[keys[i]] == -1) { ctx->h_pool_slot[keys[i]] = -2; fresh.push_back(keys[i]); }
-    for (size_t key : fresh) ctx->h_pool_slot[key] = -1;
-    std::sort(fresh.begin(), fresh.end());
-    const size_t avail = ctx->pool_free.size() + (size_t)(ctx->pool_max - ctx->pool_used);
-    if (fresh.size() > avail) {
-        const size_t k = fresh.size() - avail;
-        std::vector<uint32_t> stamp(ctx->h_slot_touch);
-        if (ctx->device >= 0 && ctx->d_pool_touch && !ctx->pool_dev_stale) {     // stale: cleared, no tick read a slot since
-            PF_CUDA(cudaSetDevice(ctx->device));
-            PF_CUDA(cudaDeviceSynchronize());         // ticks on any stream may still be stamping slots (eviction is rare)
-            std::vector<uint32_t> dev(ctx->pool_max);
-            PF_CUDA(cudaMemcpy(dev.data(), ctx->d_pool_touch, (size_t)ctx->pool_max * 4, cudaMemcpyDeviceToHost));
-            for (int s = 0; s < ctx->pool_max; s++) stamp[s] = std::max(stamp[s], dev[s]);
-        }
-        std::vector<uint8_t> pinned(ctx->pool_max, 0);
-        for (size_t i = 0; i < n; i++) { const int s = ctx->h_pool_slot[keys[i]]; if (s >= 0) pinned[s] = 1; }
-        std::vector<int32_t> cand;
-        for (int s = 0; s < ctx->pool_used; s++)
-            if (ctx->h_slot_owner[s] >= 0 && !pinned[s]) cand.push_back(s);
-        if (cand.size() < k) {
-            pfnav_set_error("field pool full: %zu new (dest, chunk) fields requested, %zu slots free, %zu evictable of %d",
-                            fresh.size(), avail, cand.size(), ctx->pool_max);
-            return PFNAV_ERR_NOMEM;
-        }
-        std::sort(cand.begin(), cand.end(), [&](int32_t a, int32_t b) { return stamp[a] != stamp[b] ? stamp[a] < stamp[b] : a < b; });
-        for (size_t i = 0; i < k; i++) {
-            const int32_t s = cand[i];
-            const size_t owner = (size_t)ctx->h_slot_owner[s];
-            ctx->h_pool_slot[owner] = -1; ctx->h_pool_ffid[owner] = 0;
-            ctx->h_pool_has[s] = 0; ctx->h_slot_owner[s] = -1;
-            ctx->pool_free.push_back(s);
-            ctx->pool_evictions++;
-        }
-        if (out_evicted) *out_evicted = true;
-        ctx->goal_batch.valid = false;
-    }
-    for (size_t key : fresh) {
-        int32_t s;
-        if (!ctx->pool_free.empty()) { s = ctx->pool_free.back(); ctx->pool_free.pop_back(); }
-        else s = ctx->pool_used++;
-        ctx->h_pool_slot[key] = s; ctx->h_slot_owner[s] = (int64_t)key; ctx->h_pool_has[s] = 0;
-    }
-    for (size_t i = 0; i < n; i++) {
-        const int32_t s = ctx->h_pool_slot[keys[i]];
-        ctx->h_slot_touch[s] = ctx->tick_no;
-        if (slots_out) slots_out[i] = s;
-    }
-    return PFNAV_OK;
-}
-
-// pf_pool_reserve changes the slot-table entries of the keys it is given and of the owners of the slots it evicts, and
-// per-slot and free-list state: save those, so that a dry run of a batch's reservations can be undone exactly
-void pf_pool_save(const pfnav_ctx *ctx, std::vector<size_t> keys, pf_pool_saved &S)
-{
-    S.keys = std::move(keys);
-    S.kslot.resize(S.keys.size());
-    for (size_t i = 0; i < S.keys.size(); i++) S.kslot[i] = ctx->h_pool_slot[S.keys[i]];
-    S.owner = ctx->h_slot_owner; S.has = ctx->h_pool_has; S.touch = ctx->h_slot_touch; S.free_slots = ctx->pool_free;
-    S.ffid.assign(ctx->pool_max, 0);
-    for (int s = 0; s < ctx->pool_max; s++) if (S.owner[s] >= 0) S.ffid[s] = ctx->h_pool_ffid[(size_t)S.owner[s]];
-    S.used = ctx->pool_used; S.evictions = ctx->pool_evictions; S.gb_valid = ctx->goal_batch.valid;
-}
-
-void pf_pool_restore(pfnav_ctx *ctx, const pf_pool_saved &S)
-{
-    for (size_t i = 0; i < S.keys.size(); i++) ctx->h_pool_slot[S.keys[i]] = S.kslot[i];
-    for (int s = 0; s < ctx->pool_max; s++)
-        if (S.owner[s] >= 0) { ctx->h_pool_slot[(size_t)S.owner[s]] = s; ctx->h_pool_ffid[(size_t)S.owner[s]] = S.ffid[s]; }
-    ctx->h_slot_owner = S.owner; ctx->h_pool_has = S.has; ctx->h_slot_touch = S.touch; ctx->pool_free = S.free_slots;
-    ctx->pool_used = S.used; ctx->pool_evictions = S.evictions; ctx->goal_batch.valid = S.gb_valid;
-}
-
 // The flow waves and the LOS dependency chains of a goal batch each get a context-owned stream (the flow kernels
 // need ~100 KB of shared memory per CTA and would otherwise queue the caller's stream behind the persistent LOS
 // CTAs that hold most of it).
@@ -505,11 +416,7 @@ static int plan_batch(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int laye
         const int32_t *fc = P.fc.data(), *fw = P.fw.data(), *lc = P.lc.data();
         // PFNAV_REQUEST_MISSING_ONLY: fields the pool still holds for this destination are kept, like a field-cache hit
         // (fieldcache.c:138-141); a rebuilt LOS field whose parent chunk is kept reads the parent out of its pool slot
-        auto held = [&](int chunk, uint8_t bit) {
-            if (!missing_only) return false;
-            const int sl = ctx->h_pool_slot[(size_t)dests[g] * chunks + chunk];
-            return sl >= 0 && (ctx->h_pool_has[sl] & bit);
-        };
+        auto held = [&](int chunk, uint8_t bit) { return missing_only && (ctx->pool.has_of((size_t)dests[g] * chunks + chunk) & bit); };
         for (int i = 0; i < nf; i++) {
             if (held(fc[i], 1)) continue;
             B.fr.push_back(fr[i]); B.fw.push_back(fw[i]);
@@ -523,7 +430,7 @@ static int plan_batch(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int laye
                 if (B.newpos[q.prev_index] >= 0) { B.depth[i] = B.depth[q.prev_index] + 1; q.prev_index = B.newpos[q.prev_index]; }
                 else {
                     q.prev_index = -2;      // parent kept: its absolute pool slot rides in _pad
-                    q._pad = ctx->h_pool_slot[(size_t)dests[g] * chunks + q.prev_chunk_r * ctx->chunk_w + q.prev_chunk_c];
+                    q._pad = ctx->pool.slot_of((size_t)dests[g] * chunks + q.prev_chunk_r * ctx->chunk_w + q.prev_chunk_c);
                 }
             }
             B.newpos[i] = (int)B.lr.size();
@@ -544,28 +451,9 @@ static int reserve_batch(pfnav_ctx *ctx, pf_planner::merged &B)
     int rc = pf_pool_reserve(ctx, B.keys.data(), B.keys.size(), B.slots.data(), nullptr);
     if (rc) return rc;
     const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
-    for (int i = 0; i < nf; i++) { ctx->h_pool_has[fs[i]] |= 1; ctx->h_pool_req[fs[i]] = B.fr[i]; }
-    for (int i = 0; i < nl; i++) ctx->h_pool_has[ls[i]] |= 2;
+    for (int i = 0; i < nf; i++) ctx->pool.built_flow(fs[i], B.fr[i]);
+    for (int i = 0; i < nl; i++) ctx->pool.built(ls[i], 2);
     return PFNAV_OK;
-}
-
-// pf_pool_reserve's verdict on `keys` without its changes
-static bool pool_fits(const pfnav_ctx *ctx, const std::vector<size_t> &keys)
-{
-    std::vector<size_t> fresh;
-    std::vector<uint8_t> pinned(ctx->pool_max, 0);
-    for (size_t key : keys) {
-        const int s = ctx->h_pool_slot[key];
-        if (s >= 0) pinned[s] = 1;
-        else fresh.push_back(key);
-    }
-    std::sort(fresh.begin(), fresh.end());
-    const size_t nfresh = (size_t)(std::unique(fresh.begin(), fresh.end()) - fresh.begin());
-    const size_t avail = ctx->pool_free.size() + (size_t)(ctx->pool_max - ctx->pool_used);
-    if (nfresh <= avail) return true;
-    size_t cand = 0;
-    for (int s = 0; s < ctx->pool_used; s++) cand += ctx->h_slot_owner[s] >= 0 && !pinned[s];
-    return cand >= nfresh - avail;
 }
 
 // n_request_path's field-building half, resident on the device, for a batch of goals: plan every
@@ -582,7 +470,7 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
                                            const int32_t *targets, uint32_t flags, void *stream, int *out_n_flow, int *out_n_los)
 {
     const bool missing_only = (flags & PFNAV_REQUEST_MISSING_ONLY) != 0;
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
+    PF_ARG(ctx && ctx->pool.d_slot, "pool not created");
     PF_NEED_DEVICE(ctx);
     PF_ARG(ngoals >= 0 && (ngoals == 0 || (dests && targets)), "goals");
     if (out_n_flow) *out_n_flow = 0;
@@ -600,12 +488,12 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
             for (size_t w = 0; w + 1 < gb.fwave_off.size(); w++) {
                 const int first = gb.fwave_off[w], cnt = gb.fwave_off[w + 1] - first;
                 if (cnt <= 0) continue;
-                rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->d_pool_flow,
+                rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->pool.d_flow,
                                        (const int32_t *)(dev + gb.b_fr) + first, ctx->flow_stream);
                 if (rc) return rc;
             }
             const int32_t one_wave[2] = {0, gb.nl};
-            rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + gb.b_fr + gb.b_fs), gb.nl, ctx->d_pool_los,
+            rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + gb.b_fr + gb.b_fs), gb.nl, ctx->pool.d_los,
                                   (const int32_t *)(dev + gb.b_fr + gb.b_fs + gb.b_lr), 1, one_wave, ctx->field_stream);
             if (rc) return rc;
             rc = los_forked(ctx);
@@ -617,7 +505,7 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
         gb.valid = false;
     }
     pf_host_timer ht(ctx);
-    for (int g = 0; g < ngoals; g++) PF_ARG(dests[g] >= 0 && dests[g] < ctx->pool_ndests, "dest");
+    for (int g = 0; g < ngoals; g++) PF_ARG(dests[g] >= 0 && dests[g] < ctx->pool.ndests, "dest");
     int rc = plan_batch(ctx, ngoals, dests, layer, targets, missing_only, ht);
     if (rc) return rc;
     pf_planner::merged &B = planner_of(ctx).batch;
@@ -639,8 +527,7 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     const size_t b_lr = (size_t)nl * sizeof(pfnav_los_req), b_ls = (size_t)nl * 4;
     const size_t total = b_fr + b_fs + b_lr + b_ls;
     // the slot table and the `has` bytes travel in the same staging buffer, behind the plan
-    const size_t b_tab = (total + 15) & ~(size_t)15, b_slot = ctx->h_pool_slot.size() * 4;
-    const size_t stage = b_tab + b_slot + (size_t)ctx->pool_max;
+    const size_t b_tab = (total + 15) & ~(size_t)15, stage = b_tab + ctx->pool.table_bytes();
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
     uint8_t *host = nullptr;
@@ -663,8 +550,6 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
             if (q.prev_index >= 0) q.prev_index = B.lnew[q.prev_index];
             hlr[B.lnew[i]] = q; hls[B.lnew[i]] = ls[i];
         }
-        memcpy(host + b_tab, ctx->h_pool_slot.data(), b_slot);
-        memcpy(host + b_tab + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
     }
     ht.lap(PF_HPROF_PACK);
     // one device plan buffer per context: the resident fast path relaunches from it, and the previous batch's forked
@@ -681,9 +566,7 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     PF_CUDA(pf_fields_join(ctx, st));
     uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
     PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_tab, b_slot, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_tab + b_slot, ctx->pool_max,
-                            cudaMemcpyHostToDevice, st));
+    if ((rc = pf_pool_stage_table(ctx, host + b_tab, st))) return rc;
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
     ht.lap(PF_HPROF_UPLOAD);
     const pfnav_field_req *dfr = (const pfnav_field_req *)dev;
@@ -695,10 +578,10 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     for (int w = 0; w <= maxw; w++) {
         const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
         if (cnt <= 0) continue;
-        rc = pfnav_flow_launch(ctx, dfr + first, cnt, ctx->d_pool_flow, dfs + first, ctx->flow_stream);
+        rc = pfnav_flow_launch(ctx, dfr + first, cnt, ctx->pool.d_flow, dfs + first, ctx->flow_stream);
         if (rc) return rc;
     }
-    if (nl) rc = pfnav_los_launch(ctx, dlr, nl, ctx->d_pool_los, dls, maxd + 1, lwave_off.data(), ctx->field_stream);
+    if (nl) rc = pfnav_los_launch(ctx, dlr, nl, ctx->pool.d_los, dls, maxd + 1, lwave_off.data(), ctx->field_stream);
     if (rc) return rc;
     rc = los_forked(ctx);
     if (rc) return rc;
@@ -802,7 +685,7 @@ int pf_job_plan(pfnav_ctx *ctx, pf_job &J)
     const bool missing_only = (J.flags & PFNAV_REQUEST_MISSING_ONLY) != 0;
     J.fits = true; J.nf = J.nl = 0;
     J.lack.assign((size_t)J.ngoals * chunks, 0);
-    for (int g = 0; g < J.ngoals; g++) PF_ARG(J.dests[g] >= 0 && J.dests[g] < ctx->pool_ndests, "dest");
+    for (int g = 0; g < J.ngoals; g++) PF_ARG(J.dests[g] >= 0 && J.dests[g] < ctx->pool.ndests, "dest");
     PF_ARG(J.layer >= 0 && J.layer < ctx->nlayers, "layer");
     if (int rc = pf_job_check_state(ctx)) return rc;
     if (J.ngoals == 0) return PFNAV_OK;
@@ -811,12 +694,10 @@ int pf_job_plan(pfnav_ctx *ctx, pf_job &J)
     if (rc) return rc;
     const pf_planner::merged &B = planner_of(ctx).batch;
     J.nf = (int)B.fr.size(); J.nl = (int)B.lr.size();
-    J.fits = pool_fits(ctx, B.keys);
+    J.fits = pf_pool_fits(ctx->pool, B.keys.data(), B.keys.size());
     for (int g = 0; g < J.ngoals; g++)
-        for (int c = 0; c < chunks; c++) {
-            const int sl = missing_only ? ctx->h_pool_slot[(size_t)J.dests[g] * chunks + c] : -1;
-            J.lack[(size_t)g * chunks + c] = (uint8_t)(~(sl >= 0 ? ctx->h_pool_has[sl] : 0) & 3);
-        }
+        for (int c = 0; c < chunks; c++)
+            J.lack[(size_t)g * chunks + c] = (uint8_t)(~(missing_only ? ctx->pool.has_of((size_t)J.dests[g] * chunks + c) : 0) & 3);
     return PFNAV_OK;
 }
 
@@ -898,7 +779,7 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
                 const int p = q.prev_index;
                 if (newpos[p] >= 0) { d = bld[newpos[p]] + 1; q.prev_index = newpos[p]; }
                 else {
-                    parents.push_back({ctx->h_pool_slot[row + P.lc[p]], extra, 1});
+                    parents.push_back({ctx->pool.slot_of(row + P.lc[p]), extra, 1});
                     q.prev_index = -2; q._pad = extra++;
                 }
             }
@@ -909,7 +790,7 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
     // ---- this member's own slots, exactly as its solo call reserves them
     int rc = 0;
     if (!B.keys.empty() && (rc = reserve_batch(ctx, B))) return rc;
-    ctx->goal_batch.valid = false;
+    ctx->goal_batch.valid = false;          // the plan buffer is about to be reused
     // ---- the fields this member lacks: staging block -> its slot (a flow field once per (goal, chunk))
     std::vector<pf_field_copy> items;
     std::vector<uint8_t> seen((size_t)ngoals * chunks, 0);
@@ -920,10 +801,10 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
             const int c = P.fc[i];
             if (!(J.lack[gi + c] & 1) || seen[gi + c]) continue;
             seen[gi + c] = 1;
-            items.push_back({fblk[gi + c], ctx->h_pool_slot[row + c], 0});
+            items.push_back({fblk[gi + c], ctx->pool.slot_of(row + c), 0});
         }
         for (int i = 0; i < P.nl; i++)
-            if (J.lack[gi + P.lc[i]] & 2) items.push_back({lblk[gi + P.lc[i]], ctx->h_pool_slot[row + P.lc[i]], 1});
+            if (J.lack[gi + P.lc[i]] & 2) items.push_back({lblk[gi + P.lc[i]], ctx->pool.slot_of(row + P.lc[i]), 1});
     }
     // ---- pack: builds in wave / depth order, the copies, then the slot table and the `has` bytes
     const int nf = (int)bfr.size(), nl = (int)blr.size(), np = (int)parents.size(), ni = (int)items.size();
@@ -940,11 +821,11 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
     const size_t o_fr = sec((size_t)nf * sizeof(pfnav_field_req)), o_fs = sec((size_t)nf * 4);
     const size_t o_lr = sec((size_t)nl * sizeof(pfnav_los_req)), o_ls = sec((size_t)nl * 4);
     const size_t o_pc = sec((size_t)np * sizeof(pf_field_copy)), o_it = sec((size_t)ni * sizeof(pf_field_copy));
-    const size_t total = off, b_slot = ctx->h_pool_slot.size() * 4;
+    const size_t total = off;
     PF_CUDA(cudaSetDevice(ctx->device));
     uint8_t *host = nullptr;
     int ri = 0;
-    if ((rc = pf_plan_host(ctx, total + b_slot + (size_t)ctx->pool_max, &host, &ri))) return rc;
+    if ((rc = pf_plan_host(ctx, total + ctx->pool.table_bytes(), &host, &ri))) return rc;
     {
         pfnav_field_req *hfr = (pfnav_field_req *)(host + o_fr);
         int32_t *hfs = (int32_t *)(host + o_fs), *hls = (int32_t *)(host + o_ls);
@@ -960,8 +841,6 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
         }
         memcpy(host + o_pc, parents.data(), (size_t)np * sizeof(pf_field_copy));
         memcpy(host + o_it, items.data(), (size_t)ni * sizeof(pf_field_copy));
-        memcpy(host + total, ctx->h_pool_slot.data(), b_slot);
-        memcpy(host + total + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
     }
     // the plan buffer and the staging buffer: the previous batch's kernels and exchange may still read them, so growing
     // either waits for the device (a group member's stream has waited for its peers' reads of its staging)
@@ -986,11 +865,9 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
     PF_CUDA(pf_fields_join(ctx, st));
     uint8_t *dev = (uint8_t *)ctx->d_plan_buf, *stage = ctx->d_job_stage;
     PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + total, b_slot, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + total + b_slot, ctx->pool_max,
-                            cudaMemcpyHostToDevice, st));
+    if ((rc = pf_pool_stage_table(ctx, host + total, st))) return rc;
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
-    if ((rc = field_copy_launch(ctx, nullptr, ctx->d_pool_los, nullptr, stage, (const pf_field_copy *)(dev + o_pc), np, st)))
+    if ((rc = field_copy_launch(ctx, nullptr, ctx->pool.d_los, nullptr, stage, (const pf_field_copy *)(dev + o_pc), np, st)))
         return rc;
     // the owner's builds: flow waves and LOS chains on the context's field streams, as in the solo call; the exchange
     // that follows on `st` reads what they wrote
@@ -1016,7 +893,7 @@ int pf_job_scatter(pfnav_ctx *ctx, pf_job &J, cudaStream_t st)
 {
     if (J.seg.empty() || J.seg.back() == 0) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
-    int rc = field_copy_launch(ctx, ctx->d_job_stage, ctx->d_job_stage, ctx->d_pool_flow, ctx->d_pool_los,
+    int rc = field_copy_launch(ctx, ctx->d_job_stage, ctx->d_job_stage, ctx->pool.d_flow, ctx->pool.d_los,
                                (const pf_field_copy *)J.d_items, J.nitems, st);
     if (rc) return rc;
     // the next pool reader on any stream joins the copies the way it joins a solo batch's forked builds
@@ -1067,7 +944,7 @@ void pf_job_layout(pfnav_ctx *ctx, pf_job &J, const std::vector<int32_t> &freq, 
 int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &items, int world, cudaStream_t st)
 {
     const size_t o_items = J.seg[world] * 4096, b_items = items.size() * sizeof(pf_field_copy);
-    const size_t b_slot = ctx->h_pool_slot.size() * 4, need = o_items + b_items;
+    const size_t need = o_items + b_items;
     // the previous batch's builds, exchange and copies may still read the staging buffer: growing it waits for the
     // device (a group member's stream has waited for its peers' reads of its staging)
     if (ctx->job_stage_bytes < need) {
@@ -1080,14 +957,10 @@ int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &it
     }
     uint8_t *host = nullptr;
     int ri = 0;
-    if (int rc = pf_plan_host(ctx, b_items + b_slot + (size_t)ctx->pool_max, &host, &ri)) return rc;
+    if (int rc = pf_plan_host(ctx, b_items + ctx->pool.table_bytes(), &host, &ri)) return rc;
     memcpy(host, items.data(), b_items);
-    memcpy(host + b_items, ctx->h_pool_slot.data(), b_slot);
-    memcpy(host + b_items + b_slot, ctx->h_pool_has.data(), ctx->pool_max);
     if (b_items) PF_CUDA(cudaMemcpyAsync(ctx->d_job_stage + o_items, host, b_items, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_items, b_slot, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_items + b_slot, ctx->pool_max,
-                            cudaMemcpyHostToDevice, st));
+    if (int rc = pf_pool_stage_table(ctx, host + b_items, st)) return rc;
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
     J.d_items = ctx->d_job_stage + o_items; J.nitems = (int)items.size();
     return PFNAV_OK;

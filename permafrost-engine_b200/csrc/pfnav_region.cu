@@ -473,7 +473,7 @@ struct aux_field { uint32_t req; int32_t cr, cc, slot; };
 static int zone_validate(const pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, std::vector<int32_t> &ctile,
                          std::vector<uint8_t> &on_map, int *dim)
 {
-    PF_ARG(ctx->d_cost && ctx->d_pool_slot, "map / pool not created");
+    PF_ARG(ctx->d_cost && ctx->pool.d_slot, "map / pool not created");
     PF_ARG(m == 0 || reqs, "reqs");
     PF_ARG(m < (1u << 24), "m");
     ctile.assign(2 * m, 0);
@@ -481,7 +481,7 @@ static int zone_validate(const pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_
     bool any_on_map = false;
     for (size_t i = 0; i < m; i++) {
         const pfnav_zone_req &q = reqs[i];
-        PF_ARG(q.dest >= 0 && q.dest < ctx->pool_ndests, "dest");
+        PF_ARG(q.dest >= 0 && q.dest < ctx->pool.ndests, "dest");
         PF_ARG(q.layer >= 0 && q.layer < ctx->nlayers, "layer");
         PF_ARG(q.radius >= 0 && q.radius <= 0xFFFF, "radius");
         on_map[i] = region_tile_for_point(ctx, q.centre_x, q.centre_z, &ctile[2 * i]);      // nav.c:3931
@@ -512,8 +512,7 @@ static uint64_t zone_flood(const pfnav_zone_req &q, const int32_t *ctile, int di
     return cdr >= 0 && cdr < dim && cdc >= 0 && cdc < dim ? budget : 0;
 }
 
-// Slots request by request, in order, by the single call's rule (a fresh slot from pool_used, no eviction, no pool_free
-// reuse, only `has` bit 0), chunk by chunk. fresh: (slot table index, slot) of every new reservation. On
+// Slots request by request, in order, by the single call's rule (pf_pool_zone_take; only `has` bit 0), chunk by chunk. fresh: (slot table index, slot) of every new reservation. On
 // PFNAV_ERR_NOMEM, *out_done is the request that did not fit: it keeps its reservations, unbuilt, as the single call
 // leaves them.
 static int zone_reserve(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, const std::vector<int32_t> &ctile,
@@ -532,24 +531,21 @@ static int zone_reserve(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t m, co
         for (int cr = ch[0]; cr <= ch[1] && rc == PFNAV_OK; cr++)
             for (int cc = ch[2]; cc <= ch[3]; cc++) {
                 const size_t si = (size_t)q.dest * nch + cr * cw + cc;
-                int32_t slot = ctx->h_pool_slot[si];
+                const bool had = ctx->pool.slot_of(si) >= 0;
+                const int32_t slot = pf_pool_zone_take(ctx, si);
                 if (slot < 0) {
-                    if (ctx->pool_used >= ctx->pool_max) {
-                        pfnav_set_error("pfnav_pool_request_zone: pool full (%d fields)", ctx->pool_max);
-                        rc = PFNAV_ERR_NOMEM;
-                        break;
-                    }
-                    slot = ctx->pool_used++;
-                    ctx->h_pool_slot[si] = slot;
-                    fresh.push_back((int32_t)si); fresh.push_back(slot);
+                    pfnav_set_error("pfnav_pool_request_zone: pool full (%d fields)", ctx->pool.max);
+                    rc = PFNAV_ERR_NOMEM;
+                    break;
                 }
+                if (!had) { fresh.push_back((int32_t)si); fresh.push_back(slot); }
                 fields.push_back({(uint32_t)done, cr, cc, slot});
             }
         if (rc) {
             fields.resize(first);
             break;
         }
-        for (size_t f = first; f < fields.size(); f++) ctx->h_pool_has[fields[f].slot] |= 1;
+        for (size_t f = first; f < fields.size(); f++) ctx->pool.built(fields[f].slot, 1);
         if (out_nfields) out_nfields[done] = (int32_t)(fields.size() - first);
     }
     *out_done = done;
@@ -596,9 +592,9 @@ static int zone_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_zone_req *req
             kreq[k].seed_n = (int32_t)(seeds.size() / 2) - kreq[k].seed_off;
         }
     }
-    // the `has` bytes of the written slots (h_pool_has after the batch)
+    // the `has` bytes of the written slots (the host mirror after the batch)
     std::vector<uint8_t> hasv(scatter ? nk : 0);
-    for (size_t k = 0; k < hasv.size(); k++) hasv[k] = ctx->h_pool_has[kslot[k]];
+    for (size_t k = 0; k < hasv.size(); k++) hasv[k] = ctx->pool.has[kslot[k]];
     // ---- one pinned staging buffer with the inputs, copied into the device scratch
     size_t b_in = 0;
     auto sec = [&](size_t bytes) { const size_t o = b_in; b_in = (b_in + bytes + 15) & ~(size_t)15; return o; };
@@ -623,9 +619,9 @@ static int zone_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_zone_req *req
     const int nscatter = (int)std::max(fresh.size() / 2, hasv.size());
     if (nscatter) {
         k_pool_scatter<<<(unsigned)((nscatter + 255) / 256), 256, 0, st>>>((const int32_t *)(dev + o_fresh), (int)(fresh.size() / 2),
-                                                                            ctx->d_pool_slot, (const int32_t *)(dev + o_slot),
+                                                                            ctx->pool.d_slot, (const int32_t *)(dev + o_slot),
                                                                             (const uint8_t *)(dev + o_hasv), (int)hasv.size(),
-                                                                            ctx->d_pool_los + (size_t)ctx->pool_max * 4096);
+                                                                            ctx->pool.d_has);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
     }
@@ -676,14 +672,13 @@ extern "C" int pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *re
     rc = zone_reserve(ctx, reqs, m, ctile, on_map, fields, fresh, out_nfields, &done);
     if (out_ndone) *out_ndone = (int)done;
     if (fields.empty() && fresh.empty()) return rc;
-    if (!fields.empty()) ctx->goal_batch.valid = false;
     // ---- one flood + one integration per slot: the last field written to it
-    std::vector<int32_t> last(ctx->pool_max, -1);
+    std::vector<int32_t> last(ctx->pool.max, -1);
     for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
     std::vector<aux_field> build;
     for (size_t f = 0; f < fields.size(); f++)
         if (last[fields[f].slot] == (int32_t)f) build.push_back(fields[f]);
-    const int lrc = zone_build(ctx, st, reqs, ctile, dim, build, fresh, true, ctx->d_pool_flow);
+    const int lrc = zone_build(ctx, st, reqs, ctile, dim, build, fresh, true, ctx->pool.d_flow);
     return lrc ? lrc : rc;
 }
 
@@ -705,8 +700,8 @@ extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const floa
 {
     PF_ARG(ctx && ctx->d_cost, "map not created");
     PF_NEED_DEVICE(ctx);
-    PF_ARG(ctx->d_pool_slot, "pool not created");
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
+    PF_ARG(ctx->pool.d_slot, "pool not created");
+    PF_ARG(dest >= 0 && dest < ctx->pool.ndests, "dest");
     if (n == 0) return PFNAV_OK;
     PF_ARG(centre_xz && pos_xz && out_vel && out_flags, "null buffer");
     PF_ARG(n < (1u << 30), "n");
@@ -719,7 +714,7 @@ extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const floa
     float2 *d_pos = reinterpret_cast<float2 *>(d_buf), *d_vel = d_pos + n;
     uint8_t *d_fl = d_buf + n * 16;
     cudaStream_t st = ctx->tick_stream;
-    ZoneView z = { ctx->d_pool_slot, ctx->d_pool_flow, ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->chunk_w, ctx->chunk_h,
+    ZoneView z = { ctx->pool.d_slot, ctx->pool.d_flow, ctx->pool.d_has, ctx->chunk_w, ctx->chunk_h,
                    ctx->map_x, ctx->map_z };
     cudaError_t e = cudaMemcpyAsync(d_pos, pos_xz, n * 8, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) {
@@ -1046,7 +1041,7 @@ struct entity_batch { int dim = 0; std::vector<enemy_bins> bins; std::vector<int
 static int entity_validate(const pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m, const pfnav_footprint *ents,
                            size_t nents, const int32_t *chunks_rc, size_t nchunks, entity_batch &E)
 {
-    PF_ARG(ctx->d_cost && ctx->d_pool_slot, "map / pool not created");
+    PF_ARG(ctx->d_cost && ctx->pool.d_slot, "map / pool not created");
     PF_ARG(m == 0 || reqs, "reqs");
     PF_ARG((nents == 0 || ents) && (nchunks == 0 || chunks_rc), "ents / chunks_rc");
     PF_ARG(m < (1u << 24) && nents < (1u << 24) && nchunks < (1u << 24), "m / nents / nchunks");
@@ -1054,7 +1049,7 @@ static int entity_validate(const pfnav_ctx *ctx, const pfnav_entity_field_req *r
     bool any_fields = false;
     for (size_t i = 0; i < m; i++) {
         const pfnav_entity_field_req &q = reqs[i];
-        PF_ARG(q.dest >= 0 && q.dest < ctx->pool_ndests, "dest");
+        PF_ARG(q.dest >= 0 && q.dest < ctx->pool.ndests, "dest");
         PF_ARG(q.layer >= 0 && q.layer < ctx->nlayers, "layer");
         PF_ARG((uint64_t)q.ent_off + q.ent_n <= nents, "footprint range");
         PF_ARG((uint64_t)q.chunk_off + q.chunk_n <= nchunks, "chunk range");
@@ -1098,13 +1093,12 @@ static int entity_validate(const pfnav_ctx *ctx, const pfnav_entity_field_req *r
 }
 
 // Slots request by request, in order: the serial calls' reservations and evictions, and the footprints each destination
-// remembers. On an error, *out_done is the request that failed. fields == nullptr: a dry run that only reserves (the
-// caller undoes it with pf_pool_restore).
+// remembers. On an error, *out_done is the request that failed.
 static int entity_reserve(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m, const pfnav_footprint *ents,
-                          const int32_t *chunks_rc, std::vector<aux_field> *fields, size_t *out_done)
+                          const int32_t *chunks_rc, std::vector<aux_field> &fields, size_t *out_done)
 {
     const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
-    if (fields && ctx->aux.size() < (size_t)ctx->pool_ndests) ctx->aux.resize(ctx->pool_ndests);
+    if (ctx->aux.size() < (size_t)ctx->pool.ndests) ctx->aux.resize(ctx->pool.ndests);
     std::vector<size_t> keys;
     std::vector<int32_t> slots;
     int rc = PFNAV_OK;
@@ -1118,19 +1112,17 @@ static int entity_reserve(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, si
             bool evicted = false;
             if ((rc = pf_pool_reserve(ctx, keys.data(), q.chunk_n, slots.data(), &evicted))) break;
         }
-        if (!fields) continue;
         // the footprints stay with the destination: the in-place repairs of its fields start from them (field.c:2334-2360)
         pfnav_ctx::aux_target &A = ctx->aux[q.dest];
         A.kind = q.target_kind; A.layer = q.layer; A.ref_layer = q.ref_layer; A.ents.assign(ents + q.ent_off, ents + q.ent_off + q.ent_n);
         for (uint32_t k = 0; k < q.chunk_n; k++) {
-            ctx->h_pool_has[slots[k]] |= 1;
             pfnav_field_req fr;
             memset(&fr, 0, sizeof(fr));
             fr.chunk_r = crc[2 * k]; fr.chunk_c = crc[2 * k + 1]; fr.layer = q.layer; fr.faction_id = PFNAV_FACTION_ID_NONE;
             fr.target_type = 2 + q.target_kind;      // beyond the chunk-local kinds: the frontier comes from ctx->aux[dest]
             fr._pad = q.dest;
-            ctx->h_pool_req[slots[k]] = fr;
-            fields->push_back({(uint32_t)done, crc[2 * k], crc[2 * k + 1], slots[k]});
+            ctx->pool.built_flow(slots[k], fr);
+            fields.push_back({(uint32_t)done, crc[2 * k], crc[2 * k + 1], slots[k]});
         }
     }
     *out_done = done;
@@ -1189,8 +1181,7 @@ static int entity_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_fiel
     const size_t o_ioff = sec(item_off.size() * 4), o_items = sec(items.size() * 4);
     const size_t o_hoff = sec(hitem_off.size() * 4), o_hitems = sec(hitems.size() * 4);
     const size_t o_jobs = sec(nj * sizeof(fp_job)), o_toff = sec(htile_off.size() * 4), o_tiles = sec(htiles.size() * 4);
-    const size_t b_slot = upload_pool ? ctx->h_pool_slot.size() * 4 : 0, b_has = upload_pool ? (size_t)ctx->pool_max : 0;
-    const size_t stage = b_in + b_slot + b_has;
+    const size_t stage = b_in + (upload_pool ? ctx->pool.table_bytes() : 0);
     const size_t o_org = b_in + 0, o_rows = o_org + ((nj * 8 + 15) & ~(size_t)15), o_bits = o_rows + nj * 128;
     const size_t need = o_bits + nk * ((size_t)dim * dim / 8);
     uint8_t *host = nullptr;
@@ -1206,18 +1197,10 @@ static int entity_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_fiel
     memcpy(host + o_jobs, jobs.data(), nj * sizeof(fp_job));
     memcpy(host + o_toff, htile_off.data(), htile_off.size() * 4);
     memcpy(host + o_tiles, htiles.data(), htiles.size() * 4);
-    if (upload_pool) {
-        memcpy(host + b_in, ctx->h_pool_slot.data(), b_slot);
-        memcpy(host + b_in + b_slot, ctx->h_pool_has.data(), b_has);
-    }
     uint8_t *dev = nullptr;
     if ((rc = batch_scratch(ctx, st, need, &dev))) return rc;
     PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
-    if (upload_pool) {
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, host + b_in, b_slot, cudaMemcpyHostToDevice, st));
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, host + b_in + b_slot, b_has,
-                                cudaMemcpyHostToDevice, st));
-    }
+    if (upload_pool && (rc = pf_pool_stage_table(ctx, host + b_in, st))) return rc;
     PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
     const pfnav_region_req *d_req = (const pfnav_region_req *)(dev + o_req);
     int2 *d_org = (int2 *)(dev + o_org);
@@ -1257,17 +1240,16 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
     PF_CUDA(pf_pool_refresh(ctx, st));
     std::vector<aux_field> fields;
     size_t done = 0;
-    rc = entity_reserve(ctx, reqs, m, ents, chunks_rc, &fields, &done);
+    rc = entity_reserve(ctx, reqs, m, ents, chunks_rc, fields, &done);
     if (out_ndone) *out_ndone = (int)done;
     if (fields.empty()) return rc;
-    ctx->goal_batch.valid = false;
     // ---- the last field written to each slot
-    std::vector<int32_t> last(ctx->pool_max, -1);
+    std::vector<int32_t> last(ctx->pool.max, -1);
     for (size_t f = 0; f < fields.size(); f++) last[fields[f].slot] = (int32_t)f;
     std::vector<aux_field> build;
     for (size_t f = 0; f < fields.size(); f++)
         if (last[fields[f].slot] == (int32_t)f) build.push_back(fields[f]);
-    const int lrc = entity_build(ctx, st, reqs, ents, nents, E, build, true, ctx->d_pool_flow);
+    const int lrc = entity_build(ctx, st, reqs, ents, nents, E, build, true, ctx->pool.d_flow);
     return lrc ? lrc : rc;
 }
 
@@ -1295,38 +1277,29 @@ int pf_aux_job_plan(pfnav_ctx *ctx, pf_job &J)
     if ((rc = pf_job_check_state(ctx))) return rc;
     J.aux = S;
     const int cw = ctx->chunk_w, nch = cw * ctx->chunk_h;
-    if (zones) {        // the distinct keys without a slot, each a fresh slot from pool_used
-        std::vector<size_t> fresh;
+    std::vector<size_t> keys;
+    if (zones) {        // every key the batch names, by the zone rule's verdict
         for (size_t i = 0; i < J.m; i++) {
             if (!S->on_map[i]) continue;
             int ch[4];
             zone_chunks(ctx, J.zreqs[i], &S->ctile[2 * i], ch);
             for (int cr = ch[0]; cr <= ch[1]; cr++)
-                for (int cc = ch[2]; cc <= ch[3]; cc++) {
-                    const size_t si = (size_t)J.zreqs[i].dest * nch + cr * cw + cc;
-                    if (ctx->h_pool_slot[si] < 0) fresh.push_back(si);
-                }
+                for (int cc = ch[2]; cc <= ch[3]; cc++) keys.push_back((size_t)J.zreqs[i].dest * nch + cr * cw + cc);
         }
-        std::sort(fresh.begin(), fresh.end());
-        J.fits = (size_t)(std::unique(fresh.begin(), fresh.end()) - fresh.begin()) <= (size_t)(ctx->pool_max - ctx->pool_used);
+        J.fits = pf_pool_zone_fits(ctx->pool, keys.data(), keys.size());
         return PFNAV_OK;
     }
-    // entity fields: the reservations with their evictions, undone
-    std::vector<size_t> keys;
-    for (size_t i = 0; i < J.m; i++) {
+    // entity fields: the serial reservations all succeed exactly when each request's does on the pool as it is now
+    for (size_t i = 0; i < J.m && J.fits; i++) {
         const pfnav_entity_field_req &q = J.ereqs[i];
+        keys.clear();
         for (uint32_t k = 0; k < q.chunk_n; k++) {
             const int32_t *c = J.chunks_rc + 2 * ((size_t)q.chunk_off + k);
             keys.push_back((size_t)q.dest * nch + c[0] * cw + c[1]);
         }
+        J.fits = pf_pool_fits(ctx->pool, keys.data(), keys.size());
     }
-    pf_pool_saved saved;
-    pf_pool_save(ctx, std::move(keys), saved);
-    size_t done = 0;
-    rc = entity_reserve(ctx, J.ereqs, J.m, J.ents, J.chunks_rc, nullptr, &done);
-    pf_pool_restore(ctx, saved);
-    if (rc == PFNAV_ERR_NOMEM) { J.fits = false; rc = PFNAV_OK; }
-    return rc;
+    return PFNAV_OK;
 }
 
 int pf_aux_job_launch(pfnav_ctx *ctx, pf_job &J, int world, int rank, cudaStream_t st)
@@ -1339,15 +1312,14 @@ int pf_aux_job_launch(pfnav_ctx *ctx, pf_job &J, int world, int rank, cudaStream
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_join(ctx, st));
     PF_CUDA(pf_pool_refresh(ctx, st));
-    // ---- this member's own slots, exactly as its solo call reserves them (the dry run said they fit)
+    // ---- this member's own slots, exactly as its solo call reserves them (the verdict said they fit)
     std::vector<aux_field> fields;
     std::vector<int32_t> fresh;
     size_t done = 0;
     J.nfields.assign(J.m, 0);
     int rc = zones ? zone_reserve(ctx, J.zreqs, J.m, S.ctile, S.on_map, fields, fresh, J.nfields.data(), &done)
-                   : entity_reserve(ctx, J.ereqs, J.m, J.ents, J.chunks_rc, &fields, &done);
+                   : entity_reserve(ctx, J.ereqs, J.m, J.ents, J.chunks_rc, fields, &done);
     if (rc) return rc;
-    if (!fields.empty()) ctx->goal_batch.valid = false;
     // ---- owners and staging blocks: `fields` lists what the serial calls write, the same on every member
     const size_t n = fields.size();
     std::vector<int32_t> freq(n), blk;
@@ -1367,7 +1339,7 @@ int pf_aux_job_launch(pfnav_ctx *ctx, pf_job &J, int world, int rank, cudaStream
     std::vector<aux_field> own;
     for (size_t f = 0; f < n; f++) {
         if (blk[f] < 0) continue;
-        const int32_t s = ctx->h_pool_slot[fkey[f]];
+        const int32_t s = ctx->pool.slot_of(fkey[f]);
         if (s >= 0) items.push_back({blk[f], s, 0});
         if (ctx->job_owner[freq[f]] == rank) own.push_back({fields[f].req, fields[f].cr, fields[f].cc, blk[f]});
     }
@@ -1385,7 +1357,7 @@ extern "C" int pfnav_pool_request_entity_fields(pfnav_ctx *ctx, int dest, int la
                                                 const pfnav_footprint *ents, size_t nents, const int32_t *chunks_rc, size_t n,
                                                 void *stream)
 {
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
+    PF_ARG(ctx && ctx->pool.d_slot, "pool not created");
     PF_ARG(nents < (1u << 24) && n < (1u << 24), "nents / n");
     const pfnav_entity_field_req q = {dest, layer, ref_layer, target_kind, 0, (uint32_t)nents, 0, (uint32_t)n};
     int rc = pfnav_pool_request_entity_fields_batch(ctx, &q, 1, ents, nents, chunks_rc, n, stream, nullptr);

@@ -929,10 +929,10 @@ static int launch_segment(pfnav_ctx *ctx, cudaStream_t st, const path_segment &S
     for (int w = 0; w <= maxw; w++) {
         const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
         if (cnt <= 0) continue;
-        int rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->d_pool_flow, (const int32_t *)(dev + b_fr) + first, st);
+        int rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->pool.d_flow, (const int32_t *)(dev + b_fr) + first, st);
         if (rc) return rc;
     }
-    if (nl) return pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + b_fr + b_fs), nl, ctx->d_pool_los,
+    if (nl) return pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + b_fr + b_fs), nl, ctx->pool.d_los,
                                     (const int32_t *)(dev + b_fr + b_fs + b_lr), maxd + 1, lwave_off.data(), st);
     return PFNAV_OK;
 }
@@ -968,7 +968,7 @@ int pf_path_batch_begin(pfnav_ctx *ctx, int n, const int32_t *dests, const int32
     B->dests.assign(dests, dests + n); B->layers.assign(layers, layers + n);
     B->plans.resize(n); B->planned.assign(n, 0);
     const int cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
-    B->mapped.resize(chunks); B->los_have.resize(chunks); B->row_touched.assign(ctx->pool_ndests, 0);
+    B->mapped.resize(chunks); B->los_have.resize(chunks); B->row_touched.assign(ctx->pool.ndests, 0);
     std::vector<tdesc> s(n), d(n);
     std::set<int> used_layers;
     for (int i = 0; i < n; i++) {
@@ -1003,11 +1003,8 @@ int pf_path_batch_probe(pf_path_batch *B, int i, pf_path_probe *out)
     PF_ARG(B->planned[i], "pfnav_route_build not called, or a position outside the map");
     const int layer = B->layers[i], cw = ctx->chunk_w, chunks = cw * ctx->chunk_h;
     const size_t row = (size_t)B->dests[i] * chunks;
-    for (int c = 0; c < chunks; c++) {
-        const int s = ctx->h_pool_slot[row + c];
-        B->los_have[c] = (s >= 0 && (ctx->h_pool_has[s] & 2)) ? 1 : 0;
-    }
-    memcpy(B->mapped.data(), ctx->h_pool_ffid.data() + row, (size_t)chunks * 8);
+    for (int c = 0; c < chunks; c++) B->los_have[c] = (ctx->pool.has_of(row + c) & 2) ? 1 : 0;
+    memcpy(B->mapped.data(), ctx->pool.ffid.data() + row, (size_t)chunks * 8);
     Router R{ctx, *route_layer(ctx, layer), layer, cw, ctx->chunk_h};
     path_emit &E = B->E;
     emit_plan(R, ctx, layer, B->plans[i], B->mapped.data(), B->los_have.data(), E);
@@ -1023,15 +1020,13 @@ int pf_path_batch_probe(pf_path_batch *B, int i, pf_path_probe *out)
     for (int k = 0; k < nl; k++) keys.push_back(row + E.lc[k]);
     for (int k = 0; k < nl; k++)
         if (E.lr[k].prev_index == -2) keys.push_back(row + E.lr[k].prev_chunk_r * cw + E.lr[k].prev_chunk_c);
-    std::vector<size_t> fresh;
-    for (size_t k = 0; k < keys.size(); k++) {
-        const int32_t s = ctx->h_pool_slot[keys[k]];
-        if (k < (size_t)(nf + nl) && s >= 0) out->write_slots.push_back(s);
-        if (s < 0) fresh.push_back(keys[k]);
+    for (size_t k = 0; k < (size_t)(nf + nl); k++) {
+        const int32_t s = ctx->pool.slot_of(keys[k]);
+        if (s >= 0) out->write_slots.push_back(s);
     }
-    std::sort(fresh.begin(), fresh.end());
-    const size_t nfresh = std::unique(fresh.begin(), fresh.end()) - fresh.begin();
-    out->would_evict = nfresh > ctx->pool_free.size() + (size_t)(ctx->pool_max - ctx->pool_used);
+    std::vector<size_t> fresh;
+    pf_pool_fresh(ctx->pool, keys.data(), keys.size(), fresh);
+    out->would_evict = fresh.size() > ctx->pool.avail();
     return PFNAV_OK;
 }
 
@@ -1057,21 +1052,20 @@ int pf_path_batch_commit(pf_path_batch *B, std::vector<int32_t> *out_slots)
         // a slot this segment writes or reads now belongs to another (dest, chunk): launch the segment first, so
         // that its writes and reads stay ordered before this request's
         bool moved = false;
-        for (const auto &u : S.used) moved |= ctx->h_slot_owner[u.first] != (int64_t)u.second;
+        for (const auto &u : S.used) moved |= ctx->pool.owner[u.first] != (int64_t)u.second;
         if (moved) { rc = launch_segment(ctx, B->st, S); if (rc) return rc; S.clear(); }
     }
     for (size_t k = 0; k < keys.size(); k++) S.used.push_back({slots[k], keys[k]});
     for (int i = 0; i < nf; i++) {
         const int32_t s = slots[i];
-        ctx->h_pool_has[s] |= 1;
-        ctx->h_pool_ffid[row + E.fc[i]] = E.fid[i];
-        ctx->h_pool_req[s] = E.fr[i];
+        ctx->pool.built_flow(s, E.fr[i]);
+        ctx->pool.ffid[row + E.fc[i]] = E.fid[i];
         S.fr.push_back(E.fr[i]); S.fs.push_back(s); S.fw.push_back(S.writes[s]++);
     }
     const int l0 = (int)S.lr.size();
     for (int i = 0; i < nl; i++) {
         const int32_t s = slots[nf + i];
-        ctx->h_pool_has[s] |= 2;
+        ctx->pool.built(s, 2);
         pfnav_los_req q = E.lr[i];
         int depth = 0;
         if (q.prev_index >= 0) { q.prev_index += l0; depth = S.ld[q.prev_index] + 1; }
@@ -1079,7 +1073,7 @@ int pf_path_batch_commit(pf_path_batch *B, std::vector<int32_t> *out_slots)
             const size_t pkey = row + q.prev_chunk_r * cw + q.prev_chunk_c;
             auto it = S.los_at.find(pkey);
             if (it != S.los_at.end()) { q.prev_index = it->second; depth = S.ld[it->second] + 1; }   // built earlier in this segment
-            else q._pad = ctx->h_pool_slot[pkey];                                                      // absolute pool slot of prev_los
+            else q._pad = ctx->pool.slot_of(pkey);                                                      // absolute pool slot of prev_los
         }
         S.los_at[row + E.lc[i]] = (int)S.lr.size();
         S.lr.push_back(q); S.ls.push_back(s); S.ld.push_back(depth);
@@ -1097,16 +1091,16 @@ int pf_path_batch_flush(pf_path_batch *B)
     if (rc) return rc;
     B->S.clear();
     if (B->any_evicted)      // entries of other destinations lost their slots
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot, ctx->h_pool_slot.data(), ctx->h_pool_slot.size() * 4, cudaMemcpyHostToDevice, st));
+        PF_CUDA(cudaMemcpyAsync(ctx->pool.d_slot, ctx->pool.slot.data(), ctx->pool.slot.size() * 4, cudaMemcpyHostToDevice, st));
     else
-        for (int d = 0; d < ctx->pool_ndests; d++)
+        for (int d = 0; d < ctx->pool.ndests; d++)
             if (B->row_touched[d])
-                PF_CUDA(cudaMemcpyAsync(ctx->d_pool_slot + (size_t)d * chunks, ctx->h_pool_slot.data() + (size_t)d * chunks,
+                PF_CUDA(cudaMemcpyAsync(ctx->pool.d_slot + (size_t)d * chunks, ctx->pool.slot.data() + (size_t)d * chunks,
                                         (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
     bool any_touched = B->any_evicted;
     for (uint8_t t : B->row_touched) any_touched |= t != 0;
     if (any_touched)
-        PF_CUDA(cudaMemcpyAsync(ctx->d_pool_los + (size_t)ctx->pool_max * 4096, ctx->h_pool_has.data(), ctx->pool_max,
+        PF_CUDA(cudaMemcpyAsync(ctx->pool.d_has, ctx->pool.has.data(), ctx->pool.max,
                                 cudaMemcpyHostToDevice, st));
     std::fill(B->row_touched.begin(), B->row_touched.end(), 0);
     B->any_evicted = false;
@@ -1156,8 +1150,8 @@ extern "C" int pfnav_pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *de
                "position outside the map");
     }
     PF_NEED_DEVICE(ctx);
-    PF_ARG(ctx->d_pool_slot, "pool not created");
-    for (int i = 0; i < n; i++) PF_ARG(dests[i] < ctx->pool_ndests, "dest");
+    PF_ARG(ctx->pool.d_slot, "pool not created");
+    for (int i = 0; i < n; i++) PF_ARG(dests[i] < ctx->pool.ndests, "dest");
     if (n == 0) return PFNAV_OK;
     return pool_request_paths(ctx, n, dests, layer, src_xz, dst_xz, stream, out_dest_ids, out_ok, out_n_flow, out_n_los, out_ndone);
 }
@@ -1168,9 +1162,9 @@ extern "C" int pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, floa
                                        float dst_z, void *stream, uint32_t *out_dest_id, int *out_ok, int *out_n_flow,
                                        int *out_n_los)
 {
-    PF_ARG(ctx && ctx->d_pool_slot, "pool not created");
+    PF_ARG(ctx && ctx->pool.d_slot, "pool not created");
     PF_NEED_DEVICE(ctx);
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests, "dest");
+    PF_ARG(dest >= 0 && dest < ctx->pool.ndests, "dest");
     PF_ARG(route_layer(ctx, layer), "pfnav_route_build not called");
     const float s[2] = {src_x, src_z}, d[2] = {dst_x, dst_z};
     tdesc t;
@@ -1184,26 +1178,6 @@ extern "C" int pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, floa
     if (out_n_flow) *out_n_flow = nf;
     if (out_n_los) *out_n_los = nl;
     return rc;
-}
-
-// Read one pool entry back to the host (4096 B each; either pointer may be NULL). *out_has: bit0 flow, bit1 LOS.
-extern "C" int pfnav_pool_get(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, uint8_t *flow_out, uint8_t *los_out,
-                              int *out_has, uint64_t *out_ffid)
-{
-    PF_ARG(ctx && ctx->d_pool_slot && out_has, "args");
-    PF_NEED_DEVICE(ctx);
-    PF_ARG(dest >= 0 && dest < ctx->pool_ndests && chunk_r >= 0 && chunk_r < ctx->chunk_h && chunk_c >= 0 && chunk_c < ctx->chunk_w, "dest/chunk");
-    const size_t si = (size_t)dest * ctx->chunk_w * ctx->chunk_h + chunk_r * ctx->chunk_w + chunk_c;
-    const int slot = ctx->h_pool_slot[si];
-    *out_has = slot < 0 ? 0 : ctx->h_pool_has[slot];
-    if (out_ffid) *out_ffid = ctx->h_pool_ffid[si];
-    if (slot < 0) return PFNAV_OK;
-    PF_CUDA(cudaSetDevice(ctx->device));
-    PF_CUDA(pf_pool_refresh(ctx, ctx->tick_stream));
-    PF_CUDA(cudaDeviceSynchronize());
-    if (flow_out && (*out_has & 1)) PF_CUDA(cudaMemcpy(flow_out, ctx->d_pool_flow + (size_t)slot * 4096, 4096, cudaMemcpyDeviceToHost));
-    if (los_out && (*out_has & 2)) PF_CUDA(cudaMemcpy(los_out, ctx->d_pool_los + (size_t)slot * 4096, 4096, cudaMemcpyDeviceToHost));
-    return PFNAV_OK;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -148,5 +148,45 @@ def test_clear_then_tick_get_repair_see_empty_pool(pf):
         nav.close()
 
 
+def test_resident_plan_only_on_an_unchanged_pool(pf):
+    """A repeated identical goal batch relaunches its resident plan without planning again. A pool_put, a pool_clear, a
+    map_commit that drops fields, a zone batch or an entity-field batch changes the pool under the plan: the next
+    identical batch plans again."""
+    capi = pf.capi
+    nav, W, dests, targets = _setup(pf, agents=False)
+    try:
+        nav.profile_enable(True)
+        x, z = -(100 * 4 + 2.0), 100 * 4 + 2.0              # world position of tile (100, 100), in chunk (1, 1)
+        zone = np.zeros(1, capi.ZONE_REQ)
+        zone["dest"], zone["centre_x"], zone["centre_z"], zone["radius"] = 0, x, z, 6
+        ent = np.zeros(1, capi.ENTITY_FIELD_REQ)
+        ent["dest"], ent["target_kind"], ent["ent_n"], ent["chunk_n"] = 1, capi.TARGET_ENTITY, 1, 1
+        fp = np.zeros(1, capi.FOOTPRINT)
+        fp["x"], fp["z"], fp["sel_radius"] = x, z, 3.0
+
+        def commit():
+            nav.blockers_incref(x, z, 3.0)
+            assert nav.map_commit() > 0
+
+        changes = {"put": lambda: nav.pool_put(0, (0, 0), flow=np.zeros(4096, np.uint8)),
+                   "clear": nav.pool_clear,
+                   "commit": commit,
+                   "zones": lambda: nav.pool_request_zones(zone),
+                   "entity": lambda: nav.pool_request_entity_fields_batch(ent, fp, np.array([[1, 1]], np.int32))}
+
+        def plans():            # planning passes of one goal batch (profile_read_host returns the counts since its last call)
+            nav.pool_request_goals(dests, targets, 0)
+            return nav.profile_read_host()["plan"][1]
+
+        assert plans() == 1
+        assert plans() == 0, "the repeated batch planned again"
+        for name, change in changes.items():
+            change()
+            assert plans() == 1, "the batch after %s reused the resident plan" % name
+            assert plans() == 0, "the repeated batch after %s planned again" % name
+    finally:
+        nav.close()
+
+
 if __name__ == "__main__":
     print(cold_batch_digest(importlib.import_module("permafrost-engine_b200")))
