@@ -910,6 +910,66 @@ int  pfnav_agents_set_blocking(pfnav_ctx *ctx, const uint32_t *uids, size_t n, i
 /* Read the (updated) entity snapshot back: agents_out / ms_out may be NULL. */
 int  pfnav_agents_read_state(pfnav_ctx *ctx, pfnav_agent *agents_out, pfnav_movestate *ms_out, size_t maxout);
 
+/* Movement commands as deltas (SURVEY 7: the host pushes deltas, not whole-state re-uploads). One record is one entity's
+ * change as move_process_cmds (movement.c:3246) leaves it in the engine's own tables; which state or flock an order gives
+ * stays the engine's decision (make_flock, movement.c:855-862). Fields are written in the order of the mask bits. 64 bytes. */
+#define PFNAV_DELTA_STATE        (1u << 0)   /* agent.state = state                                                      */
+#define PFNAV_DELTA_FLOCK        (1u << 1)   /* agent.flock = flock (-1: none): an index into the flock table AFTER the call */
+#define PFNAV_DELTA_AUX_DEST     (1u << 2)   /* agent.aux_dest1                                                          */
+#define PFNAV_DELTA_FLAGS        (1u << 3)   /* agent.flags = flags & 0xFFFFFF (GARRISONED, COMBAT_HELD, WATER / AIR ...)  */
+#define PFNAV_DELTA_SPEEDS       (1u << 4)   /* agent.max_speed, agent.speed                                             */
+#define PFNAV_DELTA_RADIUS       (1u << 5)   /* agent.radius (may move the entity to another navigation layer)           */
+#define PFNAV_DELTA_VELOCITY     (1u << 6)   /* agent.velocity (the velocity history is not touched)                     */
+#define PFNAV_DELTA_POSITION     (1u << 7)   /* teleport (MOVE_CMD_UPDATE_POS): pos = prev_pos = position,
+                                              * movestate.next_pos x and z = position, step = 0, left = 0                */
+#define PFNAV_DELTA_CLEAR_HIST   (1u << 8)   /* move_notify_motion_start: zero movestate.vel_hist unless the entity is
+                                              * COMBAT_HELD at that point -- pfnav_agents_apply_updates' SET_MOVING rule   */
+#define PFNAV_DELTA_TARGET       (1u << 9)   /* movestate_ext.surround_target_uid = target_uid (PFNAV_NULL_UID: none),
+                                              * movestate_ext.target_range = target_range                                */
+typedef struct pfnav_agent_delta {
+    uint32_t uid, mask;
+    uint32_t state;
+    int32_t  flock;
+    uint32_t aux_dest1, flags;
+    float    position[2], velocity[2], max_speed, speed, radius;
+    uint32_t target_uid;
+    float    target_range;
+    uint32_t _pad;
+} pfnav_agent_delta;
+/* Apply n deltas (HOST array) to the device-resident population, and optionally replace the flock table.
+ * - flocks == NULL: the flock table is unchanged (nflocks is ignored). Otherwise flocks[0 .. nflocks) is the whole new
+ *   table: it may grow, shrink (when no entity keeps an index it drops) and entries may change.
+ * - deltas and flocks are read before the call returns, whatever memory they are in: they can be reused at once.
+ * - Deltas apply in array order; several deltas for one uid compose exactly as if applied one after the other.
+ * - Everything is validated before anything changes: uid in the context's own range, no unknown mask bit, state within
+ *   enum pfnav_move_state, -1 <= flock < the table's length after the call, finite floats, the entity's resulting
+ *   navigation layer (Entity_NavLayerWithRadius of its flags and radius) created, POSITION / CLEAR_HIST only with an
+ *   uploaded movestate table, TARGET only with an uploaded movestate_ext table and target_uid inside the population.
+ *   Failure: PFNAV_ERR_ARG, device and host state untouched.
+ * - Flock member lists (when a delta carried FLOCK or the table's length changed), neighbour records and the facts the
+ *   tick keeps on the host (largest radius, any GARRISONED, arrival constants per (flock, layer) in use) are brought to
+ *   what pfnav_agents_upload of the resulting population would leave. Member lists are rebuilt on the device.
+ * - Asynchronous on `stream`, ordered like pfnav_agents_apply_updates_ex, except that it waits for the stream to read
+ *   the new flock offsets (nflocks + 1 words) when the member lists were rebuilt and 8 bytes of population facts when a
+ *   delta carried RADIUS or FLAGS. The device flock buffers and the call's scratch regrow (a device synchronisation)
+ *   when the table or the batch outgrows them.
+ * - Like pfnav_agents_apply_updates it leaves the spatial index stale: follow with pfnav_agents_rebuild_index. It does
+ *   not touch the blocking table (pfnav_agents_set_blocking is the call for that) or the work list
+ *   (pfnav_agents_set_work_dev).
+ * - PFNAV_ERR_NO_DEVICE on a host-only context. PFNAV_ERR_STATE (nothing changed) on a context in a multi-GPU job
+ *   (pfnav_mgpu_init / pfnav_group_create, or an own range that is not the whole population). */
+int  pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n,
+                           const pfnav_flock *flocks, size_t nflocks, void *stream);
+/* pfnav_agents_set_work(ctx, NULL, 0) from the state resident on the device: the uids of the context's own range whose
+ * state is neither ARRIVED nor WAITING, ascending, compacted on the device on `stream`. It waits for the stream once, to
+ * read the 4-byte count that sizes the per-work-item buffers; it waits for the whole device only when the list outgrows
+ * those buffers (they are then reallocated with room to spare) or the call's scratch has to grow. out_nwork may be NULL.
+ * pfnav_agents_commands and this call share one device scratch buffer: order them on one stream (or with an event). */
+int  pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *out_nwork);
+/* Inspection and tests only, not for the tick loop: the current work list, in order. It waits for the whole device.
+ * *out_n: the list's length; at most maxout uids are written (out may be NULL when maxout is 0). */
+int  pfnav_agents_read_work(pfnav_ctx *ctx, uint32_t *out, size_t maxout, size_t *out_n);
+
 /* N_FlowFieldUpdate with TARGET_ENEMIES / TARGET_ENTITY straight into the pool (what N_RequestAsyncEnemySeekField /
  * N_RequestAsyncSurroundField + N_AwaitAsyncFields leave in the field cache, nav.c:3769-3960): the fields of the listed
  * chunks become the flow fields of pool destination `dest`; entities name it through pfnav_agent::aux_dest1. The

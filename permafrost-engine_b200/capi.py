@@ -66,6 +66,13 @@ BLOCKING = np.dtype([("blocking", "<u4"), ("faction_id", "<i4"), ("stop_x", "<f4
                      ("_pad", "<u4", 3)])
 assert BLOCKING.itemsize == 32
 APPLY_BLOCKERS = 1
+AGENT_DELTA = np.dtype([
+    ("uid", "<u4"), ("mask", "<u4"), ("state", "<u4"), ("flock", "<i4"), ("aux_dest1", "<u4"), ("flags", "<u4"),
+    ("position", "<f4", 2), ("velocity", "<f4", 2), ("max_speed", "<f4"), ("speed", "<f4"), ("radius", "<f4"),
+    ("target_uid", "<u4"), ("target_range", "<f4"), ("_pad", "<u4")])
+assert AGENT_DELTA.itemsize == 64
+(DELTA_STATE, DELTA_FLOCK, DELTA_AUX_DEST, DELTA_FLAGS, DELTA_SPEEDS, DELTA_RADIUS, DELTA_VELOCITY, DELTA_POSITION,
+ DELTA_CLEAR_HIST, DELTA_TARGET) = (1 << i for i in range(10))
 TODO_SURROUND_QUERY, TODO_USE_SURROUND_FIELD, TODO_DROP_SURROUND_FIELD = 1, 2, 4
 
 REGION_REQ = np.dtype([
@@ -123,6 +130,7 @@ SYMBOLS = [
     "pfnav_mgpu_request_goals_ex", "pfnav_group_request_goals_ex", "pfnav_mgpu_fields_stats",
     "pfnav_mgpu_request_zones", "pfnav_group_request_zones", "pfnav_mgpu_request_entity_fields_batch",
     "pfnav_group_request_entity_fields_batch",
+    "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
 ]
 
 _lib = None
@@ -192,6 +200,9 @@ def load():
     L.pfnav_agents_read_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_set_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
     L.pfnav_agents_read_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_agents_commands.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_agents_set_work_dev.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
+    L.pfnav_agents_read_work.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.pfnav_map_refresh_chunk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
@@ -947,6 +958,29 @@ class Nav:
         """the engine's entity_block (block=True) / entity_unblock for the listed uids; repeats change nothing"""
         u = np.ascontiguousarray(uids, np.uint32).reshape(-1)
         _chk(self.L.pfnav_agents_set_blocking(self.h, _p(u) if len(u) else None, len(u), 1 if block else 0, C.c_void_p(stream)))
+
+    def agents_commands(self, deltas, flocks=None, stream=0):
+        """pfnav_agents_commands: AGENT_DELTA records applied in order; flocks (FLOCK records): the whole new flock
+        table, None: unchanged. Follow with agents_rebuild_index."""
+        d = np.ascontiguousarray(deltas, AGENT_DELTA).reshape(-1)
+        fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
+        fp = None if fl is None else _p(fl if len(fl) else np.zeros(1, FLOCK))     # an empty table is still a table
+        _chk(self.L.pfnav_agents_commands(self.h, _p(d) if len(d) else None, len(d), fp, 0 if fl is None else len(fl),
+                                          C.c_void_p(stream)))
+
+    def agents_set_work_dev(self, stream=0):
+        """pfnav_agents_set_work_dev: agents_set_work(None) built on the device -> the number of work items"""
+        n = C.c_size_t(0)
+        _chk(self.L.pfnav_agents_set_work_dev(self.h, C.c_void_p(stream), C.byref(n)))
+        self.nwork = n.value
+        return n.value
+
+    def agents_read_work(self):
+        n = C.c_size_t(0)
+        _chk(self.L.pfnav_agents_read_work(self.h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, np.uint32)
+        _chk(self.L.pfnav_agents_read_work(self.h, _p(out) if n.value else None, n.value, C.byref(n)))
+        return out
 
     def agents_read_state(self, n, movestate=True):
         a = np.zeros(n, AGENT)

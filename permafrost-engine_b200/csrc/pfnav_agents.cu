@@ -958,6 +958,7 @@ void pfnav_agents_free(pfnav_ctx *ctx)
     cudaFree(ctx->d_rep_buf); ctx->d_rep_buf = nullptr; ctx->rep_buf_bytes = 0;
     cudaFree(ctx->d_blocking); ctx->d_blocking = nullptr; ctx->blocking_n = 0;
     cudaFree(ctx->d_block_uids); ctx->d_block_uids = nullptr; ctx->cap_block_uids = 0;
+    cudaFree(ctx->d_cmd_buf); ctx->d_cmd_buf = nullptr; ctx->cmd_buf_bytes = 0;
     ctx->d_agents = nullptr; ctx->d_records = nullptr; ctx->d_flocks = nullptr; ctx->d_flock_start = nullptr;
     ctx->d_flock_members = nullptr; ctx->d_cohesion = nullptr; ctx->d_cell_count = nullptr; ctx->d_cell_start = nullptr;
     ctx->d_cell_fill = nullptr; ctx->d_sorted_ix = nullptr; ctx->d_sorted_iy = nullptr; ctx->d_sorted_id = nullptr;
@@ -1119,6 +1120,7 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
         // what the host needs to know about the entities it will run work items for (its own range)
         ctx->flock_layer_used.assign(nflocks * PFNAV_NAV_LAYER_MAX, 0);
         ctx->has_unsupported_state = false;
+        ctx->cmd_mirror.reset(hi - lo, nflocks);      // (flock, layer) per own entity, for pfnav_agents_commands
         for (size_t i = 0; i < hi - lo; i++) {
             PF_ARG(agents[i].flock < (int)nflocks, "agent flock index out of range");
             // Entity_NavLayerWithRadius (entity.c:554): the layer this agent's tile probes read
@@ -1127,6 +1129,7 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
             const int layer = base + (r >= 15.0f ? 3 : r >= 10.0f ? 2 : r >= 5.0f ? 1 : 0);
             PF_ARG(layer < ctx->nlayers, "agent needs a navigation layer that was not created (radius/flags)");
             if (agents[i].flock >= 0) ctx->flock_layer_used[(size_t)agents[i].flock * PFNAV_NAV_LAYER_MAX + layer] = 1;
+            ctx->cmd_mirror.set(i, std::max(agents[i].flock, -1), layer);
             const uint32_t stt = agents[i].state;
             if (stt == PFNAV_STATE_MOVING_IN_FORMATION || stt == PFNAV_STATE_SURROUND_ENTITY ||
                 stt == PFNAV_STATE_ENTER_ENTITY_RANGE || stt == PFNAV_STATE_TURNING || stt == PFNAV_STATE_ARRIVING_TO_CELL)
@@ -1176,21 +1179,25 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
     return pfnav_agents_finish_snapshot(ctx, st, !same);
 }
 
+int pfnav_agents_refresh_facts(pfnav_ctx *ctx, cudaStream_t st)
+{
+    const int n = (int)ctx->n_agents;
+    PF_CUDA(cudaMemsetAsync(ctx->d_facts, 0, 8, st));
+    if (n) { k_population_facts<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(ctx->d_records, n, ctx->d_facts); ctx->launches++; }
+    uint32_t facts[2] = {0, 0};
+    PF_CUDA(cudaMemcpyAsync(facts, ctx->d_facts, 8, cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    memcpy(&ctx->max_radius, &facts[0], 4);
+    ctx->any_garrisoned = facts[1] != 0;
+    return PFNAV_OK;
+}
+
 // Everything that needs the WHOLE population's records: member lists, population facts, spatial index.
 int pfnav_agents_finish_snapshot(pfnav_ctx *ctx, cudaStream_t st, bool members)
 {
     int rc;
-    const int n = (int)ctx->n_agents;
     if (members && (rc = rebuild_flock_members(ctx, st))) return rc;
-    if (members) {
-        PF_CUDA(cudaMemsetAsync(ctx->d_facts, 0, 8, st));
-        if (n) { k_population_facts<<<std::min((n + 255) / 256, 1024), 256, 0, st>>>(ctx->d_records, n, ctx->d_facts); ctx->launches++; }
-        uint32_t facts[2] = {0, 0};
-        PF_CUDA(cudaMemcpyAsync(facts, ctx->d_facts, 8, cudaMemcpyDeviceToHost, st));
-        PF_CUDA(cudaStreamSynchronize(st));
-        memcpy(&ctx->max_radius, &facts[0], 4);
-        ctx->any_garrisoned = facts[1] != 0;
-    }
+    if (members && (rc = pfnav_agents_refresh_facts(ctx, st))) return rc;
     if ((rc = build_index(ctx, st))) return rc;
     PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;

@@ -1,0 +1,345 @@
+// pfnav_commands.cu -- the engine's movement commands on the device-resident population (sm_90a).
+//
+// pfnav_agents_commands applies per-entity deltas (pfnav_commands_host.h validates and merges them, one record per uid)
+// with one thread per entity, replaces the flock table, and rebuilds the flock member lists from the flock id column
+// with a stable counting sort: every warp owns a contiguous uid range, counts its entities per flock, the counts are
+// scanned per flock across the warps and over the flocks, and every warp writes its entities behind the offsets of its
+// range. Members are therefore ascending by uid within a flock, as the host pass of an upload leaves them.
+// pfnav_agents_set_work_dev compacts the uids that are not still into the work list, in uid order.
+#include "pfnav_internal.cuh"
+#include <algorithm>
+
+#define FULL 0xFFFFFFFFu
+
+__global__ void k_apply_deltas(const pfnav_agent_delta *__restrict__ deltas, int n, pfnav_agent *__restrict__ agents,
+                               pfnav_movestate *__restrict__ mss, pfnav_movestate_ext *__restrict__ exts,
+                               int32_t *__restrict__ flock_of, pf_record *__restrict__ rec)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const pfnav_agent_delta d = deltas[i];
+    pfnav_agent a = agents[d.uid];
+    // the host refuses the bits that write a table that was not uploaded, so these pointers are valid when used
+    pf_delta_apply(&a, mss ? mss + d.uid : nullptr, exts ? exts + d.uid : nullptr, d);
+    agents[d.uid] = a;
+    flock_of[d.uid] = a.flock;
+    pf_record r;                       // as k_make_records / k_entity_apply pack it
+    r.px = a.pos[0]; r.pz = a.pos[1]; r.vx = a.velocity[0]; r.vz = a.velocity[1];
+    r.radius = a.radius;
+    r.state_flags = (a.state << 24) | (a.flags & 0xFFFFFFu);
+    rec[d.uid] = r;
+}
+
+// ---- flock member lists: stable counting sort of the uids by flock ----
+// Warp w owns uids [w * per, (w + 1) * per), per a multiple of 32; hist is [nflocks][W]. Only the warp itself touches
+// its column, one leader lane per flock and step, so plain read-modify-writes ordered by __syncwarp are enough.
+__global__ void k_flock_hist(const int32_t *__restrict__ flock_of, int n, int per, int W, uint32_t *hist)
+{
+    const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (w >= W) return;
+    const int lo = w * per, hi = min(lo + per, n);
+    for (int base = lo; base < hi; base += 32) {
+        const int i = base + lane;
+        const int32_t f = i < hi ? flock_of[i] : -1;
+        const unsigned m = __match_any_sync(FULL, f);
+        if (f >= 0 && lane == __ffs(m) - 1) hist[(size_t)f * W + w] += __popc(m);
+        __syncwarp();
+    }
+}
+
+// exclusive scan over the 1024 threads of a block; wsum: 32 words of shared memory; total: the block's sum
+__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *wsum, uint32_t &total)
+{
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t x = v;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, x, o); if (lane >= o) x += y; }
+    if (lane == 31) wsum[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        uint32_t s = wsum[lane];
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, s, o); if (lane >= o) s += y; }
+        wsum[lane] = s;
+    }
+    __syncthreads();
+    const uint32_t before = wid ? wsum[wid - 1] : 0;
+    total = wsum[31];
+    __syncthreads();
+    return before + x - v;
+}
+
+// block f: the counts of flock f become each warp's offset within the flock; the flock's size goes to start[f + 1]
+__global__ void __launch_bounds__(1024) k_flock_scan(uint32_t *hist, int W, uint32_t *__restrict__ start)
+{
+    __shared__ uint32_t wsum[32];
+    uint32_t *row = hist + (size_t)blockIdx.x * W;
+    uint32_t carry = 0;
+    for (int base = 0; base < W; base += 1024) {
+        const int w = base + threadIdx.x;
+        const uint32_t v = w < W ? row[w] : 0;
+        uint32_t total;
+        const uint32_t e = block_excl_scan(v, wsum, total);
+        if (w < W) row[w] = carry + e;
+        carry += total;
+    }
+    if (threadIdx.x == 0) start[blockIdx.x + 1] = carry;
+}
+
+// one block: start[1 .. nflocks] holds the flock sizes; make start[0 .. nflocks] the offsets
+__global__ void __launch_bounds__(1024) k_flock_starts(uint32_t *__restrict__ start, int nflocks)
+{
+    __shared__ uint32_t wsum[32];
+    uint32_t carry = 0;
+    for (int base = 0; base < nflocks; base += 1024) {
+        const int f = base + threadIdx.x;
+        const uint32_t v = f < nflocks ? start[f + 1] : 0;
+        uint32_t total;
+        const uint32_t e = block_excl_scan(v, wsum, total);
+        if (f < nflocks) start[f + 1] = carry + e + v;
+        carry += total;
+    }
+    if (threadIdx.x == 0) start[0] = 0;
+}
+
+__global__ void k_flock_scatter(const int32_t *__restrict__ flock_of, int n, int per, int W, uint32_t *hist,
+                                const uint32_t *__restrict__ start, uint32_t *__restrict__ members)
+{
+    const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (w >= W) return;
+    const int lo = w * per, hi = min(lo + per, n);
+    for (int base = lo; base < hi; base += 32) {
+        const int i = base + lane;
+        const int32_t f = i < hi ? flock_of[i] : -1;
+        const unsigned m = __match_any_sync(FULL, f);
+        const int leader = __ffs(m) - 1;
+        uint32_t off = 0;
+        if (f >= 0 && lane == leader) { off = hist[(size_t)f * W + w]; hist[(size_t)f * W + w] = off + __popc(m); }
+        off = __shfl_sync(FULL, off, leader);
+        if (f >= 0) members[start[f] + off + __popc(m & ((1u << lane) - 1))] = (uint32_t)i;
+        __syncwarp();
+    }
+}
+
+// ---- work list: the own range's uids that are not still (ent_still, movement.c:652), ascending ----
+// Block b owns uids [lo + b * per, lo + (b + 1) * per), per a multiple of 1024.
+// The state is read from the 24-byte neighbour records (state << 24 | flags), which every writer of agent.state keeps
+// current (k_make_records, k_entity_apply, k_apply_deltas): a seventh of the agent table's stride.
+__device__ __forceinline__ bool not_still(const pf_record *__restrict__ rec, int i)
+{
+    const uint32_t s = rec[i].state_flags >> 24;
+    return s != PFNAV_STATE_ARRIVED && s != PFNAV_STATE_WAITING;
+}
+
+__global__ void __launch_bounds__(1024) k_work_count(const pf_record *__restrict__ rec, int lo, int hi, int per,
+                                                     uint32_t *__restrict__ part)
+{
+    __shared__ uint32_t wsum[32];
+    const int b0 = lo + blockIdx.x * per, b1 = min(b0 + per, hi);
+    uint32_t c = 0;
+    for (int i = b0 + threadIdx.x; i < b1; i += 1024) c += not_still(rec, i) ? 1u : 0u;
+    uint32_t total;
+    block_excl_scan(c, wsum, total);
+    if (threadIdx.x == 0) part[blockIdx.x] = total;
+}
+
+// one block: part[0 .. nb) (nb <= 1024) become offsets, part[nb] the number of work items
+__global__ void __launch_bounds__(1024) k_work_scan(uint32_t *__restrict__ part, int nb)
+{
+    __shared__ uint32_t wsum[32];
+    const uint32_t v = (int)threadIdx.x < nb ? part[threadIdx.x] : 0;
+    uint32_t total;
+    const uint32_t e = block_excl_scan(v, wsum, total);
+    if ((int)threadIdx.x < nb) part[threadIdx.x] = e;
+    if (threadIdx.x == 0) part[nb] = total;
+}
+
+__global__ void __launch_bounds__(1024) k_work_compact(const pf_record *__restrict__ rec, int lo, int hi, int per,
+                                                       const uint32_t *__restrict__ part, uint32_t *__restrict__ work)
+{
+    __shared__ uint32_t wsum[32];
+    const int b0 = lo + blockIdx.x * per, b1 = min(b0 + per, hi);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t out = part[blockIdx.x];
+    for (int base = b0; base < b1; base += 1024) {
+        const int i = base + threadIdx.x;
+        const bool keep = i < b1 && not_still(rec, i);
+        const unsigned bal = __ballot_sync(FULL, keep);
+        if (lane == 0) wsum[wid] = __popc(bal);
+        __syncthreads();
+        if (wid == 0) {
+            uint32_t s = wsum[lane];
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, s, o); if (lane >= o) s += y; }
+            wsum[lane] = s;
+        }
+        __syncthreads();
+        if (keep) work[out + (wid ? wsum[wid - 1] : 0) + __popc(bal & ((1u << lane) - 1))] = (uint32_t)i;
+        out += wsum[31];
+        __syncthreads();
+    }
+}
+
+// ------------------------------------------------------------------------------------------
+// Host side
+// ------------------------------------------------------------------------------------------
+static int cmd_buf(pfnav_ctx *ctx, size_t bytes)
+{
+    if (bytes <= ctx->cmd_buf_bytes) return 0;
+    cudaFree(ctx->d_cmd_buf); ctx->d_cmd_buf = nullptr; ctx->cmd_buf_bytes = 0;       // waits for the device
+    bytes = std::max<size_t>(bytes + bytes / 2, 1 << 16);
+    PF_CUDA(cudaMalloc(&ctx->d_cmd_buf, bytes));
+    ctx->cmd_buf_bytes = bytes;
+    return 0;
+}
+
+template <typename T>
+static int regrow(T *&p, size_t count)
+{
+    cudaFree(p); p = nullptr;
+    PF_CUDA(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
+    return 0;
+}
+
+// d_flock_start / d_flock_members from d_flock_of on `st`; hist: nflocks * W words of scratch
+static int members_on_device(pfnav_ctx *ctx, cudaStream_t st, uint32_t *hist, int per, int W)
+{
+    const int n = (int)ctx->n_agents, nflocks = (int)ctx->n_flocks;
+    PF_CUDA(cudaMemsetAsync(ctx->d_flock_start, 0, ((size_t)nflocks + 1) * 4, st));
+    if (n && nflocks) {
+        PF_CUDA(cudaMemsetAsync(hist, 0, (size_t)nflocks * W * 4, st));
+        PF_CUDA(cudaMemsetAsync(ctx->d_flock_members, 0, (size_t)n * 4, st));      // the tail behind the last flock, as an upload leaves it
+        const int ctas = (W + 7) / 8;
+        k_flock_hist<<<ctas, 256, 0, st>>>(ctx->d_flock_of, n, per, W, hist);
+        k_flock_scan<<<nflocks, 1024, 0, st>>>(hist, W, ctx->d_flock_start);
+        k_flock_starts<<<1, 1024, 0, st>>>(ctx->d_flock_start, nflocks);
+        k_flock_scatter<<<ctas, 256, 0, st>>>(ctx->d_flock_of, n, per, W, hist, ctx->d_flock_start, ctx->d_flock_members);
+        ctx->launches += 4;
+        PF_CUDA(cudaGetLastError());
+    }
+    // the tick sizes its cohesion pass from the biggest flock
+    std::vector<uint32_t> fstart((size_t)nflocks + 1, 0);
+    PF_CUDA(cudaMemcpyAsync(fstart.data(), ctx->d_flock_start, fstart.size() * 4, cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    ctx->h_flock_start.swap(fstart);
+    return 0;
+}
+
+extern "C" int pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks,
+                                     size_t nflocks, void *stream)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_agents, "agents not uploaded");
+    if (ctx->mgpu || ctx->shard_lo > 0 || ctx->shard_hi < ctx->n_agents) {
+        pfnav_set_error("pfnav_agents_commands: the context is part of a multi-GPU job (the other members would keep the old "
+                        "flock table and flock column)");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(deltas || n == 0, "deltas == NULL");
+    PF_ARG(n < (1u << 31) && nflocks < (1u << 31), "n / nflocks");
+    if (!flocks) nflocks = ctx->n_flocks;
+    pf_cmd_limits lim = {ctx->shard_lo, ctx->shard_hi, ctx->n_agents, nflocks, ctx->movestate_set && ctx->d_movestate != nullptr,
+                         ctx->d_ms_ext != nullptr};
+    std::vector<pfnav_agent_delta> merged;
+    std::vector<pf_cmd_change> changes;
+    const char *err = pf_cmd_merge(deltas, n, lim, merged);
+    if (!err) err = pf_cmd_plan(ctx->cmd_mirror, ctx->shard_lo, merged, nflocks, ctx->nlayers, changes);
+    PF_ARG(!err, err);
+    if (merged.empty() && !flocks) return PFNAV_OK;
+    uint32_t any = 0;
+    for (const pfnav_agent_delta &m : merged) any |= m.mask;
+    const bool members = (any & PFNAV_DELTA_FLOCK) || nflocks != ctx->n_flocks;
+
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    int rc;
+    // warps of the member sort: at most 4096 ranges, and at most 16 M histogram words
+    const size_t max_w = std::max<size_t>(1, std::min<size_t>(4096, ((size_t)1 << 24) / std::max<size_t>(nflocks, 1)));
+    const int per = (int)(((ctx->n_agents + max_w - 1) / max_w + 31) / 32 * 32);
+    const int W = per ? (int)((ctx->n_agents + per - 1) / per) : 0;
+    const size_t b_deltas = merged.size() * sizeof(pfnav_agent_delta);
+    if ((rc = cmd_buf(ctx, b_deltas + (members ? nflocks * (size_t)W * 4 : 0)))) return rc;
+    if (nflocks + 1 > ctx->cap_flocks) {       // keeps no content: the table follows, the offsets are rebuilt (members)
+        PF_CUDA(cudaDeviceSynchronize());
+        const size_t cap = std::max(nflocks + 1, ctx->cap_flocks * 2);
+        if ((rc = regrow(ctx->d_flocks, cap))) return rc;
+        if ((rc = regrow(ctx->d_flock_start, cap + 1))) return rc;
+        ctx->cap_flocks = cap;
+    }
+    if (flocks) {
+        // from the context's own pageable copy, which is staged before the call returns: the caller's array may be pinned
+        ctx->h_flocks.assign(flocks, flocks + nflocks);
+        if (nflocks) PF_CUDA(cudaMemcpyAsync(ctx->d_flocks, ctx->h_flocks.data(), nflocks * sizeof(pfnav_flock), cudaMemcpyHostToDevice, st));
+        ctx->n_flocks = nflocks;
+    }
+    if (!merged.empty()) {
+        PF_CUDA(cudaMemcpyAsync(ctx->d_cmd_buf, merged.data(), b_deltas, cudaMemcpyHostToDevice, st));
+        k_apply_deltas<<<((int)merged.size() + 127) / 128, 128, 0, st>>>((const pfnav_agent_delta *)ctx->d_cmd_buf, (int)merged.size(),
+            ctx->d_agents, lim.have_ms ? ctx->d_movestate : nullptr, ctx->d_ms_ext, ctx->d_flock_of, ctx->d_records);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+    }
+    // host facts, as a fresh upload of the resulting population would leave them
+    pf_cmd_commit(ctx->cmd_mirror, changes, nflocks);
+    std::vector<uint8_t> used;
+    ctx->cmd_mirror.used(used);
+    if (flocks || used != ctx->flock_layer_used) ctx->arrival_valid = false;
+    ctx->flock_layer_used.swap(used);
+    if (members && (rc = members_on_device(ctx, st, (uint32_t *)((uint8_t *)ctx->d_cmd_buf + b_deltas), per, W))) return rc;
+    if ((any & (PFNAV_DELTA_RADIUS | PFNAV_DELTA_FLAGS)) && (rc = pfnav_agents_refresh_facts(ctx, st))) return rc;
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *out_nwork)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_agents, "agents not uploaded");
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    const int lo = (int)ctx->shard_lo, hi = (int)ctx->shard_hi, cnt = hi - lo;
+    int rc;
+    uint32_t nwork = 0;
+    const int nb = std::min(1024, (cnt + 1023) / 1024);
+    const int per = nb ? ((cnt + nb - 1) / nb + 1023) / 1024 * 1024 : 0;
+    if (cnt) {
+        if ((rc = cmd_buf(ctx, ((size_t)nb + 1) * 4))) return rc;
+        uint32_t *part = (uint32_t *)ctx->d_cmd_buf;
+        k_work_count<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, part);
+        k_work_scan<<<1, 1024, 0, st>>>(part, nb);
+        ctx->launches += 2;
+        PF_CUDA(cudaGetLastError());
+        PF_CUDA(cudaMemcpyAsync(&nwork, part + nb, 4, cudaMemcpyDeviceToHost, st));
+        PF_CUDA(cudaStreamSynchronize(st));
+    }
+    if (nwork > ctx->cap_work) {
+        // room to spare: units wake a few at a time, and every regrowth waits for the device
+        const size_t cap = std::min<size_t>((size_t)cnt, (size_t)nwork + nwork / 4 + 1024);
+        PF_CUDA(cudaDeviceSynchronize());
+        if ((rc = regrow(ctx->d_work, cap))) return rc;
+        if ((rc = regrow(ctx->d_vel_out, cap))) return rc;
+        if ((rc = regrow(ctx->d_vpref_out, cap))) return rc;
+        if ((rc = regrow(ctx->d_vdes_out, cap))) return rc;
+        if ((rc = regrow(ctx->d_los_out, cap))) return rc;
+        ctx->cap_work = cap;
+    }
+    if (!ctx->d_work_count) PF_CUDA(cudaMalloc(&ctx->d_work_count, 16));
+    if (nwork) {
+        k_work_compact<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, (const uint32_t *)ctx->d_cmd_buf, ctx->d_work);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+    }
+    ctx->n_work = nwork;
+    if (out_nwork) *out_nwork = nwork;
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_agents_read_work(pfnav_ctx *ctx, uint32_t *out, size_t maxout, size_t *out_n)
+{
+    PF_ARG(ctx && ctx->d_agents, "agents not uploaded");
+    PF_ARG(out || maxout == 0, "out == NULL");
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(cudaDeviceSynchronize());
+    const size_t n = std::min(maxout, ctx->n_work);
+    if (n) PF_CUDA(cudaMemcpy(out, ctx->d_work, n * 4, cudaMemcpyDeviceToHost));
+    if (out_n) *out_n = ctx->n_work;
+    return PFNAV_OK;
+}

@@ -12,6 +12,7 @@
 #include <vector>
 #include "../../include/pfnav.h"
 #include "pfnav_pool_host.h"
+#include "pfnav_commands_host.h"
 
 #define PFNAV_VERSION 100
 
@@ -190,6 +191,10 @@ struct pfnav_ctx {
     // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
     pfnav_blocking *d_blocking = nullptr; size_t blocking_n = 0; bool blocking_any_fac = false;
     uint32_t *d_block_uids = nullptr; size_t cap_block_uids = 0;
+    // pfnav_agents_commands (pfnav_commands.cu): (flock, layer) of every own entity, filled by every full upload, and the device
+    // scratch of a batch (merged deltas, per-warp flock histograms, block sums of the work compaction), grown on demand
+    pf_cmd_mirror cmd_mirror;
+    void *d_cmd_buf = nullptr; size_t cmd_buf_bytes = 0;
     // goal, zone and entity-field batches of a multi-GPU job (pfnav_mgpu_request_goals_ex, ..._zones,
     // ..._entity_fields_batch): the staging buffer of the fields built for the job, 4096-byte blocks (a zone or entity
     // batch keeps its copy list behind them), grown on demand; the last call's owner of every goal or request and the
@@ -429,6 +434,8 @@ int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint
 void pfnav_agents_free(pfnav_ctx *ctx);
 int pfnav_agents_init(pfnav_ctx *ctx);
 int pfnav_agents_finish_snapshot(pfnav_ctx *ctx, cudaStream_t st, bool members);
+// max_radius and any_garrisoned from the records of the whole population (k_population_facts); waits for `st`
+int pfnav_agents_refresh_facts(pfnav_ctx *ctx, cudaStream_t st);
 
 // ---- device helpers shared by kernels ----
 __device__ __forceinline__ uint32_t pf_lane() { return threadIdx.x & 31; }
