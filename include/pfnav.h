@@ -568,7 +568,11 @@ int  pfnav_agents_upload(pfnav_ctx *ctx, const pfnav_agent *agents, size_t n,
  *       -> pfnav_agents_set_blocking for commands, on the rank that owns the uids
  *       -> pfnav_mgpu_exchange_blocker_ops (every rank) / pfnav_group_exchange_blocker_ops (once)
  *       -> pfnav_blockers_* / pfnav_blockers_batch for host ops (buildings, load-time blocks), on every rank
- *       -> pfnav_map_commit -> pfnav_mgpu_gather / pfnav_group_gather */
+ *       -> pfnav_map_commit -> pfnav_mgpu_gather / pfnav_group_gather
+ * The engine's orders reach a job as one batch of deltas that every member receives whole (pfnav_mgpu_commands /
+ * pfnav_group_commands, after pfnav_agents_commands), before the blocking calls of those commands:
+ *       apply_updates_ex -> job commands + pfnav_agents_set_blocking -> exchange -> pfnav_map_commit -> gather
+ *       -> pfnav_agents_set_work_dev -> tick */
 typedef struct pfnav_group pfnav_group;
 #define PFNAV_MGPU_ID_BYTES 128
 int  pfnav_mgpu_shard_range(size_t n_total, int rank, int world, size_t *lo, size_t *hi);
@@ -960,6 +964,36 @@ typedef struct pfnav_agent_delta {
  *   (pfnav_mgpu_init / pfnav_group_create, or an own range that is not the whole population). */
 int  pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n,
                            const pfnav_flock *flocks, size_t nflocks, void *stream);
+/* pfnav_agents_commands for a whole multi-GPU job. Every rank calls the NCCL form with the same arguments, the job's
+ * whole batch (uids global, in [0, n_total)); the group form is called once. Delta format, masks and the flock-table
+ * rule are those of pfnav_agents_commands.
+ * - Equivalence: after the call and the next pfnav_mgpu_gather / pfnav_group_gather, every member's snapshot is what
+ *   one context holding the whole population would have after pfnav_agents_commands(same arguments): its own range's
+ *   agent, movestate and movestate_ext records, the whole flock id column, the flock table, the member lists, largest
+ *   radius and any GARRISONED, flock_layer_used of its own range (as pfnav_agents_upload_shard of the resulting range
+ *   would leave it) and the arrival constants' invalidation.
+ * - A member applies the deltas of the uids it owns as the solo call does. For every other uid it writes only what no
+ *   tick step changes: the flock id, the neighbour record's radius and its low 24 flag bits (only uploads and command
+ *   batches write those). Position, velocity and state of other members' entities arrive with the next gather, as
+ *   always. From its complete flock column and records each member rebuilds the member lists and population facts on
+ *   its device, so the next gather does not carry the flock column and rebuilds nothing on the host.
+ * - All or nothing across the job: each member validates the deltas against the population (the checks of
+ *   pfnav_agents_commands with [0, n_total) as the range) and its own entities' layers and flock indices, then the
+ *   members exchange one verdict record {status, n_agents, n_flocks}: NCCL all-gathers it on `stream` and reads it, a
+ *   group reads its members' host state. If any member refuses, every member returns that member's error and the text
+ *   names it; members whose population or flock table sizes differ return PFNAV_ERR_ARG. Nothing changes anywhere.
+ *   POSITION / CLEAR_HIST need every member's movestate table, TARGET every member's movestate_ext table.
+ * - Streams: the NCCL form runs on `stream`, the group form on each member's context stream. Host waits as in the solo
+ *   call (flock offsets, population facts), plus the verdict read of the NCCL form. It does not touch blocker ops or the
+ *   work list: pfnav_agents_set_blocking for commands stays on the rank that owns the uids, before the exchange.
+ * - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE (nothing changed) on a context in no job, for
+ *   the NCCL form on a group member, and on every member when one of them has uploaded its range with
+ *   pfnav_agents_upload_shard (without PFNAV_UPLOAD_SAME_FLOCKS) and not gathered since: its flock column is not
+ *   complete. An empty batch without a table does nothing and exchanges nothing. */
+int  pfnav_mgpu_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n,
+                         const pfnav_flock *flocks, size_t nflocks, void *stream);
+int  pfnav_group_commands(pfnav_group *g, const pfnav_agent_delta *deltas, size_t n,
+                          const pfnav_flock *flocks, size_t nflocks);
 /* pfnav_agents_set_work(ctx, NULL, 0) from the state resident on the device: the uids of the context's own range whose
  * state is neither ARRIVED nor WAITING, ascending, compacted on the device on `stream`. It waits for the stream once, to
  * read the 4-byte count that sizes the per-work-item buffers; it waits for the whole device only when the list outgrows

@@ -131,6 +131,7 @@ SYMBOLS = [
     "pfnav_mgpu_request_zones", "pfnav_group_request_zones", "pfnav_mgpu_request_entity_fields_batch",
     "pfnav_group_request_entity_fields_batch",
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
+    "pfnav_mgpu_commands", "pfnav_group_commands",
 ]
 
 _lib = None
@@ -201,6 +202,8 @@ def load():
     L.pfnav_agents_set_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
     L.pfnav_agents_read_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_commands.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_mgpu_commands.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_group_commands.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
     L.pfnav_agents_set_work_dev.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
     L.pfnav_agents_read_work.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
@@ -296,6 +299,15 @@ class PfnavError(RuntimeError):
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
+
+
+def _command_args(deltas, flocks):
+    """(deltas, n, flocks, nflocks) of the command calls; flocks None: the table is unchanged (the pointers keep their
+    arrays alive)"""
+    d = np.ascontiguousarray(deltas, AGENT_DELTA).reshape(-1)
+    fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
+    fp = None if fl is None else _p(fl if len(fl) else np.zeros(1, FLOCK))     # an empty table is still a table
+    return _p(d) if len(d) else None, len(d), fp, 0 if fl is None else len(fl)
 
 
 def _chk(rc):
@@ -962,11 +974,12 @@ class Nav:
     def agents_commands(self, deltas, flocks=None, stream=0):
         """pfnav_agents_commands: AGENT_DELTA records applied in order; flocks (FLOCK records): the whole new flock
         table, None: unchanged. Follow with agents_rebuild_index."""
-        d = np.ascontiguousarray(deltas, AGENT_DELTA).reshape(-1)
-        fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
-        fp = None if fl is None else _p(fl if len(fl) else np.zeros(1, FLOCK))     # an empty table is still a table
-        _chk(self.L.pfnav_agents_commands(self.h, _p(d) if len(d) else None, len(d), fp, 0 if fl is None else len(fl),
-                                          C.c_void_p(stream)))
+        _chk(self.L.pfnav_agents_commands(self.h, *_command_args(deltas, flocks), C.c_void_p(stream)))
+
+    def mgpu_commands(self, deltas, flocks=None, stream=0):
+        """collective: agents_commands for the whole job -- every rank passes the job's whole batch (global uids) and
+        the same table; all or nothing across the ranks. Follow with mgpu_gather."""
+        _chk(self.L.pfnav_mgpu_commands(self.h, *_command_args(deltas, flocks), C.c_void_p(stream)))
 
     def agents_set_work_dev(self, stream=0):
         """pfnav_agents_set_work_dev: agents_set_work(None) built on the device -> the number of work items"""
@@ -1094,6 +1107,11 @@ class Group:
         _chk(load().pfnav_group_request_entity_fields_batch(self.g, _p(reqs) if len(reqs) else None, len(reqs),
                                                             _p(fp) if len(fp) else None, len(fp), _p(ch) if len(ch) else None,
                                                             len(ch)))
+
+    def commands(self, deltas, flocks=None):
+        """agents_commands for the whole group: the job's whole batch (global uids), each member applying its own
+        entities' deltas; all or nothing across the members. Follow with gather."""
+        _chk(load().pfnav_group_commands(self.g, *_command_args(deltas, flocks)))
 
     def close(self):
         if self.g:

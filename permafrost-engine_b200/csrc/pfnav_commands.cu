@@ -5,6 +5,9 @@
 // with a stable counting sort: every warp owns a contiguous uid range, counts its entities per flock, the counts are
 // scanned per flock across the warps and over the flocks, and every warp writes its entities behind the offsets of its
 // range. Members are therefore ascending by uid within a flock, as the host pass of an upload leaves them.
+// A member of a multi-GPU job takes the job's whole batch (pf_cmd_job_check / pf_cmd_job_apply, for pfnav_mgpu.cu): the
+// deltas of its own uids as above, and for the others the flock id, radius and flag bits (k_apply_foreign), so that it
+// rebuilds the member lists and population facts from its own complete columns.
 // pfnav_agents_set_work_dev compacts the uids that are not still into the work list, in uid order.
 #include "pfnav_internal.cuh"
 #include <algorithm>
@@ -28,6 +31,16 @@ __global__ void k_apply_deltas(const pfnav_agent_delta *__restrict__ deltas, int
     r.radius = a.radius;
     r.state_flags = (a.state << 24) | (a.flags & 0xFFFFFFu);
     rec[d.uid] = r;
+}
+
+// a job member's writes for the entities other members own (pf_foreign_apply): flock column, radius, low flag bits
+__global__ void k_apply_foreign(const pf_cmd_foreign *__restrict__ f, int n, int32_t *__restrict__ flock_of,
+                                pf_record *__restrict__ rec)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const pf_cmd_foreign x = f[i];
+    pf_foreign_apply(x, flock_of[x.uid], rec[x.uid].radius, rec[x.uid].state_flags);
 }
 
 // ---- flock member lists: stable counting sort of the uids by flock ----
@@ -222,6 +235,10 @@ static int members_on_device(pfnav_ctx *ctx, cudaStream_t st, uint32_t *hist, in
     return 0;
 }
 
+static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_agent_delta> &merged,
+                     const std::vector<pf_cmd_foreign> &foreign, const std::vector<pf_cmd_change> &changes,
+                     const pfnav_flock *flocks, size_t nflocks);
+
 extern "C" int pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks,
                                      size_t nflocks, void *stream)
 {
@@ -244,19 +261,27 @@ extern "C" int pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *de
     if (!err) err = pf_cmd_plan(ctx->cmd_mirror, ctx->shard_lo, merged, nflocks, ctx->nlayers, changes);
     PF_ARG(!err, err);
     if (merged.empty() && !flocks) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    return cmd_apply(ctx, pf_stream(ctx, stream), merged, {}, changes, flocks, nflocks);
+}
+
+// Everything after validation, on `st`: the flock table, the merged records of the own range (k_apply_deltas), a job
+// member's foreign records (k_apply_foreign), the host facts, the member lists and the population facts.
+static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_agent_delta> &merged,
+                     const std::vector<pf_cmd_foreign> &foreign, const std::vector<pf_cmd_change> &changes,
+                     const pfnav_flock *flocks, size_t nflocks)
+{
     uint32_t any = 0;
     for (const pfnav_agent_delta &m : merged) any |= m.mask;
+    for (const pf_cmd_foreign &f : foreign) any |= f.mask;
     const bool members = (any & PFNAV_DELTA_FLOCK) || nflocks != ctx->n_flocks;
-
-    PF_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = pf_stream(ctx, stream);
     int rc;
     // warps of the member sort: at most 4096 ranges, and at most 16 M histogram words
     const size_t max_w = std::max<size_t>(1, std::min<size_t>(4096, ((size_t)1 << 24) / std::max<size_t>(nflocks, 1)));
     const int per = (int)(((ctx->n_agents + max_w - 1) / max_w + 31) / 32 * 32);
     const int W = per ? (int)((ctx->n_agents + per - 1) / per) : 0;
-    const size_t b_deltas = merged.size() * sizeof(pfnav_agent_delta);
-    if ((rc = cmd_buf(ctx, b_deltas + (members ? nflocks * (size_t)W * 4 : 0)))) return rc;
+    const size_t b_deltas = merged.size() * sizeof(pfnav_agent_delta), b_foreign = foreign.size() * sizeof(pf_cmd_foreign);
+    if ((rc = cmd_buf(ctx, b_deltas + b_foreign + (members ? nflocks * (size_t)W * 4 : 0)))) return rc;
     if (nflocks + 1 > ctx->cap_flocks) {       // keeps no content: the table follows, the offsets are rebuilt (members)
         PF_CUDA(cudaDeviceSynchronize());
         const size_t cap = std::max(nflocks + 1, ctx->cap_flocks * 2);
@@ -271,21 +296,59 @@ extern "C" int pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *de
         ctx->n_flocks = nflocks;
     }
     if (!merged.empty()) {
+        const bool have_ms = ctx->movestate_set && ctx->d_movestate != nullptr;
         PF_CUDA(cudaMemcpyAsync(ctx->d_cmd_buf, merged.data(), b_deltas, cudaMemcpyHostToDevice, st));
         k_apply_deltas<<<((int)merged.size() + 127) / 128, 128, 0, st>>>((const pfnav_agent_delta *)ctx->d_cmd_buf, (int)merged.size(),
-            ctx->d_agents, lim.have_ms ? ctx->d_movestate : nullptr, ctx->d_ms_ext, ctx->d_flock_of, ctx->d_records);
+            ctx->d_agents, have_ms ? ctx->d_movestate : nullptr, ctx->d_ms_ext, ctx->d_flock_of, ctx->d_records);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
     }
-    // host facts, as a fresh upload of the resulting population would leave them
+    if (!foreign.empty()) {
+        pf_cmd_foreign *d_foreign = (pf_cmd_foreign *)((uint8_t *)ctx->d_cmd_buf + b_deltas);
+        PF_CUDA(cudaMemcpyAsync(d_foreign, foreign.data(), b_foreign, cudaMemcpyHostToDevice, st));
+        k_apply_foreign<<<((int)foreign.size() + 127) / 128, 128, 0, st>>>(d_foreign, (int)foreign.size(), ctx->d_flock_of,
+                                                                             ctx->d_records);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+    }
+    // host facts, as a fresh upload of the resulting population (of the own range, on a job member) would leave them
     pf_cmd_commit(ctx->cmd_mirror, changes, nflocks);
     std::vector<uint8_t> used;
     ctx->cmd_mirror.used(used);
     if (flocks || used != ctx->flock_layer_used) ctx->arrival_valid = false;
     ctx->flock_layer_used.swap(used);
-    if (members && (rc = members_on_device(ctx, st, (uint32_t *)((uint8_t *)ctx->d_cmd_buf + b_deltas), per, W))) return rc;
+    if (members && (rc = members_on_device(ctx, st, (uint32_t *)((uint8_t *)ctx->d_cmd_buf + b_deltas + b_foreign), per, W))) return rc;
     if ((any & (PFNAV_DELTA_RADIUS | PFNAV_DELTA_FLAGS)) && (rc = pfnav_agents_refresh_facts(ctx, st))) return rc;
     return PFNAV_OK;
+}
+
+// A job member: the whole batch is checked against the population, the own records against the member's mirror. Its
+// flock column must be complete -- a full pfnav_agents_upload_shard leaves the other ranges' entries to the next
+// gather -- because the member lists are rebuilt from it.
+int pf_cmd_job_check(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks, size_t nflocks,
+                     pf_cmd_job &J)
+{
+    PF_ARG(ctx->d_agents, "agents not uploaded");
+    if (ctx->members_stale) {
+        pfnav_set_error("the member's flock column is incomplete until the gather that follows pfnav_agents_upload_shard");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(deltas || n == 0, "deltas == NULL");
+    PF_ARG(n < (1u << 31) && nflocks < (1u << 31), "n / nflocks");
+    J.flocks = flocks;
+    J.nflocks = flocks ? nflocks : ctx->n_flocks;
+    const pf_cmd_limits lim = {0, ctx->n_agents, ctx->n_agents, J.nflocks, ctx->movestate_set && ctx->d_movestate != nullptr,
+                               ctx->d_ms_ext != nullptr};
+    const char *err = pf_cmd_job_plan(deltas, n, lim, ctx->shard_lo, ctx->shard_hi, ctx->cmd_mirror, ctx->nlayers, J.own,
+                                      J.foreign, J.changes);
+    PF_ARG(!err, err);
+    return PFNAV_OK;
+}
+
+int pf_cmd_job_apply(pfnav_ctx *ctx, const pf_cmd_job &J, cudaStream_t st)
+{
+    if (J.own.empty() && J.foreign.empty() && !J.flocks) return PFNAV_OK;
+    return cmd_apply(ctx, st, J.own, J.foreign, J.changes, J.flocks, J.nflocks);
 }
 
 extern "C" int pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *out_nwork)

@@ -1,6 +1,7 @@
 // pfnav_commands_host.h -- the host side of pfnav_agents_commands and the write rule its kernel applies, CUDA-free:
 // delta validation, per-uid merging in array order, the navigation layer rule and the (flock, layer) mirror that keeps
-// flock_layer_used equal to a fresh upload's. tests/emu/commands_emu.cpp builds this header with g++.
+// flock_layer_used equal to a fresh upload's; and the split of a multi-GPU job's batch into a member's own and foreign
+// parts. tests/emu/commands_emu.cpp and tests/emu/commands_job_emu.cpp build this header with g++.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -174,4 +175,38 @@ static inline void pf_cmd_commit(pf_cmd_mirror &M, const std::vector<pf_cmd_chan
     }
     M.count.resize(nflocks_new * PFNAV_NAV_LAYER_MAX);         // a dropped tail holds no entity (pf_cmd_plan)
     M.nflocks = nflocks_new;
+}
+
+// ---- the job form (pfnav_mgpu_commands / pfnav_group_commands) ----
+// Every member gets the job's whole batch. It applies the merged records of the uids it owns as the solo call does, and
+// for every other uid writes only what no tick step changes -- the flock column entry and the neighbour record's radius
+// and low 24 flag bits (k_make_records and k_entity_apply copy those from the agent unchanged) -- so that its flock
+// column, radii and flag bits equal the owners' after the call. Position, velocity and state of other members' entities
+// arrive with the next gather.
+#define PF_DELTA_FOREIGN (PFNAV_DELTA_FLOCK | PFNAV_DELTA_RADIUS | PFNAV_DELTA_FLAGS)
+struct pf_cmd_foreign { uint32_t uid, mask; int32_t flock; float radius; uint32_t flags; };     // mask: PF_DELTA_FOREIGN bits
+
+PF_HD void pf_foreign_apply(const pf_cmd_foreign &f, int32_t &flock, float &radius, uint32_t &state_flags)
+{
+    if (f.mask & PFNAV_DELTA_FLOCK) flock = f.flock;
+    if (f.mask & PFNAV_DELTA_RADIUS) radius = f.radius;
+    if (f.mask & PFNAV_DELTA_FLAGS) state_flags = (state_flags & 0xFF000000u) | (f.flags & 0xFFFFFFu);
+}
+
+// A member's part of a job batch, changing nothing: validation of every delta against the population (L.lo = 0,
+// L.hi = n_total), merging, the split into the merged records of the own range [lo, hi) and the foreign part of the
+// others, and pf_cmd_plan of the own records on the member's mirror (layers and stranded flock indices, which only the
+// owner can check). Returns NULL or what was wrong.
+static inline const char *pf_cmd_job_plan(const pfnav_agent_delta *d, size_t n, const pf_cmd_limits &L, size_t lo, size_t hi,
+                                          const pf_cmd_mirror &M, int nlayers, std::vector<pfnav_agent_delta> &own,
+                                          std::vector<pf_cmd_foreign> &foreign, std::vector<pf_cmd_change> &changes)
+{
+    std::vector<pfnav_agent_delta> merged;
+    own.clear(); foreign.clear(); changes.clear();
+    if (const char *e = pf_cmd_merge(d, n, L, merged)) return e;
+    for (const pfnav_agent_delta &m : merged) {
+        if (m.uid >= lo && m.uid < hi) own.push_back(m);
+        else if (m.mask & PF_DELTA_FOREIGN) foreign.push_back({m.uid, m.mask & PF_DELTA_FOREIGN, m.flock, m.radius, m.flags});
+    }
+    return pf_cmd_plan(M, lo, own, L.nflocks, nlayers, changes);
 }

@@ -437,6 +437,19 @@ int pfnav_agents_finish_snapshot(pfnav_ctx *ctx, cudaStream_t st, bool members);
 // max_radius and any_garrisoned from the records of the whole population (k_population_facts); waits for `st`
 int pfnav_agents_refresh_facts(pfnav_ctx *ctx, cudaStream_t st);
 
+// ---- pfnav_commands.cu: a job member's part of a command batch (pfnav_mgpu.cu runs the verdict exchange) ----
+// pf_cmd_job_check validates the batch against the member's state and plans it, changing nothing (the error is set);
+// pf_cmd_job_apply applies a checked batch on `st` (the caller has selected the member's device).
+struct pf_cmd_job {
+    std::vector<pfnav_agent_delta> own;
+    std::vector<pf_cmd_foreign> foreign;
+    std::vector<pf_cmd_change> changes;
+    const pfnav_flock *flocks = nullptr; size_t nflocks = 0;
+};
+int pf_cmd_job_check(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks, size_t nflocks,
+                     pf_cmd_job &J);
+int pf_cmd_job_apply(pfnav_ctx *ctx, const pf_cmd_job &J, cudaStream_t st);
+
 // ---- device helpers shared by kernels ----
 __device__ __forceinline__ uint32_t pf_lane() { return threadIdx.x & 31; }
 

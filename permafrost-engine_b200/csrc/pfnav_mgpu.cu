@@ -66,10 +66,12 @@ struct pf_mgpu {
     pf_nccl_comm comm = nullptr;                 // NCCL transport
     pfnav_group *group = nullptr;                // in-process transport
     bool share_blockers = false;                 // pfnav_mgpu_share_blockers / pfnav_group_share_blockers
-    uint32_t *d_xcnt = nullptr;                  // NCCL: the exchange's all-gathered count records, PF_XCNT words per rank
+    uint32_t *d_xcnt = nullptr;                  // NCCL: all-gathered records of PF_XCNT words per rank: the blocker
+                                                 // exchange's counts, a command batch's verdicts; read before the call returns
     uint8_t *d_xgoal = nullptr; size_t xgoal_bytes = 0;   // NCCL: the goal batch's all-gathered member records
 };
 #define PF_XCNT 8                                // {narrow, wide, sent narrow, sent wide, faction flag, 0, 0, 0}
+                                                 // or {status, n_agents, n_flocks, 0, 0, 0, 0, 0}
 
 bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx)
 {
@@ -483,8 +485,8 @@ static void job_init_entity(pf_job &J, const pfnav_entity_field_req *reqs, size_
     J.kind = PF_JOB_ENTITY; J.ereqs = reqs; J.m = m; J.ents = ents; J.nents = nents; J.chunks_rc = chunks_rc; J.nchunks = nchunks;
 }
 
-// the NCCL form's member: a context of a job, not of an in-process group
-static int nccl_member(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_mgpu **out)
+// the NCCL form's rank: a context of a job, not of an in-process group
+static int nccl_rank(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_mgpu **out)
 {
     PF_ARG(ctx, "ctx");
     PF_NEED_DEVICE(ctx);
@@ -497,8 +499,15 @@ static int nccl_member(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_
         pfnav_set_error("%s: member of an in-process group: %s", fn, group_fn);
         return PFNAV_ERR_STATE;
     }
-    PF_ARG(ctx->pool.d_slot, "pool not created");
     *out = m;
+    return PFNAV_OK;
+}
+
+// ... of a field batch: with a pool
+static int nccl_member(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_mgpu **out)
+{
+    if (int rc = nccl_rank(ctx, fn, group_fn, out)) return rc;
+    PF_ARG(ctx->pool.d_slot, "pool not created");
     return PFNAV_OK;
 }
 
@@ -727,4 +736,74 @@ extern "C" int pfnav_group_request_entity_fields_batch(pfnav_group *g, const pfn
     std::vector<pf_job> J(g->ctxs.size());
     for (pf_job &j : J) job_init_entity(j, reqs, m, ents, nents, chunks_rc, nchunks);
     return group_job(g, J, __func__);
+}
+
+// ------------------------------------------------------------------------------------------
+// Movement commands of a job (pfnav_commands.cu: pf_cmd_job_*). Every member gets the job's whole batch, checks what it
+// owns and describes itself in one record {status, n_agents, n_flocks}; every member reads every record before anything
+// changes, because a member cannot check another's layers or flock indices, and a flock table taken by some members only
+// would split the job's member lists.
+// ------------------------------------------------------------------------------------------
+extern "C" int pfnav_mgpu_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks,
+                                   size_t nflocks, void *stream)
+{
+    pf_mgpu *m = nullptr;
+    if (int rc = nccl_rank(ctx, __func__, "pfnav_group_commands", &m)) return rc;
+    if (n == 0 && !flocks) return PFNAV_OK;                 // the same arguments on every rank: none of them exchanges
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    pf_cmd_job J;
+    int local = check_shard(ctx, m);
+    if (!local) local = pf_cmd_job_check(ctx, deltas, n, flocks, nflocks, J);
+    const std::string local_err = local ? pfnav_last_error() : "";
+    const int world = m->world, rank = m->rank;
+    if (!m->d_xcnt) PF_CUDA(cudaMalloc(&m->d_xcnt, (size_t)world * PF_XCNT * sizeof(uint32_t)));
+    uint32_t *mine = m->d_xcnt + (size_t)rank * PF_XCNT;
+    const uint32_t verdict[PF_XCNT] = {(uint32_t)local, (uint32_t)ctx->n_agents, (uint32_t)ctx->n_flocks, 0, 0, 0, 0, 0};
+    PF_CUDA(cudaMemcpyAsync(mine, verdict, sizeof(verdict), cudaMemcpyHostToDevice, st));
+    PF_NCCL(g_nccl.AllGather(mine, m->d_xcnt, PF_XCNT * sizeof(uint32_t), /*ncclInt8*/ 0, m->comm, st));
+    std::vector<uint32_t> all((size_t)world * PF_XCNT);
+    PF_CUDA(cudaMemcpyAsync(all.data(), m->d_xcnt, all.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    for (int r = 0; r < world; r++) {
+        const uint32_t *x = &all[(size_t)r * PF_XCNT];
+        if (!x[0]) continue;
+        if (r == rank) pfnav_set_error("%s: rank %d refused the batch (%s); no rank changed anything", __func__, r, local_err.c_str());
+        else pfnav_set_error("%s: rank %d refused the batch (error %d); no rank changed anything", __func__, r, (int)x[0]);
+        return (int)x[0];
+    }
+    for (int r = 0; r < world; r++)
+        PF_ARG(all[(size_t)r * PF_XCNT + 1] == all[1] && all[(size_t)r * PF_XCNT + 2] == all[2],
+               "ranks hold populations or flock tables of different sizes; no rank changed anything");
+    return pf_cmd_job_apply(ctx, J, st);
+}
+
+// In-process group: the members' verdicts are their host state, so nothing is exchanged on the devices; each member then
+// applies the batch on its context stream.
+extern "C" int pfnav_group_commands(pfnav_group *g, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks,
+                                    size_t nflocks)
+{
+    PF_ARG(g, "group");
+    if (n == 0 && !flocks) return PFNAV_OK;
+    const int world = (int)g->ctxs.size();
+    std::vector<pf_cmd_job> J(world);
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        int rc = check_shard(c, (pf_mgpu *)c->mgpu);
+        if (!rc) rc = pf_cmd_job_check(c, deltas, n, flocks, nflocks, J[i]);
+        if (rc) {
+            const std::string e = pfnav_last_error();
+            pfnav_set_error("%s: member %d refused the batch (%s); no member changed anything", __func__, i, e.c_str());
+            return rc;
+        }
+    }
+    for (int i = 0; i < world; i++)
+        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents && g->ctxs[i]->n_flocks == g->ctxs[0]->n_flocks,
+               "members hold populations or flock tables of different sizes; no member changed anything");
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        if (int rc = pf_cmd_job_apply(c, J[i], c->tick_stream)) return rc;
+    }
+    return PFNAV_OK;
 }
