@@ -782,31 +782,20 @@ int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector
     const int ngroups = (int)off.size() - 1;
     const size_t b_item = sorted.size() * sizeof(pf_chain_item), b_mask = masks.size() * 8, b_off = off.size() * 4;
     const size_t a_mask = (b_item + 15) & ~(size_t)15, a_off = a_mask + b_mask, total = a_off + b_off;
-    if (ctx->plan_buf_bytes < total) {
-        PF_CUDA(cudaStreamSynchronize(st));
-        cudaFree(ctx->d_plan_buf);
-        ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
-        ctx->plan_buf_bytes = total * 2;
-    }
-    // staged in the pinned ring (pf_plan_host): the copy is asynchronous and the host does not wait for it
-    uint8_t *host = nullptr;
-    int ri = 0;
-    int rc = pf_plan_host(ctx, total, &host, &ri);
+    pf_stage S;
+    int rc = pf_stage_begin(ctx, st, total, total, false, &S);
     if (rc) return rc;
-    memcpy(host, sorted.data(), b_item);
-    if (b_mask) memcpy(host + a_mask, masks.data(), b_mask);
-    memcpy(host + a_off, off.data(), b_off);
-    uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
-    ctx->goal_batch.valid = false;          // the staging buffer is reused
-    PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    memcpy(S.host, sorted.data(), b_item);
+    if (b_mask) memcpy(S.host + a_mask, masks.data(), b_mask);
+    memcpy(S.host + a_off, off.data(), b_off);
+    if ((rc = pf_stage_upload(ctx, st, S, total))) return rc;
+    const uint8_t *dev = S.dev;
     k_repair_chain<<<(unsigned)std::min(ngroups, ctx->sm_count * 8), FLOWG_THREADS, 0, st>>>(
         grids_of(ctx), (const pf_chain_item *)dev, (const int32_t *)(dev + a_off), ngroups, (const uint64_t *)(dev + a_mask),
         ctx->pool.d_flow, d_count);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
-    return PFNAV_OK;
+    return pf_stage_done(ctx, st);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1281,12 +1270,7 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
     if (ctx->device < 0) { delete ctx; return; }
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
-    for (int i = 0; i < 2; i++) {
-        cudaFreeHost(ctx->plan_host[i]);
-        if (ctx->plan_host_ev[i]) cudaEventDestroy(ctx->plan_host_ev[i]);
-    }
-    cudaFree(ctx->d_ent_buf);
-    if (ctx->ent_ev) cudaEventDestroy(ctx->ent_ev);
+    pf_stage_free(ctx);
     cudaFree(ctx->d_mq_buf);
     cudaFree(ctx->d_job_stage);
     pfnav_fields_free(ctx);
@@ -1842,27 +1826,26 @@ int pfnav_flow_repair_pool(pfnav_ctx *ctx, const pfnav_field_req *targets, const
     return PFNAV_OK;
 }
 
-int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint8_t *d_out_fields,
-                     const int32_t *d_out_slot, int n_waves, const int32_t *h_wave_offsets, void *stream);
-
+// The wave arguments stay for the ABI and are only checked: the requests are dependency-sorted, and the kernel schedules
+// them itself.
 extern "C" int pfnav_los_fields_create_dev(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint8_t *d_out_fields,
                                            int n_waves, const int32_t *h_wave_offsets, void *stream)
 {
-    return pfnav_los_launch(ctx, d_reqs, n, d_out_fields, nullptr, n_waves, h_wave_offsets, stream);
+    PF_ARG(n == 0 || (n_waves >= 1 && h_wave_offsets), "null buffer");
+    return pfnav_los_launch(ctx, d_reqs, n, d_out_fields, nullptr, stream);
 }
 
 int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint8_t *d_out_fields,
-                     const int32_t *d_out_slot, int n_waves, const int32_t *h_wave_offsets, void *stream)
+                     const int32_t *d_out_slot, void *stream)
 {
     PF_ARG(ctx && ctx->d_cost, "map not created");
     PF_NEED_DEVICE(ctx);
     if (n == 0) return PFNAV_OK;
-    PF_ARG(d_reqs && d_out_fields && n_waves >= 1 && h_wave_offsets, "null buffer");
+    PF_ARG(d_reqs && d_out_fields, "null buffer");
     PF_CUDA(cudaSetDevice(ctx->device));
     const FlowGrids g = grids_of(ctx);
     LosMapInfo mi{ctx->map_x, ctx->map_z};
     const size_t smem = LOS_WARPS_PER_CTA * (ctx->los_variant != 0 ? sizeof(LosSmemB) : sizeof(LosSmem));
-    (void)n_waves; (void)h_wave_offsets;        // requests are dependency-sorted; the kernel schedules them itself
     cudaStream_t st = pf_stream(ctx, stream);
     // scheduler state: [counter][done flags]. ONE buffer per context: the warps of a launch spin on its flags, so a
     // later launch (on any stream) must not reset or free it while an earlier one is still running -- every launch
@@ -1914,10 +1897,10 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
     PF_NEED_DEVICE(ctx);
     if (n == 0) return PFNAV_OK;
     PF_ARG(reqs && out_fields, "null buffer");
-    // dependency depth = wave; requests are re-ordered wave-major on the device side
-    std::vector<int> depth(n, 0), order(n), newidx(n);
+    // requests go to the device in dependency order (pfnav_waves_host.h); caller-held previous fields ride in extra
+    // slots behind the n outputs and are named like pool slots (-2)
+    pf_wave_pack W;
     std::vector<size_t> inplace;
-    int maxd = 0;
     for (size_t i = 0; i < n; i++) {
         const pfnav_los_req &q = reqs[i];
         PF_ARG(q.layer >= 0 && q.layer < ctx->nlayers, "los req: layer");
@@ -1931,30 +1914,17 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
         else if (q.prev_index == PFNAV_LOS_PREV_INPLACE) {
             // N_LOSFieldCreate(..., prev) with a caller-held previous field: its bytes arrive in out_fields[i]
             PF_ARG(abs(q.prev_chunk_r - q.chunk_r) + abs(q.prev_chunk_c - q.chunk_c) == 1, "los req: prev chunk must be adjacent");
+            W.los_kept(q, 0, (int32_t)(n + inplace.size()));
             inplace.push_back(i);
+            continue;
         } else {
             PF_ARG(q.prev_index >= 0 && (size_t)q.prev_index < i, "los req: prev_index must name an earlier request");
             PF_ARG(abs(q.prev_chunk_r - q.chunk_r) + abs(q.prev_chunk_c - q.chunk_c) == 1, "los req: prev chunk must be adjacent");
-            depth[i] = depth[q.prev_index] + 1;
-            maxd = std::max(maxd, depth[i]);
         }
+        W.los(q, 0);
     }
-    std::vector<int32_t> wave_off(maxd + 2, 0);
-    for (size_t i = 0; i < n; i++) wave_off[depth[i] + 1]++;
-    for (int w = 0; w <= maxd; w++) wave_off[w + 1] += wave_off[w];
-    std::vector<int32_t> cursor(wave_off.begin(), wave_off.end() - 1);
-    for (size_t i = 0; i < n; i++) { newidx[i] = cursor[depth[i]]++; order[newidx[i]] = (int)i; }
-    std::vector<pfnav_los_req> sorted(n);
-    for (size_t k = 0; k < n; k++) {
-        sorted[k] = reqs[order[k]];
-        if (sorted[k].prev_index >= 0) sorted[k].prev_index = newidx[sorted[k].prev_index];
-    }
-    // caller-held previous fields ride in extra slots behind the n outputs and are named like pool slots (-2)
-    for (size_t j = 0; j < inplace.size(); j++) {
-        pfnav_los_req &q = sorted[newidx[inplace[j]]];
-        q.prev_index = -2;
-        q._pad = (int32_t)(n + j);
-    }
+    std::vector<uint8_t> packed(W.layout());
+    W.pack(packed.data());
     PF_CUDA(cudaSetDevice(ctx->device));
     pfnav_los_req *d_reqs = nullptr;
     uint8_t *d_fields = nullptr;
@@ -1962,12 +1932,12 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
     if (cudaMalloc(&d_fields, (n + inplace.size()) * 4096) != cudaSuccess) { cudaFree(d_reqs); pfnav_set_error("cudaMalloc fields"); return PFNAV_ERR_NOMEM; }
     cudaStream_t st = ctx->tick_stream;
     std::vector<uint8_t> tmp(n * 4096);
-    cudaError_t e = cudaMemcpyAsync(d_reqs, sorted.data(), n * sizeof(pfnav_los_req), cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_reqs, packed.data() + W.out.o_lr, n * sizeof(pfnav_los_req), cudaMemcpyHostToDevice, st);
     for (size_t j = 0; j < inplace.size() && e == cudaSuccess; j++)
         e = cudaMemcpyAsync(d_fields + (n + j) * 4096, out_fields + inplace[j] * 4096, 4096, cudaMemcpyHostToDevice, st);
     int rc = 0;
     if (e == cudaSuccess) {
-        rc = pfnav_los_fields_create_dev(ctx, d_reqs, n, d_fields, maxd + 1, wave_off.data(), st);
+        rc = pfnav_los_launch(ctx, d_reqs, n, d_fields, nullptr, st);
         if (rc == 0) e = cudaMemcpyAsync(tmp.data(), d_fields, n * 4096, cudaMemcpyDeviceToHost, st);
     }
     cudaError_t e2 = cudaStreamSynchronize(st);
@@ -1977,7 +1947,7 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
         pfnav_set_error("pfnav_los_fields_create: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
         return PFNAV_ERR_CUDA;
     }
-    for (size_t k = 0; k < n; k++) memcpy(out_fields + (size_t)order[k] * 4096, tmp.data() + k * 4096, 4096);
+    for (size_t i = 0; i < n; i++) memcpy(out_fields + i * 4096, tmp.data() + (size_t)W.lpos[i] * 4096, 4096);
     return PFNAV_OK;
 }
 

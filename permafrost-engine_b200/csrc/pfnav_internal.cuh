@@ -13,6 +13,7 @@
 #include "../../include/pfnav.h"
 #include "pfnav_pool_host.h"
 #include "pfnav_commands_host.h"
+#include "pfnav_waves_host.h"
 
 #define PFNAV_VERSION 100
 
@@ -98,13 +99,12 @@ struct pfnav_ctx {
 
     // ---- field pool (pfnav_pool.cu, pfnav_pool_host.h) ----
     pf_pool pool;
-    void *d_plan_buf = nullptr; size_t plan_buf_bytes = 0;    // request staging for pfnav_pool_request_goal
-    // The plan of the last goal batch stays resident on the device: re-requesting the same goals on an
+    // The plan of the last goal batch stays resident in the staging device buffer: re-requesting the same goals on an
     // unchanged map (map_epoch) relaunches the kernels without re-planning or re-uploading anything.
     uint64_t map_epoch = 0;
     struct goal_batch_t {
         bool valid = false; uint64_t epoch = 0; int layer = 0; std::vector<int32_t> dests, targets;
-        int nf = 0, nl = 0; std::vector<int32_t> fwave_off; size_t b_fr = 0, b_fs = 0, b_lr = 0, b_ls = 0;
+        pf_waves waves;
     } goal_batch;
     uint32_t tick_no = 1;                         // advanced by pfnav_agents_tick
     // TARGET_ENEMIES / TARGET_ENTITY destinations (pfnav_pool_request_entity_fields): what their repairs start from
@@ -176,14 +176,10 @@ struct pfnav_ctx {
     bool vel_timed = false; float last_los_ms = -1.0f, last_vel_ms = -1.0f;
     bool los_inflight = false;
 
-    // cold goal batches: the plan is staged in a ring of two pinned buffers (event-guarded reuse) and the goals are
-    // planned on a persistent host thread pool with per-goal scratch (pfnav_plan.cu)
-    void *plan_host[2] = {nullptr, nullptr}; size_t plan_host_bytes[2] = {0, 0};
-    cudaEvent_t plan_host_ev[2] = {nullptr, nullptr}; int plan_host_next = 0;
+    // pfnav_plan.cu: the buffers of the request staging (pf_stage_*), and the persistent host threads and per-goal
+    // scratch of the goal planner
+    void *stager = nullptr;
     void *planner = nullptr;
-    // entity-field batches (pfnav_region.cu): device scratch for the staged inputs, footprint rows and seed bitmaps,
-    // grown on demand; ent_ev is recorded after the last kernel that reads it
-    void *d_ent_buf = nullptr; size_t ent_buf_bytes = 0; cudaEvent_t ent_ev = nullptr;
     // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand
     void *d_rep_buf = nullptr; size_t rep_buf_bytes = 0;
     int repair_stats[6] = {0, 0, 0, 0, 0, 0};                  // the last call: representatives per phase, rounds ended per rule
@@ -328,9 +324,24 @@ void pf_pool_drop(pfnav_ctx *ctx, int dest, int chunk);    // pfnav_map_commit: 
 // the device on `st`; the caller records the event that guards the reuse of `host` after them
 int pf_pool_stage_table(pfnav_ctx *ctx, uint8_t *host, cudaStream_t st);
 void pf_planner_destroy(pfnav_ctx *ctx);                         // pfnav_plan.cu: join the goal planner threads
-// the next of the two pinned staging buffers (plan_host), at least `bytes` long, once the copy that last read it is done;
-// record plan_host_ev[*out_ri] after the copies from it (pfnav_plan.cu)
-int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri);
+
+// ---- pfnav_plan.cu: request staging. A batch built on the host goes through the next of two pinned buffers into the
+// context's one device buffer, which the batch's kernels then read.
+//   pf_stage_begin  S->host: host_bytes, then the pool's slot table and `has` bytes when `table`, once the copy that last
+//                   read the pinned buffer is done. S->dev: dev_bytes (none when 0), with `st` ordered after the buffer's
+//                   last readers: the forked field work (pf_fields_join) and the stream-ordered reader that called
+//                   pf_stage_done. Growing it waits for both on the host. Drops the resident goal plan, which lives there.
+//   pf_stage_upload copies host[0, bytes) to S.dev on `st`, then the table when asked for; guards the pinned buffer.
+//   pf_stage_done   after the last kernel on `st` that reads S.dev; forked readers are joined instead.
+struct pf_stage { uint8_t *host = nullptr, *dev = nullptr, *table = nullptr; int ri = 0; };
+int pf_stage_begin(pfnav_ctx *ctx, cudaStream_t st, size_t host_bytes, size_t dev_bytes, bool table, pf_stage *S);
+int pf_stage_upload(pfnav_ctx *ctx, cudaStream_t st, const pf_stage &S, size_t bytes);
+int pf_stage_done(pfnav_ctx *ctx, cudaStream_t st);
+void pf_stage_free(pfnav_ctx *ctx);                              // pfnav_destroy, after the device is idle
+// a packed batch (pfnav_waves_host.h) at `dev`: every flow wave on `flow_st`, one launch each, then its LOS requests in
+// one launch on `los_st`, into the fields (pool or staging blocks) their destinations name
+int pf_waves_launch(pfnav_ctx *ctx, const uint8_t *dev, const pf_waves &W, uint8_t *flow_fields, uint8_t *los_fields,
+                    cudaStream_t flow_st, cudaStream_t los_st);
 
 // One member's part of a goal batch of a multi-GPU job (pfnav_plan.cu; the transports are in pfnav_mgpu.cu).
 //   pf_job_plan   plans the batch on the member's planner threads and describes what pfnav_pool_request_goals_ex would
@@ -428,7 +439,7 @@ void pfnav_fields_free(pfnav_ctx *ctx);
 int pfnav_flow_launch(pfnav_ctx *ctx, const pfnav_field_req *d_reqs, size_t n, uint8_t *d_inout_fields,
                       const int32_t *d_out_slot, void *stream);
 int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint8_t *d_out_fields,
-                     const int32_t *d_out_slot, int n_waves, const int32_t *h_wave_offsets, void *stream);
+                     const int32_t *d_out_slot, void *stream);
 
 // ---- pfnav_agents.cu ----
 void pfnav_agents_free(pfnav_ctx *ctx);

@@ -312,15 +312,109 @@ static int los_forked(pfnav_ctx *ctx)
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------
+// Request staging (pfnav_internal.cuh: pf_stage_*). Every batch built on the host reaches its kernels the same way: it is
+// written into the next of two pinned buffers, a ring whose buffer is reused once the copy that last read it is done,
+// and copied on the batch's stream into one device buffer per context. The buffers only grow, by doubling.
+// ------------------------------------------------------------------------------------------
+struct pf_stager {
+    uint8_t *host[2] = {nullptr, nullptr}; size_t host_bytes[2] = {0, 0}; cudaEvent_t host_ev[2] = {nullptr, nullptr};
+    int next = 0;
+    uint8_t *dev = nullptr; size_t dev_bytes = 0;
+    cudaEvent_t read_ev = nullptr;            // pf_stage_done: after the last stream-ordered reader of `dev`
+};
+
+static pf_stager &stager_of(pfnav_ctx *ctx)
+{
+    if (!ctx->stager) ctx->stager = new pf_stager;
+    return *(pf_stager *)ctx->stager;
+}
+
+int pf_stage_begin(pfnav_ctx *ctx, cudaStream_t st, size_t host_bytes, size_t dev_bytes, bool table, pf_stage *S)
+{
+    pf_stager &G = stager_of(ctx);
+    const int ri = G.next;
+    G.next ^= 1;
+    const size_t hb = host_bytes + (table ? ctx->pool.table_bytes() : 0);
+    if (!G.host_ev[ri]) PF_CUDA(cudaEventCreateWithFlags(&G.host_ev[ri], cudaEventDisableTiming));
+    else PF_CUDA(cudaEventSynchronize(G.host_ev[ri]));
+    if (G.host_bytes[ri] < hb) {
+        cudaFreeHost(G.host[ri]);
+        G.host[ri] = nullptr; G.host_bytes[ri] = 0;
+        PF_CUDA(cudaMallocHost(&G.host[ri], hb * 2));
+        G.host_bytes[ri] = hb * 2;
+    }
+    if (!G.read_ev) PF_CUDA(cudaEventCreateWithFlags(&G.read_ev, cudaEventDisableTiming));
+    ctx->goal_batch.valid = false;            // the resident goal plan lives in `dev`
+    if (dev_bytes) {
+        PF_CUDA(pf_fields_join(ctx, st));
+        PF_CUDA(cudaStreamWaitEvent(st, G.read_ev, 0));
+        if (G.dev_bytes < dev_bytes) {
+            PF_CUDA(pf_fields_sync(ctx));
+            PF_CUDA(cudaEventSynchronize(G.read_ev));
+            cudaFree(G.dev);
+            G.dev = nullptr; G.dev_bytes = 0;
+            PF_CUDA(cudaMalloc(&G.dev, dev_bytes * 2));
+            G.dev_bytes = dev_bytes * 2;
+        }
+    }
+    S->host = G.host[ri]; S->dev = G.dev; S->ri = ri;
+    S->table = table ? S->host + host_bytes : nullptr;
+    return PFNAV_OK;
+}
+
+int pf_stage_upload(pfnav_ctx *ctx, cudaStream_t st, const pf_stage &S, size_t bytes)
+{
+    if (bytes) PF_CUDA(cudaMemcpyAsync(S.dev, S.host, bytes, cudaMemcpyHostToDevice, st));
+    if (S.table)
+        if (int rc = pf_pool_stage_table(ctx, S.table, st)) return rc;
+    PF_CUDA(cudaEventRecord(stager_of(ctx).host_ev[S.ri], st));
+    return PFNAV_OK;
+}
+
+int pf_stage_done(pfnav_ctx *ctx, cudaStream_t st)
+{
+    PF_CUDA(cudaEventRecord(stager_of(ctx).read_ev, st));
+    return PFNAV_OK;
+}
+
+void pf_stage_free(pfnav_ctx *ctx)
+{
+    pf_stager *G = (pf_stager *)ctx->stager;
+    if (!G) return;
+    for (int i = 0; i < 2; i++) {
+        cudaFreeHost(G->host[i]);
+        if (G->host_ev[i]) cudaEventDestroy(G->host_ev[i]);
+    }
+    cudaFree(G->dev);
+    if (G->read_ev) cudaEventDestroy(G->read_ev);
+    delete G;
+    ctx->stager = nullptr;
+}
+
+int pf_waves_launch(pfnav_ctx *ctx, const uint8_t *dev, const pf_waves &W, uint8_t *flow_fields, uint8_t *los_fields,
+                    cudaStream_t flow_st, cudaStream_t los_st)
+{
+    for (size_t w = 0; w + 1 < W.fwave_off.size(); w++) {
+        const int first = W.fwave_off[w], cnt = W.fwave_off[w + 1] - first;
+        if (cnt <= 0) continue;
+        int rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, flow_fields,
+                                   (const int32_t *)(dev + W.o_fs) + first, flow_st);
+        if (rc) return rc;
+    }
+    return pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + W.o_lr), W.nl, los_fields, (const int32_t *)(dev + W.o_ls),
+                            los_st);
+}
+
 // Host side of a cold goal batch, owned by the context: persistent planner threads (created on the first batch,
 // joined by pfnav_destroy) and per-goal / merge scratch that keeps its capacity across batches, so that a batch
 // neither spawns threads nor allocates.
 struct pf_planner {
     struct goal_plan { std::vector<pfnav_field_req> fr; std::vector<pfnav_los_req> lr; std::vector<int32_t> fc, fw, lc; int nf = 0, nl = 0, rc = 0; std::string err; };
+    // the batch's requests (their destinations are the slots reserve_batch reserves) and keys: flow keys, then LOS keys
     struct merged {
-        std::vector<pfnav_field_req> fr; std::vector<pfnav_los_req> lr;
-        std::vector<int32_t> fw, ld, slots; std::vector<int> depth, newpos, lnew; std::vector<size_t> fkeys, lkeys, keys;
-        void clear() { fr.clear(); lr.clear(); fw.clear(); ld.clear(); fkeys.clear(); lkeys.clear(); }
+        pf_wave_pack W; std::vector<size_t> keys, lkeys; std::vector<int32_t> slots;
+        void clear() { W.clear(); keys.clear(); lkeys.clear(); }
     };
     std::vector<goal_plan> plans;
     merged batch;
@@ -411,34 +505,19 @@ static int plan_batch(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int laye
     for (int g = 0; g < ngoals; g++) {
         pf_planner::goal_plan &P = PL.plans[g];
         if (P.rc) { pfnav_set_error("%s", P.err.c_str()); return P.rc; }
-        const int nf = P.nf, nl = P.nl;
-        const pfnav_field_req *fr = P.fr.data(); const pfnav_los_req *lr = P.lr.data();
-        const int32_t *fc = P.fc.data(), *fw = P.fw.data(), *lc = P.lc.data();
+        const size_t row = (size_t)dests[g] * chunks;
+        const int32_t *fc = P.fc.data(), *lc = P.lc.data();
         // PFNAV_REQUEST_MISSING_ONLY: fields the pool still holds for this destination are kept, like a field-cache hit
         // (fieldcache.c:138-141); a rebuilt LOS field whose parent chunk is kept reads the parent out of its pool slot
-        auto held = [&](int chunk, uint8_t bit) { return missing_only && (ctx->pool.has_of((size_t)dests[g] * chunks + chunk) & bit); };
-        for (int i = 0; i < nf; i++) {
+        auto held = [&](int chunk, uint8_t bit) { return missing_only && (ctx->pool.has_of(row + chunk) & bit); };
+        for (int i = 0; i < P.nf; i++) {
             if (held(fc[i], 1)) continue;
-            B.fr.push_back(fr[i]); B.fw.push_back(fw[i]);
-            B.fkeys.push_back((size_t)dests[g] * chunks + fc[i]);
+            B.W.flow(P.fr[i], P.fw[i], -1);
+            B.keys.push_back(row + fc[i]);
         }
-        B.depth.assign(nl, 0); B.newpos.assign(nl, -1);
-        for (int i = 0; i < nl; i++) {
-            if (held(lc[i], 2)) continue;
-            pfnav_los_req q = lr[i];
-            if (q.prev_index >= 0) {
-                if (B.newpos[q.prev_index] >= 0) { B.depth[i] = B.depth[q.prev_index] + 1; q.prev_index = B.newpos[q.prev_index]; }
-                else {
-                    q.prev_index = -2;      // parent kept: its absolute pool slot rides in _pad
-                    q._pad = ctx->pool.slot_of((size_t)dests[g] * chunks + q.prev_chunk_r * ctx->chunk_w + q.prev_chunk_c);
-                }
-            }
-            B.newpos[i] = (int)B.lr.size();
-            B.lr.push_back(q); B.ld.push_back(B.depth[i]);
-            B.lkeys.push_back((size_t)dests[g] * chunks + lc[i]);
-        }
+        B.W.los_chain(P.lr.data(), P.nl, [&](int i) { return !held(lc[i], 2); }, [&](int i) { B.lkeys.push_back(row + lc[i]); return -1; },
+                      [&](int p) { return ctx->pool.slot_of(row + lc[p]); });
     }
-    B.keys.assign(B.fkeys.begin(), B.fkeys.end());
     B.keys.insert(B.keys.end(), B.lkeys.begin(), B.lkeys.end());
     return PFNAV_OK;
 }
@@ -446,13 +525,13 @@ static int plan_batch(pfnav_ctx *ctx, int ngoals, const int32_t *dests, int laye
 // slots for everything a merged batch writes, all or nothing, and their `has` bits and flow requests
 static int reserve_batch(pfnav_ctx *ctx, pf_planner::merged &B)
 {
-    const int nf = (int)B.fr.size(), nl = (int)B.lr.size();
+    pf_wave_pack &W = B.W;
+    const int nf = (int)W.fr.size(), nl = (int)W.lr.size();
     B.slots.resize(B.keys.size());
     int rc = pf_pool_reserve(ctx, B.keys.data(), B.keys.size(), B.slots.data(), nullptr);
     if (rc) return rc;
-    const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
-    for (int i = 0; i < nf; i++) ctx->pool.built_flow(fs[i], B.fr[i]);
-    for (int i = 0; i < nl; i++) ctx->pool.built(ls[i], 2);
+    for (int i = 0; i < nf; i++) { W.fdst[i] = B.slots[i]; ctx->pool.built_flow(W.fdst[i], W.fr[i]); }
+    for (int i = 0; i < nl; i++) { W.ldst[i] = B.slots[nf + i]; ctx->pool.built(W.ldst[i], 2); }
     return PFNAV_OK;
 }
 
@@ -482,24 +561,15 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
             memcmp(gb.dests.data(), dests, (size_t)ngoals * 4) == 0 && memcmp(gb.targets.data(), targets, (size_t)ngoals * 16) == 0) {
             PF_CUDA(cudaSetDevice(ctx->device));
             cudaStream_t st = pf_stream(ctx, stream);
-            const uint8_t *dev = (const uint8_t *)ctx->d_plan_buf;
             int rc = los_fork(ctx, st);          // the LOS chains do not read flow fields: fork before the flow waves
             if (rc) return rc;
-            for (size_t w = 0; w + 1 < gb.fwave_off.size(); w++) {
-                const int first = gb.fwave_off[w], cnt = gb.fwave_off[w + 1] - first;
-                if (cnt <= 0) continue;
-                rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->pool.d_flow,
-                                       (const int32_t *)(dev + gb.b_fr) + first, ctx->flow_stream);
-                if (rc) return rc;
-            }
-            const int32_t one_wave[2] = {0, gb.nl};
-            rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + gb.b_fr + gb.b_fs), gb.nl, ctx->pool.d_los,
-                                  (const int32_t *)(dev + gb.b_fr + gb.b_fs + gb.b_lr), 1, one_wave, ctx->field_stream);
+            rc = pf_waves_launch(ctx, stager_of(ctx).dev, gb.waves, ctx->pool.d_flow, ctx->pool.d_los, ctx->flow_stream,
+                                 ctx->field_stream);
             if (rc) return rc;
             rc = los_forked(ctx);
             if (rc) return rc;
-            if (out_n_flow) *out_n_flow = gb.nf;
-            if (out_n_los) *out_n_los = gb.nl;
+            if (out_n_flow) *out_n_flow = gb.waves.nf;
+            if (out_n_los) *out_n_los = gb.waves.nl;
             return PFNAV_OK;
         }
         gb.valid = false;
@@ -509,109 +579,37 @@ extern "C" int pfnav_pool_request_goals_ex(pfnav_ctx *ctx, int ngoals, const int
     int rc = plan_batch(ctx, ngoals, dests, layer, targets, missing_only, ht);
     if (rc) return rc;
     pf_planner::merged &B = planner_of(ctx).batch;
-    if (B.fr.empty() && B.lr.empty()) return PFNAV_OK;
-    const int nf = (int)B.fr.size(), nl = (int)B.lr.size();
-    // stable order by wave / depth
-    int maxw = 0, maxd = 0;
-    for (int i = 0; i < nf; i++) maxw = std::max(maxw, B.fw[i]);
-    for (int i = 0; i < nl; i++) maxd = std::max(maxd, B.ld[i]);
-    std::vector<int32_t> fwave_off(maxw + 2, 0), lwave_off(maxd + 2, 0);
-    for (int i = 0; i < nf; i++) fwave_off[B.fw[i] + 1]++;
-    for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
-    for (int i = 0; i < nl; i++) lwave_off[B.ld[i] + 1]++;
-    for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
+    pf_wave_pack &W = B.W;
+    if (W.fr.empty() && W.lr.empty()) return PFNAV_OK;
     ht.lap(PF_HPROF_MERGE);
     if ((rc = reserve_batch(ctx, B))) return rc;       // all or nothing: nothing is published before this succeeds
     ht.lap(PF_HPROF_RESERVE);
-    const size_t b_fr = (size_t)nf * sizeof(pfnav_field_req), b_fs = (size_t)nf * 4;
-    const size_t b_lr = (size_t)nl * sizeof(pfnav_los_req), b_ls = (size_t)nl * 4;
-    const size_t total = b_fr + b_fs + b_lr + b_ls;
-    // the slot table and the `has` bytes travel in the same staging buffer, behind the plan
-    const size_t b_tab = (total + 15) & ~(size_t)15, stage = b_tab + ctx->pool.table_bytes();
+    const size_t bytes = W.layout();
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
-    uint8_t *host = nullptr;
-    int ri = 0;
-    if (int rc = pf_plan_host(ctx, stage, &host, &ri)) return rc;
+    // the slot table and the `has` bytes travel in the same staging buffer, behind the plan; the plan stays in the
+    // device buffer for the resident fast path
+    pf_stage S;
+    if ((rc = pf_stage_begin(ctx, st, bytes, bytes, true, &S))) return rc;
     ht.lap(PF_HPROF_WAIT);
-    pfnav_field_req *hfr = (pfnav_field_req *)host;
-    int32_t *hfs = (int32_t *)(host + b_fr);
-    pfnav_los_req *hlr = (pfnav_los_req *)(host + b_fr + b_fs);
-    int32_t *hls = (int32_t *)(host + b_fr + b_fs + b_lr);
-    {
-        const int32_t *fs = B.slots.data(), *ls = B.slots.data() + nf;
-        std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1);
-        for (int i = 0; i < nf; i++) { const int k = cur[B.fw[i]]++; hfr[k] = B.fr[i]; hfs[k] = fs[i]; }
-        std::vector<int32_t> cur2(lwave_off.begin(), lwave_off.end() - 1);
-        B.lnew.resize(nl);
-        for (int i = 0; i < nl; i++) B.lnew[i] = cur2[B.ld[i]]++;
-        for (int i = 0; i < nl; i++) {
-            pfnav_los_req q = B.lr[i];
-            if (q.prev_index >= 0) q.prev_index = B.lnew[q.prev_index];
-            hlr[B.lnew[i]] = q; hls[B.lnew[i]] = ls[i];
-        }
-    }
+    W.pack(S.host);
     ht.lap(PF_HPROF_PACK);
-    // one device plan buffer per context: the resident fast path relaunches from it, and the previous batch's forked
-    // kernels read it until they finish -- its overwrite is ordered after them (join), growing it waits for them
-    if (ctx->plan_buf_bytes < total) {
-        PF_CUDA(pf_fields_sync(ctx));
-        PF_CUDA(cudaStreamSynchronize(st));
-        cudaFree(ctx->d_plan_buf);
-        ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
-        ctx->plan_buf_bytes = total * 2;
-    }
     PF_CUDA(pf_pool_refresh(ctx, st));       // after pfnav_pool_clear: reset the touch stamps (the table is uploaded below)
-    PF_CUDA(pf_fields_join(ctx, st));
-    uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
-    PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
-    if ((rc = pf_pool_stage_table(ctx, host + b_tab, st))) return rc;
-    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    if ((rc = pf_stage_upload(ctx, st, S, bytes))) return rc;
     ht.lap(PF_HPROF_UPLOAD);
-    const pfnav_field_req *dfr = (const pfnav_field_req *)dev;
-    const int32_t *dfs = (const int32_t *)(dev + b_fr);
-    const pfnav_los_req *dlr = (const pfnav_los_req *)(dev + b_fr + b_fs);
-    const int32_t *dls = (const int32_t *)(dev + b_fr + b_fs + b_lr);
-    rc = los_fork(ctx, st);
+    if ((rc = los_fork(ctx, st))) return rc;
+    rc = pf_waves_launch(ctx, S.dev, W.out, ctx->pool.d_flow, ctx->pool.d_los, ctx->flow_stream, ctx->field_stream);
     if (rc) return rc;
-    for (int w = 0; w <= maxw; w++) {
-        const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
-        if (cnt <= 0) continue;
-        rc = pfnav_flow_launch(ctx, dfr + first, cnt, ctx->pool.d_flow, dfs + first, ctx->flow_stream);
-        if (rc) return rc;
-    }
-    if (nl) rc = pfnav_los_launch(ctx, dlr, nl, ctx->pool.d_los, dls, maxd + 1, lwave_off.data(), ctx->field_stream);
-    if (rc) return rc;
-    rc = los_forked(ctx);
-    if (rc) return rc;
+    if ((rc = los_forked(ctx))) return rc;
     ht.lap(PF_HPROF_LAUNCH);
     {
         auto &gb = ctx->goal_batch;
         gb.valid = !missing_only; gb.epoch = ctx->map_epoch; gb.layer = layer;
         gb.dests.assign(dests, dests + ngoals); gb.targets.assign(targets, targets + 4 * (size_t)ngoals);
-        gb.nf = nf; gb.nl = nl; gb.fwave_off = fwave_off; gb.b_fr = b_fr; gb.b_fs = b_fs; gb.b_lr = b_lr; gb.b_ls = b_ls;
+        gb.waves = W.out;
     }
-    if (out_n_flow) *out_n_flow = nf;
-    if (out_n_los) *out_n_los = nl;
-    return PFNAV_OK;
-}
-
-// pinned staging ring of two: buffer `ri` was last copied from two batches ago (its event guards the reuse)
-int pf_plan_host(pfnav_ctx *ctx, size_t bytes, uint8_t **out, int *out_ri)
-{
-    const int ri = ctx->plan_host_next;
-    ctx->plan_host_next ^= 1;
-    if (!ctx->plan_host_ev[ri]) PF_CUDA(cudaEventCreateWithFlags(&ctx->plan_host_ev[ri], cudaEventDisableTiming));
-    else PF_CUDA(cudaEventSynchronize(ctx->plan_host_ev[ri]));
-    if (ctx->plan_host_bytes[ri] < bytes) {      // grow-only
-        cudaFreeHost(ctx->plan_host[ri]);
-        ctx->plan_host[ri] = nullptr; ctx->plan_host_bytes[ri] = 0;
-        PF_CUDA(cudaMallocHost(&ctx->plan_host[ri], bytes * 2));
-        ctx->plan_host_bytes[ri] = bytes * 2;
-    }
-    *out = (uint8_t *)ctx->plan_host[ri];
-    *out_ri = ri;
+    if (out_n_flow) *out_n_flow = W.out.nf;
+    if (out_n_los) *out_n_los = W.out.nl;
     return PFNAV_OK;
 }
 
@@ -667,6 +665,20 @@ static int field_copy_launch(pfnav_ctx *ctx, const uint8_t *flow_src, const uint
     return 0;
 }
 
+// the staging buffer of a job, at least `need` bytes. The previous batch's builds, exchange and copies may still read it,
+// so growing it waits for the device (a group member's stream has waited for its peers' reads of its staging)
+static int job_stage_reserve(pfnav_ctx *ctx, size_t need)
+{
+    if (ctx->job_stage_bytes >= need) return PFNAV_OK;
+    PF_CUDA(pf_fields_sync(ctx));
+    PF_CUDA(cudaDeviceSynchronize());
+    cudaFree(ctx->d_job_stage);
+    ctx->d_job_stage = nullptr; ctx->job_stage_bytes = 0;
+    PF_CUDA(cudaMalloc(&ctx->d_job_stage, need * 2));
+    ctx->job_stage_bytes = need * 2;
+    return PFNAV_OK;
+}
+
 // a job's batch reads the replicated map: refused while this member holds device blocker ops its peers have not seen
 int pf_job_check_state(pfnav_ctx *ctx)
 {
@@ -693,7 +705,7 @@ int pf_job_plan(pfnav_ctx *ctx, pf_job &J)
     int rc = plan_batch(ctx, J.ngoals, J.dests, J.layer, J.targets, missing_only, ht);
     if (rc) return rc;
     const pf_planner::merged &B = planner_of(ctx).batch;
-    J.nf = (int)B.fr.size(); J.nl = (int)B.lr.size();
+    J.nf = (int)B.W.fr.size(); J.nl = (int)B.W.lr.size();
     J.fits = pf_pool_fits(ctx->pool, B.keys.data(), B.keys.size());
     for (int g = 0; g < J.ngoals; g++)
         for (int c = 0; c < chunks; c++)
@@ -758,10 +770,8 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
     // ---- what this member builds: its goals' union fields, into staging. A rebuilt LOS field whose parent is in the
     // union reads the parent from staging; a parent that every member keeps is copied from this member's pool into a
     // block behind the segments first, before anything of this batch is written.
-    std::vector<pfnav_field_req> bfr; std::vector<int32_t> bfw, bfs;
-    std::vector<pfnav_los_req> blr; std::vector<int32_t> bld, bls;
+    pf_wave_pack W;
     std::vector<pf_field_copy> parents;
-    std::vector<int> newpos;
     int32_t extra = next;
     for (int g = 0; g < ngoals; g++) {
         if (owner[g] != rank) continue;
@@ -769,28 +779,13 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
         const uint8_t *u = uni + (size_t)g * chunks;
         const size_t gi = (size_t)g * chunks, row = (size_t)J.dests[g] * chunks;
         for (int i = 0; i < P.nf; i++)
-            if (u[P.fc[i]] & 1) { bfr.push_back(P.fr[i]); bfw.push_back(P.fw[i]); bfs.push_back(fblk[gi + P.fc[i]]); }
-        newpos.assign(P.nl, -1);
-        for (int i = 0; i < P.nl; i++) {
-            if (!(u[P.lc[i]] & 2)) continue;
-            pfnav_los_req q = P.lr[i];
-            int d = 0;
-            if (q.prev_index >= 0) {
-                const int p = q.prev_index;
-                if (newpos[p] >= 0) { d = bld[newpos[p]] + 1; q.prev_index = newpos[p]; }
-                else {
-                    parents.push_back({ctx->pool.slot_of(row + P.lc[p]), extra, 1});
-                    q.prev_index = -2; q._pad = extra++;
-                }
-            }
-            newpos[i] = (int)blr.size();
-            blr.push_back(q); bld.push_back(d); bls.push_back(lblk[gi + P.lc[i]]);
-        }
+            if (u[P.fc[i]] & 1) W.flow(P.fr[i], P.fw[i], fblk[gi + P.fc[i]]);
+        W.los_chain(P.lr.data(), P.nl, [&](int i) { return (u[P.lc[i]] & 2) != 0; }, [&](int i) { return lblk[gi + P.lc[i]]; },
+                    [&](int p) { parents.push_back({ctx->pool.slot_of(row + P.lc[p]), extra, 1}); return extra++; });
     }
     // ---- this member's own slots, exactly as its solo call reserves them
     int rc = 0;
     if (!B.keys.empty() && (rc = reserve_batch(ctx, B))) return rc;
-    ctx->goal_batch.valid = false;          // the plan buffer is about to be reused
     // ---- the fields this member lacks: staging block -> its slot (a flow field once per (goal, chunk))
     std::vector<pf_field_copy> items;
     std::vector<uint8_t> seen((size_t)ngoals * chunks, 0);
@@ -806,86 +801,30 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
         for (int i = 0; i < P.nl; i++)
             if (J.lack[gi + P.lc[i]] & 2) items.push_back({lblk[gi + P.lc[i]], ctx->pool.slot_of(row + P.lc[i]), 1});
     }
-    // ---- pack: builds in wave / depth order, the copies, then the slot table and the `has` bytes
-    const int nf = (int)bfr.size(), nl = (int)blr.size(), np = (int)parents.size(), ni = (int)items.size();
-    int maxw = 0, maxd = 0;
-    for (int i = 0; i < nf; i++) maxw = std::max(maxw, bfw[i]);
-    for (int i = 0; i < nl; i++) maxd = std::max(maxd, bld[i]);
-    std::vector<int32_t> fwave_off(maxw + 2, 0), lwave_off(maxd + 2, 0);
-    for (int i = 0; i < nf; i++) fwave_off[bfw[i] + 1]++;
-    for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
-    for (int i = 0; i < nl; i++) lwave_off[bld[i] + 1]++;
-    for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
-    size_t off = 0;
-    auto sec = [&](size_t bytes) { const size_t o = off; off = (off + bytes + 15) & ~(size_t)15; return o; };
-    const size_t o_fr = sec((size_t)nf * sizeof(pfnav_field_req)), o_fs = sec((size_t)nf * 4);
-    const size_t o_lr = sec((size_t)nl * sizeof(pfnav_los_req)), o_ls = sec((size_t)nl * 4);
-    const size_t o_pc = sec((size_t)np * sizeof(pf_field_copy)), o_it = sec((size_t)ni * sizeof(pf_field_copy));
-    const size_t total = off;
+    // ---- stage: the builds in wave / depth order, the copies, then the slot table and the `has` bytes
+    const size_t b_pc = parents.size() * sizeof(pf_field_copy), b_it = items.size() * sizeof(pf_field_copy);
+    const size_t o_pc = W.layout(), o_it = o_pc + pf_wave_pack::align16(b_pc), total = o_it + pf_wave_pack::align16(b_it);
     PF_CUDA(cudaSetDevice(ctx->device));
-    uint8_t *host = nullptr;
-    int ri = 0;
-    if ((rc = pf_plan_host(ctx, total + ctx->pool.table_bytes(), &host, &ri))) return rc;
-    {
-        pfnav_field_req *hfr = (pfnav_field_req *)(host + o_fr);
-        int32_t *hfs = (int32_t *)(host + o_fs), *hls = (int32_t *)(host + o_ls);
-        pfnav_los_req *hlr = (pfnav_los_req *)(host + o_lr);
-        std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1);
-        for (int i = 0; i < nf; i++) { const int k = cur[bfw[i]]++; hfr[k] = bfr[i]; hfs[k] = bfs[i]; }
-        std::vector<int32_t> cur2(lwave_off.begin(), lwave_off.end() - 1), lnew(nl);
-        for (int i = 0; i < nl; i++) lnew[i] = cur2[bld[i]]++;
-        for (int i = 0; i < nl; i++) {
-            pfnav_los_req q = blr[i];
-            if (q.prev_index >= 0) q.prev_index = lnew[q.prev_index];
-            hlr[lnew[i]] = q; hls[lnew[i]] = bls[i];
-        }
-        memcpy(host + o_pc, parents.data(), (size_t)np * sizeof(pf_field_copy));
-        memcpy(host + o_it, items.data(), (size_t)ni * sizeof(pf_field_copy));
-    }
-    // the plan buffer and the staging buffer: the previous batch's kernels and exchange may still read them, so growing
-    // either waits for the device (a group member's stream has waited for its peers' reads of its staging)
-    const size_t need = (size_t)extra * 4096;
-    if (ctx->plan_buf_bytes < total || ctx->job_stage_bytes < need) {
-        PF_CUDA(pf_fields_sync(ctx));
-        PF_CUDA(cudaDeviceSynchronize());
-        if (ctx->plan_buf_bytes < total) {
-            cudaFree(ctx->d_plan_buf);
-            ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
-            PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
-            ctx->plan_buf_bytes = total * 2;
-        }
-        if (ctx->job_stage_bytes < need) {
-            cudaFree(ctx->d_job_stage);
-            ctx->d_job_stage = nullptr; ctx->job_stage_bytes = 0;
-            PF_CUDA(cudaMalloc(&ctx->d_job_stage, need * 2));
-            ctx->job_stage_bytes = need * 2;
-        }
-    }
+    if ((rc = job_stage_reserve(ctx, (size_t)extra * 4096))) return rc;
+    pf_stage S;
+    if ((rc = pf_stage_begin(ctx, st, total, total, true, &S))) return rc;
+    W.pack(S.host);
+    memcpy(S.host + o_pc, parents.data(), b_pc);
+    memcpy(S.host + o_it, items.data(), b_it);
     PF_CUDA(pf_pool_refresh(ctx, st));
-    PF_CUDA(pf_fields_join(ctx, st));
-    uint8_t *dev = (uint8_t *)ctx->d_plan_buf, *stage = ctx->d_job_stage;
-    PF_CUDA(cudaMemcpyAsync(dev, host, total, cudaMemcpyHostToDevice, st));
-    if ((rc = pf_pool_stage_table(ctx, host + total, st))) return rc;
-    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
-    if ((rc = field_copy_launch(ctx, nullptr, ctx->pool.d_los, nullptr, stage, (const pf_field_copy *)(dev + o_pc), np, st)))
+    if ((rc = pf_stage_upload(ctx, st, S, total))) return rc;
+    uint8_t *stage = ctx->d_job_stage;
+    if ((rc = field_copy_launch(ctx, nullptr, ctx->pool.d_los, nullptr, stage, (const pf_field_copy *)(S.dev + o_pc),
+                                (int)parents.size(), st)))
         return rc;
     // the owner's builds: flow waves and LOS chains on the context's field streams, as in the solo call; the exchange
     // that follows on `st` reads what they wrote
     if ((rc = los_fork(ctx, st))) return rc;
-    for (int w = 0; w <= maxw; w++) {
-        const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
-        if (cnt <= 0) continue;
-        rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)(dev + o_fr) + first, cnt, stage,
-                               (const int32_t *)(dev + o_fs) + first, ctx->flow_stream);
-        if (rc) return rc;
-    }
-    if (nl && (rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + o_lr), nl, stage, (const int32_t *)(dev + o_ls),
-                                     maxd + 1, lwave_off.data(), ctx->field_stream)))
-        return rc;
+    if ((rc = pf_waves_launch(ctx, S.dev, W.out, stage, stage, ctx->flow_stream, ctx->field_stream))) return rc;
     if ((rc = los_forked(ctx))) return rc;
     PF_CUDA(pf_fields_join(ctx, st));
-    ctx->job_built[0] = nf; ctx->job_built[1] = nl;
-    J.d_items = dev + o_it; J.nitems = ni;
+    ctx->job_built[0] = W.out.nf; ctx->job_built[1] = W.out.nl;
+    J.d_items = S.dev + o_it; J.nitems = (int)items.size();
     return PFNAV_OK;
 }
 
@@ -944,24 +883,12 @@ void pf_job_layout(pfnav_ctx *ctx, pf_job &J, const std::vector<int32_t> &freq, 
 int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &items, int world, cudaStream_t st)
 {
     const size_t o_items = J.seg[world] * 4096, b_items = items.size() * sizeof(pf_field_copy);
-    const size_t need = o_items + b_items;
-    // the previous batch's builds, exchange and copies may still read the staging buffer: growing it waits for the
-    // device (a group member's stream has waited for its peers' reads of its staging)
-    if (ctx->job_stage_bytes < need) {
-        PF_CUDA(pf_fields_sync(ctx));
-        PF_CUDA(cudaDeviceSynchronize());
-        cudaFree(ctx->d_job_stage);
-        ctx->d_job_stage = nullptr; ctx->job_stage_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_job_stage, need * 2));
-        ctx->job_stage_bytes = need * 2;
-    }
-    uint8_t *host = nullptr;
-    int ri = 0;
-    if (int rc = pf_plan_host(ctx, b_items + ctx->pool.table_bytes(), &host, &ri)) return rc;
-    memcpy(host, items.data(), b_items);
-    if (b_items) PF_CUDA(cudaMemcpyAsync(ctx->d_job_stage + o_items, host, b_items, cudaMemcpyHostToDevice, st));
-    if (int rc = pf_pool_stage_table(ctx, host + b_items, st)) return rc;
-    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    if (int rc = job_stage_reserve(ctx, o_items + b_items)) return rc;
+    pf_stage S;
+    if (int rc = pf_stage_begin(ctx, st, b_items, 0, true, &S)) return rc;
+    memcpy(S.host, items.data(), b_items);
+    if (b_items) PF_CUDA(cudaMemcpyAsync(ctx->d_job_stage + o_items, S.host, b_items, cudaMemcpyHostToDevice, st));
+    if (int rc = pf_stage_upload(ctx, st, S, 0)) return rc;
     J.d_items = ctx->d_job_stage + o_items; J.nitems = (int)items.size();
     return PFNAV_OK;
 }

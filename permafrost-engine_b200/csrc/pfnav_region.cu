@@ -436,24 +436,6 @@ extern "C" int pfnav_zone_fields(pfnav_ctx *ctx, int layer, int centre_r, int ce
     return rc;
 }
 
-// The device scratch of the entity and zone field batches (context-owned, grow-only): the next batch may run on another
-// stream, so its overwrite is ordered after the last batch's kernels through ent_ev; record ent_ev after the kernels
-// that read it.
-static int batch_scratch(pfnav_ctx *ctx, cudaStream_t st, size_t need, uint8_t **out)
-{
-    if (!ctx->ent_ev) PF_CUDA(cudaEventCreateWithFlags(&ctx->ent_ev, cudaEventDisableTiming));
-    else PF_CUDA(cudaStreamWaitEvent(st, ctx->ent_ev, 0));
-    if (ctx->ent_buf_bytes < need) {        // grow-only: the old buffer may still be read by the previous batch
-        PF_CUDA(cudaEventSynchronize(ctx->ent_ev));
-        cudaFree(ctx->d_ent_buf);
-        ctx->d_ent_buf = nullptr; ctx->ent_buf_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_ent_buf, need * 2));
-        ctx->ent_buf_bytes = need * 2;
-    }
-    *out = (uint8_t *)ctx->d_ent_buf;
-    return PFNAV_OK;
-}
-
 // the pool entries a zone batch changed: slot table entries fresh[2i] = fresh[2i + 1], `has` bytes has[slot[i]] = hasv[i]
 __global__ void k_pool_scatter(const int32_t *__restrict__ fresh, int nfresh, int32_t *__restrict__ slot_table,
                                const int32_t *__restrict__ slot, const uint8_t *__restrict__ hasv, int nhas, uint8_t *__restrict__ has)
@@ -595,27 +577,24 @@ static int zone_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_zone_req *req
     // the `has` bytes of the written slots (the host mirror after the batch)
     std::vector<uint8_t> hasv(scatter ? nk : 0);
     for (size_t k = 0; k < hasv.size(); k++) hasv[k] = ctx->pool.has[kslot[k]];
-    // ---- one pinned staging buffer with the inputs, copied into the device scratch
+    // ---- the inputs, staged; the seed bitmaps follow them in the device buffer
     size_t b_in = 0;
     auto sec = [&](size_t bytes) { const size_t o = b_in; b_in = (b_in + bytes + 15) & ~(size_t)15; return o; };
     const size_t o_req = sec(nk * sizeof(pfnav_region_req)), o_slot = sec(nk * 4);
     const size_t o_jobs = sec(host_floods ? 0 : nk * sizeof(zone_job)), o_seeds = sec(seeds.size() * 4);
     const size_t o_fresh = sec(fresh.size() * 4), o_hasv = sec(hasv.size());
-    const size_t stage = b_in;
     const size_t o_bits = b_in, need = o_bits + (host_floods ? 0 : nk * ((size_t)dim * dim / 8)) + 16;
-    uint8_t *host = nullptr, *dev = nullptr;
-    int ri = 0;
-    int lrc = pf_plan_host(ctx, stage, &host, &ri);
+    pf_stage S;
+    int lrc = pf_stage_begin(ctx, st, b_in, need, false, &S);
     if (lrc) return lrc;
+    uint8_t *host = S.host, *dev = S.dev;
     memcpy(host + o_req, kreq.data(), nk * sizeof(pfnav_region_req));
     memcpy(host + o_slot, kslot.data(), nk * 4);
     if (!host_floods) memcpy(host + o_jobs, jobs.data(), nk * sizeof(zone_job));
     memcpy(host + o_seeds, seeds.data(), seeds.size() * 4);
     memcpy(host + o_fresh, fresh.data(), fresh.size() * 4);
     memcpy(host + o_hasv, hasv.data(), hasv.size());
-    if ((lrc = batch_scratch(ctx, st, need, &dev))) return lrc;
-    PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    if ((lrc = pf_stage_upload(ctx, st, S, b_in))) return lrc;
     const int nscatter = (int)std::max(fresh.size() / 2, hasv.size());
     if (nscatter) {
         k_pool_scatter<<<(unsigned)((nscatter + 255) / 256), 256, 0, st>>>((const int32_t *)(dev + o_fresh), (int)(fresh.size() / 2),
@@ -643,8 +622,7 @@ static int zone_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_zone_req *req
                                  (const int32_t *)(dev + o_slot))))
             return lrc;
     }
-    PF_CUDA(cudaEventRecord(ctx->ent_ev, st));
-    return PFNAV_OK;
+    return pf_stage_done(ctx, st);
 }
 
 // N_RequestAsyncGroupArrivalField (nav.c:3921) for m requests, in the order of the serial calls (zone_reserve). The
@@ -1174,20 +1152,19 @@ static int entity_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_fiel
         item_off.push_back((uint32_t)items.size()); hitem_off.push_back((uint32_t)hitems.size());
     }
     const size_t nk = kreq.size(), nj = jobs.size();
-    // ---- one pinned staging buffer: the inputs (copied into the device scratch), then the slot table and `has` bytes
+    // ---- the inputs, staged (then the slot table and `has` bytes); footprint rows and seed bitmaps follow them on the device
     size_t b_in = 0;
     auto sec = [&](size_t bytes) { const size_t o = b_in; b_in = (b_in + bytes + 15) & ~(size_t)15; return o; };
     const size_t o_req = sec(nk * sizeof(pfnav_region_req)), o_slot = sec(nk * 4);
     const size_t o_ioff = sec(item_off.size() * 4), o_items = sec(items.size() * 4);
     const size_t o_hoff = sec(hitem_off.size() * 4), o_hitems = sec(hitems.size() * 4);
     const size_t o_jobs = sec(nj * sizeof(fp_job)), o_toff = sec(htile_off.size() * 4), o_tiles = sec(htiles.size() * 4);
-    const size_t stage = b_in + (upload_pool ? ctx->pool.table_bytes() : 0);
     const size_t o_org = b_in + 0, o_rows = o_org + ((nj * 8 + 15) & ~(size_t)15), o_bits = o_rows + nj * 128;
     const size_t need = o_bits + nk * ((size_t)dim * dim / 8);
-    uint8_t *host = nullptr;
-    int ri = 0;
-    int rc = pf_plan_host(ctx, stage, &host, &ri);
+    pf_stage S;
+    int rc = pf_stage_begin(ctx, st, b_in, need, upload_pool, &S);
     if (rc) return rc;
+    uint8_t *host = S.host, *dev = S.dev;
     memcpy(host + o_req, kreq.data(), nk * sizeof(pfnav_region_req));
     memcpy(host + o_slot, kslot.data(), nk * 4);
     memcpy(host + o_ioff, item_off.data(), item_off.size() * 4);
@@ -1197,11 +1174,7 @@ static int entity_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_fiel
     memcpy(host + o_jobs, jobs.data(), nj * sizeof(fp_job));
     memcpy(host + o_toff, htile_off.data(), htile_off.size() * 4);
     memcpy(host + o_tiles, htiles.data(), htiles.size() * 4);
-    uint8_t *dev = nullptr;
-    if ((rc = batch_scratch(ctx, st, need, &dev))) return rc;
-    PF_CUDA(cudaMemcpyAsync(dev, host, b_in, cudaMemcpyHostToDevice, st));
-    if (upload_pool && (rc = pf_pool_stage_table(ctx, host + b_in, st))) return rc;
-    PF_CUDA(cudaEventRecord(ctx->plan_host_ev[ri], st));
+    if ((rc = pf_stage_upload(ctx, st, S, b_in))) return rc;
     const pfnav_region_req *d_req = (const pfnav_region_req *)(dev + o_req);
     int2 *d_org = (int2 *)(dev + o_org);
     uint32_t *d_rows = (uint32_t *)(dev + o_rows), *d_bits = (uint32_t *)(dev + o_bits);
@@ -1220,8 +1193,7 @@ static int entity_build(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_fiel
     if ((rc = region_launch(ctx, dim, d_req, nk, (const int32_t *)dev, (const int32_t *)dev, d_out, st, 1, d_bits,
                             (const int32_t *)(dev + o_slot))))
         return rc;
-    PF_CUDA(cudaEventRecord(ctx->ent_ev, st));
-    return PFNAV_OK;
+    return pf_stage_done(ctx, st);
 }
 
 extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,

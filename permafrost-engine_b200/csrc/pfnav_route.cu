@@ -877,64 +877,26 @@ namespace {
 // The flow waves and LOS requests of consecutive requests of a batch that go to the device together. Within one
 // segment no pool slot changes owner, so (dest, chunk) keys and slots correspond one to one.
 struct path_segment {
-    std::vector<pfnav_field_req> fr; std::vector<int32_t> fs, fw;
-    std::vector<pfnav_los_req> lr; std::vector<int32_t> ls, ld;
+    pf_wave_pack W;                                   // flow requests by wave, LOS requests with their parents
     std::unordered_map<int32_t, int> writes;          // slot -> flow writes to it so far: the next one goes a wave later
-    std::unordered_map<size_t, int> los_at;           // (dest, chunk) -> its LOS request in lr
+    std::unordered_map<size_t, int> los_at;           // (dest, chunk) -> its LOS request in W
     std::vector<std::pair<int32_t, size_t>> used;     // (slot, key) of every slot written or read
-    void clear() { fr.clear(); fs.clear(); fw.clear(); lr.clear(); ls.clear(); ld.clear(); writes.clear(); los_at.clear(); used.clear(); }
+    void clear() { W.clear(); writes.clear(); los_at.clear(); used.clear(); }
 };
 
-// Upload a segment's requests and launch its flow waves and its one LOS launch on `st`.
-static int launch_segment(pfnav_ctx *ctx, cudaStream_t st, const path_segment &S)
+// Stage a segment's requests and launch its flow waves and its one LOS launch on `st`.
+static int launch_segment(pfnav_ctx *ctx, cudaStream_t st, path_segment &S)
 {
-    const int nf = (int)S.fr.size(), nl = (int)S.lr.size();
-    if (nf == 0 && nl == 0) return PFNAV_OK;
-    int maxw = 0, maxd = 0;
-    for (int i = 0; i < nf; i++) maxw = std::max(maxw, S.fw[i]);
-    for (int i = 0; i < nl; i++) maxd = std::max(maxd, S.ld[i]);
-    std::vector<int32_t> fwave_off(maxw + 2, 0), lwave_off(maxd + 2, 0);
-    for (int i = 0; i < nf; i++) fwave_off[S.fw[i] + 1]++;
-    for (int w = 0; w <= maxw; w++) fwave_off[w + 1] += fwave_off[w];
-    for (int i = 0; i < nl; i++) lwave_off[S.ld[i] + 1]++;
-    for (int d = 0; d <= maxd; d++) lwave_off[d + 1] += lwave_off[d];
-    const size_t b_fr = (size_t)nf * sizeof(pfnav_field_req), b_fs = (size_t)nf * 4;
-    const size_t b_lr = (size_t)nl * sizeof(pfnav_los_req), b_ls = (size_t)nl * 4;
-    const size_t total = b_fr + b_fs + b_lr + b_ls;
-    std::vector<uint8_t> host(total);
-    pfnav_field_req *hfr = (pfnav_field_req *)host.data();
-    int32_t *hfs = (int32_t *)(host.data() + b_fr);
-    pfnav_los_req *hlr = (pfnav_los_req *)(host.data() + b_fr + b_fs);
-    int32_t *hls = (int32_t *)(host.data() + b_fr + b_fs + b_lr);
-    {   // stable order by wave / depth: an LOS request follows the one it reads
-        std::vector<int32_t> cur(fwave_off.begin(), fwave_off.end() - 1), cur2(lwave_off.begin(), lwave_off.end() - 1), lnew(nl);
-        for (int i = 0; i < nf; i++) { const int k = cur[S.fw[i]]++; hfr[k] = S.fr[i]; hfs[k] = S.fs[i]; }
-        for (int i = 0; i < nl; i++) lnew[i] = cur2[S.ld[i]]++;
-        for (int i = 0; i < nl; i++) {
-            pfnav_los_req q = S.lr[i];
-            if (q.prev_index >= 0) q.prev_index = lnew[q.prev_index];
-            hlr[lnew[i]] = q; hls[lnew[i]] = S.ls[i];
-        }
-    }
-    if (ctx->plan_buf_bytes < total) {
-        PF_CUDA(cudaStreamSynchronize(st));
-        cudaFree(ctx->d_plan_buf);
-        ctx->d_plan_buf = nullptr; ctx->plan_buf_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_plan_buf, total * 2));
-        ctx->plan_buf_bytes = total * 2;
-    }
-    uint8_t *dev = (uint8_t *)ctx->d_plan_buf;
-    PF_CUDA(cudaMemcpyAsync(dev, host.data(), total, cudaMemcpyHostToDevice, st));
-    PF_CUDA(cudaStreamSynchronize(st));      // `host` is pageable and about to go out of scope
-    for (int w = 0; w <= maxw; w++) {
-        const int first = fwave_off[w], cnt = fwave_off[w + 1] - first;
-        if (cnt <= 0) continue;
-        int rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)dev + first, cnt, ctx->pool.d_flow, (const int32_t *)(dev + b_fr) + first, st);
-        if (rc) return rc;
-    }
-    if (nl) return pfnav_los_launch(ctx, (const pfnav_los_req *)(dev + b_fr + b_fs), nl, ctx->pool.d_los,
-                                    (const int32_t *)(dev + b_fr + b_fs + b_lr), maxd + 1, lwave_off.data(), st);
-    return PFNAV_OK;
+    pf_wave_pack &W = S.W;
+    if (W.fr.empty() && W.lr.empty()) return PFNAV_OK;
+    const size_t bytes = W.layout();
+    pf_stage G;
+    int rc = pf_stage_begin(ctx, st, bytes, bytes, false, &G);
+    if (rc) return rc;
+    W.pack(G.host);
+    if ((rc = pf_stage_upload(ctx, st, G, bytes))) return rc;
+    if ((rc = pf_waves_launch(ctx, G.dev, W.out, ctx->pool.d_flow, ctx->pool.d_los, st, st))) return rc;
+    return pf_stage_done(ctx, st);
 }
 
 }   // namespace
@@ -1039,7 +1001,6 @@ int pf_path_batch_commit(pf_path_batch *B, std::vector<int32_t> *out_slots)
     const int nf = (int)E.fr.size(), nl = (int)E.lr.size();
     if (out_slots) out_slots->clear();
     if (nf == 0 && nl == 0) return PFNAV_OK;
-    ctx->goal_batch.valid = false;          // the staging buffer is about to be reused
     const std::vector<size_t> &keys = B->keys;
     std::vector<int32_t> slots(keys.size());
     bool evicted = false;
@@ -1060,23 +1021,21 @@ int pf_path_batch_commit(pf_path_batch *B, std::vector<int32_t> *out_slots)
         const int32_t s = slots[i];
         ctx->pool.built_flow(s, E.fr[i]);
         ctx->pool.ffid[row + E.fc[i]] = E.fid[i];
-        S.fr.push_back(E.fr[i]); S.fs.push_back(s); S.fw.push_back(S.writes[s]++);
+        S.W.flow(E.fr[i], S.writes[s]++, s);
     }
-    const int l0 = (int)S.lr.size();
+    const int l0 = (int)S.W.lr.size();
     for (int i = 0; i < nl; i++) {
         const int32_t s = slots[nf + i];
         ctx->pool.built(s, 2);
         pfnav_los_req q = E.lr[i];
-        int depth = 0;
-        if (q.prev_index >= 0) { q.prev_index += l0; depth = S.ld[q.prev_index] + 1; }
+        if (q.prev_index >= 0) q.prev_index += l0;
         else if (q.prev_index == -2) {
             const size_t pkey = row + q.prev_chunk_r * cw + q.prev_chunk_c;
             auto it = S.los_at.find(pkey);
-            if (it != S.los_at.end()) { q.prev_index = it->second; depth = S.ld[it->second] + 1; }   // built earlier in this segment
-            else q._pad = ctx->pool.slot_of(pkey);                                                      // absolute pool slot of prev_los
+            if (it != S.los_at.end()) q.prev_index = it->second;        // built earlier in this segment
+            else q._pad = ctx->pool.slot_of(pkey);                      // absolute pool slot of prev_los
         }
-        S.los_at[row + E.lc[i]] = (int)S.lr.size();
-        S.lr.push_back(q); S.ls.push_back(s); S.ld.push_back(depth);
+        S.los_at[row + E.lc[i]] = S.W.los(q, s);
     }
     if (out_slots) out_slots->assign(slots.begin(), slots.begin() + nf + nl);
     return PFNAV_OK;
