@@ -2354,6 +2354,17 @@ __global__ void k_collect_misses(MapView m, PoolView pool, const uint16_t *__res
     out[k] = r;
 }
 
+// The in-place repair of the field in pool slot `slot` for miss r: to the nearest pathable tile from a blocked tile,
+// else to the nearest tile of the entity's local island. pf_chain_item_seeds sets its mask.
+static pf_chain_item chain_item_of(const pfnav_ctx *ctx, const pf_miss &r, int slot, int always)
+{
+    pf_chain_item it;
+    it.q = ctx->pool.req[slot]; it.slot = slot; it.tile = r.tile; it.always = always;
+    if (r.liid == 0xFFFF) { it.kind = PFNAV_REPAIR_NEAREST_PATHABLE; it.arg = ((r.tile >> 6) << 8) | (r.tile & 63); }
+    else                  { it.kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; it.arg = r.liid; }
+    return it;
+}
+
 // The on-miss branches of one navigation tick against the device pool, in the reference's order: first every
 // work item's LOS state (compute_los_state, movement.c:4129: a (dest, chunk) without LOS field requests the path
 // from the entity's previous position), then every work item's desired velocity (compute_desired_velocity, :4163:
@@ -2419,6 +2430,14 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
         if (nf + nl > 0) nreq++;
         return 0;
     };
+    auto repair = [&](const pf_miss &r, int slot) -> int {        // blocking, as the read-back that follows expects
+        pf_chain_item it = chain_item_of(ctx, r, slot, 1);
+        std::vector<uint64_t> masks;
+        int rc2 = pf_chain_item_seeds(ctx, it, masks);
+        if (!rc2) rc2 = pfnav_repair_chain_launch(ctx, st, {it}, masks, ctx->pool.d_flow, 0, nullptr);
+        if (!rc2) PF_CUDA(cudaStreamSynchronize(st));
+        return rc2;
+    };
     std::vector<pf_miss> reps;
     // ---- LOS state (N_HasDestLOS, nav.c:4038-4045) ----
     if (!(rc = collect(0, reps))) {
@@ -2449,13 +2468,7 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
             if (!ok) continue;                                            // no path from here: zero vector, nothing repaired (nav.c:3501)
             if ((rc = dir_now(&dir))) break;
             if (dir != 0) continue;                                       // case 1: the path query fixed it (or no field: no path)
-            const int slot = ctx->pool.slot[(size_t)r.dest * chunks + r.chunk];
-            const pfnav_field_req tg = ctx->pool.req[slot];
-            int32_t kind, arg;
-            if (r.liid == 0xFFFF) { kind = PFNAV_REPAIR_NEAREST_PATHABLE; arg = ((r.tile >> 6) << 8) | (r.tile & 63); }
-            else                  { kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; arg = r.liid; }
-            const int32_t sl = slot;
-            if ((rc = pfnav_flow_repair_pool(ctx, &tg, &kind, &arg, &sl, 1))) break;
+            if ((rc = repair(r, ctx->pool.slot[(size_t)r.dest * chunks + r.chunk]))) break;
             nrep++;
         }
     }
@@ -2472,16 +2485,12 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
             const pfnav_field_req tg = ctx->pool.req[slot];
             if ((tg.target_type & 0xFF) < 2) continue;
             const bool surround = (tg.target_type & 0xFF) == 2 + PFNAV_TARGET_ENTITY;
-            int32_t kind, arg;
             if (r.liid == 0xFFFF) {
                 if ((d & 0xF) != 0 && !surround) continue;
-                kind = PFNAV_REPAIR_NEAREST_PATHABLE; arg = ((r.tile >> 6) << 8) | (r.tile & 63);
             } else {
                 if ((d & 0xF) != 0) continue;
-                kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; arg = r.liid;
             }
-            const int32_t sl = slot;
-            if ((rc = pfnav_flow_repair_pool(ctx, &tg, &kind, &arg, &sl, 1))) break;
+            if ((rc = repair(r, slot))) break;
             nrep++;
         }
     }
@@ -2725,7 +2734,7 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
         auto boundary = [&](size_t from) -> int {
             int r2 = pf_path_batch_flush(pb);
             if (r2) return r2;
-            if ((r2 = pfnav_repair_chain_launch(ctx, st, items, masks, d_cnt + 2))) return r2;
+            if ((r2 = pfnav_repair_chain_launch(ctx, st, items, masks, ctx->pool.d_flow, 0, d_cnt + 2))) return r2;
             nrounds += pending;
             items.clear(); masks.clear();
             for (int32_t s : touched) written[s] = chained[s] = 0;
@@ -2773,14 +2782,8 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
             if (!pr.ok) { i++; continue; }                           // no path from here: zero vector, nothing repaired
             const int sl = ctx->pool.slot[key];
             if (!has_flow(sl)) { i++; continue; }                    // no field: nothing to repair
-            pf_chain_item it;
-            it.q = ctx->pool.req[sl]; it.slot = sl; it.tile = r.tile; it.always = 0; it.mask = -1;
-            if (r.liid == 0xFFFF) { it.kind = PFNAV_REPAIR_NEAREST_PATHABLE; it.arg = ((r.tile >> 6) << 8) | (r.tile & 63); }
-            else                  { it.kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; it.arg = r.liid; }
-            std::vector<uint64_t> mask(64);
-            const int src = it.kind == 0 ? pfnav_repair_start_check(ctx, it.q, it.arg)
-                                         : pfnav_repair_seeds(ctx, it.q, it.kind, it.arg, mask.data());
-            if (src) {
+            pf_chain_item it = chain_item_of(ctx, r, sl, 0);
+            if (const int src = pf_chain_item_seeds(ctx, it, masks)) {
                 // the serial loop fails here only if the repair runs: decide on the byte as the round leaves it. With
                 // nothing pending, nothing ran since the last gather and the byte read there is still the pool's.
                 const int keep = src;
@@ -2789,7 +2792,6 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
                 i++;
                 continue;
             }
-            if (it.kind == 1) { it.mask = (int32_t)(masks.size() / 64); masks.insert(masks.end(), mask.begin(), mask.end()); }
             items.push_back(it);
             mark(chained, sl);
             pending = true;
@@ -2816,16 +2818,10 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
             const pfnav_field_req tg = ctx->pool.req[slot];
             if ((tg.target_type & 0xFF) < 2) continue;
             const bool surround = (tg.target_type & 0xFF) == 2 + PFNAV_TARGET_ENTITY;
-            pf_chain_item it;
-            it.q = tg; it.slot = slot; it.tile = r.tile; it.mask = -1;
-            if (r.liid == 0xFFFF) { it.kind = PFNAV_REPAIR_NEAREST_PATHABLE; it.arg = ((r.tile >> 6) << 8) | (r.tile & 63); it.always = surround; }
-            else                  { it.kind = PFNAV_REPAIR_ISLAND_TO_NEAREST; it.arg = r.liid; it.always = 0; }
-            std::vector<uint64_t> mask(64);
-            const int src = it.kind == 0 ? pfnav_repair_start_check(ctx, it.q, it.arg)
-                                         : pfnav_repair_seeds(ctx, it.q, it.kind, it.arg, mask.data());
-            if (src) {
+            pf_chain_item it = chain_item_of(ctx, r, slot, r.liid == 0xFFFF && surround);
+            if (const int src = pf_chain_item_seeds(ctx, it, masks)) {
                 // fails only if the repair runs: apply what comes before it, then read the byte
-                if ((rc = pfnav_repair_chain_launch(ctx, st, items, masks, d_cnt + 2))) return rc;
+                if ((rc = pfnav_repair_chain_launch(ctx, st, items, masks, ctx->pool.d_flow, 0, d_cnt + 2))) return rc;
                 if (!items.empty()) nrounds++;
                 items.clear(); masks.clear();
                 uint8_t d = 0;
@@ -2834,11 +2830,10 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
                 if (it.always || (d & 0xF) == 0) { rc = src; break; }
                 continue;
             }
-            if (it.kind == 1) { it.mask = (int32_t)(masks.size() / 64); masks.insert(masks.end(), mask.begin(), mask.end()); }
             items.push_back(it);
         }
         if (!items.empty()) {
-            const int rc2 = pfnav_repair_chain_launch(ctx, st, items, masks, d_cnt + 2);
+            const int rc2 = pfnav_repair_chain_launch(ctx, st, items, masks, ctx->pool.d_flow, 0, d_cnt + 2);
             if (!rc) rc = rc2;
             nrounds++;
         }

@@ -481,16 +481,78 @@ k_flow_unit(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__
 }
 
 // ------------------------------------------------------------------------------------------
-// K1g: flow field, general u8 costs. One CTA (128 threads) per field.
+// The integration and direction pass of the CTA-per-field kernels (k_flow_general, k_repair_chain), 128 threads.
+// Every thread calls it once dist / cost / dom hold the field's start state: dom 0 = outside the integration, 1 = relaxed
+// (edge weight = cost of the tile entered, field_build_integration, field.c:556-563), 2 = seed (dist 0). The relaxation
+// runs to the unique shortest-distance fixpoint, so the order tiles are visited in cannot change a result. The
+// directions then go to dst (4096 bytes) by the 8-neighbour rule; both exceptions key on the distance value, since a
+// zero-cost tile (the transient 0 of nav.c:359) next to a seed reaches 0 without being one:
+//   unreached tiles get 0 when zero_unreached and keep their byte otherwise;
+//   tiles at distance 0 get the portal fix-up (field_fixup_portal_edges, field.c:830) or 0 when set_dist0, and keep
+//   their byte otherwise.
+// Returns after a barrier: the caller may reuse the arrays and read dst.
 // ------------------------------------------------------------------------------------------
 #define FLOWG_THREADS 128
+__device__ __forceinline__ void flow_integrate(uint32_t *dist, const uint8_t *cost, const uint8_t *dom, int &changed,
+                                               const pfnav_field_req &q, bool zero_unreached, bool set_dist0,
+                                               uint8_t *__restrict__ dst)
+{
+    const int tid = threadIdx.x;
+    do {
+        __syncthreads();
+        if (tid == 0) changed = 0;
+        __syncthreads();
+        bool ch = false;
+        for (int t = tid; t < 4096; t += FLOWG_THREADS) {
+            if (dom[t] != 1) continue;
+            const int r = t >> 6, cc = t & 63;
+            uint32_t m = 0xFFFFFFFFu;
+            if (r > 0)   m = min(m, dist[t - 64]);
+            if (r < 63)  m = min(m, dist[t + 64]);
+            if (cc > 0)  m = min(m, dist[t - 1]);
+            if (cc < 63) m = min(m, dist[t + 1]);
+            if (m != 0xFFFFFFFFu && m + cost[t] < dist[t]) { dist[t] = m + cost[t]; ch = true; }
+        }
+        if (ch) changed = 1;
+        __syncthreads();
+    } while (changed);
+
+    const bool up = q.next_chunk_r < q.chunk_r, down = q.next_chunk_r > q.chunk_r;
+    const bool left = q.next_chunk_c < q.chunk_c;
+    const uint8_t fix = up ? 2 : down ? 7 : left ? 4 : 5;
+    for (int t = tid; t < 4096; t += FLOWG_THREADS) {
+        const uint32_t d = dist[t];
+        if (d == 0xFFFFFFFFu) { if (zero_unreached) dst[t] = 0; continue; }
+        if (d == 0) { if (set_dist0) dst[t] = (q.target_type == PFNAV_TARGET_PORTAL) ? fix : 0; continue; }
+        const int r = t >> 6, c = t & 63;
+        const uint32_t INF = 0xFFFFFFFFu;
+        const uint32_t dn = r > 0 ? dist[t - 64] : INF, ds = r < 63 ? dist[t + 64] : INF;
+        const uint32_t dw = c > 0 ? dist[t - 1] : INF, de = c < 63 ? dist[t + 1] : INF;
+        const uint32_t dnw = (r > 0 && c > 0) ? dist[t - 65] : INF, dne = (r > 0 && c < 63) ? dist[t - 63] : INF;
+        const uint32_t dsw = (r < 63 && c > 0) ? dist[t + 63] : INF, dse = (r < 63 && c < 63) ? dist[t + 65] : INF;
+        uint32_t m = min(min(dn, ds), min(dw, de));
+        if (dn != INF && dw != INF) m = min(m, dnw);
+        if (dn != INF && de != INF) m = min(m, dne);
+        if (ds != INF && dw != INF) m = min(m, dsw);
+        if (ds != INF && de != INF) m = min(m, dse);
+        uint8_t dir;   // field.c:405-428 priority N,S,E,W,NW,NE,SW,SE
+        if (dn == m) dir = 2; else if (ds == m) dir = 7; else if (de == m) dir = 5; else if (dw == m) dir = 4;
+        else if (dnw == m) dir = 1; else if (dne == m) dir = 3; else if (dsw == m) dir = 6; else dir = 8;
+        dst[t] = dir;
+    }
+    __syncthreads();
+}
+
+// ------------------------------------------------------------------------------------------
+// K1g: flow field, general u8 costs. One CTA (128 threads) per field.
+// ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(FLOWG_THREADS)
 k_flow_general(FlowGrids g, const pfnav_field_req *__restrict__ reqs, int n, uint8_t *__restrict__ fields,
                const int32_t *__restrict__ out_slot, int only_nonunit)
 {
     __shared__ uint32_t dist[4096];
     __shared__ uint8_t cost[4096];       // 0xFF = impassable or blocked
-    __shared__ uint8_t seed[4096];
+    __shared__ uint8_t dom[4096];        // flow_integrate's domain: 0 = impassable, 1 = passable, 2 = seed
     __shared__ int changed;
     const int tid = threadIdx.x;
     for (int i = blockIdx.x; i < n; i += gridDim.x) {
@@ -505,13 +567,13 @@ k_flow_general(FlowGrids g, const pfnav_field_req *__restrict__ reqs, int n, uin
             if (blocked_for(g, q.faction_id, off)) c = 0xFF;
             cost[t] = c;
             dist[t] = 0xFFFFFFFFu;
-            seed[t] = 0;
+            dom[t] = c != 0xFF;
         }
         __syncthreads();
         if (q.target_type == PFNAV_TARGET_TILE) {
             if (tid == 0) {
                 int t = q.tile_r * 64 + q.tile_c;
-                if (cost[t] != 0xFF) { seed[t] = 1; dist[t] = 0; }
+                if (cost[t] != 0xFF) { dom[t] = 2; dist[t] = 0; }
             }
         } else {
             const int nc = q.port_c1 - q.port_c0 + 1, ntiles = (q.port_r1 - q.port_r0 + 1) * nc;
@@ -532,148 +594,25 @@ k_flow_general(FlowGrids g, const pfnav_field_req *__restrict__ reqs, int n, uin
                     if (tr < q.next_r0 || tr > q.next_r1 || tc < q.next_c0 || tc > q.next_c1) continue;
                     if (g.liid[lbase + (size_t)ngr * g.W64 + ngc] == q.next_iid) adj = true;
                 }
-                if (adj) { seed[r * 64 + c] = 1; dist[r * 64 + c] = 0; }
+                if (adj) { dom[r * 64 + c] = 2; dist[r * 64 + c] = 0; }
             }
         }
-        __syncthreads();
-        // Bellman-Ford to the unique shortest-distance fixpoint; edge weight = cost of the tile
-        // entered (field_build_integration, field.c:556-563).
-        do {
-            __syncthreads();
-            if (tid == 0) changed = 0;
-            __syncthreads();
-            bool ch = false;
-            for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-                const uint8_t c = cost[t];
-                if (c == 0xFF || seed[t]) continue;
-                const int r = t >> 6, cc = t & 63;
-                uint32_t m = 0xFFFFFFFFu;
-                if (r > 0)   m = min(m, dist[t - 64]);
-                if (r < 63)  m = min(m, dist[t + 64]);
-                if (cc > 0)  m = min(m, dist[t - 1]);
-                if (cc < 63) m = min(m, dist[t + 1]);
-                if (m != 0xFFFFFFFFu && m + c < dist[t]) { dist[t] = m + c; ch = true; }
-            }
-            if (ch) changed = 1;
-            __syncthreads();
-        } while (changed);
-
-        const bool up = q.next_chunk_r < q.chunk_r, down = q.next_chunk_r > q.chunk_r;
-        const bool left = q.next_chunk_c < q.chunk_c;
-        const uint8_t fix = up ? 2 : down ? 7 : left ? 4 : 5;
-        uint8_t *dst = fields + (size_t)(out_slot ? out_slot[i] : i) * 4096;
-        for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-            const uint32_t d = dist[t];
-            if (d == 0xFFFFFFFFu) { if (q.init) dst[t] = 0; continue; }
-            if (d == 0) { dst[t] = (q.target_type == PFNAV_TARGET_PORTAL) ? fix : 0; continue; }
-            const int r = t >> 6, c = t & 63;
-            const uint32_t INF = 0xFFFFFFFFu;
-            const uint32_t dn = r > 0 ? dist[t - 64] : INF, ds = r < 63 ? dist[t + 64] : INF;
-            const uint32_t dw = c > 0 ? dist[t - 1] : INF, de = c < 63 ? dist[t + 1] : INF;
-            const uint32_t dnw = (r > 0 && c > 0) ? dist[t - 65] : INF, dne = (r > 0 && c < 63) ? dist[t - 63] : INF;
-            const uint32_t dsw = (r < 63 && c > 0) ? dist[t + 63] : INF, dse = (r < 63 && c < 63) ? dist[t + 65] : INF;
-            uint32_t m = min(min(dn, ds), min(dw, de));
-            if (dn != INF && dw != INF) m = min(m, dnw);
-            if (dn != INF && de != INF) m = min(m, dne);
-            if (ds != INF && dw != INF) m = min(m, dsw);
-            if (ds != INF && de != INF) m = min(m, dse);
-            uint8_t dir;   // field.c:405-428 priority N,S,E,W,NW,NE,SW,SE
-            if (dn == m) dir = 2; else if (ds == m) dir = 7; else if (de == m) dir = 5; else if (dw == m) dir = 4;
-            else if (dnw == m) dir = 1; else if (dne == m) dir = 3; else if (dsw == m) dir = 6; else dir = 8;
-            dst[t] = dir;
-        }
-        __syncthreads();
+        flow_integrate(dist, cost, dom, changed, q, q.init != 0, true, fields + (size_t)(out_slot ? out_slot[i] : i) * 4096);
     }
 }
 
 // ------------------------------------------------------------------------------------------
-// K1r: repair chain of N_DesiredPointSeekVelocity (nav.c:3508-3554) on one cached field, in place.
-// One CTA per field, Bellman-Ford to the unique fixpoint like k_flow_general; the seeds come from the host
-// (pfnav_repair_seeds). kind 0 = N_FlowFieldUpdateToNearestPathable (field.c:2247): the integration runs
-// over NON-passable tiles only (field_build_integration_nonpass, field.c:643; edge weight = raw cost_base
-// of the tile entered) and only tiles with 0 < cost < INF get a direction. kind 1 =
-// N_FlowFieldUpdateIslandToNearest (field.c:2307): ordinary integration / flow / portal fixup from the
-// substitute frontier.
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(FLOWG_THREADS)
-k_flow_repair(FlowGrids g, const pfnav_field_req *__restrict__ reqs, const int32_t *__restrict__ kinds,
-              const uint64_t *__restrict__ seed_masks, int n, uint8_t *__restrict__ fields,
-              const int32_t *__restrict__ out_slot)
-{
-    __shared__ uint32_t dist[4096];
-    __shared__ uint8_t cost[4096];       // raw cost_base
-    __shared__ uint8_t dom[4096];        // 1 = tile takes part in the integration
-    __shared__ int changed;
-    const int tid = threadIdx.x;
-    for (int i = blockIdx.x; i < n; i += gridDim.x) {
-        const pfnav_field_req q = reqs[i];
-        const int kind = kinds[i];
-        const size_t lbase = (size_t)q.layer * g.H64 * g.W64;
-        for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-            const size_t off = lbase + (size_t)(q.chunk_r * 64 + (t >> 6)) * g.W64 + q.chunk_c * 64 + (t & 63);
-            const uint8_t c = g.cost[off];
-            const bool pass = c != 0xFF && !blocked_for(g, q.faction_id, off);
-            const bool seed = (seed_masks[(size_t)i * 64 + (t >> 6)] >> (t & 63)) & 1;
-            cost[t] = c;
-            dom[t] = seed ? 2 : (kind == 0 ? !pass : pass) ? 1 : 0;      // 2 = seed (distance pinned at 0)
-            dist[t] = seed ? 0u : 0xFFFFFFFFu;
-        }
-        do {
-            __syncthreads();
-            if (tid == 0) changed = 0;
-            __syncthreads();
-            bool ch = false;
-            for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-                if (dom[t] != 1) continue;
-                const int r = t >> 6, cc = t & 63;
-                uint32_t m = 0xFFFFFFFFu;
-                if (r > 0)   m = min(m, dist[t - 64]);
-                if (r < 63)  m = min(m, dist[t + 64]);
-                if (cc > 0)  m = min(m, dist[t - 1]);
-                if (cc < 63) m = min(m, dist[t + 1]);
-                if (m != 0xFFFFFFFFu && m + cost[t] < dist[t]) { dist[t] = m + cost[t]; ch = true; }
-            }
-            if (ch) changed = 1;
-            __syncthreads();
-        } while (changed);
-
-        const bool up = q.next_chunk_r < q.chunk_r, down = q.next_chunk_r > q.chunk_r;
-        const bool left = q.next_chunk_c < q.chunk_c;
-        const uint8_t fix = up ? 2 : down ? 7 : left ? 4 : 5;
-        uint8_t *dst = fields + (size_t)(out_slot ? out_slot[i] : i) * 4096;
-        for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-            const uint32_t d = dist[t];
-            if (d == 0xFFFFFFFFu) continue;
-            if (d == 0) {
-                if (kind == 1) dst[t] = (q.target_type == PFNAV_TARGET_PORTAL) ? fix : 0;
-                continue;
-            }
-            const int r = t >> 6, c = t & 63;
-            const uint32_t INF = 0xFFFFFFFFu;
-            const uint32_t dn = r > 0 ? dist[t - 64] : INF, ds = r < 63 ? dist[t + 64] : INF;
-            const uint32_t dw = c > 0 ? dist[t - 1] : INF, de = c < 63 ? dist[t + 1] : INF;
-            const uint32_t dnw = (r > 0 && c > 0) ? dist[t - 65] : INF, dne = (r > 0 && c < 63) ? dist[t - 63] : INF;
-            const uint32_t dsw = (r < 63 && c > 0) ? dist[t + 63] : INF, dse = (r < 63 && c < 63) ? dist[t + 65] : INF;
-            uint32_t m = min(min(dn, ds), min(dw, de));
-            if (dn != INF && dw != INF) m = min(m, dnw);
-            if (dn != INF && de != INF) m = min(m, dne);
-            if (ds != INF && dw != INF) m = min(m, dsw);
-            if (ds != INF && de != INF) m = min(m, dse);
-            uint8_t dir;   // field.c:405-428 priority N,S,E,W,NW,NE,SW,SE
-            if (dn == m) dir = 2; else if (ds == m) dir = 7; else if (de == m) dir = 5; else if (dw == m) dir = 4;
-            else if (dnw == m) dir = 1; else if (dne == m) dir = 3; else if (dsw == m) dir = 6; else dir = 8;
-            dst[t] = dir;
-        }
-        __syncthreads();
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// K1c: one round of the on-miss chain of pfnav_pool_repair_batch. One CTA per pool slot that has items in the round;
-// it walks the slot's items in the serial loop's order and applies an item only if the tile it names still has no
-// direction when the item's turn comes (or always, for the surround variant on a blocked tile): the serial loop's
-// read-back before the repair, answered where the byte lives. The integration is k_flow_repair's, restated so that
-// kernel stays as it is; kind-0 seeds are flooded in the CTA (pfnav_repair_kernel.cuh), kind-1 seeds come from the host.
+// K1c: the repair chain of N_DesiredPointSeekVelocity (nav.c:3508-3554) on cached fields, in place. One CTA per field
+// slot that has items in the launch; it walks the slot's items in order and applies an item only if the tile it names
+// still has no direction when the item's turn comes, or always when the item says so (pfnav_flow_fields_repair, the
+// serial pfnav_pool_repair, the surround variant on a blocked tile): the serial loop's read-back before the repair,
+// answered where the byte lives.
+//   kind 0 = N_FlowFieldUpdateToNearestPathable (field.c:2247): seeds flooded in the CTA (pfnav_repair_kernel.cuh); the
+//            integration runs over NON-passable tiles only (field_build_integration_nonpass, field.c:643; edge weight =
+//            raw cost_base of the tile entered) and distance-0 tiles keep their byte.
+//   kind 1 = N_FlowFieldUpdateIslandToNearest (field.c:2307): seeds from the host; ordinary integration / flow / portal
+//            fix-up from the substitute frontier.
+// count: the repairs applied are added to it when given.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(FLOWG_THREADS)
 k_repair_chain(FlowGrids g, const pf_chain_item *__restrict__ items, const int32_t *__restrict__ group_off, int ngroups,
@@ -711,53 +650,8 @@ k_repair_chain(FlowGrids g, const pf_chain_item *__restrict__ items, const int32
                 dom[t] = sd ? 2 : (kind == 0 ? !pass : pass) ? 1 : 0;
                 dist[t] = sd ? 0u : 0xFFFFFFFFu;
             }
-            do {
-                __syncthreads();
-                if (tid == 0) changed = 0;
-                __syncthreads();
-                bool ch = false;
-                for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-                    if (dom[t] != 1) continue;
-                    const int r = t >> 6, cc = t & 63;
-                    uint32_t m = 0xFFFFFFFFu;
-                    if (r > 0)   m = min(m, dist[t - 64]);
-                    if (r < 63)  m = min(m, dist[t + 64]);
-                    if (cc > 0)  m = min(m, dist[t - 1]);
-                    if (cc < 63) m = min(m, dist[t + 1]);
-                    if (m != 0xFFFFFFFFu && m + cost[t] < dist[t]) { dist[t] = m + cost[t]; ch = true; }
-                }
-                if (ch) changed = 1;
-                __syncthreads();
-            } while (changed);
-
-            const bool up = q.next_chunk_r < q.chunk_r, down = q.next_chunk_r > q.chunk_r;
-            const bool left = q.next_chunk_c < q.chunk_c;
-            const uint8_t fix = up ? 2 : down ? 7 : left ? 4 : 5;
-            for (int t = tid; t < 4096; t += FLOWG_THREADS) {
-                const uint32_t d = dist[t];
-                if (d == 0xFFFFFFFFu) continue;
-                if (d == 0) {
-                    if (kind == 1) dst[t] = (q.target_type == PFNAV_TARGET_PORTAL) ? fix : 0;
-                    continue;
-                }
-                const int r = t >> 6, c = t & 63;
-                const uint32_t INF = 0xFFFFFFFFu;
-                const uint32_t dn = r > 0 ? dist[t - 64] : INF, ds = r < 63 ? dist[t + 64] : INF;
-                const uint32_t dw = c > 0 ? dist[t - 1] : INF, de = c < 63 ? dist[t + 1] : INF;
-                const uint32_t dnw = (r > 0 && c > 0) ? dist[t - 65] : INF, dne = (r > 0 && c < 63) ? dist[t - 63] : INF;
-                const uint32_t dsw = (r < 63 && c > 0) ? dist[t + 63] : INF, dse = (r < 63 && c < 63) ? dist[t + 65] : INF;
-                uint32_t m = min(min(dn, ds), min(dw, de));
-                if (dn != INF && dw != INF) m = min(m, dnw);
-                if (dn != INF && de != INF) m = min(m, dne);
-                if (ds != INF && dw != INF) m = min(m, dsw);
-                if (ds != INF && de != INF) m = min(m, dse);
-                uint8_t dir;   // field.c:405-428 priority N,S,E,W,NW,NE,SW,SE
-                if (dn == m) dir = 2; else if (ds == m) dir = 7; else if (de == m) dir = 5; else if (dw == m) dir = 4;
-                else if (dnw == m) dir = 1; else if (dne == m) dir = 3; else if (dsw == m) dir = 6; else dir = 8;
-                dst[t] = dir;
-            }
-            if (tid == 0) atomicAdd(count, 1u);
-            __syncthreads();      // the next item of this slot reads the bytes written here
+            flow_integrate(dist, cost, dom, changed, q, false, kind == 1, dst);     // the next item reads the bytes after it
+            if (tid == 0 && count) atomicAdd(count, 1u);
         }
     }
 }
@@ -765,7 +659,7 @@ k_repair_chain(FlowGrids g, const pf_chain_item *__restrict__ items, const int32
 static FlowGrids grids_of(const pfnav_ctx *ctx);
 
 int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pf_chain_item> &items,
-                              const std::vector<uint64_t> &masks, uint32_t *d_count)
+                              const std::vector<uint64_t> &masks, uint8_t *fields, size_t host_fields, uint32_t *d_count)
 {
     if (items.empty()) return PFNAV_OK;
     // group by slot, serial order inside a group (a stable sort)
@@ -781,20 +675,24 @@ int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector
     off.push_back((int32_t)sorted.size());
     const int ngroups = (int)off.size() - 1;
     const size_t b_item = sorted.size() * sizeof(pf_chain_item), b_mask = masks.size() * 8, b_off = off.size() * 4;
-    const size_t a_mask = (b_item + 15) & ~(size_t)15, a_off = a_mask + b_mask, total = a_off + b_off;
+    const size_t b_f = host_fields * 4096;
+    const size_t a_mask = (b_item + 15) & ~(size_t)15, a_off = a_mask + b_mask, a_f = (a_off + b_off + 15) & ~(size_t)15;
+    const size_t total = a_f + b_f;
     pf_stage S;
     int rc = pf_stage_begin(ctx, st, total, total, false, &S);
     if (rc) return rc;
     memcpy(S.host, sorted.data(), b_item);
     if (b_mask) memcpy(S.host + a_mask, masks.data(), b_mask);
     memcpy(S.host + a_off, off.data(), b_off);
+    if (b_f) memcpy(S.host + a_f, fields, b_f);
     if ((rc = pf_stage_upload(ctx, st, S, total))) return rc;
-    const uint8_t *dev = S.dev;
+    uint8_t *dev = S.dev;
     k_repair_chain<<<(unsigned)std::min(ngroups, ctx->sm_count * 8), FLOWG_THREADS, 0, st>>>(
         grids_of(ctx), (const pf_chain_item *)dev, (const int32_t *)(dev + a_off), ngroups, (const uint64_t *)(dev + a_mask),
-        ctx->pool.d_flow, d_count);
+        b_f ? dev + a_f : fields, d_count);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
+    if (b_f) PF_CUDA(cudaMemcpyAsync(fields, dev + a_f, b_f, cudaMemcpyDeviceToHost, st));
     return pf_stage_done(ctx, st);
 }
 
@@ -1761,68 +1659,18 @@ extern "C" int pfnav_flow_fields_repair(pfnav_ctx *ctx, const pfnav_field_req *t
     PF_ARG(targets && kinds && args && inout_fields, "null buffer");
     int rc = validate_field_reqs(ctx, targets, n);
     if (rc) return rc;
-    std::vector<uint64_t> masks(n * 64);
+    std::vector<pf_chain_item> items(n);
+    std::vector<uint64_t> masks;
     for (size_t i = 0; i < n; i++) {
         PF_ARG(kinds[i] == PFNAV_REPAIR_NEAREST_PATHABLE || kinds[i] == PFNAV_REPAIR_ISLAND_TO_NEAREST, "repair kind");
-        if ((rc = pfnav_repair_seeds(ctx, targets[i], kinds[i], args[i], masks.data() + i * 64))) return rc;
+        pf_chain_item &it = items[i];
+        it.q = targets[i]; it.slot = (int32_t)i; it.tile = 0; it.kind = kinds[i]; it.arg = args[i]; it.always = 1;
+        if ((rc = pf_chain_item_seeds(ctx, it, masks))) return rc;
     }
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->tick_stream;
-    uint8_t *d_buf = nullptr;
-    const size_t b_req = n * sizeof(pfnav_field_req), b_kind = n * 4, b_mask = n * 512, b_f = n * 4096;
-    PF_CUDA(cudaMalloc(&d_buf, b_req + b_kind + b_mask + b_f));
-    uint8_t *d_req = d_buf, *d_mask = d_buf + b_req, *d_kind = d_mask + b_mask, *d_f = d_kind + b_kind;   // masks stay 8-byte aligned
-    cudaError_t e = cudaMemcpyAsync(d_req, targets, b_req, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_mask, masks.data(), b_mask, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_kind, kinds, b_kind, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_f, inout_fields, b_f, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        k_flow_repair<<<(unsigned)std::min<size_t>(n, (size_t)ctx->sm_count * 8), FLOWG_THREADS, 0, st>>>(
-            grids_of(ctx), (const pfnav_field_req *)d_req, (const int32_t *)d_kind, (const uint64_t *)d_mask, (int)n, d_f, nullptr);
-        ctx->launches++;
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(inout_fields, d_f, b_f, cudaMemcpyDeviceToHost, st);
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_buf);
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("pfnav_flow_fields_repair: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
-    return PFNAV_OK;
-}
-
-// Repairs applied straight to pool slots (pfnav_pool_repair). Host arrays in, blocking.
-int pfnav_flow_repair_pool(pfnav_ctx *ctx, const pfnav_field_req *targets, const int32_t *kinds, const int32_t *args,
-                           const int32_t *slots, size_t n)
-{
-    if (n == 0) return PFNAV_OK;
-    int rc;
-    std::vector<uint64_t> masks(n * 64);
-    for (size_t i = 0; i < n; i++)
-        if ((rc = pfnav_repair_seeds(ctx, targets[i], kinds[i], args[i], masks.data() + i * 64))) return rc;
-    cudaStream_t st = ctx->tick_stream;
-    uint8_t *d_buf = nullptr;
-    const size_t b_req = n * sizeof(pfnav_field_req), b_mask = n * 512, b_kind = n * 4, b_slot = n * 4;
-    PF_CUDA(cudaMalloc(&d_buf, b_req + b_mask + b_kind + b_slot));
-    uint8_t *d_req = d_buf, *d_mask = d_buf + b_req, *d_kind = d_mask + b_mask, *d_slot = d_kind + b_kind;
-    cudaError_t e = cudaMemcpyAsync(d_req, targets, b_req, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_mask, masks.data(), b_mask, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_kind, kinds, b_kind, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_slot, slots, b_slot, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        // one CTA per request, serialised per slot by launching requests that share a slot one after another
-        k_flow_repair<<<1, FLOWG_THREADS, 0, st>>>(grids_of(ctx), (const pfnav_field_req *)d_req, (const int32_t *)d_kind,
-                                                  (const uint64_t *)d_mask, (int)n, ctx->pool.d_flow, (const int32_t *)d_slot);
-        ctx->launches++;
-        e = cudaGetLastError();
-    }
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_buf);
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("pfnav_flow_repair_pool: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
+    if ((rc = pfnav_repair_chain_launch(ctx, st, items, masks, inout_fields, n, nullptr))) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 

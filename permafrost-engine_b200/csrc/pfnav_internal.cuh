@@ -244,25 +244,22 @@ int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arriv
 // the layer's routing structure is not built (pfnav_route.cu)
 const uint16_t *pfnav_route_dev_islands(const pfnav_ctx *ctx, int layer);
 
-// seeds of the flow-field repair chain (pfnav_route.cu), 64 rows x 64 bits
-int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int arg, uint64_t *mask);
-
-int pfnav_flow_repair_pool(pfnav_ctx *ctx, const pfnav_field_req *targets, const int32_t *kinds, const int32_t *args,
-                           const int32_t *slots, size_t n);
-// the argument checks pfnav_repair_seeds makes of a kind-0 repair, without building its seeds (pfnav_route.cu)
-int pfnav_repair_start_check(pfnav_ctx *ctx, const pfnav_field_req &q, int arg);
-
-// One predicated repair of pfnav_pool_repair_batch (k_repair_chain, pfnav_fields.cu): applied to pool slot `slot` when its
-// turn comes if the direction of `tile` is FD_NONE then, or always (`always`: the surround variant on a blocked tile).
-// kind 0 builds its seeds on the device from start tile `arg`; kind 1 reads mask row block `mask` (64 x u64).
+// One repair of the flow-field repair chain (k_repair_chain, pfnav_fields.cu): applied to field `slot` when its turn
+// comes if the direction of `tile` is FD_NONE then, or always (`always`). kind 0 builds its seeds on the device from
+// start tile `arg`; kind 1 reads mask row block `mask` (64 x u64).
 struct pf_chain_item {
     pfnav_field_req q;
     int32_t slot, tile, kind, arg, always, mask;
 };
-// Launch one round of chain items on `st`: items grouped by slot (one CTA per group, items in order); the repairs
-// applied are added to *d_count. The item and mask arrays are copied on `st` before the call returns.
+// The seeds of item `it` (q, kind and arg set; pfnav_route.cu): kind 0 checks its start tile, kind 1 appends its mask
+// (pfnav_repair_seeds) to `masks` and sets it.mask. Returns the error and changes nothing when the repair cannot run.
+int pf_chain_item_seeds(pfnav_ctx *ctx, pf_chain_item &it, std::vector<uint64_t> &masks);
+// Launch chain items on `st`: items grouped by slot (one CTA per group, items in order) into `fields`, 4096 bytes per
+// slot: the pool's d_flow, or, when host_fields > 0, that many host fields, staged with the items and copied back on
+// `st`. The repairs applied are added to *d_count when it is given. The item and mask arrays are copied on `st` before
+// the call returns.
 int pfnav_repair_chain_launch(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pf_chain_item> &items,
-                              const std::vector<uint64_t> &masks, uint32_t *d_count);
+                              const std::vector<uint64_t> &masks, uint8_t *fields, size_t host_fields, uint32_t *d_count);
 
 // Staged path requests against the pool (pfnav_route.cu), shared by pfnav_pool_request_paths and pfnav_pool_repair_batch:
 // begin plans requests i = 0 .. n-1 (each on its own layer) up front; probe emits request i against the pool mirrors as

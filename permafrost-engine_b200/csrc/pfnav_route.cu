@@ -1232,15 +1232,16 @@ int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arriv
 // ------------------------------------------------------------------------------------------
 // Seeds of the repair chain of N_DesiredPointSeekVelocity (nav.c:3508-3554), host side (they need the
 // global islands and breadth-first ring searches over the chunk; the integration itself runs on the
-// device, k_flow_repair):
+// device, k_repair_chain):
 //   kind 0  N_FlowFieldUpdateToNearestPathable (field.c:2247): the passable tiles that border the
 //           non-passable blob containing (start_r, start_c)   (field_passable_frontier, field.c:1441)
 //   kind 1  N_FlowFieldUpdateIslandToNearest (field.c:2307): the tiles of local island `local_iid`
 //           nearest (Manhattan) to the field's own frontier     (field_closest_tiles_local, field.c:1010)
-// mask: 64 rows of 64 bits.
+// mask: 64 rows of 64 bits. The chain builds kind-0 seeds itself (pfnav_repair_kernel.cuh); the host search of kind 0
+// is the reference pfnav_repair_seed_mask exposes.
 // ------------------------------------------------------------------------------------------
-// The argument checks of a kind-0 repair (its seeds are built on the device by pfnav_repair_batch).
-int pfnav_repair_start_check(pfnav_ctx *ctx, const pfnav_field_req &q, int arg)
+// The argument checks of a kind-0 repair.
+static int pfnav_repair_start_check(pfnav_ctx *ctx, const pfnav_field_req &q, int arg)
 {
     const int chunk = q.chunk_r * ctx->chunk_w + q.chunk_c;
     const uint8_t *cost = L_cost(ctx, q.layer, chunk);
@@ -1252,7 +1253,7 @@ int pfnav_repair_start_check(pfnav_ctx *ctx, const pfnav_field_req &q, int arg)
     return PFNAV_OK;
 }
 
-int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int arg, uint64_t *mask)
+static int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int arg, uint64_t *mask)
 {
     memset(mask, 0, 64 * sizeof(uint64_t));
     const int layer = q.layer, cw = ctx->chunk_w;
@@ -1354,6 +1355,20 @@ int pfnav_repair_seeds(pfnav_ctx *ctx, const pfnav_field_req &q, int kind, int a
         newf.insert(newf.end(), tmp.begin(), tmp.end());
     }
     for (int t : newf) mask[t >> 6] |= 1ull << (t & 63);
+    return PFNAV_OK;
+}
+
+int pf_chain_item_seeds(pfnav_ctx *ctx, pf_chain_item &it, std::vector<uint64_t> &masks)
+{
+    if (it.kind == 0) {
+        if (int rc = pfnav_repair_start_check(ctx, it.q, it.arg)) return rc;
+        it.mask = -1;
+        return PFNAV_OK;
+    }
+    uint64_t mask[64];
+    if (int rc = pfnav_repair_seeds(ctx, it.q, it.kind, it.arg, mask)) return rc;
+    it.mask = (int32_t)(masks.size() / 64);
+    masks.insert(masks.end(), mask, mask + 64);
     return PFNAV_OK;
 }
 

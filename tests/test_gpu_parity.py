@@ -563,6 +563,56 @@ def test_repair_chain_golden(nav, pforacle):
     assert len(bad) == 0, (bad[:10], g["kinds"][bad[:10]])
 
 
+@pytest.mark.parametrize("seed", [41, 42])
+def test_repair_chain_vs_port(nav, pforacle, seed):
+    """pfnav_flow_fields_repair against the plain-C port (field.c:2247, 2307) on maps whose blockers were committed
+    through the device: both kinds, tile targets (passable and blocked) and portal targets, every chunk, many start
+    tiles and islands. Blocker operations queued after the commit do not reach the repair: kind-0 seeds are flooded
+    on the device images, the start check and kind-1 seeds come from the host mirrors, and both are the committed map."""
+    cw, ch = 3, 2
+    rng = np.random.default_rng(seed)
+    cost = synth.cost_from_pathable(cases.noise_map(cw, ch, seed, 0.2), cw, ch)
+    nav.map_create(cw, ch, 1)
+    nav.map_upload_layer(0, cost)
+    nav.map_build_nav(0)
+
+    def place_blockers(n):
+        for _ in range(n):
+            nav.blockers_incref(float(-rng.uniform(10, cw * 256 - 10)), float(rng.uniform(10, ch * 256 - 10)),
+                                float(rng.uniform(2, 16)), 0, 0)
+
+    place_blockers(70)
+    assert nav.map_commit() > 0
+    nav.route_build(0)
+    blk, liid, gisl = nav.blockers(0), nav.local_islands(0), nav.route_islands(0)
+    om = pforacle.OracleMap(cw, ch, cost, blk, liid)
+    specs = cases.portal_specs(nav.portals(0), liid, cw)
+    T, K, A, B, E = [], [], [], [], []
+    for chunk in range(cw * ch):
+        cr, cc = divmod(chunk, cw)
+        free = np.argwhere((cost[chunk] != 255) & (blk[chunk] == 0))
+        blocked = np.argwhere((cost[chunk] != 255) & (blk[chunk] > 0))
+        nonp = np.argwhere((cost[chunk] == 255) | (blk[chunk] > 0))
+        reqs = [capi.tile_req((cr, cc), tuple(int(v) for v in t[rng.integers(len(t))])) for t in (free, blocked) if len(t)]
+        reqs += [cases.portal_reqs([s]) for s in specs if s[0] == (cr, cc)][:3]
+        iids = [int(i) for i in np.unique(liid[chunk]) if i != 0xFFFF]
+        for q in reqs:
+            base = om.flow_fields_update(q)[0]
+            for s in nonp[rng.integers(0, len(nonp), 8)] if len(nonp) else []:
+                T.append(q); K.append(0); A.append((int(s[0]) << 8) | int(s[1])); B.append(base)
+                E.append(om.flow_nearest_pathable((cr, cc), (int(s[0]), int(s[1])), base))
+            for iid in iids[:8]:
+                T.append(q); K.append(1); A.append(iid); B.append(base)
+                E.append(om.flow_island_to_nearest(gisl, q, iid, base))
+    T, K, A, B, E = np.concatenate(T), np.array(K, np.int32), np.array(A, np.int32), np.stack(B), np.stack(E)
+    assert (T["target_type"] == capi.TARGET_PORTAL).any() and (K == 0).any() and (K == 1).any()
+    assert (B != E).any()
+    place_blockers(30)                                   # queued, not committed
+    got = nav.flow_fields_repair(T, K, A, B)
+    bad = np.nonzero((got != E).reshape(len(T), -1).any(axis=1))[0]
+    assert len(bad) == 0, (len(bad), len(T), bad[:10], K[bad[:10]])
+
+
 def test_pool_repair_chain_golden(nav):
     """a-4 end to end: N_DesiredPointSeekVelocity's on-miss chain (nav.c:3484-3554) against the device pool.
     Entities on blocked tiles, inside walls, on islands cut off by blockers and in chunks the first request never
