@@ -360,7 +360,7 @@ int  pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nrepairs);
  * launch. A round ends only where a request's emission depends on a byte written earlier in the round, would write a
  * slot with a pending repair, or would evict. *out_nrounds: the rounds that launched work. Pointers may be NULL.
  * Ordered on `stream` (NULL: the context's stream) after forked field work and pfnav_pool_clear; it waits for the device
- * only to read back each phase's representatives and the bytes they stand on, at round boundaries (the round's request
+ * only when its scratch has to grow and to read back each phase's representatives and the bytes they stand on, at round boundaries (the round's request
  * upload and its gather) and once at the end, never per entity. Errors as
  * pfnav_pool_repair's: PFNAV_ERR_ARG (no agents / pool, pfnav_route_build missing where a request needs it),
  * PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_NOMEM at representative k leaves 0 .. k-1 done as the serial

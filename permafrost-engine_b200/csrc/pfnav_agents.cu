@@ -939,43 +939,24 @@ int pfnav_agents_init(pfnav_ctx *ctx)
 
 void pfnav_agents_free(pfnav_ctx *ctx)
 {
-    cudaFree(ctx->d_agents); cudaFree(ctx->d_records); cudaFree(ctx->d_flocks);
-    cudaFree(ctx->d_flock_start); cudaFree(ctx->d_flock_members); cudaFree(ctx->d_cohesion);
-    cudaFree(ctx->d_cell_count); cudaFree(ctx->d_cell_start); cudaFree(ctx->d_cell_fill);
-    cudaFree(ctx->d_sorted_ix); cudaFree(ctx->d_sorted_iy); cudaFree(ctx->d_sorted_id); cudaFree(ctx->d_sorted_flock);
-    cudaFree(ctx->d_coh_fallback); ctx->d_sorted_flock = nullptr; ctx->d_coh_fallback = nullptr; ctx->cap_coh = 0;
-    cudaFree(ctx->d_coh_part); ctx->d_coh_part = nullptr; ctx->cap_coh_part = 0;
-    cudaFree(ctx->d_cp_stats); ctx->d_cp_stats = nullptr;
-    cudaFree(ctx->d_scan_part); ctx->d_scan_part = nullptr;
-    cudaFree(ctx->d_work); cudaFree(ctx->d_vel_out); cudaFree(ctx->d_vpref_out); cudaFree(ctx->d_vdes_out);
-    cudaFree(ctx->d_movestate); cudaFree(ctx->d_patches); cudaFree(ctx->d_arrival); cudaFree(ctx->d_nb_scratch);
-    cudaFree(ctx->d_member_pos); cudaFree(ctx->d_prep); cudaFree(ctx->d_flock_of); cudaFree(ctx->d_facts);
-    cudaFree(ctx->d_formation); cudaFree(ctx->d_ms_ext); cudaFree(ctx->d_enter); cudaFree(ctx->d_ttiles);
-    ctx->d_flock_of = nullptr; ctx->d_facts = nullptr; ctx->d_formation = nullptr; ctx->d_ms_ext = nullptr;
-    ctx->d_enter = nullptr; ctx->d_ttiles = nullptr; ctx->cap_formation = ctx->cap_ms_ext = ctx->cap_enter = ctx->cap_ttiles = 0;
     if (ctx->update_done) cudaEventDestroy(ctx->update_done);
-    cudaFree(ctx->d_los_out); cudaFree(ctx->d_work_count); cudaFree(ctx->d_scan_tmp);
-    cudaFree(ctx->d_rep_buf); ctx->d_rep_buf = nullptr; ctx->rep_buf_bytes = 0;
-    cudaFree(ctx->d_blocking); ctx->d_blocking = nullptr; ctx->blocking_n = 0;
-    cudaFree(ctx->d_block_uids); ctx->d_block_uids = nullptr; ctx->cap_block_uids = 0;
-    cudaFree(ctx->d_cmd_buf); ctx->d_cmd_buf = nullptr; ctx->cmd_buf_bytes = 0;
-    ctx->d_agents = nullptr; ctx->d_records = nullptr; ctx->d_flocks = nullptr; ctx->d_flock_start = nullptr;
-    ctx->d_flock_members = nullptr; ctx->d_cohesion = nullptr; ctx->d_cell_count = nullptr; ctx->d_cell_start = nullptr;
-    ctx->d_cell_fill = nullptr; ctx->d_sorted_ix = nullptr; ctx->d_sorted_iy = nullptr; ctx->d_sorted_id = nullptr;
-    ctx->d_work = nullptr; ctx->d_vel_out = nullptr; ctx->d_vpref_out = nullptr; ctx->d_vdes_out = nullptr;
-    ctx->d_los_out = nullptr; ctx->d_work_count = nullptr; ctx->d_scan_tmp = nullptr;
-    ctx->cap_agents = ctx->cap_flocks = ctx->cap_cells = ctx->cap_work = 0;
 }
 
 // ---- agents ----
-template <typename T>
-static int ensure(T *&p, size_t &cap, size_t need)
+int pf_flocks_reserve(pfnav_ctx *ctx, size_t nflocks)
 {
-    if (cap >= need && p) return 0;
-    cudaFree(p);
-    p = nullptr;
-    PF_CUDA(cudaMalloc(&p, std::max<size_t>(need, 1) * sizeof(T)));
-    return 0;
+    int rc = ctx->d_flocks.reserve(nflocks + 1);
+    if (!rc) rc = ctx->d_flock_start.reserve(nflocks + 2);
+    if (rc) { ctx->d_flocks.release(); ctx->d_flock_start.release(); }
+    return rc;
+}
+
+int pf_work_reserve(pfnav_ctx *ctx, size_t nwork)
+{
+    int rc = pf_dbuf_reserve_all(nwork, ctx->d_work, ctx->d_vel_out, ctx->d_vpref_out, ctx->d_vdes_out, ctx->d_los_out);
+    if (!rc) rc = ctx->d_work_count.reserve(4);
+    if (rc) ctx->n_work = 0;
+    return rc;
 }
 
 static GridView grid_of(const pfnav_ctx *ctx)
@@ -999,10 +980,10 @@ static int build_index(pfnav_ctx *ctx, cudaStream_t st)
         k_cell_count<<<(n + 255) / 256, 256, 0, st>>>(ctx->d_records, n, g, ctx->d_cell_count);
         const int nsb = (ncells + 4095) / 4096;
         if (nsb > 1 && nsb <= 1024) {
-            if (!ctx->d_scan_part) PF_CUDA(cudaMalloc(&ctx->d_scan_part, 1024 * sizeof(uint32_t)));
-            k_cell_scan_sum<<<nsb, 1024, 0, st>>>(ctx->d_cell_count, (uint32_t *)ctx->d_scan_part, ncells);
-            k_cell_scan_parts<<<1, 1024, 0, st>>>((uint32_t *)ctx->d_scan_part, nsb, ctx->d_cell_start, ncells);
-            k_cell_scan_apply<<<nsb, 1024, 0, st>>>(ctx->d_cell_count, (const uint32_t *)ctx->d_scan_part, ctx->d_cell_start, ncells);
+            if (int rc = ctx->d_scan_part.reserve(1024)) return rc;
+            k_cell_scan_sum<<<nsb, 1024, 0, st>>>(ctx->d_cell_count, ctx->d_scan_part, ncells);
+            k_cell_scan_parts<<<1, 1024, 0, st>>>(ctx->d_scan_part, nsb, ctx->d_cell_start, ncells);
+            k_cell_scan_apply<<<nsb, 1024, 0, st>>>(ctx->d_cell_count, ctx->d_scan_part, ctx->d_cell_start, ncells);
             ctx->launches += 2;
         } else
             k_cell_scan<<<1, 1024, 0, st>>>(ctx->d_cell_count, ctx->d_cell_start, ncells);
@@ -1095,26 +1076,11 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
     const bool same = (flags & PFNAV_UPLOAD_SAME_FLOCKS) && ctx->n_agents == n && ctx->n_flocks == nflocks &&
                       ctx->shard_lo == lo && ctx->shard_hi == hi && ctx->hz == hz;
     ctx->hz = hz;
-    int rc;
-    if (n > ctx->cap_agents) {
-        size_t cap = 0;
-        if ((rc = ensure(ctx->d_agents, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_records, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_flock_members, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_flock_of, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_sorted_ix, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_sorted_iy, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_sorted_flock, cap, n))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_sorted_id, cap, n))) return rc;
-        ctx->cap_agents = n;
-    }
-    if (nflocks + 1 > ctx->cap_flocks) {
-        size_t cap = 0;
-        if ((rc = ensure(ctx->d_flocks, cap, nflocks + 1))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_flock_start, cap, nflocks + 2))) return rc;
-        ctx->cap_flocks = nflocks + 1;
-    }
-    if (!ctx->d_facts) PF_CUDA(cudaMalloc(&ctx->d_facts, 8));
+    int rc = pf_dbuf_reserve_all(n, ctx->d_agents, ctx->d_records, ctx->d_flock_members, ctx->d_flock_of, ctx->d_sorted_ix,
+                                 ctx->d_sorted_iy, ctx->d_sorted_flock, ctx->d_sorted_id);
+    if (!rc) rc = pf_flocks_reserve(ctx, nflocks);
+    if (!rc) rc = ctx->d_facts.reserve(2);
+    if (rc) return rc;
     ctx->n_agents = n; ctx->n_flocks = nflocks; ctx->shard_lo = lo; ctx->shard_hi = hi;
     if (!same) {
         // what the host needs to know about the entities it will run work items for (its own range)
@@ -1138,8 +1104,8 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
         ctx->h_flocks.assign(flocks, flocks + nflocks);
         ctx->arrival_valid = false;
         // optional per-entity inputs of the previous population do not carry over
-        cudaFree(ctx->d_formation); ctx->d_formation = nullptr; ctx->cap_formation = 0;
-        cudaFree(ctx->d_ms_ext); ctx->d_ms_ext = nullptr; ctx->cap_ms_ext = 0;
+        ctx->d_formation.release();
+        ctx->d_ms_ext.release();
     }
     if (hi > lo) PF_CUDA(cudaMemcpyAsync(ctx->d_agents + lo, agents, (hi - lo) * sizeof(pfnav_agent), cudaMemcpyHostToDevice, st));
     if (nflocks && !same) PF_CUDA(cudaMemcpyAsync(ctx->d_flocks, flocks, nflocks * sizeof(pfnav_flock), cudaMemcpyHostToDevice, st));
@@ -1155,13 +1121,7 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
         ctx->grid_w = std::max(1, (int)(((uint32_t)span_x + 4095u) >> 12));
         ctx->grid_h = std::max(1, (int)(((uint32_t)span_y + 4095u) >> 12));
         const size_t ncells = (size_t)ctx->grid_w * ctx->grid_h;
-        if (ncells + 1 > ctx->cap_cells) {
-            size_t cap = 0;
-            if ((rc = ensure(ctx->d_cell_count, cap, ncells + 1))) return rc; cap = 0;
-            if ((rc = ensure(ctx->d_cell_start, cap, ncells + 1))) return rc; cap = 0;
-            if ((rc = ensure(ctx->d_cell_fill, cap, ncells + 1))) return rc;
-            ctx->cap_cells = ncells + 1;
-        }
+        if ((rc = pf_dbuf_reserve_all(ncells + 1, ctx->d_cell_count, ctx->d_cell_start, ctx->d_cell_fill))) return rc;
     }
     if (hi > lo) {
         k_make_records<<<((int)(hi - lo) + 255) / 256, 256, 0, st>>>(ctx->d_agents, ctx->d_records, ctx->d_flock_of, (int)lo, (int)hi);
@@ -1251,16 +1211,7 @@ extern "C" int pfnav_agents_set_work(pfnav_ctx *ctx, const uint32_t *uids, size_
     }
     for (size_t i = 0; i < nwork; i++)
         PF_ARG(uids[i] >= ctx->shard_lo && uids[i] < ctx->shard_hi, "work uid outside this context's own entity range");
-    if (nwork > ctx->cap_work) {
-        size_t cap = 0; int rc;
-        if ((rc = ensure(ctx->d_work, cap, nwork))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_vel_out, cap, nwork))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_vpref_out, cap, nwork))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_vdes_out, cap, nwork))) return rc; cap = 0;
-        if ((rc = ensure(ctx->d_los_out, cap, nwork))) return rc;
-        ctx->cap_work = nwork;
-    }
-    if (!ctx->d_work_count) PF_CUDA(cudaMalloc(&ctx->d_work_count, 16));
+    if (int rc = pf_work_reserve(ctx, nwork)) return rc;
     if (nwork) PF_CUDA(cudaMemcpy(ctx->d_work, uids, nwork * 4, cudaMemcpyHostToDevice));
     ctx->n_work = nwork;
     return PFNAV_OK;
@@ -1292,27 +1243,19 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
     tp.hz = ctx->hz;
     tp.scaled_max_force_d = (double)(0.75f / (float)ctx->hz) * 20.0;
     tp.scaled_max_force = (float)tp.scaled_max_force_d;
-    if (!ctx->d_cp_stats) {
-        PF_CUDA(cudaMalloc(&ctx->d_cp_stats, 16 * sizeof(unsigned long long)));
-        PF_CUDA(cudaMemsetAsync(ctx->d_cp_stats, 0, 16 * sizeof(unsigned long long), st));
-    }
-    tp.stats = (unsigned long long *)ctx->d_cp_stats;
+    bool grew;
+    if (int rc = ctx->d_cp_stats.reserve(16, &grew)) return rc;
+    if (grew) PF_CUDA(cudaMemsetAsync(ctx->d_cp_stats, 0, 16 * sizeof(unsigned long long), st));
+    tp.stats = ctx->d_cp_stats;
     tp.queue = (unsigned int *)(tp.stats + 8);
     PF_CUDA(cudaMemsetAsync(tp.queue, 0, 4 * sizeof(unsigned int), st));
     PF_CUDA(cudaMemsetAsync(ctx->d_work_count, 0, 4, st));
     {
     pf_prof_scope prof(ctx, st, PF_PROF_COHESION);
-    if (ctx->cap_member_pos < ctx->n_agents) {
-        cudaFree(ctx->d_member_pos); ctx->d_member_pos = nullptr; ctx->cap_member_pos = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_member_pos, std::max<size_t>(ctx->n_agents, 1) * sizeof(float2)));
-        ctx->cap_member_pos = ctx->n_agents;
-    }
-    if (ctx->cap_coh < ctx->n_agents) {
-        cudaFree(ctx->d_cohesion); cudaFree(ctx->d_coh_fallback); ctx->d_cohesion = nullptr; ctx->d_coh_fallback = nullptr; ctx->cap_coh = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_cohesion, std::max<size_t>(ctx->n_agents, 1) * sizeof(float2)));
-        PF_CUDA(cudaMalloc(&ctx->d_coh_fallback, (std::max<size_t>(ctx->n_agents, 1) + 4) * sizeof(uint32_t)));
-        ctx->cap_coh = ctx->n_agents;
-    }
+    const size_t n1 = std::max<size_t>(ctx->n_agents, 1);
+    if (int rc = ctx->d_member_pos.reserve(n1)) return rc;
+    if (int rc = ctx->d_cohesion.reserve(n1)) return rc;
+    if (int rc = ctx->d_coh_fallback.reserve(n1 + 4)) return rc;
     k_gather_flock_pos<<<((int)ctx->n_agents + 255) / 256, 256, 0, st>>>(ctx->d_records, ctx->d_flock_members, (int)ctx->n_agents,
                                                                         ctx->d_member_pos);
     // big flocks: windowed pass over the position index + full-list fall-back for entities without company; small
@@ -1326,19 +1269,16 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
         const int nblk = ((int)ctx->n_agents + COH_THREADS - 1) / COH_THREADS;     // one 128-entry run each: the hardware scheduler balances them
         // fewer runs than ~8 blocks per SM: split every run's window rows over blockIdx.y
         const int nsplit = std::max(1, std::min(8, (ctx->sm_count * 8 + nblk - 1) / nblk));
-        if (nsplit > 1 && ctx->cap_coh_part < (size_t)nsplit * ctx->n_agents) {
-            cudaFree(ctx->d_coh_part); ctx->d_coh_part = nullptr; ctx->cap_coh_part = 0;
-            PF_CUDA(cudaMalloc(&ctx->d_coh_part, (size_t)8 * ctx->n_agents * sizeof(float4)));
-            ctx->cap_coh_part = (size_t)8 * ctx->n_agents;
-        }
+        if (nsplit > 1)
+            if (int rc = ctx->d_coh_part.reserve((size_t)nsplit * ctx->n_agents)) return rc;
         k_cohesion_window<<<dim3(nblk, nsplit), COH_THREADS, 0, st>>>(grid_of(ctx), ctx->d_records, ctx->d_sorted_flock, ctx->d_flock_start,
                                                         (int)ctx->n_agents, (uint32_t)ctx->shard_lo, (uint32_t)ctx->shard_hi,
                                                         tp.scaled_max_force, ctx->d_cohesion, ctx->d_coh_fallback, d_nfb,
-                                                        (float4 *)ctx->d_coh_part, nsplit);
+                                                        ctx->d_coh_part, nsplit);
         if (nsplit > 1) {
             k_cohesion_finish<<<((int)ctx->n_agents + 127) / 128, 128, 0, st>>>(grid_of(ctx), ctx->d_records, ctx->d_sorted_flock,
                 ctx->d_flock_start, (int)ctx->n_agents, (uint32_t)ctx->shard_lo, (uint32_t)ctx->shard_hi, tp.scaled_max_force,
-                ctx->d_cohesion, ctx->d_coh_fallback, d_nfb, (const float4 *)ctx->d_coh_part, nsplit);
+                ctx->d_cohesion, ctx->d_coh_fallback, d_nfb, ctx->d_coh_part, nsplit);
             ctx->launches++;
         }
         // fall-back entities: the grid is sized for the worst case, the kernel reads the count on the device
@@ -1353,12 +1293,9 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
     }
     }
     const int ctas = std::min((nwork + VEL_WARPS_PER_CTA - 1) / VEL_WARPS_PER_CTA, ctx->sm_count * 8 * 4);
-    if (ctx->any_garrisoned && ctx->nb_scratch_warps < (size_t)ctas * VEL_WARPS_PER_CTA) {
-        // per-warp raw neighbour lists for the garrisoned-filter path (find_neighbours, 512 ids each)
-        cudaFree(ctx->d_nb_scratch); ctx->d_nb_scratch = nullptr; ctx->nb_scratch_warps = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_nb_scratch, (size_t)ctas * VEL_WARPS_PER_CTA * 512 * sizeof(uint32_t)));
-        ctx->nb_scratch_warps = (size_t)ctas * VEL_WARPS_PER_CTA;
-    }
+    // per-warp raw neighbour lists for the garrisoned-filter path (find_neighbours, 512 ids each)
+    if (ctx->any_garrisoned)
+        if (int rc = ctx->d_nb_scratch.reserve((size_t)ctas * VEL_WARPS_PER_CTA * 512)) return rc;
     // Two-phase velocity update while LOS chains are still in flight on the field stream: the part of
     // ClearPath that does not depend on the preferred velocity (neighbours, velocity obstacles, admissible
     // ray intersections) runs now, next to them; only the choice waits for the fields.
@@ -1376,11 +1313,7 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
                                         (worth && ctx->los_inflight && cudaEventQuery(ctx->ev_los) == cudaErrorNotReady));
     cudaGetLastError();
     PF_CUDA(cudaEventRecord(ctx->ev_vel0, st));
-    if (two_phase && ctx->cap_prep < (size_t)nwork) {
-        cudaFree(ctx->d_prep); ctx->d_prep = nullptr; ctx->cap_prep = 0;
-        if (cudaMalloc(&ctx->d_prep, (size_t)nwork * sizeof(pf_prep)) == cudaSuccess) ctx->cap_prep = (size_t)nwork;
-        else { cudaGetLastError(); two_phase = false; }         // no room: fall back to the single pass
-    }
+    if (two_phase && ctx->d_prep.reserve((size_t)nwork)) two_phase = false;       // no room: fall back to the single pass
     if (two_phase) {
         pf_prof_scope prof(ctx, st, PF_PROF_VELOCITY);
         // phase A has the whole LOS phase to hide in: a smaller persistent grid leaves the schedulers to the
@@ -1389,7 +1322,7 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
         k_agent_velocity<1><<<ctas_a, VEL_WARPS_PER_CTA * 32, VEL_SMEM_BYTES, st>>>(m, grid_of(ctx), tp, ctx->d_agents, ctx->d_records, ctx->d_flocks,
                                                                     ctx->d_work, nwork, ctx->d_vdes_out, ctx->d_los_out,
                                                                     ctx->d_cohesion, ctx->d_vel_out, ctx->d_vpref_out,
-                                                                    ctx->any_garrisoned ? 1 : 0, ctx->d_nb_scratch, (pf_prep *)ctx->d_prep, ctx->d_formation);
+                                                                    ctx->any_garrisoned ? 1 : 0, ctx->d_nb_scratch, ctx->d_prep, ctx->d_formation);
         ctx->launches++;
     }
     // everything above is independent of the flow/LOS fields; the LOS chains forked by
@@ -1413,7 +1346,7 @@ extern "C" int pfnav_agents_tick(pfnav_ctx *ctx, uint32_t flags, void *stream)
         k_agent_velocity<2><<<ctas, VEL_WARPS_PER_CTA * 32, VEL_SMEM_BYTES, st>>>(m, grid_of(ctx), tp, ctx->d_agents, ctx->d_records, ctx->d_flocks,
                                                                     ctx->d_work, nwork, ctx->d_vdes_out, ctx->d_los_out,
                                                                     ctx->d_cohesion, ctx->d_vel_out, ctx->d_vpref_out,
-                                                                    ctx->any_garrisoned ? 1 : 0, ctx->d_nb_scratch, (pf_prep *)ctx->d_prep, ctx->d_formation);
+                                                                    ctx->any_garrisoned ? 1 : 0, ctx->d_nb_scratch, ctx->d_prep, ctx->d_formation);
     else
         k_agent_velocity<0><<<ctas, VEL_WARPS_PER_CTA * 32, VEL_SMEM_BYTES, st>>>(m, grid_of(ctx), tp, ctx->d_agents, ctx->d_records, ctx->d_flocks,
                                                                     ctx->d_work, nwork, ctx->d_vdes_out, ctx->d_los_out,
@@ -2019,11 +1952,7 @@ extern "C" int pfnav_agents_upload_blocking(pfnav_ctx *ctx, const pfnav_blocking
     }
     PF_CUDA(cudaSetDevice(ctx->device));
     const size_t all = ctx->n_agents;        // uid-indexed; only the own range is held
-    if (all > ctx->blocking_n || !ctx->d_blocking) {
-        PF_CUDA(cudaDeviceSynchronize());
-        cudaFree(ctx->d_blocking); ctx->d_blocking = nullptr; ctx->blocking_n = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_blocking, std::max<size_t>(all, 1) * sizeof(pfnav_blocking)));
-    }
+    if ((rc = ctx->d_blocking.reserve(std::max<size_t>(all, 1)))) { ctx->blocking_n = 0; return rc; }
     if (n) PF_CUDA(cudaMemcpy(ctx->d_blocking + ctx->shard_lo, b, n * sizeof(pfnav_blocking), cudaMemcpyHostToDevice));
     ctx->blocking_n = all; ctx->blocking_any_fac = any_fac;
     return PFNAV_OK;
@@ -2057,12 +1986,7 @@ extern "C" int pfnav_agents_set_blocking(pfnav_ctx *ctx, const uint32_t *uids, s
     if (list.empty()) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
-    if (list.size() > ctx->cap_block_uids) {
-        PF_CUDA(cudaDeviceSynchronize());
-        cudaFree(ctx->d_block_uids); ctx->d_block_uids = nullptr; ctx->cap_block_uids = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_block_uids, list.size() * 2 * sizeof(uint32_t)));
-        ctx->cap_block_uids = list.size() * 2;
-    }
+    if ((rc = ctx->d_block_uids.reserve(list.size()))) return rc;
     PF_CUDA(cudaMemcpyAsync(ctx->d_block_uids, list.data(), list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     return blocking_emit(ctx, st, ctx->d_block_uids, (int)list.size(), nullptr, block ? 1 : 0);
 }
@@ -2072,11 +1996,7 @@ extern "C" int pfnav_agents_upload_movestate(pfnav_ctx *ctx, const pfnav_movesta
     PF_ARG(ctx && ctx->d_agents && ms, "agents not uploaded / ms == NULL");
     PF_ARG(n == ctx->shard_hi - ctx->shard_lo, "one movestate record per uploaded agent (of this context's own range)");
     PF_CUDA(cudaSetDevice(ctx->device));
-    int rc;
-    if (ctx->n_agents > ctx->cap_movestate) {
-        if ((rc = ensure(ctx->d_movestate, ctx->cap_movestate, ctx->n_agents))) return rc;
-        ctx->cap_movestate = ctx->n_agents;
-    }
+    if (int rc = ctx->d_movestate.reserve(ctx->n_agents)) return rc;
     PF_CUDA(cudaMemcpy(ctx->d_movestate + ctx->shard_lo, ms, n * sizeof(pfnav_movestate), cudaMemcpyHostToDevice));
     ctx->movestate_set = true;
     return PFNAV_OK;
@@ -2087,12 +2007,9 @@ extern "C" int pfnav_agents_upload_formation(pfnav_ctx *ctx, const pfnav_formati
     PF_ARG(ctx && ctx->d_agents && f, "agents not uploaded / null");
     PF_ARG(n == ctx->shard_hi - ctx->shard_lo, "one record per uploaded agent (of this context's own range)");
     PF_CUDA(cudaSetDevice(ctx->device));
-    if (ctx->n_agents > ctx->cap_formation) {
-        cudaFree(ctx->d_formation); ctx->d_formation = nullptr; ctx->cap_formation = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_formation, ctx->n_agents * sizeof(pfnav_formation_in)));
-        PF_CUDA(cudaMemset(ctx->d_formation, 0, ctx->n_agents * sizeof(pfnav_formation_in)));
-        ctx->cap_formation = ctx->n_agents;
-    }
+    bool grew;
+    if (int rc = ctx->d_formation.reserve(ctx->n_agents, &grew)) return rc;
+    if (grew) PF_CUDA(cudaMemset(ctx->d_formation, 0, ctx->n_agents * sizeof(pfnav_formation_in)));
     PF_CUDA(cudaMemcpy(ctx->d_formation + ctx->shard_lo, f, n * sizeof(pfnav_formation_in), cudaMemcpyHostToDevice));
     return PFNAV_OK;
 }
@@ -2102,11 +2019,7 @@ extern "C" int pfnav_agents_upload_movestate_ext(pfnav_ctx *ctx, const pfnav_mov
     PF_ARG(ctx && ctx->d_agents && ms, "agents not uploaded / null");
     PF_ARG(n == ctx->shard_hi - ctx->shard_lo, "one record per uploaded agent (of this context's own range)");
     PF_CUDA(cudaSetDevice(ctx->device));
-    if (ctx->n_agents > ctx->cap_ms_ext) {
-        cudaFree(ctx->d_ms_ext); ctx->d_ms_ext = nullptr; ctx->cap_ms_ext = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_ms_ext, ctx->n_agents * sizeof(pfnav_movestate_ext)));
-        ctx->cap_ms_ext = ctx->n_agents;
-    }
+    if (int rc = ctx->d_ms_ext.reserve(ctx->n_agents)) return rc;
     PF_CUDA(cudaMemcpy(ctx->d_ms_ext + ctx->shard_lo, ms, n * sizeof(pfnav_movestate_ext), cudaMemcpyHostToDevice));
     return PFNAV_OK;
 }
@@ -2146,14 +2059,10 @@ static int refresh_arrival_consts(pfnav_ctx *ctx, cudaStream_t st)
             for (int i = 0; i < c.mc_n; i++) tiles.push_back(make_float2(c.mc[i][0], c.mc[i][1]));
         }
     const size_t b0 = dev.size() * sizeof(pf_arrival_dev), b1 = std::max<size_t>(tiles.size(), 1) * sizeof(float2);
-    if (b0 + b1 > ctx->arrival_bytes) {
-        cudaFree(ctx->d_arrival); ctx->d_arrival = nullptr; ctx->arrival_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_arrival, b0 + b1));
-        ctx->arrival_bytes = b0 + b1;
-    }
+    if (int rc = ctx->d_arrival.reserve(b0 + b1)) return rc;
     PF_CUDA(cudaStreamSynchronize(st));
     if (b0) PF_CUDA(cudaMemcpy(ctx->d_arrival, dev.data(), b0, cudaMemcpyHostToDevice));
-    if (!tiles.empty()) PF_CUDA(cudaMemcpy((uint8_t *)ctx->d_arrival + b0, tiles.data(), tiles.size() * sizeof(float2), cudaMemcpyHostToDevice));
+    if (!tiles.empty()) PF_CUDA(cudaMemcpy(ctx->d_arrival + b0, tiles.data(), tiles.size() * sizeof(float2), cudaMemcpyHostToDevice));
     ctx->arrival_valid = true; ctx->arrival_epoch = ctx->map_epoch;
     return 0;
 }
@@ -2166,10 +2075,7 @@ extern "C" int pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream)
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
     int rc;
-    if (ctx->n_work > ctx->cap_patches) {
-        if ((rc = ensure(ctx->d_patches, ctx->cap_patches, ctx->n_work))) return rc;
-        ctx->cap_patches = ctx->n_work;
-    }
+    if ((rc = ctx->d_patches.reserve(ctx->n_work))) return rc;
     if ((rc = refresh_arrival_consts(ctx, st))) return rc;
     if (!ctx->update_done) PF_CUDA(cudaEventCreateWithFlags(&ctx->update_done, cudaEventDisableTiming));
     MapView m;
@@ -2185,13 +2091,9 @@ extern "C" int pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream)
     // stands; they are computed on the host per work item in that state (a handful of units at a time)
     const pf_arrival_dev *d_tarr = nullptr; const float2 *d_ttiles = nullptr;
     if (ctx->d_ms_ext) {
-        if ((size_t)nwork > ctx->cap_enter) {
-            cudaFree(ctx->d_enter); ctx->d_enter = nullptr; ctx->cap_enter = 0;
-            PF_CUDA(cudaMalloc(&ctx->d_enter, (size_t)nwork * (sizeof(pf_enter_item) + sizeof(pf_arrival_dev)) + 16));
-            ctx->cap_enter = (size_t)nwork;
-        }
-        uint32_t *d_cnt = (uint32_t *)ctx->d_enter;
-        pf_enter_item *d_items = (pf_enter_item *)((uint8_t *)ctx->d_enter + 16);
+        if ((rc = ctx->d_enter.reserve((size_t)nwork * (sizeof(pf_enter_item) + sizeof(pf_arrival_dev)) + 16))) return rc;
+        uint32_t *d_cnt = (uint32_t *)ctx->d_enter.p;
+        pf_enter_item *d_items = (pf_enter_item *)(ctx->d_enter + 16);
         pf_arrival_dev *d_t = (pf_arrival_dev *)(d_items + nwork);
         PF_CUDA(cudaMemsetAsync(d_cnt, 0, 4, st));
         k_collect_enter_range<<<(nwork + 127) / 128, 128, 0, st>>>(ctx->d_agents, ctx->d_ms_ext, ctx->d_records, ctx->d_work, nwork, d_items, d_cnt);
@@ -2211,19 +2113,15 @@ extern "C" int pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream)
                 tarr[it.wi].mc_n = c.mc_n; tarr[it.wi].mc_off = (int32_t)tiles.size();
                 for (int i = 0; i < c.mc_n; i++) tiles.push_back(make_float2(c.mc[i][0], c.mc[i][1]));
             }
-            if (tiles.size() * sizeof(float2) > ctx->cap_ttiles) {
-                cudaFree(ctx->d_ttiles); ctx->d_ttiles = nullptr; ctx->cap_ttiles = 0;
-                PF_CUDA(cudaMalloc(&ctx->d_ttiles, tiles.size() * sizeof(float2) * 2));
-                ctx->cap_ttiles = tiles.size() * sizeof(float2) * 2;
-            }
+            if ((rc = ctx->d_ttiles.reserve(tiles.size()))) return rc;
             PF_CUDA(cudaMemcpy(d_t, tarr.data(), tarr.size() * sizeof(pf_arrival_dev), cudaMemcpyHostToDevice));
             if (!tiles.empty()) PF_CUDA(cudaMemcpy(ctx->d_ttiles, tiles.data(), tiles.size() * sizeof(float2), cudaMemcpyHostToDevice));
-            d_tarr = d_t; d_ttiles = (const float2 *)ctx->d_ttiles;
+            d_tarr = d_t; d_ttiles = ctx->d_ttiles;
         }
     }
     pf_prof_scope prof(ctx, st, PF_PROF_UPDATE);
     k_entity_update<<<(nwork + 127) / 128, 128, 0, st>>>(m, grid_of(ctx), up, ctx->d_agents, ctx->d_records, ctx->d_movestate,
-        ctx->d_flocks, (const pf_arrival_dev *)ctx->d_arrival, (const float2 *)((const uint8_t *)ctx->d_arrival + b0),
+        ctx->d_flocks, (const pf_arrival_dev *)ctx->d_arrival.p, (const float2 *)(ctx->d_arrival + b0),
         ctx->nlayers, ctx->d_work, nwork, ctx->d_vel_out, ctx->d_vdes_out, ctx->d_patches, ctx->d_flock_of,
         ctx->d_ms_ext, ctx->d_formation, d_tarr, d_ttiles);
     ctx->launches++;
@@ -2606,14 +2504,8 @@ extern "C" int pfnav_pool_repair_batch(pfnav_ctx *ctx, void *stream, int *out_nr
     const size_t o_bywi = b_m, o_reps = 2 * b_m, o_flag = 3 * b_m, o_hkey = (o_flag + (size_t)nwork * 4 + 7) & ~(size_t)7;
     const size_t o_hwi = o_hkey + (size_t)cap * 8, o_cnt = o_hwi + (size_t)cap * 4, o_gin = (o_cnt + 16 + 7) & ~(size_t)7;
     const size_t o_gout = o_gin + (size_t)nwork * 8, total = o_gout + (size_t)nwork;
-    if (ctx->rep_buf_bytes < total) {
-        PF_CUDA(cudaStreamSynchronize(st));
-        cudaFree(ctx->d_rep_buf);
-        ctx->d_rep_buf = nullptr; ctx->rep_buf_bytes = 0;
-        if (cudaMalloc(&ctx->d_rep_buf, total) != cudaSuccess) { pfnav_set_error("cudaMalloc"); return PFNAV_ERR_NOMEM; }
-        ctx->rep_buf_bytes = total;
-    }
-    uint8_t *buf = (uint8_t *)ctx->d_rep_buf;
+    if (int rc = ctx->d_rep_buf.reserve(total)) return rc;
+    uint8_t *buf = ctx->d_rep_buf;
     pf_miss *d_miss = (pf_miss *)buf, *d_bywi = (pf_miss *)(buf + o_bywi), *d_reps = (pf_miss *)(buf + o_reps);
     uint32_t *d_flag = (uint32_t *)(buf + o_flag), *d_hwi = (uint32_t *)(buf + o_hwi), *d_cnt = (uint32_t *)(buf + o_cnt);
     unsigned long long *d_hkey = (unsigned long long *)(buf + o_hkey);

@@ -180,11 +180,12 @@ struct tile_op { int32_t layer, ar, ac, faction, delta; };
 struct blk_state {
     std::vector<pfnav_blocker_op> circles;
     std::vector<tile_op> tiles;
-    uint8_t *d_fac = nullptr;               // [layer][15][H64][W64] u8, allocated with the first faction-tagged op
-    uint8_t *d_touched = nullptr, *d_ftouched = nullptr, *d_res = nullptr;      // [nlayers * chunks]
+    pf_dbuf<uint8_t> d_fac;                 // [layer][15][H64][W64] u8, allocated with the first faction-tagged op
+    pf_dbuf<uint8_t> d_touched;             // touched, ftouched and res, [nlayers * chunks] each
+    uint8_t *d_ftouched = nullptr, *d_res = nullptr;
     int nslots = 0;
-    void *d_ops = nullptr; size_t ops_bytes = 0;
-    void *d_out = nullptr; size_t out_bytes = 0;
+    pf_dbuf<uint8_t> d_ops;
+    pf_dbuf<uint16_t> d_out;
     uint64_t applied_ops = 0;
     // ops decided on the device (pf_blocker_ops_*): narrow ones for k_blockers_circles, wide ones for the host rasteriser,
     // d_dev_cnt = {narrow, wide} pending; dev_bound: an upper bound of either count, known without reading them
@@ -439,15 +440,6 @@ __global__ void __launch_bounds__(256) k_chunks_gather(const int32_t *__restrict
     }
 }
 
-static int ensure_buf(void **p, size_t *cap, size_t bytes)
-{
-    if (*cap >= bytes) return 0;
-    cudaFree(*p); *p = nullptr; *cap = 0;
-    PF_CUDA(cudaMalloc(p, bytes));
-    *cap = bytes;
-    return 0;
-}
-
 static size_t stage_blocks(size_t items) { return (items + PF_OPS_BLOCK - 1) / PF_OPS_BLOCK; }
 static size_t stage_desc_off(size_t items) { return items * 2 * sizeof(pfnav_blocker_op); }
 static size_t stage_bsum_off(size_t items) { return (stage_desc_off(items) + items + 7) & ~(size_t)7; }
@@ -506,9 +498,9 @@ static int device_flush(pfnav_ctx *ctx)
     }
     const int chunks = ctx->chunk_w * ctx->chunk_h, nslots = chunks * ctx->nlayers;
     const size_t ltiles = (size_t)ctx->W64 * ctx->H64;
+    int rc;
     if (st->nslots != nslots) {
-        cudaFree(st->d_touched); st->d_touched = nullptr;
-        PF_CUDA(cudaMalloc(&st->d_touched, (size_t)nslots * 3));
+        if ((rc = st->d_touched.reserve((size_t)nslots * 3))) return rc;
         PF_CUDA(cudaMemset(st->d_touched, 0, (size_t)nslots * 3));
         st->d_ftouched = st->d_touched + nslots; st->d_res = st->d_touched + 2 * (size_t)nslots;
         st->nslots = nslots;
@@ -518,23 +510,23 @@ static int device_flush(pfnav_ctx *ctx)
     for (const auto &o : st->tiles) need_fac |= (o.faction >= 0 && o.faction < 15);
     need_fac |= dev_cnt[0] && st->dev_fac;
     if (need_fac && !st->d_fac) {
-        PF_CUDA(cudaMalloc(&st->d_fac, ltiles * 15 * ctx->nlayers));
-        for (int l = 0; l < ctx->nlayers; l++) { int rc = fac_push_layer(ctx, st, l); if (rc) return rc; }
+        if ((rc = st->d_fac.reserve(ltiles * 15 * ctx->nlayers))) return rc;
+        for (int l = 0; l < ctx->nlayers; l++) if ((rc = fac_push_layer(ctx, st, l))) return rc;
     }
     apply_args a;
     a.g = geom_of(ctx); a.nlayers = ctx->nlayers; a.W64 = ctx->W64; a.H64 = ctx->H64;
     a.blk = ctx->d_blk; a.fac = st->d_fac; a.touched = st->d_touched; a.ftouched = st->d_ftouched;
     const size_t nc = st->circles.size(), ntl = st->tiles.size();
-    if (ensure_buf(&st->d_ops, &st->ops_bytes, std::max(nc * sizeof(pfnav_blocker_op), std::max(ntl * sizeof(tile_op), (size_t)nslots * 4))))
-        return PFNAV_ERR_CUDA;
+    if ((rc = st->d_ops.reserve(std::max(nc * sizeof(pfnav_blocker_op), std::max(ntl * sizeof(tile_op), (size_t)nslots * 4)))))
+        return rc;
     if (nc) {
         PF_CUDA(cudaMemcpy(st->d_ops, st->circles.data(), nc * sizeof(pfnav_blocker_op), cudaMemcpyHostToDevice));
-        k_blockers_circles<<<(unsigned)((nc + 3) / 4), 128>>>((const pfnav_blocker_op *)st->d_ops, (int)nc, a);
+        k_blockers_circles<<<(unsigned)((nc + 3) / 4), 128>>>((const pfnav_blocker_op *)st->d_ops.p, (int)nc, a);
         ctx->launches++;
     }
     if (ntl) {
         PF_CUDA(cudaMemcpy(st->d_ops, st->tiles.data(), ntl * sizeof(tile_op), cudaMemcpyHostToDevice));   // after the circles kernel (same stream)
-        k_blockers_tiles<<<(unsigned)((ntl + 255) / 256), 256>>>((const tile_op *)st->d_ops, (int)ntl, a);
+        k_blockers_tiles<<<(unsigned)((ntl + 255) / 256), 256>>>((const tile_op *)st->d_ops.p, (int)ntl, a);
         ctx->launches++;
     }
     if (dev_cnt[0]) {
@@ -564,10 +556,10 @@ static int device_flush(pfnav_ctx *ctx)
         if (res[s] & 4) ctx->fdirty.insert({s / chunks, s % chunks});
     }
     if (!slots.empty()) {
-        if (ensure_buf(&st->d_out, &st->out_bytes, slots.size() * 8192 * sizeof(uint16_t))) return PFNAV_ERR_CUDA;
+        if ((rc = st->d_out.reserve(slots.size() * 8192))) return rc;
         PF_CUDA(cudaMemcpy(st->d_ops, slots.data(), slots.size() * 4, cudaMemcpyHostToDevice));
-        k_chunks_gather<<<(unsigned)slots.size(), 256>>>((const int32_t *)st->d_ops, ctx->chunk_w, ctx->chunk_h, ctx->W64, ctx->H64,
-                                                         ctx->d_blk, ctx->d_liid, (uint16_t *)st->d_out);
+        k_chunks_gather<<<(unsigned)slots.size(), 256>>>((const int32_t *)st->d_ops.p, ctx->chunk_w, ctx->chunk_h, ctx->W64, ctx->H64,
+                                                         ctx->d_blk, ctx->d_liid, st->d_out);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
         std::vector<uint16_t> out(slots.size() * 8192);
@@ -823,7 +815,6 @@ void pfnav_blockers_forget(pfnav_ctx *ctx)
     if (ctx->device >= 0) {
         cudaSetDevice(ctx->device);
         cudaDeviceSynchronize();
-        cudaFree(st->d_fac); cudaFree(st->d_touched); cudaFree(st->d_ops); cudaFree(st->d_out);
         cudaFree(st->d_dev_narrow); cudaFree(st->d_dev_wide); cudaFree(st->d_dev_cnt); cudaFree(st->d_stage);
     }
     delete st;

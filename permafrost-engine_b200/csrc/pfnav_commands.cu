@@ -193,24 +193,6 @@ __global__ void __launch_bounds__(1024) k_work_compact(const pf_record *__restri
 // ------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------
-static int cmd_buf(pfnav_ctx *ctx, size_t bytes)
-{
-    if (bytes <= ctx->cmd_buf_bytes) return 0;
-    cudaFree(ctx->d_cmd_buf); ctx->d_cmd_buf = nullptr; ctx->cmd_buf_bytes = 0;       // waits for the device
-    bytes = std::max<size_t>(bytes + bytes / 2, 1 << 16);
-    PF_CUDA(cudaMalloc(&ctx->d_cmd_buf, bytes));
-    ctx->cmd_buf_bytes = bytes;
-    return 0;
-}
-
-template <typename T>
-static int regrow(T *&p, size_t count)
-{
-    cudaFree(p); p = nullptr;
-    PF_CUDA(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
-    return 0;
-}
-
 // d_flock_start / d_flock_members from d_flock_of on `st`; hist: nflocks * W words of scratch
 static int members_on_device(pfnav_ctx *ctx, cudaStream_t st, uint32_t *hist, int per, int W)
 {
@@ -281,14 +263,9 @@ static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_ag
     const int per = (int)(((ctx->n_agents + max_w - 1) / max_w + 31) / 32 * 32);
     const int W = per ? (int)((ctx->n_agents + per - 1) / per) : 0;
     const size_t b_deltas = merged.size() * sizeof(pfnav_agent_delta), b_foreign = foreign.size() * sizeof(pf_cmd_foreign);
-    if ((rc = cmd_buf(ctx, b_deltas + b_foreign + (members ? nflocks * (size_t)W * 4 : 0)))) return rc;
-    if (nflocks + 1 > ctx->cap_flocks) {       // keeps no content: the table follows, the offsets are rebuilt (members)
-        PF_CUDA(cudaDeviceSynchronize());
-        const size_t cap = std::max(nflocks + 1, ctx->cap_flocks * 2);
-        if ((rc = regrow(ctx->d_flocks, cap))) return rc;
-        if ((rc = regrow(ctx->d_flock_start, cap + 1))) return rc;
-        ctx->cap_flocks = cap;
-    }
+    if ((rc = ctx->d_cmd_buf.reserve(b_deltas + b_foreign + (members ? nflocks * (size_t)W * 4 : 0)))) return rc;
+    // keeps no content: the table follows, the offsets are rebuilt (members)
+    if ((rc = pf_flocks_reserve(ctx, nflocks))) return rc;
     if (flocks) {
         // from the context's own pageable copy, which is staged before the call returns: the caller's array may be pinned
         ctx->h_flocks.assign(flocks, flocks + nflocks);
@@ -298,13 +275,13 @@ static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_ag
     if (!merged.empty()) {
         const bool have_ms = ctx->movestate_set && ctx->d_movestate != nullptr;
         PF_CUDA(cudaMemcpyAsync(ctx->d_cmd_buf, merged.data(), b_deltas, cudaMemcpyHostToDevice, st));
-        k_apply_deltas<<<((int)merged.size() + 127) / 128, 128, 0, st>>>((const pfnav_agent_delta *)ctx->d_cmd_buf, (int)merged.size(),
-            ctx->d_agents, have_ms ? ctx->d_movestate : nullptr, ctx->d_ms_ext, ctx->d_flock_of, ctx->d_records);
+        k_apply_deltas<<<((int)merged.size() + 127) / 128, 128, 0, st>>>((const pfnav_agent_delta *)ctx->d_cmd_buf.p, (int)merged.size(),
+            ctx->d_agents, have_ms ? ctx->d_movestate.p : nullptr, ctx->d_ms_ext, ctx->d_flock_of, ctx->d_records);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
     }
     if (!foreign.empty()) {
-        pf_cmd_foreign *d_foreign = (pf_cmd_foreign *)((uint8_t *)ctx->d_cmd_buf + b_deltas);
+        pf_cmd_foreign *d_foreign = (pf_cmd_foreign *)(ctx->d_cmd_buf + b_deltas);
         PF_CUDA(cudaMemcpyAsync(d_foreign, foreign.data(), b_foreign, cudaMemcpyHostToDevice, st));
         k_apply_foreign<<<((int)foreign.size() + 127) / 128, 128, 0, st>>>(d_foreign, (int)foreign.size(), ctx->d_flock_of,
                                                                              ctx->d_records);
@@ -317,7 +294,7 @@ static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_ag
     ctx->cmd_mirror.used(used);
     if (flocks || used != ctx->flock_layer_used) ctx->arrival_valid = false;
     ctx->flock_layer_used.swap(used);
-    if (members && (rc = members_on_device(ctx, st, (uint32_t *)((uint8_t *)ctx->d_cmd_buf + b_deltas + b_foreign), per, W))) return rc;
+    if (members && (rc = members_on_device(ctx, st, (uint32_t *)(ctx->d_cmd_buf + b_deltas + b_foreign), per, W))) return rc;
     if ((any & (PFNAV_DELTA_RADIUS | PFNAV_DELTA_FLAGS)) && (rc = pfnav_agents_refresh_facts(ctx, st))) return rc;
     return PFNAV_OK;
 }
@@ -364,8 +341,8 @@ extern "C" int pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *o
     const int nb = std::min(1024, (cnt + 1023) / 1024);
     const int per = nb ? ((cnt + nb - 1) / nb + 1023) / 1024 * 1024 : 0;
     if (cnt) {
-        if ((rc = cmd_buf(ctx, ((size_t)nb + 1) * 4))) return rc;
-        uint32_t *part = (uint32_t *)ctx->d_cmd_buf;
+        if ((rc = ctx->d_cmd_buf.reserve(((size_t)nb + 1) * 4))) return rc;
+        uint32_t *part = (uint32_t *)ctx->d_cmd_buf.p;
         k_work_count<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, part);
         k_work_scan<<<1, 1024, 0, st>>>(part, nb);
         ctx->launches += 2;
@@ -373,20 +350,9 @@ extern "C" int pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *o
         PF_CUDA(cudaMemcpyAsync(&nwork, part + nb, 4, cudaMemcpyDeviceToHost, st));
         PF_CUDA(cudaStreamSynchronize(st));
     }
-    if (nwork > ctx->cap_work) {
-        // room to spare: units wake a few at a time, and every regrowth waits for the device
-        const size_t cap = std::min<size_t>((size_t)cnt, (size_t)nwork + nwork / 4 + 1024);
-        PF_CUDA(cudaDeviceSynchronize());
-        if ((rc = regrow(ctx->d_work, cap))) return rc;
-        if ((rc = regrow(ctx->d_vel_out, cap))) return rc;
-        if ((rc = regrow(ctx->d_vpref_out, cap))) return rc;
-        if ((rc = regrow(ctx->d_vdes_out, cap))) return rc;
-        if ((rc = regrow(ctx->d_los_out, cap))) return rc;
-        ctx->cap_work = cap;
-    }
-    if (!ctx->d_work_count) PF_CUDA(cudaMalloc(&ctx->d_work_count, 16));
+    if ((rc = pf_work_reserve(ctx, nwork))) return rc;
     if (nwork) {
-        k_work_compact<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, (const uint32_t *)ctx->d_cmd_buf, ctx->d_work);
+        k_work_compact<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, (const uint32_t *)ctx->d_cmd_buf.p, ctx->d_work);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
     }

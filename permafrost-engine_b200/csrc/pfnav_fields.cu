@@ -1148,9 +1148,6 @@ static void free_map(pfnav_ctx *ctx)
 void pfnav_fields_free(pfnav_ctx *ctx)
 {
     free_map(ctx);
-    cudaFree(ctx->d_stage); ctx->d_stage = nullptr;
-    cudaFree(ctx->d_los_sched); ctx->d_los_sched = nullptr; ctx->los_sched_bytes = 0;
-    cudaFree(ctx->d_los_trace); ctx->d_los_trace = nullptr; ctx->los_trace_cap = 0;
     pf_pool_free(ctx);
     if (ctx->ev_los_sched) { cudaEventDestroy(ctx->ev_los_sched); ctx->ev_los_sched = nullptr; }
 }
@@ -1169,8 +1166,6 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     pf_stage_free(ctx);
-    cudaFree(ctx->d_mq_buf);
-    cudaFree(ctx->d_job_stage);
     pfnav_fields_free(ctx);
     pfnav_agents_free(ctx);
     if (ctx->tick_done) cudaEventDestroy(ctx->tick_done);
@@ -1225,16 +1220,6 @@ extern "C" int pfnav_set_tma(pfnav_ctx *ctx, int enable)
     PF_ARG(ctx, "ctx");
     ctx->use_tma = enable != 0;
     return PFNAV_OK;
-}
-
-static int ensure_stage(pfnav_ctx *ctx, size_t bytes)
-{
-    if (ctx->stage_bytes >= bytes) return 0;
-    cudaFree(ctx->d_stage);
-    ctx->d_stage = nullptr; ctx->stage_bytes = 0;
-    PF_CUDA(cudaMalloc(&ctx->d_stage, bytes));
-    ctx->stage_bytes = bytes;
-    return 0;
 }
 
 extern "C" int pfnav_map_create(pfnav_ctx *ctx, int chunk_w, int chunk_h, int nlayers, float map_x, float map_z)
@@ -1323,7 +1308,7 @@ extern "C" int pfnav_map_upload_layer(pfnav_ctx *ctx, int layer, const uint8_t *
     }
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(cudaDeviceSynchronize());     // the kernels below run on the default stream: nothing may still read the old grids
-    int rc = ensure_stage(ctx, ltiles * 2);
+    int rc = ctx->d_stage.reserve(ltiles * 2);
     if (rc) return rc;
     const int nblk = std::min<size_t>((ltiles + 255) / 256, (size_t)ctx->sm_count * 8);
     memmove(ctx->h_cost.data() + ltiles * layer, cost_base, ltiles);      // callers may pass the mirrors themselves
@@ -1331,18 +1316,18 @@ extern "C" int pfnav_map_upload_layer(pfnav_ctx *ctx, int layer, const uint8_t *
     else std::fill(ctx->h_blk.begin() + ltiles * layer, ctx->h_blk.begin() + ltiles * (layer + 1), 0);
     if (local_islands) memmove(ctx->h_liid.data() + ltiles * layer, local_islands, ltiles * 2);
     PF_CUDA(cudaMemcpy(ctx->d_stage, cost_base, ltiles, cudaMemcpyHostToDevice));
-    k_deblock<uint8_t><<<nblk, 256>>>((const uint8_t *)ctx->d_stage, ctx->d_cost + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
+    k_deblock<uint8_t><<<nblk, 256>>>((const uint8_t *)ctx->d_stage.p, ctx->d_cost + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
     ctx->launches++;
     if (blockers) {
         PF_CUDA(cudaMemcpy(ctx->d_stage, blockers, ltiles * 2, cudaMemcpyHostToDevice));
-        k_deblock<uint16_t><<<nblk, 256>>>((const uint16_t *)ctx->d_stage, ctx->d_blk + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
+        k_deblock<uint16_t><<<nblk, 256>>>((const uint16_t *)ctx->d_stage.p, ctx->d_blk + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
         ctx->launches++;
     } else {
         PF_CUDA(cudaMemset(ctx->d_blk + ltiles * layer, 0, ltiles * 2));
     }
     if (local_islands) {
         PF_CUDA(cudaMemcpy(ctx->d_stage, local_islands, ltiles * 2, cudaMemcpyHostToDevice));
-        k_deblock<uint16_t><<<nblk, 256>>>((const uint16_t *)ctx->d_stage, ctx->d_liid + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
+        k_deblock<uint16_t><<<nblk, 256>>>((const uint16_t *)ctx->d_stage.p, ctx->d_liid + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
         ctx->launches++;
     }
     PF_CUDA(cudaGetLastError());
@@ -1379,12 +1364,12 @@ extern "C" int pfnav_map_cost_from_tiles(pfnav_ctx *ctx, int layer, int ref_laye
                     make_char4((char)(rec[0] != 0), (char)type, (char)bh, (char)rh);
             }
         }
-    int rc = ensure_stage(ctx, std::max(ntiles * 4, ltiles * 2));
+    int rc = ctx->d_stage.reserve(std::max(ntiles * 4, ltiles * 2));
     if (rc) return rc;
     ctx->map_epoch++;
     PF_CUDA(cudaMemcpy(ctx->d_stage, packed.data(), ntiles * 4, cudaMemcpyHostToDevice));
     dim3 blk(32, 8), grd((W32 + 31) / 32, (H32 + 7) / 8);
-    k_cost_from_tiles<<<grd, blk>>>((const char4 *)ctx->d_stage, ctx->d_cost + ltiles * layer, W32, H32, ref_layer / 4);
+    k_cost_from_tiles<<<grd, blk>>>((const char4 *)ctx->d_stage.p, ctx->d_cost + ltiles * layer, W32, H32, ref_layer / 4);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
     PF_CUDA(cudaMemset(ctx->d_blk + ltiles * layer, 0, ltiles * 2));       // nav.c:2332
@@ -1456,11 +1441,11 @@ extern "C" int pfnav_map_upload_factions(pfnav_ctx *ctx, int layer, const uint8_
     ctx->map_epoch++;
     if (ctx->device < 0) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
-    int rc = ensure_stage(ctx, ltiles * 2);
+    int rc = ctx->d_stage.reserve(ltiles * 2);
     if (rc) return rc;
     PF_CUDA(cudaMemcpy(ctx->d_stage, fm, ltiles * 2, cudaMemcpyHostToDevice));
     const int nblk = (int)std::min<size_t>((ltiles + 255) / 256, (size_t)ctx->sm_count * 8);
-    k_deblock<uint16_t><<<nblk, 256>>>((const uint16_t *)ctx->d_stage, ctx->d_fmask + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
+    k_deblock<uint16_t><<<nblk, 256>>>((const uint16_t *)ctx->d_stage.p, ctx->d_fmask + ltiles * layer, ctx->chunk_w, ctx->chunk_h);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
     PF_CUDA(cudaDeviceSynchronize());
@@ -1700,21 +1685,10 @@ int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint
     // is ordered after the previous one through ev_los_sched, and growing the buffer waits for the whole device.
     if (!ctx->ev_los_sched) PF_CUDA(cudaEventCreateWithFlags(&ctx->ev_los_sched, cudaEventDisableTiming));
     else PF_CUDA(cudaStreamWaitEvent(st, ctx->ev_los_sched, 0));
-    const size_t need = (n + 1) * sizeof(int);
-    if (ctx->los_sched_bytes < need) {
-        PF_CUDA(cudaDeviceSynchronize());
-        cudaFree(ctx->d_los_sched);
-        ctx->d_los_sched = nullptr; ctx->los_sched_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_los_sched, need * 2));
-        ctx->los_sched_bytes = need * 2;
-    }
-    PF_CUDA(cudaMemsetAsync(ctx->d_los_sched, 0, need, st));
-    if (ctx->los_trace_on && ctx->los_trace_cap < n) {
-        PF_CUDA(cudaStreamSynchronize(st));
-        cudaFree(ctx->d_los_trace); ctx->d_los_trace = nullptr; ctx->los_trace_cap = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_los_trace, n * 4 * sizeof(unsigned long long)));
-        ctx->los_trace_cap = n;
-    }
+    if (int rc = ctx->d_los_sched.reserve(n + 1)) return rc;
+    PF_CUDA(cudaMemsetAsync(ctx->d_los_sched, 0, (n + 1) * sizeof(int), st));
+    if (ctx->los_trace_on)
+        if (int rc = ctx->d_los_trace.reserve(n * 4)) return rc;
     pf_prof_scope prof(ctx, st, PF_PROF_LOS);
     // 2 persistent CTAs per SM (117 KB of shared memory): a flow CTA (98 KB) still fits beside them, so the flow
     // waves of the same batch -- and with them every later launch, the block scheduler serves grids in order --
@@ -1722,17 +1696,17 @@ int pfnav_los_launch(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint
     const int grid = std::max(1, std::min((int)((n + LOS_WARPS_PER_CTA - 1) / LOS_WARPS_PER_CTA), ctx->sm_count * 2));
     if (ctx->los_variant == 2)
         k_los_level<<<grid, LOS_WARPS_PER_CTA * 32, smem, st>>>(g, mi, d_reqs, (int)n, d_out_fields, d_out_slot,
-                                                                (unsigned *)ctx->d_los_sched, (int *)ctx->d_los_sched + 1,
-                                                                ctx->los_trace_on ? ctx->d_los_trace : nullptr);
+                                                                (unsigned *)ctx->d_los_sched.p, ctx->d_los_sched + 1,
+                                                                ctx->los_trace_on ? ctx->d_los_trace.p : nullptr);
     else if (ctx->los_variant == 1)
         k_los_b<<<grid, LOS_WARPS_PER_CTA * 32, smem, st>>>(g, mi, d_reqs, (int)n, d_out_fields, d_out_slot,
-                                                            (unsigned *)ctx->d_los_sched, (int *)ctx->d_los_sched + 1,
-                                                            ctx->los_trace_on ? ctx->d_los_trace : nullptr);
+                                                            (unsigned *)ctx->d_los_sched.p, ctx->d_los_sched + 1,
+                                                            ctx->los_trace_on ? ctx->d_los_trace.p : nullptr);
     else
         k_los<<<grid, LOS_WARPS_PER_CTA * 32, smem, st>>>(g, mi, d_reqs, (int)n, d_out_fields, d_out_slot,
-                                                          (unsigned *)ctx->d_los_sched, (int *)ctx->d_los_sched + 1,
-                                                          ctx->los_trace_on ? ctx->d_los_trace : nullptr);
-    ctx->los_trace_n = ctx->los_trace_on ? std::min(n, ctx->los_trace_cap) : 0;
+                                                          (unsigned *)ctx->d_los_sched.p, ctx->d_los_sched + 1,
+                                                          ctx->los_trace_on ? ctx->d_los_trace.p : nullptr);
+    ctx->los_trace_n = ctx->los_trace_on ? std::min(n, ctx->d_los_trace.cap / 4) : 0;
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
     PF_CUDA(cudaEventRecord(ctx->ev_los_sched, st));

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <algorithm>
 #include <chrono>
 #include <memory>
 #include <set>
@@ -43,6 +44,57 @@
         }                                                                                   \
     } while (0)
 
+// A device array that grows on demand; it owns its pointer and its capacity in elements. reserve(n) keeps the array when
+// it holds n elements. Otherwise it waits for the current device and frees the array, if there is one (a launch still in
+// flight may read it), then allocates max(n, 2 * capacity) elements (the first allocation is exact); the old content is
+// gone. A failed allocation leaves (nullptr, 0) and returns PFNAV_ERR_NOMEM. *grew, when given, tells whether the array
+// was reallocated. A pointer stays null until the first reserve, so an optional input can use null as "absent". The
+// owner is destroyed after cudaSetDevice of its device.
+template <typename T>
+struct pf_dbuf {
+    T *p = nullptr;
+    size_t cap = 0;
+    pf_dbuf() = default;
+    pf_dbuf(const pf_dbuf &) = delete;
+    pf_dbuf &operator=(const pf_dbuf &) = delete;
+    ~pf_dbuf() { release(); }
+    operator T *() const { return p; }
+    void release()
+    {
+        if (p) cudaFree(p);
+        p = nullptr; cap = 0;
+    }
+    int reserve(size_t n, bool *grew = nullptr)
+    {
+        if (grew) *grew = false;
+        if (n <= cap) return PFNAV_OK;
+        const size_t want = std::max(n, 2 * cap);
+        if (p) {
+            PF_CUDA(cudaDeviceSynchronize());
+            release();
+        }
+        if (cudaMalloc(&p, want * sizeof(T)) != cudaSuccess) {
+            cudaGetLastError();
+            p = nullptr;
+            pfnav_set_error("cudaMalloc of %zu bytes failed", want * sizeof(T));
+            return PFNAV_ERR_NOMEM;
+        }
+        cap = want;
+        if (grew) *grew = true;
+        return PFNAV_OK;
+    }
+};
+// Reserve n elements in every buffer of a group that shares one length. If an allocation fails the whole group is
+// released, so a group is either complete or empty.
+template <typename... B>
+static int pf_dbuf_reserve_all(size_t n, B &...bufs)
+{
+    int rc = PFNAV_OK;
+    ((rc = rc ? rc : bufs.reserve(n)), ...);
+    if (rc) (bufs.release(), ...);
+    return rc;
+}
+
 // 24-byte neighbour record: exactly what one agent needs to know about another
 // (SURVEY.md 8e). This is also the unit of the per-tick NCCL all-gather.
 struct __align__(8) pf_record {
@@ -52,6 +104,7 @@ struct __align__(8) pf_record {
     uint32_t state_flags;     // state << 24 | (flags & 0xFFFFFF)
 };
 static_assert(sizeof(pf_record) == 24, "pf_record must be 24 bytes");
+struct pf_prep;                          // pfnav_clearpath_kernel.cuh
 
 struct pfnav_ctx {
     int device = 0;
@@ -79,10 +132,10 @@ struct pfnav_ctx {
     uint8_t  *d_unit = nullptr;      // [layer][chunk] 1 if every passable cost in the chunk == 1
     std::vector<uint8_t> h_unit;     // host mirror
     CUtensorMap tmap_cost, tmap_blk; // rank-3 {x, y, layer}, box 64x64x1
-    void *d_stage = nullptr; size_t stage_bytes = 0;   // upload staging
-    unsigned long long *d_los_trace = nullptr; size_t los_trace_cap = 0, los_trace_n = 0; bool los_trace_on = false;
+    pf_dbuf<uint8_t> d_stage;                                  // upload staging
+    pf_dbuf<unsigned long long> d_los_trace; size_t los_trace_n = 0; bool los_trace_on = false;   // 4 words per request
     int los_variant = 2;
-    void *d_los_sched = nullptr; size_t los_sched_bytes = 0;   // LOS scheduler: work counter + per-request done flags
+    pf_dbuf<int> d_los_sched;                                  // LOS scheduler: work counter + per-request done flags
     cudaEvent_t ev_los_sched = nullptr;                        // recorded after every LOS launch: the next one waits for it
     // host mirrors (chunk-blocked, [layer][chunk][64][64]) for the host-side planner
     std::vector<uint8_t>  h_cost;
@@ -92,8 +145,8 @@ struct pfnav_ctx {
     // host-side derived state, owned by the context (no process-global tables: contexts on different threads are independent)
     void *route_state = nullptr;                               // pfnav_route.cu: std::vector<pfnav_route_layer>
     void *route_dev_state = nullptr;                           // pfnav_route.cu: device copies of the routing tables (k_portal_graph_path_warp)
-    uint16_t *d_gisl = nullptr;                                // pfnav_route.cu: global islands, [layer][H64][W64] (pfnav_map_query)
-    void *d_mq_buf = nullptr; size_t mq_buf_bytes = 0;         // pfnav_query.cu: the inputs and outputs of one query batch
+    pf_dbuf<uint16_t> d_gisl;                                  // pfnav_route.cu: global islands, [layer][H64][W64] (pfnav_map_query)
+    pf_dbuf<uint8_t> d_mq_buf;                                 // pfnav_query.cu: the inputs and outputs of one query batch
     std::set<std::pair<int, int>> dirty, fdirty;               // pfnav_blockers.cu: (layer, chunk) occupancy / faction mask changed
     void *blk_state = nullptr;                                 // pfnav_blockers.cu: queued blocker ops + device-side refcount state
 
@@ -112,58 +165,58 @@ struct pfnav_ctx {
     std::vector<aux_target> aux;
 
     // ---- agents ----
-    size_t n_agents = 0, cap_agents = 0, n_flocks = 0, cap_flocks = 0;
+    size_t n_agents = 0, n_flocks = 0;
     int hz = 20;
-    pfnav_agent *d_agents = nullptr;      // AoS input as uploaded
-    pf_record   *d_records = nullptr;     // 24-B records (uid order)
-    pfnav_flock *d_flocks = nullptr;
-    uint32_t *d_flock_start = nullptr;    // [nflocks+1] offsets into d_flock_members
-    uint32_t *d_flock_members = nullptr;  // agent ids grouped by flock, ascending uid
-    int32_t  *d_flock_of = nullptr;       // [n_agents] flock id column (all-gathered with the records)
-    pfnav_formation_in  *d_formation = nullptr; size_t cap_formation = 0;   // optional formation inputs, uid order
-    pfnav_movestate_ext *d_ms_ext = nullptr;    size_t cap_ms_ext = 0;      // optional: the movestate beyond point seeking
-    void *d_enter = nullptr; size_t cap_enter = 0; void *d_ttiles = nullptr; size_t cap_ttiles = 0;   // ENTER_ENTITY_RANGE scratch
-    uint32_t *d_facts = nullptr;          // {max radius bits, any garrisoned}
+    // per-entity arrays (pf_agents_reserve)
+    pf_dbuf<pfnav_agent> d_agents;        // AoS input as uploaded
+    pf_dbuf<pf_record> d_records;         // 24-B records (uid order)
+    pf_dbuf<uint32_t> d_flock_members;    // agent ids grouped by flock, ascending uid
+    pf_dbuf<int32_t> d_flock_of;          // [n_agents] flock id column (all-gathered with the records)
+    // flock table (pf_flocks_reserve)
+    pf_dbuf<pfnav_flock> d_flocks;
+    pf_dbuf<uint32_t> d_flock_start;      // [nflocks+1] offsets into d_flock_members
+    pf_dbuf<pfnav_formation_in> d_formation;    // optional formation inputs, uid order
+    pf_dbuf<pfnav_movestate_ext> d_ms_ext;      // optional: the movestate beyond point seeking
+    pf_dbuf<uint8_t> d_enter; pf_dbuf<float2> d_ttiles;   // ENTER_ENTITY_RANGE scratch
+    pf_dbuf<uint32_t> d_facts;            // {max radius bits, any garrisoned}
     // multi-GPU: this context owns the entity index range [shard_lo, shard_hi) of the population (pfnav_mgpu.cu)
     size_t shard_lo = 0, shard_hi = 0;
     void *mgpu = nullptr;                 // pf_mgpu: NCCL communicator or in-process group membership
     bool members_stale = false;           // flock member lists must be rebuilt at the next gather
-    float2   *d_cohesion = nullptr;       // per-agent cohesion force (pre-pass)
-    float2   *d_member_pos = nullptr; size_t cap_member_pos = 0;   // positions in flock-member order
-    void *d_prep = nullptr; size_t cap_prep = 0;                   // phase-A results of the two-phase velocity update
+    pf_dbuf<float2> d_cohesion;           // per-agent cohesion force (pre-pass)
+    pf_dbuf<float2> d_member_pos;         // positions in flock-member order
+    pf_dbuf<pf_prep> d_prep;              // phase-A results of the two-phase velocity update
     bool two_phase = true, two_phase_force = false;
     int phase_a_ctas_per_sm = 0;
     // spatial index (bitmap_grid.h equivalent)
     int grid_w = 0, grid_h = 0; int32_t origin_x = 0, origin_y = 0;
-    uint32_t *d_cell_count = nullptr, *d_cell_start = nullptr, *d_cell_fill = nullptr;
-    size_t cap_cells = 0;
-    int32_t  *d_sorted_ix = nullptr, *d_sorted_iy = nullptr;
-    uint32_t *d_sorted_id = nullptr;
-    int32_t  *d_sorted_flock = nullptr;                  // flock id of every index entry (windowed cohesion)
-    uint32_t *d_coh_fallback = nullptr; size_t cap_coh = 0;
-    void *d_scan_part = nullptr;                              // block sums of the cell-count scan
-    void *d_cp_stats = nullptr;                               // ClearPath event counters (pfnav_agents_clearpath_stats)
-    void *d_coh_part = nullptr; size_t cap_coh_part = 0;      // windowed cohesion: partial sums of split runs, float4 [nsplit][n]
+    pf_dbuf<uint32_t> d_cell_count, d_cell_start, d_cell_fill;      // cell index: ncells + 1 each
+    pf_dbuf<int32_t> d_sorted_ix, d_sorted_iy;                       // per-entity (pf_agents_reserve)
+    pf_dbuf<uint32_t> d_sorted_id;
+    pf_dbuf<int32_t> d_sorted_flock;                                 // flock id of every index entry (windowed cohesion)
+    pf_dbuf<uint32_t> d_coh_fallback;
+    pf_dbuf<uint32_t> d_scan_part;                                   // block sums of the cell-count scan
+    pf_dbuf<unsigned long long> d_cp_stats;                          // ClearPath event counters (pfnav_agents_clearpath_stats)
+    pf_dbuf<float4> d_coh_part;                                      // windowed cohesion: partial sums of split runs, [nsplit][n]
     std::vector<uint32_t> h_flock_start;
     int cohesion_mode = 0;
-    void *d_scan_tmp = nullptr; size_t scan_tmp_bytes = 0;
-    // work list + outputs
-    size_t n_work = 0, cap_work = 0;
-    uint32_t *d_work = nullptr;
-    float2 *d_vel_out = nullptr, *d_vpref_out = nullptr, *d_vdes_out = nullptr;
-    uint8_t *d_los_out = nullptr;
-    uint32_t *d_work_count = nullptr;
+    // work list + outputs (pf_work_reserve)
+    size_t n_work = 0;
+    pf_dbuf<uint32_t> d_work;
+    pf_dbuf<float2> d_vel_out, d_vpref_out, d_vdes_out;
+    pf_dbuf<uint8_t> d_los_out;
+    pf_dbuf<uint32_t> d_work_count;
     // state update (entity_compute_update)
-    pfnav_movestate *d_movestate = nullptr; size_t cap_movestate = 0; bool movestate_set = false;
-    pfnav_patch *d_patches = nullptr; size_t cap_patches = 0;
-    void *d_arrival = nullptr; size_t arrival_bytes = 0;     // [nflocks][nlayers] pf_arrival_dev + tile lists
+    pf_dbuf<pfnav_movestate> d_movestate; bool movestate_set = false;
+    pf_dbuf<pfnav_patch> d_patches;
+    pf_dbuf<uint8_t> d_arrival;                              // [nflocks][nlayers] pf_arrival_dev + tile lists
     uint64_t arrival_epoch = ~0ull; bool arrival_valid = false;
     std::vector<uint8_t> flock_layer_used;                   // [nflocks][12]
     std::vector<pfnav_flock> h_flocks;
     float max_radius = 0.0f;
     bool has_unsupported_state = false;
     bool any_garrisoned = false;                             // G_Pos_EntsInCircleFrom filters + reorders (position.c:100)
-    uint32_t *d_nb_scratch = nullptr; size_t nb_scratch_warps = 0;
+    pf_dbuf<uint32_t> d_nb_scratch;
     cudaEvent_t update_done = nullptr;
     cudaStream_t tick_stream = nullptr;
     cudaEvent_t tick_done = nullptr;
@@ -181,21 +234,21 @@ struct pfnav_ctx {
     void *stager = nullptr;
     void *planner = nullptr;
     // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand
-    void *d_rep_buf = nullptr; size_t rep_buf_bytes = 0;
+    pf_dbuf<uint8_t> d_rep_buf;
     int repair_stats[6] = {0, 0, 0, 0, 0, 0};                  // the last call: representatives per phase, rounds ended per rule
     // blocking table of pfnav_agents_upload_blocking (uid order, blocking_n records, of which the own range
     // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
-    pfnav_blocking *d_blocking = nullptr; size_t blocking_n = 0; bool blocking_any_fac = false;
-    uint32_t *d_block_uids = nullptr; size_t cap_block_uids = 0;
+    pf_dbuf<pfnav_blocking> d_blocking; size_t blocking_n = 0; bool blocking_any_fac = false;
+    pf_dbuf<uint32_t> d_block_uids;
     // pfnav_agents_commands (pfnav_commands.cu): (flock, layer) of every own entity, filled by every full upload, and the device
     // scratch of a batch (merged deltas, per-warp flock histograms, block sums of the work compaction), grown on demand
     pf_cmd_mirror cmd_mirror;
-    void *d_cmd_buf = nullptr; size_t cmd_buf_bytes = 0;
+    pf_dbuf<uint8_t> d_cmd_buf;
     // goal, zone and entity-field batches of a multi-GPU job (pfnav_mgpu_request_goals_ex, ..._zones,
     // ..._entity_fields_batch): the staging buffer of the fields built for the job, 4096-byte blocks (a zone or entity
     // batch keeps its copy list behind them), grown on demand; the last call's owner of every goal or request and the
     // requests this member built
-    uint8_t *d_job_stage = nullptr; size_t job_stage_bytes = 0;
+    pf_dbuf<uint8_t> d_job_stage;
     std::vector<int32_t> job_owner; int job_built[2] = {0, 0};
 
     // ---- optional per-kernel timing (pfnav_profile_enable) ----
@@ -444,6 +497,11 @@ int pfnav_agents_init(pfnav_ctx *ctx);
 int pfnav_agents_finish_snapshot(pfnav_ctx *ctx, cudaStream_t st, bool members);
 // max_radius and any_garrisoned from the records of the whole population (k_population_facts); waits for `st`
 int pfnav_agents_refresh_facts(pfnav_ctx *ctx, cudaStream_t st);
+// the one sizing of each group of arrays that share a length (pf_dbuf_reserve_all): the flock table for nflocks flocks
+// (d_flocks nflocks + 1, d_flock_start nflocks + 2), and the work list and its outputs for nwork items with the 4-word
+// d_work_count. A failed work list also empties the list (n_work = 0), so no tick reads the released arrays.
+int pf_flocks_reserve(pfnav_ctx *ctx, size_t nflocks);
+int pf_work_reserve(pfnav_ctx *ctx, size_t nwork);
 
 // ---- pfnav_commands.cu: a job member's part of a command batch (pfnav_mgpu.cu runs the verdict exchange) ----
 // pf_cmd_job_check validates the batch against the member's state and plans it, changing nothing (the error is set);

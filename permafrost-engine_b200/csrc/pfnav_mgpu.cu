@@ -66,9 +66,9 @@ struct pf_mgpu {
     pf_nccl_comm comm = nullptr;                 // NCCL transport
     pfnav_group *group = nullptr;                // in-process transport
     bool share_blockers = false;                 // pfnav_mgpu_share_blockers / pfnav_group_share_blockers
-    uint32_t *d_xcnt = nullptr;                  // NCCL: all-gathered records of PF_XCNT words per rank: the blocker
+    pf_dbuf<uint32_t> d_xcnt;                    // NCCL: all-gathered records of PF_XCNT words per rank: the blocker
                                                  // exchange's counts, a command batch's verdicts; read before the call returns
-    uint8_t *d_xgoal = nullptr; size_t xgoal_bytes = 0;   // NCCL: the goal batch's all-gathered member records
+    pf_dbuf<uint8_t> d_xgoal;                    // NCCL: the goal batch's all-gathered member records
 };
 #define PF_XCNT 8                                // {narrow, wide, sent narrow, sent wide, faction flag, 0, 0, 0}
                                                  // or {status, n_agents, n_flocks, 0, 0, 0, 0, 0}
@@ -139,8 +139,6 @@ extern "C" int pfnav_mgpu_finalize(pfnav_ctx *ctx)
     if (!m) return PFNAV_OK;
     PF_ARG(!m->group, "member of an in-process group: pfnav_group_destroy");
     if (ctx->device >= 0) { cudaSetDevice(ctx->device); cudaDeviceSynchronize(); }
-    cudaFree(m->d_xcnt);
-    cudaFree(m->d_xgoal);
     if (m->comm) g_nccl.CommDestroy(m->comm);
     delete m;
     ctx->mgpu = nullptr;
@@ -251,7 +249,7 @@ extern "C" int pfnav_mgpu_exchange_blocker_ops(pfnav_ctx *ctx, void *stream)
     int rc = pf_blocker_ops_view(ctx, &v);
     if (rc) return rc;
     const int world = m->world, rank = m->rank;
-    if (!m->d_xcnt) PF_CUDA(cudaMalloc(&m->d_xcnt, (size_t)world * PF_XCNT * sizeof(uint32_t)));
+    if ((rc = m->d_xcnt.reserve((size_t)world * PF_XCNT))) return rc;
     uint32_t *mine = m->d_xcnt + (size_t)rank * PF_XCNT;
     const uint32_t tail[PF_XCNT - 2] = {v.sent[0], v.sent[1], v.fac ? 1u : 0u, 0, 0, 0};
     PF_CUDA(cudaMemcpyAsync(mine, v.d_cnt, 2 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
@@ -522,12 +520,7 @@ static int nccl_job(pfnav_ctx *ctx, pf_mgpu *m, pf_job &J, cudaStream_t st, cons
     const int world = m->world, rank = m->rank;
     const size_t nlack = J.kind == PF_JOB_GOALS ? (size_t)J.ngoals * ctx->chunk_w * ctx->chunk_h : 0;
     const size_t rec = 16 + ((nlack + 15) & ~(size_t)15);
-    if (m->xgoal_bytes < rec * world) {
-        cudaFree(m->d_xgoal);
-        m->d_xgoal = nullptr; m->xgoal_bytes = 0;
-        PF_CUDA(cudaMalloc(&m->d_xgoal, rec * world));
-        m->xgoal_bytes = rec * world;
-    }
+    if (int rc = m->d_xgoal.reserve(rec * world)) return rc;
     std::vector<uint8_t> all(rec * world, 0);
     uint8_t *mine = all.data() + rec * rank;
     const int32_t hdr[4] = {local, J.fits ? 1 : 0, 0, 0};
@@ -757,7 +750,7 @@ extern "C" int pfnav_mgpu_commands(pfnav_ctx *ctx, const pfnav_agent_delta *delt
     if (!local) local = pf_cmd_job_check(ctx, deltas, n, flocks, nflocks, J);
     const std::string local_err = local ? pfnav_last_error() : "";
     const int world = m->world, rank = m->rank;
-    if (!m->d_xcnt) PF_CUDA(cudaMalloc(&m->d_xcnt, (size_t)world * PF_XCNT * sizeof(uint32_t)));
+    if (int rc = m->d_xcnt.reserve((size_t)world * PF_XCNT)) return rc;
     uint32_t *mine = m->d_xcnt + (size_t)rank * PF_XCNT;
     const uint32_t verdict[PF_XCNT] = {(uint32_t)local, (uint32_t)ctx->n_agents, (uint32_t)ctx->n_flocks, 0, 0, 0, 0, 0};
     PF_CUDA(cudaMemcpyAsync(mine, verdict, sizeof(verdict), cudaMemcpyHostToDevice, st));

@@ -665,20 +665,6 @@ static int field_copy_launch(pfnav_ctx *ctx, const uint8_t *flow_src, const uint
     return 0;
 }
 
-// the staging buffer of a job, at least `need` bytes. The previous batch's builds, exchange and copies may still read it,
-// so growing it waits for the device (a group member's stream has waited for its peers' reads of its staging)
-static int job_stage_reserve(pfnav_ctx *ctx, size_t need)
-{
-    if (ctx->job_stage_bytes >= need) return PFNAV_OK;
-    PF_CUDA(pf_fields_sync(ctx));
-    PF_CUDA(cudaDeviceSynchronize());
-    cudaFree(ctx->d_job_stage);
-    ctx->d_job_stage = nullptr; ctx->job_stage_bytes = 0;
-    PF_CUDA(cudaMalloc(&ctx->d_job_stage, need * 2));
-    ctx->job_stage_bytes = need * 2;
-    return PFNAV_OK;
-}
-
 // a job's batch reads the replicated map: refused while this member holds device blocker ops its peers have not seen
 int pf_job_check_state(pfnav_ctx *ctx)
 {
@@ -805,7 +791,10 @@ int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int 
     const size_t b_pc = parents.size() * sizeof(pf_field_copy), b_it = items.size() * sizeof(pf_field_copy);
     const size_t o_pc = W.layout(), o_it = o_pc + pf_wave_pack::align16(b_pc), total = o_it + pf_wave_pack::align16(b_it);
     PF_CUDA(cudaSetDevice(ctx->device));
-    if ((rc = job_stage_reserve(ctx, (size_t)extra * 4096))) return rc;
+    // the job staging: the previous batch's builds, exchange and copies may still read it, so growing it waits for the
+    // device and the forked field work (a group member's stream has waited for its peers' reads of its staging)
+    if ((size_t)extra * 4096 > ctx->d_job_stage.cap) PF_CUDA(pf_fields_sync(ctx));
+    if ((rc = ctx->d_job_stage.reserve((size_t)extra * 4096))) return rc;
     pf_stage S;
     if ((rc = pf_stage_begin(ctx, st, total, total, true, &S))) return rc;
     W.pack(S.host);
@@ -883,7 +872,8 @@ void pf_job_layout(pfnav_ctx *ctx, pf_job &J, const std::vector<int32_t> &freq, 
 int pf_job_stage(pfnav_ctx *ctx, pf_job &J, const std::vector<pf_field_copy> &items, int world, cudaStream_t st)
 {
     const size_t o_items = J.seg[world] * 4096, b_items = items.size() * sizeof(pf_field_copy);
-    if (int rc = job_stage_reserve(ctx, o_items + b_items)) return rc;
+    if (o_items + b_items > ctx->d_job_stage.cap) PF_CUDA(pf_fields_sync(ctx));      // as in pf_job_launch
+    if (int rc = ctx->d_job_stage.reserve(o_items + b_items)) return rc;
     pf_stage S;
     if (int rc = pf_stage_begin(ctx, st, b_items, 0, true, &S)) return rc;
     memcpy(S.host, items.data(), b_items);

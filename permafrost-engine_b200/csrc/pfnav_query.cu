@@ -48,14 +48,8 @@ extern "C" int pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, siz
     const size_t ns = search.size();
     const size_t o_res = n * sizeof(pfnav_map_query_req), o_idx = o_res + n * sizeof(pfnav_map_query_result);
     const size_t o_fb = o_idx + ns * 4, need = o_fb + ns;
-    if (ctx->mq_buf_bytes < need) {
-        PF_CUDA(cudaStreamSynchronize(st));
-        cudaFree(ctx->d_mq_buf);
-        ctx->d_mq_buf = nullptr; ctx->mq_buf_bytes = 0;
-        PF_CUDA(cudaMalloc(&ctx->d_mq_buf, need));
-        ctx->mq_buf_bytes = need;
-    }
-    uint8_t *dev = (uint8_t *)ctx->d_mq_buf;
+    if (int rc = ctx->d_mq_buf.reserve(need)) return rc;
+    uint8_t *dev = ctx->d_mq_buf;
     const pfnav_map_query_req *d_q = (const pfnav_map_query_req *)dev;
     pfnav_map_query_result *d_out = (pfnav_map_query_result *)(dev + o_res);
     PF_CUDA(cudaMemcpyAsync(dev, q, o_res, cudaMemcpyHostToDevice, st));

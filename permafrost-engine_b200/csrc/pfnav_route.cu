@@ -216,7 +216,7 @@ static int route_upload_islands(pfnav_ctx *ctx, int layer, const pfnav_route_lay
 {
     const size_t ltiles = (size_t)ctx->W64 * ctx->H64;
     PF_CUDA(cudaSetDevice(ctx->device));
-    if (!ctx->d_gisl) PF_CUDA(cudaMalloc(&ctx->d_gisl, ltiles * ctx->nlayers * 2));
+    if (int rc = ctx->d_gisl.reserve(ltiles * ctx->nlayers)) return rc;
     std::vector<uint16_t> img(ltiles);
     for (int ch = 0; ch < ctx->chunk_w * ctx->chunk_h; ch++)
         for (int r = 0; r < 64; r++)
@@ -1450,10 +1450,10 @@ struct gp_scratch {
     uint16_t queue[4096];
 };
 struct route_dev_state {
-    dev_portal *d_ports = nullptr; int32_t *d_nports = nullptr, *d_port_base = nullptr; dev_edge *d_edges = nullptr;
-    uint16_t *d_travel = nullptr; size_t travel_rows = 0, nedges = 0;
-    gp_scratch *d_scratch = nullptr; int scratch_n = 0; uint32_t stamp = 0;
-    void *d_req = nullptr, *d_out = nullptr; size_t req_bytes = 0, out_bytes = 0;
+    pf_dbuf<dev_portal> d_ports; pf_dbuf<int32_t> d_nports, d_port_base; pf_dbuf<dev_edge> d_edges;
+    pf_dbuf<uint16_t> d_travel; size_t travel_rows = 0;
+    pf_dbuf<gp_scratch> d_scratch; uint32_t stamp = 0;
+    pf_dbuf<int32_t> d_req, d_out;
     int layer = -1; uint64_t epoch = ~0ull, generation = 0;
 };
 
@@ -1713,19 +1713,9 @@ static route_dev_state *route_dev(pfnav_ctx *ctx)
 
 void pfnav_route_dev_forget(pfnav_ctx *ctx)
 {
-    if (ctx->d_gisl) {
-        cudaSetDevice(ctx->device);
-        cudaDeviceSynchronize();
-        cudaFree(ctx->d_gisl);
-        ctx->d_gisl = nullptr;
-    }
     route_dev_state *D = (route_dev_state *)ctx->route_dev_state;
     if (!D) return;
-    if (ctx->device >= 0) {
-        cudaSetDevice(ctx->device);
-        cudaFree(D->d_ports); cudaFree(D->d_nports); cudaFree(D->d_port_base); cudaFree(D->d_edges); cudaFree(D->d_travel);
-        cudaFree(D->d_scratch); cudaFree(D->d_req); cudaFree(D->d_out);
-    }
+    if (ctx->device >= 0) cudaSetDevice(ctx->device);
     delete D;
     ctx->route_dev_state = nullptr;
 }
@@ -1753,23 +1743,16 @@ static int route_dev_sync(pfnav_ctx *ctx, int layer, pfnav_route_layer &RL, rout
         }
     }
     const bool retravel = D->layer != layer || D->generation != RL.generation || D->travel_rows != rows;
-    if (!D->d_ports) {
-        PF_CUDA(cudaMalloc(&D->d_ports, ports.size() * sizeof(dev_portal)));
-        PF_CUDA(cudaMalloc(&D->d_nports, (size_t)chunks * 4));
-        PF_CUDA(cudaMalloc(&D->d_port_base, (size_t)chunks * 4));
-    }
-    if (D->nedges < edges.size()) {
-        cudaFree(D->d_edges); D->d_edges = nullptr;
-        PF_CUDA(cudaMalloc(&D->d_edges, std::max<size_t>(edges.size(), 1) * sizeof(dev_edge)));
-        D->nedges = edges.size();
-    }
+    int rc;
+    if ((rc = D->d_ports.reserve(ports.size())) || (rc = D->d_nports.reserve(chunks)) || (rc = D->d_port_base.reserve(chunks)) ||
+        (rc = D->d_edges.reserve(std::max<size_t>(edges.size(), 1))))
+        return rc;
     PF_CUDA(cudaMemcpy(D->d_ports, ports.data(), ports.size() * sizeof(dev_portal), cudaMemcpyHostToDevice));
     PF_CUDA(cudaMemcpy(D->d_nports, nports.data(), (size_t)chunks * 4, cudaMemcpyHostToDevice));
     PF_CUDA(cudaMemcpy(D->d_port_base, base.data(), (size_t)chunks * 4, cudaMemcpyHostToDevice));
     if (!edges.empty()) PF_CUDA(cudaMemcpy(D->d_edges, edges.data(), edges.size() * sizeof(dev_edge), cudaMemcpyHostToDevice));
     if (retravel) {
-        cudaFree(D->d_travel); D->d_travel = nullptr;
-        PF_CUDA(cudaMalloc(&D->d_travel, std::max<size_t>(rows, 1) * 4096 * 2));
+        if ((rc = D->d_travel.reserve(std::max<size_t>(rows, 1) * 4096))) return rc;
         for (int ch = 0; ch < chunks; ch++)
             if (nports[ch])
                 PF_CUDA(cudaMemcpy(D->d_travel + (size_t)base[ch] * 4096, RL.chunks[ch].travel.data(), (size_t)nports[ch] * 4096 * 2,
@@ -1787,18 +1770,18 @@ static int route_dev_search(pfnav_ctx *ctx, int layer, pfnav_route_layer &RL, co
     PF_CUDA(cudaSetDevice(ctx->device));
     route_dev_state *D = route_dev(ctx);
     D->epoch = ~0ull;                                                                  // edge states were just refreshed
-    if (route_dev_sync(ctx, layer, RL, D)) return PFNAV_ERR_CUDA;
+    if (int rc = route_dev_sync(ctx, layer, RL, D)) return rc;
     const size_t ostride = 4 + 3 * (size_t)max_hops;
     const int batch = 4096;                                                            // 588 KB of scratch per search in flight
     const int want = std::min(std::max(n, 1), batch);
-    if (D->scratch_n < want) {
-        cudaFree(D->d_scratch); D->d_scratch = nullptr; D->scratch_n = 0;
-        PF_CUDA(cudaMalloc(&D->d_scratch, (size_t)want * sizeof(gp_scratch)));
-        PF_CUDA(cudaMemset(D->d_scratch, 0, (size_t)want * sizeof(gp_scratch)));     // no slot carries a stamp yet
-        D->scratch_n = want; D->stamp = 0;
+    bool grew;
+    if (int rc = D->d_scratch.reserve((size_t)want, &grew)) return rc;
+    if (grew) {
+        PF_CUDA(cudaMemset(D->d_scratch, 0, D->d_scratch.cap * sizeof(gp_scratch)));     // no slot carries a stamp yet
+        D->stamp = 0;
     }
-    if (D->req_bytes < (size_t)batch * 32) { cudaFree(D->d_req); PF_CUDA(cudaMalloc(&D->d_req, (size_t)batch * 32)); D->req_bytes = (size_t)batch * 32; }
-    if (D->out_bytes < (size_t)batch * ostride * 4) { cudaFree(D->d_out); PF_CUDA(cudaMalloc(&D->d_out, (size_t)batch * ostride * 4)); D->out_bytes = (size_t)batch * ostride * 4; }
+    if (int rc = D->d_req.reserve((size_t)batch * 8)) return rc;
+    if (int rc = D->d_out.reserve((size_t)batch * ostride)) return rc;
     dev_route R;
     R.ports = D->d_ports; R.nports = D->d_nports; R.port_base = D->d_port_base; R.edges = D->d_edges; R.travel = D->d_travel;
     R.liid = ctx->d_liid + (size_t)ctx->W64 * ctx->H64 * layer; R.cw = ctx->chunk_w; R.chh = ctx->chunk_h; R.W64 = ctx->W64;
@@ -1807,12 +1790,12 @@ static int route_dev_search(pfnav_ctx *ctx, int layer, pfnav_route_layer &RL, co
     for (int b0 = 0; b0 < n; b0 += batch) {
         const int nb = std::min(batch, n - b0);
         if (++D->stamp == 0) {                                                         // the stamps wrapped: start the tables over
-            PF_CUDA(cudaMemset(D->d_scratch, 0, (size_t)D->scratch_n * sizeof(gp_scratch)));
+            PF_CUDA(cudaMemset(D->d_scratch, 0, D->d_scratch.cap * sizeof(gp_scratch)));
             D->stamp = 1;
         }
         PF_CUDA(cudaMemcpy(D->d_req, req + (size_t)b0 * 8, (size_t)nb * 32, cudaMemcpyHostToDevice));
-        k_portal_graph_path_warp<<<(nb + GP_WARPS - 1) / GP_WARPS, GP_WARPS * 32>>>(R, (const int32_t *)D->d_req, nb, D->d_scratch,
-                                                                                  (int32_t *)D->d_out, max_hops, D->stamp);
+        k_portal_graph_path_warp<<<(nb + GP_WARPS - 1) / GP_WARPS, GP_WARPS * 32>>>(R, D->d_req, nb, D->d_scratch,
+                                                                                  D->d_out, max_hops, D->stamp);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
         PF_CUDA(cudaMemcpy(out + (size_t)b0 * ostride, D->d_out, (size_t)nb * ostride * 4, cudaMemcpyDeviceToHost));

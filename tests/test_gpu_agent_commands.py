@@ -418,3 +418,51 @@ def test_more_flocks_than_one_scan_pass(pf):
         assert A.agents_read_velocities(nw).tobytes() == B.agents_read_velocities(nw).tobytes()
     finally:
         A.close(); B.close()
+
+
+@pytest.mark.gpu
+def test_work_list_and_flock_table_sized_by_both_writers(pf):
+    """A's work list is sized in turn by agents_set_work and agents_set_work_dev, its flock table by agents_commands and
+    agents_upload, each growing and shrinking; after every step the twins agree through resident ticks"""
+    T, rec, fl = _case(seed=606)
+    try:
+        s = T.tick()
+        # 1. a short explicit list
+        short = np.nonzero(s["state"] == ST_MOVING)[0][:40].astype(np.uint32)
+        for X in (T.A, T.B):
+            X.agents_set_work(short)
+        T.ticks(2)
+        # 2. most units awake: Twin.commands builds A's list with agents_set_work_dev
+        s = T.compare()
+        still = np.nonzero((s["state"] == ST_ARRIVED) | (s["state"] == ST_WAITING))[0]
+        T.commands(cr.deltas(still[: len(still) * 3 // 4], state=ST_MOVING, clear_hist=True))
+        assert len(T.A.agents_read_work()) > T.n // 2
+        T.ticks(3)
+        # 3. a longer explicit list: every entity
+        for X in (T.A, T.B):
+            X.agents_set_work(np.arange(T.n, dtype=np.uint32))
+        T.ticks(2)
+        # 4. a flock table more than twice as long, rows copied from the current ones, and units moved into the new rows
+        s = T.compare()
+        nf = len(T.fl)
+        big = T.fl[np.arange(2 * nf + 3) % nf].copy()
+        who = np.nonzero(s["state"] == ST_MOVING)[0][::5]
+        T.commands(cr.deltas(who, flock=nf + np.arange(len(who)) % (nf + 3)), big)
+        T.ticks(3)
+        # 5. a re-upload of the population with fewer flocks on both twins
+        s, ms = T.A.agents_read_state(T.n)
+        s["flock"] = np.where(s["flock"] >= nf, s["flock"] % nf, s["flock"])
+        T.fl = T.fl[:nf].copy()
+        for X in (T.A, T.B):
+            X.agents_upload(s, T.fl, T.hz)
+            X.agents_upload_movestate(ms)
+        T.work_lists()
+        T.compare()
+        T.ticks(2)
+        # 6. commands again: a table one row longer, some units moved into the new row
+        s = T.compare()
+        who = np.nonzero(s["state"] == ST_MOVING)[0][::7]
+        T.commands(cr.deltas(who, flock=nf), _grown(T.fl, s["pos"][who].mean(axis=0), nf))
+        T.ticks(3)
+    finally:
+        T.close()
