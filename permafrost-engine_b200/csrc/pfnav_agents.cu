@@ -1389,17 +1389,20 @@ extern "C" int pfnav_ents_in_circle(pfnav_ctx *ctx, float x, float z, float rang
     PF_ARG(ctx && ctx->d_records && out && out_n && maxout > 0, "args");
     PF_CUDA(cudaSetDevice(ctx->device));
     if (range < 0.0f) { *out_n = 0; return PFNAV_OK; }
-    uint32_t *d_out = nullptr; int *d_n = nullptr;
-    PF_CUDA(cudaMalloc(&d_out, (size_t)maxout * 4));
-    PF_CUDA(cudaMalloc(&d_n, 4));
-    k_ents_in_circle<<<1, 32, 0, ctx->tick_stream>>>(grid_of(ctx), x, z, range, d_out, maxout, d_n, ctx->d_records,
-                                                     ctx->any_garrisoned ? 1 : 0);
+    cudaStream_t st = ctx->tick_stream;
+    // staged: the count, then the ids; only the ids found are copied back
+    pf_stage S;
+    if (int rc = pf_stage_begin(ctx, st, 0, 16 + (size_t)maxout * 4, false, &S)) return rc;
+    int *d_n = (int *)S.dev;
+    uint32_t *d_out = (uint32_t *)(S.dev + 16);
+    k_ents_in_circle<<<1, 32, 0, st>>>(grid_of(ctx), x, z, range, d_out, maxout, d_n, ctx->d_records, ctx->any_garrisoned ? 1 : 0);
     ctx->launches++;
-    cudaError_t e = cudaStreamSynchronize(ctx->tick_stream);
-    if (e == cudaSuccess) e = cudaMemcpy(out_n, d_n, 4, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess && *out_n > 0) e = cudaMemcpy(out, d_out, (size_t)*out_n * 4, cudaMemcpyDeviceToHost);
-    cudaFree(d_out); cudaFree(d_n);
-    if (e != cudaSuccess) { pfnav_set_error("pfnav_ents_in_circle: %s", cudaGetErrorString(e)); return PFNAV_ERR_CUDA; }
+    PF_CUDA(cudaGetLastError());
+    PF_CUDA(cudaMemcpyAsync(out_n, d_n, 4, cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    if (*out_n > 0) PF_CUDA(cudaMemcpyAsync(out, d_out, (size_t)*out_n * 4, cudaMemcpyDeviceToHost, st));
+    if (int rc = pf_stage_done(ctx, st)) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 
@@ -2284,9 +2287,12 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
     PF_CUDA(cudaDeviceSynchronize());
     const int nwork = (int)ctx->n_work;
     const int chunks = ctx->chunk_w * ctx->chunk_h;
-    pf_miss *d_miss = nullptr; uint32_t *d_cnt = nullptr;
-    PF_CUDA(cudaMalloc(&d_miss, (size_t)nwork * sizeof(pf_miss)));
-    if (cudaMalloc(&d_cnt, 4) != cudaSuccess) { cudaFree(d_miss); pfnav_set_error("cudaMalloc"); return PFNAV_ERR_NOMEM; }
+    // the misses and their counter in the scratch of pfnav_pool_repair_batch: the path requests and repairs between the
+    // collections restage their own inputs
+    const size_t b_m = (size_t)nwork * sizeof(pf_miss);
+    if (int rc = ctx->d_rep_buf.reserve(b_m + 4)) return rc;
+    pf_miss *d_miss = (pf_miss *)ctx->d_rep_buf.p;
+    uint32_t *d_cnt = (uint32_t *)(ctx->d_rep_buf + b_m);
     MapView m;
     m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
     m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
@@ -2392,7 +2398,6 @@ extern "C" int pfnav_pool_repair(pfnav_ctx *ctx, int *out_nrequests, int *out_nr
             nrep++;
         }
     }
-    cudaFree(d_miss); cudaFree(d_cnt);
     if (rc) return rc;
     if (nrep) ctx->goal_batch.valid = false;      // pool bytes changed under a resident plan
     if (out_nrequests) *out_nrequests = nreq;

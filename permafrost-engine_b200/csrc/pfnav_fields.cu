@@ -1611,26 +1611,20 @@ extern "C" int pfnav_flow_fields_update(pfnav_ctx *ctx, const pfnav_field_req *r
     int rc = validate_field_reqs(ctx, reqs, n);
     if (rc) return rc;
     PF_CUDA(cudaSetDevice(ctx->device));
-    pfnav_field_req *d_reqs = nullptr;
-    uint8_t *d_fields = nullptr;
-    PF_CUDA(cudaMalloc(&d_reqs, n * sizeof(pfnav_field_req)));
-    if (cudaMalloc(&d_fields, n * 4096) != cudaSuccess) { cudaFree(d_reqs); pfnav_set_error("cudaMalloc fields"); return PFNAV_ERR_NOMEM; }
     cudaStream_t st = ctx->tick_stream;
+    // staged: the requests, then the fields, which go up only when a request updates its field in place
     bool need_in = false;
     for (size_t i = 0; i < n; i++) need_in |= (reqs[i].init == 0);
-    cudaError_t e = cudaMemcpyAsync(d_reqs, reqs, n * sizeof(pfnav_field_req), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && need_in) e = cudaMemcpyAsync(d_fields, inout_fields, n * 4096, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        rc = pfnav_flow_fields_update_dev(ctx, d_reqs, n, d_fields, st);
-        if (rc == 0) e = cudaMemcpyAsync(inout_fields, d_fields, n * 4096, cudaMemcpyDeviceToHost, st);
-    }
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_reqs); cudaFree(d_fields);
-    if (rc) return rc;
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("pfnav_flow_fields_update: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
+    const size_t b_req = n * sizeof(pfnav_field_req), a_f = (b_req + 15) & ~(size_t)15, b_f = n * 4096;
+    pf_stage S;
+    if ((rc = pf_stage_begin(ctx, st, need_in ? a_f + b_f : b_req, a_f + b_f, false, &S))) return rc;
+    memcpy(S.host, reqs, b_req);
+    if (need_in) memcpy(S.host + a_f, inout_fields, b_f);
+    if ((rc = pf_stage_upload(ctx, st, S, need_in ? a_f + b_f : b_req))) return rc;
+    if ((rc = pfnav_flow_launch(ctx, (const pfnav_field_req *)S.dev, n, S.dev + a_f, nullptr, st))) return rc;
+    PF_CUDA(cudaMemcpyAsync(inout_fields, S.dev + a_f, b_f, cudaMemcpyDeviceToHost, st));
+    if ((rc = pf_stage_done(ctx, st))) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 
@@ -1719,9 +1713,6 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
     PF_NEED_DEVICE(ctx);
     if (n == 0) return PFNAV_OK;
     PF_ARG(reqs && out_fields, "null buffer");
-    // requests go to the device in dependency order (pfnav_waves_host.h); caller-held previous fields ride in extra
-    // slots behind the n outputs and are named like pool slots (-2)
-    pf_wave_pack W;
     std::vector<size_t> inplace;
     for (size_t i = 0; i < n; i++) {
         const pfnav_los_req &q = reqs[i];
@@ -1736,40 +1727,35 @@ extern "C" int pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs
         else if (q.prev_index == PFNAV_LOS_PREV_INPLACE) {
             // N_LOSFieldCreate(..., prev) with a caller-held previous field: its bytes arrive in out_fields[i]
             PF_ARG(abs(q.prev_chunk_r - q.chunk_r) + abs(q.prev_chunk_c - q.chunk_c) == 1, "los req: prev chunk must be adjacent");
-            W.los_kept(q, 0, (int32_t)(n + inplace.size()));
             inplace.push_back(i);
-            continue;
         } else {
             PF_ARG(q.prev_index >= 0 && (size_t)q.prev_index < i, "los req: prev_index must name an earlier request");
             PF_ARG(abs(q.prev_chunk_r - q.chunk_r) + abs(q.prev_chunk_c - q.chunk_c) == 1, "los req: prev chunk must be adjacent");
         }
-        W.los(q, 0);
     }
-    std::vector<uint8_t> packed(W.layout());
-    W.pack(packed.data());
+    // requests go to the device in dependency order (pfnav_waves_host.h). Staged: the packed requests, then the field
+    // blocks: the caller-held previous fields first, named like pool slots (-2), then request i's output in block k + i
+    const size_t k = inplace.size();
+    pf_wave_pack W;
+    for (size_t i = 0, j = 0; i < n; i++) {
+        if (j < k && inplace[j] == i) W.los_kept(reqs[i], (int32_t)(k + i), (int32_t)j++);
+        else W.los(reqs[i], (int32_t)(k + i));
+    }
+    const size_t a_f = W.layout(), b_in = a_f + k * 4096;
     PF_CUDA(cudaSetDevice(ctx->device));
-    pfnav_los_req *d_reqs = nullptr;
-    uint8_t *d_fields = nullptr;
-    PF_CUDA(cudaMalloc(&d_reqs, n * sizeof(pfnav_los_req)));
-    if (cudaMalloc(&d_fields, (n + inplace.size()) * 4096) != cudaSuccess) { cudaFree(d_reqs); pfnav_set_error("cudaMalloc fields"); return PFNAV_ERR_NOMEM; }
     cudaStream_t st = ctx->tick_stream;
-    std::vector<uint8_t> tmp(n * 4096);
-    cudaError_t e = cudaMemcpyAsync(d_reqs, packed.data() + W.out.o_lr, n * sizeof(pfnav_los_req), cudaMemcpyHostToDevice, st);
-    for (size_t j = 0; j < inplace.size() && e == cudaSuccess; j++)
-        e = cudaMemcpyAsync(d_fields + (n + j) * 4096, out_fields + inplace[j] * 4096, 4096, cudaMemcpyHostToDevice, st);
-    int rc = 0;
-    if (e == cudaSuccess) {
-        rc = pfnav_los_launch(ctx, d_reqs, n, d_fields, nullptr, st);
-        if (rc == 0) e = cudaMemcpyAsync(tmp.data(), d_fields, n * 4096, cudaMemcpyDeviceToHost, st);
-    }
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_reqs); cudaFree(d_fields);
+    pf_stage S;
+    int rc = pf_stage_begin(ctx, st, b_in, b_in + n * 4096, false, &S);
     if (rc) return rc;
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("pfnav_los_fields_create: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
-    for (size_t i = 0; i < n; i++) memcpy(out_fields + i * 4096, tmp.data() + (size_t)W.lpos[i] * 4096, 4096);
+    W.pack(S.host);
+    for (size_t j = 0; j < k; j++) memcpy(S.host + a_f + j * 4096, out_fields + inplace[j] * 4096, 4096);
+    if ((rc = pf_stage_upload(ctx, st, S, b_in))) return rc;
+    if ((rc = pfnav_los_launch(ctx, (const pfnav_los_req *)(S.dev + W.out.o_lr), n, S.dev + a_f,
+                               (const int32_t *)(S.dev + W.out.o_ls), st)))
+        return rc;
+    PF_CUDA(cudaMemcpyAsync(out_fields, S.dev + b_in, n * 4096, cudaMemcpyDeviceToHost, st));
+    if ((rc = pf_stage_done(ctx, st))) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 

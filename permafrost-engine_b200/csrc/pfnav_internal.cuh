@@ -233,7 +233,8 @@ struct pfnav_ctx {
     // scratch of the goal planner
     void *stager = nullptr;
     void *planner = nullptr;
-    // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand
+    // pfnav_pool_repair_batch (pfnav_agents.cu): misses, representatives, their hash table and the gather, grown on demand;
+    // the serial pfnav_pool_repair keeps its misses here too
     pf_dbuf<uint8_t> d_rep_buf;
     int repair_stats[6] = {0, 0, 0, 0, 0, 0};                  // the last call: representatives per phase, rounds ended per rule
     // blocking table of pfnav_agents_upload_blocking (uid order, blocking_n records, of which the own range
@@ -376,7 +377,8 @@ int pf_pool_stage_table(pfnav_ctx *ctx, uint8_t *host, cudaStream_t st);
 void pf_planner_destroy(pfnav_ctx *ctx);                         // pfnav_plan.cu: join the goal planner threads
 
 // ---- pfnav_plan.cu: request staging. A batch built on the host goes through the next of two pinned buffers into the
-// context's one device buffer, which the batch's kernels then read.
+// context's one device buffer, which the batch's kernels then read. The blocking calls on host arrays (pfnav_flow_fields_update
+// and the like) also write their outputs behind their inputs there and copy them back before they return.
 //   pf_stage_begin  S->host: host_bytes, then the pool's slot table and `has` bytes when `table`, once the copy that last
 //                   read the pinned buffer is done. S->dev: dev_bytes (none when 0), with `st` ordered after the buffer's
 //                   last readers: the forked field work (pf_fields_join) and the stream-ordered reader that called

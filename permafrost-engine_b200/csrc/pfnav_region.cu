@@ -112,28 +112,24 @@ extern "C" int pfnav_region_fields(pfnav_ctx *ctx, int dim, const pfnav_region_r
     const size_t fbytes = (size_t)dim * dim / 2;
     bool need_in = false;
     for (size_t i = 0; i < n; i++) need_in |= !(reqs[i].flags & PFNAV_REGION_CREATE);
-    const size_t b_req = n * sizeof(pfnav_region_req), b_seed = std::max<size_t>(nseeds, 1) * 8, b_ov = std::max<size_t>(noverlay, 1) * 8;
-    uint8_t *d_buf = nullptr, *d_fields = nullptr;
-    PF_CUDA(cudaMalloc(&d_buf, b_req + b_seed + b_ov));
-    if (cudaMalloc(&d_fields, n * fbytes) != cudaSuccess) { cudaFree(d_buf); pfnav_set_error("cudaMalloc region fields"); return PFNAV_ERR_NOMEM; }
-    pfnav_region_req *d_reqs = reinterpret_cast<pfnav_region_req *>(d_buf);
-    int32_t *d_seeds = reinterpret_cast<int32_t *>(d_buf + b_req), *d_ov = reinterpret_cast<int32_t *>(d_buf + b_req + b_seed);
+    // staged: requests, seeds, overlay, then the fields, which go up only when a request fixes up its field in place
+    const size_t b_req = n * sizeof(pfnav_region_req), b_f = n * fbytes;
+    const size_t a_seed = (b_req + 15) & ~(size_t)15, a_ov = a_seed + nseeds * 8, a_f = (a_ov + noverlay * 8 + 15) & ~(size_t)15;
+    const size_t b_in = need_in ? a_f + b_f : a_f;
     cudaStream_t st = ctx->tick_stream;
-    cudaError_t e = cudaMemcpyAsync(d_reqs, reqs, b_req, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && nseeds) e = cudaMemcpyAsync(d_seeds, seeds_rc, nseeds * 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && noverlay) e = cudaMemcpyAsync(d_ov, overlay_rc, noverlay * 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && need_in) e = cudaMemcpyAsync(d_fields, inout_fields, n * fbytes, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        rc = region_launch(ctx, dim, d_reqs, n, d_seeds, d_ov, d_fields, st);
-        if (rc == 0) e = cudaMemcpyAsync(inout_fields, d_fields, n * fbytes, cudaMemcpyDeviceToHost, st);
-    }
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_buf); cudaFree(d_fields);
-    if (rc) return rc;
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("pfnav_region_fields: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
+    pf_stage S;
+    if ((rc = pf_stage_begin(ctx, st, b_in, a_f + b_f, false, &S))) return rc;
+    memcpy(S.host, reqs, b_req);
+    if (nseeds) memcpy(S.host + a_seed, seeds_rc, nseeds * 8);
+    if (noverlay) memcpy(S.host + a_ov, overlay_rc, noverlay * 8);
+    if (need_in) memcpy(S.host + a_f, inout_fields, b_f);
+    if ((rc = pf_stage_upload(ctx, st, S, b_in))) return rc;
+    if ((rc = region_launch(ctx, dim, (const pfnav_region_req *)S.dev, n, (const int32_t *)(S.dev + a_seed),
+                            (const int32_t *)(S.dev + a_ov), S.dev + a_f, st)))
+        return rc;
+    PF_CUDA(cudaMemcpyAsync(inout_fields, S.dev + a_f, b_f, cudaMemcpyDeviceToHost, st));
+    if ((rc = pf_stage_done(ctx, st))) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 
@@ -350,36 +346,34 @@ static int zone_dim(const pfnav_ctx *ctx, int *out_dim)
     return PFNAV_ERR_ARG;
 }
 
-// Padded-chunk fields from per-chunk seed lists (seed_off[i] .. seed_off[i + 1] pairs of chunk i); d_out = n x 4096
-// direction bytes. Shared by the zone, entity and enemies targets (field_update_zone / _entity / _enemies).
-static int chunk_fields_launch(pfnav_ctx *ctx, int layer, int dim, const int32_t *chunks_rc, size_t n, const std::vector<int32_t> &seeds,
-                               const std::vector<size_t> &seed_off, uint8_t *d_out, cudaStream_t st)
+// Padded-chunk fields from per-chunk seed lists (seed_off[i] .. seed_off[i + 1] pairs of chunk i) into out_fields, n x 4096
+// direction bytes on the host; blocking. Shared by the host-array zone and entity / enemies calls (field_update_zone /
+// _entity / _enemies).
+static int chunk_fields(pfnav_ctx *ctx, int layer, int dim, const int32_t *chunks_rc, size_t n, const std::vector<int32_t> &seeds,
+                        const std::vector<size_t> &seed_off, uint8_t *out_fields)
 {
-    std::vector<pfnav_region_req> reqs(n);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->tick_stream;
+    // staged: the requests, their seeds, then the fields
+    const size_t b_req = n * sizeof(pfnav_region_req), a_seed = (b_req + 15) & ~(size_t)15;
+    const size_t a_f = (a_seed + seeds.size() * 4 + 15) & ~(size_t)15;
+    pf_stage S;
+    int rc = pf_stage_begin(ctx, st, a_f, a_f + n * 4096, false, &S);
+    if (rc) return rc;
     for (size_t i = 0; i < n; i++) {
         pfnav_region_req q = {};
         q.layer = layer; q.center_r = chunks_rc[2 * i]; q.center_c = chunks_rc[2 * i + 1];
         q.seed_off = (int32_t)seed_off[i]; q.seed_n = (int32_t)(seed_off[i + 1] - seed_off[i]);
         q.flags = PFNAV_REGION_CREATE;
-        reqs[i] = q;
+        memcpy(S.host + i * sizeof(pfnav_region_req), &q, sizeof(q));
     }
-    const size_t b_req = n * sizeof(pfnav_region_req), b_seed = std::max<size_t>(seeds.size(), 2) * 4;
-    uint8_t *d_buf = nullptr;
-    PF_CUDA(cudaMalloc(&d_buf, b_req + b_seed + 8));
-    int rc = PFNAV_OK;
-    cudaError_t e = cudaMemcpyAsync(d_buf, reqs.data(), b_req, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && !seeds.empty()) e = cudaMemcpyAsync(d_buf + b_req, seeds.data(), seeds.size() * 4, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess)
-        rc = region_launch(ctx, dim, reinterpret_cast<const pfnav_region_req *>(d_buf), n, reinterpret_cast<const int32_t *>(d_buf + b_req),
-                           reinterpret_cast<const int32_t *>(d_buf + b_req + b_seed), d_out, st, 1);
-    // the staging buffer is read by the kernel: free it once the stream has passed it
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_buf);
-    if (rc) return rc;
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("chunk fields: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
+    memcpy(S.host + a_seed, seeds.data(), seeds.size() * 4);
+    if ((rc = pf_stage_upload(ctx, st, S, a_f))) return rc;
+    const int32_t *d_seeds = (const int32_t *)(S.dev + a_seed);
+    if ((rc = region_launch(ctx, dim, (const pfnav_region_req *)S.dev, n, d_seeds, d_seeds, S.dev + a_f, st, 1))) return rc;
+    PF_CUDA(cudaMemcpyAsync(out_fields, S.dev + a_f, n * 4096, cudaMemcpyDeviceToHost, st));
+    if ((rc = pf_stage_done(ctx, st))) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 
@@ -390,10 +384,17 @@ static inline void chunk_region_base(int dim, int cr, int cc, int *base_r, int *
     *base_c = (cc > 0 && dim > 64) ? cc * 64 - 32 : cc * 64;
 }
 
-// zone seeds of every requested chunk + the device launch
-static int zone_fields_launch(pfnav_ctx *ctx, int layer, int centre_r, int centre_c, int radius, const int32_t *chunks_rc, size_t n,
-                              uint8_t *d_out, cudaStream_t st)
+extern "C" int pfnav_zone_fields(pfnav_ctx *ctx, int layer, int centre_r, int centre_c, int radius, const int32_t *chunks_rc,
+                                 size_t n, uint8_t *out_fields)
 {
+    PF_ARG(ctx && ctx->d_cost, "map not created");
+    PF_NEED_DEVICE(ctx);
+    if (n == 0) return PFNAV_OK;
+    PF_ARG(chunks_rc && out_fields, "null buffer");
+    PF_ARG(layer >= 0 && layer < ctx->nlayers, "layer");
+    PF_ARG(centre_r >= 0 && centre_r < ctx->H64 && centre_c >= 0 && centre_c < ctx->W64, "zone centre outside the map");
+    PF_ARG(radius >= 0 && radius <= 0xFFFF, "radius");
+    PF_ARG(n < (1u << 24), "n");
     int dim = 0;
     int rc = zone_dim(ctx, &dim);
     if (rc) return rc;
@@ -411,29 +412,7 @@ static int zone_fields_launch(pfnav_ctx *ctx, int layer, int centre_r, int centr
         zone_initial_frontier(zm, centre_r, centre_c, base_r, base_c, dim, budget, seeds);
         off[i + 1] = seeds.size() / 2;
     }
-    return chunk_fields_launch(ctx, layer, dim, chunks_rc, n, seeds, off, d_out, st);
-}
-
-extern "C" int pfnav_zone_fields(pfnav_ctx *ctx, int layer, int centre_r, int centre_c, int radius, const int32_t *chunks_rc,
-                                 size_t n, uint8_t *out_fields)
-{
-    PF_ARG(ctx && ctx->d_cost, "map not created");
-    PF_NEED_DEVICE(ctx);
-    if (n == 0) return PFNAV_OK;
-    PF_ARG(chunks_rc && out_fields, "null buffer");
-    PF_ARG(layer >= 0 && layer < ctx->nlayers, "layer");
-    PF_ARG(centre_r >= 0 && centre_r < ctx->H64 && centre_c >= 0 && centre_c < ctx->W64, "zone centre outside the map");
-    PF_ARG(radius >= 0 && radius <= 0xFFFF, "radius");
-    PF_ARG(n < (1u << 24), "n");
-    PF_CUDA(cudaSetDevice(ctx->device));
-    uint8_t *d_out = nullptr;
-    PF_CUDA(cudaMalloc(&d_out, n * 4096));
-    int rc = zone_fields_launch(ctx, layer, centre_r, centre_c, radius, chunks_rc, n, d_out, ctx->tick_stream);
-    if (rc == 0 && cudaMemcpy(out_fields, d_out, n * 4096, cudaMemcpyDeviceToHost) != cudaSuccess) {
-        pfnav_set_error("pfnav_zone_fields: copy back failed"); rc = PFNAV_ERR_CUDA;
-    }
-    cudaFree(d_out);
-    return rc;
+    return chunk_fields(ctx, layer, dim, chunks_rc, n, seeds, off, out_fields);
 }
 
 // the pool entries a zone batch changed: slot table entries fresh[2i] = fresh[2i + 1], `has` bytes has[slot[i]] = hasv[i]
@@ -686,28 +665,25 @@ extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const floa
     PF_ARG(radius >= 0 && radius <= 0xFFFF, "radius");
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
-    PF_CUDA(pf_pool_refresh(ctx, ctx->tick_stream));
-    uint8_t *d_buf = nullptr;
-    PF_CUDA(cudaMalloc(&d_buf, n * 17));
-    float2 *d_pos = reinterpret_cast<float2 *>(d_buf), *d_vel = d_pos + n;
-    uint8_t *d_fl = d_buf + n * 16;
     cudaStream_t st = ctx->tick_stream;
+    PF_CUDA(pf_pool_refresh(ctx, st));
+    // staged: the positions, then the velocities and the flags
+    pf_stage S;
+    if (int rc = pf_stage_begin(ctx, st, n * 8, n * 17, false, &S)) return rc;
+    memcpy(S.host, pos_xz, n * 8);
+    if (int rc = pf_stage_upload(ctx, st, S, n * 8)) return rc;
+    const float2 *d_pos = (const float2 *)S.dev;
+    float2 *d_vel = (float2 *)(S.dev + n * 8);
+    uint8_t *d_fl = S.dev + n * 16;
     ZoneView z = { ctx->pool.d_slot, ctx->pool.d_flow, ctx->pool.d_has, ctx->chunk_w, ctx->chunk_h,
                    ctx->map_x, ctx->map_z };
-    cudaError_t e = cudaMemcpyAsync(d_pos, pos_xz, n * 8, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        k_group_arrival_velocity<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(z, dest, centre_xz[0], centre_xz[1], radius, d_pos, (int)n, d_vel, d_fl);
-        ctx->launches++;
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_vel, d_vel, n * 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_flags, d_fl, n, cudaMemcpyDeviceToHost, st);
-    cudaError_t e2 = cudaStreamSynchronize(st);
-    cudaFree(d_buf);
-    if (e != cudaSuccess || e2 != cudaSuccess) {
-        pfnav_set_error("pfnav_group_arrival_velocity: %s", cudaGetErrorString(e != cudaSuccess ? e : e2));
-        return PFNAV_ERR_CUDA;
-    }
+    k_group_arrival_velocity<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(z, dest, centre_xz[0], centre_xz[1], radius, d_pos, (int)n, d_vel, d_fl);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    PF_CUDA(cudaMemcpyAsync(out_vel, d_vel, n * 8, cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaMemcpyAsync(out_flags, d_fl, n, cudaMemcpyDeviceToHost, st));
+    if (int rc = pf_stage_done(ctx, st)) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
 }
 
@@ -852,15 +828,7 @@ extern "C" int pfnav_entity_fields(pfnav_ctx *ctx, int layer, int ref_layer, int
         if (rc) return rc;
         off[i + 1] = seeds.size() / 2;
     }
-    PF_CUDA(cudaSetDevice(ctx->device));
-    uint8_t *d_out = nullptr;
-    PF_CUDA(cudaMalloc(&d_out, n * 4096));
-    rc = chunk_fields_launch(ctx, layer, dim, chunks_rc, n, seeds, off, d_out, ctx->tick_stream);
-    if (rc == 0 && cudaMemcpy(out_fields, d_out, n * 4096, cudaMemcpyDeviceToHost) != cudaSuccess) {
-        pfnav_set_error("pfnav_entity_fields: copy back failed"); rc = PFNAV_ERR_CUDA;
-    }
-    cudaFree(d_out);
-    return rc;
+    return chunk_fields(ctx, layer, dim, chunks_rc, n, seeds, off, out_fields);
 }
 
 
