@@ -760,6 +760,9 @@ typedef struct pfnav_movestate_ext {
 } pfnav_movestate_ext;
 /* HOST array, own range, uid order. Optional: zero / NULL_UID defaults. */
 int  pfnav_agents_upload_movestate_ext(pfnav_ctx *ctx, const pfnav_movestate_ext *ms, size_t n);
+/* Inspection: read the own range's movestate_ext table back (at most maxout records; waits for the device).
+ * PFNAV_ERR_ARG when no table was uploaded. */
+int  pfnav_agents_read_movestate_ext(pfnav_ctx *ctx, pfnav_movestate_ext *out, size_t maxout);
 
 /* enum movestate_flags (movement.c:226-242), same bit values */
 #define PFNAV_UPDATE_SET_STATE        (1u << 0)
@@ -964,6 +967,42 @@ typedef struct pfnav_agent_delta {
  *   (pfnav_mgpu_init / pfnav_group_create, or an own range that is not the whole population). */
 int  pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n,
                            const pfnav_flock *flocks, size_t nflocks, void *stream);
+/* Units produced and units that die: remove entities from the device-resident population and append new ones.
+ * - Numbering: a stable compaction followed by an append. remove_uids name entities of the population before the call
+ *   (each < n_agents; a repeated uid is removed once). Survivor u gets the uid u - |{removed r < u}|, so survivors keep
+ *   their order; appended entity k (add[k]) gets n_keep + k. There is no remap output: the engine updates its own
+ *   uid -> index map with the same rule.
+ * - Equivalence: afterwards every device table and host fact equals what reading the population back, deleting the
+ *   removed rows, appending the new ones and uploading the result would leave (pfnav_agents_upload + _upload_movestate +
+ *   _upload_movestate_ext + _upload_formation + _upload_blocking, for whichever tables exist): agents, neighbour records,
+ *   movestate, movestate_ext, formation and blocking tables, the flock table and member lists, the largest radius, any
+ *   GARRISONED, the (flock, layer) pairs in use and the arrival constants' invalidation. Beyond a re-upload:
+ *     - every removed entity that holds a block (blocking record) queues the unblock op pfnav_agents_set_blocking(uid, 0)
+ *       would queue, decided before the compaction; the next pfnav_map_commit applies it;
+ *     - a survivor's movestate_ext.surround_target_uid is renumbered; a removed target becomes PFNAV_NULL_UID.
+ * - Appended records: add_ms is required exactly when a movestate table was uploaded, add_blocking exactly when a
+ *   blocking table covers the population (its records describe blocks already counted and queue no op: a new stationary
+ *   unit takes its block with pfnav_agents_set_blocking after the call). add_ext and add_formation may be NULL where
+ *   their table exists: defaults (ext zeroed with surround_target_uid = PFNAV_NULL_UID and rot = {0, 0, 0, 1}; formation
+ *   zeroed: no formation). Appended ext targets name uids after the call. Records for a table that was never uploaded
+ *   are refused.
+ * - flocks == NULL keeps the flock table; otherwise flocks[0 .. nflocks) is the whole new table, as in
+ *   pfnav_agents_commands; a table that would leave a surviving or appended entity with a dropped flock index is refused.
+ * - Everything is validated before anything changes: remove uids in range, the upload's checks of appended agents
+ *   (flock index within the table after the call, navigation layer created) and blocking records, finite floats,
+ *   appended ext targets < the new population or PFNAV_NULL_UID. Failure: PFNAV_ERR_ARG, device and host state untouched.
+ *   No removal, no addition and no table: nothing happens.
+ * - The spatial index is rebuilt for the new population; the work list is emptied (follow with pfnav_agents_set_work_dev).
+ * - Asynchronous on `stream`. It waits for the stream to read the new flock offsets and 8 bytes of population facts, and
+ *   4 bytes more when removals may change whether any blocking record names a faction; it waits for the device when a
+ *   per-entity buffer or the call's scratch regrows. Shares the scratch of pfnav_agents_commands and
+ *   pfnav_agents_set_work_dev: order them on one stream. Input arrays are read before the call returns.
+ * - PFNAV_ERR_NO_DEVICE on a host-only context. PFNAV_ERR_STATE (nothing changed) on a context in a multi-GPU job, as
+ *   for pfnav_agents_commands. */
+int  pfnav_agents_change_population(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove,
+                                    const pfnav_agent *add, const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                    const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking, size_t nadd,
+                                    const pfnav_flock *flocks, size_t nflocks, void *stream);
 /* pfnav_agents_commands for a whole multi-GPU job. Every rank calls the NCCL form with the same arguments, the job's
  * whole batch (uids global, in [0, n_total)); the group form is called once. Delta format, masks and the flock-table
  * rule are those of pfnav_agents_commands.

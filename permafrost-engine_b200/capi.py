@@ -132,6 +132,7 @@ SYMBOLS = [
     "pfnav_group_request_entity_fields_batch",
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
     "pfnav_mgpu_commands", "pfnav_group_commands",
+    "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
 ]
 
 _lib = None
@@ -206,6 +207,9 @@ def load():
     L.pfnav_group_commands.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
     L.pfnav_agents_set_work_dev.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_size_t)]
     L.pfnav_agents_read_work.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.pfnav_agents_change_population.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_agents_read_movestate_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.pfnav_map_refresh_chunk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
@@ -980,6 +984,31 @@ class Nav:
         """collective: agents_commands for the whole job -- every rank passes the job's whole batch (global uids) and
         the same table; all or nothing across the ranks. Follow with mgpu_gather."""
         _chk(self.L.pfnav_mgpu_commands(self.h, *_command_args(deltas, flocks), C.c_void_p(stream)))
+
+    def agents_change_population(self, remove, add, ms=None, ext=None, formation=None, blocking=None, flocks=None, stream=0):
+        """pfnav_agents_change_population: remove the uids `remove` (numbering before the call; repeats removed once) and
+        append the AGENT records `add`, with their MOVESTATE / MOVESTATE_EXT / FORMATION_IN / BLOCKING records (None: no
+        records; ext and formation then take the defaults). Survivors keep their order and are renumbered densely, the
+        appended entities follow. flocks (FLOCK records): the whole new flock table, None: unchanged. The work list is
+        emptied: follow with agents_set_work_dev."""
+        rm = np.ascontiguousarray(remove if remove is not None else [], np.uint32).reshape(-1)
+        add = np.ascontiguousarray(add if add is not None else np.zeros(0, AGENT), AGENT).reshape(-1)
+        recs = [None if r is None else np.ascontiguousarray(r, dt).reshape(-1)
+                for r, dt in ((ms, MOVESTATE), (ext, MOVESTATE_EXT), (formation, FORMATION_IN), (blocking, BLOCKING))]
+        for r in recs:
+            assert r is None or len(r) == len(add)
+        fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
+        ptr = lambda a: _p(a) if a is not None and len(a) else None
+        _chk(self.L.pfnav_agents_change_population(self.h, ptr(rm), len(rm), ptr(add), *[ptr(r) for r in recs], len(add),
+                                                   _p(fl) if fl is not None else None, 0 if fl is None else len(fl),
+                                                   C.c_void_p(stream)))
+        self.nagents = getattr(self, "nagents", 0) - len(np.unique(rm)) + len(add)
+        self.nwork = 0
+
+    def agents_read_movestate_ext(self, n):
+        out = np.zeros(n, MOVESTATE_EXT)
+        _chk(self.L.pfnav_agents_read_movestate_ext(self.h, _p(out) if n else None, n))
+        return out
 
     def agents_set_work_dev(self, stream=0):
         """pfnav_agents_set_work_dev: agents_set_work(None) built on the device -> the number of work items"""

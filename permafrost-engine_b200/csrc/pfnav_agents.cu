@@ -968,7 +968,7 @@ static GridView grid_of(const pfnav_ctx *ctx)
     return g;
 }
 
-static int build_index(pfnav_ctx *ctx, cudaStream_t st)
+int build_index(pfnav_ctx *ctx, cudaStream_t st)
 {
     const int n = (int)ctx->n_agents;
     const int ncells = ctx->grid_w * ctx->grid_h;
@@ -1088,12 +1088,10 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
         ctx->has_unsupported_state = false;
         ctx->cmd_mirror.reset(hi - lo, nflocks);      // (flock, layer) per own entity, for pfnav_agents_commands
         for (size_t i = 0; i < hi - lo; i++) {
-            PF_ARG(agents[i].flock < (int)nflocks, "agent flock index out of range");
             // Entity_NavLayerWithRadius (entity.c:554): the layer this agent's tile probes read
-            const uint32_t f = agents[i].flags; const float r = agents[i].radius;
-            const int base = (f & PFNAV_FLAG_WATER) ? 4 : (f & PFNAV_FLAG_AIR) ? 8 : 0;
-            const int layer = base + (r >= 15.0f ? 3 : r >= 10.0f ? 2 : r >= 5.0f ? 1 : 0);
-            PF_ARG(layer < ctx->nlayers, "agent needs a navigation layer that was not created (radius/flags)");
+            int layer;
+            const char *err = pf_agent_check(agents[i], nflocks, ctx->nlayers, &layer);
+            PF_ARG(!err, err);
             if (agents[i].flock >= 0) ctx->flock_layer_used[(size_t)agents[i].flock * PFNAV_NAV_LAYER_MAX + layer] = 1;
             ctx->cmd_mirror.set(i, std::max(agents[i].flock, -1), layer);
             const uint32_t stt = agents[i].state;
@@ -1928,7 +1926,7 @@ static int blocking_check(pfnav_ctx *ctx, bool need_records)
     return PFNAV_OK;
 }
 
-static int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n, const pfnav_patch *d_patches, int mode)
+int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n, const pfnav_patch *d_patches, int mode)
 {
     pf_op_stage s;
     int rc = pf_blocker_ops_stage(ctx, (size_t)n, &s);
@@ -1949,8 +1947,8 @@ extern "C" int pfnav_agents_upload_blocking(pfnav_ctx *ctx, const pfnav_blocking
     PF_ARG(n == ctx->shard_hi - ctx->shard_lo, "one blocking record per uploaded agent (of this context's own range)");
     bool any_fac = false;
     for (size_t i = 0; i < n; i++) {
-        PF_ARG(b[i].blocking <= 1, "blocking must be 0 or 1");
-        PF_ARG(b[i].faction_id >= 0 && b[i].faction_id <= 15, "faction_id must lie in 0..15");
+        const char *err = pf_blocking_check(b[i]);
+        PF_ARG(!err, err);
         any_fac |= b[i].faction_id < 15;
     }
     PF_CUDA(cudaSetDevice(ctx->device));
@@ -2024,6 +2022,19 @@ extern "C" int pfnav_agents_upload_movestate_ext(pfnav_ctx *ctx, const pfnav_mov
     PF_CUDA(cudaSetDevice(ctx->device));
     if (int rc = ctx->d_ms_ext.reserve(ctx->n_agents)) return rc;
     PF_CUDA(cudaMemcpy(ctx->d_ms_ext + ctx->shard_lo, ms, n * sizeof(pfnav_movestate_ext), cudaMemcpyHostToDevice));
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_agents_read_movestate_ext(pfnav_ctx *ctx, pfnav_movestate_ext *out, size_t maxout)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_agents && ctx->d_ms_ext, "no movestate_ext table uploaded");
+    PF_ARG(out || maxout == 0, "out == NULL");
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(cudaDeviceSynchronize());
+    const size_t n = std::min(maxout, ctx->shard_hi - ctx->shard_lo);       // this context's own entity range
+    if (n) PF_CUDA(cudaMemcpy(out, ctx->d_ms_ext + ctx->shard_lo, n * sizeof(pfnav_movestate_ext), cudaMemcpyDeviceToHost));
     return PFNAV_OK;
 }
 

@@ -9,6 +9,9 @@
 // deltas of its own uids as above, and for the others the flock id, radius and flag bits (k_apply_foreign), so that it
 // rebuilds the member lists and population facts from its own complete columns.
 // pfnav_agents_set_work_dev compacts the uids that are not still into the work list, in uid order.
+// pfnav_agents_change_population removes and appends entities (pfnav_commands_host.h plans the batch and holds the
+// numbering rule): k_pop_gather writes every new row of every table with one thread per row, then the member lists,
+// population facts and spatial index are rebuilt for the new population.
 #include "pfnav_internal.cuh"
 #include <algorithm>
 
@@ -190,6 +193,70 @@ __global__ void __launch_bounds__(1024) k_work_compact(const pf_record *__restri
     }
 }
 
+// ---- population change: new rows [row0, n_new) of every table, by the numbering rule of pf_pop_source ----
+// Rows below n_keep are survivors, gathered from the tables as they were (surround targets renumbered); rows from n_keep
+// on are the appended records, or the defaults the tick uses for a missing table. o_ms / o_ext / o_form / o_blk are null
+// for a table that does not exist; a_ext / a_form null for defaults.
+struct pf_pop_gather {
+    const pfnav_agent *agents; const pfnav_movestate *ms; const pfnav_movestate_ext *ext;
+    const pfnav_formation_in *form; const pfnav_blocking *blk;
+    const pfnav_agent *a_agents; const pfnav_movestate *a_ms; const pfnav_movestate_ext *a_ext;
+    const pfnav_formation_in *a_form; const pfnav_blocking *a_blk;
+    pfnav_agent *o_agents; pf_record *o_rec; int32_t *o_flock; pfnav_movestate *o_ms; pfnav_movestate_ext *o_ext;
+    pfnav_formation_in *o_form; pfnav_blocking *o_blk;
+    const uint32_t *removed, *key; uint32_t R, n_old;
+    int row0, n_keep, n_new;
+    uint32_t *any_fac;           // set when a written blocking record names a faction other than 15
+};
+
+__global__ void k_pop_gather(const pf_pop_gather g)
+{
+    const int i = g.row0 + blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= g.n_new) return;
+    pfnav_agent a;
+    pfnav_blocking b;
+    if (i < g.n_keep) {
+        const uint32_t s = pf_pop_source(g.key, g.R, (uint32_t)i);
+        a = g.agents[s];
+        if (g.o_ms) g.o_ms[i] = g.ms[s];
+        if (g.o_ext) {
+            pfnav_movestate_ext x = g.ext[s];
+            if (x.surround_target_uid != PFNAV_NULL_UID)
+                x.surround_target_uid = pf_pop_renumber(g.removed, g.R, g.n_old, x.surround_target_uid);
+            g.o_ext[i] = x;
+        }
+        if (g.o_form) g.o_form[i] = g.form[s];
+        if (g.o_blk) b = g.blk[s];
+    } else {
+        const int k = i - g.n_keep;
+        a = g.a_agents[k];
+        if (g.o_ms) g.o_ms[i] = g.a_ms[k];
+        if (g.o_ext) {
+            pfnav_movestate_ext x = {};
+            if (g.a_ext) x = g.a_ext[k];
+            else { x.surround_target_uid = PFNAV_NULL_UID; x.rot[3] = 1.0f; }
+            g.o_ext[i] = x;
+        }
+        if (g.o_form) {
+            pfnav_formation_in f = {};
+            if (g.a_form) f = g.a_form[k];
+            g.o_form[i] = f;
+        }
+        if (g.o_blk) b = g.a_blk[k];
+    }
+    g.o_agents[i] = a;
+    g.o_flock[i] = a.flock;
+    pf_record r;                       // as k_make_records packs it
+    r.px = a.pos[0]; r.pz = a.pos[1]; r.vx = a.velocity[0]; r.vz = a.velocity[1];
+    r.radius = a.radius;
+    r.state_flags = (a.state << 24) | (a.flags & 0xFFFFFFu);
+    g.o_rec[i] = r;
+    if (g.o_blk) {
+        g.o_blk[i] = b;
+        if (b.faction_id < 15) *g.any_fac = 1u;
+    }
+}
+
 // ------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------
@@ -215,6 +282,15 @@ static int members_on_device(pfnav_ctx *ctx, cudaStream_t st, uint32_t *hist, in
     PF_CUDA(cudaStreamSynchronize(st));
     ctx->h_flock_start.swap(fstart);
     return 0;
+}
+
+// warps of the member sort of n entities over nflocks flocks: at most 4096 ranges of `per` uids (a multiple of 32), and at
+// most 16 M histogram words
+static void member_sort_shape(size_t n, size_t nflocks, int &per, int &W)
+{
+    const size_t max_w = std::max<size_t>(1, std::min<size_t>(4096, ((size_t)1 << 24) / std::max<size_t>(nflocks, 1)));
+    per = (int)(((n + max_w - 1) / max_w + 31) / 32 * 32);
+    W = per ? (int)((n + per - 1) / per) : 0;
 }
 
 static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_agent_delta> &merged,
@@ -257,11 +333,8 @@ static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_ag
     for (const pfnav_agent_delta &m : merged) any |= m.mask;
     for (const pf_cmd_foreign &f : foreign) any |= f.mask;
     const bool members = (any & PFNAV_DELTA_FLOCK) || nflocks != ctx->n_flocks;
-    int rc;
-    // warps of the member sort: at most 4096 ranges, and at most 16 M histogram words
-    const size_t max_w = std::max<size_t>(1, std::min<size_t>(4096, ((size_t)1 << 24) / std::max<size_t>(nflocks, 1)));
-    const int per = (int)(((ctx->n_agents + max_w - 1) / max_w + 31) / 32 * 32);
-    const int W = per ? (int)((ctx->n_agents + per - 1) / per) : 0;
+    int rc, per, W;
+    member_sort_shape(ctx->n_agents, nflocks, per, W);
     const size_t b_deltas = merged.size() * sizeof(pfnav_agent_delta), b_foreign = foreign.size() * sizeof(pf_cmd_foreign);
     if ((rc = ctx->d_cmd_buf.reserve(b_deltas + b_foreign + (members ? nflocks * (size_t)W * 4 : 0)))) return rc;
     // keeps no content: the table follows, the offsets are rebuilt (members)
@@ -297,6 +370,152 @@ static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_ag
     if (members && (rc = members_on_device(ctx, st, (uint32_t *)(ctx->d_cmd_buf + b_deltas + b_foreign), per, W))) return rc;
     if ((any & (PFNAV_DELTA_RADIUS | PFNAV_DELTA_FLAGS)) && (rc = pfnav_agents_refresh_facts(ctx, st))) return rc;
     return PFNAV_OK;
+}
+
+// Everything after validation, on `st`. The tables are gathered by k_pop_gather: in place when nothing is removed and no
+// table regrows (only the appended rows are written), otherwise into the command scratch and copied back once the tables
+// have regrown, since pf_dbuf::reserve drops the contents of a buffer it grows. Scratch: [gathered tables] [removals, keys,
+// appended records, the any-faction word]; the member sort's histogram reuses it from the start afterwards.
+static int pop_apply(pfnav_ctx *ctx, cudaStream_t st, const pf_pop_tables &T, const pf_pop_plan &P, const pfnav_agent *add,
+                     const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext, const pfnav_formation_in *add_form,
+                     const pfnav_blocking *add_blk, size_t nadd, const pfnav_flock *flocks, size_t nflocks)
+{
+    const size_t R = P.removed.size(), n_new = P.n_new;
+    const bool full = R > 0 || std::min({ctx->d_agents.cap, ctx->d_records.cap, ctx->d_flock_of.cap}) < n_new ||
+                      (T.ms && ctx->d_movestate.cap < n_new) || (T.ext && ctx->d_ms_ext.cap < n_new) ||
+                      (T.formation && ctx->d_formation.cap < n_new) || (T.blocking && ctx->d_blocking.cap < n_new);
+    size_t top = 0;
+    auto take = [&top](size_t bytes) { const size_t o = top; top += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t rows = full ? n_new : 0;
+    const size_t g_agents = take(rows * sizeof(pfnav_agent)), g_rec = take(rows * sizeof(pf_record)), g_flock = take(rows * 4);
+    const size_t g_ms = take(T.ms ? rows * sizeof(pfnav_movestate) : 0), g_ext = take(T.ext ? rows * sizeof(pfnav_movestate_ext) : 0);
+    const size_t g_form = take(T.formation ? rows * sizeof(pfnav_formation_in) : 0);
+    const size_t g_blk = take(T.blocking ? rows * sizeof(pfnav_blocking) : 0);
+    // the staged inputs, one copy from one host image
+    const size_t s0 = top;
+    const size_t s_removed = take(R * 4) - s0, s_key = take(R * 4) - s0, s_agents = take(nadd * sizeof(pfnav_agent)) - s0;
+    const size_t s_ms = take(add_ms ? nadd * sizeof(pfnav_movestate) : 0) - s0;
+    const size_t s_ext = take(add_ext ? nadd * sizeof(pfnav_movestate_ext) : 0) - s0;
+    const size_t s_form = take(add_form ? nadd * sizeof(pfnav_formation_in) : 0) - s0;
+    const size_t s_blk = take(add_blk ? nadd * sizeof(pfnav_blocking) : 0) - s0;
+    const size_t s_fac = take(4) - s0;
+    std::vector<uint8_t> h(top - s0, 0);
+    auto put = [&h](size_t off, const void *src, size_t bytes) { if (bytes) memcpy(h.data() + off, src, bytes); };
+    put(s_removed, P.removed.data(), R * 4); put(s_key, P.key.data(), R * 4);
+    put(s_agents, add, nadd * sizeof(pfnav_agent));
+    if (add_ms) put(s_ms, add_ms, nadd * sizeof(pfnav_movestate));
+    if (add_ext) put(s_ext, add_ext, nadd * sizeof(pfnav_movestate_ext));
+    if (add_form) put(s_form, add_form, nadd * sizeof(pfnav_formation_in));
+    if (add_blk) put(s_blk, add_blk, nadd * sizeof(pfnav_blocking));
+    int per, W;
+    member_sort_shape(n_new, nflocks, per, W);
+    int rc;
+    if ((rc = ctx->d_cmd_buf.reserve(std::max(top, nflocks * (size_t)W * 4)))) return rc;
+    if ((rc = pf_flocks_reserve(ctx, nflocks))) return rc;        // keeps no content: the table follows, the offsets are rebuilt
+    uint8_t *buf = ctx->d_cmd_buf.p, *stage = buf + s0;
+    PF_CUDA(cudaMemcpyAsync(stage, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+    const uint32_t *d_removed = (const uint32_t *)(stage + s_removed);
+    // the blocks of removed entities are released as pfnav_agents_set_blocking(removed, 0) would, before the compaction
+    if (T.blocking && R && (rc = blocking_emit(ctx, st, d_removed, (int)R, nullptr, 0))) return rc;
+    if (flocks) {
+        // from the context's own pageable copy, which is staged before the call returns: the caller's array may be pinned
+        ctx->h_flocks.assign(flocks, flocks + nflocks);
+        if (nflocks) PF_CUDA(cudaMemcpyAsync(ctx->d_flocks, ctx->h_flocks.data(), nflocks * sizeof(pfnav_flock), cudaMemcpyHostToDevice, st));
+    }
+    pf_pop_gather g = {};
+    g.agents = ctx->d_agents; g.ms = T.ms ? ctx->d_movestate.p : nullptr; g.ext = ctx->d_ms_ext; g.form = ctx->d_formation;
+    g.blk = T.blocking ? ctx->d_blocking.p : nullptr;
+    g.a_agents = (const pfnav_agent *)(stage + s_agents);
+    g.a_ms = add_ms ? (const pfnav_movestate *)(stage + s_ms) : nullptr;
+    g.a_ext = add_ext ? (const pfnav_movestate_ext *)(stage + s_ext) : nullptr;
+    g.a_form = add_form ? (const pfnav_formation_in *)(stage + s_form) : nullptr;
+    g.a_blk = add_blk ? (const pfnav_blocking *)(stage + s_blk) : nullptr;
+    if (full) {
+        g.o_agents = (pfnav_agent *)(buf + g_agents); g.o_rec = (pf_record *)(buf + g_rec); g.o_flock = (int32_t *)(buf + g_flock);
+        g.o_ms = T.ms ? (pfnav_movestate *)(buf + g_ms) : nullptr;
+        g.o_ext = T.ext ? (pfnav_movestate_ext *)(buf + g_ext) : nullptr;
+        g.o_form = T.formation ? (pfnav_formation_in *)(buf + g_form) : nullptr;
+        g.o_blk = T.blocking ? (pfnav_blocking *)(buf + g_blk) : nullptr;
+    } else {
+        g.o_agents = ctx->d_agents; g.o_rec = ctx->d_records; g.o_flock = ctx->d_flock_of;
+        g.o_ms = T.ms ? ctx->d_movestate.p : nullptr; g.o_ext = ctx->d_ms_ext; g.o_form = ctx->d_formation;
+        g.o_blk = T.blocking ? ctx->d_blocking.p : nullptr;
+    }
+    g.removed = d_removed; g.key = (const uint32_t *)(stage + s_key); g.R = (uint32_t)R; g.n_old = (uint32_t)P.n_old;
+    g.row0 = full ? 0 : (int)P.n_keep; g.n_keep = (int)P.n_keep; g.n_new = (int)n_new;
+    uint32_t *d_fac = (uint32_t *)(stage + s_fac);
+    g.any_fac = d_fac;
+    if (n_new > (size_t)g.row0) {
+        k_pop_gather<<<((int)n_new - g.row0 + 127) / 128, 128, 0, st>>>(g);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+    }
+    // the tables at their new length (a regrowth waits for the device, so the gather has finished), then the copy back
+    if ((rc = pf_dbuf_reserve_all(n_new, ctx->d_agents, ctx->d_records, ctx->d_flock_members, ctx->d_flock_of, ctx->d_sorted_ix,
+                                  ctx->d_sorted_iy, ctx->d_sorted_flock, ctx->d_sorted_id))) return rc;
+    if (T.ms && (rc = ctx->d_movestate.reserve(n_new))) return rc;
+    if (T.ext && (rc = ctx->d_ms_ext.reserve(n_new))) return rc;
+    if (T.formation && (rc = ctx->d_formation.reserve(n_new))) return rc;
+    if (T.blocking && (rc = ctx->d_blocking.reserve(std::max<size_t>(n_new, 1)))) { ctx->blocking_n = 0; return rc; }
+    if (full && n_new) {
+        auto back = [&](void *dst, size_t off, size_t elem) { return cudaMemcpyAsync(dst, buf + off, n_new * elem, cudaMemcpyDeviceToDevice, st); };
+        PF_CUDA(back(ctx->d_agents, g_agents, sizeof(pfnav_agent)));
+        PF_CUDA(back(ctx->d_records, g_rec, sizeof(pf_record)));
+        PF_CUDA(back(ctx->d_flock_of, g_flock, 4));
+        if (T.ms) PF_CUDA(back(ctx->d_movestate, g_ms, sizeof(pfnav_movestate)));
+        if (T.ext) PF_CUDA(back(ctx->d_ms_ext, g_ext, sizeof(pfnav_movestate_ext)));
+        if (T.formation) PF_CUDA(back(ctx->d_formation, g_form, sizeof(pfnav_formation_in)));
+        if (T.blocking) PF_CUDA(back(ctx->d_blocking, g_blk, sizeof(pfnav_blocking)));
+    }
+    // host facts, as a fresh upload of the resulting population would leave them
+    ctx->n_agents = n_new; ctx->shard_lo = 0; ctx->shard_hi = n_new; ctx->n_flocks = nflocks;
+    ctx->cmd_mirror.compact_append(P.removed, P.add_flock.data(), P.add_layer.data(), nadd, nflocks);
+    std::vector<uint8_t> used;
+    ctx->cmd_mirror.used(used);
+    if (flocks || used != ctx->flock_layer_used) ctx->arrival_valid = false;
+    ctx->flock_layer_used.swap(used);
+    ctx->n_work = 0;
+    if (T.blocking) {
+        ctx->blocking_n = n_new;
+        if (ctx->blocking_any_fac && R) {
+            // some survivor may have held the only faction other than 15: the gather, which wrote every row, tells
+            uint32_t fac = 0;
+            PF_CUDA(cudaMemcpyAsync(&fac, d_fac, 4, cudaMemcpyDeviceToHost, st));
+            PF_CUDA(cudaStreamSynchronize(st));
+            ctx->blocking_any_fac = fac != 0;
+        } else {
+            ctx->blocking_any_fac = ctx->blocking_any_fac || P.add_any_fac;
+        }
+    }
+    if ((rc = members_on_device(ctx, st, (uint32_t *)buf, per, W))) return rc;
+    if ((rc = pfnav_agents_refresh_facts(ctx, st))) return rc;
+    return build_index(ctx, st);
+}
+
+extern "C" int pfnav_agents_change_population(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove, const pfnav_agent *add,
+                                              const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                              const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking,
+                                              size_t nadd, const pfnav_flock *flocks, size_t nflocks, void *stream)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_agents, "agents not uploaded");
+    if (ctx->mgpu || ctx->shard_lo > 0 || ctx->shard_hi < ctx->n_agents) {
+        pfnav_set_error("pfnav_agents_change_population: the context is part of a multi-GPU job (a population change would "
+                        "move the other members' entity ranges)");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(nremove < (1u << 31) && nadd < (1u << 31) && nflocks < (1u << 31), "nremove / nadd / nflocks");
+    if (!flocks) nflocks = ctx->n_flocks;
+    const pf_pop_tables T = {ctx->movestate_set && ctx->d_movestate != nullptr, ctx->d_ms_ext != nullptr,
+                             ctx->d_formation != nullptr, ctx->d_blocking != nullptr && ctx->blocking_n == ctx->n_agents};
+    pf_pop_plan P;
+    const char *err = pf_pop_plan_batch(ctx->cmd_mirror, ctx->nlayers, T, remove_uids, nremove, add, add_ms, add_ext,
+                                        add_formation, add_blocking, nadd, nflocks, P);
+    PF_ARG(!err, err);
+    if (P.removed.empty() && nadd == 0 && !flocks) return PFNAV_OK;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    return pop_apply(ctx, pf_stream(ctx, stream), T, P, add, add_ms, add_ext, add_formation, add_blocking, nadd, flocks, nflocks);
 }
 
 // A job member: the whole batch is checked against the population, the own records against the member's mirror. Its

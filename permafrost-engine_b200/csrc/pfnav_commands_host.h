@@ -1,9 +1,11 @@
 // pfnav_commands_host.h -- the host side of pfnav_agents_commands and the write rule its kernel applies, CUDA-free:
 // delta validation, per-uid merging in array order, the navigation layer rule and the (flock, layer) mirror that keeps
 // flock_layer_used equal to a fresh upload's; and the split of a multi-GPU job's batch into a member's own and foreign
-// parts. tests/emu/commands_emu.cpp and tests/emu/commands_job_emu.cpp build this header with g++.
+// parts; and the validation, numbering rule and mirror update of pfnav_agents_change_population.
+// tests/emu/commands_emu.cpp, tests/emu/commands_job_emu.cpp and tests/emu/population_emu.cpp build this header with g++.
 #pragma once
 #include <math.h>
+#include <algorithm>
 #include <stdint.h>
 #include <unordered_map>
 #include <vector>
@@ -48,6 +50,25 @@ PF_HD void pf_delta_apply(pfnav_agent *a, pfnav_movestate *ms, pfnav_movestate_e
     if (clear)
         for (int i = 0; i < PFNAV_VEL_HIST_LEN; i++) { ms->vel_hist[i][0] = 0.0f; ms->vel_hist[i][1] = 0.0f; }
     if (d.mask & PFNAV_DELTA_TARGET) { ex->surround_target_uid = d.target_uid; ex->target_range = d.target_range; }
+}
+
+// The per-entity checks of an agent record that pfnav_agents_upload and pfnav_agents_change_population both make: its
+// flock index below the length of the flock table it will be read against, and its navigation layer created. *layer:
+// that layer. Returns NULL or what was wrong.
+static inline const char *pf_agent_check(const pfnav_agent &a, size_t nflocks, int nlayers, int *layer)
+{
+    if (a.flock >= (int64_t)nflocks) return "agent flock index out of range";
+    *layer = pf_layer_base(a.flags) + pf_layer_class(a.radius);
+    if (*layer >= nlayers) return "agent needs a navigation layer that was not created (radius/flags)";
+    return nullptr;
+}
+
+// pfnav_agents_upload_blocking's check of one record
+static inline const char *pf_blocking_check(const pfnav_blocking &b)
+{
+    if (b.blocking > 1) return "blocking must be 0 or 1";
+    if (b.faction_id < 0 || b.faction_id > 15) return "faction_id must lie in 0..15";
+    return nullptr;
 }
 
 struct pf_cmd_limits {
@@ -137,6 +158,27 @@ struct pf_cmd_mirror {
         out.resize(count.size());
         for (size_t k = 0; k < count.size(); k++) out[k] = count[k] ? 1 : 0;
     }
+    // pfnav_agents_change_population: drop the entities `removed` names (sorted, unique), keep the others in order, append
+    // (flock[k], layer[k]) for k < nadd, and resize the counts to a table of nflocks_new flocks, which holds every flock
+    // index left (pf_pop_plan checked it)
+    void compact_append(const std::vector<uint32_t> &removed, const int32_t *add_flock, const uint8_t *add_layer, size_t nadd,
+                        size_t nflocks_new)
+    {
+        if (nflocks_new > nflocks) count.resize(nflocks_new * PFNAV_NAV_LAYER_MAX, 0);
+        size_t w = 0, m = 0;
+        for (size_t i = 0; i < flock.size(); i++) {
+            if (m < removed.size() && removed[m] == i) {
+                if (flock[i] >= 0) count[(size_t)flock[i] * PFNAV_NAV_LAYER_MAX + layer[i]]--;
+                m++;
+                continue;
+            }
+            flock[w] = flock[i]; layer[w] = layer[i]; w++;
+        }
+        flock.resize(w + nadd); layer.resize(w + nadd);
+        for (size_t k = 0; k < nadd; k++) set(w + k, add_flock[k] < 0 ? -1 : add_flock[k], add_layer[k]);
+        count.resize(nflocks_new * PFNAV_NAV_LAYER_MAX);
+        nflocks = nflocks_new;
+    }
 };
 
 struct pf_cmd_change { uint32_t idx; int32_t flock; uint8_t layer; };     // idx: index into the own range
@@ -175,6 +217,104 @@ static inline void pf_cmd_commit(pf_cmd_mirror &M, const std::vector<pf_cmd_chan
     }
     M.count.resize(nflocks_new * PFNAV_NAV_LAYER_MAX);         // a dropped tail holds no entity (pf_cmd_plan)
     M.nflocks = nflocks_new;
+}
+
+// ---- pfnav_agents_change_population ----
+// The numbering rule is a stable compaction followed by an append: survivor u gets u - |{removed r < u}|, appended
+// entity k gets n_keep + k. removed: the removed uids, sorted and unique; key[m] = removed[m] - m, the number of
+// survivors before removed[m] (non-decreasing).
+// New row j < n_keep: the uid it had before the call, j plus the number of removals with key <= j.
+PF_HD uint32_t pf_pop_source(const uint32_t *key, uint32_t R, uint32_t j)
+{
+    uint32_t lo = 0, hi = R;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (key[mid] <= j) lo = mid + 1; else hi = mid; }
+    return j + lo;
+}
+// A uid of the population before the call (n_old entities) -> its uid after the call; PFNAV_NULL_UID when it was
+// removed or names no entity.
+PF_HD uint32_t pf_pop_renumber(const uint32_t *removed, uint32_t R, uint32_t n_old, uint32_t u)
+{
+    if (u >= n_old) return PFNAV_NULL_UID;
+    uint32_t lo = 0, hi = R;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (removed[mid] < u) lo = mid + 1; else hi = mid; }
+    return lo < R && removed[lo] == u ? PFNAV_NULL_UID : u - lo;
+}
+
+// the optional tables a population change writes (blocking: a blocking table covers the population)
+struct pf_pop_tables { bool ms, ext, formation, blocking; };
+
+struct pf_pop_plan {
+    std::vector<uint32_t> removed, key;       // sorted unique removals and their keys (pf_pop_source)
+    std::vector<int32_t> add_flock;           // flock and navigation layer of every appended entity, for the mirror
+    std::vector<uint8_t> add_layer;
+    size_t n_old = 0, n_keep = 0, n_new = 0, nflocks = 0;
+    bool add_any_fac = false;                 // an appended blocking record names a faction other than 15
+};
+
+static inline bool pf_finite(const float *p, int n)
+{
+    for (int i = 0; i < n; i++)
+        if (!isfinite(p[i])) return false;
+    return true;
+}
+
+// Validate a population change against the mirror of the population (n_old entities) and plan it, changing nothing:
+// removal uids in range (repeats removed once), appended records for exactly the tables that exist (ext and formation
+// optional, movestate and blocking required), the upload's checks of appended agents and blocking records against the
+// flock table after the call (nflocks_new), finite floats, appended ext targets inside the new population, and no
+// survivor left with a flock index the new table drops. Returns NULL or what was wrong.
+static inline const char *pf_pop_plan_batch(const pf_cmd_mirror &M, int nlayers, const pf_pop_tables &T,
+                                            const uint32_t *rm, size_t nrm, const pfnav_agent *add, const pfnav_movestate *add_ms,
+                                            const pfnav_movestate_ext *add_ext, const pfnav_formation_in *add_form,
+                                            const pfnav_blocking *add_blk, size_t nadd, size_t nflocks_new, pf_pop_plan &P)
+{
+    const size_t n_old = M.flock.size();
+    if (!rm && nrm) return "remove_uids == NULL";
+    if (!add && nadd) return "add == NULL";
+    if (add_ms && !T.ms) return "movestate records for a table that was not uploaded";
+    if (add_ext && !T.ext) return "movestate_ext records for a table that was not uploaded";
+    if (add_form && !T.formation) return "formation records for a table that was not uploaded";
+    if (add_blk && !T.blocking) return "blocking records without a blocking table for the population";
+    if (nadd && T.ms && !add_ms) return "appended entities need movestate records: a movestate table was uploaded";
+    if (nadd && T.blocking && !add_blk) return "appended entities need blocking records: a blocking table covers the population";
+    P.removed.assign(rm, rm + nrm);
+    for (uint32_t u : P.removed)
+        if (u >= n_old) return "remove uid outside the population";
+    std::sort(P.removed.begin(), P.removed.end());
+    P.removed.erase(std::unique(P.removed.begin(), P.removed.end()), P.removed.end());
+    const size_t R = P.removed.size();
+    P.n_old = n_old; P.n_keep = n_old - R; P.n_new = P.n_keep + nadd; P.nflocks = nflocks_new;
+    if (P.n_new >= (1u << 31)) return "population too large";
+    P.key.resize(R);
+    for (size_t m = 0; m < R; m++) P.key[m] = P.removed[m] - (uint32_t)m;
+    P.add_flock.resize(nadd); P.add_layer.resize(nadd);
+    P.add_any_fac = false;
+    for (size_t k = 0; k < nadd; k++) {
+        int layer;
+        if (const char *e = pf_agent_check(add[k], nflocks_new, nlayers, &layer)) return e;
+        if (!pf_finite(add[k].pos, 11)) return "appended agent with a float that is not finite";      // pos .. speed
+        P.add_flock[k] = add[k].flock; P.add_layer[k] = (uint8_t)layer;
+        if (add_ms && !pf_finite(add_ms[k].next_pos, 40)) return "appended movestate with a float that is not finite";
+        if (add_ext) {
+            const pfnav_movestate_ext &x = add_ext[k];
+            if (x.surround_target_uid != PFNAV_NULL_UID && x.surround_target_uid >= P.n_new)
+                return "appended movestate_ext target outside the population after the call";
+            if (!pf_finite(&x.target_range, 3) || !pf_finite(x.target_dir, 8)) return "appended movestate_ext with a float that is not finite";
+        }
+        if (add_form && !pf_finite(add_form[k].cell_pos, 14)) return "appended formation record with a float that is not finite";
+        if (add_blk) {
+            if (const char *e = pf_blocking_check(add_blk[k])) return e;
+            if (!pf_finite(&add_blk[k].stop_x, 3)) return "appended blocking record with a float that is not finite";
+            P.add_any_fac |= add_blk[k].faction_id < 15;
+        }
+    }
+    int64_t stranded = 0;
+    for (size_t f = nflocks_new; f < M.nflocks; f++)
+        for (int l = 0; l < PFNAV_NAV_LAYER_MAX; l++) stranded += M.count[f * PFNAV_NAV_LAYER_MAX + l];
+    for (uint32_t u : P.removed)
+        if (M.flock[u] >= (int64_t)nflocks_new) stranded--;
+    if (stranded > 0) return "the new flock table is shorter than the flock index some surviving entity keeps";
+    return nullptr;
 }
 
 // ---- the job form (pfnav_mgpu_commands / pfnav_group_commands) ----

@@ -504,6 +504,11 @@ int pfnav_agents_refresh_facts(pfnav_ctx *ctx, cudaStream_t st);
 // d_work_count. A failed work list also empties the list (n_work = 0), so no tick reads the released arrays.
 int pf_flocks_reserve(pfnav_ctx *ctx, size_t nflocks);
 int pf_work_reserve(pfnav_ctx *ctx, size_t nwork);
+// the spatial index of the current records (pfnav_agents_rebuild_index), on `st`
+int build_index(pfnav_ctx *ctx, cudaStream_t st);
+// entity_block (mode 1) / entity_unblock (mode 0) of the n uids at d_uids (unique) through k_blocking_decide, appended to
+// the device-decided ops that pfnav_map_commit applies; d_patches != nullptr: the rules of PFNAV_APPLY_BLOCKERS instead
+int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n, const pfnav_patch *d_patches, int mode);
 
 // ---- pfnav_commands.cu: a job member's part of a command batch (pfnav_mgpu.cu runs the verdict exchange) ----
 // pf_cmd_job_check validates the batch against the member's state and plans it, changing nothing (the error is set);
