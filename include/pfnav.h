@@ -998,7 +998,7 @@ int  pfnav_agents_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size
  *   per-entity buffer or the call's scratch regrows. Shares the scratch of pfnav_agents_commands and
  *   pfnav_agents_set_work_dev: order them on one stream. Input arrays are read before the call returns.
  * - PFNAV_ERR_NO_DEVICE on a host-only context. PFNAV_ERR_STATE (nothing changed) on a context in a multi-GPU job, as
- *   for pfnav_agents_commands. */
+ *   for pfnav_agents_commands: a job takes pfnav_mgpu_change_population / pfnav_group_change_population. */
 int  pfnav_agents_change_population(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove,
                                     const pfnav_agent *add, const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
                                     const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking, size_t nadd,
@@ -1033,6 +1033,47 @@ int  pfnav_mgpu_commands(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t
                          const pfnav_flock *flocks, size_t nflocks, void *stream);
 int  pfnav_group_commands(pfnav_group *g, const pfnav_agent_delta *deltas, size_t n,
                           const pfnav_flock *flocks, size_t nflocks);
+/* pfnav_agents_change_population for a whole multi-GPU job. Every rank calls the NCCL form with the same arguments, the
+ * job's whole batch (uids global, in [0, n_total)); the group form is called once. Arguments, their meaning and the
+ * record rules are those of pfnav_agents_change_population.
+ * - Numbering: the solo rule. Survivor u gets u - |{removed r < u}|, appended entity k gets n_keep + k. After the call
+ *   every member owns pfnav_mgpu_shard_range(n_new, rank, world): its entity range moves with the population.
+ * - Equivalence: after the call and the next pfnav_mgpu_gather / pfnav_group_gather, every member's snapshot is what one
+ *   context holding the whole population would have after pfnav_agents_change_population(same arguments), restricted to
+ *   the member's new range: the own range's agent, movestate, movestate_ext, formation and blocking records, the whole
+ *   flock id column and neighbour records, the flock table and member lists, largest radius and any GARRISONED,
+ *   flock_layer_used, blocking_n and blocking_any_fac of the own range (as pfnav_agents_upload_shard of the new range
+ *   would leave them) and the arrival constants' invalidation.
+ * - Moves: each member compacts its own survivors, and the flock id column and neighbour records of the whole population
+ *   it holds; the survivors that cross a member boundary (at most nremove + nadd rows per boundary) move with all their
+ *   records, NCCL broadcasts on `stream` for the NCCL form, peer copies on the members' context streams for the group.
+ *   Each member writes the appended entities of its new range.
+ * - Blocks and targets: a removed entity that holds a block queues its unblock op on its old owner, decided before any
+ *   row moves; exchange the ops (pfnav_mgpu_exchange_blocker_ops / pfnav_group_exchange_blocker_ops) before
+ *   pfnav_map_commit. Surround and enter-range targets are renumbered on every member; a removed target becomes
+ *   PFNAV_NULL_UID.
+ * - All or nothing across the job: each member validates the batch as the solo call does, its own survivors' flock
+ *   indices against a shorter flock table included, then the members exchange one verdict record {status, n_agents,
+ *   n_flocks, tables present}: NCCL all-gathers it on `stream` and reads it, a group reads its members' host state. If any
+ *   member refuses, every member returns that member's error and the text names it; members whose population size, flock
+ *   table size or set of uploaded tables differ return PFNAV_ERR_ARG. Nothing changes anywhere.
+ * - After the call the work list is empty (follow with pfnav_agents_set_work_dev) and the spatial index is left to the
+ *   gather that follows, which carries the neighbour records only: the member lists and population facts are rebuilt on
+ *   each member's device. Host waits: the verdict read of the NCCL form, the received rows' flock ids and records (for the
+ *   member's (flock, layer) facts), the flock offsets, population facts and, with a blocking table, one 4-byte fact;
+ *   buffer regrowths wait for the device. Shares the scratch of pfnav_agents_commands and pfnav_agents_set_work_dev.
+ * - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE (nothing changed) on a context in no job, for the
+ *   NCCL form on a group member, and on every member when one of them has uploaded its range with
+ *   pfnav_agents_upload_shard (without PFNAV_UPLOAD_SAME_FLOCKS) and not gathered since; for a group whose members sit
+ *   on devices without peer access between them. An empty batch without a table does nothing and exchanges nothing. */
+int  pfnav_mgpu_change_population(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove,
+                                  const pfnav_agent *add, const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                  const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking, size_t nadd,
+                                  const pfnav_flock *flocks, size_t nflocks, void *stream);
+int  pfnav_group_change_population(pfnav_group *g, const uint32_t *remove_uids, size_t nremove,
+                                   const pfnav_agent *add, const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                   const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking, size_t nadd,
+                                   const pfnav_flock *flocks, size_t nflocks);
 /* pfnav_agents_set_work(ctx, NULL, 0) from the state resident on the device: the uids of the context's own range whose
  * state is neither ARRIVED nor WAITING, ascending, compacted on the device on `stream`. It waits for the stream once, to
  * read the 4-byte count that sizes the per-work-item buffers; it waits for the whole device only when the list outgrows

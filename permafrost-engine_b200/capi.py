@@ -133,6 +133,7 @@ SYMBOLS = [
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
     "pfnav_mgpu_commands", "pfnav_group_commands",
     "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
+    "pfnav_mgpu_change_population", "pfnav_group_change_population",
 ]
 
 _lib = None
@@ -210,6 +211,8 @@ def load():
     L.pfnav_agents_change_population.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_agents_read_movestate_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_mgpu_change_population.argtypes = L.pfnav_agents_change_population.argtypes
+    L.pfnav_group_change_population.argtypes = L.pfnav_agents_change_population.argtypes[:-1]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     L.pfnav_map_refresh_chunk.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
@@ -303,6 +306,21 @@ class PfnavError(RuntimeError):
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
+
+
+def _population_args(remove, add, ms, ext, formation, blocking, flocks):
+    """the arguments of pfnav_agents_change_population after ctx, without the stream; and the arrays they point into"""
+    rm = np.ascontiguousarray(remove if remove is not None else [], np.uint32).reshape(-1)
+    add = np.ascontiguousarray(add if add is not None else np.zeros(0, AGENT), AGENT).reshape(-1)
+    recs = [None if r is None else np.ascontiguousarray(r, dt).reshape(-1)
+            for r, dt in ((ms, MOVESTATE), (ext, MOVESTATE_EXT), (formation, FORMATION_IN), (blocking, BLOCKING))]
+    for r in recs:
+        assert r is None or len(r) == len(add)
+    fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
+    ptr = lambda a: _p(a) if a is not None and len(a) else None
+    args = (ptr(rm), len(rm), ptr(add), *[ptr(r) for r in recs], len(add), _p(fl) if fl is not None else None,
+            0 if fl is None else len(fl))
+    return args, (rm, add, recs, fl)
 
 
 def _command_args(deltas, flocks):
@@ -991,18 +1009,17 @@ class Nav:
         records; ext and formation then take the defaults). Survivors keep their order and are renumbered densely, the
         appended entities follow. flocks (FLOCK records): the whole new flock table, None: unchanged. The work list is
         emptied: follow with agents_set_work_dev."""
-        rm = np.ascontiguousarray(remove if remove is not None else [], np.uint32).reshape(-1)
-        add = np.ascontiguousarray(add if add is not None else np.zeros(0, AGENT), AGENT).reshape(-1)
-        recs = [None if r is None else np.ascontiguousarray(r, dt).reshape(-1)
-                for r, dt in ((ms, MOVESTATE), (ext, MOVESTATE_EXT), (formation, FORMATION_IN), (blocking, BLOCKING))]
-        for r in recs:
-            assert r is None or len(r) == len(add)
-        fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
-        ptr = lambda a: _p(a) if a is not None and len(a) else None
-        _chk(self.L.pfnav_agents_change_population(self.h, ptr(rm), len(rm), ptr(add), *[ptr(r) for r in recs], len(add),
-                                                   _p(fl) if fl is not None else None, 0 if fl is None else len(fl),
-                                                   C.c_void_p(stream)))
-        self.nagents = getattr(self, "nagents", 0) - len(np.unique(rm)) + len(add)
+        args, keep = _population_args(remove, add, ms, ext, formation, blocking, flocks)
+        _chk(self.L.pfnav_agents_change_population(self.h, *args, C.c_void_p(stream)))
+        self.nagents = getattr(self, "nagents", 0) - len(np.unique(keep[0])) + len(keep[1])
+        self.nwork = 0
+
+    def mgpu_change_population(self, remove, add, ms=None, ext=None, formation=None, blocking=None, flocks=None, stream=0):
+        """collective: agents_change_population for the whole job -- every rank passes the job's whole batch (global
+        uids) and the same table; all or nothing across the ranks. Afterwards the rank owns
+        mgpu_shard_range(n_new, rank, world). Follow with mgpu_gather and agents_set_work_dev."""
+        args, keep = _population_args(remove, add, ms, ext, formation, blocking, flocks)
+        _chk(self.L.pfnav_mgpu_change_population(self.h, *args, C.c_void_p(stream)))
         self.nwork = 0
 
     def agents_read_movestate_ext(self, n):
@@ -1141,6 +1158,14 @@ class Group:
         """agents_commands for the whole group: the job's whole batch (global uids), each member applying its own
         entities' deltas; all or nothing across the members. Follow with gather."""
         _chk(load().pfnav_group_commands(self.g, *_command_args(deltas, flocks)))
+
+    def change_population(self, remove, add, ms=None, ext=None, formation=None, blocking=None, flocks=None):
+        """agents_change_population for the whole group: the job's whole batch (global uids); member i then owns
+        mgpu_shard_range(n_new, i, world). All or nothing across the members. Follow with gather and agents_set_work_dev."""
+        args, keep = _population_args(remove, add, ms, ext, formation, blocking, flocks)
+        _chk(load().pfnav_group_change_population(self.g, *args))
+        for nv in self.navs:
+            nv.nwork = 0
 
     def close(self):
         if self.g:

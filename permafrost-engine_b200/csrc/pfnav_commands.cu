@@ -11,7 +11,9 @@
 // pfnav_agents_set_work_dev compacts the uids that are not still into the work list, in uid order.
 // pfnav_agents_change_population removes and appends entities (pfnav_commands_host.h plans the batch and holds the
 // numbering rule): k_pop_gather writes every new row of every table with one thread per row, then the member lists,
-// population facts and spatial index are rebuilt for the new population.
+// population facts and spatial index are rebuilt for the new population. Its job form (pf_pop_job_*, for pfnav_mgpu.cu)
+// compacts each member's own survivors with k_pop_gather over a row window and the replicated record and flock columns
+// with k_pop_columns; the segments of survivors that cross a member boundary move between the stages.
 #include "pfnav_internal.cuh"
 #include <algorithm>
 
@@ -205,56 +207,90 @@ struct pf_pop_gather {
     pfnav_agent *o_agents; pf_record *o_rec; int32_t *o_flock; pfnav_movestate *o_ms; pfnav_movestate_ext *o_ext;
     pfnav_formation_in *o_form; pfnav_blocking *o_blk;
     const uint32_t *removed, *key; uint32_t R, n_old;
-    int row0, n_keep, n_new;
+    int row0, row1, out0, n_keep, n_new;     // new rows [row0, row1), written at index row - out0 of the o_ tables
     uint32_t *any_fac;           // set when a written blocking record names a faction other than 15
 };
+
+__device__ __forceinline__ pf_record pop_record(const pfnav_agent &a)
+{
+    pf_record r;                       // as k_make_records packs it
+    r.px = a.pos[0]; r.pz = a.pos[1]; r.vx = a.velocity[0]; r.vz = a.velocity[1];
+    r.radius = a.radius;
+    r.state_flags = (a.state << 24) | (a.flags & 0xFFFFFFu);
+    return r;
+}
 
 __global__ void k_pop_gather(const pf_pop_gather g)
 {
     const int i = g.row0 + blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= g.n_new) return;
+    if (i >= g.row1) return;
+    const int o = i - g.out0;
     pfnav_agent a;
     pfnav_blocking b;
     if (i < g.n_keep) {
         const uint32_t s = pf_pop_source(g.key, g.R, (uint32_t)i);
         a = g.agents[s];
-        if (g.o_ms) g.o_ms[i] = g.ms[s];
+        if (g.o_ms) g.o_ms[o] = g.ms[s];
         if (g.o_ext) {
             pfnav_movestate_ext x = g.ext[s];
             if (x.surround_target_uid != PFNAV_NULL_UID)
                 x.surround_target_uid = pf_pop_renumber(g.removed, g.R, g.n_old, x.surround_target_uid);
-            g.o_ext[i] = x;
+            g.o_ext[o] = x;
         }
-        if (g.o_form) g.o_form[i] = g.form[s];
+        if (g.o_form) g.o_form[o] = g.form[s];
         if (g.o_blk) b = g.blk[s];
     } else {
         const int k = i - g.n_keep;
         a = g.a_agents[k];
-        if (g.o_ms) g.o_ms[i] = g.a_ms[k];
+        if (g.o_ms) g.o_ms[o] = g.a_ms[k];
         if (g.o_ext) {
             pfnav_movestate_ext x = {};
             if (g.a_ext) x = g.a_ext[k];
             else { x.surround_target_uid = PFNAV_NULL_UID; x.rot[3] = 1.0f; }
-            g.o_ext[i] = x;
+            g.o_ext[o] = x;
         }
         if (g.o_form) {
             pfnav_formation_in f = {};
             if (g.a_form) f = g.a_form[k];
-            g.o_form[i] = f;
+            g.o_form[o] = f;
         }
         if (g.o_blk) b = g.a_blk[k];
     }
-    g.o_agents[i] = a;
-    g.o_flock[i] = a.flock;
-    pf_record r;                       // as k_make_records packs it
-    r.px = a.pos[0]; r.pz = a.pos[1]; r.vx = a.velocity[0]; r.vz = a.velocity[1];
-    r.radius = a.radius;
-    r.state_flags = (a.state << 24) | (a.flags & 0xFFFFFFu);
-    g.o_rec[i] = r;
+    g.o_agents[o] = a;
+    g.o_flock[o] = a.flock;
+    g.o_rec[o] = pop_record(a);
     if (g.o_blk) {
-        g.o_blk[i] = b;
+        g.o_blk[o] = b;
         if (b.faction_id < 15) *g.any_fac = 1u;
     }
+}
+
+// A job member's replicated columns over the new population. It holds valid agent rows for its own range only, so the
+// survivors' records and flock ids are compacted from the columns themselves (their radius, flag bits and flock id are
+// current on every member; position, velocity and state of other members' entities arrive with the next gather) and
+// the appended entities' are packed from their agent records.
+__global__ void k_pop_columns(const pf_record *__restrict__ rec, const int32_t *__restrict__ flock, const uint32_t *__restrict__ key,
+                              uint32_t R, int n_keep, int n_new, const pfnav_agent *__restrict__ a_agents,
+                              pf_record *__restrict__ o_rec, int32_t *__restrict__ o_flock)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_new) return;
+    if (i < n_keep) {
+        const uint32_t s = pf_pop_source(key, R, (uint32_t)i);
+        o_rec[i] = rec[s];
+        o_flock[i] = flock[s];
+    } else {
+        const pfnav_agent a = a_agents[i - n_keep];
+        o_rec[i] = pop_record(a);
+        o_flock[i] = a.flock;
+    }
+}
+
+// *word = 1 when a blocking record of [lo, hi) names a faction other than 15 (pfnav_agents_upload_blocking's fact)
+__global__ void k_pop_any_fac(const pfnav_blocking *__restrict__ b, int lo, int hi, uint32_t *word)
+{
+    const int i = lo + blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < hi && b[i].faction_id < 15) *word = 1u;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -442,7 +478,7 @@ static int pop_apply(pfnav_ctx *ctx, cudaStream_t st, const pf_pop_tables &T, co
         g.o_blk = T.blocking ? ctx->d_blocking.p : nullptr;
     }
     g.removed = d_removed; g.key = (const uint32_t *)(stage + s_key); g.R = (uint32_t)R; g.n_old = (uint32_t)P.n_old;
-    g.row0 = full ? 0 : (int)P.n_keep; g.n_keep = (int)P.n_keep; g.n_new = (int)n_new;
+    g.row0 = full ? 0 : (int)P.n_keep; g.row1 = (int)n_new; g.out0 = 0; g.n_keep = (int)P.n_keep; g.n_new = (int)n_new;
     uint32_t *d_fac = (uint32_t *)(stage + s_fac);
     g.any_fac = d_fac;
     if (n_new > (size_t)g.row0) {
@@ -516,6 +552,248 @@ extern "C" int pfnav_agents_change_population(pfnav_ctx *ctx, const uint32_t *re
     if (P.removed.empty() && nadd == 0 && !flocks) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
     return pop_apply(ctx, pf_stream(ctx, stream), T, P, add, add_ms, add_ext, add_formation, add_blocking, nadd, flocks, nflocks);
+}
+
+// ---- the job form of a population change (pfnav_mgpu.cu runs the verdict exchange and moves the segments) ----
+int pf_pop_job_check(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove, const pfnav_agent *add,
+                     const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext, const pfnav_formation_in *add_form,
+                     const pfnav_blocking *add_blk, size_t nadd, const pfnav_flock *flocks, size_t nflocks, int world, int rank,
+                     pf_pop_member &M)
+{
+    PF_ARG(ctx->d_agents, "agents not uploaded");
+    if (ctx->members_stale) {
+        pfnav_set_error("the member's flock column is incomplete until the gather that follows pfnav_agents_upload_shard");
+        return PFNAV_ERR_STATE;
+    }
+    PF_ARG(nremove < (1u << 31) && nadd < (1u << 31) && nflocks < (1u << 31), "nremove / nadd / nflocks");
+    M.flocks = flocks;
+    M.nflocks = flocks ? nflocks : ctx->n_flocks;
+    M.T = {ctx->movestate_set && ctx->d_movestate != nullptr, ctx->d_ms_ext != nullptr, ctx->d_formation != nullptr,
+           ctx->d_blocking != nullptr && ctx->blocking_n == ctx->n_agents};
+    M.add = add; M.add_ms = add_ms; M.add_ext = add_ext; M.add_form = add_form; M.add_blk = add_blk; M.nadd = nadd;
+    const char *err = pf_pop_job_plan(ctx->cmd_mirror, ctx->n_agents, world, rank, ctx->nlayers, M.T, remove_uids, nremove, add,
+                                      add_ms, add_ext, add_form, add_blk, nadd, M.nflocks, M.J);
+    PF_ARG(!err, err);
+    return PFNAV_OK;
+}
+
+// a block of `rows` rows of every table that exists, taken from the scratch at base + top (base null: sizing only)
+static pf_pop_rows pop_rows(uint8_t *base, size_t &top, size_t rows, const pf_pop_tables &T, size_t first, int device)
+{
+    auto take = [&](size_t bytes) { uint8_t *p = (uint8_t *)((uintptr_t)base + top); top += (bytes + 255) & ~(size_t)255; return p; };
+    pf_pop_rows b;
+    b.agents = (pfnav_agent *)take(rows * sizeof(pfnav_agent));
+    b.rec = (pf_record *)take(rows * sizeof(pf_record));
+    b.flock = (int32_t *)take(rows * 4);
+    if (T.ms) b.ms = (pfnav_movestate *)take(rows * sizeof(pfnav_movestate));
+    if (T.ext) b.ext = (pfnav_movestate_ext *)take(rows * sizeof(pfnav_movestate_ext));
+    if (T.formation) b.form = (pfnav_formation_in *)take(rows * sizeof(pfnav_formation_in));
+    if (T.blocking) b.blk = (pfnav_blocking *)take(rows * sizeof(pfnav_blocking));
+    b.first = first; b.device = device;
+    return b;
+}
+
+// the rows of every table for the new uids [a, a + n) of this member, from block b (on this or a peer device)
+static int pop_copy_rows(pfnav_ctx *ctx, const pf_pop_rows &b, const pf_pop_tables &T, size_t a, size_t n, cudaStream_t st)
+{
+    const size_t k = a - b.first;
+    auto cp = [&](void *dst, const void *src, size_t bytes) { return cudaMemcpyPeerAsync(dst, ctx->device, src, b.device, bytes, st); };
+    PF_CUDA(cp(ctx->d_agents + a, b.agents + k, n * sizeof(pfnav_agent)));
+    PF_CUDA(cp(ctx->d_records + a, b.rec + k, n * sizeof(pf_record)));
+    PF_CUDA(cp(ctx->d_flock_of + a, b.flock + k, n * 4));
+    if (T.ms) PF_CUDA(cp(ctx->d_movestate + a, b.ms + k, n * sizeof(pfnav_movestate)));
+    if (T.ext) PF_CUDA(cp(ctx->d_ms_ext + a, b.ext + k, n * sizeof(pfnav_movestate_ext)));
+    if (T.formation) PF_CUDA(cp(ctx->d_formation + a, b.form + k, n * sizeof(pfnav_formation_in)));
+    if (T.blocking) PF_CUDA(cp(ctx->d_blocking + a, b.blk + k, n * sizeof(pfnav_blocking)));
+    return 0;
+}
+
+// k_pop_gather of the new rows [row0, row1) from the member's tables as they were and the staged appended records
+static pf_pop_gather pop_gather_args(pfnav_ctx *ctx, const pf_pop_member &M, size_t row0, size_t row1, size_t out0)
+{
+    const pf_pop_tables &T = M.T;
+    const pf_pop_plan &P = M.J.P;
+    uint8_t *st = M.stage;
+    pf_pop_gather g = {};
+    g.agents = ctx->d_agents; g.ms = T.ms ? ctx->d_movestate.p : nullptr; g.ext = ctx->d_ms_ext; g.form = ctx->d_formation;
+    g.blk = T.blocking ? ctx->d_blocking.p : nullptr;
+    g.a_agents = (const pfnav_agent *)(st + M.s_agents);
+    g.a_ms = M.add_ms ? (const pfnav_movestate *)(st + M.s_ms) : nullptr;
+    g.a_ext = M.add_ext ? (const pfnav_movestate_ext *)(st + M.s_ext) : nullptr;
+    g.a_form = M.add_form ? (const pfnav_formation_in *)(st + M.s_form) : nullptr;
+    g.a_blk = M.add_blk ? (const pfnav_blocking *)(st + M.s_blk) : nullptr;
+    g.removed = (const uint32_t *)(st + M.s_removed); g.key = (const uint32_t *)(st + M.s_key);
+    g.R = (uint32_t)P.removed.size(); g.n_old = (uint32_t)P.n_old;
+    g.row0 = (int)row0; g.row1 = (int)row1; g.out0 = (int)out0; g.n_keep = (int)P.n_keep; g.n_new = (int)P.n_new;
+    g.any_fac = (uint32_t *)(st + M.s_fac);              // word 0: the gathers' (unused), word 1: k_pop_any_fac's
+    return g;
+}
+
+static void pop_launch(pfnav_ctx *ctx, const pf_pop_gather &g, cudaStream_t st)
+{
+    k_pop_gather<<<(g.row1 - g.row0 + 127) / 128, 128, 0, st>>>(g);
+    ctx->launches++;
+}
+
+// Scratch: [own survivors' block] [compacted record column] [compacted flock column] [receive blocks] [staged inputs]; the
+// member sort's histogram reuses it from the start in pf_pop_job_commit.
+int pf_pop_job_stage(pfnav_ctx *ctx, pf_pop_member &M, bool receive_all, cudaStream_t st)
+{
+    const pf_pop_job &J = M.J;
+    const pf_pop_plan &P = J.P;
+    const pf_pop_tables &T = M.T;
+    const int r = J.rank, world = J.world;
+    const size_t R = P.removed.size(), n_new = P.n_new, nadd = M.nadd;
+    auto layout = [&](uint8_t *base) {
+        size_t top = 0;
+        auto take = [&](size_t bytes) { const size_t o = top; top += (bytes + 255) & ~(size_t)255; return o; };
+        M.own = pop_rows(base, top, J.keep_lo[r + 1] - J.keep_lo[r], T, J.keep_lo[r], ctx->device);
+        M.c_rec = (pf_record *)((uintptr_t)base + take(n_new * sizeof(pf_record)));
+        M.c_flock = (int32_t *)((uintptr_t)base + take(n_new * 4));
+        M.pair.clear();
+        if (receive_all)
+            for (int s = 0; s < world; s++)
+                for (int q = 0; q < world; q++)
+                    M.pair.push_back(pop_rows(base, top, s == q ? 0 : J.seg_hi(s, q) - J.seg_lo(s, q), T, J.seg_lo(s, q), ctx->device));
+        const size_t s0 = top;
+        M.stage = (uint8_t *)((uintptr_t)base + s0);
+        M.s_removed = take(R * 4) - s0; M.s_key = take(R * 4) - s0; M.s_agents = take(nadd * sizeof(pfnav_agent)) - s0;
+        M.s_ms = take(M.add_ms ? nadd * sizeof(pfnav_movestate) : 0) - s0;
+        M.s_ext = take(M.add_ext ? nadd * sizeof(pfnav_movestate_ext) : 0) - s0;
+        M.s_form = take(M.add_form ? nadd * sizeof(pfnav_formation_in) : 0) - s0;
+        M.s_blk = take(M.add_blk ? nadd * sizeof(pfnav_blocking) : 0) - s0;
+        M.s_fac = take(8) - s0;
+        return std::make_pair(s0, top);
+    };
+    int per, W, rc;
+    member_sort_shape(n_new, M.nflocks, per, W);
+    const size_t top = layout(nullptr).second;
+    if ((rc = ctx->d_cmd_buf.reserve(std::max(top, M.nflocks * (size_t)W * 4)))) return rc;
+    if ((rc = pf_flocks_reserve(ctx, M.nflocks))) return rc;     // keeps no content: the table follows, the offsets are rebuilt
+    const size_t s0 = layout(ctx->d_cmd_buf.p).first;
+    M.from.assign(world, pf_pop_rows());
+    for (int s = 0; s < world; s++) M.from[s] = s == r ? M.own : receive_all ? M.pair[(size_t)s * world + r] : pf_pop_rows();
+    // the staged inputs, one copy from one host image
+    std::vector<uint8_t> h(top - s0, 0);
+    auto put = [&h](size_t off, const void *src, size_t bytes) { if (bytes) memcpy(h.data() + off, src, bytes); };
+    put(M.s_removed, P.removed.data(), R * 4); put(M.s_key, P.key.data(), R * 4);
+    put(M.s_agents, M.add, nadd * sizeof(pfnav_agent));
+    if (M.add_ms) put(M.s_ms, M.add_ms, nadd * sizeof(pfnav_movestate));
+    if (M.add_ext) put(M.s_ext, M.add_ext, nadd * sizeof(pfnav_movestate_ext));
+    if (M.add_form) put(M.s_form, M.add_form, nadd * sizeof(pfnav_formation_in));
+    if (M.add_blk) put(M.s_blk, M.add_blk, nadd * sizeof(pfnav_blocking));
+    PF_CUDA(cudaMemcpyAsync(M.stage, h.data(), h.size(), cudaMemcpyHostToDevice, st));
+    // the blocks of the member's removed entities are released as pfnav_agents_set_blocking(removed, 0) would, before
+    // anything moves
+    const size_t m0 = std::lower_bound(P.removed.begin(), P.removed.end(), (uint32_t)J.old_lo[r]) - P.removed.begin();
+    const size_t m1 = std::lower_bound(P.removed.begin(), P.removed.end(), (uint32_t)J.old_lo[r + 1]) - P.removed.begin();
+    if (T.blocking && m1 > m0 && (rc = blocking_emit(ctx, st, (const uint32_t *)(M.stage + M.s_removed) + m0, (int)(m1 - m0), nullptr, 0)))
+        return rc;
+    if (M.flocks) {
+        // from the context's own pageable copy, which is staged before the call returns: the caller's array may be pinned
+        ctx->h_flocks.assign(M.flocks, M.flocks + M.nflocks);
+        if (M.nflocks) PF_CUDA(cudaMemcpyAsync(ctx->d_flocks, ctx->h_flocks.data(), M.nflocks * sizeof(pfnav_flock), cudaMemcpyHostToDevice, st));
+    }
+    if (J.keep_lo[r + 1] > J.keep_lo[r]) {
+        pf_pop_gather g = pop_gather_args(ctx, M, J.keep_lo[r], J.keep_lo[r + 1], J.keep_lo[r]);
+        g.o_agents = M.own.agents; g.o_rec = M.own.rec; g.o_flock = M.own.flock; g.o_ms = M.own.ms; g.o_ext = M.own.ext;
+        g.o_form = M.own.form; g.o_blk = M.own.blk;
+        pop_launch(ctx, g, st);
+    }
+    if (n_new) {
+        k_pop_columns<<<((int)n_new + 127) / 128, 128, 0, st>>>(ctx->d_records, ctx->d_flock_of, (const uint32_t *)(M.stage + M.s_key),
+                                                                (uint32_t)R, (int)P.n_keep, (int)n_new,
+                                                                (const pfnav_agent *)(M.stage + M.s_agents), M.c_rec, M.c_flock);
+        ctx->launches++;
+    }
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
+}
+
+int pf_pop_job_write(pfnav_ctx *ctx, pf_pop_member &M, cudaStream_t st)
+{
+    const pf_pop_job &J = M.J;
+    const pf_pop_tables &T = M.T;
+    const int r = J.rank, world = J.world;
+    const size_t n_new = J.P.n_new, lo = J.new_lo[r], hi = J.new_lo[r + 1];
+    // the mirror: the received rows' flock ids, radii and flag bits from the member's own compacted columns
+    size_t nrecv = 0;
+    for (int s = 0; s < world; s++)
+        if (s != r) nrecv += J.seg_hi(s, r) - J.seg_lo(s, r);
+    std::vector<int32_t> fl(nrecv);
+    std::vector<pf_record> rec(nrecv);
+    for (int s = 0, k = 0; s < world; s++) {
+        const size_t a = J.seg_lo(s, r), n = J.seg_hi(s, r) - a;
+        if (s == r || !n) continue;
+        PF_CUDA(cudaMemcpyAsync(fl.data() + k, M.c_flock + a, n * 4, cudaMemcpyDeviceToHost, st));
+        PF_CUDA(cudaMemcpyAsync(rec.data() + k, M.c_rec + a, n * sizeof(pf_record), cudaMemcpyDeviceToHost, st));
+        k += (int)n;
+    }
+    if (nrecv) PF_CUDA(cudaStreamSynchronize(st));
+    std::vector<float> rad(nrecv);
+    std::vector<uint32_t> sf(nrecv);
+    for (size_t k = 0; k < nrecv; k++) { rad[k] = rec[k].radius; sf[k] = rec[k].state_flags; }
+    pf_pop_job_mirror(ctx->cmd_mirror, J, fl.data(), rad.data(), sf.data(), M.mirror);
+    // the tables at their new length (a regrowth waits for the device and drops the contents: everything is in the scratch)
+    int rc;
+    if ((rc = pf_dbuf_reserve_all(n_new, ctx->d_agents, ctx->d_records, ctx->d_flock_members, ctx->d_flock_of, ctx->d_sorted_ix,
+                                  ctx->d_sorted_iy, ctx->d_sorted_flock, ctx->d_sorted_id))) return rc;
+    if (T.ms && (rc = ctx->d_movestate.reserve(n_new))) return rc;
+    if (T.ext && (rc = ctx->d_ms_ext.reserve(n_new))) return rc;
+    if (T.formation && (rc = ctx->d_formation.reserve(n_new))) return rc;
+    if (T.blocking && (rc = ctx->d_blocking.reserve(std::max<size_t>(n_new, 1)))) { ctx->blocking_n = 0; return rc; }
+    if (n_new) {
+        PF_CUDA(cudaMemcpyAsync(ctx->d_records, M.c_rec, n_new * sizeof(pf_record), cudaMemcpyDeviceToDevice, st));
+        PF_CUDA(cudaMemcpyAsync(ctx->d_flock_of, M.c_flock, n_new * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    // the new own range: the senders' segments (the member's own survivors that stay among them), then the appended rows
+    for (int s = 0; s < world; s++) {
+        const size_t a = J.seg_lo(s, r), n = J.seg_hi(s, r) - a;
+        if (n && (rc = pop_copy_rows(ctx, M.from[s], T, a, n, st))) return rc;
+    }
+    if (J.app_hi(r) > J.app_lo(r)) {
+        pf_pop_gather g = pop_gather_args(ctx, M, J.app_lo(r), J.app_hi(r), 0);
+        g.o_agents = ctx->d_agents; g.o_rec = ctx->d_records; g.o_flock = ctx->d_flock_of;
+        g.o_ms = T.ms ? ctx->d_movestate.p : nullptr; g.o_ext = ctx->d_ms_ext; g.o_form = ctx->d_formation;
+        g.o_blk = T.blocking ? ctx->d_blocking.p : nullptr;
+        pop_launch(ctx, g, st);
+    }
+    if (T.blocking && hi > lo) {
+        uint32_t *word = (uint32_t *)(M.stage + M.s_fac) + 1;
+        PF_CUDA(cudaMemsetAsync(word, 0, 4, st));
+        k_pop_any_fac<<<(int)(hi - lo + 255) / 256, 256, 0, st>>>(ctx->d_blocking, (int)lo, (int)hi, word);
+        ctx->launches++;
+    }
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
+}
+
+// host facts as pfnav_agents_upload_shard of the new range would leave them, then the member lists and population facts
+// from the member's complete columns
+int pf_pop_job_commit(pfnav_ctx *ctx, pf_pop_member &M, cudaStream_t st)
+{
+    const pf_pop_job &J = M.J;
+    const size_t n_new = J.P.n_new, lo = J.new_lo[J.rank], hi = J.new_lo[J.rank + 1];
+    if (M.T.blocking) {
+        uint32_t fac = 0;
+        if (hi > lo) {
+            PF_CUDA(cudaMemcpyAsync(&fac, (uint32_t *)(M.stage + M.s_fac) + 1, 4, cudaMemcpyDeviceToHost, st));
+            PF_CUDA(cudaStreamSynchronize(st));
+        }
+        ctx->blocking_n = n_new;
+        ctx->blocking_any_fac = fac != 0;
+    }
+    ctx->n_agents = n_new; ctx->shard_lo = lo; ctx->shard_hi = hi; ctx->n_flocks = M.nflocks;
+    ctx->cmd_mirror = std::move(M.mirror);
+    std::vector<uint8_t> used;
+    ctx->cmd_mirror.used(used);
+    if (M.flocks || used != ctx->flock_layer_used) ctx->arrival_valid = false;
+    ctx->flock_layer_used.swap(used);
+    ctx->n_work = 0;
+    int per, W, rc;
+    member_sort_shape(n_new, M.nflocks, per, W);
+    if ((rc = members_on_device(ctx, st, (uint32_t *)ctx->d_cmd_buf.p, per, W))) return rc;
+    return pfnav_agents_refresh_facts(ctx, st);
 }
 
 // A job member: the whole batch is checked against the population, the own records against the member's mirror. Its

@@ -1,8 +1,9 @@
 // pfnav_commands_host.h -- the host side of pfnav_agents_commands and the write rule its kernel applies, CUDA-free:
 // delta validation, per-uid merging in array order, the navigation layer rule and the (flock, layer) mirror that keeps
 // flock_layer_used equal to a fresh upload's; and the split of a multi-GPU job's batch into a member's own and foreign
-// parts; and the validation, numbering rule and mirror update of pfnav_agents_change_population.
-// tests/emu/commands_emu.cpp, tests/emu/commands_job_emu.cpp and tests/emu/population_emu.cpp build this header with g++.
+// parts; and the validation, numbering rule and mirror update of pfnav_agents_change_population, and its job form's
+// ranges, segments and member mirror. tests/emu/commands_emu.cpp, tests/emu/commands_job_emu.cpp,
+// tests/emu/population_emu.cpp and tests/emu/population_job_emu.cpp build this header with g++.
 #pragma once
 #include <math.h>
 #include <algorithm>
@@ -263,12 +264,13 @@ static inline bool pf_finite(const float *p, int n)
 // optional, movestate and blocking required), the upload's checks of appended agents and blocking records against the
 // flock table after the call (nflocks_new), finite floats, appended ext targets inside the new population, and no
 // survivor left with a flock index the new table drops. Returns NULL or what was wrong.
-static inline const char *pf_pop_plan_batch(const pf_cmd_mirror &M, int nlayers, const pf_pop_tables &T,
+// M mirrors the entities [lo, lo + M.flock.size()) of a population of n_old: the whole population for the solo call, a
+// job member's own range for the job form, where only the stranded flock indices of that range are checked.
+static inline const char *pf_pop_plan_range(const pf_cmd_mirror &M, size_t lo, size_t n_old, int nlayers, const pf_pop_tables &T,
                                             const uint32_t *rm, size_t nrm, const pfnav_agent *add, const pfnav_movestate *add_ms,
                                             const pfnav_movestate_ext *add_ext, const pfnav_formation_in *add_form,
                                             const pfnav_blocking *add_blk, size_t nadd, size_t nflocks_new, pf_pop_plan &P)
 {
-    const size_t n_old = M.flock.size();
     if (!rm && nrm) return "remove_uids == NULL";
     if (!add && nadd) return "add == NULL";
     if (add_ms && !T.ms) return "movestate records for a table that was not uploaded";
@@ -312,9 +314,95 @@ static inline const char *pf_pop_plan_batch(const pf_cmd_mirror &M, int nlayers,
     for (size_t f = nflocks_new; f < M.nflocks; f++)
         for (int l = 0; l < PFNAV_NAV_LAYER_MAX; l++) stranded += M.count[f * PFNAV_NAV_LAYER_MAX + l];
     for (uint32_t u : P.removed)
-        if (M.flock[u] >= (int64_t)nflocks_new) stranded--;
+        if (u >= lo && u - lo < M.flock.size() && M.flock[u - lo] >= (int64_t)nflocks_new) stranded--;
     if (stranded > 0) return "the new flock table is shorter than the flock index some surviving entity keeps";
     return nullptr;
+}
+
+static inline const char *pf_pop_plan_batch(const pf_cmd_mirror &M, int nlayers, const pf_pop_tables &T,
+                                            const uint32_t *rm, size_t nrm, const pfnav_agent *add, const pfnav_movestate *add_ms,
+                                            const pfnav_movestate_ext *add_ext, const pfnav_formation_in *add_form,
+                                            const pfnav_blocking *add_blk, size_t nadd, size_t nflocks_new, pf_pop_plan &P)
+{
+    return pf_pop_plan_range(M, 0, M.flock.size(), nlayers, T, rm, nrm, add, add_ms, add_ext, add_form, add_blk, nadd,
+                             nflocks_new, P);
+}
+
+// ---- the job form of a population change (pfnav_mgpu_change_population / pfnav_group_change_population) ----
+// Every member gets the job's whole batch and derives the same plan from it. Member r owns the balanced range
+// [old_lo[r], old_lo[r + 1]) before the call and [new_lo[r], new_lo[r + 1]) after it. Compaction keeps order, so the
+// survivors of member s occupy the contiguous new uids [keep_lo[s], keep_lo[s + 1]); the part of that run inside r's new
+// range is the one segment s sends r (s == r: the own survivors that stay). Appended entities [n_keep, n_new) are written
+// by the member whose new range holds them.
+struct pf_pop_job {
+    pf_pop_plan P;
+    int world = 1, rank = 0;
+    std::vector<size_t> old_lo, new_lo, keep_lo;      // world + 1 boundaries each
+    size_t seg_lo(int s, int r) const { return std::min(std::max(keep_lo[s], new_lo[r]), new_lo[r + 1]); }
+    size_t seg_hi(int s, int r) const { return std::max(seg_lo(s, r), std::min(keep_lo[s + 1], new_lo[r + 1])); }
+    size_t app_lo(int r) const { return std::min(std::max(P.n_keep, new_lo[r]), new_lo[r + 1]); }
+    size_t app_hi(int r) const { return new_lo[r + 1]; }
+};
+
+// pfnav_mgpu_shard_range's balanced split of n entities over world members, as world + 1 boundaries
+static inline void pf_balanced_bounds(size_t n, int world, std::vector<size_t> &b)
+{
+    b.resize((size_t)world + 1);
+    const size_t base = n / world, rem = n % world;
+    for (int r = 0; r <= world; r++) b[r] = (size_t)r * base + std::min<size_t>(r, rem);
+}
+
+// A member's part of a job's population change, changing nothing: the solo validation with the member's mirror M of its
+// own range (removal range, appended records, tables present, stranded flock indices of its own entities), then the
+// ranges and segments of every member. Returns NULL or what was wrong.
+static inline const char *pf_pop_job_plan(const pf_cmd_mirror &M, size_t n_old, int world, int rank, int nlayers,
+                                          const pf_pop_tables &T, const uint32_t *rm, size_t nrm, const pfnav_agent *add,
+                                          const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                          const pfnav_formation_in *add_form, const pfnav_blocking *add_blk, size_t nadd,
+                                          size_t nflocks_new, pf_pop_job &J)
+{
+    J.world = world; J.rank = rank;
+    pf_balanced_bounds(n_old, world, J.old_lo);
+    if (M.flock.size() != J.old_lo[rank + 1] - J.old_lo[rank]) return "the member does not hold its balanced range";
+    if (const char *e = pf_pop_plan_range(M, J.old_lo[rank], n_old, nlayers, T, rm, nrm, add, add_ms, add_ext, add_form,
+                                          add_blk, nadd, nflocks_new, J.P))
+        return e;
+    pf_balanced_bounds(J.P.n_new, world, J.new_lo);
+    J.keep_lo.resize((size_t)world + 1);
+    for (int r = 0; r <= world; r++) {
+        const size_t u = J.old_lo[r];
+        J.keep_lo[r] = u - (size_t)(std::lower_bound(J.P.removed.begin(), J.P.removed.end(), (uint32_t)u) - J.P.removed.begin());
+    }
+    return nullptr;
+}
+
+// The member's mirror after the call, over its new range: its own survivors that stay keep their entries, appended
+// entities take pf_pop_plan::add_flock / add_layer, and the k-th received row (in uid order: the segments of the senders
+// in rank order) takes flock[k] and the layer of radius[k] and state_flags[k] (the record's state << 24 | flags) by
+// pf_agent_check's rule: the member's own copies of those columns after compaction, current on every member.
+static inline void pf_pop_job_mirror(const pf_cmd_mirror &M, const pf_pop_job &J, const int32_t *flock, const float *radius,
+                                     const uint32_t *state_flags, pf_cmd_mirror &out)
+{
+    const int r = J.rank;
+    const size_t lo = J.new_lo[r], hi = J.new_lo[r + 1];
+    const size_t s0 = J.seg_lo(r, r), s1 = J.seg_hi(r, r);
+    pf_cmd_mirror N;
+    N.reset(hi - lo, J.P.nflocks);
+    size_t k = 0;
+    for (size_t j = lo; j < hi; j++) {
+        if (j >= J.P.n_keep) {
+            const size_t a = j - J.P.n_keep;
+            N.set(j - lo, std::max(J.P.add_flock[a], -1), J.P.add_layer[a]);
+        } else if (j >= s0 && j < s1) {
+            const size_t i = pf_pop_source(J.P.key.data(), (uint32_t)J.P.removed.size(), (uint32_t)j) - J.old_lo[r];
+            N.set(j - lo, M.flock[i], M.layer[i]);
+        } else {
+            const uint32_t f = state_flags[k] & 0xFFFFFFu;
+            N.set(j - lo, std::max(flock[k], -1), pf_layer_base(f) + pf_layer_class(radius[k]));
+            k++;
+        }
+    }
+    out = std::move(N);
 }
 
 // ---- the job form (pfnav_mgpu_commands / pfnav_group_commands) ----

@@ -523,6 +523,44 @@ int pf_cmd_job_check(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, 
                      pf_cmd_job &J);
 int pf_cmd_job_apply(pfnav_ctx *ctx, const pf_cmd_job &J, cudaStream_t st);
 
+// ---- pfnav_commands.cu: a job member's part of a population change (pfnav_mgpu.cu runs the verdict exchange and moves
+// the segments between the stages) ----
+// One block of rows of every table a population change writes, in a member's command scratch; row 0 has the new uid
+// `first`. Tables that do not exist are null.
+struct pf_pop_rows {
+    pfnav_agent *agents = nullptr; pf_record *rec = nullptr; int32_t *flock = nullptr; pfnav_movestate *ms = nullptr;
+    pfnav_movestate_ext *ext = nullptr; pfnav_formation_in *form = nullptr; pfnav_blocking *blk = nullptr;
+    size_t first = 0;
+    int device = 0;
+};
+struct pf_pop_member {
+    pf_pop_job J;
+    pf_pop_tables T = {};
+    const pfnav_agent *add = nullptr; const pfnav_movestate *add_ms = nullptr; const pfnav_movestate_ext *add_ext = nullptr;
+    const pfnav_formation_in *add_form = nullptr; const pfnav_blocking *add_blk = nullptr; size_t nadd = 0;
+    const pfnav_flock *flocks = nullptr; size_t nflocks = 0;
+    pf_pop_rows own;                     // the member's survivors, new uids [keep_lo[rank], keep_lo[rank + 1])
+    std::vector<pf_pop_rows> from;       // per sender: the block holding its segment for this member (own for itself)
+    std::vector<pf_pop_rows> pair;       // receive_all: one block per (sender, receiver) segment, [s * world + r]
+    pf_record *c_rec = nullptr; int32_t *c_flock = nullptr;       // the compacted columns of the whole new population
+    uint8_t *stage = nullptr;            // the staged inputs, at these offsets
+    size_t s_removed = 0, s_key = 0, s_agents = 0, s_ms = 0, s_ext = 0, s_form = 0, s_blk = 0, s_fac = 0;
+    pf_cmd_mirror mirror;                // the mirror of the new range, committed by pf_pop_job_commit
+};
+// pf_pop_job_check: validation and plan, changing nothing (the error is set). pf_pop_job_stage (on `st`): the scratch, the
+// blocks released by the member's removed entities, its survivors compacted into `own`, the replicated record and flock
+// columns compacted in the scratch; receive_all also lays out `pair` (the NCCL form receives every segment). Between
+// stage and write every `from` block must be final. pf_pop_job_write: the tables at their new length and the member's
+// new range written from `from`, its appended entities and the compacted columns. pf_pop_job_commit: the host facts,
+// member lists and population facts; the scratch is reused from here on, so no peer may still read `own`.
+int pf_pop_job_check(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove, const pfnav_agent *add,
+                     const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext, const pfnav_formation_in *add_form,
+                     const pfnav_blocking *add_blk, size_t nadd, const pfnav_flock *flocks, size_t nflocks, int world, int rank,
+                     pf_pop_member &M);
+int pf_pop_job_stage(pfnav_ctx *ctx, pf_pop_member &M, bool receive_all, cudaStream_t st);
+int pf_pop_job_write(pfnav_ctx *ctx, pf_pop_member &M, cudaStream_t st);
+int pf_pop_job_commit(pfnav_ctx *ctx, pf_pop_member &M, cudaStream_t st);
+
 // ---- device helpers shared by kernels ----
 __device__ __forceinline__ uint32_t pf_lane() { return threadIdx.x & 31; }
 

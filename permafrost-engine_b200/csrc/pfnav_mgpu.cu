@@ -71,7 +71,7 @@ struct pf_mgpu {
     pf_dbuf<uint8_t> d_xgoal;                    // NCCL: the goal batch's all-gathered member records
 };
 #define PF_XCNT 8                                // {narrow, wide, sent narrow, sent wide, faction flag, 0, 0, 0}
-                                                 // or {status, n_agents, n_flocks, 0, 0, 0, 0, 0}
+                                                 // or {status, n_agents, n_flocks, tables present, 0, 0, 0, 0}
 
 bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx)
 {
@@ -797,6 +797,144 @@ extern "C" int pfnav_group_commands(pfnav_group *g, const pfnav_agent_delta *del
         pfnav_ctx *c = g->ctxs[i];
         PF_CUDA(cudaSetDevice(c->device));
         if (int rc = pf_cmd_job_apply(c, J[i], c->tick_stream)) return rc;
+    }
+    return PFNAV_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Population change of a job (pfnav_commands.cu: pf_pop_job_*). Every member gets the job's whole batch, checks it and its
+// own entities' flock indices, and describes itself in one record {status, n_agents, n_flocks, tables present}; every
+// member reads every record before anything changes. Then each member releases its removed entities' blocks, compacts its
+// own survivors and the replicated columns into its scratch, the segments of survivors that cross a member boundary move
+// (at most R + A rows per boundary), and each member writes its new range and rebuilds its member lists.
+// ------------------------------------------------------------------------------------------
+static uint32_t pop_tables_bits(const pf_pop_tables &T)
+{
+    return (T.ms ? 1u : 0u) | (T.ext ? 2u : 0u) | (T.formation ? 4u : 0u) | (T.blocking ? 8u : 0u);
+}
+
+// NCCL: per segment (sender s, receiver q) and table one broadcast from s, grouped; every rank receives every segment into
+// its receive block for the pair, so every rank makes the same calls from the plan alone
+static int nccl_pop_segments(pf_mgpu *m, pf_pop_member &M, cudaStream_t st)
+{
+    const pf_pop_job &J = M.J;
+    const int world = m->world, rank = m->rank;
+    PF_NCCL(g_nccl.GroupStart());
+    for (int s = 0; s < world; s++)
+        for (int q = 0; q < world; q++) {
+            const size_t a = J.seg_lo(s, q), n = J.seg_hi(s, q) - a;
+            if (s == q || !n) continue;
+            const pf_pop_rows &dst = M.pair[(size_t)s * world + q];
+            const size_t k = s == rank ? a - M.own.first : 0;      // the sender's rows, read on the root only
+            auto bc = [&](const void *src, void *recv, size_t bytes) {
+                return g_nccl.Broadcast(s == rank ? src : recv, recv, bytes, /*ncclInt8*/ 0, s, m->comm, st);
+            };
+            PF_NCCL(bc(M.own.agents + k, dst.agents, n * sizeof(pfnav_agent)));
+            PF_NCCL(bc(M.own.rec + k, dst.rec, n * sizeof(pf_record)));
+            PF_NCCL(bc(M.own.flock + k, dst.flock, n * 4));
+            if (M.T.ms) PF_NCCL(bc(M.own.ms + k, dst.ms, n * sizeof(pfnav_movestate)));
+            if (M.T.ext) PF_NCCL(bc(M.own.ext + k, dst.ext, n * sizeof(pfnav_movestate_ext)));
+            if (M.T.formation) PF_NCCL(bc(M.own.form + k, dst.form, n * sizeof(pfnav_formation_in)));
+            if (M.T.blocking) PF_NCCL(bc(M.own.blk + k, dst.blk, n * sizeof(pfnav_blocking)));
+        }
+    PF_NCCL(g_nccl.GroupEnd());
+    return 0;
+}
+
+extern "C" int pfnav_mgpu_change_population(pfnav_ctx *ctx, const uint32_t *remove_uids, size_t nremove, const pfnav_agent *add,
+                                            const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                            const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking,
+                                            size_t nadd, const pfnav_flock *flocks, size_t nflocks, void *stream)
+{
+    pf_mgpu *m = nullptr;
+    if (int rc = nccl_rank(ctx, __func__, "pfnav_group_change_population", &m)) return rc;
+    if (nremove == 0 && nadd == 0 && !flocks) return PFNAV_OK;     // the same arguments on every rank: none of them exchanges
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    pf_pop_member M;
+    int local = check_shard(ctx, m);
+    if (!local) local = pf_pop_job_check(ctx, remove_uids, nremove, add, add_ms, add_ext, add_formation, add_blocking, nadd, flocks,
+                                         nflocks, m->world, m->rank, M);
+    const std::string local_err = local ? pfnav_last_error() : "";
+    const int world = m->world, rank = m->rank;
+    if (int rc = m->d_xcnt.reserve((size_t)world * PF_XCNT)) return rc;
+    uint32_t *mine = m->d_xcnt + (size_t)rank * PF_XCNT;
+    const uint32_t verdict[PF_XCNT] = {(uint32_t)local, (uint32_t)ctx->n_agents, (uint32_t)ctx->n_flocks, local ? 0u : pop_tables_bits(M.T),
+                                       0, 0, 0, 0};
+    PF_CUDA(cudaMemcpyAsync(mine, verdict, sizeof(verdict), cudaMemcpyHostToDevice, st));
+    PF_NCCL(g_nccl.AllGather(mine, m->d_xcnt, PF_XCNT * sizeof(uint32_t), /*ncclInt8*/ 0, m->comm, st));
+    std::vector<uint32_t> all((size_t)world * PF_XCNT);
+    PF_CUDA(cudaMemcpyAsync(all.data(), m->d_xcnt, all.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    for (int r = 0; r < world; r++) {
+        const uint32_t *x = &all[(size_t)r * PF_XCNT];
+        if (!x[0]) continue;
+        if (r == rank) pfnav_set_error("%s: rank %d refused the batch (%s); no rank changed anything", __func__, r, local_err.c_str());
+        else pfnav_set_error("%s: rank %d refused the batch (error %d); no rank changed anything", __func__, r, (int)x[0]);
+        return (int)x[0];
+    }
+    for (int r = 0; r < world; r++)
+        PF_ARG(all[(size_t)r * PF_XCNT + 1] == all[1] && all[(size_t)r * PF_XCNT + 2] == all[2] && all[(size_t)r * PF_XCNT + 3] == all[3],
+               "ranks hold populations, flock tables or sets of uploaded tables that differ; no rank changed anything");
+    int rc;
+    if ((rc = pf_pop_job_stage(ctx, M, true, st))) return rc;
+    if (world > 1 && (rc = nccl_pop_segments(m, M, st))) return rc;
+    if ((rc = pf_pop_job_write(ctx, M, st))) return rc;
+    return pf_pop_job_commit(ctx, M, st);
+}
+
+// In-process group: the verdicts are the members' host state. Every member stages on its context stream; a receiver
+// pulls each segment straight from the sender's scratch with cudaMemcpyPeerAsync once the sender's stream has compacted
+// it (ready), and no member reuses its scratch (the member sort of the commit) before every member has pulled (pulled).
+extern "C" int pfnav_group_change_population(pfnav_group *g, const uint32_t *remove_uids, size_t nremove, const pfnav_agent *add,
+                                             const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
+                                             const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking,
+                                             size_t nadd, const pfnav_flock *flocks, size_t nflocks)
+{
+    PF_ARG(g, "group");
+    if (int rc = peer_check(g, __func__)) return rc;
+    if (nremove == 0 && nadd == 0 && !flocks) return PFNAV_OK;
+    const int world = (int)g->ctxs.size();
+    std::vector<pf_pop_member> M(world);
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        int rc = check_shard(c, (pf_mgpu *)c->mgpu);
+        if (!rc) rc = pf_pop_job_check(c, remove_uids, nremove, add, add_ms, add_ext, add_formation, add_blocking, nadd, flocks,
+                                       nflocks, world, i, M[i]);
+        if (rc) {
+            const std::string e = pfnav_last_error();
+            pfnav_set_error("%s: member %d refused the batch (%s); no member changed anything", __func__, i, e.c_str());
+            return rc;
+        }
+    }
+    for (int i = 0; i < world; i++)
+        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents && g->ctxs[i]->n_flocks == g->ctxs[0]->n_flocks &&
+               pop_tables_bits(M[i].T) == pop_tables_bits(M[0].T),
+               "members hold populations, flock tables or sets of uploaded tables that differ; no member changed anything");
+    int rc;
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        if ((rc = pf_pop_job_stage(c, M[i], false, c->tick_stream))) return rc;
+        PF_CUDA(cudaEventRecord(g->ready[i], c->tick_stream));             // member i's survivors are compacted
+    }
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        for (int s = 0; s < world; s++) {
+            if (s == i) continue;
+            M[i].from[s] = M[s].own;
+            if (M[i].J.seg_hi(s, i) > M[i].J.seg_lo(s, i)) PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->ready[s], 0));
+        }
+        if ((rc = pf_pop_job_write(c, M[i], c->tick_stream))) return rc;
+        PF_CUDA(cudaEventRecord(g->pulled[i], c->tick_stream));
+    }
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        for (int p = 0; p < world; p++)
+            if (p != i) PF_CUDA(cudaStreamWaitEvent(c->tick_stream, g->pulled[p], 0));
+        if ((rc = pf_pop_job_commit(c, M[i], c->tick_stream))) return rc;
     }
     return PFNAV_OK;
 }
