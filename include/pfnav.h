@@ -572,7 +572,9 @@ int  pfnav_agents_upload(pfnav_ctx *ctx, const pfnav_agent *agents, size_t n,
  * The engine's orders reach a job as one batch of deltas that every member receives whole (pfnav_mgpu_commands /
  * pfnav_group_commands, after pfnav_agents_commands), before the blocking calls of those commands:
  *       apply_updates_ex -> job commands + pfnav_agents_set_blocking -> exchange -> pfnav_map_commit -> gather
- *       -> pfnav_agents_set_work_dev -> tick */
+ *       -> pfnav_agents_set_work_dev -> tick
+ * After a gather every member holds the whole record column and position index, so any member answers
+ * pfnav_ents_in_circles for any query, with global uids as centres, without a collective. */
 typedef struct pfnav_group pfnav_group;
 #define PFNAV_MGPU_ID_BYTES 128
 int  pfnav_mgpu_shard_range(size_t n_total, int rank, int world, size_t *lo, size_t *hi);
@@ -1167,9 +1169,41 @@ int  pfnav_agents_read_debug(pfnav_ctx *ctx, float *out_vpref_xz, float *out_vde
                              uint8_t *out_has_los, size_t maxout);
 
 /* G_Pos_EntsInCircleFrom (position.c:379): neighbour query through the device spatial index,
- * returning uids in the reference's order. For parity tests of the index itself. */
+ * returning uids in the reference's order. One query of pfnav_ents_in_circles at a point (maxout > 0; range < 0
+ * gives 0 uids); for parity tests of the index itself. */
 int  pfnav_ents_in_circle(pfnav_ctx *ctx, float x, float z, float range, uint32_t *out,
                           int maxout, int *out_n);
+
+/* G_Pos_EntsInCircle / G_Pos_EntsInCircleFrom (position.c:379) for a batch of n queries, answered on the device from the
+ * position index. 24 bytes per query. */
+typedef struct pfnav_ents_query {
+    float    x, z;       /* centre, when uid == PFNAV_NULL_UID                                          */
+    float    range;      /* G_Pos_EntsInCircleFrom's range                                              */
+    uint32_t uid;        /* != PFNAV_NULL_UID: the centre is that entity's resident position instead   */
+    int32_t  maxout;     /* the reference's maxout: the raw hits are cut here, before the garrison filter */
+    uint32_t _pad;
+} pfnav_ents_query;
+/* - Answers: query i's uids are out_ids[out_offsets[i] .. out_offsets[i + 1]), *out_total = out_offsets[n]. Each is what
+ *   pfnav_ents_in_circle(x, z, range, maxout) returns: the same uids in the same order, including the cut at maxout and
+ *   filter_garrisoned's swap-remove when the population holds GARRISONED entities. range < 0, maxout == 0 or a centre
+ *   off the grid give an empty answer.
+ * - Uid centres: rec[uid].pos, the position the index was built from (G_Pos_EntsInCircle(G_Pos_GetXZ(uid), ...)).
+ * - Snapshot: answers come from the index of the last rebuild (pfnav_agents_rebuild_index, a gather, an upload, a solo
+ *   population change). pfnav_agents_apply_updates[_ex], the solo and job command calls, the job population change and
+ *   pfnav_agents_upload_shard on a job member write records after it; until the next rebuild the call returns
+ *   PFNAV_ERR_STATE and changes nothing, so that centres and hits always come from one snapshot.
+ * - Validation, before anything runs (PFNAV_ERR_ARG, outputs untouched): q, out_offsets and out_total non-NULL when
+ *   n > 0; out_ids non-NULL when cap > 0; x, z and range finite; maxout >= 0; uid == PFNAV_NULL_UID or uid < the whole
+ *   population (global uids on a job member); the answers' bound (the sum of min(maxout, population)) below 2^32.
+ *   n == 0 is valid (*out_total = 0). PFNAV_ERR_NO_DEVICE on a host-only context.
+ * - Capacity: *out_total > cap returns PFNAV_ERR_NOMEM with out_offsets and *out_total written and out_ids untouched:
+ *   grow the buffer and call again (cap = 0 asks for the sizes only). PFNAV_ERR_NOMEM with *out_total <= cap: the
+ *   device could not hold the answers.
+ * - Streams: queued on `stream` (NULL: the context's stream) after the rebuild and after the field work forked by
+ *   pfnav_pool_request_goals; returns when the outputs are filled. One host wait (the totals) before the final copy;
+ *   only the hits are copied back. */
+int  pfnav_ents_in_circles(pfnav_ctx *ctx, const pfnav_ents_query *q, size_t n, uint32_t *out_offsets /* n + 1 */,
+                           uint32_t *out_ids, size_t cap, size_t *out_total, void *stream);
 
 /* Device-side hooks for zero-copy callers (bench `value` leg, multi-GPU all-gather):
  * raw device pointers to the resident 24-byte neighbour records (pos.xz, vel.xz, radius,

@@ -96,6 +96,8 @@ MAP_QUERY = np.dtype([("kind", "<i4"), ("layer", "<i4"), ("x", "<f4"), ("z", "<f
 assert MAP_QUERY.itemsize == 32
 MAP_QUERY_RESULT = np.dtype([("ok", "<i4"), ("dest_id", "<u4"), ("x", "<f4"), ("z", "<f4")])
 assert MAP_QUERY_RESULT.itemsize == 16
+ENTS_QUERY = np.dtype([("x", "<f4"), ("z", "<f4"), ("range", "<f4"), ("uid", "<u4"), ("maxout", "<i4"), ("_pad", "<u4")])
+assert ENTS_QUERY.itemsize == 24
 
 LOS_PREV_INPLACE = -3
 TICK_VDES_FROM_POOL = 1
@@ -133,7 +135,7 @@ SYMBOLS = [
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
     "pfnav_mgpu_commands", "pfnav_group_commands",
     "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
-    "pfnav_mgpu_change_population", "pfnav_group_change_population",
+    "pfnav_mgpu_change_population", "pfnav_group_change_population", "pfnav_ents_in_circles",
 ]
 
 _lib = None
@@ -291,6 +293,8 @@ def load():
     L.pfnav_agents_read_velocities.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_ents_in_circle.argtypes = [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
+    L.pfnav_ents_in_circles.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t,
+                                        C.POINTER(C.c_size_t), C.c_void_p]
     L.pfnav_agents_device_ptrs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]
     L.pfnav_agents_rebuild_index.argtypes = [C.c_void_p, C.c_void_p]
     L.pfnav_profile_enable.argtypes = [C.c_void_p, C.c_int]
@@ -1059,6 +1063,24 @@ class Nav:
         n = C.c_int(0)
         _chk(self.L.pfnav_ents_in_circle(self.h, x, z, r, _p(out), maxout, C.byref(n)))
         return out[:n.value].copy()
+
+    def ents_in_circles(self, queries, cap=None, stream=0):
+        """pfnav_ents_in_circles: ENTS_QUERY records -> (offsets uint32[n + 1], ids uint32[offsets[n]]); query i's uids are
+        ids[offsets[i]:offsets[i + 1]]. `cap`: the room of the first call (default 0: it only sizes the answers); a call
+        that returns PFNAV_ERR_NOMEM is made again with room for the total it reported."""
+        q = np.ascontiguousarray(queries, ENTS_QUERY)
+        n = len(q)
+        offsets = np.zeros(n + 1, np.uint32)
+        total = C.c_size_t(0)
+        qp, op = (_p(q), _p(offsets)) if n else (None, None)
+        while True:
+            ids = np.zeros(max(cap or 0, 1), np.uint32)
+            rc = self.L.pfnav_ents_in_circles(self.h, qp, n, op, _p(ids), cap or 0, C.byref(total), C.c_void_p(stream))
+            if rc != ERR_NOMEM or cap == total.value:
+                break
+            cap = total.value
+        _chk(rc)
+        return offsets, ids[:total.value].copy()
 
     def agents_device_ptrs(self):
         a, b, n = C.c_void_p(), C.c_void_p(), C.c_size_t()

@@ -32,6 +32,7 @@
 #include "pfnav_map_view.cuh"
 
 #include "pfnav_clearpath_kernel.cuh"   // v2 helpers, ClearPath: build_vos ... clearpath_retry, clearpath_collect / _finish
+#include "pfnav_ents_query_kernel.cuh"  // GridView, the index walk grid_query / filter_garrisoned, pfnav_ents_in_circles
 
 // ------------------------------------------------------------------------------------------
 // Map / pool views
@@ -47,11 +48,6 @@ struct PoolView {
 };
 // touch == nullptr: the kernel stamps no slot
 static PoolView pool_view(const pf_pool &P, uint32_t *touch, uint32_t tick_no) { return {P.d_slot, P.d_flow, P.d_los, P.d_has, P.ndests, touch, tick_no}; }
-struct GridView {
-    const uint32_t *cell_start, *cell_count;
-    const int32_t *ix, *iy; const uint32_t *id;
-    int grid_w, grid_h; int32_t origin_x, origin_y;
-};
 
 // Entity_NavLayerWithRadius (entity.c:554)
 __device__ __forceinline__ int nav_layer_for(uint32_t flags, float radius)
@@ -212,14 +208,6 @@ __global__ void k_gather_flock_pos(const pf_record *__restrict__ rec, const uint
     if (i >= n) return;
     const pf_record r = rec[flock_members[i]];
     out[i] = make_float2(r.px, r.pz);
-}
-
-// scaled integer coordinates + cell of the position index (bitmap_grid.h: 16-wu cells)
-__device__ __forceinline__ int32_t bg_scale(float x) { return __float2int_rn(x * 256.0f); }   // BG_SCALE_F
-__device__ __forceinline__ int cell_of(int32_t i, int32_t origin, int n)
-{
-    int c = (i - origin) >> 12;
-    return min(max(c, 0), n - 1);
 }
 
 // cohesion weight exp(-6 (|d| - 37.5) / 50) = 2^(|d| * (-0.12 log2 e) + 4.5 log2 e) on the SFU (rsqrt + ex2, flush-to-zero
@@ -521,94 +509,6 @@ __global__ void k_cell_sort(const pf_record *__restrict__ rec, GridView g, const
         siy[i] = bg_scale(r.pz);
         sfl[i] = flock_of[sid[i]];
     }
-}
-
-// bg_ent_inrange_circle (bitmap_grid.h:1376): visit hits in the reference's order and hand them,
-// 32 candidates at a time, to `emit(hit, id)` (called convergently by all lanes; returns a
-// warp-uniform "stop").
-template <class F>
-__device__ __forceinline__ void grid_query(const GridView &g, float x, float z, float range, uint32_t lane,
-                                           F &&emit)
-{
-    const int32_t icx = bg_scale(x), icy = bg_scale(z), ir = bg_scale(range);
-    const long long ir2 = (long long)ir * ir;
-    const int32_t imnx = icx - ir, imxx = icx + ir, imny = icy - ir, imxy = icy + ir;
-    // _bg_cell_extent (bitmap_grid.h:1236)
-    if (imxx < g.origin_x || imxy < g.origin_y) return;
-    if (imnx >= g.origin_x + (g.grid_w << 12) || imny >= g.origin_y + (g.grid_h << 12)) return;
-    const int cx_lo = max((imnx - g.origin_x) >> 12, 0), cx_hi = min((imxx - g.origin_x) >> 12, g.grid_w - 1);
-    const int cy_lo = max((imny - g.origin_y) >> 12, 0), cy_hi = min((imxy - g.origin_y) >> 12, g.grid_h - 1);
-    // wide-query fast path: whole pool in pool order == cells in row-major order
-    const bool wide = (long long)(cx_hi - cx_lo + 1) * (cy_hi - cy_lo + 1) * 4 >= (long long)g.grid_w * g.grid_h * 3;
-    const int ax_lo = wide ? 0 : cx_lo, ax_hi = wide ? g.grid_w - 1 : cx_hi;
-    const int ay_lo = wide ? 0 : cy_lo, ay_hi = wide ? g.grid_h - 1 : cy_hi;
-    const int cstep = wide ? (1 << 30) : 8;                    // one "coarse block" spans everything when wide
-    const bool small = !wide && ir >= 0 && ir <= 12000;         // <= 46 wu
-    const int cyc_lo = wide ? 0 : ay_lo >> 3, cyc_hi = wide ? 0 : ay_hi >> 3;
-    const int cxc_lo = wide ? 0 : ax_lo >> 3, cxc_hi = wide ? 0 : ax_hi >> 3;
-    for (int cyc = cyc_lo; cyc <= cyc_hi; cyc++) {
-        for (int cxc = cxc_lo; cxc <= cxc_hi; cxc++) {
-            const int fy0 = wide ? ay_lo : max(cyc * cstep, ay_lo), fy1 = wide ? ay_hi + 1 : min(cyc * cstep + cstep, ay_hi + 1);
-            const int fx0 = wide ? ax_lo : max(cxc * cstep, ax_lo), fx1 = wide ? ax_hi + 1 : min(cxc * cstep + cstep, ax_hi + 1);
-            for (int fy = fy0; fy < fy1; fy++) {
-                // the cells fx0..fx1-1 of one fine row are adjacent in the cell-major index: one contiguous run of entries,
-                // visited in ascending cell x, in-cell order -- the reference's order
-                const uint32_t b = g.cell_start[fy * g.grid_w + fx0], e = g.cell_start[fy * g.grid_w + fx1];
-                for (uint32_t k0 = b; k0 < e; k0 += 32) {
-                    const uint32_t k = k0 + lane;
-                    bool hit = false;
-                    uint32_t id = 0;
-                    if (k < e) {
-                        if (small) {        // |d| <= range + one cell on either side: the squares fit 32 bits
-                            const int32_t dx = g.ix[k] - icx, dy = g.iy[k] - icy;
-                            hit = abs(dx) <= ir && abs(dy) <= ir && dx * dx + dy * dy <= (int32_t)ir2;
-                        } else {
-                            const long long dx = (long long)g.ix[k] - icx, dy = (long long)g.iy[k] - icy;
-                            hit = dx * dx + dy * dy <= ir2;
-                        }
-                        id = g.id[k];
-                    }
-                    if (emit(hit, id)) return;
-                }
-            }
-        }
-    }
-}
-
-__device__ __forceinline__ int filter_garrisoned(uint32_t *ids, int count, const pf_record *__restrict__ rec, uint32_t lane);
-
-__global__ void k_ents_in_circle(GridView g, float x, float z, float range, uint32_t *out, int maxout, int *out_n,
-                                 const pf_record *__restrict__ rec, int filter_garr)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    int written = 0;
-    grid_query(g, x, z, range, lane, [&](bool hit, uint32_t id) -> bool {
-        const uint32_t m = __ballot_sync(FULL, hit);
-        const int rank = __popc(m & ((1u << lane) - 1));
-        if (hit && written + rank < maxout) out[written + rank] = id;
-        written += __popc(m);
-        return written >= maxout;
-    });
-    written = min(written, maxout);
-    __syncwarp();
-    if (filter_garr) written = filter_garrisoned(out, written, rec, lane);      // position.c:379
-    if (lane == 0) *out_n = written;
-}
-
-// filter_garrisoned (position.c:100-119): swap-remove from the back, applied by G_Pos_EntsInCircleFrom
-// (position.c:379) AFTER the raw query was cut at maxout; it reorders the survivors. Serial on lane 0
-// (only runs when the population holds garrisoned entities at all); returns the new count to all lanes.
-__device__ __forceinline__ int filter_garrisoned(uint32_t *ids, int count, const pf_record *__restrict__ rec, uint32_t lane)
-{
-    int ret = count;
-    if (lane == 0) {
-        for (int i = count - 1; i >= 0; i--) {
-            if (rec[ids[i]].state_flags & PFNAV_FLAG_GARRISONED) { ids[i] = ids[ret - 1]; ret--; }
-        }
-    }
-    ret = __shfl_sync(FULL, ret, 0);
-    __syncwarp();
-    return ret;
 }
 
 #define VEL_WARPS_PER_CTA 4
@@ -968,6 +868,23 @@ static GridView grid_of(const pfnav_ctx *ctx)
     return g;
 }
 
+// The exclusive scan of count[0 .. n) into start[0 .. n], start[n] = the total, on `st`: the three k_cell_scan_* launches over
+// block sums in part (1024 words) when n spans 2 .. 1024 blocks of 4096 (scan_uses_part), else the single-CTA k_cell_scan.
+static bool scan_uses_part(int n) { const int nsb = (n + 4095) / 4096; return nsb > 1 && nsb <= 1024; }
+static void excl_scan(pfnav_ctx *ctx, const uint32_t *count, uint32_t *part, uint32_t *start, int n, cudaStream_t st)
+{
+    if (scan_uses_part(n)) {
+        const int nsb = (n + 4095) / 4096;
+        k_cell_scan_sum<<<nsb, 1024, 0, st>>>(count, part, n);
+        k_cell_scan_parts<<<1, 1024, 0, st>>>(part, nsb, start, n);
+        k_cell_scan_apply<<<nsb, 1024, 0, st>>>(count, part, start, n);
+        ctx->launches += 3;
+    } else {
+        k_cell_scan<<<1, 1024, 0, st>>>(count, start, n);
+        ctx->launches++;
+    }
+}
+
 int build_index(pfnav_ctx *ctx, cudaStream_t st)
 {
     const int n = (int)ctx->n_agents;
@@ -978,24 +895,19 @@ int build_index(pfnav_ctx *ctx, cudaStream_t st)
     if (n > 0) {
         const GridView g = grid_of(ctx);
         k_cell_count<<<(n + 255) / 256, 256, 0, st>>>(ctx->d_records, n, g, ctx->d_cell_count);
-        const int nsb = (ncells + 4095) / 4096;
-        if (nsb > 1 && nsb <= 1024) {
+        if (scan_uses_part(ncells))
             if (int rc = ctx->d_scan_part.reserve(1024)) return rc;
-            k_cell_scan_sum<<<nsb, 1024, 0, st>>>(ctx->d_cell_count, ctx->d_scan_part, ncells);
-            k_cell_scan_parts<<<1, 1024, 0, st>>>(ctx->d_scan_part, nsb, ctx->d_cell_start, ncells);
-            k_cell_scan_apply<<<nsb, 1024, 0, st>>>(ctx->d_cell_count, ctx->d_scan_part, ctx->d_cell_start, ncells);
-            ctx->launches += 2;
-        } else
-            k_cell_scan<<<1, 1024, 0, st>>>(ctx->d_cell_count, ctx->d_cell_start, ncells);
+        excl_scan(ctx, ctx->d_cell_count, ctx->d_scan_part, ctx->d_cell_start, ncells, st);
         k_cell_scatter<<<(n + 255) / 256, 256, 0, st>>>(ctx->d_records, n, g, ctx->d_cell_start, ctx->d_cell_fill,
                                                        ctx->d_sorted_id);
         k_cell_sort<<<(ncells + 127) / 128, 128, 0, st>>>(ctx->d_records, g, ctx->d_cell_start, ctx->d_sorted_id,
                                                          ctx->d_sorted_ix, ctx->d_sorted_iy, ncells, ctx->d_flock_of, ctx->d_sorted_flock);
-        ctx->launches += 4;
+        ctx->launches += 3;
     } else {
         PF_CUDA(cudaMemsetAsync(ctx->d_cell_start, 0, (size_t)(ncells + 1) * 4, st));
     }
     PF_CUDA(cudaGetLastError());
+    ctx->index_stale = false;
     return 0;
 }
 
@@ -1131,6 +1043,7 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
         // the other ranges' records (and, when membership may have changed, flock ids) come from the peers;
         // pfnav_mgpu_gather / pfnav_group_gather follows and finishes the snapshot (index, facts, member lists)
         ctx->members_stale = !same;
+        ctx->index_stale = true;
         PF_CUDA(cudaStreamSynchronize(st));
         return PFNAV_OK;
     }
@@ -1382,26 +1295,100 @@ extern "C" int pfnav_agents_read_debug(pfnav_ctx *ctx, float *out_vpref_xz, floa
     return PFNAV_OK;
 }
 
+// The queries q[0 .. n) on `st` (validated; n > 0): the count pass, the scan of the answer lengths (and of the garrison
+// scratch), one host wait for the offsets and totals, then the write pass into d_eq_ids and the copy of the hits. The
+// queries, counts and offsets live in the request staging; the answers in d_eq_ids, whose size the count pass decides.
+static int ents_query_run(pfnav_ctx *ctx, cudaStream_t st, const pfnav_ents_query *q, size_t n, uint32_t *out_offsets,
+                          uint32_t *out_ids, size_t cap, size_t *out_total)
+{
+    const int garr = ctx->any_garrisoned ? 1 : 0;
+    const auto up16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t o_cnt = up16(n * sizeof(pfnav_ents_query)), o_off = o_cnt + up16(n * 4), o_scr = o_off + up16((n + 1) * 4);
+    const size_t o_soff = o_scr + (garr ? up16(n * 4) : 0), o_part = o_soff + (garr ? up16((n + 1) * 4) : 0);
+    pf_stage S;
+    if (int rc = pf_stage_begin(ctx, st, std::max(n * sizeof(pfnav_ents_query), (n + 2) * 4), o_part + 1024 * 4, false, &S))
+        return rc;
+    memcpy(S.host, q, n * sizeof(pfnav_ents_query));
+    if (int rc = pf_stage_upload(ctx, st, S, n * sizeof(pfnav_ents_query))) return rc;
+    const pfnav_ents_query *d_q = (const pfnav_ents_query *)S.dev;
+    uint32_t *d_cnt = (uint32_t *)(S.dev + o_cnt), *d_off = (uint32_t *)(S.dev + o_off), *d_part = (uint32_t *)(S.dev + o_part);
+    uint32_t *d_scr = garr ? (uint32_t *)(S.dev + o_scr) : nullptr, *d_soff = garr ? (uint32_t *)(S.dev + o_soff) : nullptr;
+    const GridView g = grid_of(ctx);
+    const unsigned grid = (unsigned)((n + EQ_WARPS - 1) / EQ_WARPS);
+    k_ents_count<<<grid, EQ_WARPS * 32, 0, st>>>(g, ctx->d_records, d_q, (int)n, garr, d_cnt, d_scr);
+    ctx->launches++;
+    excl_scan(ctx, d_cnt, d_part, d_off, (int)n, st);
+    if (garr) excl_scan(ctx, d_scr, d_part, d_soff, (int)n, st);
+    PF_CUDA(cudaGetLastError());
+    // the offsets and the scratch total come back through the pinned buffer: the one host wait
+    uint32_t *h = (uint32_t *)S.host;
+    PF_CUDA(cudaMemcpyAsync(h, d_off, (n + 1) * 4, cudaMemcpyDeviceToHost, st));
+    if (garr) PF_CUDA(cudaMemcpyAsync(h + n + 1, d_soff + n, 4, cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    const size_t total = h[n], scr_total = garr ? h[n + 1] : 0;
+    memcpy(out_offsets, h, (n + 1) * 4);
+    *out_total = total;
+    if (total > cap) {
+        if (int rc = pf_stage_done(ctx, st)) return rc;
+        pfnav_set_error("pfnav_ents_in_circles: the answers hold %zu uids, out_ids %zu", total, cap);
+        return PFNAV_ERR_NOMEM;
+    }
+    if (total > 0) {
+        if (int rc = ctx->d_eq_ids.reserve(total + scr_total)) return rc;
+        k_ents_write<<<grid, EQ_WARPS * 32, 0, st>>>(g, ctx->d_records, d_q, (int)n, d_off, d_soff, ctx->d_eq_ids,
+                                                     ctx->d_eq_ids + total);
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+        PF_CUDA(cudaMemcpyAsync(out_ids, ctx->d_eq_ids, total * 4, cudaMemcpyDeviceToHost, st));
+    }
+    if (int rc = pf_stage_done(ctx, st)) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
+    return PFNAV_OK;
+}
+
 extern "C" int pfnav_ents_in_circle(pfnav_ctx *ctx, float x, float z, float range, uint32_t *out, int maxout, int *out_n)
 {
     PF_ARG(ctx && ctx->d_records && out && out_n && maxout > 0, "args");
     PF_CUDA(cudaSetDevice(ctx->device));
     if (range < 0.0f) { *out_n = 0; return PFNAV_OK; }
-    cudaStream_t st = ctx->tick_stream;
-    // staged: the count, then the ids; only the ids found are copied back
-    pf_stage S;
-    if (int rc = pf_stage_begin(ctx, st, 0, 16 + (size_t)maxout * 4, false, &S)) return rc;
-    int *d_n = (int *)S.dev;
-    uint32_t *d_out = (uint32_t *)(S.dev + 16);
-    k_ents_in_circle<<<1, 32, 0, st>>>(grid_of(ctx), x, z, range, d_out, maxout, d_n, ctx->d_records, ctx->any_garrisoned ? 1 : 0);
-    ctx->launches++;
-    PF_CUDA(cudaGetLastError());
-    PF_CUDA(cudaMemcpyAsync(out_n, d_n, 4, cudaMemcpyDeviceToHost, st));
-    PF_CUDA(cudaStreamSynchronize(st));
-    if (*out_n > 0) PF_CUDA(cudaMemcpyAsync(out, d_out, (size_t)*out_n * 4, cudaMemcpyDeviceToHost, st));
-    if (int rc = pf_stage_done(ctx, st)) return rc;
-    PF_CUDA(cudaStreamSynchronize(st));
+    const pfnav_ents_query q = {x, z, range, PFNAV_NULL_UID, maxout, 0u};
+    uint32_t off[2];
+    size_t total = 0;
+    if (int rc = ents_query_run(ctx, ctx->tick_stream, &q, 1, off, out, (size_t)maxout, &total)) return rc;
+    *out_n = (int)total;
     return PFNAV_OK;
+}
+
+extern "C" int pfnav_ents_in_circles(pfnav_ctx *ctx, const pfnav_ents_query *q, size_t n, uint32_t *out_offsets,
+                                     uint32_t *out_ids, size_t cap, size_t *out_total, void *stream)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(ctx->d_records, "agents not uploaded");
+    PF_ARG(n == 0 || (q && out_offsets && out_total), "null argument");
+    PF_ARG(cap == 0 || out_ids, "out_ids == NULL with cap > 0");
+    PF_ARG(n <= 0x7fffffff, "n");
+    uint64_t bound = 0;
+    for (size_t i = 0; i < n; i++) {
+        const pfnav_ents_query &a = q[i];
+        PF_ARG(isfinite(a.x) && isfinite(a.z) && isfinite(a.range), "query x, z and range must be finite");
+        PF_ARG(a.maxout >= 0, "query maxout < 0");
+        PF_ARG(a.uid == PFNAV_NULL_UID || a.uid < ctx->n_agents, "query uid outside the population");
+        if (a.range >= 0.0f) bound += std::min<uint64_t>((uint64_t)a.maxout, ctx->n_agents);
+    }
+    PF_ARG(bound <= 0xffffffffull, "the answers could exceed 2^32 uids");
+    if (ctx->index_stale) {
+        pfnav_set_error("pfnav_ents_in_circles: records were written after the last index build (pfnav_agents_rebuild_index "
+                        "or a gather first)");
+        return PFNAV_ERR_STATE;
+    }
+    if (n == 0) {
+        if (out_offsets) out_offsets[0] = 0;
+        if (out_total) *out_total = 0;
+        return PFNAV_OK;
+    }
+    PF_CUDA(cudaSetDevice(ctx->device));
+    return ents_query_run(ctx, pf_stream(ctx, stream), q, n, out_offsets, out_ids, cap, out_total);
 }
 
 
@@ -2177,6 +2164,7 @@ extern "C" int pfnav_agents_apply_updates_ex(pfnav_ctx *ctx, uint32_t flags, voi
         if (rc) return rc;
     }
     pf_prof_scope prof(ctx, st, PF_PROF_APPLY);
+    ctx->index_stale = true;
     k_entity_apply<<<(nwork + 127) / 128, 128, 0, st>>>(ctx->d_agents, ctx->d_movestate, ctx->d_records, ctx->d_work, nwork,
                                                        ctx->d_patches, ctx->d_ms_ext);
     ctx->launches++;

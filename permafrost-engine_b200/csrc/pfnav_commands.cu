@@ -365,6 +365,7 @@ static int cmd_apply(pfnav_ctx *ctx, cudaStream_t st, const std::vector<pfnav_ag
                      const std::vector<pf_cmd_foreign> &foreign, const std::vector<pf_cmd_change> &changes,
                      const pfnav_flock *flocks, size_t nflocks)
 {
+    ctx->index_stale = true;            // the deltas write records: the position index waits for the next rebuild
     uint32_t any = 0;
     for (const pfnav_agent_delta &m : merged) any |= m.mask;
     for (const pf_cmd_foreign &f : foreign) any |= f.mask;
@@ -712,6 +713,7 @@ int pf_pop_job_stage(pfnav_ctx *ctx, pf_pop_member &M, bool receive_all, cudaStr
 
 int pf_pop_job_write(pfnav_ctx *ctx, pf_pop_member &M, cudaStream_t st)
 {
+    ctx->index_stale = true;            // new records until the gather rebuilds the index
     const pf_pop_job &J = M.J;
     const pf_pop_tables &T = M.T;
     const int r = J.rank, world = J.world;

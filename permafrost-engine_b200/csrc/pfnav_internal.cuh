@@ -194,6 +194,10 @@ struct pfnav_ctx {
     pf_dbuf<int32_t> d_sorted_ix, d_sorted_iy;                       // per-entity (pf_agents_reserve)
     pf_dbuf<uint32_t> d_sorted_id;
     pf_dbuf<int32_t> d_sorted_flock;                                 // flock id of every index entry (windowed cohesion)
+    // records written since the last index build (pfnav_ents_in_circles refuses then): set by the record writers,
+    // cleared by build_index
+    bool index_stale = false;
+    pf_dbuf<uint32_t> d_eq_ids;                                      // pfnav_ents_in_circles: the answers, then the garrison scratch
     pf_dbuf<uint32_t> d_coh_fallback;
     pf_dbuf<uint32_t> d_scan_part;                                   // block sums of the cell-count scan
     pf_dbuf<unsigned long long> d_cp_stats;                          // ClearPath event counters (pfnav_agents_clearpath_stats)
