@@ -1131,6 +1131,41 @@ int  pfnav_mgpu_request_entity_fields_batch(pfnav_ctx *ctx, const pfnav_entity_f
 int  pfnav_group_request_entity_fields_batch(pfnav_group *g, const pfnav_entity_field_req *reqs, size_t m,
                                              const pfnav_footprint *ents, size_t nents,
                                              const int32_t *chunks_rc, size_t nchunks);
+/* pfnav_pool_request_entity_fields_batch with the moving entities and the seekers named by uid, resolved on the device
+ * from the resident records, so that the device-resident loop needs no positions on the host.
+ * - Footprints: footprint k is ents[k] when ent_uids is NULL or ent_uids[k] == PFNAV_NULL_UID; otherwise it is the circle
+ *   of resident entity ent_uids[k]: x, z = rec[uid].pos, sel_radius = rec[uid].radius, is_building = 0. ents may be NULL
+ *   only when every entry names a uid. Buildings, and anything else outside the population, come in as footprints in
+ *   the same array, so one enemy list can mix the two.
+ * - Chunks: request i's chunk_off / chunk_n index seeker_uids, not chunks_rc. Its chunks are those of the tiles under
+ *   those seekers' resident positions (M_Tile_DescForPoint2D, as the tick takes it), each once, in the order of its
+ *   first seeker. A seeker whose position has no tile under it is PFNAV_ERR_ARG.
+ * - Equivalence: the call leaves everything exactly as pfnav_pool_request_entity_fields_batch leaves it when given the
+ *   footprints and chunk lists these rules resolve from the records as they are at the call: flow bytes, `has` bytes,
+ *   the ff_id pfnav_pool_get reports, LRU slot choices and evictions, the footprints pfnav_pool_repair[_batch] starts
+ *   from, *out_ndone and the NOMEM stop, and "a later request wins".
+ * - Snapshot: as pfnav_ents_in_circles. Records written since the last index build (apply, commands, a job member's
+ *   population change, pfnav_agents_upload_shard on a job member) give PFNAV_ERR_STATE and nothing changes. In the
+ *   resident loop the call goes after pfnav_agents_rebuild_index / the gather and before pfnav_agents_set_work_dev and
+ *   the tick.
+ * - Validation before anything changes: everything the batch validates, applied to the resolved inputs; every uid below
+ *   the whole population (global uids on a job member); nents, nseekers < 2^24; the NULL rules above. m == 0 is valid
+ *   and resolves nothing. PFNAV_ERR_NO_DEVICE on a host-only context.
+ * - Streams: queued on `stream` (NULL: the context's stream) after the forked field work, like the batch. One host wait
+ *   reads the resolved values back (12 bytes per named footprint, 4 per seeker); after it, the batch's own behaviour.
+ * The job forms relate to pfnav_mgpu_request_entity_fields_batch / pfnav_group_request_entity_fields_batch the same way
+ * and keep their all or nothing: each member resolves from its own record column (equal on every member after a
+ * gather), and a member that cannot resolve the batch (stale records, a seeker off the map) refuses it, so every
+ * member returns that error and no pool changes. */
+int  pfnav_pool_request_entity_fields_resident(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                               const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents,
+                                               const uint32_t *seeker_uids, size_t nseekers, void *stream, int *out_ndone);
+int  pfnav_mgpu_request_entity_fields_resident(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                               const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents,
+                                               const uint32_t *seeker_uids, size_t nseekers, void *stream);
+int  pfnav_group_request_entity_fields_resident(pfnav_group *g, const pfnav_entity_field_req *reqs, size_t m,
+                                                const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents,
+                                                const uint32_t *seeker_uids, size_t nseekers);
 
 /* Test / tuning hook for pfnav_agents_tick: 0 = single-pass velocity kernel; 1 (default) = while LOS chains of
  * pfnav_pool_request_goals are still in flight, run the part of the update that does not depend on the

@@ -131,7 +131,8 @@ SYMBOLS = [
     "pfnav_mgpu_exchange_blocker_ops", "pfnav_group_exchange_blocker_ops",
     "pfnav_mgpu_request_goals_ex", "pfnav_group_request_goals_ex", "pfnav_mgpu_fields_stats",
     "pfnav_mgpu_request_zones", "pfnav_group_request_zones", "pfnav_mgpu_request_entity_fields_batch",
-    "pfnav_group_request_entity_fields_batch",
+    "pfnav_group_request_entity_fields_batch", "pfnav_pool_request_entity_fields_resident",
+    "pfnav_mgpu_request_entity_fields_resident", "pfnav_group_request_entity_fields_resident",
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
     "pfnav_mgpu_commands", "pfnav_group_commands",
     "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
@@ -289,6 +290,12 @@ def load():
                                                          C.c_size_t, C.c_void_p]
     L.pfnav_group_request_entity_fields_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                                           C.c_size_t]
+    L.pfnav_pool_request_entity_fields_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                            C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]
+    L.pfnav_mgpu_request_entity_fields_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                            C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_group_request_entity_fields_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                                             C.c_size_t, C.c_void_p, C.c_size_t]
     L.pfnav_agents_tick.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     L.pfnav_agents_read_velocities.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
@@ -334,6 +341,20 @@ def _command_args(deltas, flocks):
     fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
     fp = None if fl is None else _p(fl if len(fl) else np.zeros(1, FLOCK))     # an empty table is still a table
     return _p(d) if len(d) else None, len(d), fp, 0 if fl is None else len(fl)
+
+
+def _resident_args(reqs, footprints, ent_uids, seekers):
+    """the pointer arguments of the *_request_entity_fields_resident calls: (reqs, m, ents, ent_uids, nents, seekers,
+    nseekers), with the arrays kept alive in the returned tuple's last item"""
+    reqs = np.ascontiguousarray(reqs, ENTITY_FIELD_REQ)
+    fp = None if footprints is None else np.ascontiguousarray(footprints, FOOTPRINT)
+    uids = None if ent_uids is None else np.ascontiguousarray(ent_uids, np.uint32)
+    sk = np.ascontiguousarray(seekers, np.uint32)
+    nents = len(fp) if fp is not None else (0 if uids is None else len(uids))
+    if fp is not None and uids is not None and len(uids) != len(fp):
+        raise ValueError("footprints and ent_uids differ in length")
+    ptr = lambda a: _p(a) if a is not None and len(a) else None
+    return (ptr(reqs), len(reqs), ptr(fp), ptr(uids), nents, ptr(sk), len(sk), (reqs, fp, uids, sk))
 
 
 def _chk(rc):
@@ -890,6 +911,12 @@ class Nav:
                                                            _p(fp) if len(fp) else None, len(fp), _p(ch) if len(ch) else None,
                                                            len(ch), C.c_void_p(stream)))
 
+    def mgpu_request_entity_fields_resident(self, reqs, footprints, ent_uids, seekers, stream=0):
+        """collective: pool_request_entity_fields_resident for the whole job, each member resolving the uids from its own
+        records and each field built on one rank; all or nothing across the ranks"""
+        a = _resident_args(reqs, footprints, ent_uids, seekers)
+        _chk(self.L.pfnav_mgpu_request_entity_fields_resident(self.h, *a[:7], C.c_void_p(stream)))
+
     def mgpu_fields_stats(self, ngoals):
         """test hook: this member's last job batch -> (fields built: flow requests or zone / entity fields, LOS requests
         built, owner per goal or request)"""
@@ -944,6 +971,18 @@ class Nav:
         rc = self.L.pfnav_pool_request_entity_fields_batch(self.h, _p(reqs) if len(reqs) else None, len(reqs), _p(fp) if len(fp) else None,
                                                            len(fp), _p(ch) if len(ch) else None, len(ch), C.c_void_p(stream),
                                                            C.byref(ndone))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        return ndone.value
+
+    def pool_request_entity_fields_resident(self, reqs, footprints, ent_uids, seekers, stream=0):
+        """pool_request_entity_fields_batch with footprints and seekers named by uid -> ndone. `footprints`: FOOTPRINT
+        records or None (every entry names a uid); `ent_uids`: uint32 per footprint (NULL_UID: use footprints[k]) or None
+        (use `footprints` as given); `seekers`: uint32 uids, which the requests' chunk ranges index. ndone < len(reqs): the
+        pool could not hold request ndone's fields (PFNAV_ERR_NOMEM); requests before it are done."""
+        a = _resident_args(reqs, footprints, ent_uids, seekers)
+        ndone = C.c_int(0)
+        rc = self.L.pfnav_pool_request_entity_fields_resident(self.h, *a[:7], C.c_void_p(stream), C.byref(ndone))
         if rc != ERR_NOMEM:
             _chk(rc)
         return ndone.value
@@ -1175,6 +1214,12 @@ class Group:
         _chk(load().pfnav_group_request_entity_fields_batch(self.g, _p(reqs) if len(reqs) else None, len(reqs),
                                                             _p(fp) if len(fp) else None, len(fp), _p(ch) if len(ch) else None,
                                                             len(ch)))
+
+    def request_entity_fields_resident(self, reqs, footprints, ent_uids, seekers):
+        """request_entity_fields_batch with footprints and seekers named by uid (Nav.pool_request_entity_fields_resident),
+        each member resolving them from its own records; all or nothing across the members"""
+        a = _resident_args(reqs, footprints, ent_uids, seekers)
+        _chk(load().pfnav_group_request_entity_fields_resident(self.g, *a[:7]))
 
     def commands(self, deltas, flocks=None):
         """agents_commands for the whole group: the job's whole batch (global uids), each member applying its own

@@ -15,6 +15,7 @@
 #include "pfnav_pool_host.h"
 #include "pfnav_commands_host.h"
 #include "pfnav_waves_host.h"
+#include "pfnav_resident_host.h"
 
 #define PFNAV_VERSION 100
 
@@ -364,6 +365,13 @@ bool pf_blocker_ops_unexchanged(pfnav_ctx *ctx);                // pfnav_blocker
 __host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(range >= 0.0f && (int)ceilf(range / 4) <= 12); }
 
 int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, std::vector<int> &out);     // pfnav_region.cu
+// The inputs of an entity-field batch named by uid (pfnav_*_request_entity_fields_resident; pfnav_region.cu): checks the
+// arguments (pf_resident_check), refuses stale records (PFNAV_ERR_STATE), resolves the named uids from the context's
+// records with k_resident_footprints on `st` (one host wait) and merges them (pf_resident_merge). m == 0 resolves
+// nothing. Changes nothing but the request staging.
+int pf_resident_resolve(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_field_req *reqs, size_t m,
+                        const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents, const uint32_t *seeker_uids,
+                        size_t nseekers, pf_resident_batch &B);
 
 // ---- pfnav_pool.cu: the device pool, and the pool mutators of a context, each of which drops the resident goal plan
 // Bring the device copies of the pool up to date after pfnav_pool_clear: empty slot table, no `has` bytes, zero touch
@@ -429,6 +437,7 @@ struct pf_job {
     std::vector<uint8_t> lack;
     std::vector<size_t> seg;                        // pf_job_launch: world + 1 block offsets
     const void *d_items = nullptr; int nitems = 0;  // the member's copies from staging into its pool
+    int refused = 0;                                // the member's verdict before planning (a resident batch it could not resolve)
 };
 int pf_job_plan(pfnav_ctx *ctx, pf_job &J);
 int pf_job_launch(pfnav_ctx *ctx, pf_job &J, const uint8_t *uni, int world, int rank, cudaStream_t st);

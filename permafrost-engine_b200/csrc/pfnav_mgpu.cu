@@ -513,7 +513,7 @@ static int nccl_member(pfnav_ctx *ctx, const char *fn, const char *group_fn, pf_
 // broadcasts (one per owner with a non-empty segment) on `stream`, the copies into the pool on `stream`.
 static int nccl_job(pfnav_ctx *ctx, pf_mgpu *m, pf_job &J, cudaStream_t st, const char *fn)
 {
-    const int local = pf_job_plan(ctx, J);
+    const int local = J.refused ? J.refused : pf_job_plan(ctx, J);
     const std::string local_err = local ? pfnav_last_error() : "";
     // record: {verdict, fits, 0, 0} then, for a goal batch, one lack byte per (goal, chunk); every rank has the same
     // arguments and map
@@ -590,7 +590,7 @@ static int group_job(pfnav_group *g, std::vector<pf_job> &J, const char *fn)
     const int world = (int)g->ctxs.size();
     int rc = 0;
     for (int i = 0; i < world; i++)
-        if ((rc = pf_job_plan(g->ctxs[i], J[i]))) return rc;            // no member has changed anything yet
+        if ((rc = J[i].refused ? J[i].refused : pf_job_plan(g->ctxs[i], J[i]))) return rc;   // no member has changed anything yet
     for (int i = 0; i < world; i++)
         if (!J[i].fits) {
             pfnav_set_error("%s: the field pool of member %d cannot hold its fields; no member changed its pool", fn, i);
@@ -728,6 +728,46 @@ extern "C" int pfnav_group_request_entity_fields_batch(pfnav_group *g, const pfn
     if (m == 0) return PFNAV_OK;
     std::vector<pf_job> J(g->ctxs.size());
     for (pf_job &j : J) job_init_entity(j, reqs, m, ents, nents, chunks_rc, nchunks);
+    return group_job(g, J, __func__);
+}
+
+// Named by uid: each member resolves the batch from its own record column, which a gather made equal on every member, so
+// every member plans the same batch. A member that cannot resolve it (stale records, a seeker off the map) enters the
+// error as its verdict, and the verdicts are exchanged as for any batch.
+extern "C" int pfnav_mgpu_request_entity_fields_resident(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                                         const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents,
+                                                         const uint32_t *seeker_uids, size_t nseekers, void *stream)
+{
+    pf_mgpu *mg = nullptr;
+    if (int rc = nccl_member(ctx, __func__, "pfnav_group_request_entity_fields_resident", &mg)) return rc;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    const cudaStream_t st = pf_stream(ctx, stream);
+    pf_resident_batch B;
+    const int rc = pf_resident_resolve(ctx, st, reqs, m, ents, ent_uids, nents, seeker_uids, nseekers, B);
+    if (m == 0) return rc;                  // nothing resolved: every rank has the same arguments and population
+    pf_job J;
+    job_init_entity(J, B.reqs.data(), m, B.ents.data(), nents, B.chunks_rc.data(), B.chunks_rc.size() / 2);
+    J.refused = rc;
+    return nccl_job(ctx, mg, J, st, __func__);
+}
+
+extern "C" int pfnav_group_request_entity_fields_resident(pfnav_group *g, const pfnav_entity_field_req *reqs, size_t m,
+                                                          const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents,
+                                                          const uint32_t *seeker_uids, size_t nseekers)
+{
+    if (int rc = group_members(g, __func__)) return rc;
+    const size_t world = g->ctxs.size();
+    std::vector<pf_resident_batch> B(world);
+    std::vector<pf_job> J(world);
+    for (size_t i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        const int rc = pf_resident_resolve(c, c->tick_stream, reqs, m, ents, ent_uids, nents, seeker_uids, nseekers, B[i]);
+        if (m == 0 && rc) return rc;
+        job_init_entity(J[i], B[i].reqs.data(), m, B[i].ents.data(), nents, B[i].chunks_rc.data(), B[i].chunks_rc.size() / 2);
+        J[i].refused = rc;
+    }
+    if (m == 0) return PFNAV_OK;
     return group_job(g, J, __func__);
 }
 

@@ -25,6 +25,7 @@
 
 namespace {
 
+#include "pfnav_map_view.cuh"
 #include "pfnav_region_kernel.cuh"
 #include "pfnav_tile_geom.cuh"
 #include "pfnav_zone_kernel.cuh"
@@ -1191,6 +1192,92 @@ extern "C" int pfnav_pool_request_entity_fields_batch(pfnav_ctx *ctx, const pfna
         if (last[fields[f].slot] == (int32_t)f) build.push_back(fields[f]);
     const int lrc = entity_build(ctx, st, reqs, ents, nents, E, build, true, ctx->pool.d_flow);
     return lrc ? lrc : rc;
+}
+
+// ------------------------------------------------------------------------------------------
+// Entity-field batches named by uid (pfnav_pool_request_entity_fields_resident and its job forms): the footprints and
+// the seekers' chunks come from the resident records, then the batch runs on them as given.
+// ------------------------------------------------------------------------------------------
+namespace {
+
+// one thread per named uid: the first nfp name footprints ({x, z, radius} of the record), the rest seekers (the chunk
+// index under the record's position, M_Tile_DescForPoint2D as the tick takes it; -1 when no tile lies under it)
+__global__ void __launch_bounds__(256) k_resident_footprints(const pf_record *__restrict__ rec, const uint32_t *__restrict__ uids,
+                                                             int nfp, int n, MapView m, float *__restrict__ fp_out,
+                                                             int32_t *__restrict__ chunk_out)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const pf_record r = rec[uids[i]];
+    if (i < nfp) {
+        fp_out[3 * i] = r.px; fp_out[3 * i + 1] = r.pz; fp_out[3 * i + 2] = r.radius;
+        return;
+    }
+    tile_desc t;
+    chunk_out[i - nfp] = desc_for_point(m, r.px, r.pz, t) ? t.chunk_r * m.chunk_w + t.chunk_c : -1;
+}
+
+}   // namespace
+
+int pf_resident_resolve(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_field_req *reqs, size_t m,
+                        const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents, const uint32_t *seeker_uids,
+                        size_t nseekers, pf_resident_batch &B)
+{
+    PF_ARG(ctx->d_cost && ctx->pool.d_slot, "map / pool not created");
+    pf_resident_names N;
+    const char *err = nullptr;
+    if (pf_resident_check(reqs, m, ents, ent_uids, nents, seeker_uids, nseekers, ctx->n_agents, N, &err)) PF_ARG(false, err);
+    if (m == 0) return PFNAV_OK;
+    if (ctx->index_stale) {
+        pfnav_set_error("entity fields by uid: records were written after the last index build (pfnav_agents_rebuild_index "
+                        "or a gather first)");
+        return PFNAV_ERR_STATE;
+    }
+    const size_t n = N.uids.size(), nfp = N.fp_index.size();
+    std::vector<float> fp_xzr(3 * nfp);
+    std::vector<int32_t> seek_chunk(nseekers);
+    if (n) {
+        // the uids in, the resolved values out, through the request staging; the one host wait
+        const auto up16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+        const size_t o_fp = up16(n * 4), o_ch = o_fp + up16(nfp * 12), need = o_ch + nseekers * 4;
+        PF_CUDA(cudaSetDevice(ctx->device));
+        pf_stage S;
+        if (int rc = pf_stage_begin(ctx, st, std::max(n * 4, need - o_fp), need, false, &S)) return rc;
+        memcpy(S.host, N.uids.data(), n * 4);
+        if (int rc = pf_stage_upload(ctx, st, S, n * 4)) return rc;
+        MapView mv = {};
+        mv.W64 = ctx->W64; mv.H64 = ctx->H64; mv.chunk_w = ctx->chunk_w; mv.chunk_h = ctx->chunk_h;
+        mv.map_x = ctx->map_x; mv.map_z = ctx->map_z;
+        k_resident_footprints<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ctx->d_records, (const uint32_t *)S.dev, (int)nfp,
+                                                                          (int)n, mv, (float *)(S.dev + o_fp),
+                                                                          (int32_t *)(S.dev + o_ch));
+        ctx->launches++;
+        PF_CUDA(cudaGetLastError());
+        PF_CUDA(cudaMemcpyAsync(S.host, S.dev + o_fp, need - o_fp, cudaMemcpyDeviceToHost, st));
+        if (int rc = pf_stage_done(ctx, st)) return rc;
+        PF_CUDA(cudaStreamSynchronize(st));
+        memcpy(fp_xzr.data(), S.host, nfp * 12);
+        memcpy(seek_chunk.data(), S.host + (o_ch - o_fp), nseekers * 4);
+    }
+    if (pf_resident_merge(reqs, m, ents, nents, N, fp_xzr.data(), seek_chunk.data(), nseekers, ctx->chunk_w, ctx->chunk_h, B, &err))
+        PF_ARG(false, err);
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_pool_request_entity_fields_resident(pfnav_ctx *ctx, const pfnav_entity_field_req *reqs, size_t m,
+                                                         const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents,
+                                                         const uint32_t *seeker_uids, size_t nseekers, void *stream,
+                                                         int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    pf_resident_batch B;
+    if (int rc = pf_resident_resolve(ctx, pf_stream(ctx, stream), reqs, m, ents, ent_uids, nents, seeker_uids, nseekers, B))
+        return rc;
+    if (m == 0) return PFNAV_OK;
+    return pfnav_pool_request_entity_fields_batch(ctx, B.reqs.data(), m, B.ents.data(), nents, B.chunks_rc.data(),
+                                                  B.chunks_rc.size() / 2, stream, out_ndone);
 }
 
 // ------------------------------------------------------------------------------------------
