@@ -911,6 +911,45 @@ int  pfnav_agents_read_blocking(pfnav_ctx *ctx, pfnav_blocking *out, size_t maxo
  * (pfnav_mgpu_share_blockers / pfnav_group_share_blockers) exchanges them before the commit; its members' tables
  * cover their own ranges (see there). On a single context the own range is the whole population. */
 int  pfnav_agents_apply_updates_ex(pfnav_ctx *ctx, uint32_t flags, void *stream);
+/* What the tick decided, for the engine to act on: one record per work item whose patch the apply applies (the entity is
+ * not GARRISONED) and that has SET_STATE, SET_MOVING or SET_DEST in its flags or a non-zero engine_todo. They drive
+ * entity_finish_moving (ARRIVED / WAITING: events, combat stance), move_notify_motion_start (SET_MOVING), the re-issued
+ * move order G_Move_SetDest (SET_DEST) and the surround decisions and field requests of engine_todo. 48 bytes. */
+typedef struct pfnav_event {
+    uint32_t uid;                     /* the work item's uid, numbered as at the collect call                           */
+    uint32_t flags;                   /* the patch's flags, PFNAV_UPDATE_* (all of them)                                 */
+    uint32_t todo;                    /* the patch's engine_todo, PFNAV_TODO_*                                          */
+    int32_t  attack;                  /* the patch's next_attack (meaningful with SET_DEST)                              */
+    uint32_t state_before;            /* agent.state before the apply                                                   */
+    uint32_t state_after;             /* agent.state as the apply leaves it: SET_STATE writes next_state, then SET_MOVING
+                                       * writes it again; neither: state_before                                         */
+    float    dest[2];                 /* the patch's next_dest (meaningful with SET_DEST)                                */
+    float    pos[2];                  /* agent.pos (x, z) as the apply leaves it: SET_POSITION ? next_pos x, z : agent.pos */
+    uint32_t _pad[2];
+} pfnav_event;
+/* Collect the events of the last update pass, in work order, into a context-owned device list. Every field is a copy of
+ * what pfnav_agents_read_patches and pfnav_agents_read_state would give (state_before and agent.pos read before the
+ * apply), so the list equals the host filter of those two read-backs bit for bit.
+ * - Call it after pfnav_agents_compute_updates and before the apply of that pass (pfnav_agents_apply_updates[_ex]), on
+ *   the same stream: it reads the state and positions the apply overwrites.
+ * - Asynchronous on `stream`: no host wait. The count stays on the device. The list is reserved for n_work records
+ *   before the launch; it waits for the device only when it has to grow. An empty work list gives an empty list.
+ * - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_ARG when no update pass has run; PFNAV_ERR_STATE
+ *   when the last update pass has already been applied. Nothing changes on an error.
+ * Multi-GPU jobs: a member collects its own work items, with global uids; no collective is involved. When the members'
+ * work lists come from pfnav_agents_set_work_dev, their lists joined in rank order equal the list of one context holding
+ * the whole population. */
+int  pfnav_agents_collect_events(pfnav_ctx *ctx, void *stream);
+/* Read the list of the last collect: *out_n = its length, out[0 .. *out_n) the records. It waits for the collect
+ * through an event recorded after it (not for later work on any stream) and copies through pinned memory.
+ * - maxout < the length: PFNAV_ERR_NOMEM with *out_n set and out untouched; the list stays readable, so grow out and
+ *   call again (maxout = 0 asks for the length only).
+ * - The list stays readable, as often as wanted, until the next collect.
+ * - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_ARG for a NULL out_n, or a NULL out with maxout > 0;
+ *   PFNAV_ERR_STATE when no collect has run, or when a call that renumbers the population has changed it since the
+ *   collect (pfnav_agents_upload, pfnav_agents_upload_shard, pfnav_agents_change_population,
+ *   pfnav_mgpu_change_population, pfnav_group_change_population): the uids would no longer name the same entities. */
+int  pfnav_agents_read_events(pfnav_ctx *ctx, pfnav_event *out, size_t maxout, size_t *out_n);
 /* The engine's own entity_block (block != 0) / entity_unblock (block == 0) for commands (stop, new move order) for n
  * uids, with the rules and the op buffer of PFNAV_APPLY_BLOCKERS: blocking at the entity's current position. Repeats
  * (within a call or across calls) change nothing. Errors as pfnav_agents_apply_updates_ex's, and PFNAV_ERR_ARG (nothing

@@ -98,6 +98,9 @@ MAP_QUERY_RESULT = np.dtype([("ok", "<i4"), ("dest_id", "<u4"), ("x", "<f4"), ("
 assert MAP_QUERY_RESULT.itemsize == 16
 ENTS_QUERY = np.dtype([("x", "<f4"), ("z", "<f4"), ("range", "<f4"), ("uid", "<u4"), ("maxout", "<i4"), ("_pad", "<u4")])
 assert ENTS_QUERY.itemsize == 24
+EVENT = np.dtype([("uid", "<u4"), ("flags", "<u4"), ("todo", "<u4"), ("attack", "<i4"), ("state_before", "<u4"),
+                  ("state_after", "<u4"), ("dest", "<f4", 2), ("pos", "<f4", 2), ("_pad", "<u4", 2)])
+assert EVENT.itemsize == 48
 
 LOS_PREV_INPLACE = -3
 TICK_VDES_FROM_POOL = 1
@@ -137,6 +140,7 @@ SYMBOLS = [
     "pfnav_mgpu_commands", "pfnav_group_commands",
     "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
     "pfnav_mgpu_change_population", "pfnav_group_change_population", "pfnav_ents_in_circles",
+    "pfnav_agents_collect_events", "pfnav_agents_read_events",
 ]
 
 _lib = None
@@ -202,6 +206,8 @@ def load():
     L.pfnav_agents_read_patches.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_apply_updates.argtypes = [C.c_void_p, C.c_void_p]
     L.pfnav_agents_apply_updates_ex.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+    L.pfnav_agents_collect_events.argtypes = [C.c_void_p, C.c_void_p]
+    L.pfnav_agents_read_events.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfnav_agents_upload_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_set_blocking.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
@@ -1020,6 +1026,25 @@ class Nav:
         """pfnav_agents_apply_updates_ex: flags = 0 is agents_apply_updates; APPLY_BLOCKERS also takes / releases the
         blockers of stopping / starting units on the device (applied by the next map_commit)"""
         _chk(self.L.pfnav_agents_apply_updates_ex(self.h, int(flags), C.c_void_p(stream)))
+
+    def agents_collect_events(self, stream=0):
+        """pfnav_agents_collect_events: the events of the last update pass, kept on the device (after
+        agents_compute_updates, before the apply)"""
+        _chk(self.L.pfnav_agents_collect_events(self.h, C.c_void_p(stream)))
+
+    def agents_read_events(self, cap=None):
+        """pfnav_agents_read_events -> EVENT records of the last collect, in work order. `cap`: the room of the first call
+        (default: the length of the work list this object last set, which no list of it exceeds); a call that returns
+        PFNAV_ERR_NOMEM is made once more with room for the length it reported."""
+        cap = max(self.nwork, 0) if cap is None else cap
+        n = C.c_size_t(0)
+        out = np.zeros(max(cap, 1), EVENT)
+        rc = self.L.pfnav_agents_read_events(self.h, _p(out), cap, C.byref(n))
+        if rc == ERR_NOMEM:
+            out = np.zeros(max(n.value, 1), EVENT)
+            rc = self.L.pfnav_agents_read_events(self.h, _p(out), n.value, C.byref(n))
+        _chk(rc)
+        return out[:n.value].copy()
 
     def agents_upload_blocking(self, b):
         """BLOCKING records, one per entity (uid order); describes blocks already counted, queues no op"""

@@ -983,6 +983,7 @@ static int agents_upload_impl(pfnav_ctx *ctx, const pfnav_agent *agents, size_t 
     PF_ARG(n < (1u << 31), "n");
     const bool sharded = ctx->mgpu != nullptr;
     PF_ARG(sharded || (lo == 0 && hi == n), "a partial upload needs pfnav_mgpu_init / pfnav_group_create first");
+    ctx->events_valid = false;              // the event list's uids name the previous population
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->tick_stream;
     const bool same = (flags & PFNAV_UPLOAD_SAME_FLOCKS) && ctx->n_agents == n && ctx->n_flocks == nflocks &&
@@ -2072,6 +2073,7 @@ extern "C" int pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream)
 {
     PF_ARG(ctx && ctx->d_agents, "agents not uploaded");
     PF_ARG(ctx->movestate_set, "pfnav_agents_upload_movestate not called");
+    ctx->updates_unapplied = true;
     if (ctx->n_work == 0) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);
@@ -2155,6 +2157,7 @@ extern "C" int pfnav_agents_apply_updates_ex(pfnav_ctx *ctx, uint32_t flags, voi
         if (rc) return rc;
     }
     PF_ARG(ctx->d_patches && ctx->update_done, "no update pass has run");
+    ctx->updates_unapplied = false;
     if (ctx->n_work == 0) return PFNAV_OK;
     PF_CUDA(cudaSetDevice(ctx->device));
     cudaStream_t st = pf_stream(ctx, stream);

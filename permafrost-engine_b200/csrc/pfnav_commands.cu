@@ -551,6 +551,7 @@ extern "C" int pfnav_agents_change_population(pfnav_ctx *ctx, const uint32_t *re
                                         add_formation, add_blocking, nadd, nflocks, P);
     PF_ARG(!err, err);
     if (P.removed.empty() && nadd == 0 && !flocks) return PFNAV_OK;
+    ctx->events_valid = false;              // the event list's uids name the previous population
     PF_CUDA(cudaSetDevice(ctx->device));
     return pop_apply(ctx, pf_stream(ctx, stream), T, P, add, add_ms, add_ext, add_formation, add_blocking, nadd, flocks, nflocks);
 }
@@ -645,6 +646,7 @@ int pf_pop_job_stage(pfnav_ctx *ctx, pf_pop_member &M, bool receive_all, cudaStr
     const pf_pop_tables &T = M.T;
     const int r = J.rank, world = J.world;
     const size_t R = P.removed.size(), n_new = P.n_new, nadd = M.nadd;
+    ctx->events_valid = false;              // the event list's uids name the previous population
     auto layout = [&](uint8_t *base) {
         size_t top = 0;
         auto take = [&](size_t bytes) { const size_t o = top; top += (bytes + 255) & ~(size_t)255; return o; };

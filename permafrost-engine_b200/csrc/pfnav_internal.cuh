@@ -223,6 +223,13 @@ struct pfnav_ctx {
     bool any_garrisoned = false;                             // G_Pos_EntsInCircleFrom filters + reorders (position.c:100)
     pf_dbuf<uint32_t> d_nb_scratch;
     cudaEvent_t update_done = nullptr;
+    bool updates_unapplied = false;                          // set by pfnav_agents_compute_updates, cleared by the apply
+    // pfnav_agents_collect_events (pfnav_events.cu): the list of the last collect, its block offsets, count and ballot
+    // words, the count's pinned copy and the event recorded behind it; the read's pinned staging. events_valid is
+    // cleared by the calls that renumber the population.
+    pf_dbuf<pfnav_event> d_events; pf_dbuf<uint32_t> d_event_aux;
+    uint32_t *h_event_count = nullptr; cudaEvent_t events_done = nullptr; bool events_valid = false;
+    pfnav_event *h_events = nullptr; size_t h_events_cap = 0;
     cudaStream_t tick_stream = nullptr;
     cudaEvent_t tick_done = nullptr;
     // LOS chains of a goal batch run on their own stream so that the parts of the tick that do not read
@@ -522,6 +529,8 @@ int build_index(pfnav_ctx *ctx, cudaStream_t st);
 // entity_block (mode 1) / entity_unblock (mode 0) of the n uids at d_uids (unique) through k_blocking_decide, appended to
 // the device-decided ops that pfnav_map_commit applies; d_patches != nullptr: the rules of PFNAV_APPLY_BLOCKERS instead
 int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n, const pfnav_patch *d_patches, int mode);
+// ---- pfnav_events.cu ----
+void pf_events_free(pfnav_ctx *ctx);                             // pfnav_destroy, after the device is idle
 
 // ---- pfnav_commands.cu: a job member's part of a command batch (pfnav_mgpu.cu runs the verdict exchange) ----
 // pf_cmd_job_check validates the batch against the member's state and plans it, changing nothing (the error is set);
