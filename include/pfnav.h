@@ -290,6 +290,31 @@ int  pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, float src_x, f
 int  pfnav_pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *dests, int layer, const float *src_xz,
                               const float *dst_xz, void *stream, uint32_t *out_dest_ids, int32_t *out_ok,
                               int32_t *out_n_flow, int32_t *out_n_los, int *out_ndone);
+/* Positions named by resident entities. pfnav_pool_request_paths_resident, pfnav_map_query_resident and
+ * pfnav_group_arrival_velocity_resident take, in place of a host position, the uid of an entity of the device-resident
+ * population, so that the device-resident loop issues orders, map queries and arrival velocities without reading
+ * positions back (pfnav_agents_read_state). They share these rules:
+ * - Equivalence: the call leaves everything exactly as the plain entry point (pfnav_pool_request_paths,
+ *   pfnav_map_query, pfnav_group_arrival_velocity) leaves it when called with each named position replaced by the
+ *   x, z of that entity's 24-byte record: pool, slots, ff_ids, LRU state, outputs, *out_ndone and the return code. On a
+ *   single context after an index build that is the pos pfnav_agents_read_state reports. The plain call's rules then
+ *   hold unchanged: a path endpoint off the map is PFNAV_ERR_ARG with nothing done, a query point off the map gives
+ *   ok = 0, an arrival position off the map clears flag bit 0.
+ * - Errors, in this order, with nothing changed and the outputs untouched: PFNAV_ERR_ARG for a uid not below the
+ *   population, n not below 2^24, or a NULL array the rules of the call forbid; PFNAV_ERR_STATE when n > 0 and records
+ *   were written since the last index build (as pfnav_ents_in_circles: the call goes after pfnav_agents_rebuild_index
+ *   or a gather); then every error of the plain entry point.
+ * - Multi-GPU: a job member resolves any uid (global uids) from its own record column, which the gather made whole, and
+ *   answers as one context holding the whole population would. There is no job form and no collective.
+ * - Host waits: map queries and arrival velocities wait only where the plain call does; path requests wait once more,
+ *   to read the resolved endpoints back for the host route planner.
+ * pfnav_pool_request_paths_resident: request i's source is the resident position of src_uids[i] unless src_uids is
+ * NULL or src_uids[i] == PFNAV_NULL_UID; then it is src_xz[2i, 2i+1]. The same holds for the destination with
+ * dst_uids / dst_xz. src_xz (dst_xz) may be NULL only when every src_uids (dst_uids) entry names a uid. */
+int  pfnav_pool_request_paths_resident(pfnav_ctx *ctx, int n, const int32_t *dests, int layer,
+                                       const uint32_t *src_uids, const float *src_xz, const uint32_t *dst_uids,
+                                       const float *dst_xz, void *stream, uint32_t *out_dest_ids, int32_t *out_ok,
+                                       int32_t *out_n_flow, int32_t *out_n_los, int *out_ndone);
 /* Read one pool entry back (4096 B each, pointers may be NULL). *out_has: bit0 flow, bit1 LOS;
  * *out_ffid: the N_FlowFieldID currently mapped for (dest, chunk). */
 int  pfnav_pool_get(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, uint8_t *flow_out,
@@ -470,6 +495,10 @@ int  pfnav_pool_request_zones(pfnav_ctx *ctx, const pfnav_zone_req *reqs, size_t
  * the map, chunk field present), bit 1 = *out_at_slot (FD_NONE within `radius` tiles of the centre). HOST buffers. */
 int  pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius, const float *pos_xz,
                                   size_t n, float *out_vel, uint8_t *out_flags);
+/* pfnav_group_arrival_velocity for n resident entities: position k is that of uids[k] (every entry names a uid). The
+ * rules of pfnav_pool_request_paths_resident apply. A whole arriving flock goes in one call. */
+int  pfnav_group_arrival_velocity_resident(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius,
+                                           const uint32_t *uids, size_t n, float *out_vel, uint8_t *out_flags);
 
 /* TARGET_ENTITY / TARGET_ENEMIES chunk fields (N_FlowFieldUpdate field.c:2040-2048 -> field_update_entity :1609,
  * field_update_enemies :1540; consumers N_DesiredSurroundVelocity / N_DesiredEnemySeekVelocity nav.c:3683, 3603).
@@ -860,6 +889,11 @@ typedef struct pfnav_map_query_result {  /* 16 bytes */
  *   pfnav_route_build(layer) (the global islands) for MAXIMALLY_CLOSE, faction_id in 0..15 for DEST_ID. Failure:
  *   PFNAV_ERR_ARG, out untouched. n == 0 is valid. Host-only context: PFNAV_ERR_NO_DEVICE. */
 int  pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfnav_map_query_result *out, void *stream);
+/* pfnav_map_query with positions that may name resident entities: pos_uids[i] replaces (x, z) of query i and
+ * dst_uids[i] replaces (dst_x, dst_z). Either array may be NULL; PFNAV_NULL_UID keeps the given value. The rules of
+ * pfnav_pool_request_paths_resident apply. */
+int  pfnav_map_query_resident(pfnav_ctx *ctx, const pfnav_map_query_req *q, const uint32_t *pos_uids,
+                              const uint32_t *dst_uids, size_t n, pfnav_map_query_result *out, void *stream);
 
 /* HOST array of n_agents records, uid == index. */
 int  pfnav_agents_upload_movestate(pfnav_ctx *ctx, const pfnav_movestate *ms, size_t n);

@@ -136,6 +136,7 @@ SYMBOLS = [
     "pfnav_mgpu_request_zones", "pfnav_group_request_zones", "pfnav_mgpu_request_entity_fields_batch",
     "pfnav_group_request_entity_fields_batch", "pfnav_pool_request_entity_fields_resident",
     "pfnav_mgpu_request_entity_fields_resident", "pfnav_group_request_entity_fields_resident",
+    "pfnav_pool_request_paths_resident", "pfnav_map_query_resident", "pfnav_group_arrival_velocity_resident",
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
     "pfnav_mgpu_commands", "pfnav_group_commands",
     "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
@@ -302,6 +303,12 @@ def load():
                                                             C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_group_request_entity_fields_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                                              C.c_size_t, C.c_void_p, C.c_size_t]
+    L.pfnav_pool_request_paths_resident.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.POINTER(C.c_int)]
+    L.pfnav_map_query_resident.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.pfnav_group_arrival_velocity_resident.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t,
+                                                        C.c_void_p, C.c_void_p]
     L.pfnav_agents_tick.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     L.pfnav_agents_read_velocities.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_read_debug.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
@@ -361,6 +368,15 @@ def _resident_args(reqs, footprints, ent_uids, seekers):
         raise ValueError("footprints and ent_uids differ in length")
     ptr = lambda a: _p(a) if a is not None and len(a) else None
     return (ptr(reqs), len(reqs), ptr(fp), ptr(uids), nents, ptr(sk), len(sk), (reqs, fp, uids, sk))
+
+
+def _named_points(n, uids, xz):
+    """one endpoint array of pool_request_paths_resident: (uint32[n] or None, float32[n, 2] or None)"""
+    u = None if uids is None else np.ascontiguousarray(uids, np.uint32).reshape(-1)
+    p = None if xz is None else np.ascontiguousarray(xz, np.float32).reshape(-1, 2)
+    if (u is not None and len(u) != n) or (p is not None and len(p) != n):
+        raise ValueError("uids / points and dests differ in length")
+    return u, p
 
 
 def _chk(rc):
@@ -980,6 +996,49 @@ class Nav:
         if rc != ERR_NOMEM:
             _chk(rc)
         return ndone.value
+
+    def pool_request_paths_resident(self, dests, src_uids, src_xz, dst_uids, dst_xz, layer=0, stream=0):
+        """pool_request_paths with endpoints that may name resident entities -> ok[n] (bool), dest_id[n], n_flow[n],
+        n_los[n], ndone. `src_uids` / `dst_uids`: uint32 per request (NULL_UID: use the given point) or None (use the
+        points as given); `src_xz` / `dst_xz`: float32 [n, 2] or None (every entry names a uid)."""
+        dests = np.ascontiguousarray(dests, np.int32).reshape(-1)
+        n = len(dests)
+        su, sx = _named_points(n, src_uids, src_xz)
+        du, dx = _named_points(n, dst_uids, dst_xz)
+        ok, nf, nl = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        did = np.zeros(n, np.uint32)
+        ndone = C.c_int(0)
+        ptr = lambda a: _p(a) if a is not None and len(a) else None
+        rc = self.L.pfnav_pool_request_paths_resident(self.h, n, ptr(dests), layer, ptr(su), ptr(sx), ptr(du), ptr(dx),
+                                                      C.c_void_p(stream), ptr(did), ptr(ok), ptr(nf), ptr(nl), C.byref(ndone))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        return ok.astype(bool), did, nf, nl, ndone.value
+
+    def map_query_resident(self, queries, pos_uids=None, dst_uids=None, stream=0, out=None):
+        """map_query with positions that may name resident entities: `pos_uids` / `dst_uids` (uint32 per query, NULL_UID
+        keeps the given value, or None) replace (x, z) / (dst_x, dst_z). `out`, when given, is the MAP_QUERY_RESULT
+        array the call fills (left untouched when the call fails)."""
+        q = np.ascontiguousarray(queries, MAP_QUERY)
+        pu = None if pos_uids is None else np.ascontiguousarray(pos_uids, np.uint32)
+        du = None if dst_uids is None else np.ascontiguousarray(dst_uids, np.uint32)
+        if (pu is not None and len(pu) != len(q)) or (du is not None and len(du) != len(q)):
+            raise ValueError("pos_uids / dst_uids and queries differ in length")
+        if out is None:
+            out = np.zeros(len(q), MAP_QUERY_RESULT)
+        assert out.dtype == MAP_QUERY_RESULT and out.flags.c_contiguous and len(out) >= len(q)
+        ptr = lambda a: _p(a) if a is not None and len(a) else None
+        _chk(self.L.pfnav_map_query_resident(self.h, ptr(q), ptr(pu), ptr(du), len(q), ptr(out) if len(q) else None,
+                                             C.c_void_p(stream)))
+        return out
+
+    def group_arrival_velocity_resident(self, dest, centre_xz, radius, uids):
+        """group_arrival_velocity for resident entities: position k is that of uids[k] -> (vel [n, 2], flags [n])"""
+        c = np.ascontiguousarray(centre_xz, np.float32); u = np.ascontiguousarray(uids, np.uint32).reshape(-1)
+        vel = np.zeros((len(u), 2), np.float32); fl = np.zeros(len(u), np.uint8)
+        _chk(self.L.pfnav_group_arrival_velocity_resident(self.h, dest, _p(c), int(radius), _p(u) if len(u) else None, len(u),
+                                                          _p(vel), _p(fl)))
+        return vel, fl
 
     def pool_request_entity_fields_resident(self, reqs, footprints, ent_uids, seekers, stream=0):
         """pool_request_entity_fields_batch with footprints and seekers named by uid -> ndone. `footprints`: FOOTPRINT

@@ -379,6 +379,17 @@ int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, st
 int pf_resident_resolve(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_field_req *reqs, size_t m,
                         const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents, const uint32_t *seeker_uids,
                         size_t nseekers, pf_resident_batch &B);
+// PFNAV_ERR_STATE, with the message "<what> by uid: ...", when records were written after the last index build.
+int pf_resident_fresh(pfnav_ctx *ctx, const char *what);
+// The calls whose positions may name resident entities (pfnav_pool_request_paths_resident, pfnav_map_query_resident,
+// pfnav_group_arrival_velocity_resident; pfnav_region.cu): pf_resident_points_check against the context's population
+// (PFNAV_ERR_ARG), then, when n > 0, pf_resident_fresh (PFNAV_ERR_STATE). Changes nothing.
+int pf_resident_points_begin(pfnav_ctx *ctx, const char *what, size_t n, const uint32_t *uids_a, bool given_a,
+                             const uint32_t *uids_b, bool given_b, pf_resident_points &P);
+// k_resident_xz on `st` for P's pairs, staged at d_pairs by P.pack: the x, z of each named record over buf[entry * stride
+// + off0] (the first array's pairs) or buf[entry * stride + off1] (the second's). Nothing when P names nothing.
+int pf_resident_xz_launch(pfnav_ctx *ctx, cudaStream_t st, const uint8_t *d_pairs, const pf_resident_points &P, int stride,
+                          int off0, int off1, float *buf);
 
 // ---- pfnav_pool.cu: the device pool, and the pool mutators of a context, each of which drops the resident goal plan
 // Bring the device copies of the pool up to date after pfnav_pool_clear: empty slot table, no `has` bytes, zero touch

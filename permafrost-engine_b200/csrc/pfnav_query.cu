@@ -11,6 +11,8 @@
 // Kernels (pfnav_query_kernel.cuh): k_map_probe, one thread per query, answers the probe kinds and DEST_ID; k_map_search,
 // one warp per CLOSEST_PATHABLE / MAXIMALLY_CLOSE query, replays the reference's search inside a window of the layer.
 // The searches that would leave the window are finished here with the host routine pfnav_arrival_consts.
+// pfnav_map_query_resident takes the positions of resident entities by uid: k_resident_xz (pfnav_region.cu) writes them
+// into the uploaded queries before the same kernels run.
 #include "pfnav_internal.cuh"
 #include <algorithm>
 #include <math.h>
@@ -21,7 +23,11 @@
 static_assert(sizeof(pfnav_map_query_req) == 32, "pfnav_map_query_req must be 32 bytes");
 static_assert(sizeof(pfnav_map_query_result) == 16, "pfnav_map_query_result must be 16 bytes");
 
-extern "C" int pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfnav_map_query_result *out, void *stream)
+// pfnav_map_query, and its resident form when P is not NULL: after the queries are uploaded, k_resident_xz writes P's
+// named positions over (x, z) (the first array) and (dst_x, dst_z) (the second) of the device copy, and the searches'
+// substituted records come back with the results for the host finish
+static int map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfnav_map_query_result *out, void *stream,
+                     const pf_resident_points *P)
 {
     PF_ARG(ctx, "ctx");
     PF_NEED_DEVICE(ctx);
@@ -54,6 +60,16 @@ extern "C" int pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, siz
     pfnav_map_query_result *d_out = (pfnav_map_query_result *)(dev + o_res);
     PF_CUDA(cudaMemcpyAsync(dev, q, o_res, cudaMemcpyHostToDevice, st));
     if (ns) PF_CUDA(cudaMemcpyAsync(dev + o_idx, search.data(), ns * 4, cudaMemcpyHostToDevice, st));
+    const bool named = P && !P->entry.empty();
+    if (named) {
+        // the pairs through the request staging; x, z are floats 2, 3 and dst_x, dst_z floats 4, 5 of a 32-byte record
+        pf_stage S;
+        if (int rc = pf_stage_begin(ctx, st, P->bytes(), P->bytes(), false, &S)) return rc;
+        P->pack(S.host);
+        if (int rc = pf_stage_upload(ctx, st, S, P->bytes())) return rc;
+        if (int rc = pf_resident_xz_launch(ctx, st, S.dev, *P, 8, 2, 4, (float *)dev)) return rc;
+        if (int rc = pf_stage_done(ctx, st)) return rc;
+    }
     MapView m;
     m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
     m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
@@ -70,12 +86,19 @@ extern "C" int pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, siz
         PF_CUDA(cudaMemcpyAsync(fallback.data(), dev + o_fb, ns, cudaMemcpyDeviceToHost, st));
     }
     PF_CUDA(cudaMemcpyAsync(out, d_out, n * sizeof(pfnav_map_query_result), cudaMemcpyDeviceToHost, st));
+    // the resident form: the substituted records from the first search to the last, which the host finish reads
+    std::vector<pfnav_map_query_req> sub;
+    if (named && ns) {
+        sub.resize((size_t)(search.back() - search.front()) + 1);
+        PF_CUDA(cudaMemcpyAsync(sub.data(), d_q + search.front(), sub.size() * sizeof(pfnav_map_query_req),
+                                cudaMemcpyDeviceToHost, st));
+    }
     PF_CUDA(cudaStreamSynchronize(st));
     // the searches that left the window: the host routine on the host mirrors, which the last commit made equal to the
     // device images
     for (size_t k = 0; k < ns; k++) {
         if (!fallback[k]) continue;
-        const pfnav_map_query_req &a = q[search[k]];
+        const pfnav_map_query_req &a = sub.empty() ? q[search[k]] : sub[search[k] - search.front()];
         pfnav_map_query_result &r = out[search[k]];
         pf_arrival_consts c;
         r = {0, 0u, 0.0f, 0.0f};
@@ -93,4 +116,18 @@ extern "C" int pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, siz
         }
     }
     return PFNAV_OK;
+}
+
+extern "C" int pfnav_map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfnav_map_query_result *out, void *stream)
+{
+    return map_query(ctx, q, n, out, stream, nullptr);
+}
+
+extern "C" int pfnav_map_query_resident(pfnav_ctx *ctx, const pfnav_map_query_req *q, const uint32_t *pos_uids,
+                                        const uint32_t *dst_uids, size_t n, pfnav_map_query_result *out, void *stream)
+{
+    PF_ARG(ctx, "ctx");
+    pf_resident_points P;
+    if (int rc = pf_resident_points_begin(ctx, "map queries", n, pos_uids, q != nullptr, dst_uids, q != nullptr, P)) return rc;
+    return map_query(ctx, q, n, out, stream, &P);
 }

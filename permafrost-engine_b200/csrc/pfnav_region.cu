@@ -653,29 +653,36 @@ extern "C" int pfnav_pool_request_zone(pfnav_ctx *ctx, int dest, int layer, cons
     return PFNAV_OK;
 }
 
-extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius, const float *pos_xz,
-                                            size_t n, float *out_vel, uint8_t *out_flags)
+// pfnav_group_arrival_velocity, and its resident form when P is not NULL: P's named positions are staged in place of
+// pos_xz and written on the device by k_resident_xz, ahead of the same kernel
+static int group_arrival(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius, const float *pos_xz,
+                         const pf_resident_points *P, size_t n, float *out_vel, uint8_t *out_flags)
 {
     PF_ARG(ctx && ctx->d_cost, "map not created");
     PF_NEED_DEVICE(ctx);
     PF_ARG(ctx->pool.d_slot, "pool not created");
     PF_ARG(dest >= 0 && dest < ctx->pool.ndests, "dest");
     if (n == 0) return PFNAV_OK;
-    PF_ARG(centre_xz && pos_xz && out_vel && out_flags, "null buffer");
+    PF_ARG(centre_xz && (pos_xz || P) && out_vel && out_flags, "null buffer");
     PF_ARG(n < (1u << 30), "n");
     PF_ARG(radius >= 0 && radius <= 0xFFFF, "radius");
     PF_CUDA(cudaSetDevice(ctx->device));
     PF_CUDA(pf_fields_sync(ctx));
     cudaStream_t st = ctx->tick_stream;
     PF_CUDA(pf_pool_refresh(ctx, st));
-    // staged: the positions, then the velocities and the flags
+    // staged: the positions (the resident form: the named pairs, then room for the positions), then the velocities and
+    // the flags
+    const size_t o_pos = P ? (P->bytes() + 15) & ~(size_t)15 : 0, up = P ? P->bytes() : n * 8;
     pf_stage S;
-    if (int rc = pf_stage_begin(ctx, st, n * 8, n * 17, false, &S)) return rc;
-    memcpy(S.host, pos_xz, n * 8);
-    if (int rc = pf_stage_upload(ctx, st, S, n * 8)) return rc;
-    const float2 *d_pos = (const float2 *)S.dev;
-    float2 *d_vel = (float2 *)(S.dev + n * 8);
-    uint8_t *d_fl = S.dev + n * 16;
+    if (int rc = pf_stage_begin(ctx, st, up, o_pos + n * 17, false, &S)) return rc;
+    if (P) P->pack(S.host);
+    else memcpy(S.host, pos_xz, n * 8);
+    if (int rc = pf_stage_upload(ctx, st, S, up)) return rc;
+    const float2 *d_pos = (const float2 *)(S.dev + o_pos);
+    float2 *d_vel = (float2 *)(S.dev + o_pos + n * 8);
+    uint8_t *d_fl = S.dev + o_pos + n * 16;
+    if (P)
+        if (int rc = pf_resident_xz_launch(ctx, st, S.dev, *P, 2, 0, 0, (float *)d_pos)) return rc;
     ZoneView z = { ctx->pool.d_slot, ctx->pool.d_flow, ctx->pool.d_has, ctx->chunk_w, ctx->chunk_h,
                    ctx->map_x, ctx->map_z };
     k_group_arrival_velocity<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(z, dest, centre_xz[0], centre_xz[1], radius, d_pos, (int)n, d_vel, d_fl);
@@ -686,6 +693,21 @@ extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const floa
     if (int rc = pf_stage_done(ctx, st)) return rc;
     PF_CUDA(cudaStreamSynchronize(st));
     return PFNAV_OK;
+}
+
+extern "C" int pfnav_group_arrival_velocity(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius, const float *pos_xz,
+                                            size_t n, float *out_vel, uint8_t *out_flags)
+{
+    return group_arrival(ctx, dest, centre_xz, radius, pos_xz, nullptr, n, out_vel, out_flags);
+}
+
+extern "C" int pfnav_group_arrival_velocity_resident(pfnav_ctx *ctx, int dest, const float *centre_xz, int radius,
+                                                     const uint32_t *uids, size_t n, float *out_vel, uint8_t *out_flags)
+{
+    PF_ARG(ctx, "ctx");
+    pf_resident_points P;
+    if (int rc = pf_resident_points_begin(ctx, "group arrival velocities", n, uids, false, nullptr, true, P)) return rc;
+    return group_arrival(ctx, dest, centre_xz, radius, nullptr, &P, n, out_vel, out_flags);
 }
 
 // The zone's seed tiles alone (host structure code, no device needed): the first `budget` open tiles of the
@@ -1217,7 +1239,49 @@ __global__ void __launch_bounds__(256) k_resident_footprints(const pf_record *__
     chunk_out[i - nfp] = desc_for_point(m, r.px, r.pz, t) ? t.chunk_r * m.chunk_w + t.chunk_c : -1;
 }
 
+// one thread per named entry: the x, z of uid[i]'s record into buf at entry[i] * stride + off, where off is off0 for the
+// first n0 entries and off1 for the rest
+__global__ void __launch_bounds__(256) k_resident_xz(const pf_record *__restrict__ rec, const uint32_t *__restrict__ entry,
+                                                     const uint32_t *__restrict__ uid, int n, int n0, int stride, int off0,
+                                                     int off1, float *__restrict__ buf)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const pf_record &r = rec[uid[i]];
+    float *p = buf + entry[i] * stride + (i < n0 ? off0 : off1);
+    p[0] = r.px; p[1] = r.pz;
+}
+
 }   // namespace
+
+int pf_resident_fresh(pfnav_ctx *ctx, const char *what)
+{
+    if (!ctx->index_stale) return PFNAV_OK;
+    pfnav_set_error("%s by uid: records were written after the last index build (pfnav_agents_rebuild_index or a gather "
+                    "first)", what);
+    return PFNAV_ERR_STATE;
+}
+
+int pf_resident_points_begin(pfnav_ctx *ctx, const char *what, size_t n, const uint32_t *uids_a, bool given_a,
+                             const uint32_t *uids_b, bool given_b, pf_resident_points &P)
+{
+    const char *err = nullptr;
+    if (pf_resident_points_check(n, uids_a, given_a, uids_b, given_b, ctx->n_agents, P, &err)) PF_ARG(false, err);
+    return n ? pf_resident_fresh(ctx, what) : PFNAV_OK;
+}
+
+int pf_resident_xz_launch(pfnav_ctx *ctx, cudaStream_t st, const uint8_t *d_pairs, const pf_resident_points &P, int stride,
+                          int off0, int off1, float *buf)
+{
+    const size_t np = P.entry.size();
+    if (!np) return PFNAV_OK;
+    const uint32_t *d_entry = (const uint32_t *)d_pairs;
+    k_resident_xz<<<(unsigned)((np + 255) / 256), 256, 0, st>>>(ctx->d_records, d_entry, d_entry + np, (int)np, (int)P.n0,
+                                                                stride, off0, off1, buf);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
+}
 
 int pf_resident_resolve(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_field_req *reqs, size_t m,
                         const pfnav_footprint *ents, const uint32_t *ent_uids, size_t nents, const uint32_t *seeker_uids,
@@ -1228,11 +1292,7 @@ int pf_resident_resolve(pfnav_ctx *ctx, cudaStream_t st, const pfnav_entity_fiel
     const char *err = nullptr;
     if (pf_resident_check(reqs, m, ents, ent_uids, nents, seeker_uids, nseekers, ctx->n_agents, N, &err)) PF_ARG(false, err);
     if (m == 0) return PFNAV_OK;
-    if (ctx->index_stale) {
-        pfnav_set_error("entity fields by uid: records were written after the last index build (pfnav_agents_rebuild_index "
-                        "or a gather first)");
-        return PFNAV_ERR_STATE;
-    }
+    if (int rc = pf_resident_fresh(ctx, "entity fields")) return rc;
     const size_t n = N.uids.size(), nfp = N.fp_index.size();
     std::vector<float> fp_xzr(3 * nfp);
     std::vector<int32_t> seek_chunk(nseekers);

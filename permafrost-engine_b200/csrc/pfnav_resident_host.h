@@ -1,12 +1,18 @@
-// pfnav_resident_host.h -- the host rule of pfnav_pool_request_entity_fields_resident and its job forms, CUDA-free: the
-// checks of the uid arguments, and the turn of what k_resident_footprints resolves from the records into the inputs of
-// pfnav_pool_request_entity_fields_batch (footprints merged with the given ones, each request's seekers as the chunks
-// under them, first seen first, each once). tests/emu/resident_emu.cpp builds this header with g++.
+// pfnav_resident_host.h -- the host rules of the calls that name resident entities by uid, CUDA-free:
+// - pfnav_pool_request_entity_fields_resident and its job forms: the checks of the uid arguments, and the turn of what
+//   k_resident_footprints resolves from the records into the inputs of pfnav_pool_request_entity_fields_batch
+//   (footprints merged with the given ones, each request's seekers as the chunks under them, first seen first, each
+//   once). tests/emu/resident_emu.cpp builds this part with g++.
+// - pfnav_pool_request_paths_resident, pfnav_map_query_resident and pfnav_group_arrival_velocity_resident: the checks
+//   of their uid arrays and the (entry, uid) pairs whose positions k_resident_xz writes over the given ones.
+//   tests/emu/resident_points_emu.cpp builds this part with g++.
 #pragma once
 #include <stdint.h>
 #include <string.h>
 #include <vector>
 #include "../../include/pfnav.h"
+
+#define PF_RES_ARG(cond, msg) do { if (!(cond)) { *err = msg; return PFNAV_ERR_ARG; } } while (0)
 
 // The uids the device resolves: the footprint entries that name one (their indices into ents, ascending) and then
 // every seeker, in the argument order.
@@ -21,6 +27,26 @@ struct pf_resident_batch {
     std::vector<int32_t> chunks_rc;
 };
 
+// Entries 0 .. n-1 of one argument array whose values may name resident entities: entry k names uids[k] unless uids is
+// NULL or uids[k] == PFNAV_NULL_UID, and then the caller's given value stands, which needs `given` (the array of given
+// values is not NULL). Appends each naming entry's index to `entry` and its uid to `uid`, in order. PFNAV_ERR_ARG with
+// *err = no_given or outside: an entry that names nothing without a given value, or a uid not below `population`.
+static inline int pf_resident_named(const uint32_t *uids, size_t n, bool given, size_t population, std::vector<uint32_t> &entry,
+                                    std::vector<uint32_t> &uid, const char *no_given, const char *outside, const char **err)
+{
+    for (size_t k = 0; k < n; k++) {
+        const uint32_t u = uids ? uids[k] : PFNAV_NULL_UID;
+        if (u == PFNAV_NULL_UID) {
+            PF_RES_ARG(given, no_given);
+            continue;
+        }
+        PF_RES_ARG(u < population, outside);
+        entry.push_back((uint32_t)k);
+        uid.push_back(u);
+    }
+    return PFNAV_OK;
+}
+
 // Checks what the uid arguments add to the batch's own validation: the non-NULL rules (ents may be NULL only when every
 // entry names a uid), nents and nseekers below 2^24, every uid below `population`, and every request's footprint and
 // seeker range inside its array. Fills N. PFNAV_ERR_ARG with *err naming the check; N is then unspecified.
@@ -28,23 +54,15 @@ static inline int pf_resident_check(const pfnav_entity_field_req *reqs, size_t m
                                     const uint32_t *ent_uids, size_t nents, const uint32_t *seeker_uids, size_t nseekers,
                                     size_t population, pf_resident_names &N, const char **err)
 {
-#define PF_RES_ARG(cond, msg) do { if (!(cond)) { *err = msg; return PFNAV_ERR_ARG; } } while (0)
     PF_RES_ARG(m < (1u << 24) && nents < (1u << 24) && nseekers < (1u << 24), "m / nents / nseekers");
     PF_RES_ARG(m == 0 || reqs, "reqs");
     PF_RES_ARG(nents == 0 || ents || ent_uids, "ents and ent_uids are both NULL");
     PF_RES_ARG(nseekers == 0 || seeker_uids, "seeker_uids");
     N.fp_index.clear();
     N.uids.clear();
-    for (size_t k = 0; k < nents; k++) {
-        const uint32_t u = ent_uids ? ent_uids[k] : PFNAV_NULL_UID;
-        if (u == PFNAV_NULL_UID) {
-            PF_RES_ARG(ents, "ents == NULL, but an entry of ent_uids names no uid");
-            continue;
-        }
-        PF_RES_ARG(u < population, "footprint uid outside the population");
-        N.fp_index.push_back((uint32_t)k);
-        N.uids.push_back(u);
-    }
+    if (int rc = pf_resident_named(ent_uids, nents, ents != nullptr, population, N.fp_index, N.uids,
+                                   "ents == NULL, but an entry of ent_uids names no uid", "footprint uid outside the population", err))
+        return rc;
     for (size_t k = 0; k < nseekers; k++) {
         PF_RES_ARG(seeker_uids[k] < population, "seeker uid outside the population");
         N.uids.push_back(seeker_uids[k]);
@@ -54,7 +72,6 @@ static inline int pf_resident_check(const pfnav_entity_field_req *reqs, size_t m
         PF_RES_ARG((uint64_t)reqs[i].chunk_off + reqs[i].chunk_n <= nseekers, "seeker range");
     }
     return PFNAV_OK;
-#undef PF_RES_ARG
 }
 
 // The batch's inputs from the resolved values: fp_xzr[3k ..] = {x, z, radius} of the record of N.uids[k] (footprint
@@ -96,3 +113,36 @@ static inline int pf_resident_merge(const pfnav_entity_field_req *reqs, size_t m
     }
     return PFNAV_OK;
 }
+
+// The positions a call names by uid (pfnav_pool_request_paths_resident: sources, destinations; pfnav_map_query_resident:
+// (x, z), (dst_x, dst_z); pfnav_group_arrival_velocity_resident: the positions): the (entry, uid) pairs of the first
+// array, then those of the second. The device reads them as entry[np] then uid[np] (np = entry.size()).
+struct pf_resident_points {
+    std::vector<uint32_t> entry, uid;
+    size_t n0 = 0;                       // how many pairs the first array names
+    size_t bytes() const { return entry.size() * 8; }
+    void pack(uint8_t *dst) const
+    {
+        if (entry.empty()) return;
+        memcpy(dst, entry.data(), entry.size() * 4);
+        memcpy(dst + entry.size() * 4, uid.data(), uid.size() * 4);
+    }
+};
+
+// Checks the uid arrays of n entries with up to two named positions each: n below 2^24; array a's entry k names uids_a[k]
+// unless uids_a is NULL or the entry is PFNAV_NULL_UID, and then it needs the given positions (given_a); every named uid
+// below `population`. uids_b / given_b the same for the second position (NULL and true when there is none). Fills P.
+// PFNAV_ERR_ARG with *err naming the check; P is then unspecified.
+static inline int pf_resident_points_check(size_t n, const uint32_t *uids_a, bool given_a, const uint32_t *uids_b, bool given_b,
+                                           size_t population, pf_resident_points &P, const char **err)
+{
+    PF_RES_ARG(n < (1u << 24), "n");
+    P.entry.clear();
+    P.uid.clear();
+    const char *no_given = "an entry names no uid, and its positions are NULL", *outside = "uid outside the population";
+    if (int rc = pf_resident_named(uids_a, n, given_a, population, P.entry, P.uid, no_given, outside, err)) return rc;
+    P.n0 = P.entry.size();
+    return pf_resident_named(uids_b, n, given_b, population, P.entry, P.uid, no_given, outside, err);
+}
+
+#undef PF_RES_ARG

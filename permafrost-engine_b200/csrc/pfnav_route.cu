@@ -1115,6 +1115,44 @@ extern "C" int pfnav_pool_request_paths(pfnav_ctx *ctx, int n, const int32_t *de
     return pool_request_paths(ctx, n, dests, layer, src_xz, dst_xz, stream, out_dest_ids, out_ok, out_n_flow, out_n_los, out_ndone);
 }
 
+// pfnav_pool_request_paths with endpoints that may name resident entities (pfnav.h): k_resident_xz writes the named
+// records' positions over the given ones in the request staging, one copy back and one wait, then the batch as given.
+extern "C" int pfnav_pool_request_paths_resident(pfnav_ctx *ctx, int n, const int32_t *dests, int layer, const uint32_t *src_uids,
+                                                 const float *src_xz, const uint32_t *dst_uids, const float *dst_xz, void *stream,
+                                                 uint32_t *out_dest_ids, int32_t *out_ok, int32_t *out_n_flow, int32_t *out_n_los,
+                                                 int *out_ndone)
+{
+    if (out_ndone) *out_ndone = 0;
+    PF_ARG(ctx, "ctx");
+    PF_ARG(n >= 0, "n");
+    pf_resident_points P;
+    if (int rc = pf_resident_points_begin(ctx, "path requests", (size_t)n, src_uids, src_xz != nullptr, dst_uids,
+                                          dst_xz != nullptr, P))
+        return rc;
+    if (P.entry.empty())
+        return pfnav_pool_request_paths(ctx, n, dests, layer, src_xz, dst_xz, stream, out_dest_ids, out_ok, out_n_flow,
+                                        out_n_los, out_ndone);
+    // the staging holds the pairs, then the sources and the destinations as given (2n floats each)
+    const size_t o_xz = (P.bytes() + 15) & ~(size_t)15, nxz = (size_t)n * 8, need = o_xz + 2 * nxz;
+    PF_NEED_DEVICE(ctx);
+    PF_CUDA(cudaSetDevice(ctx->device));
+    const cudaStream_t st = pf_stream(ctx, stream);
+    pf_stage S;
+    if (int rc = pf_stage_begin(ctx, st, need, need, false, &S)) return rc;
+    P.pack(S.host);
+    if (src_xz) memcpy(S.host + o_xz, src_xz, nxz);
+    if (dst_xz) memcpy(S.host + o_xz + nxz, dst_xz, nxz);
+    if (int rc = pf_stage_upload(ctx, st, S, need)) return rc;
+    if (int rc = pf_resident_xz_launch(ctx, st, S.dev, P, 2, 0, 2 * n, (float *)(S.dev + o_xz))) return rc;
+    PF_CUDA(cudaMemcpyAsync(S.host + o_xz, S.dev + o_xz, 2 * nxz, cudaMemcpyDeviceToHost, st));
+    if (int rc = pf_stage_done(ctx, st)) return rc;
+    PF_CUDA(cudaStreamSynchronize(st));
+    std::vector<float> xz(4 * (size_t)n);
+    memcpy(xz.data(), S.host + o_xz, 2 * nxz);
+    return pfnav_pool_request_paths(ctx, n, dests, layer, xz.data(), xz.data() + 2 * (size_t)n, stream, out_dest_ids, out_ok,
+                                    out_n_flow, out_n_los, out_ndone);
+}
+
 // N_RequestPath (nav.c:3386) against the device field pool: route src -> dst exactly as the reference
 // does, then build only the fields the pool does not hold yet, in place, on the device. The one-request batch.
 extern "C" int pfnav_pool_request_path(pfnav_ctx *ctx, int dest, int layer, float src_x, float src_z, float dst_x,
