@@ -269,10 +269,11 @@ __global__ void k_cohesion(const pf_record *__restrict__ rec, const int32_t *__r
 // the window's entries stream through shared memory in tiles, every thread accumulates its own entity's sum. An entity
 // whose window holds too little weight to make the cut-off harmless (sum < N * exp(4.5 - 0.12 * 230) * 1e7, i.e. the
 // dropped members could matter at the 1e-7 level) is handed to the full-list kernel instead, so the result never
-// depends on the cut-off by more than float rounding. Index coordinates are the 1/256-wu integers of the position index.
+// depends on the cut-off by more than float rounding. The index picks the cells; the weights and the sum use the
+// members' float positions from their records, as the full-list kernel does.
 #define COH_R 230.0f
 #define COH_THREADS 128
-__device__ __forceinline__ void coh_finish(float ax, float az, float wsum, float self_w, float six_f, float siy_f, float sx, float sz,
+__device__ __forceinline__ void coh_finish(float ax, float az, float wsum, float self_w, float sx, float sz,
                                            uint32_t N, float thresh_unit, float scaled_max_force, uint32_t uid,
                                            float2 *__restrict__ out_by_uid, uint32_t *__restrict__ fallback,
                                            uint32_t *__restrict__ nfallback)
@@ -280,7 +281,7 @@ __device__ __forceinline__ void coh_finish(float ax, float az, float wsum, float
     if (N <= 1) out_by_uid[uid] = make_float2(0.0f, 0.0f);
     else if (wsum - self_w >= (float)N * thresh_unit) {
         // the entity's own index entry was summed too: take it out again (weight exp(4.5) at distance 0)
-        v2 com = {ax - six_f * self_w, az - siy_f * self_w};
+        v2 com = {ax - sx * self_w, az - sz * self_w};
         com = v2_scale(com, 1.0f / (float)(N - 1));
         v2 ret = v2_sub(com, v2{sx, sz});
         ret = v2_truncate(ret, scaled_max_force);
@@ -300,13 +301,12 @@ k_cohesion_window(GridView g, const pf_record *__restrict__ rec, const int32_t *
     for (int base = blockIdx.x * COH_THREADS; base < n; base += gridDim.x * COH_THREADS) {
         const int k = base + tid;
         uint32_t uid = 0; int fl = -1; bool active = false;
-        float sx = 0.0f, sz = 0.0f, six_f = 0.0f, siy_f = 0.0f, self_w = 0.0f;
+        float sx = 0.0f, sz = 0.0f, self_w = 0.0f;
         int mycx = 0, mycy = 0;
         if (k < n) {
             uid = g.id[k]; fl = sfl[k];
             active = uid >= lo && uid < hi && fl >= 0;
             mycx = cell_of(g.ix[k], g.origin_x, g.grid_w); mycy = cell_of(g.iy[k], g.origin_y, g.grid_h);
-            six_f = (float)g.ix[k] * (1.0f / 256.0f); siy_f = (float)g.iy[k] * (1.0f / 256.0f);
         }
         if (!__syncthreads_or(active)) continue;
         if (tid == 0) { bb[0] = 0x7fffffff; bb[1] = -1; bb[2] = 0x7fffffff; bb[3] = -1; }
@@ -314,7 +314,7 @@ k_cohesion_window(GridView g, const pf_record *__restrict__ rec, const int32_t *
         if (active) {
             const pf_record self = rec[uid];
             sx = self.px; sz = self.pz;
-            self_w = coh_weight(six_f - sx, siy_f - sz);       // what the loop below adds for the entity's own entry
+            self_w = coh_weight(0.0f, 0.0f);                   // what the loop below adds for the entity's own entry
             atomicMin(&bb[0], mycx); atomicMax(&bb[1], mycx); atomicMin(&bb[2], mycy); atomicMax(&bb[3], mycy);
         }
         __syncthreads();
@@ -341,8 +341,12 @@ k_cohesion_window(GridView g, const pf_record *__restrict__ rec, const int32_t *
                 const uint32_t s0 = g.cell_start[ry * g.grid_w + x0], s1 = g.cell_start[ry * g.grid_w + x1 + 1];
                 for (uint32_t t0 = s0; t0 < s1; t0 += COH_THREADS) {
                     const uint32_t e = t0 + tid;
-                    if (e < s1)
-                        tile[tid] = make_float4((float)g.ix[e] * (1.0f / 256.0f), (float)g.iy[e] * (1.0f / 256.0f), __int_as_float(sfl[e]), 0.0f);
+                    // the members' own positions, as cohesion_force sums them: the index's 1/256-wu integers would move
+                    // the centre of mass by up to 1/512 wu per member
+                    if (e < s1) {
+                        const pf_record r = rec[g.id[e]];
+                        tile[tid] = make_float4(r.px, r.pz, __int_as_float(sfl[e]), 0.0f);
+                    }
                     __syncthreads();
                     const int nt = (int)min((uint32_t)COH_THREADS, s1 - t0);
                     if (mine) {
@@ -360,7 +364,7 @@ k_cohesion_window(GridView g, const pf_record *__restrict__ rec, const int32_t *
         if (nsplit > 1) {                    // a small population split over blockIdx.y: k_cohesion_finish adds the parts up
             if (k < n) part[(size_t)blockIdx.y * n + k] = make_float4(ax, az, wsum, 0.0f);
         } else if (active) {
-            coh_finish(ax, az, wsum, self_w, six_f, siy_f, sx, sz, flock_start[fl + 1] - flock_start[fl], thresh_unit,
+            coh_finish(ax, az, wsum, self_w, sx, sz, flock_start[fl + 1] - flock_start[fl], thresh_unit,
                        scaled_max_force, uid, out_by_uid, fallback, nfallback);
         }
     }
@@ -381,9 +385,7 @@ __global__ void k_cohesion_finish(GridView g, const pf_record *__restrict__ rec,
     float ax = 0.0f, az = 0.0f, wsum = 0.0f;
     for (int sp = 0; sp < nsplit; sp++) { const float4 p = part[(size_t)sp * n + k]; ax += p.x; az += p.y; wsum += p.z; }
     const pf_record self = rec[uid];
-    const float six_f = (float)g.ix[k] * (1.0f / 256.0f), siy_f = (float)g.iy[k] * (1.0f / 256.0f);
-    const float self_w = coh_weight(six_f - self.px, siy_f - self.pz);
-    coh_finish(ax, az, wsum, self_w, six_f, siy_f, self.px, self.pz, flock_start[fl + 1] - flock_start[fl],
+    coh_finish(ax, az, wsum, coh_weight(0.0f, 0.0f), self.px, self.pz, flock_start[fl + 1] - flock_start[fl],
                __expf(4.5f - 0.12f * COH_R) * 1e7f, scaled_max_force, uid, out_by_uid, fallback, nfallback);
 }
 

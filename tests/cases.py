@@ -323,12 +323,268 @@ def port_tick(omap, agents, flocks, movestate, work, hz, arrival, pool=None, vde
     rec["has_dest_los"][work] = los
     world = pforacle.OracleWorld(omap, rec, flocks, hz)
     try:
-        vel, _ = world.velocity_work(work)
+        vel, vpref = world.velocity_work(work)
         patches = world.entity_updates(movestate, arrival, work, vel, vdes, capi.PATCH)
     finally:
         world.close()
     a2, ms2 = pforacle.entity_apply(rec, movestate, work, patches)
-    return dict(vdes=vdes, los=los, vel=vel, patches=patches, agents=a2, movestate=ms2)
+    return dict(vdes=vdes, los=los, vel=vel, vpref=vpref, patches=patches, agents=a2, movestate=ms2)
+
+
+def nav_layer(flags, radius):
+    """Entity_NavLayerWithRadius (entity.c:554) for arrays: ground 0-3, water 4-7, air 8-11 by radius class
+    (< 5, < 10, < 15, >= 15 wu)"""
+    flags = np.asarray(flags, np.uint32); radius = np.asarray(radius, np.float32)
+    base = np.where(flags & capi.FLAG_WATER, 4, np.where(flags & capi.FLAG_AIR, 8, 0))
+    return (base + (radius >= 5.0) + (radius >= 10.0) + (radius >= 15.0)).astype(np.int32)
+
+
+def port_tick_layers(omaps, agents, flocks, movestate, work, hz, arrivals, layer_of_unit, pool):
+    """port_tick for a population on several navigation layers. The port's world holds one layer, and a unit's layer
+    only changes its own tile probes and arrival constants (neighbours are the whole population on every layer), so
+    the port runs once per layer in use and every unit's results come from the run of its own layer.
+    omaps / arrivals: per layer (OracleMap, route_arrival_consts of every flock target on that layer). pool=None: the
+    desired velocities and LOS bits of the agent records."""
+    work = np.ascontiguousarray(work, np.uint32)
+    lw = np.asarray(layer_of_unit)[work]
+    out = None
+    for L in np.unique(lw):
+        sel = np.nonzero(lw == L)[0]
+        own = {} if pool is not None else dict(vdes=agents["vdes"][work[sel]], los=agents["has_dest_los"][work[sel]])
+        r = port_tick(omaps[L], agents, flocks, movestate, work[sel], hz, arrivals[L], pool=pool, **own)
+        if out is None:
+            out = {k: v.copy() if k in ("agents", "movestate") else np.zeros((len(work),) + v.shape[1:], v.dtype)
+                   for k, v in r.items()}
+        for k in ("vdes", "los", "vel", "vpref", "patches"):
+            out[k][sel] = r[k]
+        for k in ("agents", "movestate"):
+            out[k][work[sel]] = r[k][work[sel]]
+    return out
+
+
+VEL_RTOL = 1e-4
+
+
+def vel_ok(vel, evel, pos, cohesion_floor=0.0):
+    """north_star's 1e-4 relative -- or ONE float spacing of the entity's position, the reference's own noise floor:
+    G_ClearPath_NewVelocity works in absolute map coordinates and returns `chosen point - position` (clearpath.c:694-715),
+    so its result is quantised at ulp(|pos|) (3e-5 wu at |pos| = 256..512) whatever the velocity's own magnitude; a
+    1e-7 relative difference in a preferred velocity (cohesion summation order) can move the chosen point by that one
+    step. cohesion_floor=c widens the floor to c * |pos|: cohesion_force (movement.c:1653) divides the weighted sum of
+    the member positions by the member count, not by the weights, so where that sum nearly cancels the position the
+    term keeps an absolute error proportional to |pos| (the float summation of both sides, and the device's 1e-6
+    relative weights), whatever the preferred velocity's own size.
+    Returns (all within bounds, number of entities that needed the floor)."""
+    d = np.abs(vel - evel).max(axis=1)
+    rel_ok = d <= VEL_RTOL * np.maximum(np.abs(evel).max(axis=1), 1e-3)
+    apos = np.abs(pos).max(axis=1).astype(np.float32)
+    floor_ok = d <= np.maximum(np.spacing(apos), cohesion_floor * apos)
+    return bool((rel_ok | floor_ok).all()), int((~rel_ok & floor_ok).sum())
+
+
+def settle_pool(nav, passes=8, pool=None):
+    """agents_tick with desired velocities from the pool, pool_repair serving the misses, until a pass requests nothing
+    (nreq + nrep == 0); then the compared tick. A pool that has not settled after `passes` fails the test.
+    pool=(ndests, nchunks): a pass without path requests whose repairs leave every pool byte as it was also counts as
+    settled. An entity on a tile that keeps no direction after the repair (its goal tile) is repaired again every
+    tick, as the reference does inline (nav.c:3508-3554), without changing the field."""
+    for _ in range(passes):
+        before = pool_fields(nav, *pool) if pool else None
+        nav.agents_tick(capi.TICK_VDES_FROM_POOL)
+        nreq, nrep = nav.pool_repair()
+        if nreq + nrep == 0:
+            break
+        if pool and nreq == 0 and all(np.array_equal(x, y) for x, y in zip(before, pool_fields(nav, *pool))):
+            break
+    else:
+        raise AssertionError("the field pool did not settle in %d passes: %d requests, %d repairs outstanding" % (passes, nreq, nrep))
+    nav.agents_tick(capi.TICK_VDES_FROM_POOL)
+
+
+def run_trajectory(nav, ref, pforacle, a, ms, cw, cost, hz, nticks, with_blockers, follow=False, ch=None,
+                   map_xz=(0.0, 0.0), nlayers=1, layer_of_unit=None, tiles=None, requests=(), cohesion_modes=(), log=None, cohesion_floor=0.0):
+    """tick -> entity_compute_update -> entity_apply_update -> next snapshot, `nticks` times, on both sides; the engine's
+    share of the apply (entity_block: N_BlockersIncref for patches with next_block, then N_Update) is done by the test
+    on our side. The device state is uploaded once and never touched again.
+    With the compiled reference (ref not None) the reference runs the same ticks. follow=True: before every tick after
+    the first the REFERENCE is re-seeded with the device's state (positions, velocities, movestates), so that every
+    tick is compared on identical inputs; free-running, the two sides are two chaotic trajectories that separate by one
+    position ulp per tick from the first ClearPath rounding step on (tests/tools/diag_traj.py prints both).
+    Without it (ref None) every tick's expectation comes from the plain-C port (port_tick_layers), re-seeded before
+    every tick with the device's state read back: desired velocities and LOS over the device pool's fields read back
+    (both sides consume identical bytes) bit-exact, preferred velocities and velocities (vel_ok), patches (flags, states
+    and blocking identical, floats within 1e-4 of max(|x|, 1)), and the state after the apply; blocker refcounts of
+    every layer from a host-only context and local islands from the numpy restatement, bit-exact. Positions are
+    compared within 1e-4 * max(1, max_speed / hz): 1e-4 of the largest per-tick displacement (at least one float
+    spacing of the map's largest coordinate).
+    The map: cw x ch chunks (ch defaults to cw) placed at map_xz, `nlayers` layers. cost: the cost grid of the one
+    layer, or [nlayers][chunks][64][64]. tiles (int32[H32][W32][4]): the device builds every layer from them
+    (map_cost_from_tiles) and its cost must equal `cost`; the host-only context takes `cost`. layer_of_unit: the
+    navigation layer of every unit (nav_layer); a["flock_layer"], when present, the layer of every flock's fields.
+    requests: (flock, src_xz) path requests (pool_request_path on the flock's layer) made before the first tick.
+    cohesion_modes: every tick's velocity pass is run and compared once per mode (set_cohesion_mode) after the pool
+    has settled. log: a list that receives one dict(work, layers, patches, nfloor) per tick. cohesion_floor: vel_ok's
+    for preferred velocities and velocities.
+    Returns the per-tick (work items, maximum position deviation, maximum velocity deviation)."""
+    ch = cw if ch is None else ch
+    nchunks = cw * ch
+    costs = [cost] if nlayers == 1 else list(cost)
+    assert len(costs) == nlayers
+    assert ref is None or (nlayers == 1 and ch == cw and tuple(map_xz) == (0.0, 0.0)), "the compiled reference runs square maps at the origin, one layer"
+    n = len(a["radius"])
+    nflocks = len(a["flock_target"])
+    lou = np.zeros(n, np.int32) if layer_of_unit is None else np.asarray(layer_of_unit, np.int32)
+    if ref is not None:
+        dest_ids = np.array([ref.dest_id((float(t[0]), float(t[1]))) for t in a["flock_target"]], np.uint32)
+        ref.agents_set(a["pos"], a["prev_pos"], a["vel"], a["radius"], a["max_speed"], a["state"], a["flags"],
+                       a["flock_of"], a["flock_target"], dest_ids, hz=hz)
+        ref.movestate_set(ms["next_pos"][:, [0, 2]], ms["next_rot"], ms["step"], ms["left"], ms["vel_hist"], ms["vel_hist_idx"],
+                          np.zeros(n, np.int32), np.zeros(n, np.int32), ms["combat_facing"])
+    nav.map_create(cw, ch, nlayers, *map_xz)
+    for L in range(nlayers):
+        if tiles is not None:
+            nav.map_cost_from_tiles(L, L, tiles)
+            assert (nav.map_get_layer(L)[0] == costs[L]).all(), L
+        else:
+            nav.map_upload_layer(L, costs[L])
+        nav.map_build_nav(L); nav.route_build(L)
+    nav.pool_create(nflocks, nflocks * nchunks)
+    aa = dict(a); aa["flock_dest_index"] = np.arange(nflocks, dtype=np.int32)
+    rec, fl = capi.pack_agents(aa)
+    if "flock_layer" in a:
+        fl["layer"] = a["flock_layer"]
+    for f, src in requests:
+        nav.pool_request_path(int(f), (float(src[0]), float(src[1])), (float(fl["target"][f][0]), float(fl["target"][f][1])),
+                              layer=int(fl["layer"][f]))
+    nav.agents_upload(rec, fl, hz)
+    nav.agents_upload_movestate(ms)
+    host = None
+    blk, liid = [None] * nlayers, [None] * nlayers
+    if ref is None:         # blockers and the arrived() constants: the host code on a host-only copy of the map
+        host = capi.Nav(hostonly=True)
+        host.map_create(cw, ch, nlayers, *map_xz)
+        for L in range(nlayers):
+            host.map_upload_layer(L, costs[L]); host.map_build_nav(L); host.route_build(L)
+    state = a["state"].copy()
+    snapshot = a["pos"].copy()              # gamestate.positions of the current tick (what entity_block reads, movement.c:583)
+    # 1e-4 of the largest per-tick displacement, and at least one float spacing of the map's largest coordinate
+    extent = max(abs(map_xz[0]), abs(map_xz[0] - cw * 256.0), abs(map_xz[1]), abs(map_xz[1] + ch * 256.0))
+    pos_tol = np.maximum(1e-4 * np.maximum(1.0, a["max_speed"] / hz), np.spacing(np.float32(extent)))
+    out = []
+    # settle both field caches before the first compared tick (the reference fills its cache inline while it walks the
+    # entities, see test_c2_desired_velocity_from_pool_vs_reference)
+    work = np.nonzero((state != 2) & (state != 4))[0].astype(np.uint32)
+    if ref is not None:
+        ref.work_set(work, np.zeros((len(work), 2), np.float32), np.zeros(len(work), np.uint8), a["speed"][work])
+        ref.desired_from_cache()
+    nfloor = 0
+    try:
+        for tick in range(nticks):
+            work = np.nonzero((state != 2) & (state != 4))[0].astype(np.uint32)
+            if len(work) == 0:
+                break
+            # reference
+            if ref is not None:
+                if follow and tick:
+                    ref.agents_set(got["pos"], got["prev_pos"], got["velocity"], a["radius"], a["max_speed"], got["state"], a["flags"],
+                                   a["flock_of"], a["flock_target"], dest_ids, hz=hz)
+                    ref.movestate_set(gms["next_pos"][:, [0, 2]], gms["next_rot"], gms["step"], gms["left"], gms["vel_hist"],
+                                      gms["vel_hist_idx"], np.zeros(n, np.int32), np.zeros(n, np.int32), gms["combat_facing"])
+                ref.work_set(work, np.zeros((len(work), 2), np.float32), np.zeros(len(work), np.uint8), a["speed"][work])
+                evdes, elos = ref.desired_from_cache()
+                evel, _ = ref.velocity_work(os.cpu_count())
+                ref.update_and_apply()
+                est = ref.state_get(n)
+            else:
+                seed_a, seed_ms = nav.agents_read_state(n)
+            # device
+            nav.agents_set_work(work)
+            settle_pool(nav, pool=(nflocks, nchunks))
+            if ref is None:
+                layers = np.unique(lou[work])
+                omaps = {L: pforacle.OracleMap(cw, ch, costs[L], blk[L], liid[L], *map_xz) for L in layers}
+                arrivals = {L: [host.route_arrival_consts(t, int(L)) for t in a["flock_target"]] for L in layers}
+                exp = port_tick_layers(omaps, seed_a, fl, seed_ms, work, hz, arrivals, lou, pool_fields(nav, nflocks, nchunks))
+                evdes, elos, evel = exp["vdes"], exp["los"], exp["vel"]
+            try:
+                for mode in tuple(cohesion_modes) or (None,):
+                    if mode is not None:
+                        nav.set_cohesion_mode(mode)
+                        nav.agents_tick(capi.TICK_VDES_FROM_POOL)
+                    vel = nav.agents_read_velocities(len(work))
+                    vpref, vdes, los = nav.agents_read_debug(len(work))
+                    assert (los == elos).all(), (tick, mode, np.nonzero(los != elos)[0][:10])
+                    if ref is None or tick == 0:
+                        assert (vdes == evdes).all(), (tick, mode, np.nonzero((vdes != evdes).any(axis=1))[0][:10])
+                    else:   # positions carry the <= 1e-6 relative deviation of the previous ticks' velocities into the blend weights
+                        assert np.abs(vdes - evdes).max() <= VEL_RTOL, (tick, np.abs(vdes - evdes).max(), np.nonzero(np.abs(vdes - evdes).max(axis=1) > VEL_RTOL)[0][:10])
+                    if ref is None:
+                        ok, _ = vel_ok(vpref, exp["vpref"], snapshot[work], cohesion_floor)
+                        assert ok, (tick, mode, "vpref", relerr(vpref, exp["vpref"]).max(), work[np.argmax(relerr(vpref, exp["vpref"]))])
+                    ok, nf = vel_ok(vel, evel, snapshot[work], cohesion_floor)
+                    assert ok, (tick, mode, relerr(vel, evel).max(), work[np.argmax(relerr(vel, evel))])
+                    nfloor += nf
+            finally:
+                if cohesion_modes:
+                    nav.set_cohesion_mode(0)
+            nav.agents_compute_updates()
+            patches = nav.agents_read_patches(len(work))
+            nav.agents_apply_updates()
+            nav.agents_rebuild_index()
+            got, gms = nav.agents_read_state(n)
+            if log is not None:
+                log.append(dict(work=work, layers=lou[work], patches=patches, nfloor=nfloor))
+            if ref is None:
+                ep = exp["patches"]
+                same = (patches["flags"] == ep["flags"]) & (patches["next_state"] == ep["next_state"]) & (patches["next_block"] == ep["next_block"])
+                assert same.all(), (tick, work[np.nonzero(~same)[0][:10]])
+                pg, pe = patch_floats(patches), patch_floats(ep)
+                perr = np.abs(pg - pe) / np.maximum(np.abs(pe), 1.0)
+                assert perr.max() <= 1e-4, (tick, perr.max(), np.unravel_index(perr.argmax(), perr.shape))
+                ea, ems = exp["agents"], exp["movestate"]
+                est = dict(state=ea["state"], pos=ea["pos"], prev_pos=ea["prev_pos"], vel=ea["velocity"])
+                for k in ("vel_hist_idx", "left", "step"):
+                    assert (gms[k] == ems[k]).all(), (tick, k, np.nonzero(gms[k] != ems[k])[0][:10])
+                herr = np.abs(gms["vel_hist"] - ems["vel_hist"]) / np.maximum(np.abs(ems["vel_hist"]), 1.0)
+                assert herr.max() <= 1e-4, (tick, herr.max())
+                e_next = np.abs(gms["next_pos"] - ems["next_pos"]).max(axis=1)
+                assert (e_next <= pos_tol).all(), (tick, e_next.max(), np.nonzero(e_next > pos_tol)[0][:10])
+            assert (got["state"] == est["state"]).all(), (tick, np.nonzero(got["state"] != est["state"])[0][:10])
+            e_pos = np.abs(got["pos"] - est["pos"]).max(axis=1); e_prev = np.abs(got["prev_pos"] - est["prev_pos"]).max(axis=1)
+            e_vel = relerr(got["velocity"], est["vel"]).max()
+            # 1e-4 of the largest per-tick displacement (max_speed / hz wu, at least 1)
+            assert (e_pos <= pos_tol).all() and (e_prev <= pos_tol).all() and vel_ok(got["velocity"], est["vel"], snapshot, cohesion_floor)[0], \
+                (tick, e_pos.max(), e_prev.max(), e_vel)
+            out.append((len(work), float(e_pos.max()), float(e_vel)))
+            if with_blockers:
+                # the engine side of entity_apply_update: entity_finish_moving -> entity_block (movement.c:685, 580)
+                stopped = np.nonzero(((patches["flags"] & 1) != 0) & (patches["next_block"] != 0) &
+                                     ((a["flags"][work] & capi.FLAG_GARRISONED) == 0))[0]
+                for w in stopped:
+                    u = work[w]
+                    # G_Pos_GetXZFrom(gamestate.positions): the snapshot position of this tick, not the new one (movement.c:583)
+                    for nv in (nav, host) if host is not None else (nav,):
+                        nv.blockers_incref(float(snapshot[u, 0]), float(snapshot[u, 1]), float(a["radius"][u]), 0, int(a["flags"][u]))
+                nav.map_commit()
+                if ref is not None:
+                    eblk, eliid = [ref.blockers()], [ref.local_islands()]
+                else:
+                    host.map_commit()
+                    eblk = [host.blockers(L) for L in range(nlayers)]
+                    eliid = [local_islands_np(costs[L], eblk[L]) for L in range(nlayers)]
+                    blk, liid = eblk, eliid         # the port's maps of the next tick
+                for L in range(nlayers):
+                    assert (nav.blockers(L) == eblk[L]).all(), (tick, L)
+                    assert (nav.local_islands(L) == eliid[L]).all(), (tick, L)
+            state = got["state"]
+            snapshot = got["pos"].copy()
+    finally:
+        if host is not None:
+            host.close()
+    # the position-ulp floor is a rare event (a rounding step of ClearPath's absolute-coordinate result), not a blanket
+    if not cohesion_floor:          # with the cohesion floor the count includes that term's noise: not a rare event
+        assert nfloor <= max(2, nticks // 2) * max(1, len(tuple(cohesion_modes))), nfloor
+    return out
 
 
 PATCH_FLOATS = ("next_velocity", "next_pos", "next_rot", "next_ppos", "next_npos", "next_step", "next_left", "next_nrot",

@@ -12,7 +12,6 @@ import numpy as np
 import pytest
 
 import cases
-import test_gpu_scale as scale
 
 capi, synth = cases.capi, cases.synth
 SET_STATE, SET_MOVING = 1, 1 << 12
@@ -93,7 +92,7 @@ class Pair:
         for X in (self.A, self.B):
             X.agents_set_work(work)
             if len(work):
-                scale._settle_pool(X, pool=(self.nflocks, self.cw * self.cw))
+                cases.settle_pool(X, pool=(self.nflocks, self.cw * self.cw))
             X.agents_compute_updates()
             out.append((X.agents_read_velocities(len(work)), X.agents_read_patches(len(work))))
         (va, pa), (vb, pb) = out
@@ -357,7 +356,7 @@ def test_errors_host_only(pf):
 
 
 class _DeviceBlockingNav:
-    """a Nav whose apply takes the blocks of stopping units on the device: _run_trajectory's own incref of every
+    """a Nav whose apply takes the blocks of stopping units on the device: cases.run_trajectory's own incref of every
     stopped unit is then the device's, and only the host-only mirror still takes it by hand"""
 
     def __init__(self, nav):
@@ -369,7 +368,7 @@ class _DeviceBlockingNav:
     def agents_upload(self, rec, fl, hz):
         self._nav.agents_upload(rec, fl, hz)
         b = np.zeros(len(rec), capi.BLOCKING)
-        b["faction_id"] = 0                     # the faction _run_trajectory increfs with
+        b["faction_id"] = 0                     # the faction cases.run_trajectory increfs with
         self._nav.agents_upload_blocking(b)
 
     def agents_apply_updates(self, stream=0):
@@ -399,7 +398,7 @@ def test_trajectory_with_device_blocking(pf, nav, pforacle, pfref_or_golden, hz)
     ms["vel_hist"] = np.repeat(a["vel"][:, None, :], 14, axis=1)
     ref = pfref_or_golden.RefMap(cw, cw, p) if pfref_or_golden else None
     try:
-        out = scale._run_trajectory(dnav, ref, pforacle, a, ms, cw, cost, hz, 8, with_blockers=True, follow=True)
+        out = cases.run_trajectory(dnav, ref, pforacle, a, ms, cw, cost, hz, 8, with_blockers=True, follow=True)
         assert len(out) == 8 and out[-1][0] > 1000, out
     finally:
         if ref is not None:
@@ -407,7 +406,7 @@ def test_trajectory_with_device_blocking(pf, nav, pforacle, pfref_or_golden, hz)
     p, cost, a, ms = cases.update_case(4242, hz)
     ref = pfref_or_golden.RefMap(cw, cw, p) if pfref_or_golden else None
     try:
-        out = scale._run_trajectory(dnav, ref, pforacle, a, ms, cw, cost, hz, 1, with_blockers=True)
+        out = cases.run_trajectory(dnav, ref, pforacle, a, ms, cw, cost, hz, 1, with_blockers=True)
         assert len(out) == 1 and out[0][0] > 1000, out
         assert nav.agents_read_blocking(len(a["radius"]))["blocking"].sum() > 50
     finally:

@@ -143,25 +143,6 @@ def test_windowed_cohesion_equals_member_list(pf, nav, bench):
         assert e_v.max() <= VEL_RTOL, (workload, e_v.max())
 
 
-def _settle_pool(nav, passes=8, pool=None):
-    """agents_tick with desired velocities from the pool, pool_repair serving the misses, until a pass requests nothing
-    (nreq + nrep == 0); then the compared tick. A pool that has not settled after `passes` fails the test.
-    pool=(ndests, nchunks): a pass without path requests whose repairs leave every pool byte as it was also counts as
-    settled. An entity on a tile that keeps no direction after the repair (its goal tile) is repaired again every
-    tick, as the reference does inline (nav.c:3508-3554), without changing the field."""
-    for _ in range(passes):
-        before = cases.pool_fields(nav, *pool) if pool else None
-        nav.agents_tick(capi.TICK_VDES_FROM_POOL)
-        nreq, nrep = nav.pool_repair()
-        if nreq + nrep == 0:
-            break
-        if pool and nreq == 0 and all(np.array_equal(x, y) for x, y in zip(before, cases.pool_fields(nav, *pool))):
-            break
-    else:
-        raise AssertionError("the field pool did not settle in %d passes: %d requests, %d repairs outstanding" % (passes, nreq, nrep))
-    nav.agents_tick(capi.TICK_VDES_FROM_POOL)
-
-
 def _pack_route_fields(entries):
     """(flow or None, ffid, los or None) per chunk -> has bits, ffids, the present flow and LOS fields"""
     has = np.array([(fl is not None) | ((lo is not None) << 1) for fl, _, lo in entries], np.uint8)
@@ -238,7 +219,7 @@ def test_c2_desired_velocity_from_pool_vs_reference(pf, nav, pforacle, c2map, be
     rec, fl = capi.pack_agents(aa)
     nav.agents_upload(rec, fl, 20)
     nav.agents_set_work(work)
-    _settle_pool(nav)
+    cases.settle_pool(nav)
     vel = nav.agents_read_velocities(len(work))
     _, vdes, los = nav.agents_read_debug(len(work))
     if ref is None:
@@ -368,155 +349,6 @@ def test_c5_churn_vs_reference(pf, nav, pforacle, c2map, bench):
             host.close()
 
 
-def _vel_ok(vel, evel, pos):
-    """north_star's 1e-4 relative -- or ONE float spacing of the entity's position, the reference's own noise floor:
-    G_ClearPath_NewVelocity works in absolute map coordinates and returns `chosen point - position` (clearpath.c:694-715),
-    so its result is quantised at ulp(|pos|) (3e-5 wu at |pos| = 256..512) whatever the velocity's own magnitude; a
-    1e-7 relative difference in a preferred velocity (cohesion summation order) can move the chosen point by that one
-    step. Returns (all within bounds, number of entities that needed the floor)."""
-    d = np.abs(vel - evel).max(axis=1)
-    rel_ok = d <= VEL_RTOL * np.maximum(np.abs(evel).max(axis=1), 1e-3)
-    floor_ok = d <= np.spacing(np.abs(pos).max(axis=1).astype(np.float32))
-    return bool((rel_ok | floor_ok).all()), int((~rel_ok & floor_ok).sum())
-
-
-def _run_trajectory(nav, ref, pforacle, a, ms, cw, cost, hz, nticks, with_blockers, follow=False):
-    """tick -> entity_compute_update -> entity_apply_update -> next snapshot, `nticks` times, on both sides; the engine's
-    share of the apply (entity_block: N_BlockersIncref for patches with next_block, then N_Update) is done by the test
-    on our side. The device state is uploaded once and never touched again.
-    With the compiled reference (ref not None) the reference runs the same ticks. follow=True: before every tick after
-    the first the REFERENCE is re-seeded with the device's state (positions, velocities, movestates), so that every
-    tick is compared on identical inputs; free-running, the two sides are two chaotic trajectories that separate by one
-    position ulp per tick from the first ClearPath rounding step on (tests/tools/diag_traj.py prints both).
-    Without it (ref None) every tick's expectation comes from the plain-C port (cases.port_tick), re-seeded before every
-    tick with the device's state read back: desired velocities and LOS over the device pool's fields read back (both
-    sides consume identical bytes) bit-exact, velocities, patches (flags, states and blocking identical, floats within
-    1e-4 of max(|x|, 1)), and the state after the apply; blocker refcounts from a host-only context and local islands
-    from the numpy restatement, bit-exact. Positions are compared within 1e-4 * max(1, max_speed / hz): 1e-4 of the
-    largest per-tick displacement.
-    Returns the per-tick (work items, maximum position deviation, maximum velocity deviation)."""
-    n = len(a["radius"])
-    nflocks = len(a["flock_target"])
-    if ref is not None:
-        dest_ids = np.array([ref.dest_id((float(t[0]), float(t[1]))) for t in a["flock_target"]], np.uint32)
-        ref.agents_set(a["pos"], a["prev_pos"], a["vel"], a["radius"], a["max_speed"], a["state"], a["flags"],
-                       a["flock_of"], a["flock_target"], dest_ids, hz=hz)
-        ref.movestate_set(ms["next_pos"][:, [0, 2]], ms["next_rot"], ms["step"], ms["left"], ms["vel_hist"], ms["vel_hist_idx"],
-                          np.zeros(n, np.int32), np.zeros(n, np.int32), ms["combat_facing"])
-    nav.map_create(cw, cw, 1); nav.map_upload_layer(0, cost); nav.map_build_nav(0); nav.route_build(0)
-    nav.pool_create(nflocks, nflocks * cw * cw)
-    aa = dict(a); aa["flock_dest_index"] = np.arange(nflocks, dtype=np.int32)
-    rec, fl = capi.pack_agents(aa)
-    nav.agents_upload(rec, fl, hz)
-    nav.agents_upload_movestate(ms)
-    host, blk, liid = None, None, None
-    if ref is None:         # blockers and the arrived() constants: the host code on a host-only copy of the map
-        host = capi.Nav(hostonly=True)
-        host.map_create(cw, cw, 1); host.map_upload_layer(0, cost); host.map_build_nav(0); host.route_build(0)
-    state = a["state"].copy()
-    snapshot = a["pos"].copy()              # gamestate.positions of the current tick (what entity_block reads, movement.c:583)
-    pos_tol = 1e-4 * np.maximum(1.0, a["max_speed"] / hz)
-    out = []
-    # settle both field caches before the first compared tick (the reference fills its cache inline while it walks the
-    # entities, see test_c2_desired_velocity_from_pool_vs_reference)
-    work = np.nonzero((state != 2) & (state != 4))[0].astype(np.uint32)
-    if ref is not None:
-        ref.work_set(work, np.zeros((len(work), 2), np.float32), np.zeros(len(work), np.uint8), a["speed"][work])
-        ref.desired_from_cache()
-    nfloor = 0
-    try:
-        for tick in range(nticks):
-            work = np.nonzero((state != 2) & (state != 4))[0].astype(np.uint32)
-            if len(work) == 0:
-                break
-            # reference
-            if ref is not None:
-                if follow and tick:
-                    ref.agents_set(got["pos"], got["prev_pos"], got["velocity"], a["radius"], a["max_speed"], got["state"], a["flags"],
-                                   a["flock_of"], a["flock_target"], dest_ids, hz=hz)
-                    ref.movestate_set(gms["next_pos"][:, [0, 2]], gms["next_rot"], gms["step"], gms["left"], gms["vel_hist"],
-                                      gms["vel_hist_idx"], np.zeros(n, np.int32), np.zeros(n, np.int32), gms["combat_facing"])
-                ref.work_set(work, np.zeros((len(work), 2), np.float32), np.zeros(len(work), np.uint8), a["speed"][work])
-                evdes, elos = ref.desired_from_cache()
-                evel, _ = ref.velocity_work(os.cpu_count())
-                ref.update_and_apply()
-                est = ref.state_get(n)
-            else:
-                seed_a, seed_ms = nav.agents_read_state(n)
-            # device
-            nav.agents_set_work(work)
-            _settle_pool(nav, pool=(nflocks, cw * cw))
-            vel = nav.agents_read_velocities(len(work))
-            _, vdes, los = nav.agents_read_debug(len(work))
-            if ref is None:
-                arrival = [host.route_arrival_consts(t) for t in a["flock_target"]]
-                exp = cases.port_tick(pforacle.OracleMap(cw, cw, cost, blk, liid), seed_a, fl, seed_ms, work, hz, arrival,
-                                      pool=cases.pool_fields(nav, nflocks, cw * cw))
-                evdes, elos, evel = exp["vdes"], exp["los"], exp["vel"]
-            assert (los == elos).all(), (tick, np.nonzero(los != elos)[0][:10])
-            if ref is None or tick == 0:
-                assert (vdes == evdes).all(), (tick, np.nonzero((vdes != evdes).any(axis=1))[0][:10])
-            else:   # positions carry the <= 1e-6 relative deviation of the previous ticks' velocities into the blend weights
-                assert np.abs(vdes - evdes).max() <= VEL_RTOL, (tick, np.abs(vdes - evdes).max(), np.nonzero(np.abs(vdes - evdes).max(axis=1) > VEL_RTOL)[0][:10])
-            ok, nf = _vel_ok(vel, evel, snapshot[work])
-            assert ok, (tick, cases.relerr(vel, evel).max())
-            nfloor += nf
-            nav.agents_compute_updates()
-            patches = nav.agents_read_patches(len(work))
-            nav.agents_apply_updates()
-            nav.agents_rebuild_index()
-            got, gms = nav.agents_read_state(n)
-            if ref is None:
-                ep = exp["patches"]
-                same = (patches["flags"] == ep["flags"]) & (patches["next_state"] == ep["next_state"]) & (patches["next_block"] == ep["next_block"])
-                assert same.all(), (tick, work[np.nonzero(~same)[0][:10]])
-                pg, pe = cases.patch_floats(patches), cases.patch_floats(ep)
-                perr = np.abs(pg - pe) / np.maximum(np.abs(pe), 1.0)
-                assert perr.max() <= 1e-4, (tick, perr.max(), np.unravel_index(perr.argmax(), perr.shape))
-                ea, ems = exp["agents"], exp["movestate"]
-                est = dict(state=ea["state"], pos=ea["pos"], prev_pos=ea["prev_pos"], vel=ea["velocity"])
-                for k in ("vel_hist_idx", "left", "step"):
-                    assert (gms[k] == ems[k]).all(), (tick, k, np.nonzero(gms[k] != ems[k])[0][:10])
-                herr = np.abs(gms["vel_hist"] - ems["vel_hist"]) / np.maximum(np.abs(ems["vel_hist"]), 1.0)
-                assert herr.max() <= 1e-4, (tick, herr.max())
-                e_next = np.abs(gms["next_pos"] - ems["next_pos"]).max(axis=1)
-                assert (e_next <= pos_tol).all(), (tick, e_next.max(), np.nonzero(e_next > pos_tol)[0][:10])
-            assert (got["state"] == est["state"]).all(), (tick, np.nonzero(got["state"] != est["state"])[0][:10])
-            e_pos = np.abs(got["pos"] - est["pos"]).max(axis=1); e_prev = np.abs(got["prev_pos"] - est["prev_pos"]).max(axis=1)
-            e_vel = cases.relerr(got["velocity"], est["vel"]).max()
-            # 1e-4 of the largest per-tick displacement (max_speed / hz wu, at least 1)
-            assert (e_pos <= pos_tol).all() and (e_prev <= pos_tol).all() and _vel_ok(got["velocity"], est["vel"], snapshot)[0], \
-                (tick, e_pos.max(), e_prev.max(), e_vel)
-            out.append((len(work), float(e_pos.max()), float(e_vel)))
-            if with_blockers:
-                # the engine side of entity_apply_update: entity_finish_moving -> entity_block (movement.c:685, 580)
-                stopped = np.nonzero(((patches["flags"] & 1) != 0) & (patches["next_block"] != 0) &
-                                     ((a["flags"][work] & capi.FLAG_GARRISONED) == 0))[0]
-                for w in stopped:
-                    u = work[w]
-                    # G_Pos_GetXZFrom(gamestate.positions): the snapshot position of this tick, not the new one (movement.c:583)
-                    for nv in (nav, host) if host is not None else (nav,):
-                        nv.blockers_incref(float(snapshot[u, 0]), float(snapshot[u, 1]), float(a["radius"][u]), 0, int(a["flags"][u]))
-                nav.map_commit()
-                if ref is not None:
-                    eblk, eliid = ref.blockers(), ref.local_islands()
-                else:
-                    host.map_commit()
-                    eblk = host.blockers(0)
-                    eliid = cases.local_islands_np(cost, eblk)
-                    blk, liid = eblk, eliid         # the port's map of the next tick
-                assert (nav.blockers(0) == eblk).all(), tick
-                assert (nav.local_islands(0) == eliid).all(), tick
-            state = got["state"]
-            snapshot = got["pos"].copy()
-    finally:
-        if host is not None:
-            host.close()
-    # the position-ulp floor is a rare event (a rounding step of ClearPath's absolute-coordinate result), not a blanket
-    assert nfloor <= max(2, nticks // 2), nfloor
-    return out
-
-
 @pytest.mark.parametrize("hz", [20, 10, 5, 1])
 def test_device_resident_trajectory_vs_reference(pf, nav, pforacle, pfref_or_golden, hz):
     """SURVEY 8f-3: positions never leave the device between ticks. Eight ticks of a marching crowd (1 500 agents, three
@@ -524,7 +356,7 @@ def test_device_resident_trajectory_vs_reference(pf, nav, pforacle, pfref_or_gol
     arriving crowd (arrivals, adjacent-arrived cascade, WAITING, interpolations left unfinished, blockers taken by the
     stopped entities and the N_Update that follows), at each of the four tick rates (movement.c:2210): against the
     reference's own entity_compute_update / entity_apply_update (movement.c:2303-2766) where it is built, else against
-    the plain-C port (oracle/pf_oracle.c) re-seeded with the device's state every tick (_run_trajectory). At 1 Hz an
+    the plain-C port (oracle/pf_oracle.c) re-seeded with the device's state every tick (cases.run_trajectory). At 1 Hz an
     agent moves up to 20 wu per tick: across index cells, tiles and chunk borders."""
     cw = 3
     # marching crowd
@@ -539,7 +371,7 @@ def test_device_resident_trajectory_vs_reference(pf, nav, pforacle, pfref_or_gol
     ms["vel_hist"] = np.repeat(a["vel"][:, None, :], 14, axis=1)
     ref = pfref_or_golden.RefMap(cw, cw, p) if pfref_or_golden else None
     try:
-        out = _run_trajectory(nav, ref, pforacle, a, ms, cw, cost, hz, 8, with_blockers=True, follow=True)
+        out = cases.run_trajectory(nav, ref, pforacle, a, ms, cw, cost, hz, 8, with_blockers=True, follow=True)
         assert len(out) == 8 and out[-1][0] > 1000, out
     finally:
         if ref is not None:
@@ -552,7 +384,7 @@ def test_device_resident_trajectory_vs_reference(pf, nav, pforacle, pfref_or_gol
     p, cost, a, ms = cases.update_case(4242, hz)
     ref = pfref_or_golden.RefMap(cw, cw, p) if pfref_or_golden else None
     try:
-        out = _run_trajectory(nav, ref, pforacle, a, ms, cw, cost, hz, 1, with_blockers=True)
+        out = cases.run_trajectory(nav, ref, pforacle, a, ms, cw, cost, hz, 1, with_blockers=True)
         assert len(out) == 1 and out[0][0] > 1000, out
     finally:
         if ref is not None:
