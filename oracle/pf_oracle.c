@@ -451,7 +451,14 @@ struct pfo_world {
     uint32_t *cell_start;        /* [ncells+1] */
     uint32_t *sid; int32_t *six, *siy;
     uint32_t *flock_start, *flock_members;
+    const pfo_formation *forms;          /* per uid, may be NULL */
+    const pfo_movestate_ext *exts;       /* per uid, may be NULL */
 };
+
+void pfo_world_set_states(pfo_world *w, const pfo_formation *forms, const pfo_movestate_ext *exts)
+{
+    w->forms = forms; w->exts = exts;
+}
 
 static int32_t bg_scale(float x) { return (int32_t)lrintf(x * 256.0f); }
 static int cell_of(int32_t i, int32_t origin, int n) { int c = (i - origin) >> 12; return c < 0 ? 0 : c >= n ? n - 1 : c; }
@@ -724,18 +731,224 @@ void pfo_line_isect(const float *lines4, long n, float *out3)
 }
 
 /* ------------------------------------------------------------------------------------------
- * move_velocity_work (game/movement.c:3395) for the point-seek states
+ * move_velocity_work (game/movement.c:3395): the state picks the steering variant (movement.c:3414-3448)
+ *   STATE_TURNING                  no preferred velocity, ClearPath only
+ *   STATE_SEEK_ENEMIES             enemy_seek_vpref (movement.c:1946)
+ *   STATE_ARRIVING_TO_CELL         cell_arrival_seek_vpref (movement.c:1908)
+ *   STATE_MOVING_IN_FORMATION      formation_seek_vpref (movement.c:1985)
+ *   every other state              point_seek_vpref (movement.c:1870)
+ * The formation variants read struct formation_state (movement.c:215-225); an entity without an assignment stands
+ * still (movement.c:3426, 3438) and a formation drag caps the speed at 75 % (movement.c:1940, 2017).
+ * The variants beyond point_seek_vpref are NOT an independent restatement: they were written without a reference
+ * checkout and follow k_agent_velocity (pfnav_agents.cu); they stay unpinned until tests/test_oracle.py's
+ * test_port_all_states_vs_ref runs against oracle/_ref (tests/golden/README.md).
  * ---------------------------------------------------------------------------------------- */
 #define FLAG_MOVABLE (1u << 3)
 #define FLAG_AIR (1u << 15)
 #define FLAG_COMBAT_HELD (1u << 21)
+#define STATE_MOVING_IN_FORMATION 1
 #define STATE_ARRIVED 2
+#define STATE_SEEK_ENEMIES 3
 #define STATE_WAITING 4
 #define STATE_TURNING 7
+#define STATE_ARRIVING_TO_CELL 8
+#define FORM_HAS_FORMATION (1u << 0)
+#define FORM_ASSIGNMENT_READY (1u << 1)
+#define FORM_ASSIGNED_TO_CELL (1u << 2)
+#define FORM_IN_RANGE_OF_CELL (1u << 3)
+#define FORM_ARRIVED_AT_CELL (1u << 4)
+#define CELL_ARRIVAL_RADIUS 30.0f           /* movement.c:1769 */
+#define MOVE_ARRIVE_FORCE_SCALE 0.5f
+#define MOVE_COHESION_FORCE_SCALE 0.15f
+#define MOVE_SEPARATION_FORCE_SCALE 0.6f
+#define MOVE_ALIGN_FORCE_SCALE 0.15f
+
+typedef struct {                    /* what the steering functions of one work item read */
+    const pfo_world *w;
+    const pfo_agent *a;
+    uint32_t uid;
+    v2 pos, velocity, vdes;
+    float smf; double smf_d;
+    pfo_formation fs;               /* zero when the world has no formation table */
+} steer_in;
+
+/* separation_force (movement.c:1690) */
+static v2 separation_force(const steer_in *s)
+{
+    uint32_t near_ents[128];
+    int num_near = pfo_ents_in_circle(s->w, s->pos.x, s->pos.z, 30.0f, near_ents, 128);
+    v2 separation = {0.0f, 0.0f};
+    for(int i = 0; i < num_near; i++) {
+        uint32_t curr = near_ents[i];
+        const pfo_agent *o = &s->w->agents[curr];
+        if(curr == s->uid) continue;
+        if(!(o->flags & FLAG_MOVABLE)) continue;
+        if((s->a->flags & FLAG_AIR) != (o->flags & FLAG_AIR)) continue;
+        v2 diff = v2_sub((v2){o->pos[0], o->pos[1]}, s->pos);
+        float radius = s->a->radius + o->radius + 0.0f;
+        if(v2_len(diff) < EPSILON_F) continue;
+        float t = (v2_len(diff) - radius * 0.85f) / v2_len(diff);
+        float mt = -20.0f * t;
+        float scale = exp(mt < 40.0f ? mt : 40.0f);
+        separation = v2_add(separation, v2_scale(diff, scale));
+    }
+    if(num_near == 0) return (v2){0.0f, 0.0f};
+    separation = v2_scale(separation, -1.0f);
+    return v2_truncate(separation, s->smf);
+}
+
+/* arrive_force_point (movement.c:1546) */
+static v2 arrive_force_point(const steer_in *s)
+{
+    const pfo_agent *a = s->a;
+    const int hz = s->w->hz;
+    v2 target = a->flock >= 0 ? (v2){s->w->flocks[a->flock].target[0], s->w->flocks[a->flock].target[1]} : s->pos;
+    v2 desired;
+    if(a->has_dest_los) {
+        desired = v2_sub(target, s->pos);
+        float distance = v2_len(desired);
+        desired = v2_normal(desired);
+        desired = v2_scale(desired, a->max_speed / hz);
+        if(distance < 10.0f) desired = v2_scale(desired, distance / 10.0f);
+    }else desired = v2_scale(s->vdes, a->max_speed / hz);
+    return v2_truncate(v2_sub(desired, s->velocity), s->smf);
+}
+
+/* arrive_force_cell (movement.c:1571): the desired velocity itself, not a correction of the current one */
+static v2 arrive_force_cell(const steer_in *s)
+{
+    v2 desired = v2_sub((v2){s->fs.cell_pos[0], s->fs.cell_pos[1]}, s->pos);
+    float distance = v2_len(desired);
+    if(distance < 10.0f) return v2_scale(desired, distance / 10.0f);
+    return v2_scale(s->vdes, s->a->max_speed / s->w->hz);
+}
+
+/* arrive_force_enemies (movement.c:1593) */
+static v2 arrive_force_enemies(const steer_in *s)
+{
+    v2 desired = v2_scale(s->vdes, s->a->max_speed / s->w->hz);
+    return v2_truncate(v2_sub(desired, s->velocity), s->smf);
+}
+
+/* cohesion_force (movement.c:1653), flock members in ascending uid */
+static v2 cohesion_force(const steer_in *s)
+{
+    const pfo_world *w = s->w;
+    const int32_t flock = s->a->flock;
+    if(flock < 0) return (v2){0.0f, 0.0f};
+    v2 com = {0.0f, 0.0f}; size_t cnt = 0;
+    for(uint32_t k = w->flock_start[flock]; k < w->flock_start[flock + 1]; k++) {
+        uint32_t cu = w->flock_members[k];
+        if(cu == s->uid) continue;
+        v2 cp = {w->agents[cu].pos[0], w->agents[cu].pos[1]};
+        v2 diff = v2_sub(cp, s->pos);
+        float t = (v2_len(diff) - 50.0f * 0.75) / 50.0f;
+        float scale = exp(-6.0f * t);
+        com = v2_add(com, v2_scale(cp, scale));
+        cnt++;
+    }
+    if(!cnt) return (v2){0.0f, 0.0f};
+    com = v2_scale(com, 1.0f / cnt);
+    return v2_truncate(v2_sub(com, s->pos), s->smf);
+}
+
+/* nullify_impass_components (movement.c:1831): the tile probes a steering force may not point into */
+typedef struct { bool on_blocked, lp, lb, rp, rb, tp, tb, bp, bb; } impass_probes;
+static impass_probes impass_probe(const pfo_map *m, v2 pos)
+{
+    impass_probes q; bool d0;
+    probe(m, pos.x, pos.z, &d0, &q.on_blocked);
+    probe(m, pos.x + 4.0f, pos.z, &q.lp, &q.lb); probe(m, pos.x - 4.0f, pos.z, &q.rp, &q.rb);
+    probe(m, pos.x, pos.z + 4.0f, &q.tp, &q.tb); probe(m, pos.x, pos.z - 4.0f, &q.bp, &q.bb);
+    return q;
+}
+static v2 nullify_impass_components(const impass_probes *q, v2 f)
+{
+    if(f.x > 0 && (!q->lp || (!q->on_blocked && q->lb))) f.x = 0.0f;
+    if(f.x < 0 && (!q->rp || (!q->on_blocked && q->rb))) f.x = 0.0f;
+    if(f.z > 0 && (!q->tp || (!q->on_blocked && q->tb))) f.z = 0.0f;
+    if(f.z < 0 && (!q->bp || (!q->on_blocked && q->bb))) f.z = 0.0f;
+    return f;
+}
+
+/* the shared tail of point_seek_vpref / cell_arrival_seek_vpref / formation_seek_vpref (movement.c:1870-1905,
+ * 1908-1944, 1985-2021): the total force first, then separation alone, then arrival alone, each with its impassable
+ * components removed, until one is longer than 1 % of SCALED_MAX_FORCE (a double comparison, movement.c:1895) */
+static v2 prioritized_vpref(const steer_in *s, v2 total, v2 separation, v2 arrive)
+{
+    const impass_probes q = impass_probe(&s->w->map, s->pos);
+    const v2 forces[3] = {total, separation, arrive};
+    v2 steer = {0.0f, 0.0f};
+    for(int prio = 0; prio < 3; prio++) {
+        steer = nullify_impass_components(&q, forces[prio]);
+        if(v2_len(steer) > s->smf_d * 0.01) break;
+    }
+    v2 accel = v2_scale(steer, 1.0f / 1.0f);
+    return v2_truncate(v2_add(s->velocity, accel), s->a->speed / s->w->hz);
+}
+
+/* formation_vpref_limits: the drag cap (movement.c:1940, 2017), then no motion without an assignment (:3426, :3438) */
+static v2 formation_vpref_limits(const steer_in *s, v2 vpref)
+{
+    if(v2_len((v2){s->fs.drag[0], s->fs.drag[1]}) > EPSILON_F)
+        vpref = v2_truncate(vpref, (float)(((double)s->a->speed * 0.75) / (double)s->w->hz));
+    if(!(s->fs.flags & FORM_ASSIGNMENT_READY)) vpref = (v2){0.0f, 0.0f};
+    return vpref;
+}
+
+/* point_seek_vpref (movement.c:1870) with point_seek_total_force (:1745) */
+static v2 point_seek_vpref(const steer_in *s)
+{
+    v2 separation = separation_force(s), arrive = arrive_force_point(s), cohesion = cohesion_force(s);
+    v2 ret = {0.0f, 0.0f};
+    ret = v2_add(ret, v2_scale(arrive, MOVE_ARRIVE_FORCE_SCALE));
+    ret = v2_add(ret, v2_scale(separation, MOVE_SEPARATION_FORCE_SCALE));
+    ret = v2_add(ret, v2_scale(cohesion, MOVE_COHESION_FORCE_SCALE));
+    return prioritized_vpref(s, v2_truncate(ret, s->smf), separation, arrive);
+}
+
+/* formation_seek_vpref (movement.c:1985) with formation_point_seek_total_force (:1960): the formation's own cohesion
+ * force in the place of the flock's */
+static v2 formation_seek_vpref(const steer_in *s)
+{
+    v2 separation = separation_force(s), arrive = arrive_force_point(s);
+    v2 cohesion = {s->fs.cohesion[0], s->fs.cohesion[1]};
+    v2 ret = {0.0f, 0.0f};
+    ret = v2_add(ret, v2_scale(arrive, MOVE_ARRIVE_FORCE_SCALE));
+    ret = v2_add(ret, v2_scale(separation, MOVE_SEPARATION_FORCE_SCALE));
+    ret = v2_add(ret, v2_scale(cohesion, MOVE_COHESION_FORCE_SCALE));
+    return formation_vpref_limits(s, prioritized_vpref(s, v2_truncate(ret, s->smf), separation, arrive));
+}
+
+/* cell_arrival_seek_vpref (movement.c:1908) with cell_seek_total_force (:1769): cohesion and alignment only while the
+ * cell is farther than CELL_ARRIVAL_RADIUS */
+static v2 cell_arrival_seek_vpref(const steer_in *s)
+{
+    v2 separation = separation_force(s), arrive = arrive_force_cell(s);
+    v2 ret = {0.0f, 0.0f};
+    ret = v2_add(ret, v2_scale(arrive, MOVE_ARRIVE_FORCE_SCALE));
+    ret = v2_add(ret, v2_scale(separation, MOVE_SEPARATION_FORCE_SCALE));
+    if(v2_len(v2_sub((v2){s->fs.cell_pos[0], s->fs.cell_pos[1]}, s->pos)) > CELL_ARRIVAL_RADIUS) {
+        ret = v2_add(ret, v2_scale((v2){s->fs.cohesion[0], s->fs.cohesion[1]}, MOVE_COHESION_FORCE_SCALE));
+        ret = v2_add(ret, v2_scale((v2){s->fs.align[0], s->fs.align[1]}, MOVE_ALIGN_FORCE_SCALE));
+    }
+    return formation_vpref_limits(s, prioritized_vpref(s, v2_truncate(ret, s->smf), separation, arrive));
+}
+
+/* enemy_seek_vpref (movement.c:1946) with enemy_seek_total_force (:1801): arrival and separation, no cohesion, no
+ * impassable-component pass and no fall-backs */
+static v2 enemy_seek_vpref(const steer_in *s)
+{
+    v2 separation = separation_force(s), arrive = arrive_force_enemies(s);
+    v2 ret = {0.0f, 0.0f};
+    ret = v2_add(ret, v2_scale(arrive, MOVE_ARRIVE_FORCE_SCALE));
+    ret = v2_add(ret, v2_scale(separation, MOVE_SEPARATION_FORCE_SCALE));
+    v2 accel = v2_scale(v2_truncate(ret, s->smf), 1.0f / 1.0f);
+    return v2_truncate(v2_add(s->velocity, accel), s->a->speed / s->w->hz);
+}
 
 void pfo_velocity_work(const pfo_world *w, const uint32_t *work, size_t nwork, float *out_vel, float *out_vpref)
 {
-    const pfo_map *m = &w->map;
     const int hz = w->hz;
     /* SCALED_MAX_FORCE (movement.c:93): (MAX_FORCE / hz_count * 20.0) is a double */
     const double smf_d = (double)(0.75f / hz) * 20.0;
@@ -750,77 +963,15 @@ void pfo_velocity_work(const pfo_world *w, const uint32_t *work, size_t nwork, f
             continue;
         }
         v2 pos = {a->pos[0], a->pos[1]}, velocity = {a->velocity[0], a->velocity[1]};
-        v2 vdes = {a->vdes[0], a->vdes[1]};
+        steer_in s = {w, a, uid, pos, velocity, {a->vdes[0], a->vdes[1]}, smf, smf_d, {{0}}};
+        if(w->forms) s.fs = w->forms[uid];
         v2 vpref = {0.0f, 0.0f};
-        if(a->state != STATE_TURNING) {
-            /* separation_force (movement.c:1690) */
-            uint32_t near_ents[128];
-            int num_near = pfo_ents_in_circle(w, pos.x, pos.z, 30.0f, near_ents, 128);
-            v2 separation = {0.0f, 0.0f};
-            for(int i = 0; i < num_near; i++) {
-                uint32_t curr = near_ents[i];
-                const pfo_agent *o = &w->agents[curr];
-                if(curr == uid) continue;
-                if(!(o->flags & FLAG_MOVABLE)) continue;
-                if((ent_flags & FLAG_AIR) != (o->flags & FLAG_AIR)) continue;
-                v2 diff = v2_sub((v2){o->pos[0], o->pos[1]}, pos);
-                float radius = a->radius + o->radius + 0.0f;
-                if(v2_len(diff) < EPSILON_F) continue;
-                float t = (v2_len(diff) - radius * 0.85f) / v2_len(diff);
-                float mt = -20.0f * t;
-                float scale = exp(mt < 40.0f ? mt : 40.0f);
-                separation = v2_add(separation, v2_scale(diff, scale));
-            }
-            if(num_near != 0) { separation = v2_scale(separation, -1.0f); separation = v2_truncate(separation, smf); }
-            else separation = (v2){0.0f, 0.0f};
-            /* arrive_force_point (movement.c:1546) */
-            v2 target = a->flock >= 0 ? (v2){w->flocks[a->flock].target[0], w->flocks[a->flock].target[1]} : pos;
-            v2 desired;
-            if(a->has_dest_los) {
-                desired = v2_sub(target, pos);
-                float distance = v2_len(desired);
-                desired = v2_normal(desired);
-                desired = v2_scale(desired, a->max_speed / hz);
-                if(distance < 10.0f) desired = v2_scale(desired, distance / 10.0f);
-            }else desired = v2_scale(vdes, a->max_speed / hz);
-            v2 arrive = v2_truncate(v2_sub(desired, velocity), smf);
-            /* cohesion_force (movement.c:1653), members in ascending uid */
-            v2 cohesion = {0.0f, 0.0f};
-            if(a->flock >= 0) {
-                v2 com = {0.0f, 0.0f}; size_t cnt = 0;
-                for(uint32_t k = w->flock_start[a->flock]; k < w->flock_start[a->flock + 1]; k++) {
-                    uint32_t cu = w->flock_members[k];
-                    if(cu == uid) continue;
-                    v2 cp = {w->agents[cu].pos[0], w->agents[cu].pos[1]};
-                    v2 diff = v2_sub(cp, pos);
-                    float t = (v2_len(diff) - 50.0f * 0.75) / 50.0f;
-                    float scale = exp(-6.0f * t);
-                    com = v2_add(com, v2_scale(cp, scale));
-                    cnt++;
-                }
-                if(cnt) { com = v2_scale(com, 1.0f / cnt); cohesion = v2_truncate(v2_sub(com, pos), smf); }
-            }
-            /* nullify_impass_components probes (movement.c:1831); ground layer 0 only */
-            bool on_blocked, d0, lp, lb, rp, rb, tp, tb, bp, bb;
-            probe(m, pos.x, pos.z, &d0, &on_blocked);
-            probe(m, pos.x + 4.0f, pos.z, &lp, &lb); probe(m, pos.x - 4.0f, pos.z, &rp, &rb);
-            probe(m, pos.x, pos.z + 4.0f, &tp, &tb); probe(m, pos.x, pos.z - 4.0f, &bp, &bb);
-            v2 steer = {0.0f, 0.0f};
-            for(int prio = 0; prio < 3; prio++) {       /* point_seek_vpref (movement.c:1870) */
-                if(prio == 0) {                         /* point_seek_total_force (movement.c:1745) */
-                    v2 A = v2_scale(arrive, 0.5f), C = v2_scale(cohesion, 0.15f), S = v2_scale(separation, 0.6f);
-                    v2 ret = {0.0f, 0.0f};
-                    ret = v2_add(ret, A); ret = v2_add(ret, S); ret = v2_add(ret, C);
-                    steer = v2_truncate(ret, smf);
-                }else if(prio == 1) steer = separation;
-                else steer = arrive;
-                if(steer.x > 0 && (!lp || (!on_blocked && lb))) steer.x = 0.0f;
-                if(steer.x < 0 && (!rp || (!on_blocked && rb))) steer.x = 0.0f;
-                if(steer.z > 0 && (!tp || (!on_blocked && tb))) steer.z = 0.0f;
-                if(steer.z < 0 && (!bp || (!on_blocked && bb))) steer.z = 0.0f;
-                if(v2_len(steer) > smf_d * 0.01) break;
-            }
-            vpref = v2_truncate(v2_add(velocity, v2_scale(steer, 1.0f / 1.0f)), a->speed / hz);
+        switch(a->state) {
+        case STATE_TURNING:             break;
+        case STATE_SEEK_ENEMIES:        vpref = enemy_seek_vpref(&s); break;
+        case STATE_ARRIVING_TO_CELL:    vpref = cell_arrival_seek_vpref(&s); break;
+        case STATE_MOVING_IN_FORMATION: vpref = formation_seek_vpref(&s); break;
+        default:                        vpref = point_seek_vpref(&s); break;
         }
         /* find_neighbours (movement.c:2768) */
         uint32_t near_ents[512];
@@ -1453,8 +1604,12 @@ void pfo_group_arrival_velocity(const pfo_map *m, const uint8_t *fields, const u
 }
 
 /* ------------------------------------------------------------------------------------------
- * State update: entity_compute_update (game/movement.c:2303-2650) for the point-seek states, no formation and
- * no arrival group. The quaternion helpers keep the reference's mix of float and double arithmetic (pf_math.c).
+ * State update: entity_compute_update (game/movement.c:2303-2670), all nine movement states, no arrival group. The
+ * quaternion helpers keep the reference's mix of float and double arithmetic (pf_math.c). The states beyond point
+ * seeking, and the movestate_ext part of the apply, are NOT an independent restatement: they were written without a
+ * reference checkout and follow k_entity_update / k_entity_apply (pfnav_agents.cu), including the heading gate's state
+ * set (MOVING_IN_FORMATION ungated, unverified, DESIGN.md §4); they stay unpinned until test_port_all_states_vs_ref runs
+ * against oracle/_ref.
  * The map of the world holds ONE layer: it stands for the layer Entity_NavLayerWithRadius picks (entity.c:554).
  * ---------------------------------------------------------------------------------------- */
 typedef struct { float x, y, z, w; } pquat;
@@ -1516,21 +1671,68 @@ static pquat turn_toward(pquat cur, pquat target, float max_deg)
     return f;
 }
 
-enum { ST_MOVING = 0, ST_ARRIVED = 2, ST_SEEK_ENEMIES = 3, ST_WAITING = 4, ST_SURROUND = 5, ST_ENTER_RANGE = 6 };
+enum { ST_MOVING = 0, ST_MOVING_IN_FORMATION, ST_ARRIVED, ST_SEEK_ENEMIES, ST_WAITING, ST_SURROUND, ST_ENTER_RANGE,
+       ST_TURNING, ST_ARRIVING_TO_CELL };
 enum { UP_STATE = 1 << 0, UP_VELOCITY = 1 << 1, UP_POSITION = 1 << 2, UP_ROTATION = 1 << 3, UP_NEXT_POS = 1 << 4,
        UP_PREV_POS = 1 << 5, UP_STEP = 1 << 6, UP_LEFT = 1 << 7, UP_NEXT_ROT = 1 << 8, UP_PREV_ROT = 1 << 9,
-       UP_TURNING_IN_PLACE = 1 << 14 };
+       UP_DEST = 1 << 10, UP_TARGET_PREV = 1 << 11, UP_MOVING = 1 << 12, UP_TARGET_DIR = 1 << 13, UP_TURNING_IN_PLACE = 1 << 14 };
+enum { TODO_SURROUND_QUERY = 1 << 0, TODO_USE_SURROUND_FIELD = 1 << 1, TODO_DROP_SURROUND_FIELD = 1 << 2 };
+#define NULL_UID 0xffffffffu
+#define WAIT_TICKS 60                       /* movement.c:97 */
+#define ADJACENCY_SEP_DIST 5.0f             /* movement.c:953 */
 #define FL_WATER (1u << 14)
 #define FL_AIR (1u << 15)
 #define FL_GARRISONED (1u << 18)
 #define FL_COMBAT_HELD (1u << 21)
 
-void pfo_entity_updates(const pfo_world *w, const pfo_movestate *mss, const pfo_arrival *arr, const uint32_t *work, size_t nwork,
-                        const float *new_vel_xz, const float *vdes_xz, pfo_patch *out)
+/* M_NavIsAdjacentToImpassable (nav.c:4745): a 4-neighbour of the tile under `pos` is not passable */
+static bool adjacent_to_impassable(const pfo_map *m, v2 pos)
+{
+    tdesc td;
+    if(!desc_for_point(m, pos.x, pos.z, &td)) return false;
+    const int ar = td.chunk_r * RES + td.tile_r, ac = td.chunk_c * RES + td.tile_c;
+    static const int dr[4] = {-1, 0, 0, 1}, dc[4] = {0, -1, 1, 0};
+    for(int e = 0; e < 4; e++) {
+        const int nr = ar + dr[e], nc = ac + dc[e];
+        if(nr < 0 || nr >= m->chunk_h * RES || nc < 0 || nc >= m->chunk_w * RES) continue;
+        if(!abs_passable(m, nr, nc)) return true;
+    }
+    return false;
+}
+
+/* M_NavIsMaximallyClose (nav.c:4707) over the precomputed tile centres: one within `tol` of `pos` */
+static bool maximally_close(const pfo_arrival *ac, v2 pos, float tol)
+{
+    for(int i = 0; i < ac->mc_n; i++)
+        if(v2_len((v2){ac->mc[2 * i] - pos.x, ac->mc[2 * i + 1] - pos.z}) <= tol) return true;
+    return false;
+}
+
+/* arrived() (movement.c:2170) then adjacent_flock_members (movement.c:953): a flock member within r + r' +
+ * ADJACENCY_SEP_DIST of the CURRENT position that has ARRIVED */
+static bool entity_arrived(const pfo_world *w, const pfo_agent *a, uint32_t uid, const pfo_arrival *ac, v2 new_pos, v2 curr)
+{
+    const pfo_flock *fl = &w->flocks[a->flock];
+    const float thresh = a->radius * 1.5f;
+    if(v2_len(v2_sub((v2){fl->target[0], fl->target[1]}, new_pos)) < thresh) return true;
+    if(adjacent_to_impassable(&w->map, new_pos) && maximally_close(ac, new_pos, thresh)) return true;
+    if(ac->nearest_ok && v2_len((v2){ac->nearest[0] - new_pos.x, ac->nearest[1] - new_pos.z}) < thresh) return true;
+    for(size_t o = 0; o < w->n; o++) {
+        if(o == uid) continue;
+        const pfo_agent *b = &w->agents[o];
+        if(b->state != ST_ARRIVED || b->flock != a->flock) continue;
+        if(v2_len((v2){curr.x - b->pos[0], curr.z - b->pos[1]}) <= a->radius + b->radius + ADJACENCY_SEP_DIST) return true;
+    }
+    return false;
+}
+
+static void set_state(pfo_patch *p, int next, int block) { p->flags |= UP_STATE; p->next_state = next; p->next_block = block; }
+
+void pfo_entity_updates(const pfo_world *w, const pfo_movestate *mss, const pfo_arrival *arr, const pfo_arrival *tarr,
+                        const uint32_t *work, size_t nwork, const float *new_vel_xz, const float *vdes_xz, pfo_patch *out)
 {
     const pfo_map *m = &w->map;
     const float EPS = 1.0f / 1024;
-    const int H64 = m->chunk_h * RES, W64 = m->chunk_w * RES;
     const float turn_rate = (float)((double)(15.0f / (float)w->hz) * 20.0);     /* SCALED_MAX_TURN_RATE (movement.c:434) */
     for(size_t wi = 0; wi < nwork; wi++) {
         const uint32_t uid = work[wi];
@@ -1539,6 +1741,12 @@ void pfo_entity_updates(const pfo_world *w, const pfo_movestate *mss, const pfo_
         pfo_patch p;
         memset(&p, 0, sizeof(p));
         p.next_state = -1;
+        pfo_movestate_ext ex;
+        if(w->exts) ex = w->exts[uid];
+        else { memset(&ex, 0, sizeof(ex)); ex.surround_target_uid = NULL_UID; ex.rot[3] = 1.0f; }
+        pfo_formation fs;
+        if(w->forms) fs = w->forms[uid]; else memset(&fs, 0, sizeof(fs));
+        p.wait_ticks_left = ex.wait_ticks_left;
         const pquat ms_rot = {ms->next_rot[0], ms->next_rot[1], ms->next_rot[2], ms->next_rot[3]};
         v2 new_vel = {new_vel_xz[2 * wi], new_vel_xz[2 * wi + 1]};
         const v2 vdes = {vdes_xz[2 * wi], vdes_xz[2 * wi + 1]};
@@ -1626,68 +1834,109 @@ void pfo_entity_updates(const pfo_world *w, const pfo_movestate *mss, const pfo_
         }
         bool cur_path, cur_blk;                              /* stuck on non-pathable terrain: keep the state (:2417) */
         probe(m, new_pos_xz.x, new_pos_xz.z, &cur_path, &cur_blk);
-        if(!cur_path || a->flock < 0 || state != ST_MOVING) { out[wi] = p; continue; }
+        if(!cur_path) { out[wi] = p; continue; }
 
-        /* STATE_MOVING (movement.c:2421-2495) */
-        const pfo_flock *fl = &w->flocks[a->flock];
-        const pfo_arrival *ac = &arr[a->flock];
-        bool arrived = false;
-        {   /* arrived() (movement.c:2170) */
-            const v2 tgt = {fl->target[0], fl->target[1]};
-            const float thresh = a->radius * 1.5f;
-            if(v2_len(v2_sub(tgt, new_pos_xz)) < thresh) arrived = true;
-            if(!arrived) {                                   /* N_IsAdjacentToImpassable (nav.c:4745) && N_IsMaximallyClose (:4707) */
-                tdesc td; bool adj = false;
-                if(desc_for_point(m, new_pos_xz.x, new_pos_xz.z, &td)) {
-                    const int ar = td.chunk_r * RES + td.tile_r, acol = td.chunk_c * RES + td.tile_c;
-                    static const int dr[4] = {-1, 0, 0, 1}, dc[4] = {0, -1, 1, 0};
-                    for(int e = 0; e < 4 && !adj; e++) {
-                        const int nr = ar + dr[e], nc = acol + dc[e];
-                        if(nr < 0 || nr >= H64 || nc < 0 || nc >= W64) continue;
-                        adj = !abs_passable(m, nr, nc);
-                    }
-                }
-                if(adj)
-                    for(int i = 0; i < ac->mc_n && !arrived; i++) {
-                        const v2 d = {ac->mc[2 * i] - new_pos_xz.x, ac->mc[2 * i + 1] - new_pos_xz.z};
-                        if(v2_len(d) <= thresh) arrived = true;
-                    }
+        const bool has_fid = (fs.flags & FORM_HAS_FORMATION) != 0;
+        const bool ready = (fs.flags & FORM_ASSIGNMENT_READY) != 0;
+        switch(state) {
+        case ST_MOVING:
+        case ST_MOVING_IN_FORMATION:                         /* movement.c:2421-2500 */
+            if(has_fid && !ready) break;                     /* wait for the formation's cell assignment */
+            if(has_fid && (fs.flags & FORM_ASSIGNED_TO_CELL) && (fs.flags & FORM_IN_RANGE_OF_CELL)) {
+                set_state(&p, ST_ARRIVING_TO_CELL, 0);
+                break;
             }
-            if(!arrived && ac->nearest_ok) {                 /* N_ClosestPathable (nav.c:4126) */
-                const v2 d = {ac->nearest[0] - new_pos_xz.x, ac->nearest[1] - new_pos_xz.z};
-                if(v2_len(d) < thresh) arrived = true;
+            if(a->flock < 0) break;
+            if(entity_arrived(w, a, uid, &arr[a->flock], new_pos_xz, curr_xz)) set_state(&p, ST_ARRIVED, 1);
+            else if(v2_len(vdes) < EPS) set_state(&p, ST_WAITING, 1);
+            break;
+        case ST_SEEK_ENEMIES:                                /* movement.c:2501: retried every tick */
+            break;
+        case ST_SURROUND:                                    /* movement.c:2505-2567 */
+            if(ex.surround_target_uid == NULL_UID) set_state(&p, ST_ARRIVED, 1);
+            else p.engine_todo |= TODO_SURROUND_QUERY;       /* the target's geometry is the engine's (deviation 4) */
+            break;
+        case ST_ENTER_RANGE: {                               /* movement.c:2569-2603 */
+            if(ex.surround_target_uid == NULL_UID) { set_state(&p, ST_ARRIVED, 1); break; }
+            const pfo_agent *t = &w->agents[ex.surround_target_uid];
+            const v2 xz_target = {t->pos[0], t->pos[1]};
+            bool in_range = v2_len(v2_sub(new_pos_xz, xz_target)) <= ex.target_range;
+            /* M_NavIsAdjacentToImpassable && M_NavIsMaximallyClose(.., tolerance 0.0f) (movement.c:2584) */
+            if(!in_range && tarr && adjacent_to_impassable(m, new_pos_xz)) in_range = maximally_close(&tarr[wi], new_pos_xz, 0.0f);
+            if(in_range) { set_state(&p, ST_WAITING, 1); break; }
+            if(v2_len(v2_sub(xz_target, (v2){ex.target_prev_pos[0], ex.target_prev_pos[1]})) > 5.0f) {
+                /* the target moved: re-issue the move order towards it (G_Move_SetDest, attack = false) */
+                p.flags |= UP_DEST | UP_TARGET_PREV;
+                p.next_dest[0] = xz_target.x; p.next_dest[1] = xz_target.z; p.next_attack = 0;
+                p.next_target_prev[0] = xz_target.x; p.next_target_prev[1] = xz_target.z;
             }
+            break;
         }
-        if(!arrived) {
-            /* adjacent_flock_members (movement.c:953): a flock member within r + r' + ADJACENCY_SEP_DIST that has ARRIVED */
-            for(size_t o = 0; o < w->n && !arrived; o++) {
-                if(o == uid) continue;
-                const pfo_agent *b = &w->agents[o];
-                if(b->state != ST_ARRIVED || b->flock != a->flock) continue;
-                const v2 d = {curr_xz.x - b->pos[0], curr_xz.z - b->pos[1]};
-                if(v2_len(d) <= a->radius + b->radius + 5.0f) arrived = true;
-            }
+        case ST_TURNING: {                                   /* movement.c:2605-2627 */
+            const pquat ent_rot = {ex.rot[0], ex.rot[1], ex.rot[2], ex.rot[3]};
+            const pquat tdir = {ex.target_dir[0], ex.target_dir[1], ex.target_dir[2], ex.target_dir[3]};
+            const float degrees = (float)((double)quat_pitch_diff(ent_rot, tdir) * (180.0f / PFO_PI_D));
+            if(fabs((double)degrees) <= 5.0f) { set_state(&p, ST_ARRIVED, 1); break; }
+            const pquat r = turn_toward(ent_rot, tdir, turn_rate);
+            p.flags |= UP_ROTATION | UP_PREV_ROT;
+            p.next_rot[0] = r.x; p.next_rot[1] = r.y; p.next_rot[2] = r.z; p.next_rot[3] = r.w;
+            p.next_prot[0] = r.x; p.next_prot[1] = r.y; p.next_prot[2] = r.z; p.next_prot[3] = r.w;
+            break;
         }
-        if(arrived) { p.flags |= UP_STATE; p.next_state = ST_ARRIVED; p.next_block = 1; }
-        else if(v2_len(vdes) < EPS) { p.flags |= UP_STATE; p.next_state = ST_WAITING; p.next_block = 1; }
+        case ST_WAITING:                                     /* movement.c:2630-2645: the countdown, then the old state */
+            p.wait_ticks_left = ex.wait_ticks_left - 1;
+            if(p.wait_ticks_left == 0) { p.flags |= UP_MOVING; p.next_state = ex.wait_prev; }
+            break;
+        case ST_ARRIVING_TO_CELL:                            /* movement.c:2648-2670 */
+            if(!has_fid) { set_state(&p, ST_MOVING, 0); break; }
+            if(!ready) break;
+            if(!(fs.flags & FORM_IN_RANGE_OF_CELL)) { set_state(&p, ST_MOVING_IN_FORMATION, 0); break; }
+            if(fs.flags & FORM_ARRIVED_AT_CELL) {
+                set_state(&p, ST_TURNING, 0);
+                p.flags |= UP_TARGET_DIR;
+                memcpy(p.next_target_dir, fs.target_orientation, sizeof(p.next_target_dir));
+            }
+            break;
+        default:                                             /* ST_ARRIVED */
+            break;
+        }
+        /* ent_update_using_surround_field (movement.c:2672-2691), on the tick's snapshot positions, for the state the
+         * entity is in after this update: start using the surround field inside a third of a chunk of the target, stop
+         * outside half a chunk */
+        const uint32_t after = (p.flags & (UP_STATE | UP_MOVING)) ? (uint32_t)p.next_state : state;
+        if(after == ST_SURROUND && ex.surround_target_uid != NULL_UID) {
+            const pfo_agent *t = &w->agents[ex.surround_target_uid];
+            const float dx = (float)fabs((double)(t->pos[0] - curr_xz.x)), dz = (float)fabs((double)(t->pos[1] - curr_xz.z));
+            const float low = (float)(256.0 / 3.0f), high = (float)(256.0 / 2.0f);
+            if(!ex.using_surround_field) { if(dx < low && dz < low) p.engine_todo |= TODO_USE_SURROUND_FIELD; }
+            else if(dx >= high || dz >= high) p.engine_todo |= TODO_DROP_SURROUND_FIELD;
+        }
         out[wi] = p;
     }
 }
 
-/* The movestate part of entity_apply_update (movement.c:2693-2757) for one patch: velocity + velocity history
- * (update_vel_hist :2025, seed_vel_hist_facing :2046 / facing_dir :2040), interpolation fields, next rotation. State
- * transitions clear the velocity (entity_finish_moving, movement.c:685). agents / mss are updated in place. */
-void pfo_entity_apply(pfo_agent *agents, pfo_movestate *mss, const uint32_t *work, size_t nwork, const pfo_patch *patches)
+/* The movestate part of entity_apply_update (movement.c:2693-2757) for one patch: the waiting countdown, the state
+ * (entity_finish_moving, movement.c:685, clears the velocity and a stop to WAITING records the state it leaves and
+ * WAIT_TICKS), velocity + velocity history (update_vel_hist :2025, seed_vel_hist_facing :2046 / facing_dir :2040),
+ * interpolation fields, rotations, the ENTER_ENTITY_RANGE / TURNING targets, SET_MOVING (move_notify_motion_start wipes
+ * the history unless combat-held) and the surround-field bit. agents / mss / exts are updated in place. */
+void pfo_entity_apply(pfo_agent *agents, pfo_movestate *mss, pfo_movestate_ext *exts, const uint32_t *work, size_t nwork,
+                      const pfo_patch *patches)
 {
     const float EPS = 1.0f / 1024;
     for(size_t wi = 0; wi < nwork; wi++) {
         pfo_agent *a = &agents[work[wi]];
         pfo_movestate *ms = &mss[work[wi]];
+        pfo_movestate_ext *ex = exts ? &exts[work[wi]] : NULL;
         const pfo_patch *p = &patches[wi];
         if(a->flags & FL_GARRISONED) continue;                                   /* movement.c:2697 */
+        if(ex) ex->wait_ticks_left = p->wait_ticks_left;
         if(p->flags & UP_STATE) {
+            if(p->next_state == ST_ARRIVED || p->next_state == ST_WAITING) {
+                if(ex && p->next_state == ST_WAITING) { ex->wait_prev = (int32_t)a->state; ex->wait_ticks_left = WAIT_TICKS; }
+                a->velocity[0] = 0.0f; a->velocity[1] = 0.0f;
+            }
             a->state = (uint32_t)p->next_state;
-            if(p->next_state == ST_ARRIVED || p->next_state == ST_WAITING) { a->velocity[0] = 0.0f; a->velocity[1] = 0.0f; }
         }
         if(p->flags & UP_VELOCITY) {
             a->velocity[0] = p->next_velocity[0]; a->velocity[1] = p->next_velocity[1];
@@ -1713,5 +1962,18 @@ void pfo_entity_apply(pfo_agent *agents, pfo_movestate *mss, const uint32_t *wor
         if(p->flags & UP_STEP) ms->step = p->next_step;
         if(p->flags & UP_LEFT) ms->left = (int)p->next_left;
         if(p->flags & UP_NEXT_ROT) memcpy(ms->next_rot, p->next_nrot, sizeof(ms->next_rot));
+        if(ex) {
+            if(p->flags & UP_ROTATION) memcpy(ex->rot, p->next_rot, sizeof(ex->rot));                  /* Entity_SetRot */
+            if(p->flags & UP_TARGET_PREV) memcpy(ex->target_prev_pos, p->next_target_prev, sizeof(ex->target_prev_pos));
+            if(p->flags & UP_TARGET_DIR) memcpy(ex->target_dir, p->next_target_dir, sizeof(ex->target_dir));
+        }
+        if(p->flags & UP_MOVING) {
+            if(!(a->flags & FL_COMBAT_HELD)) memset(ms->vel_hist, 0, sizeof(ms->vel_hist));
+            a->state = (uint32_t)p->next_state;
+        }
+        if(ex && a->state == ST_SURROUND) {
+            if(p->engine_todo & TODO_USE_SURROUND_FIELD) ex->using_surround_field = 1;
+            if(p->engine_todo & TODO_DROP_SURROUND_FIELD) ex->using_surround_field = 0;
+        }
     }
 }

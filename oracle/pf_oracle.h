@@ -62,8 +62,24 @@ typedef struct pfo_world pfo_world;
 pfo_world *pfo_world_create(const pfo_map *map, const pfo_agent *agents, size_t n,
                             const pfo_flock *flocks, size_t nflocks, int hz);
 void pfo_world_destroy(pfo_world *w);
+/* The inputs of the states beyond point seeking, per uid (layout-identical to pfnav_formation_in / pfnav_movestate_ext):
+ * struct formation_state + cell_pos + cell_arrival_vdes of struct move_work_in (movement.c:215-225, 264-276) and the
+ * rest of struct movestate (movement.c:146-215). Either may be NULL: no formation / NULL_UID targets, zero counters. The
+ * world keeps the pointers; the caller keeps the arrays alive. */
+typedef struct pfo_formation {
+    float cell_pos[2], cell_arrival_vdes[2], cohesion[2], align[2], drag[2], target_orientation[4];
+    uint32_t flags, _pad;
+} pfo_formation;
+typedef struct pfo_movestate_ext {
+    int32_t wait_prev, wait_ticks_left;
+    uint32_t surround_target_uid, using_surround_field;
+    float target_range, target_prev_pos[2], _padf, target_dir[4], rot[4];
+} pfo_movestate_ext;
+void pfo_world_set_states(pfo_world *w, const pfo_formation *forms, const pfo_movestate_ext *exts);
 int  pfo_ents_in_circle(const pfo_world *w, float x, float z, float range, uint32_t *out, int maxout);
-/* vdes / has_dest_los are taken from the agent records. out_vel/out_vpref: 2 floats per work item */
+/* vdes / has_dest_los are taken from the agent records (for STATE_ARRIVING_TO_CELL the caller puts cell_arrival_vdes
+ * there, ent_desired_velocity, movement.c:1507). The state picks the steering variant (movement.c:3414-3448).
+ * out_vel/out_vpref: 2 floats per work item */
 void pfo_velocity_work(const pfo_world *w, const uint32_t *work, size_t nwork, float *out_vel,
                        float *out_vpref);
 /* G_ClearPath_NewVelocity (clearpath.c:694) then vec2_truncate(max_len) (movement.c:3464), as pfo_velocity_work runs it.
@@ -98,23 +114,30 @@ void pfo_group_arrival_field(const pfo_map *m, int dim, uint16_t enemies, const 
                              const float *center_xz, const int32_t *overlay, int noverlay, uint8_t *out);
 void pfo_region_field_update_to_nearest_pathable(const pfo_map *m, int dim, int start_r, int start_c, int center_r, int center_c,
                                                  const int32_t *overlay, int noverlay, uint8_t *inout);
-/* State update: entity_compute_update (movement.c:2303-2650) for the point-seek states. Records are layout-identical to
- * pfnav_movestate / pfnav_patch. arr[flock]: the two map searches of arrived() (movement.c:2170) for the flock's target:
- * N_ClosestPathable (nav.c:4126) and the tile centres N_IsMaximallyClose compares with (nav.c:4707, n_closest_island_tiles
- * :1226), mc = 2 floats per tile. out: one patch per work item. */
+/* State update: entity_compute_update (movement.c:2303-2670), all nine movement states. Records are layout-identical to
+ * pfnav_movestate / pfnav_patch (160 B, struct movestate_patch, movement.c:245-262). arr[flock]: the two map searches of
+ * arrived() (movement.c:2170) for the flock's target: N_ClosestPathable (nav.c:4126) and the tile centres
+ * N_IsMaximallyClose compares with (nav.c:4707, n_closest_island_tiles :1226), mc = 2 floats per tile. tarr[work item]
+ * (may be NULL): the same tile centres for the target entity's position of a STATE_ENTER_ENTITY_RANGE item
+ * (movement.c:2584). The STATE_WAITING countdown is reported in the patch's wait_ticks_left, the movestate_ext records
+ * are not modified. out: one patch per work item. */
 typedef struct pfo_movestate {
     float next_pos[3], step, next_rot[4], combat_facing[4], vel_hist[14][2];
     int32_t left, vel_hist_idx, _pad[2];
 } pfo_movestate;
 typedef struct pfo_patch {
-    uint32_t flags; int32_t next_state, next_block, _pad;
-    float next_velocity[2], next_pos[3], next_rot[4], next_ppos[3], next_npos[3], next_step, next_left, next_nrot[4], next_prot[4], _padf[3];
+    uint32_t flags; int32_t next_state, next_block, next_attack;
+    float next_velocity[2], next_pos[3], next_rot[4], next_ppos[3], next_npos[3], next_step, next_left, next_nrot[4], next_prot[4];
+    int32_t wait_ticks_left; uint32_t engine_todo; float _padf;
+    float next_dest[2], next_target_prev[2], next_target_dir[4];
 } pfo_patch;
 typedef struct pfo_arrival { int32_t nearest_ok; float nearest[2]; int32_t mc_n; const float *mc; } pfo_arrival;
-void pfo_entity_updates(const pfo_world *w, const pfo_movestate *mss, const pfo_arrival *arr, const uint32_t *work, size_t nwork,
-                        const float *new_vel_xz, const float *vdes_xz, pfo_patch *out);
-/* the movestate part of entity_apply_update (movement.c:2693-2757), in place on agents / movestate records */
-void pfo_entity_apply(pfo_agent *agents, pfo_movestate *mss, const uint32_t *work, size_t nwork, const pfo_patch *patches);
+void pfo_entity_updates(const pfo_world *w, const pfo_movestate *mss, const pfo_arrival *arr, const pfo_arrival *tarr,
+                        const uint32_t *work, size_t nwork, const float *new_vel_xz, const float *vdes_xz, pfo_patch *out);
+/* the movestate part of entity_apply_update (movement.c:2693-2757), in place on agents / movestate / movestate_ext records
+ * (exts may be NULL) */
+void pfo_entity_apply(pfo_agent *agents, pfo_movestate *mss, pfo_movestate_ext *exts, const uint32_t *work, size_t nwork,
+                      const pfo_patch *patches);
 /* TARGET_ZONE chunk fields: N_FlowFieldUpdate -> field_update_zone (field.c:2050, 1810), its seed flood
  * field_zone_initial_frontier (field.c:1683) and the per-entity consumer N_DesiredGroupArrivalVelocity (nav.c:3561).
  * centre in absolute tile coordinates; inout = 64 x 64 direction bytes of chunk (chunk_r, chunk_c). */

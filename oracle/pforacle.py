@@ -43,8 +43,10 @@ def lib():
                                               C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         L.pfo_group_arrival_field.argtypes = [C.POINTER(_Map), C.c_int, C.c_uint16, C.c_void_p, C.c_int, C.c_void_p,
                                               C.c_void_p, C.c_int, C.c_void_p]
-        L.pfo_entity_updates.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.pfo_entity_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        L.pfo_world_set_states.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pfo_entity_updates.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]
+        L.pfo_entity_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         L.pfo_zone_seeds.restype = C.c_int
         L.pfo_zone_seeds.argtypes = [C.POINTER(_Map)] + [C.c_int] * 5 + [C.c_void_p]
         L.pfo_chunk_field_seeded.argtypes = [C.POINTER(_Map), C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
@@ -205,32 +207,38 @@ def line_isect(lines):
     return out
 
 
-def entity_apply(agents, movestate, work, patches):
-    """entity_apply_update's movestate part -> (agents, movestate) copies after the patches"""
+def entity_apply(agents, movestate, work, patches, ext=None):
+    """entity_apply_update's movestate part -> (agents, movestate) copies after the patches, and the movestate_ext copy
+    (64-B records, uid order) when `ext` is given: (agents, movestate, ext)"""
     a = np.ascontiguousarray(agents).copy(); ms = np.ascontiguousarray(movestate).copy()
+    ex = None if ext is None else np.ascontiguousarray(ext).copy()
+    assert ex is None or ex.dtype.itemsize == 64
     work = np.ascontiguousarray(work, np.uint32); p = np.ascontiguousarray(patches)
-    lib().pfo_entity_apply(_p(a), _p(ms), _p(work), len(work), _p(p))
-    return a, ms
+    assert p.dtype.itemsize == 160
+    lib().pfo_entity_apply(_p(a), _p(ms), _p(ex), _p(work), len(work), _p(p))
+    return (a, ms) if ext is None else (a, ms, ex)
 
 
 class _Arrival(C.Structure):
     _fields_ = [("nearest_ok", C.c_int32), ("nearest", C.c_float * 2), ("mc_n", C.c_int32), ("mc", C.c_void_p)]
 
 
-PATCH128 = np.dtype([
-    ("flags", "<u4"), ("next_state", "<i4"), ("next_block", "<i4"), ("_pad", "<i4"),
-    ("next_velocity", "<f4", 2), ("next_pos", "<f4", 3), ("next_rot", "<f4", 4), ("next_ppos", "<f4", 3),
-    ("next_npos", "<f4", 3), ("next_step", "<f4"), ("next_left", "<f4"), ("next_nrot", "<f4", 4),
-    ("next_prot", "<f4", 4), ("_padf", "<f4", 3)])
 
 
 class OracleWorld:
-    def __init__(self, omap, agents, flocks, hz=20):
+    def __init__(self, omap, agents, flocks, hz=20, formation=None, ext=None):
+        """formation / ext: per-uid FORMATION_IN / MOVESTATE_EXT records (64 B each) of the states beyond point seeking,
+        or None (no formation; NULL_UID targets and zero counters)"""
         self.omap = omap
         self.agents = np.ascontiguousarray(agents)
         self.flocks = np.ascontiguousarray(flocks)
+        self.formation = None if formation is None else np.ascontiguousarray(formation)
+        self.ext = None if ext is None else np.ascontiguousarray(ext)
+        for r in (self.formation, self.ext):
+            assert r is None or (r.dtype.itemsize == 64 and len(r) == len(self.agents))
         self.h = lib().pfo_world_create(C.byref(omap.m), _p(self.agents), len(self.agents), _p(self.flocks),
                                         len(self.flocks), hz)
+        lib().pfo_world_set_states(self.h, _p(self.formation), _p(self.ext))
 
     def close(self):
         if self.h:
@@ -242,19 +250,30 @@ class OracleWorld:
         n = lib().pfo_ents_in_circle(self.h, x, z, r, _p(out), maxout)
         return out[:n].copy()
 
-    def entity_updates(self, movestate, arrival, work, new_vel, vdes, patch_dtype):
+    @staticmethod
+    def _arrivals(arrival):
+        """(nearest_ok, nearest[2], mc[n, 2]) tuples (None: no tiles) -> ctypes array, arrays kept alive"""
+        keep = [np.zeros((0, 2), np.float32) if a is None else np.ascontiguousarray(a[2], np.float32).reshape(-1, 2) for a in arrival]
+        arr = (_Arrival * max(len(arrival), 1))()
+        for i, a in enumerate(arrival):
+            if a is not None:
+                arr[i].nearest_ok = int(a[0]); arr[i].nearest[0], arr[i].nearest[1] = float(a[1][0]), float(a[1][1])
+            arr[i].mc_n = len(keep[i]); arr[i].mc = keep[i].ctypes.data
+        return arr, keep
+
+    def entity_updates(self, movestate, arrival, work, new_vel, vdes, patch_dtype, target_arrival=None):
         """entity_compute_update per work item. movestate: 176-B records (uid order); arrival: per flock
-        (nearest_ok, nearest[2], mc[n, 2]); -> record array of patch_dtype (128 B)"""
+        (nearest_ok, nearest[2], mc[n, 2]); target_arrival: per work item the same for the target of an
+        ENTER_ENTITY_RANGE item (None for the others), or None; -> record array of patch_dtype (160 B)"""
         ms = np.ascontiguousarray(movestate); work = np.ascontiguousarray(work, np.uint32)
         nv = np.ascontiguousarray(new_vel, np.float32); vd = np.ascontiguousarray(vdes, np.float32)
-        keep = [np.ascontiguousarray(a[2], np.float32).reshape(-1, 2) for a in arrival]
-        arr = (_Arrival * len(arrival))()
-        for i, a in enumerate(arrival):
-            arr[i].nearest_ok = int(a[0]); arr[i].nearest[0], arr[i].nearest[1] = float(a[1][0]), float(a[1][1])
-            arr[i].mc_n = len(keep[i]); arr[i].mc = keep[i].ctypes.data
-        out = np.zeros(len(work), PATCH128)        # the port's pfo_patch (the point-seek subset of struct movestate_patch)
-        assert out.dtype.itemsize == 128 and ms.dtype.itemsize == 176
-        lib().pfo_entity_updates(self.h, _p(ms), C.byref(arr), _p(work), len(work), _p(nv), _p(vd), _p(out))
+        arr, keep = self._arrivals(arrival)
+        tarr, tkeep = (None, None) if target_arrival is None else self._arrivals(target_arrival)
+        assert target_arrival is None or len(target_arrival) == len(work)
+        out = np.zeros(len(work), patch_dtype)
+        assert out.dtype.itemsize == 160 and ms.dtype.itemsize == 176
+        lib().pfo_entity_updates(self.h, _p(ms), C.byref(arr), None if tarr is None else C.byref(tarr), _p(work), len(work),
+                                 _p(nv), _p(vd), _p(out))
         return out
 
     def velocity_work(self, work):

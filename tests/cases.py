@@ -306,14 +306,17 @@ def pool_fields(nav, ndests, nchunks):
     return slot, np.array(flow, np.uint8).reshape(-1, 64, 64), np.array(los, np.uint8).reshape(-1, 64, 64)
 
 
-def port_tick(omap, agents, flocks, movestate, work, hz, arrival, pool=None, vdes=None, los=None):
-    """One tick of the point-seek pipeline in the plain-C port (oracle/pf_oracle.c): desired velocity and LOS bit
-    (pfo_desired_velocity over `pool`, else the given `vdes` / `los`), the velocity pass on them (pfo_velocity_work),
-    entity_compute_update on the new velocities (pfo_entity_updates) and the movestate part of entity_apply_update
+def port_tick(omap, agents, flocks, movestate, work, hz, arrival, pool=None, vdes=None, los=None, formation=None, ext=None,
+              target_arrival=None):
+    """One tick in the plain-C port (oracle/pf_oracle.c): desired velocity and LOS bit (pfo_desired_velocity over `pool`,
+    else the given `vdes` / `los`), the velocity pass on them (pfo_velocity_work, every steering variant), entity_compute_update
+    on the new velocities (pfo_entity_updates, all nine states) and the movestate part of entity_apply_update
     (pfo_entity_apply).
     agents / movestate: AGENT / MOVESTATE records of the whole population (not modified); flocks: FLOCK records;
     work: the uids of this tick; arrival: route_arrival_consts of every flock target; pool: pool_fields().
-    -> dict(vdes, los, vel, patches, agents, movestate), the last two after the apply."""
+    formation / ext: FORMATION_IN / MOVESTATE_EXT records of the whole population (not modified) or None;
+    target_arrival: per work item route_arrival_consts of an ENTER_ENTITY_RANGE item's target (None elsewhere), or None.
+    -> dict(vdes, los, vel, vpref, patches, agents, movestate[, ext]), the last ones after the apply."""
     import pforacle
     work = np.ascontiguousarray(work, np.uint32)
     rec = np.array(agents, capi.AGENT)
@@ -321,14 +324,18 @@ def port_tick(omap, agents, flocks, movestate, work, hz, arrival, pool=None, vde
         vdes, los = omap.desired_velocity(rec, flocks, work, *pool)
     rec["vdes"][work] = vdes
     rec["has_dest_los"][work] = los
-    world = pforacle.OracleWorld(omap, rec, flocks, hz)
+    world = pforacle.OracleWorld(omap, rec, flocks, hz, formation, ext)
     try:
         vel, vpref = world.velocity_work(work)
-        patches = world.entity_updates(movestate, arrival, work, vel, vdes, capi.PATCH)
+        patches = world.entity_updates(movestate, arrival, work, vel, vdes, capi.PATCH, target_arrival)
     finally:
         world.close()
-    a2, ms2 = pforacle.entity_apply(rec, movestate, work, patches)
-    return dict(vdes=vdes, los=los, vel=vel, vpref=vpref, patches=patches, agents=a2, movestate=ms2)
+    out = dict(vdes=vdes, los=los, vel=vel, vpref=vpref, patches=patches)
+    if ext is None:
+        out["agents"], out["movestate"] = pforacle.entity_apply(rec, movestate, work, patches)
+    else:
+        out["agents"], out["movestate"], out["ext"] = pforacle.entity_apply(rec, movestate, work, patches, ext)
+    return out
 
 
 def nav_layer(flags, radius):
@@ -339,27 +346,64 @@ def nav_layer(flags, radius):
     return (base + (radius >= 5.0) + (radius >= 10.0) + (radius >= 15.0)).astype(np.int32)
 
 
-def port_tick_layers(omaps, agents, flocks, movestate, work, hz, arrivals, layer_of_unit, pool):
+def port_tick_layers(omaps, agents, flocks, movestate, work, hz, arrivals, layer_of_unit, pool, formation=None, ext=None,
+                     target_arrival=None):
     """port_tick for a population on several navigation layers. The port's world holds one layer, and a unit's layer
     only changes its own tile probes and arrival constants (neighbours are the whole population on every layer), so
     the port runs once per layer in use and every unit's results come from the run of its own layer.
     omaps / arrivals: per layer (OracleMap, route_arrival_consts of every flock target on that layer). pool=None: the
-    desired velocities and LOS bits of the agent records."""
+    desired velocities and LOS bits of the agent records. formation / ext / target_arrival: as port_tick (target_arrival
+    per work item of `work`, each computed on its unit's layer)."""
     work = np.ascontiguousarray(work, np.uint32)
     lw = np.asarray(layer_of_unit)[work]
     out = None
     for L in np.unique(lw):
         sel = np.nonzero(lw == L)[0]
         own = {} if pool is not None else dict(vdes=agents["vdes"][work[sel]], los=agents["has_dest_los"][work[sel]])
-        r = port_tick(omaps[L], agents, flocks, movestate, work[sel], hz, arrivals[L], pool=pool, **own)
+        ta = None if target_arrival is None else [target_arrival[i] for i in sel]
+        r = port_tick(omaps[L], agents, flocks, movestate, work[sel], hz, arrivals[L], pool=pool, formation=formation, ext=ext,
+                      target_arrival=ta, **own)
+        whole = ("agents", "movestate", "ext")
         if out is None:
-            out = {k: v.copy() if k in ("agents", "movestate") else np.zeros((len(work),) + v.shape[1:], v.dtype)
-                   for k, v in r.items()}
+            out = {k: v.copy() if k in whole else np.zeros((len(work),) + v.shape[1:], v.dtype) for k, v in r.items()}
         for k in ("vdes", "los", "vel", "vpref", "patches"):
             out[k][sel] = r[k]
-        for k in ("agents", "movestate"):
-            out[k][work[sel]] = r[k][work[sel]]
+        for k in whole:
+            if k in r:
+                out[k][work[sel]] = r[k][work[sel]]
     return out
+
+
+def pforacle_map(cw, ch, cost, map_xz=(0.0, 0.0)):
+    """the port's map of one layer without blockers"""
+    import pforacle
+    return pforacle.OracleMap(cw, ch, cost, None, None, *map_xz)
+
+
+def target_arrivals(host, rec, ext, work, layer_of_unit=None):
+    """per work item: N_IsMaximallyClose's tiles around the target's position of an ENTER_ENTITY_RANGE item, on the unit's
+    own layer (route_arrival_consts), as pfnav_agents_compute_updates computes them; None for the other items"""
+    lou = np.zeros(len(rec), np.int32) if layer_of_unit is None else np.asarray(layer_of_unit, np.int32)
+    tarr = [None] * len(work)
+    for i, u in enumerate(work):
+        t = ext["surround_target_uid"][u]
+        if rec["state"][u] == 6 and t != capi.NULL_UID:
+            tarr[i] = host.route_arrival_consts(rec["pos"][t], int(lou[u]))
+    return tarr
+
+
+def states_port_tick(host, omaps, rec, fl, ms, form, ext, work, hz, layer_of_unit=None):
+    """One tick of every movement state in the port, with the arrival constants the device computes: arrived()'s per
+    (flock, layer) and, for each ENTER_ENTITY_RANGE item with a target, N_IsMaximallyClose's tiles around the target's
+    position on the unit's own layer (pfnav_agents_compute_updates). host: a host-only Nav holding the same map;
+    omaps: {layer: OracleMap}; rec / fl / ms / form / ext: AGENT (vdes and has_dest_los set for the work items) / FLOCK
+    / MOVESTATE / FORMATION_IN / MOVESTATE_EXT records of the whole population. -> port_tick_layers' dict"""
+    work = np.ascontiguousarray(work, np.uint32)
+    lou = np.zeros(len(rec), np.int32) if layer_of_unit is None else np.asarray(layer_of_unit, np.int32)
+    arrivals = {int(L): [host.route_arrival_consts(t, int(L)) for t in fl["target"]] for L in np.unique(lou[work])}
+    tarr = target_arrivals(host, rec, ext, work, lou)
+    return port_tick_layers({int(L): omaps[int(L)] for L in arrivals}, rec, fl, ms, work, hz, arrivals, lou, None,
+                            formation=form, ext=ext, target_arrival=tarr)
 
 
 VEL_RTOL = 1e-4

@@ -19,6 +19,13 @@ ST_MOVING, ST_FORMATION, ST_ARRIVED, ST_SEEK, ST_WAITING, ST_SURROUND, ST_ENTER,
 def _scenario(seed, hz):
     """1 500 agents of cases.update_case with the movement states spread over them and all the inputs those states read"""
     p, cost, a, ms = cases.update_case(seed, hz)
+    form, ext = _spread_states(a, ms, seed)
+    return p, cost, a, ms, form, ext
+
+
+def _spread_states(a, ms, seed):
+    """spread the movement states over the MOVING units of `a` (in place: state, flock_of) -> the formation inputs and
+    the movestate beyond point seeking those states read (FORMATION_IN, MOVESTATE_EXT)"""
     n = len(a["radius"])
     rng = np.random.default_rng(seed + 7)
     st = a["state"].copy()
@@ -70,7 +77,23 @@ def _scenario(seed, hz):
     ext["target_dir"][close] = ext["rot"][close]            # already facing the target direction -> ARRIVED
     ext["wait_prev"] = ST_MOVING
     ext["wait_ticks_left"] = rng.integers(1, 5, n)
-    return p, cost, a, ms, form, ext
+    return form, ext
+
+
+def _work_inputs(a, form, seed=99):
+    """the work list of a one-tick all-states case (every state but ARRIVED: the WAITING countdown runs in
+    entity_compute_update, movement.c:2630) and its desired velocities and LOS bits -> (work, vdes, los)"""
+    rng = np.random.default_rng(seed)
+    work = np.nonzero(a["state"] != ST_ARRIVED)[0].astype(np.uint32)
+    vdes = rng.normal(size=(len(work), 2)).astype(np.float32)
+    vdes /= np.linalg.norm(vdes, axis=1, keepdims=True)
+    vdes[rng.random(len(work)) < 0.08] = 0
+    cell = a["state"][work] == ST_CELL
+    vdes[cell] = form["cell_arrival_vdes"][work][cell]       # ent_desired_velocity (movement.c:1507)
+    vdes[a["state"][work] == ST_TURNING] = 0
+    los = (rng.random(len(work)) < 0.25).astype(np.uint8)
+    los[a["flock_of"][work] < 0] = 0
+    return work, vdes, los
 
 
 def _ref_setup(ref, a, ms, form, ext, hz, work, vdes, los):
@@ -98,17 +121,7 @@ def test_all_movement_states_vs_reference(nav, pfref_or_golden, hz):
     p, cost, a, ms, form, ext = _scenario(5151, hz)
     n = len(a["radius"])
     cw = 3
-    rng = np.random.default_rng(99)
-    # WAITING entities are in the work list too (their countdown runs in entity_compute_update, movement.c:2630)
-    work = np.nonzero(a["state"] != ST_ARRIVED)[0].astype(np.uint32)
-    vdes = rng.normal(size=(len(work), 2)).astype(np.float32)
-    vdes /= np.linalg.norm(vdes, axis=1, keepdims=True)
-    vdes[rng.random(len(work)) < 0.08] = 0
-    cell = a["state"][work] == ST_CELL
-    vdes[cell] = form["cell_arrival_vdes"][work][cell]       # ent_desired_velocity (movement.c:1507)
-    vdes[a["state"][work] == ST_TURNING] = 0
-    los = (rng.random(len(work)) < 0.25).astype(np.uint8)
-    los[a["flock_of"][work] < 0] = 0
+    work, vdes, los = _work_inputs(a, form)
     ref = pfref_or_golden.RefMap(cw, cw, p) if pfref_or_golden else None
     E = cases.Expected("movement_states_hz%d" % hz, ref)
     ref_out = {}

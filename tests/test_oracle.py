@@ -403,6 +403,113 @@ def test_port_tick_golden(pforacle, name):
     assert (t["agents"]["state"][work][garr] == a["state"][work][garr]).all()
 
 
+# ---- every movement state: the steering variants and the state machine beyond point seeking -------------------------
+UNPINNED = ("the port's states beyond point seeking (formation, cell arrival, enemy seek, entity range, turning, the "
+            "waiting countdown, surround) follow the CUDA kernels' structure and stay UNPINNED to the reference: ")
+
+
+def _states_case(hz):
+    """test_gpu_states' all-states scenario and its work inputs, and the port's tick on them"""
+    import test_gpu_states as S
+    p, cost, a, ms, form, ext = S._scenario(5151, hz)
+    work, vdes, los = S._work_inputs(a, form)
+    aa = dict(a)
+    n = len(a["radius"])
+    aa["vdes"] = np.zeros((n, 2), np.float32); aa["vdes"][work] = vdes
+    aa["has_los"] = np.zeros(n, np.uint32); aa["has_los"][work] = los
+    rec, fl = capi.pack_agents(aa)
+    host = capi.Nav(hostonly=True)
+    host.map_create(3, 3, 1); host.map_upload_layer(0, cost); host.map_build_nav(0); host.route_build(0)
+    try:
+        t = cases.states_port_tick(host, {0: cases.pforacle_map(3, 3, cost)}, rec, fl, ms, form, ext, work, hz)
+    finally:
+        host.close()
+    return dict(cost=cost, a=a, ms=ms, form=form, ext=ext, work=work, vdes=vdes, los=los, rec=rec, fl=fl, port=t)
+
+
+def _port_patches_from(c, vel, hz):
+    """the port's entity_compute_update on given velocities (the reference's), with the scenario's arrival constants"""
+    import pforacle
+    host = capi.Nav(hostonly=True)
+    host.map_create(3, 3, 1); host.map_upload_layer(0, c["cost"]); host.map_build_nav(0); host.route_build(0)
+    try:
+        arrival = [host.route_arrival_consts(t) for t in c["fl"]["target"]]
+        tarr = cases.target_arrivals(host, c["rec"], c["ext"], c["work"])
+    finally:
+        host.close()
+    rec = c["rec"].copy(); rec["vdes"][c["work"]] = c["vdes"]; rec["has_dest_los"][c["work"]] = c["los"]
+    w = pforacle.OracleWorld(cases.pforacle_map(3, 3, c["cost"]), rec, c["fl"], hz, c["form"], c["ext"])
+    try:
+        return w.entity_updates(c["ms"], arrival, c["work"], vel, c["vdes"], capi.PATCH, tarr)
+    finally:
+        w.close()
+
+
+def _check_port_states(c, hz, evel, oi, of, ox):
+    """the port against reference values of the all-states scenario: velocities within 1e-4; from the reference's
+    velocities, flags / states / blocking / wait ticks identical and the patch floats within 1e-4 of max(|x|, 1)"""
+    assert cases.vel_ok(c["port"]["vel"], evel, c["a"]["pos"][c["work"]])[0]
+    p = _port_patches_from(c, evel, hz)
+    assert (p["flags"] == oi[:, 0].astype(np.uint32)).all() and (p["next_state"] == oi[:, 1]).all()
+    assert (p["next_block"] == oi[:, 2]).all() and (p["wait_ticks_left"] == oi[:, 3]).all()
+    got = cases.patch_floats(p)
+    assert (np.abs(got - of[:, :25]) <= 1e-4 * np.maximum(np.abs(of[:, :25]), 1.0)).all()
+    gx = np.concatenate([p["next_dest"], p["next_target_prev"], p["next_target_dir"], p["next_attack"][:, None].astype(np.float32)], axis=1)
+    assert np.abs(gx - ox).max() <= 1e-5
+
+
+@pytest.mark.parametrize("hz", [20, 10])
+def test_port_all_states_vs_ref(pforacle, hz):
+    """the port's every-state tick on test_gpu_states' scenario against the compiled reference"""
+    import pfref
+    if not pfref.available():
+        pytest.skip(UNPINNED + "oracle/_ref/libpfref.so is not built")
+    import test_gpu_states as S
+    c = _states_case(hz)
+    p, cost, a, ms, form, ext = S._scenario(5151, hz)
+    ref = pfref.RefMap(3, 3, p)
+    try:
+        S._ref_setup(ref, a, ms, form, ext, hz, c["work"], c["vdes"], c["los"])
+        evel, _ = ref.velocity_work(os.cpu_count())
+        oi, of, ox = ref.compute_updates_ext(evel)
+    finally:
+        ref.close()
+    _check_port_states(c, hz, evel, oi, of, ox)
+
+
+@pytest.mark.parametrize("hz", [20, 10])
+def test_port_all_states_golden(pforacle, hz):
+    """the port's every-state tick against movement_states_hz*.npz where those hold reference values (recorded with the
+    compiled reference, PFNAV_RECORD_GOLDEN without _SELF); a file recorded from the CUDA path pins nothing"""
+    g = gold("movement_states_hz%d" % hz)
+    if str(g["source"]) != "reference":
+        pytest.skip(UNPINNED + "movement_states_hz%d.npz was recorded from the CUDA path, not from the reference" % hz)
+    c = _states_case(hz)
+    _check_port_states(c, hz, g["vel"], g["patch_i"], g["patch_f"], g["patch_x"])
+
+
+@pytest.mark.parametrize("hz", [20, 10, 5, 1])
+def test_port_all_states_cover_the_state_machine(pforacle, hz):
+    """the port's every-state tick on test_gpu_states' scenario reaches every state and every kind of transition that
+    tests/test_gpu_states_port.py compares the device with, at every tick rate"""
+    c = _states_case(hz)
+    stw = c["a"]["state"][c["work"]]
+    for s_ in (0, 1, 3, 4, 5, 6, 7, 8):
+        assert (stw == s_).sum() > 10, s_
+    p = c["port"]["patches"]
+    assert {-1, 0, 1, 2, 4, 7, 8} <= set(p["next_state"].tolist())
+    for bit in (10, 11, 12, 13, 14):
+        assert (p["flags"] & (1 << bit)).any(), bit
+    # WAITING counts down by one (not garrisoned or stuck units, which return before the state switch); on 0 the unit
+    # returns to wait_prev (SET_MOVING) and the apply leaves it there
+    wt = stw == 4
+    before = c["ext"]["wait_ticks_left"][c["work"]]
+    assert np.isin(p["wait_ticks_left"][wt] - before[wt], (-1, 0)).all() and (p["wait_ticks_left"][wt] == before[wt] - 1).mean() > 0.9
+    back = wt & (p["wait_ticks_left"] == 0)
+    assert back.any() and ((p["flags"][back] & (1 << 12)) != 0).all()
+    assert (c["port"]["agents"]["state"][c["work"]][back] == c["ext"]["wait_prev"][c["work"]][back]).all()
+
+
 def test_port_desired_velocity_golden(pforacle):
     g = gold("agents_3x3")
     a = _agents_from_gold(g)
