@@ -93,6 +93,59 @@ def test_chunk_window_kernel_source_on_cpu_threads(emu, pforacle):
         assert (got == g["zexp"][k]).all(), k
 
 
+@pytest.mark.parametrize("cw,ch,map_xz,seed", [(2, 5, (601.3, -250.9), 0x5EED0C10), (1, 1, (0.0, 0.0), 0x5EED0C11)],
+                         ids=["2x5_offset", "1x1"])
+def test_chunk_window_kernel_source_vs_port(emu, pforacle, cw, ch, map_xz, seed):
+    """the padded-chunk mode on generated inputs: a non-square 2 x 5 map at an offset that is not tile-aligned (windows
+    of 128, the last row's and column's running past the map) and a 1 x 1 map (a window of 64), with committed
+    blockers. Zone seeds from the port, entity / enemies seeds from the host code; every chunk's field from the kernel
+    source on CPU threads == OracleMap.flow_field_zone / chunk_field_seeded"""
+    rng = np.random.default_rng(seed)
+    H, W = ch * 64, cw * 64
+    cost = synth.cost_from_pathable(synth.make_map(cw, ch, seed, rivers=cw > 1 and ch > 1), cw, ch)
+    nav = capi.Nav(hostonly=True)
+    try:
+        nav.map_create(cw, ch, 1, *map_xz); nav.map_upload_layer(0, cost); nav.map_build_nav(0)
+        for _ in range(30 * cw * ch):
+            nav.blockers_incref(map_xz[0] - rng.uniform(0, W * 4), map_xz[1] + rng.uniform(0, H * 4), rng.uniform(2, 12), 0)
+        nav.map_commit()
+        blk = nav.blockers(0)
+        om = pforacle.OracleMap(cw, ch, cost, blk, None, map_x=map_xz[0], map_z=map_xz[1])
+        chunks = [divmod(c, cw) for c in range(cw * ch)]
+        open_ = np.argwhere(synth.blocked_to_image(cost, cw, ch) != 0xFF)
+        zones = [(tuple(int(v) for v in open_[i]), r) for i, r in zip(rng.integers(0, len(open_), 6), (0, 2, 13, 40, 73, 90))]
+        zones += [((0, 0), 20), ((H - 1, W - 1), 50), ((H - 1, 0), 90)]
+        fp = capi.Nav.footprints(np.stack([map_xz[0] - rng.uniform(0, W * 4, 40), map_xz[1] + rng.uniform(0, H * 4, 40)], 1),
+                                 rng.choice(np.array([0.0, 6.0, 20.0, 40.0, 60.0], np.float32), 40))
+        ents = [(capi.TARGET_ENEMIES, fp, L) for L in (0, 3)] + [(capi.TARGET_ENTITY, fp[i:i + 1], 1) for i in range(0, 40, 8)]
+        jobs, sds = [], []
+        for c in chunks:
+            for centre, r in zones:
+                jobs.append((c, om.flow_field_zone(c, centre, r)))
+                sds.append(om.zone_seeds(c, centre, r))
+            for kind, f, L in ents:
+                s = nav.entity_seeds(kind, f, c, L)
+                jobs.append((c, om.chunk_field_seeded(c, s)))
+                sds.append(s)
+    finally:
+        nav.close()
+    rec = np.zeros(len(jobs), capi.REGION_REQ)
+    for i, ((cr, cc), _) in enumerate(jobs):
+        rec["center_r"][i], rec["center_c"][i] = cr, cc
+        rec["seed_off"][i], rec["seed_n"][i] = sum(len(x) for x in sds[:i]), len(sds[i])
+        rec["flags"][i] = capi.REGION_CREATE
+    dim = 128 if cw > 1 and ch > 1 else 64
+    got = _run(emu, _image(cost, cw, ch), _image(blk, cw, ch), np.zeros((H, W), np.uint16), dim, rec,
+               np.concatenate(sds).astype(np.int32).reshape(-1, 2), np.zeros((0, 2), np.int32),
+               np.zeros((len(jobs), 64, 64), np.uint8), 1)
+    bad = [(i, jobs[i][0]) for i in range(len(jobs)) if (got[i] != jobs[i][1]).any()]
+    assert not bad, bad[:8]
+    # the fields reach the last chunk row and column, and some seed sets are empty (windows without the zone centre)
+    nonempty = [jobs[i][0] for i in range(len(jobs)) if jobs[i][1].any()]
+    assert any(c[0] == ch - 1 for c in nonempty) and any(c[1] == cw - 1 for c in nonempty)
+    assert any(len(s) == 0 for s in sds) and sum(len(s) > 0 for s in sds) > len(sds) // 4
+
+
 @pytest.mark.parametrize("seed,dim,n", [(92, 64, 40), (93, 128, 16), (94, 96, 60)])
 def test_region_kernel_source_vs_port(emu, pforacle, seed, dim, n):
     """further window sizes (incl. PFNAV_REGION_DIM_MAX) and a 4 x 4-chunk map: kernel source on CPU threads vs the port"""
