@@ -775,6 +775,9 @@ typedef struct pfnav_formation_in {
 /* HOST array, one record per entity of this context's own range (uid order). Optional: without it every entity is
  * outside any formation (fid == NULL_FID). */
 int  pfnav_agents_upload_formation(pfnav_ctx *ctx, const pfnav_formation_in *f, size_t n);
+/* Inspection: read the own range's formation table back (at most maxout records; waits for the device).
+ * PFNAV_ERR_ARG when no table exists. */
+int  pfnav_agents_read_formation(pfnav_ctx *ctx, pfnav_formation_in *out, size_t maxout);
 
 /* The rest of struct movestate (movement.c:146-215) that the states beyond point seeking read. 64 bytes. */
 #define PFNAV_NULL_UID 0xffffffffu
@@ -1149,6 +1152,62 @@ int  pfnav_group_change_population(pfnav_group *g, const uint32_t *remove_uids, 
                                    const pfnav_agent *add, const pfnav_movestate *add_ms, const pfnav_movestate_ext *add_ext,
                                    const pfnav_formation_in *add_formation, const pfnav_blocking *add_blocking, size_t nadd,
                                    const pfnav_flock *flocks, size_t nflocks);
+/* Inputs beyond point seeking as deltas: the fields of pfnav_movestate_ext and the pfnav_formation_in records that the
+ * engine decides, written for a subset of the population without reading or uploading the whole tables. The library
+ * writes fields; which field an engine action sets stays the engine's decision (a turn order: TARGET_DIR, with the
+ * TURNING state through pfnav_agents_commands; Entity_SetRot: ROT; a new surround or enter-range order: TARGET_PREV and
+ * SURROUND_FIELD, with its target through PFNAV_DELTA_TARGET; a flock entering, moving in or leaving a formation:
+ * FORMATION). surround_target_uid and target_range are PFNAV_DELTA_TARGET's; wait_prev and wait_ticks_left are decided
+ * by the device. 128 bytes. */
+#define PFNAV_INPUT_TARGET_PREV    (1u << 0)  /* movestate_ext.target_prev_pos                      */
+#define PFNAV_INPUT_TARGET_DIR     (1u << 1)  /* movestate_ext.target_dir (STATE_TURNING)            */
+#define PFNAV_INPUT_ROT            (1u << 2)  /* movestate_ext.rot (Entity_SetRot)                   */
+#define PFNAV_INPUT_SURROUND_FIELD (1u << 3)  /* movestate_ext.using_surround_field, 0 or 1          */
+#define PFNAV_INPUT_FORMATION      (1u << 4)  /* the whole pfnav_formation_in record                 */
+typedef struct pfnav_input_delta {
+    uint32_t uid, mask;
+    float    target_prev_pos[2];
+    float    target_dir[4];
+    float    rot[4];
+    uint32_t using_surround_field;
+    uint32_t _pad[3];
+    pfnav_formation_in formation;             /* offset 64 */
+} pfnav_input_delta;                          /* 128 bytes */
+/* Write n input deltas (HOST array) into the device-resident movestate_ext and formation tables.
+ * - Order: records apply in array order; several records for one uid compose as if applied one after the other (per
+ *   field, the last writer wins).
+ * - Everything is validated before anything changes: uid in the context's own range, no unknown mask bit, every float
+ *   the mask selects finite, using_surround_field 0 or 1, formation flags within the five PFNAV_FORM_* bits, the four
+ *   movestate_ext bits only with an uploaded movestate_ext table. Failure: PFNAV_ERR_ARG, device and host state
+ *   untouched. n == 0 does nothing.
+ * - Formation table: when none exists, PFNAV_INPUT_FORMATION first creates one exactly as pfnav_agents_upload_formation
+ *   of all-zero records would, then writes. A present table is not the same as no table (the velocity pass of
+ *   ARRIVING_TO_CELL and MOVING_IN_FORMATION reads it), so a batch that creates it changes what the tick does for every
+ *   entity in those states.
+ * - Equivalence: afterwards both tables equal what reading them back (pfnav_agents_read_movestate_ext /
+ *   pfnav_agents_read_formation), applying the records in order on the host and uploading them whole would leave.
+ * - The call writes those two tables and nothing else: it leaves the spatial index, the arrival constants, the blocker
+ *   ops and the work list as they are.
+ * - Asynchronous on `stream`: the records go through the request staging and are read before the call returns, so the
+ *   array can be reused at once. It waits for the device only when a table is created or the staging buffer grows.
+ * - PFNAV_ERR_NO_DEVICE on a host-only context. PFNAV_ERR_STATE (nothing changed) on a context in a multi-GPU job, as
+ *   for pfnav_agents_commands: a job takes pfnav_mgpu_input_deltas / pfnav_group_input_deltas. */
+int  pfnav_agents_input_deltas(pfnav_ctx *ctx, const pfnav_input_delta *d, size_t n, void *stream);
+/* pfnav_agents_input_deltas for a whole multi-GPU job. Every rank calls the NCCL form with the same arguments, the job's
+ * whole batch (uids global, in [0, n_total)); the group form is called once. Record format and rules are the solo call's.
+ * - Each member writes the records of the uids it owns. A batch with PFNAV_INPUT_FORMATION creates the formation table on
+ *   every member that has none, so the members' sets of tables stay equal.
+ * - All or nothing across the job: each member validates the whole batch (the solo checks with [0, n_total) as the
+ *   range), then the members exchange one verdict record {status, n_agents, n_flocks, tables present}: NCCL all-gathers
+ *   it on `stream` and reads it (the exchange of pfnav_mgpu_commands), a group reads its members' host state. If any
+ *   member refuses, every member returns that member's error and the text names it; members whose population size or
+ *   set of tables (movestate_ext, formation) differ return PFNAV_ERR_ARG. Nothing changes anywhere.
+ * - Streams: the NCCL form runs on `stream` and waits for the verdict read, the group form on each member's context
+ *   stream. n == 0 does nothing and exchanges nothing.
+ * - Errors: PFNAV_ERR_NO_DEVICE on a host-only context; PFNAV_ERR_STATE (nothing changed) on a context in no job and
+ *   for the NCCL form on a group member. */
+int  pfnav_mgpu_input_deltas(pfnav_ctx *ctx, const pfnav_input_delta *d, size_t n, void *stream);
+int  pfnav_group_input_deltas(pfnav_group *g, const pfnav_input_delta *d, size_t n);
 /* pfnav_agents_set_work(ctx, NULL, 0) from the state resident on the device: the uids of the context's own range whose
  * state is neither ARRIVED nor WAITING, ascending, compacted on the device on `stream`. It waits for the stream once, to
  * read the 4-byte count that sizes the per-work-item buffers; it waits for the whole device only when the list outgrows

@@ -74,6 +74,11 @@ assert AGENT_DELTA.itemsize == 64
 (DELTA_STATE, DELTA_FLOCK, DELTA_AUX_DEST, DELTA_FLAGS, DELTA_SPEEDS, DELTA_RADIUS, DELTA_VELOCITY, DELTA_POSITION,
  DELTA_CLEAR_HIST, DELTA_TARGET) = (1 << i for i in range(10))
 TODO_SURROUND_QUERY, TODO_USE_SURROUND_FIELD, TODO_DROP_SURROUND_FIELD = 1, 2, 4
+INPUT_DELTA = np.dtype([
+    ("uid", "<u4"), ("mask", "<u4"), ("target_prev_pos", "<f4", 2), ("target_dir", "<f4", 4), ("rot", "<f4", 4),
+    ("using_surround_field", "<u4"), ("_pad", "<u4", 3), ("formation", FORMATION_IN)])
+assert INPUT_DELTA.itemsize == 128 and INPUT_DELTA.fields["formation"][1] == 64
+INPUT_TARGET_PREV, INPUT_TARGET_DIR, INPUT_ROT, INPUT_SURROUND_FIELD, INPUT_FORMATION = (1 << i for i in range(5))
 
 REGION_REQ = np.dtype([
     ("layer", "<i4"), ("center_r", "<i4"), ("center_c", "<i4"), ("start_r", "<i4"), ("start_c", "<i4"),
@@ -142,6 +147,7 @@ SYMBOLS = [
     "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
     "pfnav_mgpu_change_population", "pfnav_group_change_population", "pfnav_ents_in_circles",
     "pfnav_agents_collect_events", "pfnav_agents_read_events",
+    "pfnav_agents_input_deltas", "pfnav_mgpu_input_deltas", "pfnav_group_input_deltas", "pfnav_agents_read_formation",
 ]
 
 _lib = None
@@ -221,6 +227,10 @@ def load():
     L.pfnav_agents_change_population.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_agents_read_movestate_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_agents_read_formation.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_agents_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_mgpu_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_group_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_mgpu_change_population.argtypes = L.pfnav_agents_change_population.argtypes
     L.pfnav_group_change_population.argtypes = L.pfnav_agents_change_population.argtypes[:-1]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
@@ -354,6 +364,12 @@ def _command_args(deltas, flocks):
     fl = None if flocks is None else np.ascontiguousarray(flocks, FLOCK).reshape(-1)
     fp = None if fl is None else _p(fl if len(fl) else np.zeros(1, FLOCK))     # an empty table is still a table
     return _p(d) if len(d) else None, len(d), fp, 0 if fl is None else len(fl)
+
+
+def _input_args(deltas):
+    """(d, n) of the input-delta calls, and the array the pointer keeps alive"""
+    d = np.ascontiguousarray(deltas, INPUT_DELTA).reshape(-1)
+    return (_p(d) if len(d) else None, len(d)), d
 
 
 def _resident_args(reqs, footprints, ent_uids, seekers):
@@ -1154,6 +1170,23 @@ class Nav:
         _chk(self.L.pfnav_agents_read_movestate_ext(self.h, _p(out) if n else None, n))
         return out
 
+    def agents_read_formation(self, n):
+        out = np.zeros(n, FORMATION_IN)
+        _chk(self.L.pfnav_agents_read_formation(self.h, _p(out) if n else None, n))
+        return out
+
+    def agents_input_deltas(self, deltas, stream=0):
+        """pfnav_agents_input_deltas: INPUT_DELTA records written in order into the movestate_ext and formation
+        tables (a FORMATION record creates a zeroed formation table when there is none)"""
+        args, keep = _input_args(deltas)
+        _chk(self.L.pfnav_agents_input_deltas(self.h, *args, C.c_void_p(stream)))
+
+    def mgpu_input_deltas(self, deltas, stream=0):
+        """collective: agents_input_deltas for the whole job -- every rank passes the job's whole batch (global uids);
+        all or nothing across the ranks"""
+        args, keep = _input_args(deltas)
+        _chk(self.L.pfnav_mgpu_input_deltas(self.h, *args, C.c_void_p(stream)))
+
     def agents_set_work_dev(self, stream=0):
         """pfnav_agents_set_work_dev: agents_set_work(None) built on the device -> the number of work items"""
         n = C.c_size_t(0)
@@ -1309,6 +1342,12 @@ class Group:
         """agents_commands for the whole group: the job's whole batch (global uids), each member applying its own
         entities' deltas; all or nothing across the members. Follow with gather."""
         _chk(load().pfnav_group_commands(self.g, *_command_args(deltas, flocks)))
+
+    def input_deltas(self, deltas):
+        """agents_input_deltas for the whole group: the job's whole batch (global uids), each member writing its own
+        entities' records; all or nothing across the members"""
+        args, keep = _input_args(deltas)
+        _chk(load().pfnav_group_input_deltas(self.g, *args))
 
     def change_population(self, remove, add, ms=None, ext=None, formation=None, blocking=None, flocks=None):
         """agents_change_population for the whole group: the job's whole batch (global uids); member i then owns

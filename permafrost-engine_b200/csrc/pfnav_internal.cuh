@@ -14,6 +14,7 @@
 #include "../../include/pfnav.h"
 #include "pfnav_pool_host.h"
 #include "pfnav_commands_host.h"
+#include "pfnav_inputs_host.h"
 #include "pfnav_waves_host.h"
 #include "pfnav_resident_host.h"
 
@@ -555,6 +556,22 @@ struct pf_cmd_job {
 int pf_cmd_job_check(pfnav_ctx *ctx, const pfnav_agent_delta *deltas, size_t n, const pfnav_flock *flocks, size_t nflocks,
                      pf_cmd_job &J);
 int pf_cmd_job_apply(pfnav_ctx *ctx, const pf_cmd_job &J, cudaStream_t st);
+
+// ---- pfnav_inputs.cu: a job member's part of an input batch (pfnav_mgpu.cu runs the verdict exchange) ----
+// pf_input_job_check validates the whole batch against the population and keeps the folded records of the member's own
+// range, changing nothing (the error is set); pf_input_job_apply writes them on `st`, creating the formation table first
+// when the batch carries PFNAV_INPUT_FORMATION and the member has none. pf_input_tables: the tables a batch may write,
+// as the verdict's bits (1 movestate_ext, 2 formation).
+struct pf_input_job {
+    std::vector<pfnav_input_delta> own;
+    bool any_form = false;
+};
+int pf_input_job_check(pfnav_ctx *ctx, const pfnav_input_delta *d, size_t n, pf_input_job &J);
+int pf_input_job_apply(pfnav_ctx *ctx, const pf_input_job &J, cudaStream_t st);
+static inline uint32_t pf_input_tables(const pfnav_ctx *ctx)
+{
+    return (ctx->d_ms_ext != nullptr ? 1u : 0u) | (ctx->d_formation != nullptr ? 2u : 0u);
+}
 
 // ---- pfnav_commands.cu: a job member's part of a population change (pfnav_mgpu.cu runs the verdict exchange and moves
 // the segments between the stages) ----

@@ -842,6 +842,73 @@ extern "C" int pfnav_group_commands(pfnav_group *g, const pfnav_agent_delta *del
 }
 
 // ------------------------------------------------------------------------------------------
+// Input deltas of a job (pfnav_inputs.cu: pf_input_job_*). Every member gets the job's whole batch, checks all of it and
+// describes itself in one record {status, n_agents, n_flocks, tables present}, exchanged as for a command batch; then each
+// member writes the records of its own uids, and creates the formation table when the batch needs one.
+// ------------------------------------------------------------------------------------------
+extern "C" int pfnav_mgpu_input_deltas(pfnav_ctx *ctx, const pfnav_input_delta *d, size_t n, void *stream)
+{
+    pf_mgpu *m = nullptr;
+    if (int rc = nccl_rank(ctx, __func__, "pfnav_group_input_deltas", &m)) return rc;
+    if (n == 0) return PFNAV_OK;                            // the same arguments on every rank: none of them exchanges
+    PF_CUDA(cudaSetDevice(ctx->device));
+    cudaStream_t st = pf_stream(ctx, stream);
+    pf_input_job J;
+    int local = check_shard(ctx, m);
+    if (!local) local = pf_input_job_check(ctx, d, n, J);
+    const std::string local_err = local ? pfnav_last_error() : "";
+    const int world = m->world, rank = m->rank;
+    if (int rc = m->d_xcnt.reserve((size_t)world * PF_XCNT)) return rc;
+    uint32_t *mine = m->d_xcnt + (size_t)rank * PF_XCNT;
+    const uint32_t verdict[PF_XCNT] = {(uint32_t)local, (uint32_t)ctx->n_agents, (uint32_t)ctx->n_flocks, pf_input_tables(ctx),
+                                       0, 0, 0, 0};
+    PF_CUDA(cudaMemcpyAsync(mine, verdict, sizeof(verdict), cudaMemcpyHostToDevice, st));
+    PF_NCCL(g_nccl.AllGather(mine, m->d_xcnt, PF_XCNT * sizeof(uint32_t), /*ncclInt8*/ 0, m->comm, st));
+    std::vector<uint32_t> all((size_t)world * PF_XCNT);
+    PF_CUDA(cudaMemcpyAsync(all.data(), m->d_xcnt, all.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    for (int r = 0; r < world; r++) {
+        const uint32_t *x = &all[(size_t)r * PF_XCNT];
+        if (!x[0]) continue;
+        if (r == rank) pfnav_set_error("%s: rank %d refused the batch (%s); no rank changed anything", __func__, r, local_err.c_str());
+        else pfnav_set_error("%s: rank %d refused the batch (error %d); no rank changed anything", __func__, r, (int)x[0]);
+        return (int)x[0];
+    }
+    for (int r = 0; r < world; r++)
+        PF_ARG(all[(size_t)r * PF_XCNT + 1] == all[1] && all[(size_t)r * PF_XCNT + 3] == all[3],
+               "ranks hold populations or sets of tables that differ; no rank changed anything");
+    return pf_input_job_apply(ctx, J, st);
+}
+
+// In-process group: the members' verdicts are their host state; each member then writes on its context stream.
+extern "C" int pfnav_group_input_deltas(pfnav_group *g, const pfnav_input_delta *d, size_t n)
+{
+    PF_ARG(g, "group");
+    if (n == 0) return PFNAV_OK;
+    const int world = (int)g->ctxs.size();
+    std::vector<pf_input_job> J(world);
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        int rc = check_shard(c, (pf_mgpu *)c->mgpu);
+        if (!rc) rc = pf_input_job_check(c, d, n, J[i]);
+        if (rc) {
+            const std::string e = pfnav_last_error();
+            pfnav_set_error("%s: member %d refused the batch (%s); no member changed anything", __func__, i, e.c_str());
+            return rc;
+        }
+    }
+    for (int i = 0; i < world; i++)
+        PF_ARG(g->ctxs[i]->n_agents == g->ctxs[0]->n_agents && pf_input_tables(g->ctxs[i]) == pf_input_tables(g->ctxs[0]),
+               "members hold populations or sets of tables that differ; no member changed anything");
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        if (int rc = pf_input_job_apply(c, J[i], c->tick_stream)) return rc;
+    }
+    return PFNAV_OK;
+}
+
+// ------------------------------------------------------------------------------------------
 // Population change of a job (pfnav_commands.cu: pf_pop_job_*). Every member gets the job's whole batch, checks it and its
 // own entities' flock indices, and describes itself in one record {status, n_agents, n_flocks, tables present}; every
 // member reads every record before anything changes. Then each member releases its removed entities' blocks, compacts its
