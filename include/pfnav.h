@@ -886,8 +886,8 @@ typedef struct pfnav_map_query_result {  /* 16 bytes */
  * - MAXIMALLY_CLOSE: ok = some tile centre n_closest_island_tiles (nav.c:1226) lists for the destination -- the
  *   closest tiles of its global island without blockers, at most 256 -- lies within `tolerance` of (x, z). It does not
  *   include the N_IsAdjacentToImpassable test that arrived() (movement.c:2170) adds; combine the two kinds for that.
- * - The searches run on the device over a window around the start tile; a search that leaves it is finished on the
- *   host in the same call. Results are identical either way.
+ * - The searches run on the device: over a window around the start tile, then over the whole layer for a search that
+ *   leaves it. Results are identical either way.
  * - Everything is validated before anything runs: null pointers (n > 0), kind, layer, a finite tolerance and
  *   pfnav_route_build(layer) (the global islands) for MAXIMALLY_CLOSE, faction_id in 0..15 for DEST_ID. Failure:
  *   PFNAV_ERR_ARG, out untouched. n == 0 is valid. Host-only context: PFNAV_ERR_NO_DEVICE. */
@@ -904,8 +904,25 @@ int  pfnav_agents_upload_movestate(pfnav_ctx *ctx, const pfnav_movestate *ms, si
  * tick's new velocities and desired velocities. Needs pfnav_route_build for every layer the agents
  * use (global islands feed arrived(), movement.c:2170). Every movement state is accepted: MOVING / MOVING_IN_FORMATION
  * (formation inputs), SEEK_ENEMIES, ENTER_ENTITY_RANGE, TURNING, WAITING, ARRIVING_TO_CELL are decided on the device;
- * SURROUND_ENTITY with a live target is flagged PFNAV_TODO_SURROUND_QUERY (see there). */
+ * SURROUND_ENTITY with a live target is flagged PFNAV_TODO_SURROUND_QUERY (see there).
+ * The map searches of arrived() run on the device, per used (flock, layer) pair. Without a movestate_ext table the call
+ * is asynchronous on `stream` and waits for the device only when one of its buffers has to grow, or, when the arrival
+ * constants are rebuilt, for the upload of the rebuild two rebuilds back (the request staging's pinned ring). With a
+ * movestate_ext table it still reads back the ENTER_ENTITY_RANGE items and searches their targets' tiles on the host.
+ * pfnav_route_build is checked on the host for every used (flock, layer) pair before anything is queued. */
 int  pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream);
+/* Inspection / test entry: the (flock, layer) table of arrived()'s constants that the last pfnav_agents_compute_updates
+ * built, one record per (flock, layer) pair some entity of the flock uses, in (flock, layer) order. Blocks until the
+ * device is idle. out: up to maxout records; *out_n (may be NULL): the number of pairs. PFNAV_ERR_ARG when the table is
+ * not current (not built yet, or the flocks, their layers or the committed map changed since). */
+typedef struct pfnav_arrival_record {
+    int32_t flock, layer;
+    int32_t nearest_ok;                  /* N_ClosestPathable (nav.c:4126) from the flock target found a tile         */
+    float   nearest[2];                  /* its (x, z): the target itself when its tile is free                       */
+    int32_t mc_n;                        /* n_closest_island_tiles (nav.c:1226): the tile centres N_IsMaximallyClose   */
+    float   mc[256][2];                  /* compares with, in the reference's order                                   */
+} pfnav_arrival_record;
+int  pfnav_agents_read_arrival_consts(pfnav_ctx *ctx, pfnav_arrival_record *out, size_t maxout, size_t *out_n);
 /* Work-item order. Blocks until the update pass has finished. */
 int  pfnav_agents_read_patches(pfnav_ctx *ctx, pfnav_patch *out, size_t maxout);
 /* Device-side entity_apply_update for the movestate fields (movement.c:2693-2757: state, velocity +

@@ -101,6 +101,9 @@ MAP_QUERY = np.dtype([("kind", "<i4"), ("layer", "<i4"), ("x", "<f4"), ("z", "<f
 assert MAP_QUERY.itemsize == 32
 MAP_QUERY_RESULT = np.dtype([("ok", "<i4"), ("dest_id", "<u4"), ("x", "<f4"), ("z", "<f4")])
 assert MAP_QUERY_RESULT.itemsize == 16
+ARRIVAL_RECORD = np.dtype([("flock", "<i4"), ("layer", "<i4"), ("nearest_ok", "<i4"), ("nearest", "<f4", 2), ("mc_n", "<i4"),
+                           ("mc", "<f4", (256, 2))])
+assert ARRIVAL_RECORD.itemsize == 2072
 ENTS_QUERY = np.dtype([("x", "<f4"), ("z", "<f4"), ("range", "<f4"), ("uid", "<u4"), ("maxout", "<i4"), ("_pad", "<u4")])
 assert ENTS_QUERY.itemsize == 24
 EVENT = np.dtype([("uid", "<u4"), ("flags", "<u4"), ("todo", "<u4"), ("attack", "<i4"), ("state_before", "<u4"),
@@ -144,7 +147,7 @@ SYMBOLS = [
     "pfnav_pool_request_paths_resident", "pfnav_map_query_resident", "pfnav_group_arrival_velocity_resident",
     "pfnav_agents_commands", "pfnav_agents_set_work_dev", "pfnav_agents_read_work",
     "pfnav_mgpu_commands", "pfnav_group_commands",
-    "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext",
+    "pfnav_agents_change_population", "pfnav_agents_read_movestate_ext", "pfnav_agents_read_arrival_consts",
     "pfnav_mgpu_change_population", "pfnav_group_change_population", "pfnav_ents_in_circles",
     "pfnav_agents_collect_events", "pfnav_agents_read_events",
     "pfnav_agents_input_deltas", "pfnav_mgpu_input_deltas", "pfnav_group_input_deltas", "pfnav_agents_read_formation",
@@ -227,6 +230,7 @@ def load():
     L.pfnav_agents_change_population.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_agents_read_movestate_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_agents_read_arrival_consts.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.pfnav_agents_read_formation.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_agents_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_mgpu_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
@@ -1168,6 +1172,16 @@ class Nav:
     def agents_read_movestate_ext(self, n):
         out = np.zeros(n, MOVESTATE_EXT)
         _chk(self.L.pfnav_agents_read_movestate_ext(self.h, _p(out) if n else None, n))
+        return out
+
+    def agents_read_arrival_consts(self):
+        """pfnav_agents_read_arrival_consts: the (flock, layer) table of arrived()'s constants the last compute_updates
+        built, as ARRIVAL_RECORD records in (flock, layer) order"""
+        n = C.c_size_t(0)
+        _chk(self.L.pfnav_agents_read_arrival_consts(self.h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, ARRIVAL_RECORD)
+        if n.value:
+            _chk(self.L.pfnav_agents_read_arrival_consts(self.h, _p(out), n.value, C.byref(n)))
         return out
 
     def agents_read_formation(self, n):

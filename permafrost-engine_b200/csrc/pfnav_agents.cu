@@ -1401,7 +1401,6 @@ extern "C" int pfnav_ents_in_circles(pfnav_ctx *ctx, const pfnav_ents_query *q, 
 // The quaternion helpers keep the reference's mix of float and double arithmetic (pf_math.c).
 // ------------------------------------------------------------------------------------------
 struct quat { float x, y, z, w; };
-struct pf_arrival_dev { int32_t nearest_ok; float nearest[2]; int32_t mc_n; int32_t mc_off; int32_t _pad[3]; };
 
 #define PF_PI_D 3.14159265358979323846
 
@@ -2044,31 +2043,74 @@ __global__ void k_collect_enter_range(const pfnav_agent *__restrict__ agents, co
     out[k] = {(uint32_t)wi, nav_layer_for(a.flags, a.radius), tr.px, tr.pz};
 }
 
+// The (flock, layer) table k_entity_update reads, rebuilt on the device when the used pairs, the flocks or the committed
+// map changed: the host packs the used pairs through the request staging, and the searches run on `st` with no host wait
+// (only a growing buffer waits, under the pf_dbuf rule).
 static int refresh_arrival_consts(pfnav_ctx *ctx, cudaStream_t st)
 {
     if (ctx->arrival_valid && ctx->arrival_epoch == ctx->map_epoch) return 0;
     const size_t nf = ctx->n_flocks, nl = (size_t)ctx->nlayers;
-    std::vector<pf_arrival_dev> dev(nf * nl);
-    std::vector<float2> tiles;
-    pf_arrival_consts c;
+    std::vector<pf_arrival_pair> pairs;
     for (size_t f = 0; f < nf; f++)
         for (size_t l = 0; l < nl; l++) {
-            pf_arrival_dev &d = dev[f * nl + l];
-            memset(&d, 0, sizeof(d));
             if (!ctx->flock_layer_used[f * PFNAV_NAV_LAYER_MAX + l]) continue;
-            int rc = pfnav_arrival_consts(ctx, (int)l, ctx->h_flocks[f].target[0], ctx->h_flocks[f].target[1], &c);
-            if (rc) return rc;
-            d.nearest_ok = c.nearest_ok; d.nearest[0] = c.nearest[0]; d.nearest[1] = c.nearest[1];
-            d.mc_n = c.mc_n; d.mc_off = (int32_t)tiles.size();
-            for (int i = 0; i < c.mc_n; i++) tiles.push_back(make_float2(c.mc[i][0], c.mc[i][1]));
+            if (!pfnav_route_dev_islands(ctx, (int)l)) {
+                pfnav_set_error("pfnav_agents_compute_updates: pfnav_route_build(layer %d) is needed (global islands, nav.c:1731)", (int)l);
+                return PFNAV_ERR_ARG;
+            }
+            pairs.push_back({(int32_t)f, (int32_t)l, ctx->h_flocks[f].target[0], ctx->h_flocks[f].target[1]});
         }
-    const size_t b0 = dev.size() * sizeof(pf_arrival_dev), b1 = std::max<size_t>(tiles.size(), 1) * sizeof(float2);
-    if (int rc = ctx->d_arrival.reserve(b0 + b1)) return rc;
-    PF_CUDA(cudaStreamSynchronize(st));
-    if (b0) PF_CUDA(cudaMemcpy(ctx->d_arrival, dev.data(), b0, cudaMemcpyHostToDevice));
-    if (!tiles.empty()) PF_CUDA(cudaMemcpy(ctx->d_arrival + b0, tiles.data(), tiles.size() * sizeof(float2), cudaMemcpyHostToDevice));
+    // from here on the old table is overwritten: it stays invalid until the new one is queued
+    ctx->arrival_valid = false;
+    ctx->arrival_pairs.swap(pairs);
+    const size_t np = ctx->arrival_pairs.size();
+    const size_t b0 = nf * nl * sizeof(pf_arrival_dev), b1 = np * PF_ARRIVAL_MC_MAX * sizeof(float2);
+    if (int rc = ctx->d_arrival.reserve(b0 + b1 + 2 * np + 1)) return rc;
+    if (b0) PF_CUDA(cudaMemsetAsync(ctx->d_arrival, 0, b0, st));
+    if (np) {
+        const size_t bytes = np * sizeof(pf_arrival_pair);
+        pf_stage S;
+        if (int rc = pf_stage_begin(ctx, st, bytes, bytes, false, &S)) return rc;
+        memcpy(S.host, ctx->arrival_pairs.data(), bytes);
+        int rc = pf_stage_upload(ctx, st, S, bytes);
+        if (!rc) rc = pf_arrival_search(ctx, st, (const pf_arrival_pair *)S.dev, (int)np, (pf_arrival_dev *)ctx->d_arrival.p,
+                                        (float2 *)(ctx->d_arrival + b0), ctx->d_arrival + b0 + b1);
+        const int rc_done = pf_stage_done(ctx, st);       // whatever was queued may read S.dev
+        if (rc) return rc;
+        if (rc_done) return rc_done;
+    }
     ctx->arrival_valid = true; ctx->arrival_epoch = ctx->map_epoch;
     return 0;
+}
+
+extern "C" int pfnav_agents_read_arrival_consts(pfnav_ctx *ctx, pfnav_arrival_record *out, size_t maxout, size_t *out_n)
+{
+    PF_ARG(ctx, "ctx");
+    PF_NEED_DEVICE(ctx);
+    PF_ARG(out || maxout == 0, "out == NULL");
+    PF_ARG(ctx->arrival_valid && ctx->arrival_epoch == ctx->map_epoch,
+           "no current arrival constants (pfnav_agents_compute_updates has not run since they or the committed map changed)");
+    PF_CUDA(cudaSetDevice(ctx->device));
+    PF_CUDA(cudaDeviceSynchronize());
+    const std::vector<pf_arrival_pair> &pairs = ctx->arrival_pairs;
+    const size_t np = pairs.size(), n = std::min(maxout, np), nl = (size_t)ctx->nlayers;
+    if (out_n) *out_n = np;
+    if (n == 0) return PFNAV_OK;
+    std::vector<pf_arrival_dev> table(ctx->n_flocks * nl);
+    std::vector<float2> tiles(np * PF_ARRIVAL_MC_MAX);
+    const size_t b0 = table.size() * sizeof(pf_arrival_dev);
+    PF_CUDA(cudaMemcpy(table.data(), ctx->d_arrival, b0, cudaMemcpyDeviceToHost));
+    PF_CUDA(cudaMemcpy(tiles.data(), ctx->d_arrival + b0, tiles.size() * sizeof(float2), cudaMemcpyDeviceToHost));
+    for (size_t s = 0; s < n; s++) {
+        const pf_arrival_dev &d = table[(size_t)pairs[s].flock * nl + pairs[s].layer];
+        pfnav_arrival_record &o = out[s];
+        memset(&o, 0, sizeof(o));
+        o.flock = pairs[s].flock; o.layer = pairs[s].layer;
+        o.nearest_ok = d.nearest_ok; o.nearest[0] = d.nearest[0]; o.nearest[1] = d.nearest[1];
+        o.mc_n = d.mc_n;
+        for (int i = 0; i < d.mc_n; i++) { o.mc[i][0] = tiles[(size_t)d.mc_off + i].x; o.mc[i][1] = tiles[(size_t)d.mc_off + i].y; }
+    }
+    return PFNAV_OK;
 }
 
 extern "C" int pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream)

@@ -97,6 +97,9 @@ static int pf_dbuf_reserve_all(size_t n, B &...bufs)
     return rc;
 }
 
+// one used (flock, layer) pair of the arrival constants and its flock's target
+struct pf_arrival_pair { int32_t flock, layer; float tx, tz; };
+
 // 24-byte neighbour record: exactly what one agent needs to know about another
 // (SURVEY.md 8e). This is also the unit of the per-tick NCCL all-gather.
 struct __align__(8) pf_record {
@@ -149,6 +152,7 @@ struct pfnav_ctx {
     void *route_dev_state = nullptr;                           // pfnav_route.cu: device copies of the routing tables (k_portal_graph_path_warp)
     pf_dbuf<uint16_t> d_gisl;                                  // pfnav_route.cu: global islands, [layer][H64][W64] (pfnav_map_query)
     pf_dbuf<uint8_t> d_mq_buf;                                 // pfnav_query.cu: the inputs and outputs of one query batch
+    pf_dbuf<int32_t> d_layer_scratch;                          // pfnav_map_query's whole-layer tier: mq_layer_cta_words per CTA
     std::set<std::pair<int, int>> dirty, fdirty;               // pfnav_blockers.cu: (layer, chunk) occupancy / faction mask changed
     void *blk_state = nullptr;                                 // pfnav_blockers.cu: queued blocker ops + device-side refcount state
 
@@ -218,6 +222,9 @@ struct pfnav_ctx {
     pf_dbuf<uint8_t> d_arrival;                              // [nflocks][nlayers] pf_arrival_dev + tile lists
     uint64_t arrival_epoch = ~0ull; bool arrival_valid = false;
     std::vector<uint8_t> flock_layer_used;                   // [nflocks][12]
+    std::vector<pf_arrival_pair> arrival_pairs;              // the used pairs of the last build, slot order
+    pf_dbuf<int32_t> d_arrival_scratch;                      // the arrival tiers' own whole-layer scratch: compute_updates
+                                                             // runs on its caller's stream, unordered with pfnav_map_query
     std::vector<pfnav_flock> h_flocks;
     float max_radius = 0.0f;
     bool has_unsupported_state = false;
@@ -305,6 +312,12 @@ struct pf_arrival_consts {
 };
 // which: the searches to run; PF_ARRIVAL_MC needs pfnav_route_build(layer)
 enum { PF_ARRIVAL_NEAREST = 1, PF_ARRIVAL_MC = 2 };
+// The device table of arrived()'s constants: [nflocks][nlayers] records, each used pair's list of mc_n tile centres at
+// mc_off in the float2 array that follows (a 256-entry slot per used pair).
+struct pf_arrival_dev { int32_t nearest_ok; float nearest[2]; int32_t mc_n; int32_t mc_off; int32_t _pad[3]; };
+// pfnav_query.cu: the constants of npairs (flock, layer) pairs into d_arr / d_tiles on `st`; d_flags: 2 bytes per pair
+int pf_arrival_search(pfnav_ctx *ctx, cudaStream_t st, const pf_arrival_pair *d_pairs, int npairs, pf_arrival_dev *d_arr,
+                      float2 *d_tiles, uint8_t *d_flags);
 int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arrival_consts *out,
                          int which = PF_ARRIVAL_NEAREST | PF_ARRIVAL_MC);
 // the device image of the global islands of `layer` ([H64][W64] u16, uploaded by pfnav_route_build), or nullptr when

@@ -10,7 +10,8 @@
 //
 // Kernels (pfnav_query_kernel.cuh): k_map_probe, one thread per query, answers the probe kinds and DEST_ID; k_map_search,
 // one warp per CLOSEST_PATHABLE / MAXIMALLY_CLOSE query, replays the reference's search inside a window of the layer.
-// The searches that would leave the window are finished here with the host routine pfnav_arrival_consts.
+// The searches that would leave the window are finished on the device by k_map_search_layer, one CTA per search over
+// the whole layer.
 // pfnav_map_query_resident takes the positions of resident entities by uid: k_resident_xz (pfnav_region.cu) writes them
 // into the uploaded queries before the same kernels run.
 #include "pfnav_internal.cuh"
@@ -19,13 +20,25 @@
 #include <string.h>
 #include "pfnav_map_view.cuh"
 #include "pfnav_query_kernel.cuh"
+#include "pfnav_layer_search.cuh"
 
 static_assert(sizeof(pfnav_map_query_req) == 32, "pfnav_map_query_req must be 32 bytes");
 static_assert(sizeof(pfnav_map_query_result) == 16, "pfnav_map_query_result must be 16 bytes");
 
+// the searches k_map_search flagged (d_fallback), finished over the whole layer on `st`
+static int pf_map_search_layer(pfnav_ctx *ctx, cudaStream_t st, const MapView &m, const pfnav_map_query_req *d_q, const int32_t *d_idx,
+                        int ns, pfnav_map_query_result *d_out, const uint8_t *d_fallback)
+{
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)ns, (size_t)ctx->sm_count);
+    if (int rc = ctx->d_layer_scratch.reserve(grid * mq_layer_cta_words(ctx->W64, ctx->H64))) return rc;
+    k_map_search_layer<<<grid, MQ_LAYER_THREADS, 0, st>>>(m, ctx->d_gisl, d_q, d_idx, ns, d_out, d_fallback, ctx->d_layer_scratch);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
+}
+
 // pfnav_map_query, and its resident form when P is not NULL: after the queries are uploaded, k_resident_xz writes P's
-// named positions over (x, z) (the first array) and (dst_x, dst_z) (the second) of the device copy, and the searches'
-// substituted records come back with the results for the host finish
+// named positions over (x, z) (the first array) and (dst_x, dst_z) (the second) of the device copy
 static int map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfnav_map_query_result *out, void *stream,
                      const pf_resident_points *P)
 {
@@ -76,45 +89,16 @@ static int map_query(pfnav_ctx *ctx, const pfnav_map_query_req *q, size_t n, pfn
     k_map_probe<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(m, d_q, (int)n, d_out);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
-    std::vector<uint8_t> fallback(ns);
     if (ns) {
         // the global islands of every layer are one image; layers without a route build are never read (validated above)
         const unsigned grid = (unsigned)std::min<size_t>(ns, (size_t)ctx->sm_count * 16);
         k_map_search<<<grid, 32, 0, st>>>(m, ctx->d_gisl, d_q, (const int32_t *)(dev + o_idx), (int)ns, d_out, dev + o_fb);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
-        PF_CUDA(cudaMemcpyAsync(fallback.data(), dev + o_fb, ns, cudaMemcpyDeviceToHost, st));
+        if (int rc = pf_map_search_layer(ctx, st, m, d_q, (const int32_t *)(dev + o_idx), (int)ns, d_out, dev + o_fb)) return rc;
     }
     PF_CUDA(cudaMemcpyAsync(out, d_out, n * sizeof(pfnav_map_query_result), cudaMemcpyDeviceToHost, st));
-    // the resident form: the substituted records from the first search to the last, which the host finish reads
-    std::vector<pfnav_map_query_req> sub;
-    if (named && ns) {
-        sub.resize((size_t)(search.back() - search.front()) + 1);
-        PF_CUDA(cudaMemcpyAsync(sub.data(), d_q + search.front(), sub.size() * sizeof(pfnav_map_query_req),
-                                cudaMemcpyDeviceToHost, st));
-    }
     PF_CUDA(cudaStreamSynchronize(st));
-    // the searches that left the window: the host routine on the host mirrors, which the last commit made equal to the
-    // device images
-    for (size_t k = 0; k < ns; k++) {
-        if (!fallback[k]) continue;
-        const pfnav_map_query_req &a = sub.empty() ? q[search[k]] : sub[search[k] - search.front()];
-        pfnav_map_query_result &r = out[search[k]];
-        pf_arrival_consts c;
-        r = {0, 0u, 0.0f, 0.0f};
-        if (a.kind == PFNAV_QUERY_CLOSEST_PATHABLE) {
-            int rc = pfnav_arrival_consts(ctx, a.layer, a.x, a.z, &c, PF_ARRIVAL_NEAREST);
-            if (rc) return rc;
-            r.ok = c.nearest_ok; r.x = c.nearest[0]; r.z = c.nearest[1];
-        } else {
-            int rc = pfnav_arrival_consts(ctx, a.layer, a.dst_x, a.dst_z, &c, PF_ARRIVAL_MC);
-            if (rc) return rc;
-            for (int i = 0; i < c.mc_n && !r.ok; i++) {
-                const float dx = c.mc[i][0] - a.x, dz = c.mc[i][1] - a.z;
-                r.ok = sqrtf(dx * dx + dz * dz) <= a.tolerance;
-            }
-        }
-    }
     return PFNAV_OK;
 }
 
@@ -130,4 +114,101 @@ extern "C" int pfnav_map_query_resident(pfnav_ctx *ctx, const pfnav_map_query_re
     pf_resident_points P;
     if (int rc = pf_resident_points_begin(ctx, "map queries", n, pos_uids, q != nullptr, dst_uids, q != nullptr, P)) return rc;
     return map_query(ctx, q, n, out, stream, &P);
+}
+
+// ------------------------------------------------------------------------------------------
+// The constants of arrived() (movement.c:2170-2196) per used (flock, layer) pair, built on the device: N_ClosestPathable
+// and the tile list of n_closest_island_tiles from the flock target, exactly as pfnav_arrival_consts computes them on the
+// host. k_arrival_window replays both searches in the 32 x 32 and 128 x 128 windows, one warp per pair, and flags the
+// searches that leave them (flags[2 s] N_ClosestPathable, flags[2 s + 1] the list); k_arrival_layer finishes the flagged
+// ones over the whole layer. Pair s writes arr[flock * nlayers + layer] and its list at tiles[s * 256].
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(32) k_arrival_window(MapView m, const uint16_t *__restrict__ gisl,
+                                                       const pf_arrival_pair *__restrict__ pairs, int npairs, int nlayers,
+                                                       pf_arrival_dev *__restrict__ arr, float2 *__restrict__ tiles,
+                                                       uint8_t *__restrict__ flags)
+{
+    __shared__ mq_shared S;
+    __shared__ pfnav_map_query_result R;
+    __shared__ uint8_t fb;
+    const int lane = threadIdx.x & 31;
+    for (int s = blockIdx.x; s < npairs; s += gridDim.x) {
+        const pf_arrival_pair P = pairs[s];
+        pf_arrival_dev d = {0, {0.0f, 0.0f}, 0, s * MQ_LIST_MAX, {0, 0, 0}};
+        tile_desc td;
+        const bool on_map = desc_for_point(m, P.tx, P.tz, td);
+        pfnav_map_query_req a = {PFNAV_QUERY_CLOSEST_PATHABLE, P.layer, P.tx, P.tz, P.tx, P.tz, 0.0f, 0};
+        mq_search(S, m, gisl, a, &R, &fb, lane);
+        d.nearest_ok = R.ok; d.nearest[0] = R.x; d.nearest[1] = R.z;
+        const uint8_t fb_cp = fb;
+        uint8_t fb_mc = 0;
+        if (on_map) {
+            a.kind = PFNAV_QUERY_MAXIMALLY_CLOSE;
+            mq_search(S, m, gisl, a, &R, &fb, lane);
+            fb_mc = fb;
+            if (!fb_mc) {
+                d.mc_n = S.n;
+                for (int i = lane; i < S.n; i += 32) {
+                    const int t = S.list[i];
+                    tiles[(size_t)s * MQ_LIST_MAX + i] = make_float2(m.map_x - (float)(S.c0 + t % S.dim) * 4.0f,
+                                                                     m.map_z + (float)(S.r0 + t / S.dim) * 4.0f);
+                }
+            }
+        }
+        if (lane == 0) {
+            arr[(size_t)P.flock * nlayers + P.layer] = d;
+            flags[2 * s] = fb_cp; flags[2 * s + 1] = fb_mc;
+        }
+        __syncwarp();
+    }
+}
+
+__global__ void __launch_bounds__(MQ_LAYER_THREADS) k_arrival_layer(MapView m, const uint16_t *__restrict__ gisl,
+                                                                    const pf_arrival_pair *__restrict__ pairs, int npairs,
+                                                                    int nlayers, pf_arrival_dev *__restrict__ arr,
+                                                                    float2 *__restrict__ tiles, const uint8_t *__restrict__ flags,
+                                                                    int32_t *scratch)
+{
+    __shared__ mq_layer_shared L;
+    int32_t *mine = scratch + blockIdx.x * mq_layer_cta_words(m.W64, m.H64);
+    for (int k = blockIdx.x; k < 2 * npairs; k += gridDim.x) {
+        if (!flags[k]) continue;
+        const int s = k >> 1;
+        const bool cp = !(k & 1);
+        const pf_arrival_pair P = pairs[s];
+        tile_desc td;
+        desc_for_point(m, P.tx, P.tz, td);
+        const int tr = td.chunk_r * 64 + td.tile_r, tc = td.chunk_c * 64 + td.tile_c;
+        mq_layer_search(L, mine, m, gisl, P.layer, cp, tr, tc, tiles + (size_t)s * MQ_LIST_MAX, threadIdx.x, blockDim.x);
+        if (threadIdx.x == 0) {
+            pf_arrival_dev &d = arr[(size_t)P.flock * nlayers + P.layer];
+            if (!cp) d.mc_n = L.n;
+            else if (L.tile >= 0) {
+                const int ar = L.tile / m.W64, ac = L.tile % m.W64;
+                d.nearest_ok = 1;
+                d.nearest[0] = (m.map_x - (float)((ac >> 6) * 256)) - (float)((ac & 63) * 4);
+                d.nearest[1] = (m.map_z + (float)((ar >> 6) * 256)) + (float)((ar & 63) * 4);
+            }
+        }
+        __syncthreads();
+    }
+}
+
+int pf_arrival_search(pfnav_ctx *ctx, cudaStream_t st, const pf_arrival_pair *d_pairs, int npairs, pf_arrival_dev *d_arr,
+                      float2 *d_tiles, uint8_t *d_flags)
+{
+    MapView m;
+    m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
+    m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)npairs, (size_t)ctx->sm_count * 16);
+    k_arrival_window<<<grid, 32, 0, st>>>(m, ctx->d_gisl, d_pairs, npairs, ctx->nlayers, d_arr, d_tiles, d_flags);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    const unsigned lgrid = (unsigned)std::min<size_t>(2 * (size_t)npairs, (size_t)ctx->sm_count);
+    if (int rc = ctx->d_arrival_scratch.reserve(lgrid * mq_layer_cta_words(ctx->W64, ctx->H64))) return rc;
+    k_arrival_layer<<<lgrid, MQ_LAYER_THREADS, 0, st>>>(m, ctx->d_gisl, d_pairs, npairs, ctx->nlayers, d_arr, d_tiles, d_flags,
+                                                        ctx->d_arrival_scratch);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
 }
