@@ -30,6 +30,7 @@
 #include <memory>
 #include <string.h>
 #include "pfnav_map_view.cuh"
+#include "pfnav_scan.cuh"
 
 #include "pfnav_clearpath_kernel.cuh"   // v2 helpers, ClearPath: build_vos ... clearpath_retry, clearpath_collect / _finish
 #include "pfnav_ents_query_kernel.cuh"  // GridView, the index walk grid_query / filter_garrisoned, pfnav_ents_in_circles
@@ -402,65 +403,38 @@ __global__ void k_cell_count(const pf_record *__restrict__ rec, int n, GridView 
     atomicAdd(&count[cy * g.grid_w + cx], 1u);
 }
 
-// single-CTA exclusive scan (cells <= 1M)
+// single-CTA exclusive scan (cells <= 1M): a serial run per thread, the runs' sums scanned over the CTA
 __global__ void k_cell_scan(const uint32_t *__restrict__ count, uint32_t *__restrict__ start, int ncells)
 {
-    __shared__ uint32_t part[1024];
+    __shared__ uint32_t warp_tot[32];
     const int tid = threadIdx.x, per = (ncells + 1023) / 1024;
     const int b = tid * per, e = min(b + per, ncells);
     uint32_t s = 0;
     for (int i = b; i < e; i++) s += count[i];
-    part[tid] = s;
-    __syncthreads();
-    for (int off = 1; off < 1024; off <<= 1) {
-        uint32_t v = tid >= off ? part[tid - off] : 0;
-        __syncthreads();
-        part[tid] += v;
-        __syncthreads();
-    }
-    uint32_t run = tid ? part[tid - 1] : 0;
+    uint32_t total;
+    uint32_t run = pf_block_excl_scan(s, warp_tot, total);
     for (int i = b; i < e; i++) { start[i] = run; run += count[i]; }
-    if (tid == 1023) start[ncells] = part[1023];
+    if (tid == 0) start[ncells] = total;
 }
 
 // the same scan for big grids, three launches: 4096 cells per block (4 per thread) -> block sums, their scan, apply
-__device__ __forceinline__ uint32_t block_excl_scan_1024(uint32_t v, uint32_t *warp_tot, uint32_t &total)
-{
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    uint32_t incl = v;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += o; }
-    if (lane == 31) warp_tot[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        uint32_t w = warp_tot[lane], wi = w;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, wi, d); if (lane >= d) wi += o; }
-        warp_tot[lane] = wi - w;                       // exclusive
-        if (lane == 31) warp_tot[32] = wi;             // block total
-    }
-    __syncthreads();
-    total = warp_tot[32];
-    return warp_tot[wid] + incl - v;
-}
-
 __global__ void __launch_bounds__(1024) k_cell_scan_sum(const uint32_t *__restrict__ count, uint32_t *__restrict__ part, int ncells)
 {
-    __shared__ uint32_t wt[33];
+    __shared__ uint32_t wt[32];
     const int i0 = (blockIdx.x * 1024 + threadIdx.x) * 4;
     uint32_t v = 0;
     for (int j = 0; j < 4; j++) if (i0 + j < ncells) v += count[i0 + j];
     uint32_t total;
-    block_excl_scan_1024(v, wt, total);
+    pf_block_excl_scan(v, wt, total);
     if (threadIdx.x == 0) part[blockIdx.x] = total;
 }
 
 __global__ void __launch_bounds__(1024) k_cell_scan_parts(uint32_t *__restrict__ part, int nb, uint32_t *__restrict__ start, int ncells)
 {
-    __shared__ uint32_t wt[33];
+    __shared__ uint32_t wt[32];
     const uint32_t v = (int)threadIdx.x < nb ? part[threadIdx.x] : 0u;
     uint32_t total;
-    const uint32_t ex = block_excl_scan_1024(v, wt, total);
+    const uint32_t ex = pf_block_excl_scan(v, wt, total);
     if ((int)threadIdx.x < nb) part[threadIdx.x] = ex;
     if (threadIdx.x == 0) start[ncells] = total;
 }
@@ -468,12 +442,12 @@ __global__ void __launch_bounds__(1024) k_cell_scan_parts(uint32_t *__restrict__
 __global__ void __launch_bounds__(1024) k_cell_scan_apply(const uint32_t *__restrict__ count, const uint32_t *__restrict__ part,
                                                           uint32_t *__restrict__ start, int ncells)
 {
-    __shared__ uint32_t wt[33];
+    __shared__ uint32_t wt[32];
     const int i0 = (blockIdx.x * 1024 + threadIdx.x) * 4;
     uint32_t c[4], v = 0;
     for (int j = 0; j < 4; j++) { c[j] = i0 + j < ncells ? count[i0 + j] : 0u; v += c[j]; }
     uint32_t total;
-    uint32_t run = part[blockIdx.x] + block_excl_scan_1024(v, wt, total);
+    uint32_t run = part[blockIdx.x] + pf_block_excl_scan(v, wt, total);
     for (int j = 0; j < 4; j++) if (i0 + j < ncells) { start[i0 + j] = run; run += c[j]; }
 }
 
@@ -2500,23 +2474,16 @@ __global__ void __launch_bounds__(REP_COMPACT_THREADS)
 k_rep_compact(const pf_miss *__restrict__ by_wi, const uint32_t *__restrict__ flag, int nwork, pf_miss *__restrict__ out,
               uint32_t *__restrict__ cnt)
 {
-    __shared__ uint32_t part[REP_COMPACT_THREADS];
+    __shared__ uint32_t warp_tot[REP_COMPACT_THREADS / 32];
     const int tid = threadIdx.x, per = (nwork + REP_COMPACT_THREADS - 1) / REP_COMPACT_THREADS;
     const int lo = min(tid * per, nwork), hi = min(lo + per, nwork);
     uint32_t n = 0;
     for (int w = lo; w < hi; w++) n += flag[w];
-    part[tid] = n;
-    __syncthreads();
-    for (int d = 1; d < REP_COMPACT_THREADS; d <<= 1) {     // inclusive scan
-        const uint32_t v = tid >= d ? part[tid - d] : 0;
-        __syncthreads();
-        part[tid] += v;
-        __syncthreads();
-    }
-    uint32_t o = part[tid] - n;
+    uint32_t total;
+    uint32_t o = pf_block_excl_scan(n, warp_tot, total);
     for (int w = lo; w < hi; w++)
         if (flag[w]) out[o++] = by_wi[w];
-    if (tid == REP_COMPACT_THREADS - 1) cnt[1] = part[tid];
+    if (tid == 0) cnt[1] = total;
 }
 
 // the direction byte of the tiles the remaining representatives stand on, at a round boundary

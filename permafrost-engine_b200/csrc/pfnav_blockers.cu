@@ -12,6 +12,7 @@
 //   N_Update + N_ApplyDeferredInvalidations            src/navigation/nav.c:2119-2223
 //   N_FC_InvalidateAllAtChunk / ...ThroughChunk        src/navigation/fieldcache.c:460-472, 481-545
 #include "pfnav_internal.cuh"
+#include "pfnav_scan.cuh"
 #include <algorithm>
 #include <limits.h>
 #include <math.h>
@@ -290,21 +291,6 @@ __global__ void k_blockers_tiles(const tile_op *__restrict__ ops, int nops, appl
     apply_tile(a, o.layer, o.ar, o.ac, o.faction, o.delta);
 }
 
-// exclusive prefix sum over the CTA of a packed pair of counts (low / high 32 bits); *total = the CTA's sum
-__device__ __forceinline__ unsigned long long cta_excl_scan(unsigned long long v, unsigned long long *warp_tot, unsigned long long *total)
-{
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    unsigned long long incl = v;
-    for (int d = 1; d < 32; d <<= 1) { const unsigned long long t = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += t; }
-    __syncthreads();                        // warp_tot may still be read by the previous call
-    if (lane == 31) warp_tot[w] = incl;
-    __syncthreads();
-    unsigned long long before = 0, all = 0;
-    for (int k = 0; k < nw; k++) { const unsigned long long t = warp_tot[k]; if (k < w) before += t; all += t; }
-    *total = all;
-    return before + incl - v;
-}
-
 // offsets of the producer blocks behind the ops already pending; advances the pending counts
 __global__ void __launch_bounds__(1024) k_ops_offsets(const unsigned long long *__restrict__ bsum, int nb, uint32_t *cnt,
                                                       unsigned long long *__restrict__ boff)
@@ -316,7 +302,7 @@ __global__ void __launch_bounds__(1024) k_ops_offsets(const unsigned long long *
         const int b = b0 + threadIdx.x;
         const unsigned long long v = b < nb ? bsum[b] : 0ull;
         unsigned long long tot;
-        const unsigned long long ex = cta_excl_scan(v, warp_tot, &tot);
+        const unsigned long long ex = pf_block_excl_scan(v, warp_tot, tot);
         if (b < nb) boff[b] = base + carry + ex;
         carry += tot;
     }
@@ -333,9 +319,10 @@ __global__ void __launch_bounds__(PF_OPS_BLOCK) k_ops_compact(const pfnav_blocke
     const unsigned d = i < n ? desc[i] : 0u, nops = d & 3u;
     unsigned nwide = 0;
     for (unsigned k = 0; k < nops; k++) nwide += (d >> (2 + k)) & 1u;
+    // one u64 scan ranks both lists: narrow counts in the low 32 bits, wide in the high (a count never reaches 2^32)
     unsigned long long tot;
     const unsigned long long off = boff[blockIdx.x] +
-        cta_excl_scan((unsigned long long)(nops - nwide) | (unsigned long long)nwide << 32, warp_tot, &tot);
+        pf_block_excl_scan((unsigned long long)(nops - nwide) | (unsigned long long)nwide << 32, warp_tot, tot);
     uint32_t on = (uint32_t)off, ow = (uint32_t)(off >> 32);
     for (unsigned k = 0; k < nops; k++) {
         if ((d >> (2 + k)) & 1u) wide[ow++] = ops[2 * (size_t)i + k];
@@ -406,12 +393,8 @@ __global__ void __launch_bounds__(256) k_chunks_finish(finish_args a)
         // island ids count the roots (= the first tile of each island in scan order) from 1
         int cnt = 0;
         for (int j = 0; j < 16; j++) cnt += (int)(L[tid * 16 + j] == tid * 16 + j);
-        int incl = cnt;
-        for (int d = 1; d < 32; d <<= 1) { const int v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((tid & 31) >= d) incl += v; }
-        if ((tid & 31) == 31) warp_tot[tid >> 5] = incl;
-        __syncthreads();
-        int before = incl - cnt;
-        for (int wv = 0; wv < (tid >> 5); wv++) before += warp_tot[wv];
+        int nroots;
+        int before = pf_block_excl_scan(cnt, warp_tot, nroots);
         for (int j = 0; j < 16; j++) if (L[tid * 16 + j] == tid * 16 + j) ids[tid * 16 + j] = (uint16_t)(++before);
         __syncthreads();
         for (int i = tid; i < 4096; i += 256) {

@@ -3,18 +3,21 @@
 // pfnav_agents_commands applies per-entity deltas (pfnav_commands_host.h validates and merges them, one record per uid)
 // with one thread per entity, replaces the flock table, and rebuilds the flock member lists from the flock id column
 // with a stable counting sort: every warp owns a contiguous uid range, counts its entities per flock, the counts are
-// scanned per flock across the warps and over the flocks, and every warp writes its entities behind the offsets of its
-// range. Members are therefore ascending by uid within a flock, as the host pass of an upload leaves them.
+// scanned (pf_block_excl_scan, pfnav_scan.cuh) per flock across the warps and over the flocks, and every warp writes
+// its entities behind the offsets of its range. Members are therefore ascending by uid within a flock, as the host pass
+// of an upload leaves them.
 // A member of a multi-GPU job takes the job's whole batch (pf_cmd_job_check / pf_cmd_job_apply, for pfnav_mgpu.cu): the
 // deltas of its own uids as above, and for the others the flock id, radius and flag bits (k_apply_foreign), so that it
 // rebuilds the member lists and population facts from its own complete columns.
-// pfnav_agents_set_work_dev compacts the uids that are not still into the work list, in uid order.
+// pfnav_agents_set_work_dev compacts the uids that are not still into the work list, in uid order, with the ordered
+// compaction of pfnav_scan.cuh: count and scan, one host read of the count to size the list, then the write.
 // pfnav_agents_change_population removes and appends entities (pfnav_commands_host.h plans the batch and holds the
 // numbering rule): k_pop_gather writes every new row of every table with one thread per row, then the member lists,
 // population facts and spatial index are rebuilt for the new population. Its job form (pf_pop_job_*, for pfnav_mgpu.cu)
 // compacts each member's own survivors with k_pop_gather over a row window and the replicated record and flock columns
 // with k_pop_columns; the segments of survivors that cross a member boundary move between the stages.
 #include "pfnav_internal.cuh"
+#include "pfnav_scan.cuh"
 #include <algorithm>
 
 #define FULL 0xFFFFFFFFu
@@ -65,26 +68,6 @@ __global__ void k_flock_hist(const int32_t *__restrict__ flock_of, int n, int pe
     }
 }
 
-// exclusive scan over the 1024 threads of a block; wsum: 32 words of shared memory; total: the block's sum
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *wsum, uint32_t &total)
-{
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    uint32_t x = v;
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[wid] = x;
-    __syncthreads();
-    if (wid == 0) {
-        uint32_t s = wsum[lane];
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, s, o); if (lane >= o) s += y; }
-        wsum[lane] = s;
-    }
-    __syncthreads();
-    const uint32_t before = wid ? wsum[wid - 1] : 0;
-    total = wsum[31];
-    __syncthreads();
-    return before + x - v;
-}
-
 // block f: the counts of flock f become each warp's offset within the flock; the flock's size goes to start[f + 1]
 __global__ void __launch_bounds__(1024) k_flock_scan(uint32_t *hist, int W, uint32_t *__restrict__ start)
 {
@@ -95,7 +78,7 @@ __global__ void __launch_bounds__(1024) k_flock_scan(uint32_t *hist, int W, uint
         const int w = base + threadIdx.x;
         const uint32_t v = w < W ? row[w] : 0;
         uint32_t total;
-        const uint32_t e = block_excl_scan(v, wsum, total);
+        const uint32_t e = pf_block_excl_scan(v, wsum, total);
         if (w < W) row[w] = carry + e;
         carry += total;
     }
@@ -111,7 +94,7 @@ __global__ void __launch_bounds__(1024) k_flock_starts(uint32_t *__restrict__ st
         const int f = base + threadIdx.x;
         const uint32_t v = f < nflocks ? start[f + 1] : 0;
         uint32_t total;
-        const uint32_t e = block_excl_scan(v, wsum, total);
+        const uint32_t e = pf_block_excl_scan(v, wsum, total);
         if (f < nflocks) start[f + 1] = carry + e + v;
         carry += total;
     }
@@ -138,62 +121,18 @@ __global__ void k_flock_scatter(const int32_t *__restrict__ flock_of, int n, int
 }
 
 // ---- work list: the own range's uids that are not still (ent_still, movement.c:652), ascending ----
-// Block b owns uids [lo + b * per, lo + (b + 1) * per), per a multiple of 1024.
-// The state is read from the 24-byte neighbour records (state << 24 | flags), which every writer of agent.state keeps
-// current (k_make_records, k_entity_apply, k_apply_deltas): a seventh of the agent table's stride.
-__device__ __forceinline__ bool not_still(const pf_record *__restrict__ rec, int i)
-{
-    const uint32_t s = rec[i].state_flags >> 24;
-    return s != PFNAV_STATE_ARRIVED && s != PFNAV_STATE_WAITING;
-}
-
-__global__ void __launch_bounds__(1024) k_work_count(const pf_record *__restrict__ rec, int lo, int hi, int per,
-                                                     uint32_t *__restrict__ part)
-{
-    __shared__ uint32_t wsum[32];
-    const int b0 = lo + blockIdx.x * per, b1 = min(b0 + per, hi);
-    uint32_t c = 0;
-    for (int i = b0 + threadIdx.x; i < b1; i += 1024) c += not_still(rec, i) ? 1u : 0u;
-    uint32_t total;
-    block_excl_scan(c, wsum, total);
-    if (threadIdx.x == 0) part[blockIdx.x] = total;
-}
-
-// one block: part[0 .. nb) (nb <= 1024) become offsets, part[nb] the number of work items
-__global__ void __launch_bounds__(1024) k_work_scan(uint32_t *__restrict__ part, int nb)
-{
-    __shared__ uint32_t wsum[32];
-    const uint32_t v = (int)threadIdx.x < nb ? part[threadIdx.x] : 0;
-    uint32_t total;
-    const uint32_t e = block_excl_scan(v, wsum, total);
-    if ((int)threadIdx.x < nb) part[threadIdx.x] = e;
-    if (threadIdx.x == 0) part[nb] = total;
-}
-
-__global__ void __launch_bounds__(1024) k_work_compact(const pf_record *__restrict__ rec, int lo, int hi, int per,
-                                                       const uint32_t *__restrict__ part, uint32_t *__restrict__ work)
-{
-    __shared__ uint32_t wsum[32];
-    const int b0 = lo + blockIdx.x * per, b1 = min(b0 + per, hi);
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    uint32_t out = part[blockIdx.x];
-    for (int base = b0; base < b1; base += 1024) {
-        const int i = base + threadIdx.x;
-        const bool keep = i < b1 && not_still(rec, i);
-        const unsigned bal = __ballot_sync(FULL, keep);
-        if (lane == 0) wsum[wid] = __popc(bal);
-        __syncthreads();
-        if (wid == 0) {
-            uint32_t s = wsum[lane];
-            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(FULL, s, o); if (lane >= o) s += y; }
-            wsum[lane] = s;
-        }
-        __syncthreads();
-        if (keep) work[out + (wid ? wsum[wid - 1] : 0) + __popc(bal & ((1u << lane) - 1))] = (uint32_t)i;
-        out += wsum[31];
-        __syncthreads();
+// The ordered compaction of pfnav_scan.cuh over the uids [lo, hi). The state is read from the 24-byte neighbour records
+// (state << 24 | flags), which every writer of agent.state keeps current (k_make_records, k_entity_apply,
+// k_apply_deltas): a seventh of the agent table's stride.
+struct work_compact {
+    const pf_record *rec; uint32_t *work;
+    __device__ bool keep(int i) const
+    {
+        const uint32_t s = rec[i].state_flags >> 24;
+        return s != PFNAV_STATE_ARRIVED && s != PFNAV_STATE_WAITING;
     }
-}
+    __device__ void emit(int i, uint32_t slot) const { work[slot] = (uint32_t)i; }
+};
 
 // ---- population change: new rows [row0, n_new) of every table, by the numbering rule of pf_pop_source ----
 // Rows below n_keep are survivors, gathered from the tables as they were (surround targets renumbered); rows from n_keep
@@ -839,21 +778,24 @@ extern "C" int pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *o
     const int lo = (int)ctx->shard_lo, hi = (int)ctx->shard_hi, cnt = hi - lo;
     int rc;
     uint32_t nwork = 0;
-    const int nb = std::min(1024, (cnt + 1023) / 1024);
-    const int per = nb ? ((cnt + nb - 1) / nb + 1023) / 1024 * 1024 : 0;
+    const pf_compact_grid g = pf_compact_grid_of(cnt);
+    // d_cmd_buf: the block offsets, the count, then one ballot word per 32 uids
     if (cnt) {
-        if ((rc = ctx->d_cmd_buf.reserve(((size_t)nb + 1) * 4))) return rc;
+        if ((rc = ctx->d_cmd_buf.reserve(((size_t)g.nb + 1 + ((size_t)cnt + 31) / 32) * 4))) return rc;
         uint32_t *part = (uint32_t *)ctx->d_cmd_buf.p;
-        k_work_count<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, part);
-        k_work_scan<<<1, 1024, 0, st>>>(part, nb);
+        k_compact_count<<<g.nb, PF_COMPACT_THREADS, 0, st>>>(work_compact{ctx->d_records, nullptr}, lo, hi, g.per,
+                                                             part + g.nb + 1, part);
+        k_compact_offsets<work_compact><<<1, PF_COMPACT_THREADS, 0, st>>>(part, g.nb, part + g.nb);
         ctx->launches += 2;
         PF_CUDA(cudaGetLastError());
-        PF_CUDA(cudaMemcpyAsync(&nwork, part + nb, 4, cudaMemcpyDeviceToHost, st));
+        PF_CUDA(cudaMemcpyAsync(&nwork, part + g.nb, 4, cudaMemcpyDeviceToHost, st));
         PF_CUDA(cudaStreamSynchronize(st));
     }
     if ((rc = pf_work_reserve(ctx, nwork))) return rc;
     if (nwork) {
-        k_work_compact<<<nb, 1024, 0, st>>>(ctx->d_records, lo, hi, per, (const uint32_t *)ctx->d_cmd_buf.p, ctx->d_work);
+        const uint32_t *part = (const uint32_t *)ctx->d_cmd_buf.p;
+        k_compact_write<<<g.nb, PF_COMPACT_THREADS, 0, st>>>(work_compact{ctx->d_records, ctx->d_work}, lo, hi, g.per,
+                                                             part + g.nb + 1, part);
         ctx->launches++;
         PF_CUDA(cudaGetLastError());
     }

@@ -4,8 +4,8 @@
 // test suite. The CUDA keywords, intrinsics and warp collectives the header uses are defined as plain C++; every
 // collective is a barrier of the warp's 32 threads. The index is built here as k_cell_* builds it (cells in row-major
 // order, descending uid inside a cell) and the answer lengths are scanned serially; the device scans them with the
-// k_cell_scan kernels. This is not a product path: nothing in libpfnav.so links or calls it, and it is built only by
-// tests/test_ents_query_emu.py.
+// index's exclusive scan (k_cell_scan or the k_cell_scan_* launches, both on pf_block_excl_scan). This is not a
+// product path: nothing in libpfnav.so links or calls it, and it is built only by tests/test_ents_query_emu.py.
 #include <math.h>
 #include <atomic>
 #include <sched.h>
