@@ -1235,6 +1235,58 @@ int  pfnav_agents_set_work_dev(pfnav_ctx *ctx, void *stream, size_t *out_nwork);
  * *out_n: the list's length; at most maxout uids are written (out may be NULL when maxout is 0). */
 int  pfnav_agents_read_work(pfnav_ctx *ctx, uint32_t *out, size_t maxout, size_t *out_n);
 
+/* Checkpoint / resume (G_Move_SaveState / G_Move_LoadState, SURVEY 5): the device-resident population as checkpoint
+ * segments, and back. The format (csrc/pfnav_checkpoint_host.h): a 64-byte header (magic, format version, record sizes,
+ * n_total, the segment's uid range [lo, hi), hz, nflocks, which of the movestate, movestate_ext, formation and blocking
+ * tables exist), the whole flock table, then for each uid in [lo, hi), in uid order, its pfnav_agent, pfnav_movestate
+ * and, where the tables exist, pfnav_movestate_ext, pfnav_formation_in and pfnav_blocking records. The field pool, its LRU
+ * state and the map are not saved: the engine rebuilds the map and re-requests the fields after a restore.
+ *
+ * Save point: after the commit that follows the apply, the commands and the population change of a tick
+ * (pfnav_agents_apply_updates[_ex] -> commands / pfnav_agents_set_blocking / population change -> exchange ->
+ * pfnav_map_commit). There no device-decided blocker op is pending and the records are those the last apply left.
+ * pfnav_agents_save writes one segment for the context's own range [shard_lo, shard_hi): on a single context the whole
+ * population, in a multi-GPU job each member's range, and the members' segments together describe the population.
+ * - out == NULL or cap < the segment's size: PFNAV_ERR_NOMEM with *out_size set, nothing written (as pfnav_ents_in_circles).
+ * - The per-entity tables are packed on the device on `stream` into one staging buffer and copied to out in one copy; the
+ *   call returns when out is filled.
+ * - PFNAV_ERR_STATE (nothing written) when the last update pass is not applied, or when device blocker ops are not
+ *   committed (in a job that shares blockers: not exchanged and committed). PFNAV_ERR_NO_DEVICE on a host-only context;
+ *   PFNAV_ERR_ARG when no population was uploaded. */
+int  pfnav_agents_save(pfnav_ctx *ctx, void *out, size_t cap, size_t *out_size, void *stream);
+/* Restore from the nseg segments segs[i] (sizes[i] bytes each, host memory, any order) of one save, on a context whose map
+ * is built (pfnav_map_build_nav, pfnav_route_build for every layer an entity of a flock stands on) and whose building
+ * blockers the engine has already queued: a fresh map, whose blocker counts hold only those buildings. The restore does not
+ * release the blocks of a population already on the context (blocking rows, or device ops not yet committed), so a load in
+ * the middle of a session rebuilds the map first. A context outside any job takes the whole population; a member of a job
+ * (pfnav_mgpu_init / pfnav_group_create) takes pfnav_mgpu_shard_range(n_total, rank, world) of its own job, whatever the
+ * number of members that saved: segments of 3 members restore onto 1, 2 or 8.
+ * - Everything is validated before anything changes: magic, version and record sizes; each segment's size; segments that
+ *   overlap, leave a gap in [0, n_total) or disagree on n_total, hz, the flock table or the tables they hold; every record
+ *   with the checks of the uploads and pfnav_agents_change_population and no others (flock index below the table's
+ *   length, navigation layer created, finite floats, movestate_ext targets below n_total, blocking 0 / 1, faction_id
+ *   0..15), so whatever the uploads accepted and pfnav_agents_save wrote restores.
+ *   Failure: PFNAV_ERR_ARG. A layer without pfnav_route_build, or blocking records on a job member whose job does not
+ *   share blockers: PFNAV_ERR_STATE. Either way nothing changes.
+ * - Afterwards every table, the flock table, the member lists and the host facts are what pfnav_agents_upload_shard
+ *   (flags 0) and pfnav_agents_upload_movestate / _movestate_ext / _formation / _blocking of the same records leave; a
+ *   table the segments do not hold is dropped. The arrival constants are invalidated, the work list is empty and the
+ *   event list is no longer readable.
+ * - Beyond those uploads: for every restored record with blocking = 1, in uid order, the incref of its recorded circle
+ *   (stop_x, stop_z, stop_radius, faction_id, on the layers of the entity's flags) is queued on the device on `stream`
+ *   as a device-decided op; the next pfnav_map_commit applies it (in a job after pfnav_*_exchange_blocker_ops).
+ * - Then, as after an upload: pfnav_map_commit, in a job pfnav_mgpu_gather / pfnav_group_gather, then
+ *   pfnav_agents_set_work_dev, and the fields re-requested into the pool.
+ * - The call waits for the device: the records go through the blocking copies of the uploads.
+ * pfnav_group_restore: the same for every member of a group, in one call. The segments are validated once, then every
+ * member's state; a refusal of either changes no member. The guarantee covers validation: a CUDA or allocation failure
+ * while member i uploads (PFNAV_ERR_CUDA / PFNAV_ERR_NOMEM) leaves members 0 .. i-1 restored and the others as they were.
+ * NCCL jobs: every rank calls pfnav_agents_restore with the same segments; no collective is involved. The verdict depends
+ * on the segments and on the rank's map (layers created, pfnav_route_build of the layers in use), so every rank must
+ * build the same layers for the ranks to agree. */
+int  pfnav_agents_restore(pfnav_ctx *ctx, const void *const *segs, const size_t *sizes, size_t nseg, void *stream);
+int  pfnav_group_restore(pfnav_group *g, const void *const *segs, const size_t *sizes, size_t nseg);
+
 /* N_FlowFieldUpdate with TARGET_ENEMIES / TARGET_ENTITY straight into the pool (what N_RequestAsyncEnemySeekField /
  * N_RequestAsyncSurroundField + N_AwaitAsyncFields leave in the field cache, nav.c:3769-3960): the fields of the listed
  * chunks become the flow fields of pool destination `dest`; entities name it through pfnav_agent::aux_dest1. The

@@ -151,6 +151,7 @@ SYMBOLS = [
     "pfnav_mgpu_change_population", "pfnav_group_change_population", "pfnav_ents_in_circles",
     "pfnav_agents_collect_events", "pfnav_agents_read_events",
     "pfnav_agents_input_deltas", "pfnav_mgpu_input_deltas", "pfnav_group_input_deltas", "pfnav_agents_read_formation",
+    "pfnav_agents_save", "pfnav_agents_restore", "pfnav_group_restore",
 ]
 
 _lib = None
@@ -236,6 +237,9 @@ def load():
     L.pfnav_mgpu_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_group_input_deltas.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_mgpu_change_population.argtypes = L.pfnav_agents_change_population.argtypes
+    L.pfnav_agents_save.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]
+    L.pfnav_agents_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_group_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_group_change_population.argtypes = L.pfnav_agents_change_population.argtypes[:-1]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -1215,6 +1219,24 @@ class Nav:
         _chk(self.L.pfnav_agents_read_work(self.h, _p(out) if n.value else None, n.value, C.byref(n)))
         return out
 
+    def agents_save(self, stream=0):
+        """pfnav_agents_save: the checkpoint segment of this context's own range -> bytes (the size is asked first)"""
+        size = C.c_size_t(0)
+        rc = self.L.pfnav_agents_save(self.h, None, 0, C.byref(size), C.c_void_p(stream))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        out = np.zeros(size.value, np.uint8)
+        _chk(self.L.pfnav_agents_save(self.h, _p(out), size.value, C.byref(size), C.c_void_p(stream)))
+        return out.tobytes()
+
+    def agents_restore(self, segments, stream=0):
+        """pfnav_agents_restore from checkpoint segments (bytes-like, any order): this context takes the whole population,
+        or its own shard range in a multi-GPU job. Follow with map_commit (the restored blocks), the gather in a job, and
+        agents_set_work_dev."""
+        args, keep = _segment_args(segments)
+        _chk(self.L.pfnav_agents_restore(self.h, *args, C.c_void_p(stream)))
+        self.nwork = 0
+
     def agents_read_state(self, n, movestate=True):
         a = np.zeros(n, AGENT)
         ms = np.zeros(n, MOVESTATE) if movestate else None
@@ -1371,10 +1393,26 @@ class Group:
         for nv in self.navs:
             nv.nwork = 0
 
+    def restore(self, segments):
+        """agents_restore for every member in one call: each takes mgpu_shard_range(n_total, i, world) from the segments.
+        Every member validates before any changes. Follow with map_commit, gather and agents_set_work_dev."""
+        args, keep = _segment_args(segments)
+        _chk(load().pfnav_group_restore(self.g, *args))
+        for nv in self.navs:
+            nv.nwork = 0
+
     def close(self):
         if self.g:
             load().pfnav_group_destroy(self.g)
             self.g = None
+
+
+def _segment_args(segments):
+    """checkpoint segments -> ((const void *const *segs, const size_t *sizes, nseg), the buffers they point into)"""
+    bufs = [np.frombuffer(bytes(sg), np.uint8) for sg in segments]
+    ptrs = (C.c_void_p * max(len(bufs), 1))(*[b.ctypes.data for b in bufs])
+    sizes = (C.c_size_t * max(len(bufs), 1))(*[len(b) for b in bufs])
+    return (ptrs, sizes, len(bufs)), bufs
 
 
 def pack_agents(a):

@@ -1822,6 +1822,22 @@ __global__ void k_entity_apply(pfnav_agent *__restrict__ agents, pfnav_movestate
     rec[uid] = r;
 }
 
+// the block's narrow | wide << 32 op count of a producer of pf_blocker_ops_append, written by thread 0 to s.bsum
+__device__ __forceinline__ void ops_block_sum(unsigned desc, unsigned nops, const pf_op_stage &s)
+{
+    __shared__ unsigned long long part[PF_OPS_BLOCK / 32];
+    const unsigned nwide = ((desc >> 2) & 1u) + ((desc >> 3) & 1u);
+    unsigned long long v = (unsigned long long)(nops - nwide) | (unsigned long long)nwide << 32;
+    for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xFFFFFFFFu, v, o);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long t = 0;
+        for (int w = 0; w < PF_OPS_BLOCK / 32; w++) t += part[w];
+        s.bsum[blockIdx.x] = t;
+    }
+}
+
 // entity_block / entity_unblock (movement.c:560-600) per item, staged for pf_blocker_ops_append: ops[2i..2i+1], desc[i],
 // per-block narrow | wide << 32 counts. patches != nullptr: the apply's rules (block on SET_STATE with next_block, unblock
 // on SET_MOVING, in that order); it runs BEFORE k_entity_apply, so a.pos is still the tick's snapshot position.
@@ -1830,7 +1846,6 @@ __global__ void __launch_bounds__(PF_OPS_BLOCK) k_blocking_decide(const pfnav_ag
                                                                   const uint32_t *__restrict__ uids, int n,
                                                                   const pfnav_patch *__restrict__ patches, int mode, pf_op_stage s)
 {
-    __shared__ unsigned long long part[PF_OPS_BLOCK / 32];
     const int i = blockIdx.x * PF_OPS_BLOCK + threadIdx.x;
     unsigned nops = 0, desc = 0;
     if (i < n) {
@@ -1860,16 +1875,27 @@ __global__ void __launch_bounds__(PF_OPS_BLOCK) k_blocking_decide(const pfnav_ag
         if (nops) blk[uid] = b;
         s.desc[i] = (uint8_t)(desc | nops);
     }
-    const unsigned nwide = ((desc >> 2) & 1u) + ((desc >> 3) & 1u);
-    unsigned long long v = (unsigned long long)(nops - nwide) | (unsigned long long)nwide << 32;
-    for (int o = 16; o; o >>= 1) v += __shfl_down_sync(0xFFFFFFFFu, v, o);
-    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long t = 0;
-        for (int w = 0; w < PF_OPS_BLOCK / 32; w++) t += part[w];
-        s.bsum[blockIdx.x] = t;
+    ops_block_sum(desc, nops, s);
+}
+
+// pfnav_agents_restore: row i of the restored range [lo, lo + n) queues the incref of its recorded block
+// (pf_ckpt_restore_op), staged like k_blocking_decide's ops; the blocking table itself is already the restored one
+__global__ void __launch_bounds__(PF_OPS_BLOCK) k_blocking_restore_decide(const pfnav_agent *__restrict__ agents,
+                                                                          const pfnav_blocking *__restrict__ blk, uint32_t lo,
+                                                                          int n, pf_op_stage s)
+{
+    const int i = blockIdx.x * PF_OPS_BLOCK + threadIdx.x;
+    unsigned nops = 0, desc = 0;
+    if (i < n) {
+        pfnav_blocker_op op;
+        if (pf_ckpt_restore_op(agents[lo + i], blk[lo + i], &op)) {
+            s.ops[2 * i] = op;
+            desc = pf_op_wide(op.range) ? 4u : 0u;
+            nops = 1;
+        }
+        s.desc[i] = (uint8_t)(desc | nops);
     }
+    ops_block_sum(desc, nops, s);
 }
 
 // the checks every entry point of the blocking table makes; need_records: the table must describe this population.
@@ -1897,6 +1923,20 @@ int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n
     PF_CUDA(cudaSetDevice(ctx->device));
     k_blocking_decide<<<(n + PF_OPS_BLOCK - 1) / PF_OPS_BLOCK, PF_OPS_BLOCK, 0, st>>>(ctx->d_agents, ctx->d_blocking, d_uids, n,
                                                                                      d_patches, mode, s);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return pf_blocker_ops_append(ctx, st, (size_t)n, ctx->blocking_any_fac);
+}
+
+int blocking_restore_emit(pfnav_ctx *ctx, cudaStream_t st, size_t lo, int n)
+{
+    if (n == 0) return PFNAV_OK;
+    pf_op_stage s;
+    int rc = pf_blocker_ops_stage(ctx, (size_t)n, &s);
+    if (rc) return rc;
+    PF_CUDA(cudaSetDevice(ctx->device));
+    k_blocking_restore_decide<<<(n + PF_OPS_BLOCK - 1) / PF_OPS_BLOCK, PF_OPS_BLOCK, 0, st>>>(ctx->d_agents, ctx->d_blocking,
+                                                                                             (uint32_t)lo, n, s);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
     return pf_blocker_ops_append(ctx, st, (size_t)n, ctx->blocking_any_fac);

@@ -775,6 +775,12 @@ bool pf_blocker_ops_unexchanged(pfnav_ctx *ctx)
     return st && st->dev_unexchanged;
 }
 
+bool pf_blocker_ops_pending(pfnav_ctx *ctx)
+{
+    const blk_state *st = state_of(ctx, false);
+    return st && st->dev_pending;
+}
+
 int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac)
 {
     blk_state *st = state_of(ctx, false);

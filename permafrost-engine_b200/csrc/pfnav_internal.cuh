@@ -17,6 +17,7 @@
 #include "pfnav_inputs_host.h"
 #include "pfnav_waves_host.h"
 #include "pfnav_resident_host.h"
+#include "pfnav_checkpoint_host.h"
 
 #define PFNAV_VERSION 100
 
@@ -261,6 +262,7 @@ struct pfnav_ctx {
     // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
     pf_dbuf<pfnav_blocking> d_blocking; size_t blocking_n = 0; bool blocking_any_fac = false;
     pf_dbuf<uint32_t> d_block_uids;
+    pf_dbuf<uint8_t> d_ckpt;                  // pfnav_agents_save: the packed rows of the own range
     // pfnav_agents_commands (pfnav_commands.cu): (flock, layer) of every own entity, filled by every full upload, and the device
     // scratch of a batch (merged deltas, per-warp flock histograms, block sums of the work compaction), grown on demand
     pf_cmd_mirror cmd_mirror;
@@ -383,6 +385,8 @@ int pf_blocker_ops_reserve(pfnav_ctx *ctx, size_t need, pf_ops_view *out);
 int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac);
 bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx);             // pfnav_mgpu.cu: member of a job that opted in
 bool pf_blocker_ops_unexchanged(pfnav_ctx *ctx);                // pfnav_blockers.cu: ops decided since the last exchange
+bool pf_blocker_ops_pending(pfnav_ctx *ctx);                    // pfnav_blockers.cu: device-decided ops not yet committed
+void pf_mgpu_rank_world(const pfnav_ctx *ctx, int *rank, int *world);    // pfnav_mgpu.cu: 0 / 1 outside a job
 __host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(range >= 0.0f && (int)ceilf(range / 4) <= 12); }
 
 int pfnav_aux_chunk_seeds(pfnav_ctx *ctx, int dest, int chunk_r, int chunk_c, std::vector<int> &out);     // pfnav_region.cu
@@ -554,6 +558,17 @@ int build_index(pfnav_ctx *ctx, cudaStream_t st);
 // entity_block (mode 1) / entity_unblock (mode 0) of the n uids at d_uids (unique) through k_blocking_decide, appended to
 // the device-decided ops that pfnav_map_commit applies; d_patches != nullptr: the rules of PFNAV_APPLY_BLOCKERS instead
 int blocking_emit(pfnav_ctx *ctx, cudaStream_t st, const uint32_t *d_uids, int n, const pfnav_patch *d_patches, int mode);
+// pfnav_agents_restore: the incref of every restored row of [lo, lo + n) that holds a block (pf_ckpt_restore_op), in uid
+// order, through k_blocking_restore_decide into the same op buffer
+int blocking_restore_emit(pfnav_ctx *ctx, cudaStream_t st, size_t lo, int n);
+// ---- pfnav_checkpoint.cu: a restore in steps, so that a group checks the segments once and every member before any
+// member changes ----
+// ready: a device context with a map. check: the member's own state against segments pf_ckpt_check accepted (route
+// builds of the layers in use, shared blockers in a job), changing nothing; [*lo, *hi): the range the context takes.
+// apply: the uploads of the range's records and the ops of its blocking rows, on `st`.
+int pf_ckpt_restore_ready(pfnav_ctx *ctx);
+int pf_ckpt_restore_check(pfnav_ctx *ctx, const pf_ckpt_set &S, size_t *lo, size_t *hi);
+int pf_ckpt_restore_apply(pfnav_ctx *ctx, const pf_ckpt_set &S, size_t lo, size_t hi, cudaStream_t st);
 // ---- pfnav_events.cu ----
 void pf_events_free(pfnav_ctx *ctx);                             // pfnav_destroy, after the device is idle
 

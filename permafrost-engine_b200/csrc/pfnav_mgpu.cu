@@ -79,6 +79,13 @@ bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx)
     return m && m->share_blockers;
 }
 
+void pf_mgpu_rank_world(const pfnav_ctx *ctx, int *rank, int *world)
+{
+    const pf_mgpu *m = (const pf_mgpu *)ctx->mgpu;
+    *rank = m ? m->rank : 0;
+    *world = m ? m->world : 1;
+}
+
 #define PF_NCCL(call)                                                                                  \
     do {                                                                                               \
         int _r = (call);                                                                               \
@@ -809,6 +816,36 @@ extern "C" int pfnav_mgpu_commands(pfnav_ctx *ctx, const pfnav_agent_delta *delt
         PF_ARG(all[(size_t)r * PF_XCNT + 1] == all[1] && all[(size_t)r * PF_XCNT + 2] == all[2],
                "ranks hold populations or flock tables of different sizes; no rank changed anything");
     return pf_cmd_job_apply(ctx, J, st);
+}
+
+// The segments are validated once, against the fewest layers any member created (a record is refused exactly when some
+// member would refuse it), then every member's own state; only then does any member change. Each member then restores
+// its range on its context stream.
+extern "C" int pfnav_group_restore(pfnav_group *g, const void *const *segs, const size_t *sizes, size_t nseg)
+{
+    PF_ARG(g, "group");
+    const int world = (int)g->ctxs.size();
+    int nlayers = PFNAV_NAV_LAYER_MAX;
+    for (int i = 0; i < world; i++) {
+        if (int rc = pf_ckpt_restore_ready(g->ctxs[i])) return rc;
+        nlayers = std::min(nlayers, g->ctxs[i]->nlayers);
+    }
+    pf_ckpt_set S;
+    const char *e = pf_ckpt_check(segs, sizes, nseg, nlayers, S);
+    PF_ARG(!e, e);
+    std::vector<size_t> lo(world), hi(world);
+    for (int i = 0; i < world; i++)
+        if (int rc = pf_ckpt_restore_check(g->ctxs[i], S, &lo[i], &hi[i])) {
+            const std::string m = pfnav_last_error();
+            pfnav_set_error("%s: member %d refused the restore (%s); no member changed anything", __func__, i, m.c_str());
+            return rc;
+        }
+    for (int i = 0; i < world; i++) {
+        pfnav_ctx *c = g->ctxs[i];
+        PF_CUDA(cudaSetDevice(c->device));
+        if (int rc = pf_ckpt_restore_apply(c, S, lo[i], hi[i], c->tick_stream)) return rc;
+    }
+    return PFNAV_OK;
 }
 
 // In-process group: the members' verdicts are their host state, so nothing is exchanged on the devices; each member then
