@@ -1239,8 +1239,9 @@ int  pfnav_agents_read_work(pfnav_ctx *ctx, uint32_t *out, size_t maxout, size_t
  * segments, and back. The format (csrc/pfnav_checkpoint_host.h): a 64-byte header (magic, format version, record sizes,
  * n_total, the segment's uid range [lo, hi), hz, nflocks, which of the movestate, movestate_ext, formation and blocking
  * tables exist), the whole flock table, then for each uid in [lo, hi), in uid order, its pfnav_agent, pfnav_movestate
- * and, where the tables exist, pfnav_movestate_ext, pfnav_formation_in and pfnav_blocking records. The field pool, its LRU
- * state and the map are not saved: the engine rebuilds the map and re-requests the fields after a restore.
+ * and, where the tables exist, pfnav_movestate_ext, pfnav_formation_in and pfnav_blocking records. The map is not saved:
+ * the engine rebuilds it. The field pool and its LRU state are not in these segments: pfnav_pool_save / pfnav_pool_restore
+ * (below) save and restore them on their own, or the engine re-requests the fields after a restore.
  *
  * Save point: after the commit that follows the apply, the commands and the population change of a tick
  * (pfnav_agents_apply_updates[_ex] -> commands / pfnav_agents_set_blocking / population change -> exchange ->
@@ -1286,6 +1287,54 @@ int  pfnav_agents_save(pfnav_ctx *ctx, void *out, size_t cap, size_t *out_size, 
  * build the same layers for the ranks to agree. */
 int  pfnav_agents_restore(pfnav_ctx *ctx, const void *const *segs, const size_t *sizes, size_t nseg, void *stream);
 int  pfnav_group_restore(pfnav_group *g, const void *const *segs, const size_t *sizes, size_t nseg);
+
+/* Field pool checkpoint (optional): the whole pool of one context as one segment, and back, so that a resumed game ticks
+ * exactly like the game that was saved. Without it a restored context starts with a cold pool and fills it through the
+ * miss path, which can build other fields than the saved pool held (a path field follows the route of the request that
+ * built it, a LOS field its parent chunk's, repairs write fields in place, evictions follow the touch stamps), so the
+ * continuation can differ from the saving game's. The format (csrc/pfnav_pool_host.h): a 64-byte header (magic "PFPL",
+ * format version, record sizes, chunk_w, chunk_h, nlayers, ndests, max_fields, used, nzone, tick number, map digest, and
+ * the counts of free-list entries, aux targets, their footprints and stored fields); the slot table, ff_ids, `has`
+ * bytes, last requests, host touch stamps, owners and free list; the TARGET_ENTITY / TARGET_ENEMIES targets with their
+ * footprints (what in-place repairs of those fields start from); the device touch stamps; then the flow and LOS bytes
+ * (8192) of every slot with a `has` bit, in ascending slot order. Every section is 16-byte aligned.
+ *
+ * The map digest is a 64-bit value over the committed map: the cost, blocker counts, local islands and faction masks of
+ * every tile of every layer, the enemy table (pfnav_set_enemy_factions), nlayers, chunk_w, chunk_h and the map position.
+ * A segment restores only onto a context whose digest equals the saved one, so fields never land on a map they were not
+ * built on.
+ *
+ * pfnav_pool_save: same sizing protocol as pfnav_agents_save.
+ * - out == NULL or cap < the segment's size: PFNAV_ERR_NOMEM with *out_size set, nothing written.
+ * - Ordered on `stream` (NULL: the context's stream) after forked field work and after a pending pfnav_pool_clear (a
+ *   cleared pool saves as empty). The fields and the device touch stamps are packed on the device and come back in one
+ *   copy; the call returns once out is filled.
+ * - PFNAV_ERR_STATE (nothing written) while blocker ops are not committed: device-decided ops, pfnav_blockers_* calls or
+ *   dirty chunks that the next pfnav_map_commit would apply, since that commit drops fields. PFNAV_ERR_NO_DEVICE on a
+ *   host-only context; PFNAV_ERR_ARG when no pool was created.
+ * pfnav_pool_restore: replaces the context's whole pool with the segment's: every slot-table entry, ff_id, `has` byte, last
+ * request, host and device touch stamp, owner, the free-list order, `used`, the zone-held count, every aux target with its
+ * footprints, the stored flow and LOS bytes, and the context's tick number (so that later evictions pick the same slots).
+ * It invalidates the resident goal plan and changes nothing else: not the agents, the map, the work list or the events.
+ * - Everything is validated before anything changes: PFNAV_ERR_ARG for a wrong magic, version or record size, a size that
+ *   is not exact, a map geometry (chunk_w, chunk_h, nlayers) or pool geometry (ndests, max_fields) other than the
+ *   context's, a map digest other than the context's committed map's, bookkeeping that breaks the pool's invariants (every
+ *   slot below `used` is free, owned by the key that maps it, or zone-held; the zone-held count; free-list entries
+ *   distinct, below `used`, unmapped and without fields; nothing at or above `used` mapped; a slot mapped by at most one
+ *   key; ff_ids only on mapped keys; `has` bits within flow | LOS; no touch stamp above the tick number), a built flow
+ *   field whose request names a layer that is not created, and an aux target with a bad kind or layer or a footprint
+ *   that is not finite. PFNAV_ERR_STATE while blocker ops are not committed on the context (as on save); PFNAV_ERR_ARG
+ *   when it has no pool. A refusal changes nothing.
+ * - The call waits for the device before it writes the pool (a tick on any stream may read it) and returns once the pool
+ *   is in place; the segment may be freed then.
+ * Resume order: map built -> buildings queued -> pfnav_agents_restore -> (job: exchange) -> pfnav_map_commit ->
+ * pfnav_pool_restore -> gather / index -> pfnav_agents_set_work_dev -> tick. Nothing needs to be re-requested.
+ * Jobs: each member saves and restores its own pool, no collective is involved. A member's pool restored onto the member of
+ * the same rank in a job with as many members gives the saving job's continuation. Any segment of the same map restores
+ * onto any context with the same pool geometry, since it is a valid pool for that map; but with another member split the
+ * work items whose misses a member serves change, and the continuation is not promised to equal the saving job's. */
+int  pfnav_pool_save(pfnav_ctx *ctx, void *out, size_t cap, size_t *out_size, void *stream);
+int  pfnav_pool_restore(pfnav_ctx *ctx, const void *seg, size_t size, void *stream);
 
 /* N_FlowFieldUpdate with TARGET_ENEMIES / TARGET_ENTITY straight into the pool (what N_RequestAsyncEnemySeekField /
  * N_RequestAsyncSurroundField + N_AwaitAsyncFields leave in the field cache, nav.c:3769-3960): the fields of the listed

@@ -151,7 +151,7 @@ SYMBOLS = [
     "pfnav_mgpu_change_population", "pfnav_group_change_population", "pfnav_ents_in_circles",
     "pfnav_agents_collect_events", "pfnav_agents_read_events",
     "pfnav_agents_input_deltas", "pfnav_mgpu_input_deltas", "pfnav_group_input_deltas", "pfnav_agents_read_formation",
-    "pfnav_agents_save", "pfnav_agents_restore", "pfnav_group_restore",
+    "pfnav_agents_save", "pfnav_agents_restore", "pfnav_group_restore", "pfnav_pool_save", "pfnav_pool_restore",
 ]
 
 _lib = None
@@ -240,6 +240,8 @@ def load():
     L.pfnav_agents_save.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]
     L.pfnav_agents_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_group_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+    L.pfnav_pool_save.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]
+    L.pfnav_pool_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     L.pfnav_group_change_population.argtypes = L.pfnav_agents_change_population.argtypes[:-1]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -845,6 +847,22 @@ class Nav:
 
     def pool_clear(self):
         _chk(self.L.pfnav_pool_clear(self.h))
+
+    def pool_save(self, stream=0):
+        """pfnav_pool_save: the whole field pool of this context as one segment -> bytes (the size is asked first)"""
+        size = C.c_size_t(0)
+        rc = self.L.pfnav_pool_save(self.h, None, 0, C.byref(size), C.c_void_p(stream))
+        if rc != ERR_NOMEM:
+            _chk(rc)
+        out = np.zeros(size.value, np.uint8)
+        _chk(self.L.pfnav_pool_save(self.h, _p(out), size.value, C.byref(size), C.c_void_p(stream)))
+        return out.tobytes()
+
+    def pool_restore(self, segment, stream=0):
+        """pfnav_pool_restore: replace this context's pool with a segment of pool_save (bytes-like), on the same map (after
+        the map_commit that follows agents_restore); nothing needs to be re-requested"""
+        buf = np.frombuffer(bytes(segment), np.uint8)
+        _chk(self.L.pfnav_pool_restore(self.h, _p(buf), len(buf), C.c_void_p(stream)))
 
     def pool_request_goal(self, dest, target_td, layer=0, stream=0):
         nf, nl = C.c_int(0), C.c_int(0)

@@ -781,6 +781,12 @@ bool pf_blocker_ops_pending(pfnav_ctx *ctx)
     return st && st->dev_pending;
 }
 
+bool pf_map_uncommitted(pfnav_ctx *ctx)
+{
+    const blk_state *st = state_of(ctx, false);
+    return !ctx->dirty.empty() || !ctx->fdirty.empty() || (st && (st->dev_pending || !st->circles.empty() || !st->tiles.empty()));
+}
+
 int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac)
 {
     blk_state *st = state_of(ctx, false);

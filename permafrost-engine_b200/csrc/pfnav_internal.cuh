@@ -168,7 +168,7 @@ struct pfnav_ctx {
     } goal_batch;
     uint32_t tick_no = 1;                         // advanced by pfnav_agents_tick
     // TARGET_ENEMIES / TARGET_ENTITY destinations (pfnav_pool_request_entity_fields): what their repairs start from
-    struct aux_target { int kind = -1, layer = 0, ref_layer = 0; std::vector<pfnav_footprint> ents; };
+    using aux_target = pf_aux_target;
     std::vector<aux_target> aux;
 
     // ---- agents ----
@@ -262,7 +262,7 @@ struct pfnav_ctx {
     // [shard_lo, shard_hi) was uploaded; 0 = none uploaded) and the uid list of pfnav_agents_set_blocking
     pf_dbuf<pfnav_blocking> d_blocking; size_t blocking_n = 0; bool blocking_any_fac = false;
     pf_dbuf<uint32_t> d_block_uids;
-    pf_dbuf<uint8_t> d_ckpt;                  // pfnav_agents_save: the packed rows of the own range
+    pf_dbuf<uint8_t> d_ckpt;                  // pfnav_agents_save / pfnav_pool_save / _restore: the packed rows or fields
     // pfnav_agents_commands (pfnav_commands.cu): (flock, layer) of every own entity, filled by every full upload, and the device
     // scratch of a batch (merged deltas, per-warp flock histograms, block sums of the work compaction), grown on demand
     pf_cmd_mirror cmd_mirror;
@@ -386,6 +386,8 @@ int pf_blocker_ops_exchanged(pfnav_ctx *ctx, const uint32_t cnt[2], bool any_fac
 bool pf_mgpu_shares_blockers(const pfnav_ctx *ctx);             // pfnav_mgpu.cu: member of a job that opted in
 bool pf_blocker_ops_unexchanged(pfnav_ctx *ctx);                // pfnav_blockers.cu: ops decided since the last exchange
 bool pf_blocker_ops_pending(pfnav_ctx *ctx);                    // pfnav_blockers.cu: device-decided ops not yet committed
+// pfnav_blockers.cu: the next pfnav_map_commit has work left: device-decided or host-queued blocker ops, or dirty chunks
+bool pf_map_uncommitted(pfnav_ctx *ctx);
 void pf_mgpu_rank_world(const pfnav_ctx *ctx, int *rank, int *world);    // pfnav_mgpu.cu: 0 / 1 outside a job
 __host__ __device__ __forceinline__ bool pf_op_wide(float range) { return !(range >= 0.0f && (int)ceilf(range / 4) <= 12); }
 

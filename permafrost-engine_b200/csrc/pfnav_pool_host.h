@@ -5,14 +5,23 @@
 // is in exactly one of three states: on the free list, owned by the key pf_pool_reserve gave it to (evictable), or taken
 // by the zone rule (pf_pool_zone_take: no owner, never evicted, held until the pool is cleared). Only the functions here
 // and in pfnav_pool.cu write the slot table, the owners, the free list and `used`.
+//
+// The pool segment of pfnav_pool_save / pfnav_pool_restore (its layout, validation and load, and the map digest that ties
+// it to the map its fields were built on) is at the end of this file; tests/emu/pool_checkpoint_emu.cpp builds it with g++.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
 #include <algorithm>
 #include <vector>
 #include "../../include/pfnav.h"
+#include "pfnav_commands_host.h"
 
 void pfnav_set_error(const char *fmt, ...);
+
+// a TARGET_ENEMIES / TARGET_ENTITY destination (pfnav_pool_request_entity_fields): the footprints its in-place repairs
+// start from (kind -1: no entity field was requested for the destination)
+struct pf_aux_target { int kind = -1, layer = 0, ref_layer = 0; std::vector<pfnav_footprint> ents; };
 
 struct pf_pool {
     int ndests = 0, max = 0, used = 0;
@@ -157,4 +166,278 @@ inline void pf_pool_drop(pf_pool &P, size_t key)
     const int32_t s = P.slot[key];
     if (s >= 0) P.has[s] = 0;
     P.ffid[key] = 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// Map digest: a 64-bit value over the committed map images, so that a saved pool is restored only onto the map its
+// fields were built on. Tile t = r * 64 + c of block (layer, chunk) gives the word v = cost | blk << 8 | liid << 24 |
+// fmask << 40 (fmask: the faction bit mask of the tile, 0 where the context keeps none); the block's hash is the wrapping
+// sum over its 4096 tiles of splitmix64(v ^ t * K); the map's value is the wrapping sum over blocks of
+// splitmix64(block hash ^ mix(layer, chunk)), folded with nlayers, chunk_w, chunk_h, the map position and the enemy table
+// (pf_digest_fold). Integer sums do not depend on their order, so every reduction order (the device's k_map_digest, the
+// host loop below) gives the same bits.
+// ------------------------------------------------------------------------------------------
+#define PF_DIGEST_K   0xD6E8FEB86659FD93ull
+#define PF_DIGEST_MIX 0xA0761D6478BD642Full
+
+PF_HD uint64_t pf_splitmix64(uint64_t x)
+{
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+PF_HD uint64_t pf_digest_tile(uint32_t t, uint32_t cost, uint32_t blk, uint32_t liid, uint32_t fmask)
+{
+    const uint64_t v = (uint64_t)cost | (uint64_t)blk << 8 | (uint64_t)liid << 24 | (uint64_t)fmask << 40;
+    return pf_splitmix64(v ^ (uint64_t)t * PF_DIGEST_K);
+}
+PF_HD uint64_t pf_digest_block(uint64_t block_hash, int layer, int chunk)
+{
+    return pf_splitmix64(block_hash ^ ((uint64_t)(uint32_t)layer << 32 | (uint32_t)chunk) * PF_DIGEST_MIX);
+}
+static inline uint64_t pf_digest_fold(uint64_t blocks, int nlayers, int chunk_w, int chunk_h, float map_x, float map_z,
+                                      const uint16_t enemies[16])
+{
+    uint32_t bx, bz;
+    memcpy(&bx, &map_x, 4); memcpy(&bz, &map_z, 4);
+    const uint64_t v[5] = {(uint64_t)nlayers, (uint64_t)chunk_w, (uint64_t)chunk_h, bx, bz};
+    uint64_t h = blocks;
+    for (uint64_t x : v) h = pf_splitmix64(h ^ x);
+    for (int f = 0; f < 16; f++) h = pf_splitmix64(h ^ enemies[f]);
+    return h;
+}
+// The digest over chunk-blocked images ([layer][chunk][64][64], the host mirrors' layout); fmask may be NULL (zeros).
+static inline uint64_t pf_map_digest_host(const uint8_t *cost, const uint16_t *blk, const uint16_t *liid, const uint16_t *fmask,
+                                          int nlayers, int chunk_w, int chunk_h, float map_x, float map_z, const uint16_t enemies[16])
+{
+    const int chunks = chunk_w * chunk_h;
+    uint64_t sum = 0;
+    for (int l = 0; l < nlayers; l++)
+        for (int c = 0; c < chunks; c++) {
+            const size_t base = ((size_t)l * chunks + c) * 4096;
+            uint64_t b = 0;
+            for (uint32_t t = 0; t < 4096; t++)
+                b += pf_digest_tile(t, cost[base + t], blk[base + t], liid[base + t], fmask ? fmask[base + t] : 0);
+            sum += pf_digest_block(b, l, c);
+        }
+    return pf_digest_fold(sum, nlayers, chunk_w, chunk_h, map_x, map_z, enemies);
+}
+
+// ------------------------------------------------------------------------------------------
+// The pool segment (pfnav_pool_save / pfnav_pool_restore). Every section starts 16-byte aligned:
+//   pf_pool_header (64 bytes)
+//   slot table int32 [ndests * chunks], ff_ids uint64 [ndests * chunks], `has` bytes [max], last requests
+//   pfnav_field_req [max], host touch stamps uint32 [max], owners int64 [max], free list int32 [nfree] (in order)
+//   aux targets pf_pool_aux_rec [naux] (destination d = record d), then their footprints pfnav_footprint [nfp] in order
+//   device touch stamps uint32 [max]
+//   for each slot with `has` != 0, ascending: its flow field (4096 bytes) and its LOS field (4096 bytes)
+// The device touch column sits right before the fields, so that it and the packed fields travel in one copy.
+// ------------------------------------------------------------------------------------------
+#define PF_POOL_MAGIC   0x4C504650u           // "PFPL" little-endian
+#define PF_POOL_VERSION 1u
+
+struct pf_pool_header {
+    uint32_t magic, version;
+    uint16_t req_size, fp_size;               // sizeof(pfnav_field_req), sizeof(pfnav_footprint)
+    uint8_t  chunk_w, chunk_h, nlayers, _pad0;
+    int32_t  ndests, max, used, nzone;
+    uint32_t tick_no;
+    uint32_t nfree, naux, nfp, nstored;       // free-list entries, aux targets, their footprints, stored fields
+    uint32_t _pad1;
+    uint64_t digest;                          // pf_map_digest of the map the fields were built on
+};
+static_assert(sizeof(pf_pool_header) == 64, "pf_pool_header is 64 bytes");
+struct pf_pool_aux_rec { int32_t kind, layer, ref_layer; uint32_t nents; };
+
+struct pf_pool_layout { size_t slot, ffid, has, req, touch, owner, free, aux, fp, dtouch, fields, size; };
+static inline pf_pool_layout pf_pool_layout_of(size_t nkeys, size_t max, size_t nfree, size_t naux, size_t nfp, size_t nstored)
+{
+    pf_pool_layout L;
+    size_t o = sizeof(pf_pool_header);
+    auto sec = [&](size_t bytes) { const size_t at = o; o = (o + bytes + 15) & ~(size_t)15; return at; };
+    L.slot = sec(nkeys * 4); L.ffid = sec(nkeys * 8); L.has = sec(max); L.req = sec(max * sizeof(pfnav_field_req));
+    L.touch = sec(max * 4); L.owner = sec(max * 8); L.free = sec(nfree * 4); L.aux = sec(naux * sizeof(pf_pool_aux_rec));
+    L.fp = sec(nfp * sizeof(pfnav_footprint)); L.dtouch = sec(max * 4); L.fields = sec(nstored * 8192);
+    L.size = o;
+    return L;
+}
+
+// what a segment must match on the restoring context: map and pool geometry, and the digest of its committed map
+struct pf_pool_target { int chunk_w, chunk_h, nlayers, ndests, max; uint64_t digest; };
+
+// The slots whose fields a save stores (`has` != 0, ascending) and the segment's layout
+static inline pf_pool_layout pf_pool_seg_plan(const pf_pool &P, const std::vector<pf_aux_target> &aux, std::vector<int32_t> &stored)
+{
+    stored.clear();
+    for (int s = 0; s < P.max; s++) if (P.has[s]) stored.push_back(s);
+    size_t nfp = 0;
+    for (const pf_aux_target &A : aux) nfp += A.ents.size();
+    return pf_pool_layout_of(P.slot.size(), P.max, P.free_list.size(), aux.size(), nfp, stored.size());
+}
+
+// The host part of a segment into out (L.size bytes, planned by pf_pool_seg_plan): the header and every section but the
+// device touch stamps and the fields, which the caller writes at L.dtouch and L.fields. Padding is zero.
+static inline void pf_pool_seg_write(const pf_pool &P, const std::vector<pf_aux_target> &aux, const pf_pool_target &G,
+                                     uint32_t tick_no, const std::vector<int32_t> &stored, const pf_pool_layout &L, uint8_t *out)
+{
+    memset(out, 0, L.dtouch);
+    pf_pool_header h;
+    memset(&h, 0, sizeof(h));
+    h.magic = PF_POOL_MAGIC; h.version = PF_POOL_VERSION;
+    h.req_size = sizeof(pfnav_field_req); h.fp_size = sizeof(pfnav_footprint);
+    h.chunk_w = (uint8_t)G.chunk_w; h.chunk_h = (uint8_t)G.chunk_h; h.nlayers = (uint8_t)G.nlayers;
+    h.ndests = P.ndests; h.max = P.max; h.used = P.used; h.nzone = P.nzone; h.tick_no = tick_no;
+    h.nfree = (uint32_t)P.free_list.size(); h.naux = (uint32_t)aux.size(); h.nstored = (uint32_t)stored.size();
+    h.digest = G.digest;
+    uint32_t nfp = 0;
+    for (const pf_aux_target &A : aux) nfp += (uint32_t)A.ents.size();
+    h.nfp = nfp;
+    memcpy(out, &h, sizeof(h));
+    memcpy(out + L.slot, P.slot.data(), P.slot.size() * 4);
+    memcpy(out + L.ffid, P.ffid.data(), P.ffid.size() * 8);
+    memcpy(out + L.has, P.has.data(), P.max);
+    memcpy(out + L.req, P.req.data(), (size_t)P.max * sizeof(pfnav_field_req));
+    memcpy(out + L.touch, P.touch.data(), (size_t)P.max * 4);
+    memcpy(out + L.owner, P.owner.data(), (size_t)P.max * 8);
+    if (!P.free_list.empty()) memcpy(out + L.free, P.free_list.data(), P.free_list.size() * 4);
+    size_t f = 0;
+    for (size_t d = 0; d < aux.size(); d++) {
+        const pf_aux_target &A = aux[d];
+        const pf_pool_aux_rec r = {A.kind, A.layer, A.ref_layer, (uint32_t)A.ents.size()};
+        memcpy(out + L.aux + d * sizeof(r), &r, sizeof(r));
+        if (!A.ents.empty()) memcpy(out + L.fp + f * sizeof(pfnav_footprint), A.ents.data(), A.ents.size() * sizeof(pfnav_footprint));
+        f += A.ents.size();
+    }
+}
+
+// A validated segment, read out of its bytes: the pool bookkeeping pf_pool_load installs, and where the device part is
+// (base + L.dtouch: the device touch stamps, then the stored fields of the slots in `stored`, in that order).
+struct pf_pool_image {
+    pf_pool_header h;
+    pf_pool_layout L;
+    const uint8_t *base = nullptr;
+    std::vector<int32_t> slot, free_list, stored;
+    std::vector<uint64_t> ffid;
+    std::vector<uint8_t> has;
+    std::vector<pfnav_field_req> req;
+    std::vector<uint32_t> touch, dtouch;
+    std::vector<int64_t> owner;
+    std::vector<pf_aux_target> aux;
+};
+
+template <typename T>
+static inline void pf_pool_read(std::vector<T> &v, const uint8_t *p, size_t n)
+{
+    v.resize(n);
+    if (n) memcpy(v.data(), p, n * sizeof(T));
+}
+
+// Validate a segment completely against the restoring context T, changing nothing: header (magic, version, record sizes,
+// padding), map and pool geometry, counts, exact size, map digest, then the bookkeeping invariants written at the top of
+// this file, the stamps, the requests of built flow fields and the aux targets. Fills I. Returns NULL or what was wrong.
+static inline const char *pf_pool_check(const void *seg, size_t size, const pf_pool_target &T, pf_pool_image &I)
+{
+    if (!seg) return "segment == NULL";
+    if (size < sizeof(pf_pool_header)) return "segment shorter than its header";
+    const uint8_t *b = (const uint8_t *)seg;
+    pf_pool_header &h = I.h;
+    memcpy(&h, b, sizeof(h));
+    if (h.magic != PF_POOL_MAGIC) return "not a pool segment (magic)";
+    if (h.version != PF_POOL_VERSION) return "pool segment format version not supported";
+    if (h.req_size != sizeof(pfnav_field_req) || h.fp_size != sizeof(pfnav_footprint)) return "pool segment record sizes differ from this library's";
+    if (h._pad0 || h._pad1) return "pool segment header padding is not zero";
+    if (h.chunk_w != T.chunk_w || h.chunk_h != T.chunk_h || h.nlayers != T.nlayers)
+        return "pool segment map geometry (chunk_w, chunk_h, nlayers) differs from the context's";
+    if (h.ndests != T.ndests || h.max != T.max) return "pool segment geometry (ndests, max_fields) differs from the context's pool";
+    const size_t chunks = (size_t)T.chunk_w * T.chunk_h, nkeys = (size_t)T.ndests * chunks, mx = (size_t)T.max;
+    if (h.used < 0 || h.used > h.max || h.nzone < 0 || h.nzone > h.used || h.nfree > (uint32_t)h.used ||
+        h.naux > (uint32_t)h.ndests || h.nstored > (uint32_t)h.used || h.nfp >= (1u << 24))
+        return "pool segment counts outside the pool";
+    I.L = pf_pool_layout_of(nkeys, mx, h.nfree, h.naux, h.nfp, h.nstored);
+    const pf_pool_layout &L = I.L;
+    if (size != L.size) return "pool segment size does not match its header (truncated or padded)";
+    if (h.digest != T.digest) return "pool segment was saved on another map (map digest differs)";
+    I.base = b;
+    pf_pool_read(I.slot, b + L.slot, nkeys);
+    pf_pool_read(I.ffid, b + L.ffid, nkeys);
+    pf_pool_read(I.has, b + L.has, mx);
+    pf_pool_read(I.req, b + L.req, mx);
+    pf_pool_read(I.touch, b + L.touch, mx);
+    pf_pool_read(I.owner, b + L.owner, mx);
+    pf_pool_read(I.free_list, b + L.free, h.nfree);
+    pf_pool_read(I.dtouch, b + L.dtouch, mx);
+    const int used = h.used;
+    // the slot table: entries in [-1, used), each slot mapped by at most one key
+    std::vector<int64_t> key_of(mx, -1);
+    for (size_t k = 0; k < nkeys; k++) {
+        const int32_t s = I.slot[k];
+        if (s < -1 || s >= h.max) return "slot-table entry outside the pool";
+        if (s < 0) {
+            if (I.ffid[k]) return "an ff_id on an unmapped key";
+            continue;
+        }
+        if (s >= used) return "a key is mapped to a slot at or above used";
+        if (key_of[s] >= 0) return "a slot is mapped by more than one key";
+        key_of[s] = (int64_t)k;
+    }
+    // the free list: distinct entries below used, unmapped, no owner, no fields
+    std::vector<uint8_t> freed(mx, 0);
+    for (int32_t s : I.free_list) {
+        if (s < 0 || s >= used) return "free-list entry outside [0, used)";
+        if (freed[s]) return "free-list entry repeated";
+        freed[s] = 1;
+        if (key_of[s] >= 0 || I.owner[s] != -1 || I.has[s]) return "free-list entry is mapped, owned or has fields";
+    }
+    // every slot below used: free, owned by the key that maps it, or zone-held (mapped, no owner); nothing above
+    int nzone = 0;
+    uint32_t nstored = 0;
+    for (int s = 0; s < h.max; s++) {
+        const int64_t o = I.owner[s];
+        if (s >= used) {
+            if (o != -1 || I.has[s]) return "a slot at or above used is owned or has fields";
+        } else if (!freed[s]) {
+            if (key_of[s] < 0) return "a used slot is neither free, owned nor zone-held";
+            if (o == -1) nzone++;
+            else if (o != key_of[s]) return "an owned slot is not mapped by its owner";
+        }
+        if (I.has[s] & ~3u) return "a has byte with bits outside flow | LOS";
+        if (I.has[s]) { nstored++; I.stored.push_back(s); }
+        if (I.touch[s] > h.tick_no || I.dtouch[s] > h.tick_no) return "a touch stamp is above tick_no";
+        if ((I.has[s] & 1) && (I.req[s].layer < 0 || I.req[s].layer >= T.nlayers))
+            return "the request of a built flow field names a layer that is not created";
+    }
+    if (nzone != h.nzone) return "nzone does not count the zone-held slots";
+    if (nstored != h.nstored) return "stored field count does not match the has bytes";
+    // aux targets and their footprints
+    I.aux.assign(h.naux, pf_aux_target());
+    size_t f = 0;
+    for (uint32_t d = 0; d < h.naux; d++) {
+        pf_pool_aux_rec r;
+        memcpy(&r, b + L.aux + (size_t)d * sizeof(r), sizeof(r));
+        if (r.kind != -1 && r.kind != PFNAV_TARGET_ENTITY && r.kind != PFNAV_TARGET_ENEMIES) return "aux target with a bad kind";
+        if (r.kind == -1 && (r.layer || r.ref_layer || r.nents)) return "aux target with a bad kind";
+        if (r.kind == PFNAV_TARGET_ENTITY && r.nents != 1) return "aux target with a bad kind";
+        if (r.layer < 0 || r.layer >= T.nlayers || r.ref_layer < 0 || r.ref_layer >= PFNAV_NAV_LAYER_MAX)
+            return "aux target with a bad layer";
+        if (r.nents > h.nfp - f) return "aux footprint counts do not add up";
+        pf_aux_target &A = I.aux[d];
+        A.kind = r.kind; A.layer = r.layer; A.ref_layer = r.ref_layer;
+        pf_pool_read(A.ents, b + L.fp + f * sizeof(pfnav_footprint), r.nents);
+        for (const pfnav_footprint &e : A.ents)
+            if (!pf_finite(&e.x, 3) || !pf_finite(e.corners_xz, 8)) return "aux footprint not finite";
+        f += r.nents;
+    }
+    if (f != h.nfp) return "aux footprint counts do not add up";
+    return nullptr;
+}
+
+// Install a validated segment's bookkeeping in P (whose geometry it matches) and the aux targets; *tick_no: the saved tick
+static inline void pf_pool_load(const pf_pool_image &I, pf_pool &P, std::vector<pf_aux_target> &aux, uint32_t *tick_no)
+{
+    P.used = I.h.used; P.nzone = I.h.nzone;
+    P.slot = I.slot; P.ffid = I.ffid; P.has = I.has; P.req = I.req; P.touch = I.touch; P.owner = I.owner;
+    P.free_list = I.free_list;
+    aux = I.aux;
+    *tick_no = I.h.tick_no;
 }
