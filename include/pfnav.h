@@ -905,11 +905,14 @@ int  pfnav_agents_upload_movestate(pfnav_ctx *ctx, const pfnav_movestate *ms, si
  * use (global islands feed arrived(), movement.c:2170). Every movement state is accepted: MOVING / MOVING_IN_FORMATION
  * (formation inputs), SEEK_ENEMIES, ENTER_ENTITY_RANGE, TURNING, WAITING, ARRIVING_TO_CELL are decided on the device;
  * SURROUND_ENTITY with a live target is flagged PFNAV_TODO_SURROUND_QUERY (see there).
- * The map searches of arrived() run on the device, per used (flock, layer) pair. Without a movestate_ext table the call
- * is asynchronous on `stream` and waits for the device only when one of its buffers has to grow, or, when the arrival
- * constants are rebuilt, for the upload of the rebuild two rebuilds back (the request staging's pinned ring). With a
- * movestate_ext table it still reads back the ENTER_ENTITY_RANGE items and searches their targets' tiles on the host.
- * pfnav_route_build is checked on the host for every used (flock, layer) pair before anything is queued. */
+ * The map searches of arrived() run on the device, per used (flock, layer) pair, and so do ENTER_ENTITY_RANGE's
+ * N_IsMaximallyClose searches around each target's position. With or without a movestate_ext table the call is
+ * asynchronous on `stream` and waits for the device only when one of its buffers has to grow, or, when the arrival
+ * constants are rebuilt, for the upload of the rebuild two rebuilds back (the request staging's pinned ring).
+ * pfnav_route_build is checked on the host for every used (flock, layer) pair before anything is queued. One
+ * configuration still waits: with a movestate_ext table, while some entity of this context stands on a layer without
+ * pfnav_route_build, the call checks its ENTER_ENTITY_RANGE items with a target on the device and waits for that check;
+ * PFNAV_ERR_ARG when one stands on such a layer. */
 int  pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream);
 /* Inspection / test entry: the (flock, layer) table of arrived()'s constants that the last pfnav_agents_compute_updates
  * built, one record per (flock, layer) pair some entity of the flock uses, in (flock, layer) order. Blocks until the

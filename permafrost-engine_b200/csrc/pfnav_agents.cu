@@ -1458,8 +1458,8 @@ k_entity_update(MapView m, GridView g, UpdateParams up, const pfnav_agent *__res
                 const float2 *__restrict__ mc_tiles, int nlayers, const uint32_t *__restrict__ work, int nwork,
                 const float2 *__restrict__ vel_in, const float2 *__restrict__ vdes_in, pfnav_patch *__restrict__ out,
                 const int32_t *__restrict__ flock_of, const pfnav_movestate_ext *__restrict__ exts,
-                const pfnav_formation_in *__restrict__ forms, const pf_arrival_dev *__restrict__ tarr,
-                const float2 *__restrict__ t_tiles)
+                const pfnav_formation_in *__restrict__ forms, pf_enter_cand *__restrict__ cands,
+                uint32_t *__restrict__ cand_count)
 {
     const int wi = blockIdx.x * blockDim.x + threadIdx.x;
     if (wi >= nwork) return;
@@ -1666,10 +1666,10 @@ k_entity_update(MapView m, GridView g, UpdateParams up, const pfnav_agent *__res
         const pf_record tr = rec[ex.surround_target_uid];
         const v2 xz_target = {tr.px, tr.pz};
         const v2 delta = v2_sub(new_pos_xz, xz_target);
-        bool stop = v2_len(delta) <= ex.target_range;
-        if (!stop && tarr) {
-            // M_NavIsAdjacentToImpassable(new_pos) && M_NavIsMaximallyClose(new_pos, target, 0): the tile list of the
-            // target is precomputed per work item on the host (pfnav_arrival_consts with the target's position)
+        const bool stop = v2_len(delta) <= ex.target_range;
+        if (!stop) {
+            // M_NavIsAdjacentToImpassable(new_pos) && M_NavIsMaximallyClose(new_pos, target, 0): the list of the target's
+            // tiles is searched after this kernel (pf_enter_range_search), which also ends the update of such an item
             tile_desc td;
             bool adj = false;
             if (desc_for_point(m, new_pos_xz.x, new_pos_xz.z, td)) {
@@ -1682,21 +1682,18 @@ k_entity_update(MapView m, GridView g, UpdateParams up, const pfnav_agent *__res
                 }
             }
             if (adj) {
-                const pf_arrival_dev ta = tarr[wi];
-                for (int i = 0; i < ta.mc_n && !stop; i++) {
-                    const float2 tc = t_tiles[ta.mc_off + i];
-                    const v2 d = {tc.x - new_pos_xz.x, tc.y - new_pos_xz.z};
-                    if (v2_len(d) <= 0.0f) stop = true;          // tolerance 0.0f (movement.c:2584)
-                }
+                // warp-aggregated append: one atomic per warp
+                const unsigned act = __activemask();
+                const int lane = threadIdx.x & 31, leader = __ffs(act) - 1;
+                uint32_t k = 0;
+                if (lane == leader) k = atomicAdd(cand_count, (uint32_t)__popc(act));
+                k = __shfl_sync(act, k, leader) + __popc(act & ((1u << lane) - 1u));
+                cands[k] = {(uint32_t)wi, layer, new_pos_xz.x, new_pos_xz.z, xz_target.x, xz_target.z,
+                            ex.target_prev_pos[0], ex.target_prev_pos[1]};
+                break;
             }
         }
-        if (stop) { p.flags |= PFNAV_UPDATE_SET_STATE; p.next_state = PFNAV_STATE_WAITING; p.next_block = 1; break; }
-        const v2 tdelta = v2_sub(xz_target, v2{ex.target_prev_pos[0], ex.target_prev_pos[1]});
-        if (v2_len(tdelta) > 5.0f) {
-            p.flags |= PFNAV_UPDATE_SET_DEST | PFNAV_UPDATE_SET_TARGET_PREV;
-            p.next_dest[0] = xz_target.x; p.next_dest[1] = xz_target.z; p.next_attack = 0;
-            p.next_target_prev[0] = xz_target.x; p.next_target_prev[1] = xz_target.z;
-        }
+        pf_enter_range_tail(p, stop, xz_target.x, xz_target.z, ex.target_prev_pos[0], ex.target_prev_pos[1]);
         break;
     }
     case PFNAV_STATE_TURNING: {
@@ -2041,20 +2038,45 @@ extern "C" int pfnav_agents_read_movestate_ext(pfnav_ctx *ctx, pfnav_movestate_e
     return PFNAV_OK;
 }
 
-// work items in STATE_ENTER_ENTITY_RANGE and where their target stands (for the N_IsMaximallyClose clause, movement.c:2583)
-struct pf_enter_item { uint32_t wi; int32_t layer; float tx, tz; };
-__global__ void k_collect_enter_range(const pfnav_agent *__restrict__ agents, const pfnav_movestate_ext *__restrict__ exts,
-                                      const pf_record *__restrict__ rec, const uint32_t *__restrict__ work, int nwork,
-                                      pf_enter_item *__restrict__ out, uint32_t *__restrict__ count)
+// The lowest layer of `unrouted` (a bit per layer) on which a work item in STATE_ENTER_ENTITY_RANGE with a target stands,
+// into *out (INT_MAX: none). N_IsMaximallyClose needs the layer's global islands for such an item (nav.c:1731).
+__global__ void k_enter_unrouted(const pfnav_agent *__restrict__ agents, const pfnav_movestate_ext *__restrict__ exts,
+                                 const uint32_t *__restrict__ work, int nwork, uint32_t unrouted, int *__restrict__ out)
 {
     const int wi = blockIdx.x * blockDim.x + threadIdx.x;
     if (wi >= nwork) return;
     const uint32_t uid = work[wi];
     const pfnav_agent a = agents[uid];
     if (a.state != PFNAV_STATE_ENTER_ENTITY_RANGE || exts[uid].surround_target_uid == PFNAV_NULL_UID) return;
-    const pf_record tr = rec[exts[uid].surround_target_uid];
-    const uint32_t k = atomicAdd(count, 1u);
-    out[k] = {(uint32_t)wi, nav_layer_for(a.flags, a.radius), tr.px, tr.pz};
+    const int layer = nav_layer_for(a.flags, a.radius);
+    if ((unrouted >> layer) & 1u) atomicMin(out, layer);
+}
+
+// ENTER_ENTITY_RANGE items on a layer without pfnav_route_build make compute_updates fail. The host mirror of the own
+// entities' layers tells whether any could: only then are the items checked, which waits for the stream.
+static int enter_range_route_check(pfnav_ctx *ctx, cudaStream_t st, int nwork)
+{
+    uint32_t unrouted = 0;
+    for (int l = 0; l < ctx->nlayers; l++)
+        if (!pfnav_route_dev_islands(ctx, l)) unrouted |= 1u << l;
+    bool any = false;
+    if (unrouted)
+        for (uint8_t l : ctx->cmd_mirror.layer)
+            if ((unrouted >> l) & 1u) { any = true; break; }
+    if (!any) return 0;
+    if (int rc = ctx->d_enter.reserve(sizeof(int))) return rc;
+    int *d_layer = (int *)ctx->d_enter.p;
+    PF_CUDA(cudaMemsetAsync(d_layer, 0x7f, sizeof(int), st));
+    k_enter_unrouted<<<(nwork + 127) / 128, 128, 0, st>>>(ctx->d_agents, ctx->d_ms_ext, ctx->d_work, nwork, unrouted, d_layer);
+    ctx->launches++;
+    int layer = 0;
+    PF_CUDA(cudaMemcpyAsync(&layer, d_layer, sizeof(int), cudaMemcpyDeviceToHost, st));
+    PF_CUDA(cudaStreamSynchronize(st));
+    if (layer != 0x7f7f7f7f) {
+        pfnav_set_error("pfnav_agents_compute_updates: pfnav_route_build(layer %d) is needed (global islands, nav.c:1731)", layer);
+        return PFNAV_ERR_ARG;
+    }
+    return 0;
 }
 
 // The (flock, layer) table k_entity_update reads, rebuilt on the device when the used pairs, the flocks or the committed
@@ -2149,44 +2171,26 @@ extern "C" int pfnav_agents_compute_updates(pfnav_ctx *ctx, void *stream)
     const int nwork = (int)ctx->n_work;
     const size_t b0 = ctx->n_flocks * (size_t)ctx->nlayers * sizeof(pf_arrival_dev);
     // STATE_ENTER_ENTITY_RANGE: the tiles N_IsMaximallyClose (nav.c:4707) compares with depend on where the TARGET entity
-    // stands; they are computed on the host per work item in that state (a handful of units at a time)
-    const pf_arrival_dev *d_tarr = nullptr; const float2 *d_ttiles = nullptr;
+    // stands. k_entity_update appends the items that need them; pf_enter_range_search searches and finishes those items.
+    // d_enter: the two counts (16 bytes), nwork candidate records, nwork flagged indices.
+    pf_enter_cand *d_cand = nullptr;
+    uint32_t *d_cnt = nullptr;
     if (ctx->d_ms_ext) {
-        if ((rc = ctx->d_enter.reserve((size_t)nwork * (sizeof(pf_enter_item) + sizeof(pf_arrival_dev)) + 16))) return rc;
-        uint32_t *d_cnt = (uint32_t *)ctx->d_enter.p;
-        pf_enter_item *d_items = (pf_enter_item *)(ctx->d_enter + 16);
-        pf_arrival_dev *d_t = (pf_arrival_dev *)(d_items + nwork);
-        PF_CUDA(cudaMemsetAsync(d_cnt, 0, 4, st));
-        k_collect_enter_range<<<(nwork + 127) / 128, 128, 0, st>>>(ctx->d_agents, ctx->d_ms_ext, ctx->d_records, ctx->d_work, nwork, d_items, d_cnt);
-        ctx->launches++;
-        uint32_t cnt = 0;
-        PF_CUDA(cudaMemcpyAsync(&cnt, d_cnt, 4, cudaMemcpyDeviceToHost, st));
-        PF_CUDA(cudaStreamSynchronize(st));
-        if (cnt) {
-            std::vector<pf_enter_item> items(cnt);
-            PF_CUDA(cudaMemcpy(items.data(), d_items, cnt * sizeof(pf_enter_item), cudaMemcpyDeviceToHost));
-            std::vector<pf_arrival_dev> tarr(nwork);
-            memset(tarr.data(), 0, tarr.size() * sizeof(pf_arrival_dev));
-            std::vector<float2> tiles;
-            pf_arrival_consts c;
-            for (const pf_enter_item &it : items) {
-                if ((rc = pfnav_arrival_consts(ctx, it.layer, it.tx, it.tz, &c))) return rc;
-                tarr[it.wi].mc_n = c.mc_n; tarr[it.wi].mc_off = (int32_t)tiles.size();
-                for (int i = 0; i < c.mc_n; i++) tiles.push_back(make_float2(c.mc[i][0], c.mc[i][1]));
-            }
-            if ((rc = ctx->d_ttiles.reserve(tiles.size()))) return rc;
-            PF_CUDA(cudaMemcpy(d_t, tarr.data(), tarr.size() * sizeof(pf_arrival_dev), cudaMemcpyHostToDevice));
-            if (!tiles.empty()) PF_CUDA(cudaMemcpy(ctx->d_ttiles, tiles.data(), tiles.size() * sizeof(float2), cudaMemcpyHostToDevice));
-            d_tarr = d_t; d_ttiles = ctx->d_ttiles;
-        }
+        if ((rc = enter_range_route_check(ctx, st, nwork))) return rc;
+        if ((rc = ctx->d_enter.reserve(16 + (size_t)nwork * (sizeof(pf_enter_cand) + sizeof(uint32_t))))) return rc;
+        d_cnt = (uint32_t *)ctx->d_enter.p;
+        d_cand = (pf_enter_cand *)(ctx->d_enter + 16);
+        PF_CUDA(cudaMemsetAsync(d_cnt, 0, 2 * sizeof(uint32_t), st));
     }
     pf_prof_scope prof(ctx, st, PF_PROF_UPDATE);
     k_entity_update<<<(nwork + 127) / 128, 128, 0, st>>>(m, grid_of(ctx), up, ctx->d_agents, ctx->d_records, ctx->d_movestate,
         ctx->d_flocks, (const pf_arrival_dev *)ctx->d_arrival.p, (const float2 *)(ctx->d_arrival + b0),
         ctx->nlayers, ctx->d_work, nwork, ctx->d_vel_out, ctx->d_vdes_out, ctx->d_patches, ctx->d_flock_of,
-        ctx->d_ms_ext, ctx->d_formation, d_tarr, d_ttiles);
+        ctx->d_ms_ext, ctx->d_formation, d_cand, d_cnt);
     ctx->launches++;
     PF_CUDA(cudaGetLastError());
+    if (d_cand && (rc = pf_enter_range_search(ctx, st, d_cand, d_cnt, (uint32_t *)(d_cand + nwork), nwork, ctx->d_patches)))
+        return rc;
     PF_CUDA(cudaEventRecord(ctx->update_done, st));
     return PFNAV_OK;
 }

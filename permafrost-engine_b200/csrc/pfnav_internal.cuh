@@ -184,7 +184,7 @@ struct pfnav_ctx {
     pf_dbuf<uint32_t> d_flock_start;      // [nflocks+1] offsets into d_flock_members
     pf_dbuf<pfnav_formation_in> d_formation;    // optional formation inputs, uid order
     pf_dbuf<pfnav_movestate_ext> d_ms_ext;      // optional: the movestate beyond point seeking
-    pf_dbuf<uint8_t> d_enter; pf_dbuf<float2> d_ttiles;   // ENTER_ENTITY_RANGE scratch
+    pf_dbuf<uint8_t> d_enter;             // ENTER_ENTITY_RANGE candidates (pfnav_agents_compute_updates)
     pf_dbuf<uint32_t> d_facts;            // {max radius bits, any garrisoned}
     // multi-GPU: this context owns the entity index range [shard_lo, shard_hi) of the population (pfnav_mgpu.cu)
     size_t shard_lo = 0, shard_hi = 0;
@@ -224,8 +224,9 @@ struct pfnav_ctx {
     uint64_t arrival_epoch = ~0ull; bool arrival_valid = false;
     std::vector<uint8_t> flock_layer_used;                   // [nflocks][12]
     std::vector<pf_arrival_pair> arrival_pairs;              // the used pairs of the last build, slot order
-    pf_dbuf<int32_t> d_arrival_scratch;                      // the arrival tiers' own whole-layer scratch: compute_updates
-                                                             // runs on its caller's stream, unordered with pfnav_map_query
+    pf_dbuf<int32_t> d_arrival_scratch;                      // the arrival and ENTER_ENTITY_RANGE tiers' own whole-layer
+                                                             // scratch: compute_updates runs on its caller's stream,
+                                                             // unordered with pfnav_map_query
     std::vector<pfnav_flock> h_flocks;
     float max_radius = 0.0f;
     bool has_unsupported_state = false;
@@ -322,6 +323,28 @@ int pf_arrival_search(pfnav_ctx *ctx, cudaStream_t st, const pf_arrival_pair *d_
                       float2 *d_tiles, uint8_t *d_flags);
 int pfnav_arrival_consts(pfnav_ctx *ctx, int layer, float tx, float tz, pf_arrival_consts *out,
                          int which = PF_ARRIVAL_NEAREST | PF_ARRIVAL_MC);
+
+// STATE_ENTER_ENTITY_RANGE (movement.c:2569-2603): an item whose stop depends on N_IsMaximallyClose(new_pos, target, 0)
+// -- not within target_range, new tile 4-adjacent to an impassable or blocked one -- leaves k_entity_update as one of these
+// records with the end of its update undecided; pf_enter_range_search decides it on the device. Each record owns the patch
+// of its work item, so the order of the records does not matter.
+struct pf_enter_cand { uint32_t wi; int32_t layer; float nx, nz, tx, tz, prev_x, prev_z; };
+// The end of the ENTER_ENTITY_RANGE update: stop (WAITING), or re-issue the order when the target moved more than 5 wu
+// since target_prev_pos (v2_len of the difference, as the rest of k_entity_update).
+__device__ __forceinline__ void pf_enter_range_tail(pfnav_patch &p, bool stop, float tx, float tz, float prev_x, float prev_z)
+{
+    if (stop) { p.flags |= PFNAV_UPDATE_SET_STATE; p.next_state = PFNAV_STATE_WAITING; p.next_block = 1; return; }
+    const float dx = tx - prev_x, dz = tz - prev_z;
+    if (sqrtf(dx * dx + dz * dz) > 5.0f) {
+        p.flags |= PFNAV_UPDATE_SET_DEST | PFNAV_UPDATE_SET_TARGET_PREV;
+        p.next_dest[0] = tx; p.next_dest[1] = tz; p.next_attack = 0;
+        p.next_target_prev[0] = tx; p.next_target_prev[1] = tz;
+    }
+}
+// pfnav_query.cu: decide the candidates k_entity_update appended (count[0] of them, at most nwork) on `st` and finish
+// their patches. count[1] and flagged[0 .. nwork) are the search's own; both counts are zero before k_entity_update.
+int pf_enter_range_search(pfnav_ctx *ctx, cudaStream_t st, const pf_enter_cand *d_cand, uint32_t *d_count,
+                          uint32_t *d_flagged, int nwork, pfnav_patch *d_patches);
 // the device image of the global islands of `layer` ([H64][W64] u16, uploaded by pfnav_route_build), or nullptr when
 // the layer's routing structure is not built (pfnav_route.cu)
 const uint16_t *pfnav_route_dev_islands(const pfnav_ctx *ctx, int layer);

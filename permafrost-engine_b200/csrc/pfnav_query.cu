@@ -212,3 +212,78 @@ int pf_arrival_search(pfnav_ctx *ctx, cudaStream_t st, const pf_arrival_pair *d_
     PF_CUDA(cudaGetLastError());
     return PFNAV_OK;
 }
+
+// ------------------------------------------------------------------------------------------
+// ENTER_ENTITY_RANGE's N_IsMaximallyClose(new_pos, target, 0) (movement.c:2583-2584) for the candidates k_entity_update
+// appended: the same query as pfnav_map_query's MAXIMALLY_CLOSE, so the same list and the same tolerance test as the host
+// routine. k_enter_window runs the window tiers, one warp per candidate, and finishes the candidate's patch; the searches
+// that leave the 128 x 128 window are appended to `flagged` and k_enter_layer finishes them over the whole layer. Both
+// read their counts on the device: with no candidates they return at once.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void enter_finish(pfnav_patch *patches, const pf_enter_cand &c, bool hit)
+{
+    pfnav_patch p = patches[c.wi];
+    pf_enter_range_tail(p, hit, c.tx, c.tz, c.prev_x, c.prev_z);
+    patches[c.wi] = p;
+}
+
+__global__ void __launch_bounds__(32) k_enter_window(MapView m, const uint16_t *__restrict__ gisl,
+                                                     const pf_enter_cand *__restrict__ cands, uint32_t *__restrict__ count,
+                                                     uint32_t *__restrict__ flagged, pfnav_patch *__restrict__ patches)
+{
+    __shared__ mq_shared S;
+    __shared__ pfnav_map_query_result R;
+    __shared__ uint8_t fb;
+    const int lane = threadIdx.x & 31;
+    const uint32_t n = count[0];
+    for (uint32_t k = blockIdx.x; k < n; k += gridDim.x) {
+        const pf_enter_cand c = cands[k];
+        const pfnav_map_query_req a = {PFNAV_QUERY_MAXIMALLY_CLOSE, c.layer, c.nx, c.nz, c.tx, c.tz, 0.0f, 0};
+        mq_search(S, m, gisl, a, &R, &fb, lane);
+        if (lane == 0) {
+            if (fb) flagged[atomicAdd(&count[1], 1u)] = k;
+            else enter_finish(patches, c, R.ok != 0);
+        }
+        __syncwarp();
+    }
+}
+
+__global__ void __launch_bounds__(MQ_LAYER_THREADS) k_enter_layer(MapView m, const uint16_t *__restrict__ gisl,
+                                                                  const pf_enter_cand *__restrict__ cands,
+                                                                  const uint32_t *__restrict__ count,
+                                                                  const uint32_t *__restrict__ flagged,
+                                                                  pfnav_patch *__restrict__ patches, int32_t *scratch)
+{
+    __shared__ mq_layer_shared L;
+    __shared__ pfnav_map_query_result R;
+    int32_t *mine = scratch + blockIdx.x * mq_layer_cta_words(m.W64, m.H64);
+    const uint32_t n = count[1];
+    for (uint32_t k = blockIdx.x; k < n; k += gridDim.x) {
+        const pf_enter_cand c = cands[flagged[k]];
+        const pfnav_map_query_req a = {PFNAV_QUERY_MAXIMALLY_CLOSE, c.layer, c.nx, c.nz, c.tx, c.tz, 0.0f, 0};
+        mq_finish_one(L, mine, m, gisl, a, &R, threadIdx.x, blockDim.x);
+        if (threadIdx.x == 0) enter_finish(patches, c, R.ok != 0);
+        __syncthreads();
+    }
+}
+
+int pf_enter_range_search(pfnav_ctx *ctx, cudaStream_t st, const pf_enter_cand *d_cand, uint32_t *d_count,
+                          uint32_t *d_flagged, int nwork, pfnav_patch *d_patches)
+{
+    MapView m;
+    m.cost = ctx->d_cost; m.blk = ctx->d_blk; m.W64 = ctx->W64; m.H64 = ctx->H64;
+    m.chunk_w = ctx->chunk_w; m.chunk_h = ctx->chunk_h; m.map_x = ctx->map_x; m.map_z = ctx->map_z;
+    // the layer tier shares the arrival tiers' scratch: both run on `st`, after refresh_arrival_consts
+    const unsigned lgrid = (unsigned)std::max(ctx->sm_count, 1);
+    if (int rc = ctx->d_arrival_scratch.reserve(lgrid * mq_layer_cta_words(ctx->W64, ctx->H64))) return rc;
+    // about 37 KB of static shared memory per window CTA: a few resident per SM, the rest follow as they retire
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)nwork, (size_t)lgrid * 4);
+    k_enter_window<<<grid, 32, 0, st>>>(m, ctx->d_gisl, d_cand, d_count, d_flagged, d_patches);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    k_enter_layer<<<lgrid, MQ_LAYER_THREADS, 0, st>>>(m, ctx->d_gisl, d_cand, d_count, d_flagged, d_patches,
+                                                      ctx->d_arrival_scratch);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
+}
