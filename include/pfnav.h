@@ -234,6 +234,16 @@ typedef struct pfnav_los_req {
  * earlier one as its prev_los). HOST buffers; out_fields: n x 4096 bytes. */
 int  pfnav_los_fields_create(pfnav_ctx *ctx, const pfnav_los_req *reqs, size_t n,
                              uint8_t *out_fields);
+/* Same, DEVICE-resident d_reqs / d_out_fields (n x 4096 bytes, field i at block i), asynchronous on
+ * `stream` (NULL: the context's own stream). The requests are taken in the caller's order, which
+ * need not be sorted by depth. They are not validated on the host: prev_index must be -1 on the
+ * destination chunk and an index < i elsewhere. PFNAV_LOS_PREV_INPLACE is for the host call only:
+ * a device request off the destination chunk with a negative prev_index reads block _pad of
+ * d_out_fields as its parent. A request that names itself or a later one as its parent never
+ * finishes: the kernel waits on it.
+ * h_wave_offsets[0 .. n_waves] is a HOST array, checked and otherwise unused: it must start at 0,
+ * not decrease and end at n (PFNAV_ERR_ARG otherwise). LOS launches of one context run one after
+ * another, on whatever streams they are queued. */
 int  pfnav_los_fields_create_dev(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n,
                                  uint8_t *d_out_fields, int n_waves, const int32_t *h_wave_offsets,
                                  void *stream);

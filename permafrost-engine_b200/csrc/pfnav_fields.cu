@@ -1574,6 +1574,8 @@ extern "C" int pfnav_flow_fields_update_general_dev(pfnav_ctx *ctx, const pfnav_
     PF_ARG(ctx && ctx->d_cost, "map not created");
     PF_NEED_DEVICE(ctx);
     if (n == 0) return PFNAV_OK;
+    PF_ARG(d_reqs && d_inout_fields, "null buffer");
+    PF_ARG(n < (1u << 30), "n");
     PF_CUDA(cudaSetDevice(ctx->device));
     const int gridg = (int)std::min<size_t>(n, (size_t)ctx->sm_count * 8);
     k_flow_general<<<gridg, FLOWG_THREADS, 0, pf_stream(ctx, stream)>>>(grids_of(ctx), d_reqs, (int)n, d_inout_fields, nullptr, 0);
@@ -1659,7 +1661,11 @@ extern "C" int pfnav_flow_fields_repair(pfnav_ctx *ctx, const pfnav_field_req *t
 extern "C" int pfnav_los_fields_create_dev(pfnav_ctx *ctx, const pfnav_los_req *d_reqs, size_t n, uint8_t *d_out_fields,
                                            int n_waves, const int32_t *h_wave_offsets, void *stream)
 {
-    PF_ARG(n == 0 || (n_waves >= 1 && h_wave_offsets), "null buffer");
+    if (n) {
+        PF_ARG(n_waves >= 1 && h_wave_offsets, "null buffer");
+        PF_ARG(h_wave_offsets[0] == 0 && (size_t)h_wave_offsets[n_waves] == n, "wave offsets must run from 0 to n");
+        for (int w = 0; w < n_waves; w++) PF_ARG(h_wave_offsets[w] <= h_wave_offsets[w + 1], "wave offsets must not decrease");
+    }
     return pfnav_los_launch(ctx, d_reqs, n, d_out_fields, nullptr, stream);
 }
 
