@@ -1349,6 +1349,76 @@ int  pfnav_group_restore(pfnav_group *g, const void *const *segs, const size_t *
 int  pfnav_pool_save(pfnav_ctx *ctx, void *out, size_t cap, size_t *out_size, void *stream);
 int  pfnav_pool_restore(pfnav_ctx *ctx, const void *seg, size_t size, void *stream);
 
+/* State digest: 64-bit digests of the device-resident game state, computed on the device, so that a lockstep or replay
+ * engine can compare a per-tick checksum between peers, or between a replay and its recording, without reading tables
+ * back, and bisect to the first entity that differs. The definitions (csrc/pfnav_digest_host.h) are functions of the
+ * bytes pfnav_agents_save / pfnav_pool_save write, so a digest can be recomputed on the host from saved segments:
+ *   PFNAV_DIGEST_POPULATION  wrapping sum over the uids of the context's own range of a hash of the uid, the tables bits
+ *                            and the row pfnav_agents_save writes for it (agent, movestate, movestate_ext, formation and
+ *                            blocking records where the tables exist). With it, a block array: the same sum over the uids
+ *                            [b << block_log2, (b + 1) << block_log2) for b < ceil(n_total >> block_log2), zero outside
+ *                            the own range. Members' values and arrays add up (wrapping) to a single context's.
+ *   PFNAV_DIGEST_FLOCKS      a chain over the flock table.
+ *   PFNAV_DIGEST_RECORDS     wrapping sum over the whole population of a hash of (uid, 24-byte neighbour record): the
+ *                            column every member of a job holds after a gather.
+ *   PFNAV_DIGEST_MAP         the committed-map digest of the pool segment header.
+ *   PFNAV_DIGEST_POOL        a digest of the segment pfnav_pool_save would write (its map digest word taken as zero).
+ * A change confined to one 8-byte word of one row changes the population value and its block's entry for certain; other
+ * changes change them except with probability about 2^-64.
+ *
+ * pfnav_state_digest queues the digest of the components in `what` on `stream` (NULL: the context's stream) and returns
+ * without waiting for the device. It is ordered after the field work forked by the goal batches, as the pool's other
+ * readers are, and hashes the state as it is at that point of `stream`; host-side parts (the flock table, the pool's
+ * bookkeeping) are taken at the call. block_log2: 6..20 when POPULATION is selected, else ignored. One digest per context
+ * is kept: a new call replaces the previous one (it is ordered after the previous one's copies).
+ * Equality promise: at a point where pfnav_agents_save / pfnav_pool_save would succeed (after the commit that follows the
+ * apply), the values equal the functions of csrc/pfnav_digest_host.h applied to the segments those calls would write;
+ * RECORDS equals the sum over the segments of every member once the record column is current (a single context after
+ * the apply; a job after the gather). Elsewhere the digest still hashes the state as it is.
+ * - PFNAV_ERR_ARG, nothing queued: unknown `what` bits or none, block_log2 outside 6..20 with POPULATION, POPULATION,
+ *   FLOCKS or RECORDS without an uploaded population, MAP without a map, POOL without a pool. PFNAV_ERR_NO_DEVICE on a
+ *   host-only context.
+ * pfnav_state_digest_read waits for that digest only (not for the stream) and writes the selected values into *out,
+ * with n_total, the own range [lo, hi), the tables bits (1 movestate, 2 movestate_ext, 4 formation, 8 blocking) and hz.
+ * blocks: NULL when the block array is not wanted; otherwise *nblocks is set to its length and, when cap is smaller,
+ * PFNAV_ERR_NOMEM is returned with nothing else written (as pfnav_ents_in_circles). The digest stays readable until the
+ * next pfnav_state_digest. PFNAV_ERR_STATE when no digest was queued. */
+#define PFNAV_DIGEST_POPULATION (1u << 0)
+#define PFNAV_DIGEST_FLOCKS     (1u << 1)
+#define PFNAV_DIGEST_RECORDS    (1u << 2)
+#define PFNAV_DIGEST_MAP        (1u << 3)
+#define PFNAV_DIGEST_POOL       (1u << 4)
+#define PFNAV_DIGEST_ALL        0x1Fu
+typedef struct pfnav_digest {
+    uint32_t what;                  /* the components held                                                   */
+    int32_t  block_log2;
+    uint32_t tables;                /* 1 movestate, 2 movestate_ext, 4 formation, 8 blocking                   */
+    int32_t  hz;
+    uint64_t n_total, lo, hi;       /* the population and the own range (a job's combined record: [0, n_total)) */
+    uint64_t nblocks;
+    uint64_t population, flocks, records, map, pool;
+    /* job forms only (zero elsewhere): bit r set when member r's value differs from member 0's (ranks 63 and above
+     * share bit 63) */
+    uint64_t differ_flocks, differ_records, differ_map;
+} pfnav_digest;
+int  pfnav_state_digest(pfnav_ctx *ctx, uint32_t what, int block_log2, void *stream);
+int  pfnav_state_digest_read(pfnav_ctx *ctx, pfnav_digest *out, uint64_t *blocks, size_t cap, size_t *nblocks);
+/* The job forms. pfnav_group_state_digest digests every member (each on its context stream) and waits for them. out has
+ * room for world + 1 records: out[0] is the job's, out[1 + r] member r's own as pfnav_state_digest_read gives it. In
+ * out[0], population and blocks are the wrapping sums of the members' values (the single context's values), flocks,
+ * records and map are member 0's with the differ_* masks, pool is zero: pools follow the member split, so each member's
+ * is in its own record. blocks / cap / nblocks: the job's summed array, as for the read.
+ * pfnav_mgpu_state_digest is the NCCL form: every rank calls it with the same arguments; it queues the rank's digest on
+ * `stream` and all-gathers the ranks' fixed-size digest records in one collective on `stream`, without a host wait.
+ * pfnav_state_digest_read then gives every rank the job's population (the sum), flocks, records and map (rank 0's) and
+ * the differ_* masks, with its own pool, range and block array; the job's block array is the element-wise sum of the
+ * ranks' arrays, which the engine forms only when it bisects.
+ * Errors: those of pfnav_state_digest (members refused before any is queued); PFNAV_ERR_STATE for the NCCL form on a
+ * context in no job or in an in-process group. */
+int  pfnav_group_state_digest(pfnav_group *g, uint32_t what, int block_log2, pfnav_digest *out, uint64_t *blocks, size_t cap,
+                              size_t *nblocks);
+int  pfnav_mgpu_state_digest(pfnav_ctx *ctx, uint32_t what, int block_log2, void *stream);
+
 /* N_FlowFieldUpdate with TARGET_ENEMIES / TARGET_ENTITY straight into the pool (what N_RequestAsyncEnemySeekField /
  * N_RequestAsyncSurroundField + N_AwaitAsyncFields leave in the field cache, nav.c:3769-3960): the fields of the listed
  * chunks become the flow fields of pool destination `dest`; entities name it through pfnav_agent::aux_dest1. The

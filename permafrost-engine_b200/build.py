@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpfnav.so")
-SOURCES = ["pfnav_fields.cu", "pfnav_agents.cu", "pfnav_plan.cu", "pfnav_route.cu", "pfnav_blockers.cu", "pfnav_region.cu", "pfnav_pfmap.cu", "pfnav_mgpu.cu", "pfnav_query.cu", "pfnav_pool.cu", "pfnav_commands.cu", "pfnav_events.cu", "pfnav_inputs.cu", "pfnav_checkpoint.cu"]
+SOURCES = ["pfnav_fields.cu", "pfnav_agents.cu", "pfnav_plan.cu", "pfnav_route.cu", "pfnav_blockers.cu", "pfnav_region.cu", "pfnav_pfmap.cu", "pfnav_mgpu.cu", "pfnav_query.cu", "pfnav_pool.cu", "pfnav_commands.cu", "pfnav_events.cu", "pfnav_inputs.cu", "pfnav_checkpoint.cu", "pfnav_digest.cu"]
 # H100 only: the kernels use Hopper's arch-specific features (TMA, mbarrier), so sm_90a code is built and nothing else
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + [

@@ -109,6 +109,14 @@ assert ENTS_QUERY.itemsize == 24
 EVENT = np.dtype([("uid", "<u4"), ("flags", "<u4"), ("todo", "<u4"), ("attack", "<i4"), ("state_before", "<u4"),
                   ("state_after", "<u4"), ("dest", "<f4", 2), ("pos", "<f4", 2), ("_pad", "<u4", 2)])
 assert EVENT.itemsize == 48
+# pfnav_digest (pfnav_state_digest_read) and its component bits
+DIGEST = np.dtype([("what", "<u4"), ("block_log2", "<i4"), ("tables", "<u4"), ("hz", "<i4"), ("n_total", "<u8"),
+                   ("lo", "<u8"), ("hi", "<u8"), ("nblocks", "<u8"), ("population", "<u8"), ("flocks", "<u8"),
+                   ("records", "<u8"), ("map", "<u8"), ("pool", "<u8"), ("differ_flocks", "<u8"),
+                   ("differ_records", "<u8"), ("differ_map", "<u8")])
+assert DIGEST.itemsize == 112
+DIGEST_POPULATION, DIGEST_FLOCKS, DIGEST_RECORDS, DIGEST_MAP, DIGEST_POOL = 1, 2, 4, 8, 16
+DIGEST_ALL = 31
 
 LOS_PREV_INPLACE = -3
 TICK_VDES_FROM_POOL = 1
@@ -152,6 +160,7 @@ SYMBOLS = [
     "pfnav_agents_collect_events", "pfnav_agents_read_events",
     "pfnav_agents_input_deltas", "pfnav_mgpu_input_deltas", "pfnav_group_input_deltas", "pfnav_agents_read_formation",
     "pfnav_agents_save", "pfnav_agents_restore", "pfnav_group_restore", "pfnav_pool_save", "pfnav_pool_restore",
+    "pfnav_state_digest", "pfnav_state_digest_read", "pfnav_group_state_digest", "pfnav_mgpu_state_digest",
 ]
 
 _lib = None
@@ -242,6 +251,11 @@ def load():
     L.pfnav_group_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     L.pfnav_pool_save.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]
     L.pfnav_pool_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    L.pfnav_state_digest.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p]
+    L.pfnav_state_digest_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.pfnav_group_state_digest.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
+                                           C.POINTER(C.c_size_t)]
+    L.pfnav_mgpu_state_digest.argtypes = [C.c_void_p, C.c_uint32, C.c_int, C.c_void_p]
     L.pfnav_group_change_population.argtypes = L.pfnav_agents_change_population.argtypes[:-1]
     L.pfnav_map_cost_from_tiles.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.pfnav_map_get_layer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -1255,6 +1269,30 @@ class Nav:
         _chk(self.L.pfnav_agents_restore(self.h, *args, C.c_void_p(stream)))
         self.nwork = 0
 
+    def state_digest(self, what=DIGEST_ALL, block_log2=10, stream=0):
+        """pfnav_state_digest: queue the digest of the components in `what` on `stream`; returns without waiting"""
+        _chk(self.L.pfnav_state_digest(self.h, what, block_log2, C.c_void_p(stream)))
+
+    def mgpu_state_digest(self, what=DIGEST_ALL, block_log2=10, stream=0):
+        """collective: state_digest on every rank and one all-gather of the ranks' digest records; state_digest_read then
+        gives the job's values and the differ_* masks"""
+        _chk(self.L.pfnav_mgpu_state_digest(self.h, what, block_log2, C.c_void_p(stream)))
+
+    def state_digest_read(self, blocks=True):
+        """pfnav_state_digest_read -> (DIGEST record, uint64 block array or None); waits for the queued digest only"""
+        d = np.zeros(1, DIGEST)
+        n = C.c_size_t(0)
+        if not blocks:
+            _chk(self.L.pfnav_state_digest_read(self.h, _p(d), None, 0, C.byref(n)))
+            return d[0], None
+        rc = self.L.pfnav_state_digest_read(self.h, _p(d), _p(np.zeros(1, np.uint64)), 0, C.byref(n))
+        if rc != ERR_NOMEM:                   # no block array: the read is done
+            _chk(rc)
+            return d[0], np.zeros(0, np.uint64)
+        b = np.zeros(max(n.value, 1), np.uint64)
+        _chk(self.L.pfnav_state_digest_read(self.h, _p(d), _p(b), n.value, C.byref(n)))
+        return d[0], b[:n.value]
+
     def agents_read_state(self, n, movestate=True):
         a = np.zeros(n, AGENT)
         ms = np.zeros(n, MOVESTATE) if movestate else None
@@ -1418,6 +1456,19 @@ class Group:
         _chk(load().pfnav_group_restore(self.g, *args))
         for nv in self.navs:
             nv.nwork = 0
+
+    def state_digest(self, what=DIGEST_ALL, block_log2=10):
+        """pfnav_group_state_digest -> (DIGEST[world + 1]: the job's record, then each member's; the job's block array)"""
+        out = np.zeros(len(self.navs) + 1, DIGEST)
+        n = C.c_size_t(0)
+        L = load()
+        rc = L.pfnav_group_state_digest(self.g, what, block_log2, _p(out), _p(np.zeros(1, np.uint64)), 0, C.byref(n))
+        if rc != ERR_NOMEM:                   # no block array: the call is done
+            _chk(rc)
+            return out, np.zeros(0, np.uint64)
+        b = np.zeros(max(n.value, 1), np.uint64)
+        _chk(L.pfnav_group_state_digest(self.g, what, block_log2, _p(out), _p(b), n.value, C.byref(n)))
+        return out, b[:n.value]
 
     def close(self):
         if self.g:

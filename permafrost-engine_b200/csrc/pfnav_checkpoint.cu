@@ -4,9 +4,6 @@
 #include "pfnav_internal.cuh"
 #include <string.h>
 
-// the per-entity tables a row is packed from, as 16-byte words: table t holds words[t] words per uid
-struct pf_ckpt_src { const uint4 *p[5]; uint32_t words[5]; };
-
 // word w of the packed rows of [lo, lo + nrows): row w / row.words, word w % row.words of it (pf_ckpt_word_source)
 __global__ void k_ckpt_pack(pf_ckpt_src src, pf_ckpt_row row, uint32_t tables, uint32_t lo, uint32_t nrows, uint4 *__restrict__ out)
 {
@@ -23,7 +20,15 @@ __global__ void k_ckpt_pack(pf_ckpt_src src, pf_ckpt_row row, uint32_t tables, u
     }
 }
 
-static uint32_t tables_of(const pfnav_ctx *ctx)
+pf_ckpt_src pf_ckpt_sources(const pfnav_ctx *ctx)
+{
+    pf_ckpt_src src;
+    const void *p[5] = {ctx->d_agents.p, ctx->d_movestate.p, ctx->d_ms_ext.p, ctx->d_formation.p, ctx->d_blocking.p};
+    for (int t = 0; t < 5; t++) { src.p[t] = (const uint4 *)p[t]; src.words[t] = pf_ckpt_sizes[t] / 16; }
+    return src;
+}
+
+uint32_t pf_ckpt_tables(const pfnav_ctx *ctx)
 {
     return (ctx->movestate_set ? PF_CKPT_MS : 0u) | (ctx->d_ms_ext != nullptr ? PF_CKPT_EXT : 0u) |
            (ctx->d_formation != nullptr ? PF_CKPT_FORM : 0u) |
@@ -45,7 +50,7 @@ extern "C" int pfnav_agents_save(pfnav_ctx *ctx, void *out, size_t cap, size_t *
                         pf_blocker_ops_unexchanged(ctx) ? " or exchanged" : "");
         return PFNAV_ERR_STATE;
     }
-    const uint32_t tables = tables_of(ctx);
+    const uint32_t tables = pf_ckpt_tables(ctx);
     const size_t lo = ctx->shard_lo, hi = ctx->shard_hi, nf = ctx->h_flocks.size();
     const size_t size = pf_ckpt_bytes(tables, nf, hi - lo);
     *out_size = size;
@@ -63,9 +68,7 @@ extern "C" int pfnav_agents_save(pfnav_ctx *ctx, void *out, size_t cap, size_t *
     const pf_ckpt_row row = pf_ckpt_row_of(tables);
     const size_t bytes = (hi - lo) * (size_t)row.words * 16;
     if (int rc = ctx->d_ckpt.reserve(bytes)) return rc;
-    pf_ckpt_src src;
-    const void *p[5] = {ctx->d_agents.p, ctx->d_movestate.p, ctx->d_ms_ext.p, ctx->d_formation.p, ctx->d_blocking.p};
-    for (int t = 0; t < 5; t++) { src.p[t] = (const uint4 *)p[t]; src.words[t] = pf_ckpt_sizes[t] / 16; }
+    const pf_ckpt_src src = pf_ckpt_sources(ctx);
     const size_t nw = bytes / 16;
     const int grid = (int)std::min<size_t>((nw + 255) / 256, (size_t)ctx->sm_count * 16);
     k_ckpt_pack<<<grid, 256, 0, st>>>(src, row, tables, (uint32_t)lo, (uint32_t)(hi - lo), (uint4 *)ctx->d_ckpt.p);

@@ -1169,6 +1169,7 @@ extern "C" void pfnav_destroy(pfnav_ctx *ctx)
     pfnav_fields_free(ctx);
     pfnav_agents_free(ctx);
     pf_events_free(ctx);
+    pf_digest_free(ctx);
     if (ctx->tick_done) cudaEventDestroy(ctx->tick_done);
     if (ctx->tick_stream) cudaStreamDestroy(ctx->tick_stream);
     if (ctx->ev_vel0) cudaEventDestroy(ctx->ev_vel0);

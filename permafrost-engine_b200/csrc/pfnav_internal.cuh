@@ -18,6 +18,7 @@
 #include "pfnav_waves_host.h"
 #include "pfnav_resident_host.h"
 #include "pfnav_checkpoint_host.h"
+#include "pfnav_digest_host.h"
 
 #define PFNAV_VERSION 100
 
@@ -240,6 +241,12 @@ struct pfnav_ctx {
     pf_dbuf<pfnav_event> d_events; pf_dbuf<uint32_t> d_event_aux;
     uint32_t *h_event_count = nullptr; cudaEvent_t events_done = nullptr; bool events_valid = false;
     pfnav_event *h_events = nullptr; size_t h_events_cap = 0;
+    // pfnav_state_digest (pfnav_digest.cu): the device records of the last digest ([world][PF_DIGEST_REC] words: the own
+    // record at rank, the peers' after an NCCL all-gather) and its block array behind them, their pinned copy, the event
+    // recorded behind the copy, and what the read reports from the call
+    pf_dbuf<unsigned long long> d_digest;
+    uint64_t *h_digest = nullptr; size_t h_digest_cap = 0; cudaEvent_t digest_done = nullptr; bool digest_valid = false;
+    pfnav_digest digest_info = {}; int digest_world = 1, digest_rank = 0;
     cudaStream_t tick_stream = nullptr;
     cudaEvent_t tick_done = nullptr;
     // LOS chains of a goal batch run on their own stream so that the parts of the tick that do not read
@@ -596,6 +603,23 @@ int pf_ckpt_restore_check(pfnav_ctx *ctx, const pf_ckpt_set &S, size_t *lo, size
 int pf_ckpt_restore_apply(pfnav_ctx *ctx, const pf_ckpt_set &S, size_t lo, size_t hi, cudaStream_t st);
 // ---- pfnav_events.cu ----
 void pf_events_free(pfnav_ctx *ctx);                             // pfnav_destroy, after the device is idle
+// ---- pfnav_digest.cu: pfnav_state_digest in steps, so that the NCCL form all-gathers the records in between ----
+// check: the arguments against the context, changing nothing. launch: the digest kernels on `st`, writing the own record
+// at rank of a world-record area and the block array. finish: the copy of the records and blocks to the pinned buffer and
+// the event behind it. A digest record holds PF_DIGEST_REC words: population, flocks, records, map, pool, 0, 0, 0.
+#define PF_DIGEST_REC 8
+int pf_digest_check(pfnav_ctx *ctx, uint32_t what, int block_log2);
+int pf_digest_launch(pfnav_ctx *ctx, uint32_t what, int block_log2, cudaStream_t st, int world, int rank);
+int pf_digest_finish(pfnav_ctx *ctx, cudaStream_t st);
+void pf_digest_free(pfnav_ctx *ctx);                             // pfnav_destroy, after the device is idle
+// ---- pfnav_checkpoint.cu / pfnav_pool.cu: what the digest shares with the saves ----
+uint32_t pf_ckpt_tables(const pfnav_ctx *ctx);                   // the PF_CKPT_* tables pfnav_agents_save writes
+// the per-entity tables a row is packed from, as 16-byte words: table t (pf_ckpt_word_source's t) holds words[t] words
+// per uid; a table the context does not hold is null
+struct pf_ckpt_src { const uint4 *p[5]; uint32_t words[5]; };
+pf_ckpt_src pf_ckpt_sources(const pfnav_ctx *ctx);
+// k_map_digest on `st`: the wrapping sum of the block terms added to *d_sum (pf_digest_fold finishes it)
+int pf_map_digest_launch(pfnav_ctx *ctx, cudaStream_t st, unsigned long long *d_sum);
 
 // ---- pfnav_commands.cu: a job member's part of a command batch (pfnav_mgpu.cu runs the verdict exchange) ----
 // pf_cmd_job_check validates the batch against the member's state and plans it, changing nothing (the error is set);

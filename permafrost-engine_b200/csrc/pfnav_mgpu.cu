@@ -1082,3 +1082,68 @@ extern "C" int pfnav_group_change_population(pfnav_group *g, const uint32_t *rem
     }
     return PFNAV_OK;
 }
+
+// ------------------------------------------------------------------------------------------
+// State digests of a job (pfnav_digest.cu). The group form digests every member on its context stream and combines the
+// members' records on the host; the NCCL form all-gathers the ranks' fixed-size records on `stream` and leaves the
+// combination to pfnav_state_digest_read.
+// ------------------------------------------------------------------------------------------
+extern "C" int pfnav_group_state_digest(pfnav_group *g, uint32_t what, int block_log2, pfnav_digest *out, uint64_t *blocks,
+                                        size_t cap, size_t *nblocks)
+{
+    PF_ARG(g && out, "group / out");
+    PF_ARG(!blocks || nblocks, "nblocks == NULL with a block array");
+    const int world = (int)g->ctxs.size();
+    for (int i = 0; i < world; i++)
+        if (int rc = pf_digest_check(g->ctxs[i], what, block_log2)) {
+            const std::string e = pfnav_last_error();
+            pfnav_set_error("%s: member %d refused the digest (%s); no member queued one", __func__, i, e.c_str());
+            return rc;
+        }
+    const size_t n_total = g->ctxs[0]->n_agents;
+    if (what & (PFNAV_DIGEST_POPULATION | PFNAV_DIGEST_RECORDS))
+        for (int i = 0; i < world; i++) PF_ARG(g->ctxs[i]->n_agents == n_total, "members hold populations of different sizes");
+    const size_t nb = (what & PFNAV_DIGEST_POPULATION) ? pf_digest_nblocks(n_total, block_log2) : 0;
+    if (nblocks) *nblocks = nb;
+    if (blocks && cap < nb) {
+        pfnav_set_error("%s: the block array holds %zu entries, cap %zu", __func__, nb, cap);
+        return PFNAV_ERR_NOMEM;
+    }
+    for (int i = 0; i < world; i++)
+        if (int rc = pfnav_state_digest(g->ctxs[i], what, block_log2, nullptr)) return rc;
+    pfnav_digest job;
+    memset(&job, 0, sizeof(job));
+    std::vector<uint64_t> mine(nb);
+    if (blocks) std::fill(blocks, blocks + nb, 0);
+    for (int i = 0; i < world; i++) {
+        pfnav_digest &d = out[1 + i];
+        size_t n = 0;
+        if (int rc = pfnav_state_digest_read(g->ctxs[i], &d, mine.data(), nb, &n)) return rc;
+        if (i == 0) {
+            job = d;
+            job.lo = 0; job.hi = n_total; job.population = 0; job.pool = 0;
+        }
+        const uint64_t bit = 1ull << std::min(i, 63);
+        job.population += d.population;
+        if (d.flocks != out[1].flocks) job.differ_flocks |= bit;
+        if (d.records != out[1].records) job.differ_records |= bit;
+        if (d.map != out[1].map) job.differ_map |= bit;
+        if (blocks)
+            for (size_t b = 0; b < nb; b++) blocks[b] += mine[b];
+    }
+    out[0] = job;
+    return PFNAV_OK;
+}
+
+extern "C" int pfnav_mgpu_state_digest(pfnav_ctx *ctx, uint32_t what, int block_log2, void *stream)
+{
+    pf_mgpu *m = nullptr;
+    if (int rc = nccl_rank(ctx, __func__, "pfnav_group_state_digest", &m)) return rc;
+    if (int rc = pf_digest_check(ctx, what, block_log2)) return rc;
+    cudaStream_t st = pf_stream(ctx, stream);
+    if (int rc = pf_digest_launch(ctx, what, block_log2, st, m->world, m->rank)) return rc;
+    unsigned long long *rec = ctx->d_digest.p;
+    PF_NCCL(g_nccl.AllGather(rec + (size_t)m->rank * PF_DIGEST_REC, rec, PF_DIGEST_REC * sizeof(uint64_t), /*ncclInt8*/ 0,
+                             m->comm, st));
+    return pf_digest_finish(ctx, st);
+}

@@ -224,16 +224,22 @@ __global__ void __launch_bounds__(256) k_pool_unpack(const int32_t *__restrict__
     }
 }
 
-// The context's map digest (pfnav_pool_host.h) on `st`; d_ckpt holds at least 16 bytes. Waits for `st`.
+int pf_map_digest_launch(pfnav_ctx *ctx, cudaStream_t st, unsigned long long *d_sum)
+{
+    const int chunks = ctx->chunk_w * ctx->chunk_h;
+    k_map_digest<<<(unsigned)(ctx->nlayers * chunks), 256, 0, st>>>(ctx->d_cost, ctx->d_blk, ctx->d_liid, ctx->d_fmask,
+                                                                     ctx->chunk_w, ctx->W64, chunks, d_sum);
+    ctx->launches++;
+    PF_CUDA(cudaGetLastError());
+    return PFNAV_OK;
+}
+
+// The context's map digest (pfnav_digest_host.h) on `st`; d_ckpt holds at least 16 bytes. Waits for `st`.
 static int map_digest(pfnav_ctx *ctx, cudaStream_t st, uint64_t *out)
 {
     unsigned long long *d = (unsigned long long *)ctx->d_ckpt.p;
-    const int chunks = ctx->chunk_w * ctx->chunk_h;
     PF_CUDA(cudaMemsetAsync(d, 0, 8, st));
-    k_map_digest<<<(unsigned)(ctx->nlayers * chunks), 256, 0, st>>>(ctx->d_cost, ctx->d_blk, ctx->d_liid, ctx->d_fmask,
-                                                                     ctx->chunk_w, ctx->W64, chunks, d);
-    ctx->launches++;
-    PF_CUDA(cudaGetLastError());
+    if (int rc = pf_map_digest_launch(ctx, st, d)) return rc;
     uint64_t sum = 0;
     PF_CUDA(cudaMemcpyAsync(&sum, d, 8, cudaMemcpyDeviceToHost, st));
     PF_CUDA(cudaStreamSynchronize(st));

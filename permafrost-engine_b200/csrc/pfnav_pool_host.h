@@ -6,8 +6,9 @@
 // by the zone rule (pf_pool_zone_take: no owner, never evicted, held until the pool is cleared). Only the functions here
 // and in pfnav_pool.cu write the slot table, the owners, the free list and `used`.
 //
-// The pool segment of pfnav_pool_save / pfnav_pool_restore (its layout, validation and load, and the map digest that ties
-// it to the map its fields were built on) is at the end of this file; tests/emu/pool_checkpoint_emu.cpp builds it with g++.
+// The pool segment of pfnav_pool_save / pfnav_pool_restore (its layout, validation and load) is at the end of this file;
+// tests/emu/pool_checkpoint_emu.cpp builds it with g++. The map digest that ties a segment to the map its fields were
+// built on is defined with the other state digests in pfnav_digest_host.h, which this header includes at its end.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -166,62 +167,6 @@ inline void pf_pool_drop(pf_pool &P, size_t key)
     const int32_t s = P.slot[key];
     if (s >= 0) P.has[s] = 0;
     P.ffid[key] = 0;
-}
-
-// ------------------------------------------------------------------------------------------
-// Map digest: a 64-bit value over the committed map images, so that a saved pool is restored only onto the map its
-// fields were built on. Tile t = r * 64 + c of block (layer, chunk) gives the word v = cost | blk << 8 | liid << 24 |
-// fmask << 40 (fmask: the faction bit mask of the tile, 0 where the context keeps none); the block's hash is the wrapping
-// sum over its 4096 tiles of splitmix64(v ^ t * K); the map's value is the wrapping sum over blocks of
-// splitmix64(block hash ^ mix(layer, chunk)), folded with nlayers, chunk_w, chunk_h, the map position and the enemy table
-// (pf_digest_fold). Integer sums do not depend on their order, so every reduction order (the device's k_map_digest, the
-// host loop below) gives the same bits.
-// ------------------------------------------------------------------------------------------
-#define PF_DIGEST_K   0xD6E8FEB86659FD93ull
-#define PF_DIGEST_MIX 0xA0761D6478BD642Full
-
-PF_HD uint64_t pf_splitmix64(uint64_t x)
-{
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
-PF_HD uint64_t pf_digest_tile(uint32_t t, uint32_t cost, uint32_t blk, uint32_t liid, uint32_t fmask)
-{
-    const uint64_t v = (uint64_t)cost | (uint64_t)blk << 8 | (uint64_t)liid << 24 | (uint64_t)fmask << 40;
-    return pf_splitmix64(v ^ (uint64_t)t * PF_DIGEST_K);
-}
-PF_HD uint64_t pf_digest_block(uint64_t block_hash, int layer, int chunk)
-{
-    return pf_splitmix64(block_hash ^ ((uint64_t)(uint32_t)layer << 32 | (uint32_t)chunk) * PF_DIGEST_MIX);
-}
-static inline uint64_t pf_digest_fold(uint64_t blocks, int nlayers, int chunk_w, int chunk_h, float map_x, float map_z,
-                                      const uint16_t enemies[16])
-{
-    uint32_t bx, bz;
-    memcpy(&bx, &map_x, 4); memcpy(&bz, &map_z, 4);
-    const uint64_t v[5] = {(uint64_t)nlayers, (uint64_t)chunk_w, (uint64_t)chunk_h, bx, bz};
-    uint64_t h = blocks;
-    for (uint64_t x : v) h = pf_splitmix64(h ^ x);
-    for (int f = 0; f < 16; f++) h = pf_splitmix64(h ^ enemies[f]);
-    return h;
-}
-// The digest over chunk-blocked images ([layer][chunk][64][64], the host mirrors' layout); fmask may be NULL (zeros).
-static inline uint64_t pf_map_digest_host(const uint8_t *cost, const uint16_t *blk, const uint16_t *liid, const uint16_t *fmask,
-                                          int nlayers, int chunk_w, int chunk_h, float map_x, float map_z, const uint16_t enemies[16])
-{
-    const int chunks = chunk_w * chunk_h;
-    uint64_t sum = 0;
-    for (int l = 0; l < nlayers; l++)
-        for (int c = 0; c < chunks; c++) {
-            const size_t base = ((size_t)l * chunks + c) * 4096;
-            uint64_t b = 0;
-            for (uint32_t t = 0; t < 4096; t++)
-                b += pf_digest_tile(t, cost[base + t], blk[base + t], liid[base + t], fmask ? fmask[base + t] : 0);
-            sum += pf_digest_block(b, l, c);
-        }
-    return pf_digest_fold(sum, nlayers, chunk_w, chunk_h, map_x, map_z, enemies);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -441,3 +386,6 @@ static inline void pf_pool_load(const pf_pool_image &I, pf_pool &P, std::vector<
     aux = I.aux;
     *tick_no = I.h.tick_no;
 }
+
+// the hash primitives and the map digest (pfnav_digest_host.h builds on the layout above, so it comes last)
+#include "pfnav_digest_host.h"
