@@ -90,6 +90,57 @@ def local_islands_np(cost, blockers=None):
     return out
 
 
+def serpentine_cost(cw=32, ch=32, gap=40):
+    """A map whose every route is forced: a 2-tile wall on every chunk-row boundary (the last nav-tile row of the upper
+    chunk row and the first of the lower one), open only over `gap` tiles at the right end of odd boundaries and at the
+    left end of even ones. A route from the top-left chunk crosses chunk row 0 to the right, goes down at the right end,
+    crosses row 1 to the left, and so on (boustrophedon). -> cost [ch * cw][64][64]"""
+    img = np.ones((ch * 64, cw * 64), np.uint8)
+    for k in range(1, ch):
+        img[64 * k - 1:64 * k + 1, :] = 0xFF
+        if k % 2:
+            img[64 * k - 1:64 * k + 1, cw * 64 - gap:] = 1
+        else:
+            img[64 * k - 1:64 * k + 1, :gap] = 1
+    return synth.image_to_blocked(img, cw, ch)
+
+
+def serpentine_order(cw, ch):
+    """the chunk indices of serpentine_cost's forced route from the top-left chunk, row by row, in travel order"""
+    return [r * cw + (c if r % 2 == 0 else cw - 1 - c) for r in range(ch) for c in range(cw)]
+
+
+PORTAL_GRID_GAPS = (6, 22, 38, 54)
+
+
+def portal_grid_cost(cw=32, ch=32, gaps=PORTAL_GRID_GAPS, region=((14, 14), (2, 2))):
+    """A map of many portals: a 2-tile wall on every chunk border, opened by a 3-tile gap at each offset of `gaps` per
+    side, so an interior chunk has 4 * len(gaps) portals. region ((chunk row, chunk column), (rows, columns)): a block of
+    chunks whose outer border has no gaps; inside it the borders keep theirs, so it holds portals of its own that
+    nothing outside it reaches. -> cost [ch * cw][64][64]"""
+    img = np.ones((ch * 64, cw * 64), np.uint8)
+    for k in range(1, ch):
+        img[64 * k - 1:64 * k + 1, :] = 0xFF
+    for k in range(1, cw):
+        img[:, 64 * k - 1:64 * k + 1] = 0xFF
+    for k in range(1, ch):                  # gaps in the walls between chunk rows
+        for c in range(cw):
+            for g in gaps:
+                img[64 * k - 1:64 * k + 1, 64 * c + g:64 * c + g + 3] = 1
+    for k in range(1, cw):                  # and between chunk columns
+        for r in range(ch):
+            for g in gaps:
+                img[64 * r + g:64 * r + g + 3, 64 * k - 1:64 * k + 1] = 1
+    if region is not None:
+        (r0, c0), (nr, nc) = region
+        R0, R1, C0, C1 = 64 * r0, 64 * (r0 + nr), 64 * c0, 64 * (c0 + nc)
+        img[R0 - 1:R0 + 1, C0 - 1:C1 + 1] = 0xFF
+        img[R1 - 1:R1 + 1, C0 - 1:C1 + 1] = 0xFF
+        img[R0 - 1:R1 + 1, C0 - 1:C0 + 1] = 0xFF
+        img[R0 - 1:R1 + 1, C1 - 1:C1 + 1] = 0xFF
+    return synth.image_to_blocked(img, cw, ch)
+
+
 def flow_tile_case(seed, dens, n=8):
     """-> cost[1,64,64], reqs"""
     p = noise_map(1, 1, seed, dens)
@@ -201,6 +252,47 @@ def execute_route(flow_exec, los_exec, fr, fc, lr, lc):
         fields[int(fc[k])] = out[0]
     los = los_exec(lr) if len(lr) else np.zeros((0, 64, 64), np.uint8)
     return fields, {int(lc[k]): los[k] for k in range(len(lr))}
+
+
+def los_depths(lr):
+    """depth of every LOS request of a batch: 1 without a parent, else its parent's + 1 (parents come first)"""
+    depth = np.zeros(len(lr), np.int64)
+    for i, q in enumerate(lr):
+        p = int(q["prev_index"])
+        depth[i] = 1 if p < 0 else depth[p] + 1
+    return depth
+
+
+def port_goal_fields(nav, om, target_td):
+    """N_RequestGoal's plan for target_td (nav.plan_goal: flow waves, chained LOS requests) executed by the port `om`
+    -> ({chunk: flow}, {chunk: los}, the plan's LOS requests, its number of flow requests)"""
+    fr, fc, fw, lr, lc = nav.plan_goal(tuple(int(v) for v in target_td))
+    fields = {}
+    for w in range(int(fw.max()) + 1):
+        sel = np.nonzero(fw == w)[0]
+        base = np.stack([fields.get(int(fc[i]), np.zeros((64, 64), np.uint8)) for i in sel])
+        out = om.flow_fields_update(fr[sel], inout=base)
+        for k, i in enumerate(sel):
+            fields[int(fc[i])] = out[k]
+    los = om.los_fields_create(lr)
+    return fields, {int(lc[k]): los[k] for k in range(len(lr))}, lr, len(fr)
+
+
+def check_goal_pool(nav, expected, cw, nchunks):
+    """every (dest, chunk) entry of the pool against port_goal_fields' results per dest: presence and bytes
+    -> the number of fields compared"""
+    n = 0
+    for d, (flows, los) in enumerate(e[:2] for e in expected):
+        for c in range(nchunks):
+            f, l, _ = nav.pool_get(d, divmod(c, cw))
+            assert (f is not None) == (c in flows) and (l is not None) == (c in los), (d, c)
+            if f is not None:
+                assert np.array_equal(f, flows[c]), (d, c)
+                n += 1
+            if l is not None:
+                assert np.array_equal(l, los[c]), (d, c)
+                n += 1
+    return n
 
 
 def tile_attr_case(cw, ch, seed, terrain=False):
